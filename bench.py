@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- fwd+bwd views/sec of the surfel-rasterizer hot path on N B200s.
+"""bench.py -- fwd+bwd views/sec of the surfel-rasterizer hot path on N GPUs (H100).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port P bench.py --gpus N --steps K --warmup W
 
@@ -24,8 +24,8 @@ Printed JSON (one line, rank 0):
             e2e.batched is the same host-in / host-out protocol through the batched public entry
             (lara_b200.multiview.render_scene_views, one autograd node per scene)
   roofline: dominant kernel (render_bwd) -- SURVEY 8d algorithmic bytes per launch / its live
-            CUDA-event duration (srf_profile_*), against MEASURED_PEAKS.json hbm_gbs; roofline.issue states
-            the bound that actually binds the blend kernels (warp-instruction issue slots)
+            CUDA-event duration (srf_profile_*), against MEASURED_PEAKS.json hbm_gbs (else the H100 SXM
+            data-sheet 3.35 TB/s)
   extra   : BASELINE configs C2 (32k / 512^2 / 1 view), C4 (256k / 1024^2, 4 views per GPU), the strong-scaling
             point (8 global views split over the ranks) and a >= 2 s sustained run
   grad_check (N > 1): rank 0 re-renders all N*V views alone and compares with the all-reduced buffer
@@ -33,6 +33,9 @@ Printed JSON (one line, rank 0):
             workload (N=1, rank 0 only)
 --impl reference times the reference's own CUDA build (oracle/_ref) through its own Python
 API on one GPU (rank 0), same workload and extras; the reference has no CPU rasterizer.
+--dump-outputs DIR writes what the last timed step computed (rank 0): colour, aux maps and radii of every
+view and the summed parameter gradients, as DIR/<name>.npy (float32).  An array of more than 2^20
+elements is stored as a fixed, seeded sample of 2^20 of its elements (flattened, in index order).
 """
 from __future__ import annotations
 
@@ -73,7 +76,12 @@ def parse_args():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the extra configurations (C2, C4, strong point, sustained)")
     ap.add_argument("--streams", type=int, default=1, help="ignored (the views of a step share one launch set)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32, at most ~25 MB)")
+    args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes this package's outputs; it cannot be combined with --impl reference")
+    return args
 
 
 class ClockSampler:
@@ -149,7 +157,7 @@ def timed_steps(step_fn, steps, warmup, flush, world, dev):
     starts = [torch.cuda.Event(enable_timing=True) for _ in range(steps)]
     ends = [torch.cuda.Event(enable_timing=True) for _ in range(steps)]
     for i in range(steps):
-        flush.zero_()               # evict the previous step's working set from the 126 MB L2
+        flush.zero_()               # evict the previous step's working set from the 50 MB L2
         starts[i].record()
         step_fn()
         ends[i].record()
@@ -215,7 +223,8 @@ def make_batched_step(wl, grads, all_reduce=True, coll_events=None):
 
     def step():
         grads.zero_()
-        sharded.render_views(wl.params, wl.sets, None, grads=grads, view_ids=wl.ids, cams=packed, upstream_stacked=G)
+        step.outs, _ = sharded.render_views(wl.params, wl.sets, None, grads=grads, view_ids=wl.ids, cams=packed,
+                                            upstream_stacked=G)
         if all_reduce:
             if coll_events is not None:
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -224,6 +233,24 @@ def make_batched_step(wl, grads, all_reduce=True, coll_events=None):
             else:
                 grads.all_reduce()
     return step
+
+
+DUMP_MAX_ELEMS = 1 << 20
+
+
+def dump_outputs(out_dir, outs, grads):
+    """Per-view colour / aux maps / radii and the parameter gradients of one batched step, as float32 .npy files."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"color": torch.stack([o[0] for o in outs]), "allmap": torch.stack([o[1] for o in outs]),
+              "radii": torch.stack([o[2] for o in outs])}
+    arrays.update({"grad_" + k: v for k, v in grads.views.items()})
+    for name, t in arrays.items():
+        a = t.detach().to(torch.float32).cpu().numpy()
+        if a.size > DUMP_MAX_ELEMS:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, DUMP_MAX_ELEMS, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def make_dropin_step(wl, mod, host_io=None, world=1):
@@ -385,15 +412,15 @@ def run_reference(args, rank, local, world):
                                                           "views_per_scene": 8, "note": "timed on one scene (8 views), step time scaled to 8 scenes"}
         v, m = measure(args.P, args.size, 8, max(3, args.steps // 2), 3)
         extra["strong_8_global_views"] = {"value": v, "unit": UNIT, "ms_per_step": m, "views_per_step": 8,
-                                          "note": "the reference is single-GPU: all 8 views on one B200"}
+                                          "note": "the reference is single-GPU: all 8 views on one GPU"}
     base.update({
         "value": value, "ms_per_step": ms_step,
         "config": {"workload": workload_string(args.P, args.size, args.views),
-                   "api_level": "reference's GaussianRasterizer + autograd, one view per call, inputs resident, 1 B200",
+                   "api_level": "reference's GaussianRasterizer + autograd, one view per call, inputs resident, 1 GPU",
                    "views_per_gpu": args.views, "l2": "flushed between steps (256 MiB write, untimed)"},
         "clocks": clocks,
         "cpu_baseline": {"value": value, "unit": UNIT, "cores": os.cpu_count(), "kind": "reference",
-                         "sample": "reference's own CUDA rasterizer (oracle/_ref) on 1 B200 -- the reference ships no CPU rasterizer"},
+                         "sample": "reference's own CUDA rasterizer (oracle/_ref) on 1 GPU -- the reference ships no CPU rasterizer"},
         "e2e": {"value": value, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "extra": extra,
     })
@@ -439,6 +466,8 @@ def main():
     if sampler:
         sampler.start()
     ms, spread = timed_steps(step, args.steps, 0, flush, world, dev)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, step.outs, grads)
     value = total_views * args.steps / (ms / 1e3)
     collective_us = None
     rank_compute_ms = None
@@ -524,7 +553,7 @@ def main():
                                               "views_per_gpu": 8 // world, "scaling": "strong"}
             del wls, gs
         # sustained: the main step back to back for >= 2 s, timed as one region (no L2 flush: the per-step working set
-        # of 8 views' state is several times the 126 MB L2)
+        # of 8 views' state is several times the 50 MB L2)
         n_sus = max(10, int(2.5 / (ms / 1e3 / args.steps)))
         torch.cuda.synchronize(dev)
         if world > 1:
@@ -575,37 +604,18 @@ def main():
         alg_bytes = 148 * r_eff + 64 * npix * nv          # K7: (76+72)*R_eff + 64*Npix per view  (SURVEY 8d), all views of the launch
         tot_ms, n_launch = kern["render_bwd"]
         dur_s = tot_ms / 1e3 / max(n_launch, 1)
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "H100 SXM data sheet (HBM3), not measured"
         try:
             with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
                 peak = float(json.load(f)["hbm_gbs"]); peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-        traffic = warp_inst = None
-        try:
-            with open(os.path.join(ROOT, "profiles", "roofline_traffic.json")) as f:
-                if args.P == 131072 and args.size == 512:      # the capture is of the default workload only
-                    j = json.load(f)
-                    # the capture is of one kernel variant: a different one running now has no ncu figures
-                    if int(j.get("bwd_variant", -1)) == _lib.select_bwd_variant(0):
-                        traffic = j.get("render_bwd_dram_bytes_per_view")
-                        if traffic is not None:
-                            traffic = traffic * nv
-                        warp_inst = j.get("render_bwd_warp_instructions_per_view")
-        except Exception:
-            pass
         achieved = alg_bytes / dur_s / 1e9
-        sm_mhz = (clocks or {}).get("sm_mhz") or 1965.0
-        issue = None
-        if warp_inst is not None:
-            slots = 148 * 4 * sm_mhz * 1e6 * dur_s          # SMs x schedulers x clock x time
-            issue = {"bound": "issue", "warp_instructions_per_launch": warp_inst * nv, "issue_slots": slots,
-                     "frac": warp_inst * nv / slots, "source": "ncu smsp__inst_executed.sum of profiles/ (per view) x views per launch"}
         roof = {"kernel": "render_bwd_kernel", "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
+                "frac": achieved / peak, "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": alg_bytes, "views_per_launch": nv, "R": R_views, "R_eff": r_eff_views,
-                "avg_launch_us": dur_s * 1e6, "issue": issue,
-                "note": "the blend kernels are fp32-issue bound, not HBM bound (DESIGN.md); per-kernel us per view in 'kernels_us'"}
+                "avg_launch_us": dur_s * 1e6,
+                "note": "per-kernel us per view in 'kernels_us'"}
 
     if rank == 0:
         nv = len(my_ids)

@@ -1,4 +1,4 @@
-/* surfel_rasterizer.h -- C ABI of the B200-native 2D-Gaussian-surfel rasterizer.
+/* surfel_rasterizer.h -- C ABI of the H100-native (sm_90a) 2D-Gaussian-surfel rasterizer.
  *
  * Drop-in boundary for LaRa's third_party/diff-surfel-rasterization ("DSR").  The
  * reference crosses Python -> native at three pybind entry points

@@ -1,4 +1,4 @@
-"""lara_b200 -- B200-native 2D-Gaussian-surfel rasterizer (drop-in for LaRa's
+"""lara_b200 -- H100-native (sm_90a) 2D-Gaussian-surfel rasterizer (drop-in for LaRa's
 ``diff_surfel_rasterization``).  Importable without a GPU; any use of the rasterizer
 requires the in-tree CUDA library ``libsurfel_b200.so`` (``python -m lara_b200.build``)."""
 from .rasterizer import (  # noqa: F401

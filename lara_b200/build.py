@@ -2,7 +2,7 @@
 
 Plain ``nvcc`` command lines (no torch, no setuptools): the library has no
 dependency on libtorch -- it takes raw device pointers and a ``cudaStream_t``.
-sm_100a only: ``-gencode arch=compute_100a,code=sm_100a``, ``-lineinfo`` so ncu's
+sm_90a only (H100): ``-gencode arch=compute_90a,code=sm_90a``, ``-lineinfo`` so ncu's
 source page maps to the .cu files, nvcc's default ``-fmad=true`` and *no*
 ``--use_fast_math`` (the integer-critical float chains are pinned with explicit
 intrinsics anyway, see csrc/surfel_common.cuh).
@@ -24,7 +24,7 @@ LIB = os.path.join(HERE, "libsurfel_b200.so")
 SOURCES = ["api.cu", "preprocess.cu", "binning.cu", "render_fwd.cu", "render_bwd.cu", "render_bwd_v1.cu", "preprocess_bwd.cu", "epilogue.cu", "loss.cu", "decoder.cu"]
 HEADERS = ["surfel_common.cuh", "surfel_kernels.h", os.path.join("..", "..", "include", "surfel_rasterizer.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
 ]
@@ -63,7 +63,7 @@ def build(force: bool = False, verbose: bool = True, ptxas_info: bool = False) -
 
     with ThreadPoolExecutor(max_workers=min(len(SOURCES), os.cpu_count() or 1)) as ex:
         objs = list(ex.map(compile_one, SOURCES))
-    cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+    cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"]
     if verbose:
         print("[lara_b200.build]", " ".join(cmd), flush=True)
     subprocess.run(cmd, check=True)

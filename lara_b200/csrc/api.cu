@@ -131,11 +131,11 @@ int sm_count() {
     // per device: a process may drive several GPUs
     static int cache[64] = {0};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
     if (cache[dev] == 0) {
         int n = 0;
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        cache[dev] = n > 0 ? n : 148;
+        cache[dev] = n > 0 ? n : 132;
     }
     return cache[dev];
 }

@@ -321,7 +321,7 @@ __global__ void __launch_bounds__(256) preprocess_fwd_kernel(PreprocessArgs a) {
             cullq.z = __uint_as_float(*reinterpret_cast<unsigned*>(&hb[2]));
             cullq.w = __uint_as_float(*reinterpret_cast<unsigned*>(&hb[3]));
             float4* r = a.rec + (size_t)idx * SRF_REC_QUADS;
-            r[0] = make_float4(Tux, Tvx, Tuy, Tvy);     // (Tu.c, Tv.c) interleaved: fp32x2 operands of eval_pair()
+            r[0] = make_float4(Tux, Tvx, Tuy, Tvy);     // (Tu.c, Tv.c) interleaved: f32x2 operands of eval_pair()
             r[1] = make_float4(Tuz, Tvz, Twx, Twy);
             r[2] = make_float4(Twz, cxs, cys, opac);
             r[3] = make_float4(nx, ny, nz, pvz);

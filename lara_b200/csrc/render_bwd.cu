@@ -27,7 +27,7 @@
 // narrow band around the forward's decision thresholds (eval_pair_bwd below).
 // What is kept from round 1: tiles in LPT order (the default variant runs one 4-warp CTA per 16x8 half tile, five per
 // SM), the list walked back to front from the tile's deepest used entry in staged rounds, warp-level octagon cull,
-// packed fp32x2 arithmetic, MUFU.RCP.
+// paired fp32 arithmetic, MUFU.RCP.
 #include "surfel_common.cuh"
 #include "surfel_kernels.h"
 
@@ -48,7 +48,7 @@ __device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float 
 }
 
 __device__ __forceinline__ f32x2 shfl_xor2(f32x2 v, int m) {
-    return (f32x2)__shfl_xor_sync(0xffffffffu, (unsigned long long)v, m);
+    return make_float2(__shfl_xor_sync(0xffffffffu, v.x, m), __shfl_xor_sync(0xffffffffu, v.y, m));
 }
 
 // explicit 32-bit shared-memory addressing for the phase-1 loop (SADDR): with pointer-typed accesses the compiler
@@ -228,11 +228,11 @@ __global__ void __launch_bounds__(NW * 32, MINB) render_bwd_kernel(RenderBwdArgs
     for (int w = 0; w < NW; ++w) n_eff = max(n_eff, s_wmax[w]);
     const int rounds = (n_eff + BATCH - 1) / BATCH;
 
-    // accum_rec / last_* recursions of backward.cu:331-385, two channels per packed fp32x2 register:
+    // accum_rec / last_* recursions of backward.cu:331-385, two channels per f32x2 pair:
     // (c0,c1) (c2,depth) (n0,n1) (n2,alpha); the matching upstream gradients are paired the same way
     // (the reference keeps the previous splat in last_* and folds it in at the top of the next iteration;
     //  folding it in at the bottom of its own iteration is the same arithmetic and needs no such state)
-    f32x2 acc_c01 = 0ull, acc_c2d = 0ull, acc_n01 = 0ull, acc_n2a = 0ull;
+    f32x2 acc_c01 = zero2(), acc_c2d = zero2(), acc_n01 = zero2(), acc_n2a = zero2();
     const f32x2 r_dpix01 = pk2(dpix0, dpix1), r_dpix2d = pk2(dpix2, dL_ddepth);
     const f32x2 r_dn01 = pk2(dn0, dn1), r_dn2a = pk2(dn2, dL_daccum);
     float last_dL_dT = 0.f;
@@ -468,7 +468,7 @@ __global__ void __launch_bounds__(NW * 32, MINB) render_bwd_kernel(RenderBwdArgs
                 const float nopac = -q2.w;
                 // accumulators, laid out as the gradient record: (DT0,DT1) (DT2,DT3) (DT4,DT5) (DT6,DT7) (DT8,DOPAC)
                 // (DN0,DN1) (DN2,DC0) (DC1,DC2) (DM0,DM1)
-                f32x2 A0 = 0ull, A1 = 0ull, A2 = 0ull, A3 = 0ull, A4 = 0ull, A5 = 0ull, A6 = 0ull, A7 = 0ull, A8 = 0ull;
+                f32x2 A0 = zero2(), A1 = zero2(), A2 = zero2(), A3 = zero2(), A4 = zero2(), A5 = zero2(), A6 = zero2(), A7 = zero2(), A8 = zero2();
                 const float* xrow = s_xw + own * 32;
                 const float ybase = by0 + (P2WALK >= 2 ? 0.0f : (float)(2 * p2_h));
                 const int pbase = wid * 32 + (P2WALK >= 2 ? 0 : 16 * p2_h);
@@ -601,26 +601,26 @@ cudaError_t launch_render_bwd(const RenderBwdArgs& a, cudaStream_t stream) {
     cudaError_t e = cudaSuccess;
     // <splats per round, warps per CTA, CTAs per SM, exact pair evaluation, phase-2 walk, upstream gradients from smem,
     //  list-entry prefetch, explicit shared addressing in phase 1, pixel centre pinned in registers>
-    // us per view at the north-star point in profiles/bwd_variants_r02.log; 2..8 are the fixed phase-2 layouts of the
-    // first two-phase kernel (7 was its default), 9..17 the steps from there to the default.
+    // 2..8 are the fixed phase-2 layouts of the first two-phase kernel, 9..17 the steps from there to the default; compare
+    // them with SRF_BWD_VARIANT=<n> python bench.py (kernels_us.render_bwd).
     switch (variant) {
         case 2: e = launch_variant<256, 8, 2, false, 1, false>(a, stream); break;      // one CTA per tile, own-half phase-2 lanes
         case 3: e = launch_variant<160, 8, 3, false, 1, true>(a, stream); break;       // three CTAs per SM
         case 4: e = launch_variant<256, 8, 2, false, 0, false>(a, stream); break;      // lock-step phase 2
         case 5: e = launch_variant<256, 8, 2, true, 1, false>(a, stream); break;       // exact pair evaluation everywhere
         case 6: e = launch_variant<256, 4, 4, false, 1, false>(a, stream); break;      // half-tile CTAs
-        case 7: e = launch_variant<256, 4, 4, false, 2, false>(a, stream); break;      // half-tile CTAs, shared phase-2 lanes (318 us)
+        case 7: e = launch_variant<256, 4, 4, false, 2, false>(a, stream); break;      // half-tile CTAs, shared phase-2 lanes
         case 8: e = launch_variant<256, 8, 2, false, 2, false>(a, stream); break;      // one CTA per tile, shared phase-2 lanes
-        case 9: e = launch_variant<256, 4, 4, false, 3, false>(a, stream); break;      // 7 + phase-2 lanes in proportion to work (274 us)
+        case 9: e = launch_variant<256, 4, 4, false, 3, false>(a, stream); break;      // 7 + phase-2 lanes in proportion to work
         case 10: e = launch_variant<256, 8, 2, false, 3, false>(a, stream); break;     // the same, one CTA per tile
         case 11: e = launch_variant<128, 4, 5, false, 3, true>(a, stream); break;      // five half-tile CTAs per SM, upstream grads from smem
-        case 12: e = launch_variant<128, 4, 5, false, 3, false>(a, stream); break;     // five half-tile CTAs per SM (267 us)
+        case 12: e = launch_variant<128, 4, 5, false, 3, false>(a, stream); break;     // five half-tile CTAs per SM
         case 13: e = launch_variant<64, 4, 6, false, 3, true>(a, stream); break;       // six CTAs per SM, 64-splat rounds
         case 14: e = launch_variant<128, 8, 3, false, 3, true>(a, stream); break;      // six CTAs' worth of warps as three 8-warp CTAs
-        case 15: e = launch_variant<128, 4, 5, false, 2, false>(a, stream); break;     // five CTAs per SM WITHOUT the allotment (325 us)
+        case 15: e = launch_variant<128, 4, 5, false, 2, false>(a, stream); break;     // five CTAs per SM WITHOUT the allotment
         case 16: e = launch_variant<128, 4, 5, false, 3, false, true>(a, stream); break;        // 12 + prefetch
         case 17: e = launch_variant<128, 4, 5, false, 3, false, true, true>(a, stream); break;  // 16 + explicit shared addressing
-        default: e = launch_variant<128, 4, 5, false, 3, false, true, true, true>(a, stream); break;   // 18: 17 + pinned pixel centre (262 us)
+        default: e = launch_variant<128, 4, 5, false, 3, false, true, true, true>(a, stream); break;   // 18: 17 + pinned pixel centre
     }
     prof_stop(K_RENDER_BWD, stream);
     return e != cudaSuccess ? e : cudaGetLastError();

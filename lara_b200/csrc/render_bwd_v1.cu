@@ -122,10 +122,10 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 768 / SRF_CTA_THREADS) render
     for (int w = 0; w < SRF_CTA_WARPS; ++w) n_eff = max(n_eff, s_wmax[w]);
     const int rounds = (n_eff + SRF_BATCH - 1) / SRF_BATCH;
 
-    // accum_rec / last_* recursions of backward.cu:331-385, two channels per packed fp32x2 register:
+    // accum_rec / last_* recursions of backward.cu:331-385, two channels per f32x2 pair:
     // (c0,c1) (c2,depth) (n0,n1) (n2,alpha); the matching upstream gradients are paired the same way
-    f32x2 acc_c01 = 0ull, acc_c2d = 0ull, acc_n01 = 0ull, acc_n2a = 0ull;
-    f32x2 last_c01 = 0ull, last_c2d = 0ull, last_n01 = 0ull, last_n2a = 0ull;
+    f32x2 acc_c01 = zero2(), acc_c2d = zero2(), acc_n01 = zero2(), acc_n2a = zero2();
+    f32x2 last_c01 = zero2(), last_c2d = zero2(), last_n01 = zero2(), last_n2a = zero2();
     float last_alpha = 0.f;
     const f32x2 dpix01 = pk2(dpix0, dpix1), dpix2d = pk2(dpix2, dL_ddepth);
     const f32x2 dn01 = pk2(dn0, dn1), dn2a = pk2(dn2, dL_daccum);

@@ -54,8 +54,8 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
     bool done = !inside;
     float T = 1.0f;
     uint32_t contributor = 0, last_contributor = 0;
-    // accumulators, two per packed fp32x2 register: (C0,C1) (C2,distortion) (N0,N1) (N2,D) (dist1,dist2)
-    f32x2 C01 = 0ull, C2r = 0ull, N01 = 0ull, N2D = 0ull, d12 = 0ull;
+    // accumulators, two per f32x2 pair: (C0,C1) (C2,distortion) (N0,N1) (N2,D) (dist1,dist2)
+    f32x2 C01 = zero2(), C2r = zero2(), N01 = zero2(), N2D = zero2(), d12 = zero2();
     float median_depth = 0.f, median_weight = 0.f;
     // 1-based list position of the median contributor, 0 = none.  (The reference keeps a float
     // initialised to -1 and converts it to u32 at the end -- 0 after saturation; for tiles with an
@@ -142,7 +142,7 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
                 median_contributor = contributor;
             }
             // every channel: acc = fma(T, channel * alpha, acc) -- the reference's rounding sequence,
-            // two channels per FMUL2 / FFMA2
+            // two channels per mul2 / fma2 pair
             const f32x2 a2 = bc2(alpha), T2 = bc2(T);
             fma2_acc(C01, T2, mul2(pk2(q4.x, q4.y), a2));
             fma2_acc(C2r, T2, mul2(pk2(q4.z, err), a2));

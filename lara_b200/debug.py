@@ -1,7 +1,7 @@
 """Views into the forward's workspaces (for tests and tooling).
 
 The reference's opaque blobs can be parsed with the layout in
-``rasterizer_impl.cu:155-194``; this is the equivalent for the B200 layout, driven by
+``rasterizer_impl.cu:155-194``; this is the equivalent for this package's layout, driven by
 ``srf_state_layout`` so the offsets never go stale.
 """
 from __future__ import annotations

@@ -152,9 +152,9 @@ def _take_readback(device: torch.device, words: int):
                 return free.pop(k)
     slot = torch.zeros(max(words, _SLOT_WORDS), dtype=torch.int32).pin_memory()
     # Spinning wait (cudaEventSynchronize without cudaEventBlockingSync).  Whoever resolves a count waits at most for the
-    # tile scan of that forward, and the thread has nothing else to do meanwhile.  A sleeping wait costs a wake-up: with 8
-    # ranks on one box some rank wakes ~0.2 ms late every step, its GPU runs dry and all ranks wait for it at the
-    # all-reduce (measured: 14 979 vs 15 460 views/s on 8 B200s).  SRF_BLOCKING_EVENT_WAIT=1 restores the sleeping wait.
+    # tile scan of that forward, and the thread has nothing else to do meanwhile.  A sleeping wait costs a wake-up: with several
+    # ranks on one machine some rank wakes late every step, its GPU runs dry and all ranks wait for it at the
+    # all-reduce.  SRF_BLOCKING_EVENT_WAIT=1 restores the sleeping wait.
     ev = torch.cuda.Event(blocking=os.environ.get("SRF_BLOCKING_EVENT_WAIT", "0") == "1")
     ev.record()          # materialises the cudaEvent_t so that the C entry point can record it between its two stages
     return slot, ev

@@ -3,9 +3,9 @@
 The reference class does three things per view: activations (``renderer_2dgs.py:183-188``), the
 rasterizer call (``:209-218``) and ~12 torch ops of post-processing (``:220-268``).  This class
 keeps the constructor, ``set_bg_color``, ``set_rasterizer`` and the ``render_img`` signature /
-returned dict, but runs the B200 rasterizer and the fused epilogue (``lara_b200.epilogue``).  It is
+returned dict, but runs this package's rasterizer and the fused epilogue (``lara_b200.epilogue``).  It is
 an *additional* entry point: LaRa's own ``renderer_2dgs.py`` keeps working unchanged on top of the
-drop-in ``diff_surfel_rasterization`` package; a maintainer who wants the extra ~0.75 ms per view
+drop-in ``diff_surfel_rasterization`` package; a maintainer who wants the fused epilogue's saving per view
 replaces ``from lightning.renderer_2dgs import Renderer`` by ``from lara_b200.renderer import Renderer``.
 """
 from __future__ import annotations

@@ -1,23 +1,23 @@
 """Build recipe for ``oracle/_ref`` -- TEST INFRASTRUCTURE ONLY, never shipped.
 
 Compiles the *unmodified* reference rasterizer (LaRa's
-``third_party/diff-surfel-rasterization``) from the sources where they lie under
-``/root/reference`` into ``oracle/_ref/diff_surfel_rasterization/`` so that
+``third_party/diff-surfel-rasterization``) from the LaRa checkout at ``REF_ROOT``
+(``LARA_REFERENCE_ROOT`` overrides it) into ``oracle/_ref/diff_surfel_rasterization/``
+so that
 
-  * ``tests/`` (``-m gpu``) can check the product kernels against the real
-    reference on the same B200, bit-exactly for tile/sort indices, and
+  * ``tests/golden/make_reference_records.py`` can record what the real reference
+    computes for the GPU parity tests (they read the records, not this build), and
   * ``bench.py --impl reference`` can time the reference's own CUDA build.
 
-Nothing under ``lara_b200/`` imports this.  ``oracle/_ref/`` is git-ignored (it
-never enters history) but not gpurun-ignored (it travels to the GPU box, where
-``/root/reference`` does not exist).
+Nothing under ``lara_b200/`` imports this.  ``oracle/_ref/`` is build output and
+git-ignored.
 
 The recipe is our own (plain nvcc / g++ command lines, no use of the
 reference's setup.py or CMake).  One extra flag is needed with gcc-13:
 ``-include cstdint`` (``rasterizer_impl.h:24`` uses ``std::uintptr_t`` without
-including it).  Device code is built for ``compute_100 / sm_100`` with nvcc's
+including it).  Device code is built for ``compute_90 / sm_90`` with nvcc's
 default optimisation and *no* fast-math -- what the reference's own
-``setup.py:22-30`` would produce with ``TORCH_CUDA_ARCH_LIST=10.0``.
+``setup.py:22-30`` would produce with ``TORCH_CUDA_ARCH_LIST=9.0``.
 """
 from __future__ import annotations
 
@@ -87,7 +87,7 @@ def build(verbose: bool = True) -> str:
             return obj
         if src.endswith(".cu"):
             cmd = [nvcc, "-c", path, "-o", obj, "-std=c++17",
-                   "-gencode=arch=compute_100,code=sm_100",
+                   "-gencode=arch=compute_90,code=sm_90",
                    "-D__CUDA_NO_HALF_OPERATORS__", "-D__CUDA_NO_HALF_CONVERSIONS__",
                    "-D__CUDA_NO_BFLOAT16_CONVERSIONS__", "-D__CUDA_NO_HALF2_OPERATORS__",
                    "--expt-relaxed-constexpr", "-include", "cstdint",

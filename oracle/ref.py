@@ -1,8 +1,9 @@
 """Loader + state parser for the reference build in ``oracle/_ref`` (built by
-``oracle/build_ref.py`` from /root/reference; git-ignored, shipped to the GPU box).
+``oracle/build_ref.py`` from a LaRa checkout; git-ignored build output).
 
-TEST INFRASTRUCTURE ONLY: used by ``tests/`` (-m gpu parity against the real reference)
-and by ``bench.py --impl reference``.  Never imported by lara_b200/.
+TEST INFRASTRUCTURE ONLY: used by ``tests/golden/make_reference_records.py`` (records of the
+real reference for the GPU parity tests) and by ``bench.py --impl reference``.  Never imported
+by lara_b200/.
 """
 from __future__ import annotations
 
@@ -27,7 +28,7 @@ def load():
     if MODNAME in sys.modules:
         return sys.modules[MODNAME]
     if not available():
-        raise ImportError("oracle/_ref is not built (python oracle/build_ref.py needs /root/reference)")
+        raise ImportError("oracle/_ref is not built (LARA_REFERENCE_ROOT=<LaRa checkout> python oracle/build_ref.py)")
     spec = importlib.util.spec_from_file_location(
         MODNAME, os.path.join(PKG, "__init__.py"), submodule_search_locations=[PKG])
     mod = importlib.util.module_from_spec(spec)

@@ -7,7 +7,7 @@
  * Parity pinning: the reference (LaRa third_party/diff-surfel-rasterization, "DSR")
  * ships no tests, fixtures or golden vectors for this path (SURVEY.md 8c).  This oracle is
  * therefore pinned against golden input/output vectors produced by running the reference's
- * own CUDA build (oracle/_ref) on a B200: tests/golden/ + tests/golden/make_golden.py.
+ * own sm_100 CUDA build on a B200: tests/golden/ + tests/golden/make_golden.py.
  *
  * Plain C, fp32 with fmaf() placed exactly where nvcc fused the reference's expressions
  * (compile with -ffp-contract=off), so everything except rsqrt/exp (approximate units on

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 @pytest.fixture(scope="session")
@@ -25,11 +25,3 @@ def cuda_device():
         pytest.skip("no CUDA device")
     return torch.device("cuda:0")
 
-
-@pytest.fixture(scope="session")
-def reference():
-    """The unmodified reference build (oracle/_ref); tests that need it skip if it is absent."""
-    from oracle import ref as REF
-    if not REF.available():
-        pytest.skip("oracle/_ref not built (needs /root/reference at build time)")
-    return REF.load()

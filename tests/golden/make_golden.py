@@ -1,13 +1,15 @@
 """Generate the golden fixtures in tests/golden/*.npz by running the UNMODIFIED reference
-rasterizer (oracle/_ref, built from /root/reference by oracle/build_ref.py) on a B200.
+rasterizer (oracle/_ref, built by oracle/build_ref.py).  The committed files were made with the reference's
+sm_100 build on a B200; this package reproduces them bit for bit (its fp32 operation order is that build's).
 
-    gpurun -- python tests/golden/make_golden.py        # writes gpurun_out/golden/*.npz
-    cp gpurun_out/golden/*.npz tests/golden/
+    python tests/golden/make_golden.py OUT_DIR
+    cp OUT_DIR/*.npz tests/golden/
 
 The reference ships no fixtures for this path (SURVEY.md 8c), so these files are what
 pins the CPU oracle (tests/test_oracle_golden.py) and, on the GPU, the product.  Each
-file holds the inputs, the reference's outputs, its internal state (radii, tiles_touched,
-sorted point list, tile ranges, n_contrib) and its gradients for fixed upstream grads.
+file holds the case name, the camera, the reference's outputs, its internal state (radii, tiles_touched,
+sorted point list, tile ranges, n_contrib) and its gradients for fixed upstream grads; the scene and the upstream
+grads are regenerated from their seeds (tests/helpers.load_golden).
 Gradients use fp32 atomics in the reference and therefore carry run-to-run noise at the
 1e-6 relative level; `grad_noise` records the measured ref-vs-ref difference.
 """
@@ -57,8 +59,11 @@ def case_inputs(name: str):
 CASES = ["basic_sh1", "ragged_sh3", "culled_ties_sh0"]
 
 
-def main():
-    out_dir = os.path.join(ROOT, "gpurun_out", "golden")
+def upstream_grads_for(cam):
+    return S.upstream_grads(cam.image_height, cam.image_width, 7)
+
+
+def main(out_dir):
     os.makedirs(out_dir, exist_ok=True)
     ref = REF.load()
     dev = torch.device("cuda:0")
@@ -68,7 +73,7 @@ def main():
         scd = {k: (v.to(dev) if isinstance(v, torch.Tensor) else v) for k, v in sc.items()}
         st = S.settings_for(cam, bg, sc["sh_degree"], dev, ref.GaussianRasterizationSettings)
         r = REF.forward_raw(ref, scd, st)
-        gc, ga = S.upstream_grads(H, W, 7)
+        gc, ga = upstream_grads_for(cam)
 
         def grads():
             leaves = {k: scd[k].clone().requires_grad_(True) for k in ("means3D", "shs", "opacities", "scales", "rotations")}
@@ -86,12 +91,11 @@ def main():
         vis = (r["radii"] > 0).cpu().numpy()
         np.savez_compressed(
             os.path.join(out_dir, name + ".npz"),
-            # inputs
-            means3D=sc["means3D"].numpy(), scales=sc["scales"].numpy(), rotations=sc["rotations"].numpy(),
-            opacities=sc["opacities"].numpy(), shs=sc["shs"].numpy(), sh_degree=np.int32(sc["sh_degree"]),
+            # inputs (the scene and the upstream grads follow from `case`)
+            case=np.str_(name), sh_degree=np.int32(sc["sh_degree"]),
             viewmatrix=cam.viewmatrix.numpy(), projmatrix=cam.projmatrix.numpy(), campos=cam.campos.numpy(),
             tanfovx=np.float64(cam.tanfovx), tanfovy=np.float64(cam.tanfovy), H=np.int32(H), W=np.int32(W),
-            bg=bg.numpy(), grad_color=gc.numpy(), grad_allmap=ga.numpy(),
+            bg=bg.numpy(),
             # reference outputs and state
             color=r["color"].cpu().numpy(), allmap=r["allmap"].cpu().numpy(), radii=r["radii"].cpu().numpy(),
             num_rendered=np.int64(r["num_rendered"]), tiles_touched=r["tiles_touched"].cpu().numpy(),
@@ -109,4 +113,4 @@ def main():
 
 
 if __name__ == "__main__":
-    main()
+    main(sys.argv[1])

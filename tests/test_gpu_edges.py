@@ -2,12 +2,14 @@
 SURVEY.md section 7 lists): empty input, everything culled, one splat covering every tile,
 thousands of instances in one tile (shared-memory and global sort paths), tied depths,
 extreme opacities, saturated pixels, capacity overflow re-run, precomputed colours,
-markVisible, non-contiguous inputs."""
+markVisible, non-contiguous inputs.  Where a case is compared with the UNMODIFIED reference, the reference's
+side is recorded in tests/golden/reference/ (record_reference below)."""
 import numpy as np
 import pytest
 import torch
 
-from helpers import rel_err, run_candidate, to_dev
+from helpers import (allmap_records, compare_records, count_record, fingerprint, reference_record, run_candidate, sampled_rel_err, to_dev,
+                     tolerance_record)
 
 pytestmark = pytest.mark.gpu
 
@@ -47,54 +49,134 @@ def test_everything_behind_camera(cuda_device):
         assert float(np.abs(out[k]).max()) == 0.0, k
 
 
-@pytest.mark.parametrize("n_big,expect_min", [(3000, 2049), (20000, 16385), (70000, 65537)])
-def test_huge_splats_cover_every_tile(cuda_device, reference, n_big, expect_min):
-    """> 2048 instances per tile -> 1024-thread shared-memory bucket sort; > 8192 -> in-place global
-    bitonic sort; > 65536 instances in one tile is the SURVEY's stress case."""
+HUGE = [(3000, 2049), (20000, 16385), (70000, 65537)]
+PILEUP = [(2000, 16), (8000, 16), (8000, 48)]
+
+
+def _huge_inputs(n_big):
     from lara_b200 import scene as S
-    from oracle import ref as REF
-    H = W = 64
     sc = S.scene(n_big, 3)
     sc["scales"][:] = 0.6                       # every splat covers the whole image
     sc["opacities"][:] = 0.02
     sc["means3D"] *= 0.2
     sc["means3D"][::7] = sc["means3D"][0]       # exact depth ties, broken by Gaussian index
-    cam = S.cameras(1, H, W, 0)[0]
-    bg = torch.zeros(3)
-    mine = run_candidate(sc, cam, bg, cuda_device, grads=S.upstream_grads(H, W, 1))
-    counts = mine["ranges"][:, 1] - mine["ranges"][:, 0]
-    assert int(counts.max()) >= expect_min
-    scd = to_dev(sc, cuda_device)
-    st = S.settings_for(cam, bg, 1, cuda_device, reference.GaussianRasterizationSettings)
-    r = REF.forward_raw(reference, scd, st)
-    assert mine["num_rendered"] == r["num_rendered"]
-    assert np.array_equal(mine["point_list"], r["point_list"].cpu().numpy())
-    assert np.array_equal(mine["ranges"], r["ranges"].cpu().numpy())
-    assert np.array_equal(mine["n_contrib"][0], r["n_contrib"][0].cpu().numpy())
-    assert np.array_equal(mine["allmap"].view(np.int32), r["allmap"].cpu().numpy().view(np.int32))
-    for k in ("g_means3D", "g_opacities", "g_scales"):
-        assert np.isfinite(mine[k]).all()
+    return sc, S.cameras(1, 64, 64, 0)[0], torch.zeros(3)
 
 
-@pytest.mark.parametrize("n,H", [(2000, 16), (8000, 16), (8000, 48)])
-def test_equal_depth_pileup_is_sorted_and_not_quadratic(cuda_device, reference, n, H):
-    """Every instance of a tile has the SAME depth (the degenerate case of the depth-bucket sort: one bucket holds the
-    whole tile, ranking inside it would be quadratic -- 8192 instances = 65k steps per thread).  The sort falls back to the
-    comparison network; order (by Gaussian index, as the reference's stable sort leaves it) and a time bound are checked."""
-    from lara_b200 import rasterizer as R, scene as S
-    from oracle import ref as REF
+def _pileup_inputs(n, H):
+    from lara_b200 import scene as S
     sc = S.scene(n, 9)
     sc["means3D"][:] = torch.tensor([0.0, 0.0, 0.0])      # all splats at the origin: identical view-space depth
     sc["scales"][:] = 0.5
     sc["opacities"][:] = 0.01
-    cam = S.cameras(1, H, H, 0)[0]
-    bg = torch.zeros(3)
+    return sc, S.cameras(1, H, H, 0)[0], torch.zeros(3)
+
+
+def _opacity_inputs():
+    from lara_b200 import scene as S
+    sc = S.scene(8000, 6)
+    sc["opacities"][0::3] = 1.0        # alpha clamps at 0.99, pixels saturate (early termination)
+    sc["opacities"][1::3] = 1e-5       # never reaches 1/255
+    sc["scales"] *= 3.0
+    return sc, S.cameras(1, 128, 128, 0)[0], torch.full((3,), 0.5)
+
+
+def _colors_precomp_inputs():
+    from lara_b200 import scene as S
+    return S.scene(5000, 8), S.cameras(1, 128, 128, 0)[0], torch.rand(5000, 3, generator=torch.Generator().manual_seed(8))
+
+
+def _mark_visible_inputs():
+    from lara_b200 import scene as S
+    sc = S.scene(10000, 9)
+    sc["means3D"] = sc["means3D"] * 4.0          # some points end up behind the near plane
+    return sc, S.cameras(1, 64, 64, 0)[0]
+
+
+def _forward_fingerprints(r, keys):
+    """Integer state as fingerprints, aux maps and per-pixel counts as samples (helpers.compare_records)."""
+    out = {k: fingerprint(r[k]) for k in keys if k in ("point_list", "ranges")}
+    if "allmap" in keys:
+        out.update(allmap_records(r["allmap"]))
+    if "n_contrib" in keys:
+        out["n_contrib"] = count_record(r["n_contrib"][0])
+    if "num_rendered" in keys:
+        out["num_rendered"] = int(r["num_rendered"])
+    return out
+
+
+def _colors_precomp_run(mod, dev):
+    from lara_b200 import scene as S
+    sc, cam, colors = _colors_precomp_inputs()
+    scd = to_dev(sc, dev)
+    gc, ga = [t.to(dev) for t in S.upstream_grads(128, 128, 0)]
+    st = S.settings_for(cam, torch.ones(3), 1, dev, mod.GaussianRasterizationSettings)
+    c_in = colors.to(dev).requires_grad_(True)
+    m3 = scd["means3D"].clone().requires_grad_(True)
+    rast = mod.GaussianRasterizer(raster_settings=st)
+    c, rd, am = rast(means3D=m3, means2D=torch.zeros_like(m3), colors_precomp=c_in, opacities=scd["opacities"],
+                     scales=scd["scales"], rotations=scd["rotations"])
+    torch.autograd.backward((c, am), (gc, ga))
+    return c.detach().cpu().numpy(), am.detach().cpu().numpy(), c_in.grad.cpu().numpy(), m3.grad.cpu().numpy()
+
+
+def _mark_visible_run(mod, dev):
+    from lara_b200 import scene as S
+    sc, cam = _mark_visible_inputs()
+    st = S.settings_for(cam, torch.ones(3), 1, dev, mod.GaussianRasterizationSettings)
+    return mod.GaussianRasterizer(raster_settings=st).markVisible(sc["means3D"].to(dev)).cpu().numpy()
+
+
+def record_reference(ref, dev):
+    """The reference's side of the comparisons below (tests/golden/make_reference_records.py)."""
+    from lara_b200 import scene as S
+    from oracle import ref as REF
+
+    def forward(sc, cam, bg):
+        st = S.settings_for(cam, bg, 1, dev, ref.GaussianRasterizationSettings)
+        r = REF.forward_raw(ref, to_dev(sc, dev), st)
+        return {k: (v.cpu().numpy() if isinstance(v, torch.Tensor) else v) for k, v in r.items()}
+    out = {}
+    for n_big, _ in HUGE:
+        out[f"huge/{n_big}"] = _forward_fingerprints(forward(*_huge_inputs(n_big)),
+                                                     ("num_rendered", "point_list", "ranges", "n_contrib", "allmap"))
+    for n, H in PILEUP:
+        out[f"pileup/{n}-{H}"] = _forward_fingerprints(forward(*_pileup_inputs(n, H)), ("num_rendered", "point_list"))
+    out["opacity"] = _forward_fingerprints(forward(*_opacity_inputs()), ("n_contrib", "allmap"))
+    color, allmap, g_colors, g_means3D = _colors_precomp_run(ref, dev)
+    out["colors_precomp"] = {"color": tolerance_record(color), **allmap_records(allmap),
+                             "g_colors": tolerance_record(g_colors), "g_means3D": tolerance_record(g_means3D)}
+    out["mark_visible"] = {"visible": fingerprint(_mark_visible_run(ref, dev))}
+    return out
+
+
+@pytest.mark.parametrize("n_big,expect_min", HUGE)
+def test_huge_splats_cover_every_tile(cuda_device, n_big, expect_min):
+    """> 2048 instances per tile -> 1024-thread shared-memory bucket sort; > 8192 -> in-place global
+    bitonic sort; > 65536 instances in one tile is the SURVEY's stress case."""
+    from lara_b200 import scene as S
+    sc, cam, bg = _huge_inputs(n_big)
+    mine = run_candidate(sc, cam, bg, cuda_device, grads=S.upstream_grads(64, 64, 1))
+    counts = mine["ranges"][:, 1] - mine["ranges"][:, 0]
+    assert int(counts.max()) >= expect_min
+    rec = reference_record("test_gpu_edges", f"huge/{n_big}")
+    assert not compare_records(_forward_fingerprints(mine, ("num_rendered", "point_list", "ranges", "n_contrib", "allmap")), rec)
+    for k in ("g_means3D", "g_opacities", "g_scales"):
+        assert np.isfinite(mine[k]).all()
+
+
+@pytest.mark.parametrize("n,H", PILEUP)
+def test_equal_depth_pileup_is_sorted_and_not_quadratic(cuda_device, n, H):
+    """Every instance of a tile has the SAME depth (the degenerate case of the depth-bucket sort: one bucket holds the
+    whole tile, ranking inside it would be quadratic -- 8192 instances = 65k steps per thread).  The sort falls back to the
+    comparison network; order (by Gaussian index, as the reference's stable sort leaves it) and a time bound are checked."""
+    from lara_b200 import rasterizer as R, scene as S
+    sc, cam, bg = _pileup_inputs(n, H)
     mine = run_candidate(sc, cam, bg, cuda_device)
     scd = to_dev(sc, cuda_device)
-    st = S.settings_for(cam, bg, 1, cuda_device, reference.GaussianRasterizationSettings)
-    r = REF.forward_raw(reference, scd, st)
-    assert mine["num_rendered"] == r["num_rendered"] >= n
-    assert np.array_equal(mine["point_list"], r["point_list"].cpu().numpy())
+    rec = reference_record("test_gpu_edges", f"pileup/{n}-{H}")
+    assert mine["num_rendered"] == int(rec["num_rendered"]) >= n
+    assert fingerprint(mine["point_list"]) == rec["point_list"]
     assert len(np.unique(mine["depths"][mine["radii"] > 0].view(np.int32))) == 1
     # time: the whole forward of this tiny image, repeated; a quadratic rank loop takes milliseconds per tile
     stm = S.settings_for(cam, bg, 1, cuda_device, R.GaussianRasterizationSettings)
@@ -128,22 +210,13 @@ def test_sorted_by_depth_then_index_within_each_tile(cuda_device):
     assert total == out["num_rendered"] == int(out["tiles_touched"].sum())
 
 
-def test_opacity_extremes_and_saturation(cuda_device, reference):
+def test_opacity_extremes_and_saturation(cuda_device):
     from lara_b200 import scene as S
-    from oracle import ref as REF
-    sc = S.scene(8000, 6)
-    sc["opacities"][0::3] = 1.0        # alpha clamps at 0.99, pixels saturate (early termination)
-    sc["opacities"][1::3] = 1e-5       # never reaches 1/255
-    sc["scales"] *= 3.0
-    cam = S.cameras(1, 128, 128, 0)[0]
-    bg = torch.full((3,), 0.5)
+    sc, cam, bg = _opacity_inputs()
     gc, ga = S.upstream_grads(128, 128, 2)
     mine = run_candidate(sc, cam, bg, cuda_device, grads=(gc, ga))
-    scd = to_dev(sc, cuda_device)
-    st = S.settings_for(cam, bg, 1, cuda_device, reference.GaussianRasterizationSettings)
-    r = REF.forward_raw(reference, scd, st)
-    assert np.array_equal(mine["n_contrib"][0], r["n_contrib"][0].cpu().numpy())
-    assert np.array_equal(mine["allmap"].view(np.int32), r["allmap"].cpu().numpy().view(np.int32))
+    rec = reference_record("test_gpu_edges", "opacity")
+    assert not compare_records(_forward_fingerprints(mine, ("n_contrib", "allmap")), rec)
     assert float(mine["accum"][0].min()) < 1e-3           # saturated pixels exist
     assert float(np.abs(mine["g_opacities"][1::3]).max()) == 0.0
     for k in ("g_means3D", "g_sh", "g_opacities", "g_scales", "g_rotations"):
@@ -164,42 +237,19 @@ def test_capacity_overflow_reruns_binning(cuda_device, monkeypatch):
     assert np.array_equal(small["allmap"].view(np.int32), base["allmap"].view(np.int32))
 
 
-def test_colors_precomp_path(cuda_device, reference):
-    from lara_b200 import scene as S
+def test_colors_precomp_path(cuda_device):
     import diff_surfel_rasterization as DSR
-    sc = S.scene(5000, 8)
-    cam = S.cameras(1, 128, 128, 0)[0]
-    bg = torch.ones(3)
-    scd = to_dev(sc, cuda_device)
-    colors = torch.rand(5000, 3, device=cuda_device)
-    gc, ga = [t.to(cuda_device) for t in S.upstream_grads(128, 128, 0)]
-    res = []
-    for mod in (DSR, reference):
-        st = S.settings_for(cam, bg, 1, cuda_device, mod.GaussianRasterizationSettings)
-        c_in = colors.clone().requires_grad_(True)
-        m3 = scd["means3D"].clone().requires_grad_(True)
-        rast = mod.GaussianRasterizer(raster_settings=st)
-        c, rd, am = rast(means3D=m3, means2D=torch.zeros_like(m3), colors_precomp=c_in, opacities=scd["opacities"],
-                         scales=scd["scales"], rotations=scd["rotations"])
-        torch.autograd.backward((c, am), (gc, ga))
-        res.append((c.detach().cpu().numpy(), am.detach().cpu().numpy(), c_in.grad.cpu().numpy(), m3.grad.cpu().numpy()))
-    assert np.array_equal(res[0][0].view(np.int32), res[1][0].view(np.int32))     # no SH -> colour bit-exact too
-    assert np.array_equal(res[0][1].view(np.int32), res[1][1].view(np.int32))
-    assert rel_err(res[0][2], res[1][2]) < 1e-4 and rel_err(res[0][3], res[1][3]) < 1e-4
+    color, allmap, g_colors, g_means3D = _colors_precomp_run(DSR, cuda_device)
+    rec = reference_record("test_gpu_edges", "colors_precomp")
+    assert not compare_records({"color": tolerance_record(color), **allmap_records(allmap)}, rec)
+    assert sampled_rel_err(g_colors, rec, "g_colors") < 1e-4 and sampled_rel_err(g_means3D, rec, "g_means3D") < 1e-4
 
 
-def test_mark_visible_matches_reference(cuda_device, reference):
-    from lara_b200 import scene as S
+def test_mark_visible_matches_reference(cuda_device):
     import diff_surfel_rasterization as DSR
-    sc = S.scene(10000, 9)
-    cam = S.cameras(1, 64, 64, 0)[0]
-    sc["means3D"] = sc["means3D"] * 4.0          # some points end up behind the near plane
-    pts = sc["means3D"].to(cuda_device)
-    outs = []
-    for mod in (DSR, reference):
-        st = S.settings_for(cam, torch.ones(3), 1, cuda_device, mod.GaussianRasterizationSettings)
-        outs.append(mod.GaussianRasterizer(raster_settings=st).markVisible(pts).cpu().numpy())
-    assert outs[0].dtype == np.bool_ and np.array_equal(outs[0], outs[1]) and 0 < outs[0].sum() < 10000
+    vis = _mark_visible_run(DSR, cuda_device)
+    rec = reference_record("test_gpu_edges", "mark_visible")
+    assert vis.dtype == np.bool_ and fingerprint(vis) == rec["visible"] and 0 < vis.sum() < 10000
 
 
 def test_non_contiguous_inputs_and_debug_flag(cuda_device):

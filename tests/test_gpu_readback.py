@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import to_dev
+from helpers import reference_record, to_dev
 
 pytestmark = pytest.mark.gpu
 
@@ -25,19 +25,30 @@ def _render(DSR, leaves, st):
                 scales=leaves["scales"], rotations=leaves["rotations"])
 
 
-def test_ctx_num_rendered_is_lazy_and_correct(cuda_device, reference):
+def _lazy_count_inputs():
+    from lara_b200 import scene as S
+    return S.scene(20000, 11), S.cameras(1, 256, 256, 1)[0]
+
+
+def record_reference(ref, dev):
+    """The reference's instance count (tests/golden/make_reference_records.py)."""
+    from lara_b200 import scene as S
+    from oracle import ref as REF
+    sc, cam = _lazy_count_inputs()
+    st = S.settings_for(cam, torch.ones(3), 1, dev, ref.GaussianRasterizationSettings)
+    return {"lazy_count": {"num_rendered": REF.forward_raw(ref, to_dev(sc, dev), st)["num_rendered"]}}
+
+
+def test_ctx_num_rendered_is_lazy_and_correct(cuda_device):
     import diff_surfel_rasterization as DSR
     from lara_b200 import rasterizer as R, scene as S
-    from oracle import ref as REF
-    sc = S.scene(20000, 11)
+    sc, cam = _lazy_count_inputs()
     scd = to_dev(sc, cuda_device)
-    cam = S.cameras(1, 256, 256, 1)[0]
     st = S.settings_for(cam, torch.ones(3), 1, cuda_device, DSR.GaussianRasterizationSettings)
     color, radii, allmap = _render(DSR, _leaves(scd), st)
     n = color.grad_fn.num_rendered                     # the reference stores an int on ctx (DSR __init__.py:95)
     assert isinstance(n, (int, R.LazyCount))
-    ref_st = S.settings_for(cam, torch.ones(3), 1, cuda_device, reference.GaussianRasterizationSettings)
-    assert int(n) == REF.forward_raw(reference, scd, ref_st)["num_rendered"]
+    assert int(n) == int(reference_record("test_gpu_readback", "lazy_count")["num_rendered"])
     assert n == int(n) and f"{n}" == str(int(n))
 
 

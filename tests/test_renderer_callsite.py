@@ -1,45 +1,16 @@
 """The consumer: LaRa's lightning/renderer_2dgs.py must run unchanged on top of this package.
 
-* CPU (only where /root/reference exists, i.e. in the build container): the reference's
-  renderer_2dgs.py is imported *as is* with this repo's `diff_surfel_rasterization` on the path and
-  builds a rasterizer from a MiniCam-like camera.
 * GPU: the call pattern of Renderer.render_img (renderer_2dgs.py:167-268) -- activations,
   zeros+0 screenspace tensor with retain_grad, keyword call, the torch post-processing of the aux
-  maps and a loss -- is replayed with this package and with the reference build; images and the
-  gradients wrt the *raw* network outputs must agree.
+  maps and a loss -- is replayed with this package and compared with the same replay on the reference
+  build (recorded in tests/golden/reference/, see record_reference); images and the gradients wrt the
+  *raw* network outputs must agree.
 """
-import importlib.util
-import os
-import sys
-
 import numpy as np
 import pytest
 import torch
 
-from helpers import rel_err
-
-REF_RENDERER = "/root/reference/lightning/renderer_2dgs.py"
-
-
-@pytest.mark.skipif(not os.path.isfile(REF_RENDERER), reason="/root/reference not present (GPU box)")
-def test_reference_renderer_imports_unchanged_on_cpu():
-    import diff_surfel_rasterization as DSR
-    assert "lara_b200" in DSR.GaussianRasterizer.__module__
-    spec = importlib.util.spec_from_file_location("ref_renderer_2dgs", REF_RENDERER)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)                      # does `from diff_surfel_rasterization import ...`
-    assert mod.GaussianRasterizer is DSR.GaussianRasterizer
-    r = mod.Renderer(sh_degree=1, white_background=True)
-
-    class Cam:
-        FoVx = FoVy = 0.75
-        image_height = image_width = 32
-        world_view_transform = torch.eye(4)
-        full_proj_transform = torch.eye(4)
-        camera_center = torch.zeros(3)
-    rast = r.set_rasterizer(Cam(), device="cpu")
-    assert isinstance(rast, DSR.GaussianRasterizer)
-    assert rast.raster_settings.sh_degree == 1 and rast.raster_settings.image_width == 32
+from helpers import allmap_records, compare_records, fingerprint, reference_record, sampled_rel_err, tolerance_record
 
 
 def _render_img_like(mod, cam, raw, bg, dev):
@@ -70,31 +41,37 @@ def _render_img_like(mod, cam, raw, bg, dev):
     return img, allmap, radii, loss, screenspace
 
 
-@pytest.mark.gpu
-def test_render_img_call_pattern_matches_reference(cuda_device, reference):
-    import diff_surfel_rasterization as DSR
+def _replay(mod, dev):
     from lara_b200 import scene as S
-    dev = cuda_device
-    P = 20000
-    sc = S.scene(P, 11)
+    sc = S.scene(20000, 11)
     cam = S.cameras(2, 160, 160, 3)[1]
-    bg = torch.ones(3)
     base = {"centers": sc["means3D"], "shs": sc["shs"], "opacity": torch.logit(sc["opacities"].clamp(1e-4, 1 - 1e-4)),
             "scales": torch.log(sc["scales"]), "rotations": sc["rotations"] * 1.7}
-    res = []
-    for mod in (DSR, reference):
-        raw = {k: v.to(dev).clone().requires_grad_(True) for k, v in base.items()}
-        with torch.autograd.set_detect_anomaly(True):
-            img, allmap, radii, loss, ss = _render_img_like(mod, cam, raw, bg, dev)
-            loss.backward()
-        res.append((img.detach().cpu().numpy(), allmap.detach().cpu().numpy(), radii.cpu().numpy(),
-                    {k: v.grad.cpu().numpy() for k, v in raw.items()}, ss.grad.cpu().numpy(), float(loss)))
-    a, b = res
-    assert np.array_equal(a[0].view(np.int32), b[0].view(np.int32))
-    assert np.array_equal(a[1].view(np.int32), b[1].view(np.int32))
-    assert np.array_equal(a[2], b[2])
-    assert a[5] == b[5]
-    for k in a[3]:
-        assert np.isfinite(a[3][k]).all()
-        assert rel_err(a[3][k], b[3][k]) < 1e-4, k
-    assert rel_err(a[4], b[4]) < 1e-4        # viewspace (means2D) gradient used for densification statistics
+    raw = {k: v.to(dev).clone().requires_grad_(True) for k, v in base.items()}
+    with torch.autograd.set_detect_anomaly(True):
+        img, allmap, radii, loss, ss = _render_img_like(mod, cam, raw, torch.ones(3), dev)
+        loss.backward()
+    return (img.detach().cpu().numpy(), allmap.detach().cpu().numpy(), radii.cpu().numpy(),
+            {k: v.grad.cpu().numpy() for k, v in raw.items()}, ss.grad.cpu().numpy(), float(loss))
+
+
+def record_reference(ref, dev):
+    """The reference's side of the replay (tests/golden/make_reference_records.py)."""
+    img, allmap, radii, grads, ss, loss = _replay(ref, dev)
+    rec = {"img": tolerance_record(img), **allmap_records(allmap), "radii": fingerprint(radii),
+           "loss": tolerance_record(loss), "screenspace": tolerance_record(ss)}
+    rec.update({"g_" + k: tolerance_record(v) for k, v in grads.items()})
+    return {"render_img": rec}
+
+
+@pytest.mark.gpu
+def test_render_img_call_pattern_matches_reference(cuda_device):
+    import diff_surfel_rasterization as DSR
+    img, allmap, radii, grads, ss, loss = _replay(DSR, cuda_device)
+    rec = reference_record("test_renderer_callsite", "render_img")
+    assert not compare_records({"img": tolerance_record(img), **allmap_records(allmap), "radii": fingerprint(radii),
+                                "loss": tolerance_record(loss)}, rec)
+    for k in grads:
+        assert np.isfinite(grads[k]).all()
+        assert sampled_rel_err(grads[k], rec, "g_" + k) < 1e-4, k
+    assert sampled_rel_err(ss, rec, "screenspace") < 1e-4        # viewspace (means2D) gradient used for densification statistics

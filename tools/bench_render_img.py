@@ -1,7 +1,7 @@
 """Per-view cost of a full Renderer.render_img + loss backward (activations + rasterizer + epilogue):
    (a) the pipeline LaRa runs today: reference rasterizer (oracle/_ref) + torch epilogue,
    (b) drop-in: this repo's rasterizer under the unchanged torch epilogue,
-   (c) lara_b200.renderer.Renderer: B200 rasterizer + fused epilogue, activations in torch,
+   (c) lara_b200.renderer.Renderer: this rasterizer + fused epilogue, activations in torch,
    (d) the same with the activations fused into the preprocess kernels."""
 import os, sys, time, types
 import torch
@@ -47,7 +47,7 @@ def torch_pipeline(mod):
 fast = Renderer(sh_degree=1, white_background=True)
 plain = Renderer(sh_degree=1, white_background=True, fused_activations=False)
 variants = [("reference rasterizer + torch epilogue (LaRa today)", torch_pipeline(ref)),
-            ("B200 rasterizer (drop-in) + torch epilogue", torch_pipeline(DSR)),
+            ("lara_b200 rasterizer (drop-in) + torch epilogue", torch_pipeline(DSR)),
             ("lara_b200.renderer.Renderer, torch activations + fused epilogue",
              lambda raw: plain.render_img(cam, rays, raw["centers"], raw["shs"], raw["opacity"], raw["scales"], raw["rotations"], dev)),
             ("lara_b200.renderer.Renderer, fused activations + fused epilogue",

@@ -75,7 +75,7 @@ def fused_loss_step(raw):
 
 
 variants = [("LaRa today: reference rasterizer, torch activations + epilogue, per-view loop", torch_loop(ref)),
-            ("drop-in B200 rasterizer under the same torch code", torch_loop(DSR)),
+            ("drop-in rasterizer (lara_b200) under the same torch code", torch_loop(DSR)),
             ("Renderer.render_img per view (fused activations + epilogue)", fast_loop),
             ("Renderer.render_views (one launch set), torch loss on the concatenated layout", batched(1)),
             ("Renderer.render_views + fused scene_loss (no concat, one loss kernel each way)", None)]

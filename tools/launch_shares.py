@@ -1,5 +1,5 @@
 """Per-kernel share of an ncu launch list (--metrics gpu__time_duration.sum --csv).
-    python tools/launch_shares.py profiles/launches_bench_r01.csv profiles/launch_shares_r01.json"""
+    python tools/launch_shares.py LAUNCHES.csv OUT.json"""
 import csv, json, sys
 rows = [r for r in csv.reader(open(sys.argv[1], errors="replace")) if len(r) > 5]
 hdr = next(r for r in rows if "Kernel Name" in r)
