@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define SRF_ABI_VERSION 3
+#define SRF_ABI_VERSION 4
 
 /* cudaStream_t without pulling in cuda_runtime.h */
 typedef void* srf_stream_t;
@@ -259,10 +259,6 @@ int srf_decoder_layout_backward(srf_stream_t stream, size_t B, int N, int K, int
 #define SRF_NUM_KERNELS 8
 int srf_profile_begin(void);
 int srf_profile_end(float* ms_out, int* launches_out, int n);
-/* A/B selection of the blend-backward kernel variant for tools/ (same meaning as the SRF_BWD_VARIANT
- * environment variable, which is read once); returns the variant that was selected before.
- * The variants differ in work decomposition, not in arithmetic; lara_b200/csrc/render_bwd.cu lists them. */
-int srf_select_bwd_variant(int variant);
 
 /* ---- markVisible (DSR/rasterize_points.cu:242-261, rasterizer_impl.cu:141-153) ----
  * present[i] = 1 iff the view-space z of means3D[i] is > 0.2 (one byte per Gaussian). */

@@ -13,7 +13,7 @@ from ctypes import POINTER, c_char_p, c_float, c_int, c_size_t, c_void_p
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libsurfel_b200.so")
-ABI_VERSION = 3
+ABI_VERSION = 4
 CAM_FLOATS, CAM_VIEW, CAM_CAMPOS, CAM_BG = 24, 0, 16, 19      # include/surfel_rasterizer.h SRF_CAM_*
 
 # name -> (restype, argtypes); mirrors include/surfel_rasterizer.h one to one
@@ -114,7 +114,6 @@ SIGNATURES = {
     "srf_epilogue_backward": (c_int, [_P, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "srf_profile_begin": (c_int, []),
     "srf_profile_end": (c_int, [POINTER(c_float), POINTER(c_int), c_int]),
-    "srf_select_bwd_variant": (c_int, [c_int]),
 }
 
 _lib = None
@@ -188,11 +187,6 @@ def layout(lib, P: int, H: int, W: int):
 
 KERNEL_NAMES = ["preprocess_fwd", "tile_scan", "scatter", "sort_small", "sort_big", "render_fwd",
                 "render_bwd", "preprocess_bwd"]
-
-
-def select_bwd_variant(variant: int, lib=None) -> int:
-    """Tools only: A/B selection of the blend-backward kernel variant; returns the previous one."""
-    return int((lib or load()).srf_select_bwd_variant(int(variant)))
 
 
 def profile_begin(lib=None) -> None:

@@ -4,10 +4,8 @@
 #include <stdarg.h>
 #include <stdint.h>
 #include <stdio.h>
-#include <stdlib.h>
 #include <string.h>
 
-#include <atomic>
 #include <mutex>
 #include <vector>
 
@@ -113,20 +111,6 @@ void prof_stop(int kernel, cudaStream_t stream) {
     g_spans.push_back(s);
 }
 
-// blend-backward kernel selection: SRF_BWD_VARIANT (read once) or srf_select_bwd_variant() (tools: A/B in one process)
-constexpr int kBwdVariantDefault = 18, kBwdVariantMax = 18;
-static std::atomic<int> g_bwd_variant{0};
-int bwd_variant() {
-    int v = g_bwd_variant.load(std::memory_order_relaxed);
-    if (v == 0) {
-        const char* e = getenv("SRF_BWD_VARIANT");
-        const int x = e ? atoi(e) : kBwdVariantDefault;
-        v = (x >= 1 && x <= kBwdVariantMax) ? x : kBwdVariantDefault;
-        g_bwd_variant.store(v, std::memory_order_relaxed);
-    }
-    return v;
-}
-
 int sm_count() {
     // per device: a process may drive several GPUs
     static int cache[64] = {0};
@@ -144,12 +128,6 @@ int sm_count() {
 extern "C" {
 
 int srf_abi_version(void) { return SRF_ABI_VERSION; }
-
-int srf_select_bwd_variant(int variant) {
-    const int prev = srf::bwd_variant();
-    if (variant >= 1 && variant <= srf::kBwdVariantMax) srf::g_bwd_variant.store(variant, std::memory_order_relaxed);
-    return prev;
-}
 
 int srf_profile_begin(void) {
     std::lock_guard<std::mutex> lk(g_prof_mu);

@@ -40,9 +40,9 @@
 
 #define SRF_NEAR_F 0.2f
 
-// Blend CTAs: a 16x16 tile is eight 8x4 warp blocks; one CTA owns SRF_CTA_WARPS of them (a 16x8 half
-// tile) and walks the tile's list in rounds of SRF_BATCH staged splats (one per thread).  Smaller CTAs
-// wait less at the per-round barriers (the warps of a tile are unevenly loaded).
+// Blend-forward CTAs: a 16x16 tile is eight 8x4 warp blocks; one CTA of SRF_CTA_WARPS = 8 warps owns all
+// of them (the full tile) and walks the tile's list in rounds of SRF_BATCH staged splats (one per thread).
+// The blend backward sizes its CTAs itself (render_bwd.cu).
 #define SRF_CTA_WARPS 8
 #define SRF_CTA_THREADS (SRF_CTA_WARPS * 32)
 #define SRF_BATCH SRF_CTA_THREADS

@@ -195,10 +195,6 @@ enum KernelId { K_PREPROCESS_FWD = 0, K_TILE_SCAN, K_SCATTER, K_SORT_SMALL, K_SO
 void prof_start(int kernel, cudaStream_t stream);
 void prof_stop(int kernel, cudaStream_t stream);
 
-// runtime A/B switch (environment, read once): SRF_BWD_VARIANT = 1 (round-1 reduce-scatter kernel, render_bwd_v1.cu),
-// 2..8 layouts of the two-phase kernel (render_bwd.cu launch_render_bwd); default 7 = half-tile CTAs, 256-splat rounds,
-// approximate pair evaluation with exact re-check, the two phase-2 lanes of a splat share its pixels
-int bwd_variant();
 // number of SMs of the current device (cached per device)
 int sm_count();
 

@@ -71,18 +71,3 @@ def test_missing_library_fails_loudly(tmp_path):
     from lara_b200 import _lib
     with pytest.raises(_lib.SurfelLibraryError):
         _lib.load(str(tmp_path / "nope.so"))
-
-
-def test_bwd_variant_selector_host_only(lib):
-    """srf_select_bwd_variant: out-of-range values only query; a valid one is returned by the next call."""
-    lib.srf_select_bwd_variant.restype = ctypes.c_int
-    lib.srf_select_bwd_variant.argtypes = [ctypes.c_int]
-    cur = lib.srf_select_bwd_variant(0)
-    assert 1 <= cur <= 64
-    assert lib.srf_select_bwd_variant(-3) == cur and lib.srf_select_bwd_variant(10 ** 6) == cur
-    try:
-        assert lib.srf_select_bwd_variant(7) == cur
-        assert lib.srf_select_bwd_variant(0) == 7
-    finally:
-        lib.srf_select_bwd_variant(cur)
-    assert lib.srf_select_bwd_variant(0) == cur

@@ -1,4 +1,4 @@
-"""Lane allotment of phase 2 of the blend backward (render_bwd.cu, P2WALK == 3), replayed lane by lane on the CPU:
+"""Lane allotment of phase 2 of the blend backward (render_bwd.cu), replayed lane by lane on the CPU:
 the warp-level steps of the kernel (shuffles, ballot, inclusive scan, lower bound, drop-the-lowest-k-bits) are
 restated with numpy in the same order and checked for what the kernel relies on -- every contributing
 (splat, pixel) pair is taken by exactly one lane, no lane takes more than C pairs, the lanes suffice, and C is the

@@ -21,7 +21,7 @@ gc, ga = S.upstream_grads(tag["H"], tag["W"], tag["seed"])
 mine = run_candidate(sc, cam, bg, dev, grads=(gc, ga))
 r, g1, g2 = T._reference_state_and_grads(ref, sc, cam, bg, tag["deg"], dev, gc, ga, twice=True)
 errs, worst = T._compare(mine, r, g1, g2, tag["H"], tag["W"])
-print(os.environ.get("SRF_BWD_VARIANT", "2"), tag, "R", mine["num_rendered"], "errs", errs)
+print(tag, "R", mine["num_rendered"], "errs", errs)
 for a_, b_ in T.GRAD_KEYS:
     d = np.abs(mine[a_].astype(np.float64) - g1[b_])
     i = np.unravel_index(np.argmax(d), d.shape)

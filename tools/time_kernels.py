@@ -3,8 +3,7 @@
 
     python tools/time_kernels.py [--P 131072] [--size 512] [--views 8] [--steps 5]
 
-Prints one JSON line: us per VIEW per kernel (launch time / views per launch) and the step time.
-SRF_BWD_VARIANT selects the blend-backward kernel (read once per process)."""
+Prints one JSON line: us per VIEW per kernel (launch time / views per launch) and the step time."""
 import argparse
 import json
 import os
@@ -22,7 +21,6 @@ ap.add_argument("--size", type=int, default=512)
 ap.add_argument("--views", type=int, default=8)
 ap.add_argument("--steps", type=int, default=5)
 ap.add_argument("--sh", type=int, default=1)
-ap.add_argument("--variants", default="", help="comma-separated blend-backward variants to time in this one process")
 args = ap.parse_args()
 
 dev = torch.device("cuda:0")
@@ -43,9 +41,7 @@ def step():
     sharded.render_views(params, sets, None, grads=grads, upstream_stacked=G, cams=packed)
 
 
-def measure(variant):
-    if variant is not None:
-        _lib.select_bwd_variant(variant)
+def measure():
     for _ in range(3):
         step()
     torch.cuda.synchronize()
@@ -61,20 +57,11 @@ def measure(variant):
         st[2 * i].record(); step(); st[2 * i + 1].record()
     torch.cuda.synchronize()
     ms = sum(st[2 * i].elapsed_time(st[2 * i + 1]) for i in range(args.steps)) / args.steps
-    v = variant if variant is not None else int(os.environ.get("SRF_BWD_VARIANT", "0") or 0)
-    per_launch = 1 if v == 1 else args.views       # the round-1 kernel is launched once per view
-    out = {"P": args.P, "size": args.size, "views": args.views, "bwd_variant": v or "default",
-           "us_per_view": {n: round(t[0] * 1e3 / max(t[1], 1) / (per_launch if n == "render_bwd" else args.views), 2)
-                           for n, t in k.items()},
+    out = {"P": args.P, "size": args.size, "views": args.views,
+           "us_per_view": {n: round(t[0] * 1e3 / max(t[1], 1) / args.views, 2) for n, t in k.items()},
            "launches": {n: t[1] for n, t in k.items()},
            "step_ms": round(ms, 4), "views_per_s": round(args.views / ms * 1e3, 1)}
     print(json.dumps(out), flush=True)
-    return out
 
 
-if args.variants:
-    res = [measure(int(v)) for v in args.variants.split(",")]
-    best = min(res, key=lambda r: r["us_per_view"]["render_bwd"])
-    print("BEST", best["bwd_variant"], best["us_per_view"]["render_bwd"], flush=True)
-else:
-    measure(None)
+measure()
