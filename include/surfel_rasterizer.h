@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define SRF_ABI_VERSION 4
+#define SRF_ABI_VERSION 5
 
 /* cudaStream_t without pulling in cuda_runtime.h */
 typedef void* srf_stream_t;
@@ -249,6 +249,25 @@ int srf_decoder_layout_forward(srf_stream_t stream, size_t B, int N, int K, int 
 int srf_decoder_layout_backward(srf_stream_t stream, size_t B, int N, int K, int sh_dim, float half_cell_size,
                                 const float* params, const float* g_centers, const float* g_shs, const float* g_opacity,
                                 const float* g_scaling, const float* g_rotation, float* g_params);
+
+/* ---- fine-pass point features (next-row: Network.get_point_feats, lightning/network.py:390-411, :182-187) ---------
+ * Each of the n points is projected into the V source views, p = K (R x + t) with `w2cs` [V,4,4] and `ixts` [V,3,3]
+ * row-major, and the 8-channel stack img_ref [V,3,H,W] | image [V,3,H,W] | acc [V,H,W] | depth [V,H,W] (all planar,
+ * contiguous) is sampled bilinearly with zero padding at grid_sample's (align_corners=False) coordinates of
+ * (p.xy/p.z + 0.5)/[W,H]*2 - 1.  feats [V,8,n]; channel 7 is |sampled depth - p.z|.  A tap whose coordinate is not
+ * finite or whose index is outside the image is not used (a point with p.z = 0 samples 0).
+ * The backward writes g_points [n,3] (summed over views) and adds the gradients of image, acc and depth into
+ * g_image / g_acc / g_depth, which it clears first; img_ref gets no gradient.  Each gradient output may be
+ * NULL (not wanted).  n == 0 launches no kernel (the backward still clears the rendering gradients) and
+ * points, feats and g_feats may then be NULL.                                                                      */
+int srf_point_feats_forward(srf_stream_t stream, int V, int n, int H, int W,
+                            const float* points, const float* w2cs, const float* ixts,
+                            const float* img_ref, const float* image, const float* acc, const float* depth,
+                            float* feats);
+int srf_point_feats_backward(srf_stream_t stream, int V, int n, int H, int W,
+                             const float* points, const float* w2cs, const float* ixts,
+                             const float* img_ref, const float* image, const float* acc, const float* depth,
+                             const float* g_feats, float* g_points, float* g_image, float* g_acc, float* g_depth);
 
 /* ---- optional per-kernel timing (no reference counterpart; used by bench.py's roofline) --
  * Between srf_profile_begin() and srf_profile_end() every kernel launch made by this

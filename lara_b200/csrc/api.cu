@@ -727,6 +727,58 @@ int srf_decoder_layout_backward(srf_stream_t stream_, size_t B, int N, int K, in
     return 0;
 }
 
+static int point_feats_check(const char* fn, int V, int n, int H, int W, const float* points, const float* w2cs,
+                             const float* ixts, const float* img_ref, const float* image, const float* acc,
+                             const float* depth) {
+    if (V <= 0 || n < 0 || H <= 0 || W <= 0) return fail("%s: bad sizes (V=%d, n=%d, H=%d, W=%d)", fn, V, n, H, W);
+    if (H > (1 << 24) || W > (1 << 24)) return fail("%s: image too large", fn);    // pixel indices exact in fp32
+    // an empty point set has no storage: points (and feats / g_feats) are only needed when n > 0
+    if ((n > 0 && !points) || !w2cs || !ixts || !img_ref || !image || !acc || !depth) return fail("%s: null input pointer", fn);
+    return 0;
+}
+
+int srf_point_feats_forward(srf_stream_t stream_, int V, int n, int H, int W,
+                            const float* points, const float* w2cs, const float* ixts,
+                            const float* img_ref, const float* image, const float* acc, const float* depth,
+                            float* feats) {
+    const char* fn = "srf_point_feats_forward";
+    if (point_feats_check(fn, V, n, H, W, points, w2cs, ixts, img_ref, image, acc, depth)) return 1;
+    if (n > 0 && !feats) return fail("%s: null output pointer", fn);
+    if (n == 0) return 0;
+    srf::PointFeatsArgs a;
+    memset(&a, 0, sizeof(a));
+    a.V = V; a.n = n; a.H = H; a.W = W;
+    a.points = points; a.w2cs = w2cs; a.ixts = ixts; a.img_ref = img_ref; a.image = image; a.acc = acc; a.depth = depth;
+    a.feats = feats;
+    cudaError_t e = srf::launch_point_feats(a, false, static_cast<cudaStream_t>(stream_));
+    if (e != cudaSuccess) return cuda_fail("point_feats_fwd launch", e);
+    return 0;
+}
+
+int srf_point_feats_backward(srf_stream_t stream_, int V, int n, int H, int W,
+                             const float* points, const float* w2cs, const float* ixts,
+                             const float* img_ref, const float* image, const float* acc, const float* depth,
+                             const float* g_feats, float* g_points, float* g_image, float* g_acc, float* g_depth) {
+    const char* fn = "srf_point_feats_backward";
+    if (point_feats_check(fn, V, n, H, W, points, w2cs, ixts, img_ref, image, acc, depth)) return 1;
+    if (n > 0 && !g_feats) return fail("%s: null upstream gradient", fn);
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    const size_t plane = (size_t)V * H * W * sizeof(float);
+    cudaError_t e = cudaSuccess;
+    if (g_image && (e = cudaMemsetAsync(g_image, 0, 3 * plane, stream)) != cudaSuccess) return cuda_fail("memset g_image", e);
+    if (g_acc && (e = cudaMemsetAsync(g_acc, 0, plane, stream)) != cudaSuccess) return cuda_fail("memset g_acc", e);
+    if (g_depth && (e = cudaMemsetAsync(g_depth, 0, plane, stream)) != cudaSuccess) return cuda_fail("memset g_depth", e);
+    if (n == 0 || (!g_points && !g_image && !g_acc && !g_depth)) return 0;
+    srf::PointFeatsArgs a;
+    memset(&a, 0, sizeof(a));
+    a.V = V; a.n = n; a.H = H; a.W = W;
+    a.points = points; a.w2cs = w2cs; a.ixts = ixts; a.img_ref = img_ref; a.image = image; a.acc = acc; a.depth = depth;
+    a.g_feats = g_feats; a.g_points = g_points; a.g_image = g_image; a.g_acc = g_acc; a.g_depth = g_depth;
+    e = srf::launch_point_feats(a, true, stream);
+    if (e != cudaSuccess) return cuda_fail("point_feats_bwd launch", e);
+    return 0;
+}
+
 int srf_mark_visible(srf_stream_t stream_, int P, const float* means3D,
                      const float* viewmatrix, const float* projmatrix, uint8_t* present) {
     (void)projmatrix;

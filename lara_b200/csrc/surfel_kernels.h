@@ -189,6 +189,24 @@ struct DecoderArgs {
 };
 cudaError_t launch_decoder_layout(const DecoderArgs& a, bool backward, cudaStream_t stream);
 
+// Fine-pass point-feature sampler (lightning/network.py:390-411, projection :182-187): n points sampled in V source
+// views from the 8-channel stack img_ref | image | acc | depth; all images planar fp32.
+struct PointFeatsArgs {
+    int V, n, H, W;
+    const float* points;         // [n,3]
+    const float* w2cs;           // [V,4,4] row-major
+    const float* ixts;           // [V,3,3] row-major
+    const float* img_ref;        // [V,3,H,W]
+    const float* image;          // [V,3,H,W]
+    const float* acc;            // [V,H,W]
+    const float* depth;          // [V,H,W]
+    float* feats;                // [V,8,n] forward output
+    const float* g_feats;        // [V,8,n] backward input
+    float* g_points;             // [n,3] written (may be null)
+    float* g_image; float* g_acc; float* g_depth;   // accumulated into, cleared by the caller (each may be null)
+};
+cudaError_t launch_point_feats(const PointFeatsArgs& a, bool backward, cudaStream_t stream);
+
 // Optional per-kernel CUDA-event timing (srf_profile_begin/end in the C ABI); no-ops unless enabled.
 enum KernelId { K_PREPROCESS_FWD = 0, K_TILE_SCAN, K_SCATTER, K_SORT_SMALL, K_SORT_BIG, K_RENDER_FWD,
                 K_RENDER_BWD, K_PREPROCESS_BWD, K_COUNT };
