@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define SRF_ABI_VERSION 5
+#define SRF_ABI_VERSION 6
 
 /* cudaStream_t without pulling in cuda_runtime.h */
 typedef void* srf_stream_t;
@@ -50,6 +50,10 @@ const char* srf_last_error(void);
  *   image : per-pixel state     (final_T/dist1/dist2 planes, n_contrib/median planes)
  *   entries / point_list : per-instance scratch and the sorted per-tile index list,
  *                          sized by an instance *capacity* chosen by the caller.
+ *                          The point_list workspace also holds, after the list (at
+ *                          byte offset 4*capacity rounded up to 256), the forward's
+ *                          contribution masks, u32 [8][capacity] (36 B per instance
+ *                          of capacity in all); keep it from forward to backward.
  */
 int srf_geom_state_bytes(int P, size_t* bytes);
 int srf_tile_state_bytes(int H, int W, size_t* bytes);

@@ -13,7 +13,7 @@ from ctypes import POINTER, c_char_p, c_float, c_int, c_size_t, c_void_p
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libsurfel_b200.so")
-ABI_VERSION = 5
+ABI_VERSION = 6
 CAM_FLOATS, CAM_VIEW, CAM_CAMPOS, CAM_BG = 24, 0, 16, 19      # include/surfel_rasterizer.h SRF_CAM_*
 
 # name -> (restype, argtypes); mirrors include/surfel_rasterizer.h one to one

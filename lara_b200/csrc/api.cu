@@ -79,6 +79,13 @@ T* at(const void* base, size_t off) {
 
 bool misaligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 255) != 0; }
 
+// One view's point_list workspace: the depth-sorted list (u32 [capacity]), then the blend forward's contribution
+// masks (u32 [8 warp blocks][capacity], indexed by list position), which the blend backward replays.
+size_t plist_masks_offset(size_t capacity) { return align_up(capacity * sizeof(uint32_t)); }
+size_t plist_stride_bytes(size_t capacity) {
+    return plist_masks_offset(capacity) + align_up(capacity * 8 * sizeof(uint32_t)) + 256;
+}
+
 // ---- optional per-kernel timing --------------------------------------------------
 struct ProfSpan { int kernel; cudaEvent_t start, stop; };
 bool g_prof_on = false;
@@ -178,7 +185,7 @@ int srf_image_state_bytes(int H, int W, size_t* bytes) {
 int srf_binning_bytes(size_t capacity, size_t* entries_bytes, size_t* point_list_bytes) {
     if (!entries_bytes || !point_list_bytes) return fail("srf_binning_bytes: bad arguments");
     *entries_bytes = align_up(capacity * sizeof(uint64_t)) + 256;
-    *point_list_bytes = align_up(capacity * sizeof(uint32_t)) + 256;
+    *point_list_bytes = plist_stride_bytes(capacity);
     return 0;
 }
 
@@ -215,7 +222,6 @@ struct Cams {               // per-view camera data: three pointers into records
 };
 
 size_t entries_stride_bytes(size_t capacity) { return align_up(capacity * sizeof(uint64_t)) + 256; }
-size_t plist_stride_bytes(size_t capacity) { return align_up(capacity * sizeof(uint32_t)) + 256; }
 size_t ggrad_stride_bytes(int P) { return align_up((size_t)P * SRF_GRAD_FLOATS * sizeof(float)) + 256; }
 
 void fill_bin_args(srf::BinArgs& b, int V, int P, const TileLayout& tl, void* tile_state) {
@@ -344,6 +350,7 @@ int forward_render_impl(const char* fn, cudaStream_t stream, int V, int P, int i
     r.ranges = b.ranges;
     r.tile_order = b.tile_order;
     r.point_list = point_list;
+    r.masks = at<uint32_t>(point_list, plist_masks_offset(capacity));
     r.rec = P > 0 ? at<float4>(geom_state, gl.rec) : nullptr;
     r.bg = background;
     r.out_color = out_color; r.out_others = out_others;
@@ -394,6 +401,7 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
     r.ranges = at<uint2>(tile_state, tl.ranges);
     r.tile_order = at<uint32_t>(tile_state, tl.order);
     r.point_list = point_list;
+    r.masks = at<const uint32_t>(point_list, plist_masks_offset(capacity));
     r.rec = at<float4>(geom_state, gl.rec);
     r.bg = cams.bg;
     r.accum = at<float>(image_state, il.accum);

@@ -13,9 +13,10 @@
 // (warp, splat) visit -- ~100 of its ~300 warp instructions per visit, at 13/32 useful lanes.
 //
 // Here the two halves run in the layout that suits each (per warp, on its 8x4 pixel block, for groups of
-// 16 splats of the tile list that can touch the block):
-//   phase 1  lane = pixel.  Every lane walks ITS OWN hits (per-pixel octagon masks, as the forward does)
-//            back to front, does the sequential part and parks (w, GdA, dL/dz) in shared memory
+// 16 splats of the tile list that the forward blended into some pixel of the block):
+//   phase 1  lane = pixel.  Every lane walks ITS OWN contributing pairs (the forward's contribution record,
+//            RenderFwdArgs::masks, transposed to per-pixel words) back to front, does the sequential part and
+//            parks (w, GdA, dL/dz) in shared memory
 //            (3 floats per pair, XOR-swizzled so that both phases are bank-conflict free or nearly so).
 //   phase 2  lanes in proportion to work.  The 32 lanes are allotted to the group's splats by their number of contributing
 //            pixels (n_i = ceil(c_i / C) lanes for splat i, C the smallest chunk size for which 32 lanes suffice); every lane
@@ -23,10 +24,9 @@
 //            registers and accumulates the 18 gradient values in registers -- no cross-lane reduction at all; the partial
 //            sums go out as 4 (5) red.global.add.v4.f32 per lane.
 // Phase 1 evaluates pairs with MUFU.RCP / MUFU.EX2 and re-evaluates with the forward's exact sequence only within a
-// narrow band around the forward's decision thresholds (eval_pair_bwd below).
+// narrow band around rho3d = rho2d (eval_pair_bwd below); which pairs were blended it takes from the record.
 // What is kept from round 1: tiles in LPT order (one 4-warp CTA per 16x8 half tile, five per SM), the list walked back
-// to front from the tile's deepest used entry in staged rounds, warp-level octagon cull, paired fp32 arithmetic,
-// MUFU.RCP.
+// to front from the tile's deepest used entry in staged rounds, paired fp32 arithmetic, MUFU.RCP.
 #include "surfel_common.cuh"
 #include "surfel_kernels.h"
 
@@ -71,15 +71,15 @@ __device__ __forceinline__ float ex2_fast(float x) {
     return r;
 }
 
-// Pair evaluation of phase 1.  What must agree with the forward BIT FOR BIT are the accept / reject decisions
-// (a pair taken by one pass and not by the other shifts the whole transmittance chain of its pixel); the values
-// only need ~1e-6.  So the two IEEE divisions and expf() of eval_pair() become MUFU.RCP / MUFU.EX2 (<= 2 ulp), and a
-// pair that lands within a 1e-4 / 1e-5 relative band of a decision threshold (alpha = 1/255, depth = 0.2, rho3d = rho2d)
-// -- one in ~1e4 -- is re-evaluated with the forward's exact sequence.  k, l and p = k x l are the forward's own operations, so the
-// p.z != 0 test is exact as is.
+// Pair evaluation of phase 1, for pairs the forward blended (its contribution record says which): the accept / reject
+// decisions are not taken again.  What must still agree with the forward BIT FOR BIT is which of the two footprints is
+// the smaller one (rho3d vs rho2d picks the depth and the gradient path: a splat whose projected sigma is ~0.707 px has
+// rho3d ~ rho2d at every pixel); the values only need ~1e-6.  So the two IEEE divisions and expf() of eval_pair() become
+// MUFU.RCP / MUFU.EX2 (<= 2 ulp), and a pair within a 1e-5 relative band of rho3d = rho2d is re-evaluated with the
+// forward's exact sequence.
 struct PairBwd {
     float depth, G, alpha;
-    bool lowpass, valid;
+    bool lowpass;
 };
 __device__ __forceinline__ void eval_pair_bwd(const float4 q0, const float4 q1, const float4 q2, const float pixx,
                                               const float pixy, PairBwd& r) {
@@ -102,16 +102,10 @@ __device__ __forceinline__ void eval_pair_bwd(const float4 q0, const float4 q1, 
     r.G = ex2_fast(rho * -0.72134752044448170f);          // exp(-rho/2)
     const float araw = q2.w * r.G;
     r.alpha = fminf(0.99f, araw);
-    r.valid = (pz != 0.0f) && !(r.depth < SRF_NEAR_F) && !(araw < 0.00392156862745098f);
-    // decisions of the forward that the approximate values could take differently: alpha vs 1/255, depth vs the
-    // near plane, and WHICH of the two footprints is the smaller one (rho3d vs rho2d picks the gradient path: a splat
-    // whose projected sigma is ~0.707 px has rho3d ~ rho2d at every pixel)
-    const bool near_thr = fabsf(araw - 0.00392156862745098f) < 4.0e-7f || fabsf(r.depth - SRF_NEAR_F) < 2.0e-5f ||
-                          fabsf(rho3d - rho2d) <= 1.0e-5f * rho2d;
-    if (near_thr && pz != 0.0f) {
+    if (fabsf(rho3d - rho2d) <= 1.0e-5f * rho2d) {
         PairEval e;
         eval_pair(q0, q1, q2, pixx, pixy, e);
-        r.depth = e.depth; r.G = e.G; r.alpha = e.alpha; r.lowpass = !(e.rho3d <= e.rho2d); r.valid = e.valid;
+        r.depth = e.depth; r.G = e.G; r.alpha = e.alpha; r.lowpass = !(e.rho3d <= e.rho2d);
     }
 }
 
@@ -120,7 +114,8 @@ struct BwdSmem {
     static constexpr size_t x = rec + sizeof(float4) * SRF_REC_QUADS * kBwdBatch;            // float [warps][3][16][32]
     static constexpr size_t pixA = x + sizeof(float) * kBwdWarps * 3 * kBwdGroup * 32;       // float4 [threads] dn0 dn1 dn2 dpix0
     static constexpr size_t pixB = pixA + sizeof(float4) * kBwdThreads;                      // float4 [threads] dpix1 dpix2 dL_ddepth dL_dalpha
-    static constexpr size_t list = pixB + sizeof(float4) * kBwdThreads;                      // uint8 [warps][kBwdBatch]
+    static constexpr size_t hm = pixB + sizeof(float4) * kBwdThreads;                        // u32 [warps][kBwdBatch]
+    static constexpr size_t list = hm + sizeof(uint32_t) * kBwdWarps * kBwdBatch;            // uint8 [warps][kBwdBatch]
     static constexpr size_t wmax = list + (size_t)kBwdWarps * kBwdBatch;                     // int [warps]
     static constexpr size_t total = wmax + sizeof(int) * kBwdWarps;
 };
@@ -138,6 +133,7 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     float* s_xw = reinterpret_cast<float*>(smem + L::x) + wid * (3 * kBwdGroup * 32);
     uint8_t* s_listw = reinterpret_cast<uint8_t*>(smem + L::list) + wid * kBwdBatch;
+    uint32_t* s_hmw = reinterpret_cast<uint32_t*>(smem + L::hm) + wid * kBwdBatch;
     uint32_t sa_base = smem_addr(smem);
     asm volatile("" : "+r"(sa_base));                     // opaque: kept in a register, not rebuilt at every use
     const uint32_t sa_rec = sa_base + (uint32_t)L::rec, sa_x = sa_base + (uint32_t)(L::x + wid * (3 * kBwdGroup * 32 * sizeof(float))),
@@ -148,6 +144,7 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
     a.ranges = view_ptr(a.ranges, view, a.tile_stride);
     a.tile_order = view_ptr(a.tile_order, view, a.tile_stride);
     a.point_list = view_ptr(a.point_list, view, a.plist_stride);
+    a.masks = view_ptr(a.masks, view, a.plist_stride);
     a.rec = view_ptr(a.rec, view, a.geom_stride);
     a.bg += (size_t)view * a.cam_stride;
     a.accum = view_ptr(a.accum, view, a.image_stride);
@@ -235,7 +232,18 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
     uint32_t next_id = 0;
     if (n_eff - 1 - tid >= 0) next_id = __ldg(a.point_list + range.x + (n_eff - 1 - tid));
 
+    // this warp's row of the forward's contribution record, by list position
+    const uint32_t* wmasks = a.masks + (size_t)gw * a.capacity + range.x;
+
     for (int b = 0; b < rounds; ++b) {
+        // ---- the warp's contribution masks of batch b, requested first so that they arrive with the records (lane
+        // takes slots lane + 32 k); positions at or behind the warp's deepest contributor were not recorded: 0
+        uint32_t mk[kBwdBatch / 32];
+#pragma unroll
+        for (int k = 0; k < kBwdBatch / 32; ++k) {
+            const int pos = n_eff - 1 - (b * kBwdBatch + k * 32 + lane);
+            mk[k] = (pos >= 0 && pos < wmax) ? __ldg(wmasks + pos) : 0u;
+        }
         // ---- stage batch b (back to front: slot j holds list position n_eff-1-(b*kBwdBatch+j))
         __syncthreads();                                  // every warp is done with the previous batch's records
         for (int jt = tid; jt < kBwdBatch; jt += kBwdThreads) {
@@ -252,33 +260,27 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
         const int npos = n_eff - 1 - ((b + 1) * kBwdBatch + tid);
         if (npos >= 0) next_id = __ldg(a.point_list + range.x + npos);
         __syncthreads();
-        const int cnt = min(kBwdBatch, n_eff - b * kBwdBatch);
 
-        // ---- warp-level cull: compacted list of the staged splats whose alpha >= 1/255 octagon can touch
-        // this warp's 8x4 block and that are not behind the warp's deepest contributor
+        // ---- compacted list of the staged splats the forward blended into some pixel of this warp's block, with
+        // their pixel masks
         int nh = 0;
-        for (int c = 0; c < cnt; c += 32) {
-            const int jt = c + lane;
-            bool hit = false;
-            if (jt < cnt && n_eff - 1 - (b * kBwdBatch + jt) < wmax) hit = octagon_hits(s_rec[2][jt], s_rec[5][jt], warp_rect_at(bx0, by0));
+#pragma unroll
+        for (int k = 0; k < kBwdBatch / 32; ++k) {
+            const bool hit = mk[k] != 0u;
             const unsigned hits = __ballot_sync(0xffffffffu, hit);
-            if (hit) s_listw[nh + __popc(hits & ((1u << lane) - 1u))] = (uint8_t)jt;
+            if (hit) {
+                const int h = nh + __popc(hits & ((1u << lane) - 1u));
+                s_listw[h] = (uint8_t)(k * 32 + lane);
+                s_hmw[h] = mk[k];
+            }
             nh += __popc(hits);
         }
         __syncwarp();
 
         for (int g0 = 0; g0 < nh; g0 += 32) {
-            // per-pixel hit words of 32 list entries: lane l rasterises splat g0+l over the block, the 32x32
-            // bit transpose hands lane p the word "which of these 32 splats can touch MY pixel"
-            uint32_t colword;
-            {
-                uint32_t m = 0;
-                if (g0 + lane < nh) {
-                    const int j = s_listw[g0 + lane];
-                    m = octagon_pixel_mask(s_rec[2][j], s_rec[5][j], warp_rect_at(bx0, by0));
-                }
-                colword = transpose32(m, lane);
-            }
+            // per-pixel contribution words of 32 list entries: the 32x32 bit transpose of their pixel masks hands
+            // lane p the word "which of these 32 splats were blended into MY pixel"
+            const uint32_t colword = transpose32(g0 + lane < nh ? s_hmw[g0 + lane] : 0u, lane);
 #pragma unroll 1
             for (int sub = 0; sub < 2; ++sub) {
                 const int gbase = g0 + sub * kBwdGroup;
@@ -287,8 +289,7 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
 
                 // ================= phase 1: lane = pixel =================
                 uint32_t bits = (colword >> (sub * kBwdGroup)) & 0xffffu;
-                if (last_contributor == 0) bits = 0;
-                uint32_t vbits = 0;
+                const uint32_t vbits = bits;
                 const int iters1 = (int)__reduce_max_sync(0xffffffffu, (unsigned)__popc(bits));
                 for (int it = 0; it < iters1; ++it) {
                     if (bits == 0) continue;
@@ -296,11 +297,9 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
                     bits &= bits - 1;
                     const int j = (int)lds_u8(sa_list + gbase + i);
                     const int pos = n_eff - 1 - (b * kBwdBatch + j);   // 0-based position in the tile list
-                    if (pos >= last_contributor) continue;
                     PairBwd e;
                     const uint32_t sa_j = sa_rec + 16u * j;
                     eval_pair_bwd(lds_f4(sa_j), lds_f4(sa_j + 16u * kBwdBatch), lds_f4(sa_j + 32u * kBwdBatch), pixx, pixy, e);
-                    if (!e.valid) continue;
                     const bool lowpass = e.lowpass;
                     const float4 q3 = lds_f4(sa_j + 48u * kBwdBatch);
                     const float4 q4 = lds_f4(sa_j + 64u * kBwdBatch);
@@ -351,7 +350,6 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
                     sts_f(xa, lowpass ? -w : w);
                     sts_f(xa + 4u * kBwdGroup * 32, e.G * dL_dalpha);
                     sts_f(xa + 8u * kBwdGroup * 32, dL_dz);
-                    vbits |= 1u << i;
                 }
 
                 __syncwarp();     // phase-1 stores to the X tile are visible to the whole warp

@@ -10,6 +10,9 @@
 // octagon rasterised over the warp's block, transposed across the warp) and every lane then
 // walks its own hits in list order, reading the records at per-lane indices (phases A / B
 // below).  Arithmetic and predicates follow the reference exactly (see eval_pair()).
+// Every warp also records, per list position, which pixels of its block the splat was blended into (one u32
+// per (position, 8x4 block), RenderFwdArgs::masks): the blend backward replays that record instead of culling,
+// masking and re-testing the pairs itself.
 #include "surfel_common.cuh"
 #include "surfel_kernels.h"
 
@@ -19,6 +22,7 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
     __shared__ float4 s_rec[SRF_REC_QUADS][SRF_BATCH];
     __shared__ uint32_t s_mask[SRF_CTA_WARPS][SRF_BATCH_CHUNKS][32];   // [warp][group of 32 hits][lane]: per-pixel hit words
     __shared__ uint8_t s_list[SRF_CTA_WARPS][SRF_BATCH];               // [warp]: batch slots of the splats that can touch the warp's block
+    __shared__ __align__(16) uint32_t s_out[SRF_CTA_WARPS][SRF_BATCH];  // [warp][batch slot]: contribution masks of the batch
 
     const int tid = threadIdx.x;
     {   // view of this CTA: per-view workspaces of identical layout, images stacked [V,C,H,W]
@@ -27,6 +31,7 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
         a.ranges = view_ptr(a.ranges, view, a.tile_stride);
         a.tile_order = view_ptr(a.tile_order, view, a.tile_stride);
         a.point_list = view_ptr(a.point_list, view, a.plist_stride);
+        a.masks = view_ptr(a.masks, view, a.plist_stride);
         a.rec = view_ptr(a.rec, view, a.geom_stride);
         a.bg += (size_t)view * a.cam_stride;
         a.accum = view_ptr(a.accum, view, a.image_stride);
@@ -83,6 +88,9 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
         // mask (bit = lane that owns the pixel) and a 32x32 bit transpose over the warp hands every lane the word
         // "which of these 32 splats can touch MY pixel".  A splat outside a pixel's word cannot reach
         // alpha >= 1/255 there, so skipping it changes no result.
+        static_assert(SRF_BATCH == 256, "s_out is cleared with two 16-byte stores per lane");
+        reinterpret_cast<uint4*>(s_out[wid])[lane] = make_uint4(0u, 0u, 0u, 0u);
+        reinterpret_cast<uint4*>(s_out[wid])[lane + 32] = make_uint4(0u, 0u, 0u, 0u);
         int nh = 0;
         for (int c0 = 0; c0 < cnt; c0 += 32) {
             const int jt = c0 + lane;
@@ -93,7 +101,6 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
         }
         __syncwarp();
         const int nchunks = (nh + 31) >> 5;
-        if (nchunks == 0) continue;
         for (int c = 0; c < nchunks; ++c) {
             const int h = (c << 5) + lane;
             uint32_t m = 0;
@@ -107,15 +114,23 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
 
         // ---- phase B: every lane walks its own hits in list order.  The warp iterates max-over-lanes
         // times instead of once per splat that touches the block anywhere (lane utilisation there was ~30 %).
+        // Each lane also records which of its hits it blended: cw collects the bits of chunk c and replaces the
+        // lane's (already read) hit word s_mask[wid][c][lane] when the lane leaves the chunk.
         int c = 0;
-        uint32_t w = s_mask[wid][0][lane];
-        if (done) { w = 0; c = nchunks; }
+        uint32_t w = 0, cw = 0;
+        if (done) {
+            for (int k = 0; k < nchunks; ++k) s_mask[wid][k][lane] = 0;
+            c = nchunks;
+        } else if (nchunks > 0) {
+            w = s_mask[wid][0][lane];
+        }
         for (;;) {
-            while (w == 0 && c < nchunks - 1) { ++c; w = s_mask[wid][c][lane]; }
+            while (w == 0 && c < nchunks - 1) { s_mask[wid][c][lane] = cw; cw = 0; ++c; w = s_mask[wid][c][lane]; }
             const bool active = (w != 0);
             if (!__any_sync(0xffffffffu, active)) break;
             if (!active) continue;
-            const int j = s_list[wid][(c << 5) + __ffs(w) - 1];
+            const int i = __ffs(w) - 1;
+            const int j = s_list[wid][(c << 5) + i];
             w &= w - 1;
             contributor = (uint32_t)(b * SRF_BATCH + j + 1);
             PairEval e;
@@ -125,9 +140,12 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
             const float test_T = fmul_(T, fadd_(1.0f, -alpha));
             if (!(test_T >= 0.0001f)) {
                 done = true;
+                s_mask[wid][c][lane] = cw;
+                for (int k = c + 1; k < nchunks; ++k) s_mask[wid][k][lane] = 0;
                 w = 0; c = nchunks;
                 continue;
             }
+            cw |= 1u << i;
             const float4 q3 = s_rec[3][j];
             const float4 q4 = s_rec[4][j];
             const float depth = e.depth;
@@ -152,6 +170,18 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
             T = test_T;
             last_contributor = contributor;
         }
+        if (c < nchunks) s_mask[wid][c][lane] = cw;
+        __syncwarp();
+
+        // ---- contribution record of the batch: transposed back, lane l holds the pixel mask of hit 32 k + l, which
+        // goes to its batch slot (the slots the cull dropped stay 0); then 32 consecutive list positions per store
+        for (int k = 0; k < nchunks; ++k) {
+            const uint32_t m = transpose32(s_mask[wid][k][lane], lane);
+            if ((k << 5) + lane < nh) s_out[wid][s_list[wid][(k << 5) + lane]] = m;
+        }
+        __syncwarp();
+        uint32_t* dst = a.masks + (size_t)gw * a.capacity + range.x + b * SRF_BATCH;
+        for (int jt = lane; jt < cnt; jt += 32) dst[jt] = s_out[wid][jt];
     }
 
     const float2 C01_ = up2(C01), C2r_ = up2(C2r), N01_ = up2(N01), N2D_ = up2(N2D), d12_f = up2(d12);

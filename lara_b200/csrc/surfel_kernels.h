@@ -73,6 +73,8 @@ struct RenderFwdArgs {
     const uint2* ranges;
     const uint32_t* tile_order;  // [ntiles]: CTA i renders tile tile_order[i] (heaviest first)
     const uint32_t* point_list;
+    uint32_t* masks;             // [8][capacity] out: bit l = the splat at this list position was blended into
+                                 //   pixel l of 8x4 block w (inside the point_list workspace, plist_stride apart)
     const float4* rec;
     const float* bg;             // [3] device (per view, cam_stride floats apart)
     float* out_color;            // [V,3,H,W]
@@ -89,6 +91,7 @@ struct RenderBwdArgs {
     const uint2* ranges;
     const uint32_t* tile_order;
     const uint32_t* point_list;
+    const uint32_t* masks;       // [8][capacity]: the forward's contribution masks (RenderFwdArgs::masks)
     const float4* rec;
     const float* bg;
     const float* accum;

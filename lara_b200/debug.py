@@ -24,6 +24,7 @@ class _View:
             return t[view * n:(view + 1) * n]
         self.geom, self.tile, self.image, self.point_list = cut(state.geom), cut(state.tile), cut(state.image), cut(state.point_list)
         self.num_rendered = state.resolve()[view]
+        self.capacity = state.capacity
 
 
 def unpack_state(state: ForwardState, P: int, H: int, W: int, view: int = 0) -> Dict[str, torch.Tensor]:
@@ -57,4 +58,9 @@ def unpack_state(state: ForwardState, P: int, H: int, W: int, view: int = 0) -> 
     out["accum"] = state.image[i_off[0]:i_off[0] + 12 * npix].view(torch.float32).view(3, H, W)
     out["n_contrib"] = state.image[i_off[1]:i_off[1] + 8 * npix].view(torch.int32).view(2, H, W)
     out["point_list"] = state.point_list[:4 * R].view(torch.int32) if R > 0 else state.point_list[:0].view(torch.int32)
+    # the blend forward's contribution record, after the list in the same workspace (include/surfel_rasterizer.h):
+    # [8 warp blocks, R list positions], bit l = the splat was blended into pixel l of the tile's 8x4 block
+    cap = state.capacity
+    moff = (4 * cap + 255) // 256 * 256
+    out["contrib_masks"] = state.point_list[moff:moff + 32 * cap].view(torch.int32).view(8, cap)[:, :R]
     return out
