@@ -50,19 +50,6 @@ __device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float 
     asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
 
-// explicit 32-bit shared-memory addressing for the phase-1 loop: with pointer-typed accesses the compiler
-// rebuilds the shared window base (S2R SR_CgaCtaId + LEA) inside the loop, in front of the first dependent load
-__device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ float4 lds_f4(uint32_t a) {
-    float4 v;
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a) : "memory");
-    return v;
-}
-__device__ __forceinline__ uint32_t lds_u8(uint32_t a) {
-    uint32_t v;
-    asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
-    return v;
-}
 __device__ __forceinline__ void sts_f(uint32_t a, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(a), "f"(v) : "memory"); }
 
 __device__ __forceinline__ float ex2_fast(float x) {

@@ -67,6 +67,14 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
     // empty list its compiled code leaves the value uninitialised.)
     uint32_t median_contributor = 0;
 
+    // phase B addresses its shared arrays explicitly (smem_addr): the staged records, the warp's hit list and the lane's
+    // hit words
+    uint32_t sa_rec = smem_addr(&s_rec[0][0]), sa_list = smem_addr(&s_list[wid][0]), sa_mask = smem_addr(&s_mask[wid][0][lane]);
+    asm volatile("" : "+r"(sa_rec), "+r"(sa_list), "+r"(sa_mask));   // opaque: kept in registers, not rebuilt at every use
+    // ptxas still rematerialises the record base (S2R SR_CgaCtaId + LEA) at both of its uses in the pair loop; a shuffled
+    // copy is a value it cannot recompute
+    sa_rec = __shfl_sync(0xffffffffu, sa_rec, 0);
+
     int todo = n;
     for (int b = 0; b < rounds; ++b, todo -= SRF_BATCH) {
         // whole tile saturated -> stop (reference forward.cu:334-336)
@@ -119,38 +127,39 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
         int c = 0;
         uint32_t w = 0, cw = 0;
         if (done) {
-            for (int k = 0; k < nchunks; ++k) s_mask[wid][k][lane] = 0;
+            for (int k = 0; k < nchunks; ++k) sts_u32(sa_mask + 128u * k, 0u);
             c = nchunks;
         } else if (nchunks > 0) {
-            w = s_mask[wid][0][lane];
+            w = lds_u32(sa_mask);
         }
         for (;;) {
-            while (w == 0 && c < nchunks - 1) { s_mask[wid][c][lane] = cw; cw = 0; ++c; w = s_mask[wid][c][lane]; }
+            while (w == 0 && c < nchunks - 1) { sts_u32(sa_mask + 128u * c, cw); cw = 0; ++c; w = lds_u32(sa_mask + 128u * c); }
             const bool active = (w != 0);
             if (!__any_sync(0xffffffffu, active)) break;
             if (!active) continue;
             const int i = __ffs(w) - 1;
-            const int j = s_list[wid][(c << 5) + i];
+            const int j = (int)lds_u8(sa_list + (c << 5) + i);
+            const uint32_t sa_j = sa_rec + 16u * j;
             w &= w - 1;
             contributor = (uint32_t)(b * SRF_BATCH + j + 1);
             PairEval e;
-            eval_pair(s_rec[0][j], s_rec[1][j], s_rec[2][j], pixx, pixy, e);
+            eval_pair(lds_f4(sa_j), lds_f4(sa_j + 16u * SRF_BATCH), lds_f4(sa_j + 32u * SRF_BATCH), pixx, pixy, e);
             if (!e.valid) continue;
             const float alpha = e.alpha;
             const float test_T = fmul_(T, fadd_(1.0f, -alpha));
             if (!(test_T >= 0.0001f)) {
                 done = true;
-                s_mask[wid][c][lane] = cw;
-                for (int k = c + 1; k < nchunks; ++k) s_mask[wid][k][lane] = 0;
+                sts_u32(sa_mask + 128u * c, cw);
+                for (int k = c + 1; k < nchunks; ++k) sts_u32(sa_mask + 128u * k, 0u);
                 w = 0; c = nchunks;
                 continue;
             }
             cw |= 1u << i;
-            const float4 q3 = s_rec[3][j];
-            const float4 q4 = s_rec[4][j];
+            const float4 q3 = lds_f4(sa_j + 48u * SRF_BATCH);
+            const float4 q4 = lds_f4(sa_j + 64u * SRF_BATCH);
             const float depth = e.depth;
             const float A = fadd_(1.0f, -T);
-            const float m = mapped_depth(depth);
+            const float m = mapped_depth_fast(depth);
             const float mm = fmul_(m, m);
             const float2 d12_ = up2(d12);
             const float err = fma_(-d12_.x, fadd_(m, m), fma_(A, mm, d12_.y));
@@ -170,7 +179,7 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
             T = test_T;
             last_contributor = contributor;
         }
-        if (c < nchunks) s_mask[wid][c][lane] = cw;
+        if (c < nchunks) sts_u32(sa_mask + 128u * c, cw);
         __syncwarp();
 
         // ---- contribution record of the batch: transposed back, lane l holds the pixel mask of hit 32 k + l, which
@@ -179,9 +188,12 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
             const uint32_t m = transpose32(s_mask[wid][k][lane], lane);
             if ((k << 5) + lane < nh) s_out[wid][s_list[wid][(k << 5) + lane]] = m;
         }
+        // a warp that saturated in this batch stores only the positions before its block's deepest contributor
+        int lim = cnt;
+        if (__all_sync(0xffffffffu, done)) lim = min(cnt, (int)__reduce_max_sync(0xffffffffu, last_contributor) - b * SRF_BATCH);
         __syncwarp();
         uint32_t* dst = a.masks + (size_t)gw * a.capacity + range.x + b * SRF_BATCH;
-        for (int jt = lane; jt < cnt; jt += 32) dst[jt] = s_out[wid][jt];
+        for (int jt = lane; jt < lim; jt += 32) dst[jt] = s_out[wid][jt];
     }
 
     const float2 C01_ = up2(C01), C2r_ = up2(C2r), N01_ = up2(N01), N2D_ = up2(N2D), d12_f = up2(d12);

@@ -140,6 +140,84 @@ __device__ __forceinline__ float mapped_depth(float depth) {
     return (float)__ddiv_rn(num, den);
 }
 
+// The same float from fp32 arithmetic: mapped_depth_fp32(d, rd, m) sets m = mapped_depth(d) and returns true,
+// or returns false when the estimate cannot settle the rounding (then the caller takes mapped_depth).  d >= 0.2f
+// or NaN, as the blend calls it; rd is a reciprocal of d within 1 ulp, or 0 where 1/d is subnormal (MUFU.RCP with
+// flush to zero on the GPU).  Host and device builds run the same operations (tests/test_fwd_fastpath.py checks every
+// float on both).
+//
+// With B = RN_d(99.8), the DP sequence returns RN_f(q_d), q_d = RN_d(RN_d(100d - 20) / RN_d(B d)), and
+// |q_d - r| < 3.01 * 2^-53 for r = (100d - 20) / (B d) = K - J / d, K = 100 / B, J = 20 / B, r in (0, K).
+// The estimate y = h + e + w of r (absolute errors, d >= 0.2f so 1/d < 5; 1 ulp of rd is < 2^-23 rd):
+//   g = RN(JH rd)          g = (JH / d)(1 + n), |n| < 1.51 * 2^-23, g < 1.0021;
+//   rem = RN(JH - g d)     exact value -JH n, |.| < 2^-24.7, rounding < 2^-48.7, / d: < 2^-46.4;
+//   s = RN(rem + JL)       |s| < 2^-24.5, rounding < 2^-48.5, / d: < 2^-46.2;  J = JH + JL to 2^-55, / d: < 2^-52.6;
+//   w = RN(KL -+ tol - s rd)  rd's error on s / d: < 2^-45.2, rounding |w| < 2^-22.1: < 2^-46.1; K = KH + KL to 2^-51.3;
+//   h = RN(KH - g), e      Fast2Sum (g < 2, so exponent(KH) >= exponent(g)): KH - g = h + e exactly, |e| <= 2^-24;
+//   RN(e + w)              |e + w| < 2^-21.9, rounding < 2^-45.9.
+// Summed with the DP's own error, |y -+ tol - q_d| stays within 5.8 * 2^-46 < 2^-43.4 of the exact y -+ tol.  So
+// hi = RN(h + RN(e + w+)) and lo = RN(h + RN(e + w-)), w+- = RN(KL +- 2^-41 - s rd), bracket q_d, and RN_f is monotonic:
+// hi == lo means RN_f(q_d) == hi.  Where rd is 0 (d >= 2^126), y = K + KL +- tol differs from r by J / d < 2^-127.
+// They differ (fallback) where y lies within ~2^-41 of a midpoint between floats: about 2^-16 of the depths with r
+// >= 0.5, more for depths closer to 0.2 (r small, its ulp fine).  NaN and inf give NaN (0 * inf in rem) and fall back.
+#define SRF_MD_KH 0x1.008356p+0f     // RN(K), K = 100 / RN_d(99.8)
+#define SRF_MD_KLP -0x1.4c6edep-26f  // RN(K - KH) + 2^-41 (exact)
+#define SRF_MD_KLM -0x1.4c72dep-26f  // RN(K - KH) - 2^-41 (exact)
+#define SRF_MD_JH 0x1.9a6bbcp-3f     // RN(J), J = 20 / RN_d(99.8)
+#define SRF_MD_JL 0x1.1f4b6ap-29f    // RN(J - JH)
+#ifdef __CUDA_ARCH__
+#define SRF_HD_ADD(a, b) __fadd_rn(a, b)
+#define SRF_HD_MUL(a, b) __fmul_rn(a, b)
+#define SRF_HD_FMA(a, b, c) __fmaf_rn(a, b, c)
+#else  // host: IEEE single, built with -ffp-contract=off
+#define SRF_HD_ADD(a, b) ((a) + (b))
+#define SRF_HD_MUL(a, b) ((a) * (b))
+#define SRF_HD_FMA(a, b, c) fmaf(a, b, c)
+#endif
+__host__ __device__ __forceinline__ bool mapped_depth_fp32(float d, float rd, float& m) {
+    const float g = SRF_HD_MUL(SRF_MD_JH, rd);
+    const float s = SRF_HD_ADD(SRF_HD_FMA(-g, d, SRF_MD_JH), SRF_MD_JL);
+    const float wp = SRF_HD_FMA(-s, rd, SRF_MD_KLP);
+    const float wm = SRF_HD_FMA(-s, rd, SRF_MD_KLM);
+    const float h = SRF_HD_ADD(SRF_MD_KH, -g);
+    const float e = SRF_HD_ADD(-g, -SRF_HD_ADD(h, -SRF_MD_KH));
+    const float hi = SRF_HD_ADD(h, SRF_HD_ADD(e, wp));
+    const float lo = SRF_HD_ADD(h, SRF_HD_ADD(e, wm));
+    m = hi;
+    return hi == lo;
+}
+__device__ __forceinline__ float rcp_approx(float x) {
+    float r;
+    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
+    return r;
+}
+// mapped_depth() for every float depth, the DP sequence only where mapped_depth_fp32 cannot decide
+__device__ __forceinline__ float mapped_depth_fast(float depth) {
+    float m;
+    if (mapped_depth_fp32(depth, rcp_approx(depth), m)) return m;
+    return mapped_depth(depth);
+}
+
+// explicit 32-bit shared-memory addressing for the blend loops: with pointer-typed accesses the compiler
+// rebuilds the shared window base (S2R SR_CgaCtaId + LEA) inside the loop, in front of the first dependent load
+__device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ float4 lds_f4(uint32_t a) {
+    float4 v;
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a) : "memory");
+    return v;
+}
+__device__ __forceinline__ uint32_t lds_u8(uint32_t a) {
+    uint32_t v;
+    asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
+    return v;
+}
+__device__ __forceinline__ uint32_t lds_u32(uint32_t a) {
+    uint32_t v;
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
+    return v;
+}
+__device__ __forceinline__ void sts_u32(uint32_t a, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
+
 // pixel owned by thread `tid` of a 256-thread tile CTA: each warp covers an 8x4 block.
 __device__ __forceinline__ void tile_pixel(int tid, int& lx, int& ly) {
     const int w = tid >> 5, l = tid & 31;
