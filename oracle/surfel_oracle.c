@@ -63,6 +63,8 @@ typedef struct {
     uint32_t* n_contrib; /* [2,H,W] */
     float* out_color;    /* [3,H,W] */
     float* out_others;   /* [8,H,W] */
+    uint32_t* masks;     /* [8, num_rendered] contribution record, the kernels' layout: bit l of block w = pixel
+                            (col (w&1)*8 + (l&7), row (w>>1)*4 + (l>>3)) of the tile blended list position j */
 } Oracle;
 
 static const float SH_C0 = 0.28209479177387814f;
@@ -236,6 +238,7 @@ static int bin_and_sort(Oracle* o) {
     qsort(kv, R, sizeof(KV), kv_cmp);
     o->keys = (uint64_t*)malloc((R ? R : 1) * sizeof(uint64_t));
     o->point_list = (uint32_t*)malloc((R ? R : 1) * sizeof(uint32_t));
+    o->masks = (uint32_t*)calloc((R ? R : 1) * 8, sizeof(uint32_t));
     for (uint64_t j = 0; j < R; ++j) { o->keys[j] = kv[j].key; o->point_list[j] = kv[j].val; }
     free(kv);
     memset(o->ranges, 0, (size_t)o->ntiles * 2 * sizeof(uint32_t));
@@ -256,8 +259,8 @@ typedef struct {
     float kx, ky, kz, lx, ly, lz, px, py, pz, sx, sy, dx, dy, rho3d, rho2d, depth, G, alpha;
 } Pair;
 
-static int eval_pair(const Oracle* o, uint32_t g, float pixx, float pixy, Pair* e) {
-    const float* T = o->T + 9 * (size_t)g;
+/* the two footprints of a pair, rho3d and rho2d; returns 0 where p.z == 0 */
+static int pair_footprints(const float* T, const float* center, float pixx, float pixy, Pair* e) {
     e->kx = fmaf(pixx, T[6], -T[0]); e->ky = fmaf(pixx, T[7], -T[1]); e->kz = fmaf(pixx, T[8], -T[2]);
     e->lx = fmaf(pixy, T[6], -T[3]); e->ly = fmaf(pixy, T[7], -T[4]); e->lz = fmaf(pixy, T[8], -T[5]);
     e->pz = fmaf(e->kx, e->ly, -(e->ky * e->lx));
@@ -266,9 +269,15 @@ static int eval_pair(const Oracle* o, uint32_t g, float pixx, float pixy, Pair* 
     if (e->pz == 0.0f) return 0;
     e->sx = e->px / e->pz; e->sy = e->py / e->pz;
     e->rho3d = fmaf(e->sx, e->sx, e->sy * e->sy);
-    e->dx = o->center[2 * (size_t)g] - pixx; e->dy = o->center[2 * (size_t)g + 1] - pixy;
+    e->dx = center[0] - pixx; e->dy = center[1] - pixy;
     /* (float)(FilterInvSquare(double) * (double)|d|^2), FilterInvSquare = 1/(0.7071..^2) (auxiliary.h:20-21) */
     e->rho2d = (float)((1 / (0.7071067811865476 * 0.7071067811865476)) * (double)fmaf(e->dx, e->dx, e->dy * e->dy));
+    return 1;
+}
+
+static int eval_pair(const Oracle* o, uint32_t g, float pixx, float pixy, Pair* e) {
+    const float* T = o->T + 9 * (size_t)g;
+    if (!pair_footprints(T, o->center + 2 * (size_t)g, pixx, pixy, e)) return 0;
     const float rho = fminf(e->rho3d, e->rho2d);
     e->depth = (e->rho3d <= e->rho2d) ? (T[8] + fmaf(T[6], e->sx, T[7] * e->sy)) : T[8];
     if ((double)e->depth < 0.2) return 0;
@@ -317,6 +326,7 @@ static void blend_forward(Oracle* o) {
                 for (int c = 0; c < 3; ++c) C[c] = fmaf(Tr, alpha * o->rgb[3 * (size_t)g + c], C[c]);
                 Tr = test_T;
                 last = contributor;
+                o->masks[(size_t)((ly >> 2) * 2 + (lx >> 3)) * o->num_rendered + j] |= 1u << ((ly & 3) * 8 + (lx & 7));
             }
             const size_t pix = (size_t)y * W + x;
             o->accum[pix] = Tr; o->accum[pix + npix] = dist1; o->accum[pix + 2 * npix] = dist2;
@@ -336,7 +346,7 @@ static void blend_forward(Oracle* o) {
 void oracle_destroy(Oracle* o) {
     if (!o) return;
     free(o->radii); free(o->depths); free(o->T); free(o->center); free(o->normal); free(o->rgb);
-    free(o->clamped); free(o->rect); free(o->tiles_touched); free(o->keys); free(o->point_list);
+    free(o->clamped); free(o->rect); free(o->tiles_touched); free(o->keys); free(o->point_list); free(o->masks);
     free(o->ranges); free(o->accum); free(o->n_contrib); free(o->out_color); free(o->out_others);
     free(o);
 }
@@ -639,6 +649,7 @@ const float* oracle_rgb(const Oracle* o) { return o->rgb; }
 const uint8_t* oracle_clamped(const Oracle* o) { return o->clamped; }
 const uint32_t* oracle_tiles_touched(const Oracle* o) { return o->tiles_touched; }
 const uint32_t* oracle_point_list(const Oracle* o) { return o->point_list; }
+const uint32_t* oracle_masks(const Oracle* o) { return o->masks; }
 const uint32_t* oracle_ranges(const Oracle* o) { return o->ranges; }
 const float* oracle_accum(const Oracle* o) { return o->accum; }
 const uint32_t* oracle_n_contrib(const Oracle* o) { return o->n_contrib; }
@@ -650,4 +661,297 @@ int oracle_threads(void) {
 #else
     return 1;
 #endif
+}
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * Float64 replay of the blend under a forward's own decisions, with a running error bound (oracle_replay).
+ *
+ * Inputs are a forward state from outside -- the per-Gaussian records (T, centre, opacity, normal, colour), the tile
+ * lists, each pixel's last and median contributor and the contribution record -- plus the background and upstream
+ * gradients.  Which pairs a pixel blended is the record's bit below the pixel's last contributor; which footprint a
+ * pair takes (rho3d <= rho2d) is not recorded and is taken from the fp32 sequence of eval_pair (pair_footprints), or
+ * from `lowpass` when the caller fixes it.  Pairs whose footprint float64 would choose otherwise are counted, and the
+ * Gaussians they touch are flagged: an fp32 kernel may take either branch there.
+ *
+ * Everything else is recomputed in double from the records (treated as exact): alpha, G, depth, the transmittance,
+ * the accumulations and T_final (the images), then the backward of backward.cu:143-449 per pair and its per-Gaussian
+ * sums, dT[9], dmean2D[2], dnormal[3], dopacity, dcolor[3].
+ *
+ * The bound.  Each value v carries e >= |v_fp32 - v|, where v_fp32 is what an fp32 evaluation of the same formula
+ * from the same records can return.  With K = 2^-23 (one fp32 ulp relative, twice the unit roundoff of round-to-
+ * nearest), first-order running error analysis gives, per operation on inputs (a, ea), (b, eb):
+ *   a +- b : ea + eb + K (|a| + |b|)          -- the summands' magnitudes, not the sum's, so that the bound holds for
+ *                                                whatever association the kernel uses within a short sum;
+ *   a * b  : |a| eb + |b| ea + ea eb + K |ab|
+ *   fma    : as a * b + c with one rounding of the result;
+ *   a / b  : (ea + |a/b| eb) / (|b| - eb) + 2K |a/b|     -- MUFU.RCP (1 ulp, PTX ISA rcp.approx) and a multiply;
+ *   exp(-r/2) : G (expm1(er/2) + 2K + K r/2)           -- 2 ulp (ex2.approx / expf) plus the rounding of the scaled
+ *                                                argument, r/2 <= ln 255 for a blended pair.
+ * Constants rounded to fp32 carry K/2 relative.  The transmittance the kernel uses at a pair is T_final / prod(1 -
+ * alpha_j) over the pairs behind it: its relative bound is T_final's (the forward's own product, bounded as above)
+ * plus, per step of the recursion T <- T / (1 - alpha), e(1 - alpha) / (1 - alpha) + 2K, so it grows with the step
+ * count.  A per-Gaussian sum of n pair terms x_i, added in any order (red.add), carries sum e_i + (n - 1) K sum |x_i|.
+ * Nothing in the bound is fitted to an observed error.
+ * ------------------------------------------------------------------------------------------------------------------ */
+typedef struct { double v, e; } B;
+#define RK (1.0 / 8388608.0)
+static inline B bx(double v) { B r = {v, 0.0}; return r; }
+static inline B bc(double v) { B r = {v, 0.5 * RK * fabs(v)}; return r; }       /* constant rounded to fp32 */
+static inline B badd(B a, B b) { B r = {a.v + b.v, a.e + b.e + RK * (fabs(a.v) + fabs(b.v))}; return r; }
+static inline B bsub(B a, B b) { B r = {a.v - b.v, a.e + b.e + RK * (fabs(a.v) + fabs(b.v))}; return r; }
+static inline B bneg(B a) { B r = {-a.v, a.e}; return r; }
+static inline B bmul(B a, B b) {
+    const double v = a.v * b.v;
+    B r = {v, fabs(a.v) * b.e + fabs(b.v) * a.e + a.e * b.e + RK * fabs(v)};
+    return r;
+}
+static inline B bfma(B a, B b, B c) {
+    const double v = a.v * b.v + c.v;
+    B r = {v, fabs(a.v) * b.e + fabs(b.v) * a.e + a.e * b.e + c.e + RK * fabs(v)};
+    return r;
+}
+static inline B bdiv(B a, B b) {
+    const double v = a.v / b.v, d = fabs(b.v) - b.e;
+    B r = {v, d > 0.0 ? (a.e + fabs(v) * b.e) / d + 2.0 * RK * fabs(v) : INFINITY};
+    return r;
+}
+
+typedef struct {
+    int P, H, W;
+    const double* T;          /* [P,9]: Tu, Tv, Tw */
+    const double* center;     /* [P,2] */
+    const double* opacity;    /* [P] */
+    const double* normal;     /* [P,3] */
+    const double* rgb;        /* [P,3] */
+    const uint32_t* ranges;   /* [ntiles,2] */
+    const uint32_t* point_list;
+    const uint32_t* n_contrib;/* [2,H,W] last, median contributor */
+    const uint32_t* masks;    /* [8, mask_stride] */
+    long long mask_stride;
+    const uint8_t* tiles;     /* [ntiles] tiles to replay, or NULL for all */
+    const float* bg;          /* [3] */
+    const float* dL_dpix;     /* [3,H,W] */
+    const float* dL_dothers;  /* [8,H,W] */
+    uint8_t* lowpass;         /* NULL, or [num_rendered, 256] footprint choice per (list position, tile pixel) */
+    int fix_lowpass;          /* 1: read `lowpass`; 0: write it (when given) */
+} ReplayIn;
+
+#define RG 18   /* per-Gaussian partials: dT[9], dmean2D[2], dnormal[3], dopacity, dcolor[3] */
+
+typedef struct {
+    double* img;      /* [14,H,W] colour[3], others[8], accum[3] (T_final, dist1, dist2); zeroed by the caller */
+    double* img_e;    /* [14,H,W] their bounds */
+    double* g;        /* [P,RG] zeroed by the caller */
+    double* g_e;      /* [P,RG] */
+    int64_t* npairs;  /* [P] blended pairs per Gaussian; zeroed */
+    int64_t* nlow;    /* [P] of which low-pass; zeroed */
+    uint8_t* band;    /* [P] 1 = touched by a pair whose footprint float64 chooses otherwise; zeroed */
+    int64_t counts[4];/* pairs, low-pass pairs, band pairs, pixels replayed */
+} ReplayOut;
+
+typedef struct {
+    B kx, ky, kz, lx, ly, lz, px, py, pz, sx, sy, depth, G, alpha;
+    double dx, dy;
+    int lowpass, band;
+} RPair;
+
+static void replay_pair(const ReplayIn* in, uint32_t g, float pixx, float pixy, int lp_fixed, RPair* r) {
+    const double* T = in->T + 9 * (size_t)g;
+    const B T0 = bx(T[0]), T1 = bx(T[1]), T2 = bx(T[2]), T3 = bx(T[3]), T4 = bx(T[4]), T5 = bx(T[5]);
+    const B T6 = bx(T[6]), T7 = bx(T[7]), T8 = bx(T[8]);
+    const B X = bx(pixx), Y = bx(pixy);
+    r->kx = bfma(X, T6, bneg(T0)); r->ky = bfma(X, T7, bneg(T1)); r->kz = bfma(X, T8, bneg(T2));
+    r->lx = bfma(Y, T6, bneg(T3)); r->ly = bfma(Y, T7, bneg(T4)); r->lz = bfma(Y, T8, bneg(T5));
+    r->pz = bfma(r->kx, r->ly, bneg(bmul(r->ky, r->lx)));
+    r->px = bfma(r->ky, r->lz, bneg(bmul(r->kz, r->ly)));
+    r->py = bfma(r->kz, r->lx, bneg(bmul(r->kx, r->lz)));
+    r->sx = bdiv(r->px, r->pz); r->sy = bdiv(r->py, r->pz);
+    const B rho3d = bfma(r->sx, r->sx, bmul(r->sy, r->sy));
+    r->dx = in->center[2 * (size_t)g] - pixx; r->dy = in->center[2 * (size_t)g + 1] - pixy;
+    const B dx = {r->dx, RK * fabs(r->dx)}, dy = {r->dy, RK * fabs(r->dy)};
+    const B rho2d = bmul(bx(2.0), bfma(dx, dx, bmul(dy, dy)));
+    int lp;
+    if (lp_fixed >= 0) {
+        lp = lp_fixed;
+    } else {
+        float Tf[9], cf[2];
+        for (int k = 0; k < 9; ++k) Tf[k] = (float)T[k];
+        cf[0] = (float)in->center[2 * (size_t)g]; cf[1] = (float)in->center[2 * (size_t)g + 1];
+        Pair e;
+        lp = pair_footprints(Tf, cf, pixx, pixy, &e) ? !(e.rho3d <= e.rho2d) : 1;
+    }
+    r->lowpass = lp;
+    r->band = lp != !(rho3d.v <= rho2d.v);
+    const B rho = lp ? rho2d : rho3d;
+    r->depth = lp ? T8 : badd(T8, bfma(T6, r->sx, bmul(T7, r->sy)));
+    const double G = exp(-0.5 * rho.v);
+    r->G.v = G;
+    r->G.e = G * (expm1(0.5 * rho.e) + 2.0 * RK + RK * 0.5 * fabs(rho.v));
+    B a = bmul(bx(in->opacity[g]), r->G);
+    if (a.v > 0.99) { a.e = a.v - a.e > 0.99 ? 0.0 : a.e; a.v = 0.99; }   /* min(0.99, .) */
+    r->alpha = a;
+}
+
+static inline void acc_g(double* g, double* ge, double* gs, size_t i, int k, B x) {
+    atomic_add_d(&g[i * RG + k], x.v);
+    atomic_add_d(&ge[i * RG + k], x.e);
+    atomic_add_d(&gs[i * RG + k], fabs(x.v));
+}
+
+int oracle_replay(const ReplayIn* in, ReplayOut* out) {
+    const int H = in->H, W = in->W, P = in->P;
+    const int gx = (W + TILE - 1) / TILE, gy = (H + TILE - 1) / TILE, ntiles = gx * gy;
+    const size_t npix = (size_t)H * W;
+    double* gs = (double*)calloc((size_t)(P > 0 ? P : 1) * RG, sizeof(double));   /* sums of |terms| */
+    if (!gs) return 1;
+    int64_t c_pairs = 0, c_low = 0, c_band = 0, c_pix = 0;
+    const double bgd[3] = {in->bg[0], in->bg[1], in->bg[2]};
+#pragma omp parallel for schedule(dynamic, 1) reduction(+ : c_pairs, c_low, c_band, c_pix)
+    for (int tile = 0; tile < ntiles; ++tile) {
+        if (in->tiles && !in->tiles[tile]) continue;
+        const int ty = tile / gx, tx = tile % gx;
+        const uint32_t r0 = in->ranges[2 * tile];
+        for (int ly = 0; ly < TILE; ++ly) for (int lx = 0; lx < TILE; ++lx) {
+            const int x = tx * TILE + lx, y = ty * TILE + ly;
+            if (x >= W || y >= H) continue;
+            const size_t pix = (size_t)y * W + x;
+            const float pixx = (float)x + 0.5f, pixy = (float)y + 0.5f;
+            const int last = (int)in->n_contrib[pix], median = (int)in->n_contrib[pix + npix];
+            const uint32_t* mrow = in->masks + (size_t)((ly >> 2) * 2 + (lx >> 3)) * in->mask_stride + r0;
+            const uint32_t bit = 1u << ((ly & 3) * 8 + (lx & 7));
+            const int tp = ly * TILE + lx;
+            ++c_pix;
+            /* ---- forward under the recorded decisions */
+            B Tr = bx(1.0), C[3] = {bx(0), bx(0), bx(0)}, N[3] = {bx(0), bx(0), bx(0)}, D = bx(0);
+            B dist1 = bx(0), dist2 = bx(0), distortion = bx(0), med_d = bx(0), med_w = bx(0);
+            for (int pos = 0; pos < last; ++pos) {
+                if (!(mrow[pos] & bit)) continue;
+                const uint32_t g = in->point_list[r0 + pos];
+                RPair e;
+                uint8_t* lpp = in->lowpass ? in->lowpass + (size_t)(r0 + pos) * 256 + tp : NULL;
+                replay_pair(in, g, pixx, pixy, (lpp && in->fix_lowpass) ? *lpp : -1, &e);
+                if (lpp && !in->fix_lowpass) *lpp = (uint8_t)e.lowpass;
+                const B al = e.alpha, w = bmul(al, Tr);
+                const B A = bsub(bx(1.0), Tr);
+                const double m_v = (100.0 * e.depth.v - 20.0) / (99.8 * e.depth.v);
+                const B m = {m_v, 0.2004008 / (e.depth.v * e.depth.v) * e.depth.e + RK * (1.0 + fabs(m_v))};
+                const B mm = bmul(m, m);
+                const B err = bfma(bneg(dist1), badd(m, m), bfma(A, mm, dist2));
+                distortion = bfma(w, err, distortion);
+                if (pos == median - 1) { med_d = e.depth; med_w = w; }
+                for (int c = 0; c < 3; ++c) N[c] = bfma(w, bx(in->normal[3 * (size_t)g + c]), N[c]);
+                D = bfma(w, e.depth, D);
+                dist1 = bfma(w, m, dist1);
+                dist2 = bfma(w, mm, dist2);
+                for (int c = 0; c < 3; ++c) C[c] = bfma(w, bx(in->rgb[3 * (size_t)g + c]), C[c]);
+                Tr = bmul(Tr, bsub(bx(1.0), al));
+                ++c_pairs; c_low += e.lowpass; c_band += e.band;
+                if (e.band) out->band[g] = 1;
+            }
+            const B Tf = Tr;
+            const B img[14] = {bfma(bx(bgd[0]), Tf, C[0]), bfma(bx(bgd[1]), Tf, C[1]), bfma(bx(bgd[2]), Tf, C[2]),
+                               D, bsub(bx(1.0), Tf), N[0], N[1], N[2], med_d, distortion, med_w, Tf, dist1, dist2};
+            for (int k = 0; k < 14; ++k) { out->img[k * npix + pix] = img[k].v; out->img_e[k * npix + pix] = img[k].e; }
+
+            /* ---- backward, back to front (backward.cu:321-446) */
+            float up[11];
+            for (int c = 0; c < 3; ++c) up[c] = in->dL_dpix[pix + c * npix];
+            for (int c = 0; c < 8; ++c) up[3 + c] = in->dL_dothers[pix + c * npix];
+            int nz = 0;
+            for (int c = 0; c < 11; ++c) nz |= up[c] != 0.0f;
+            if (!nz) continue;
+            const B dpix[3] = {bx(up[0]), bx(up[1]), bx(up[2])};
+            const B dL_ddepth = bx(up[3]), dL_daccum = bx(up[4]), dn[3] = {bx(up[5]), bx(up[6]), bx(up[7])};
+            const B dL_dmed = bx(up[8]), dL_dreg = bx(up[9]), dL_dmaxw = bx(up[10]);
+            const B final_A = bsub(bx(1.0), Tf);
+            const B bg_dot = badd(badd(bmul(bx(bgd[0]), dpix[0]), bmul(bx(bgd[1]), dpix[1])), bmul(bx(bgd[2]), dpix[2]));
+            const B nTf_bg = bneg(bmul(Tf, bg_dot));
+            const B A_r = bmul(final_A, dL_dreg), nD_r = bmul(bmul(bx(-2.0), dist1), dL_dreg), D2_r = bmul(dist2, dL_dreg);
+            const B c2 = bc(20.0 / 99.8);
+            /* the eight recursions of accum_rec: colour, depth, normal, alpha; and their upstream gradients */
+            B acc[8] = {bx(0), bx(0), bx(0), bx(0), bx(0), bx(0), bx(0), bx(0)};
+            const B dch[8] = {dpix[0], dpix[1], dpix[2], dL_ddepth, dn[0], dn[1], dn[2], dL_daccum};
+            B last_dL_dT = bx(0);
+            double Tv = Tf.v, relT = Tf.v > 0.0 ? Tf.e / Tf.v : INFINITY;
+            for (int pos = last - 1; pos >= 0; --pos) {
+                if (!(mrow[pos] & bit)) continue;
+                const uint32_t g = in->point_list[r0 + pos];
+                RPair e;
+                const uint8_t* lpp = in->lowpass ? in->lowpass + (size_t)(r0 + pos) * 256 + tp : NULL;
+                replay_pair(in, g, pixx, pixy, lpp ? *lpp : -1, &e);
+                const B al = e.alpha, om = bsub(bx(1.0), al);
+                Tv = Tv / om.v;
+                relT += om.e / om.v + 2.0 * RK;
+                const B T = {Tv, Tv * relT};
+                const B w = bmul(al, T);
+                const B cur[8] = {bx(in->rgb[3 * (size_t)g]), bx(in->rgb[3 * (size_t)g + 1]), bx(in->rgb[3 * (size_t)g + 2]),
+                                  e.depth, bx(in->normal[3 * (size_t)g]), bx(in->normal[3 * (size_t)g + 1]),
+                                  bx(in->normal[3 * (size_t)g + 2]), bx(1.0)};
+                B dsum = bx(0);
+                for (int c = 0; c < 8; ++c) {
+                    const B d = bsub(cur[c], acc[c]);
+                    dsum = bfma(d, dch[c], dsum);
+                    acc[c] = bfma(d, al, acc[c]);
+                }
+                B dL_dz = bmul(w, dL_ddepth);
+                const B rcd = bdiv(bx(1.0), e.depth);
+                const B m = bsub(bc(100.0 / 99.8), bmul(c2, rcd));
+                B dL_dweight = bfma(m, bfma(m, A_r, nD_r), D2_r);
+                if (pos == median - 1) { dL_dz = badd(dL_dz, dL_dmed); dL_dweight = badd(dL_dweight, dL_dmaxw); }
+                const B ddw = bsub(dL_dweight, last_dL_dT);
+                B dL_dalpha = badd(dsum, ddw);
+                last_dL_dT = bfma(al, ddw, last_dL_dT);
+                /* dL_dmd * dm/dd = 2 w (m A - D) dL_dreg * c2 / d^2 */
+                dL_dz = bfma(bmul(w, bfma(m, bmul(bmul(bx(2.0), c2), A_r), bmul(c2, nD_r))), bmul(rcd, rcd), dL_dz);
+                dL_dalpha = bmul(dL_dalpha, T);
+                dL_dalpha = badd(dL_dalpha, bdiv(nTf_bg, om));
+                const B GdA = bmul(e.G, dL_dalpha);
+                const B opac = bx(in->opacity[g]);
+                for (int c = 0; c < 3; ++c) {
+                    acc_g(out->g, out->g_e, gs, g, 15 + c, bmul(w, dpix[c]));
+                    acc_g(out->g, out->g_e, gs, g, 11 + c, bmul(w, dn[c]));
+                }
+                acc_g(out->g, out->g_e, gs, g, 14, GdA);
+                if (!e.lowpass) {
+                    /* vjp through s = p.xy / p.z, p = k x l (backward.cu:405-435) */
+                    const B nOG = bneg(bmul(opac, GdA));
+                    const B dsx = bfma(e.sx, nOG, bmul(bx(in->T[9 * (size_t)g + 6]), dL_dz));
+                    const B dsy = bfma(e.sy, nOG, bmul(bx(in->T[9 * (size_t)g + 7]), dL_dz));
+                    const B dp0 = bdiv(dsx, e.pz), dp1 = bdiv(dsy, e.pz);
+                    const B dp2 = bneg(badd(bmul(dp0, e.sx), bmul(dp1, e.sy)));
+                    const B dk[3] = {bsub(bmul(e.ly, dp2), bmul(e.lz, dp1)), bsub(bmul(e.lz, dp0), bmul(e.lx, dp2)),
+                                     bsub(bmul(e.lx, dp1), bmul(e.ly, dp0))};
+                    const B dl[3] = {bsub(bmul(dp1, e.kz), bmul(dp2, e.ky)), bsub(bmul(dp2, e.kx), bmul(dp0, e.kz)),
+                                     bsub(bmul(dp0, e.ky), bmul(dp1, e.kx))};
+                    const B dzw[3] = {e.sx, e.sy, bx(1.0)};
+                    for (int c = 0; c < 3; ++c) {
+                        acc_g(out->g, out->g_e, gs, g, c, bneg(dk[c]));
+                        acc_g(out->g, out->g_e, gs, g, 3 + c, bneg(dl[c]));
+                        acc_g(out->g, out->g_e, gs, g, 6 + c,
+                              bfma(bx(pixx), dk[c], bfma(bx(pixy), dl[c], bmul(dL_dz, dzw[c]))));
+                    }
+                } else {
+                    /* low-pass branch (backward.cu:436-443), FilterInvSquare = 2 */
+                    const B k = bmul(bx(-2.0), bmul(opac, GdA));
+                    acc_g(out->g, out->g_e, gs, g, 9, bmul(k, (B){e.dx, RK * fabs(e.dx)}));
+                    acc_g(out->g, out->g_e, gs, g, 10, bmul(k, (B){e.dy, RK * fabs(e.dy)}));
+                    acc_g(out->g, out->g_e, gs, g, 8, dL_dz);
+                }
+#pragma omp atomic
+                out->npairs[g] += 1;
+                if (e.lowpass) {
+#pragma omp atomic
+                    out->nlow[g] += 1;
+                }
+            }
+        }
+    }
+    /* summation bound of the per-Gaussian sums, in any order */
+    for (int i = 0; i < P; ++i) {
+        const double n1 = out->npairs[i] > 1 ? (double)(out->npairs[i] - 1) : 0.0;
+        for (int k = 0; k < RG; ++k) out->g_e[(size_t)i * RG + k] += n1 * RK * gs[(size_t)i * RG + k];
+    }
+    free(gs);
+    out->counts[0] = c_pairs; out->counts[1] = c_low; out->counts[2] = c_band; out->counts[3] = c_pix;
+    return 0;
 }
