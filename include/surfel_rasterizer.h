@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define SRF_ABI_VERSION 6
+#define SRF_ABI_VERSION 7
 
 /* cudaStream_t without pulling in cuda_runtime.h */
 typedef void* srf_stream_t;
@@ -211,6 +211,25 @@ int srf_views_backward(srf_stream_t stream, int V, int P, int D, int M, int imag
                        float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
                        float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
                        int raw_activations);
+/* Deterministic variant of srf_views_backward (also for V = 1): same arguments and results, but the blend
+ * backward's per-lane partial sums are added in 64-bit fixed point (two passes of the blend backward: per-channel
+ * bounds, then the sums), so two calls on the same inputs give bit-identical gradients.  `scratch` (256-byte aligned)
+ * is srf_views_backward_deterministic_scratch_bytes(V, P) bytes.  Waits for the stream before it returns: if a partial
+ * sum is not finite or beyond the fixed-point range it returns an error instead of a gradient (the output arrays then
+ * hold no meaningful values, and with accumulate != 0 they have been added to).                                       */
+int srf_views_backward_deterministic_scratch_bytes(int V, int P, size_t* bytes);
+int srf_views_backward_deterministic(srf_stream_t stream, int V, int P, int D, int M, int image_height, int image_width,
+                                     size_t capacity, const float* cams,
+                                     const float* means3D, const float* shs, int colors_were_precomputed,
+                                     const float* scales, const float* rotations, int transmat_was_precomputed,
+                                     float tan_fovx, float tan_fovy, const int* radii,
+                                     const void* geom_state, const void* tile_state, const uint32_t* point_list,
+                                     const void* image_state,
+                                     const float* dL_dout_color, const float* dL_dout_others,
+                                     void* scratch, int accumulate,
+                                     float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
+                                     float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
+                                     int raw_activations);
 /* the fused render_img epilogue over V stacked views ([V,C,H,W] images, rays [V,H,W,6], `cams` as above) */
 int srf_views_epilogue_forward(srf_stream_t stream, int V, int image_height, int image_width, float depth_ratio,
                                const float* color, const float* allmap, const float* rays, const float* cams,
@@ -234,6 +253,13 @@ int srf_views_epilogue_backward(srf_stream_t stream, int V, int image_height, in
 int srf_loss_forward(srf_stream_t stream, int V, int image_height, int image_width, int with_reg,
                      const float* image, const float* target_hwc, const float* rend_normal, const float* depth_normal,
                      const float* acc_map, const float* rend_dist, double* sums);
+/* Deterministic srf_loss_forward: the per-block partial sums go to `workspace` (8-byte aligned,
+ * srf_loss_deterministic_workspace_bytes) and are reduced in a fixed order, on a grid that does not depend on the device. */
+int srf_loss_deterministic_workspace_bytes(int V, int image_height, int image_width, size_t* bytes);
+int srf_loss_forward_deterministic(srf_stream_t stream, int V, int image_height, int image_width, int with_reg,
+                                   const float* image, const float* target_hwc, const float* rend_normal,
+                                   const float* depth_normal, const float* acc_map, const float* rend_dist, double* sums,
+                                   void* workspace);
 int srf_loss_backward(srf_stream_t stream, int V, int image_height, int image_width, int with_reg,
                       float w_mse, float w_dist, float w_normal,
                       const float* image, const float* target_hwc, const float* rend_normal, const float* depth_normal,
@@ -272,6 +298,15 @@ int srf_point_feats_backward(srf_stream_t stream, int V, int n, int H, int W,
                              const float* points, const float* w2cs, const float* ixts,
                              const float* img_ref, const float* image, const float* acc, const float* depth,
                              const float* g_feats, float* g_points, float* g_image, float* g_acc, float* g_depth);
+/* Deterministic srf_point_feats_backward: the rendering gradients are summed in 64-bit fixed point in `workspace`
+ * (256-byte aligned, srf_point_feats_deterministic_workspace_bytes) and then written, so two calls give identical bits.
+ * Waits for the stream; returns an error instead of a gradient if g_feats holds a non-finite value.                */
+int srf_point_feats_deterministic_workspace_bytes(int V, int H, int W, size_t* bytes);
+int srf_point_feats_backward_deterministic(srf_stream_t stream, int V, int n, int H, int W,
+                                           const float* points, const float* w2cs, const float* ixts,
+                                           const float* img_ref, const float* image, const float* acc, const float* depth,
+                                           const float* g_feats, float* g_points, float* g_image, float* g_acc,
+                                           float* g_depth, void* workspace);
 
 /* ---- fused MS-SSIM (next-row: lightning/loss.py:44-47, pytorch-msssim 1.0.0 MS_SSIM, channel = C) -------------
  * The 5-level MS-SSIM of X (rendering) and Y (target), logical images B x C x H x W, with the library's valid 11-tap
@@ -300,7 +335,8 @@ int srf_ms_ssim_backward(srf_stream_t stream, int B, int C, int H, int W,
  * library is bracketed by CUDA events on its launching stream.  srf_profile_end waits for
  * them and returns, per kernel id, the summed device time in ms and the launch count.
  * Kernel ids: 0 preprocess_fwd, 1 tile_scan, 2 scatter, 3 sort_small, 4 sort_big,
- * 5 render_fwd, 6 render_bwd, 7 preprocess_bwd (SRF_NUM_KERNELS entries).  Not thread-safe. */
+ * 5 render_fwd, 6 render_bwd, 7 preprocess_bwd (SRF_NUM_KERNELS entries).  Not thread-safe.
+ * The deterministic backward runs the blend backward twice: two render_bwd launches per call.            */
 #define SRF_NUM_KERNELS 8
 int srf_profile_begin(void);
 int srf_profile_end(float* ms_out, int* launches_out, int n);

@@ -10,10 +10,11 @@ from __future__ import annotations
 import ctypes
 import os
 from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int64, c_size_t, c_void_p
+from typing import Optional
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libsurfel_b200.so")
-ABI_VERSION = 6
+ABI_VERSION = 7
 CAM_FLOATS, CAM_VIEW, CAM_CAMPOS, CAM_BG = 24, 0, 16, 19      # include/surfel_rasterizer.h SRF_CAM_*
 
 
@@ -111,14 +112,33 @@ SIGNATURES = {
         _P, _P, _P, _P,                          # dL_dopacity, dL_dscales, dL_drotations, dL_dtransMat
         c_int,                                   # raw_activations
     ]),
+    "srf_views_backward_deterministic_scratch_bytes": (c_int, [c_int, c_int, POINTER(c_size_t)]),
+    "srf_views_backward_deterministic": (c_int, [
+        _P, c_int, c_int, c_int, c_int, c_int, c_int,   # stream, V, P, D, M, H, W
+        c_size_t, _P,                            # capacity, cams
+        _P, _P, c_int,                           # means3D, shs, colors_were_precomputed
+        _P, _P, c_int,                           # scales, rotations, transmat_was_precomputed
+        c_float, c_float, _P,                    # tan_fovx, tan_fovy, radii
+        _P, _P, _P, _P,                          # geom_state, tile_state, point_list, image_state
+        _P, _P,                                  # dL_dout_color, dL_dout_others
+        _P, c_int,                               # scratch, accumulate
+        _P, _P, _P, _P,                          # dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors
+        _P, _P, _P, _P,                          # dL_dopacity, dL_dscales, dL_drotations, dL_dtransMat
+        c_int,                                   # raw_activations
+    ]),
     "srf_views_epilogue_forward": (c_int, [_P, c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "srf_views_epilogue_backward": (c_int, [_P, c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "srf_loss_forward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P]),
+    "srf_loss_deterministic_workspace_bytes": (c_int, [c_int, c_int, c_int, POINTER(c_size_t)]),
+    "srf_loss_forward_deterministic": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P]),
     "srf_loss_backward": (c_int, [_P, c_int, c_int, c_int, c_int, c_float, c_float, c_float, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "srf_decoder_layout_forward": (c_int, [_P, c_size_t, c_int, c_int, c_int, c_float, c_float, c_float, _P, _P, _P, _P, _P, _P, _P]),
     "srf_decoder_layout_backward": (c_int, [_P, c_size_t, c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P]),
     "srf_point_feats_forward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P]),
     "srf_point_feats_backward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "srf_point_feats_deterministic_workspace_bytes": (c_int, [c_int, c_int, c_int, POINTER(c_size_t)]),
+    "srf_point_feats_backward_deterministic": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P,
+                                                       _P, _P, _P, _P, _P]),
     "srf_ms_ssim_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, POINTER(c_size_t)]),
     "srf_ms_ssim_forward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _A, _P, _A, c_float, c_int, _P, _P]),
     "srf_ms_ssim_backward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _A, _P, _A, c_float, c_int, _P, _P, _P, _A]),
@@ -188,6 +208,41 @@ def views_sizes(lib, V: int, P: int, H: int, W: int, capacity: int):
     b = (c_size_t * 6)()
     check(lib.srf_views_workspace_bytes(V, P, H, W, capacity, b), lib)
     return tuple(int(x) for x in b)
+
+
+def _size_query(fn, *args) -> int:
+    b = c_size_t()
+    check(fn(*args, ctypes.byref(b)))
+    return int(b.value)
+
+
+def det_backward_scratch_bytes(lib, V: int, P: int) -> int:
+    """Scratch of srf_views_backward_deterministic."""
+    return _size_query(lib.srf_views_backward_deterministic_scratch_bytes, V, P)
+
+
+def det_point_feats_workspace_bytes(lib, V: int, H: int, W: int) -> int:
+    return _size_query(lib.srf_point_feats_deterministic_workspace_bytes, V, H, W)
+
+
+def det_loss_workspace_bytes(lib, V: int, H: int, W: int) -> int:
+    return _size_query(lib.srf_loss_deterministic_workspace_bytes, V, H, W)
+
+
+def use_deterministic(requested: Optional[bool], enabled: bool, warn_only: bool) -> bool:
+    """Whether an op takes its deterministic path: ``requested`` when given, else torch's switch
+    (``torch.use_deterministic_algorithms``).  Warn-only mode counts as on: a deterministic implementation exists, so
+    there is nothing to warn about."""
+    if requested is not None:
+        return bool(requested)
+    return bool(enabled or warn_only)
+
+
+def deterministic(requested: Optional[bool] = None) -> bool:
+    """:func:`use_deterministic` with torch's current setting, read when the op runs."""
+    import torch
+    return use_deterministic(requested, torch.are_deterministic_algorithms_enabled(),
+                             torch.is_deterministic_algorithms_warn_only_enabled())
 
 
 def layout(lib, P: int, H: int, W: int):

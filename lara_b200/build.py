@@ -22,7 +22,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libsurfel_b200.so")
 SOURCES = ["api.cu", "preprocess.cu", "binning.cu", "render_fwd.cu", "render_bwd.cu", "preprocess_bwd.cu", "epilogue.cu", "loss.cu", "decoder.cu", "point_feats.cu", "ms_ssim.cu"]
-HEADERS = ["surfel_common.cuh", "surfel_kernels.h", os.path.join("..", "..", "include", "surfel_rasterizer.h")]
+HEADERS = ["surfel_common.cuh", "surfel_kernels.h", "det_sum.cuh", os.path.join("..", "..", "include", "surfel_rasterizer.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",

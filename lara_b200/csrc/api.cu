@@ -224,6 +224,22 @@ struct Cams {               // per-view camera data: three pointers into records
 size_t entries_stride_bytes(size_t capacity) { return align_up(capacity * sizeof(uint64_t)) + 256; }
 size_t ggrad_stride_bytes(int P) { return align_up((size_t)P * SRF_GRAD_FLOATS * sizeof(float)) + 256; }
 
+// Scratch of the deterministic backward: V fp32 gradient-record arrays (as srf_views_backward's scratch), then V arrays
+// of fixed-point records, then the overflow flag.
+size_t det_stride_bytes(int P) { return align_up((size_t)P * srf::det_record_bytes()); }
+size_t det_scratch_bytes(int V, int P) { return (ggrad_stride_bytes(P) + det_stride_bytes(P)) * (size_t)V + 256; }
+
+// reads a device flag that the work enqueued so far sets: waits for the stream
+int check_overflow_flag(const char* fn, const uint32_t* flag, cudaStream_t stream) {
+    uint32_t h = 0;
+    cudaError_t e = cudaMemcpyAsync(&h, flag, sizeof(h), cudaMemcpyDeviceToHost, stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+    if (e != cudaSuccess) return cuda_fail("deterministic overflow flag read-back", e);
+    if (h) return fail("%s: a gradient term is not finite or beyond the range of the deterministic fixed-point sum; "
+                       "no gradient was produced", fn);
+    return 0;
+}
+
 void fill_bin_args(srf::BinArgs& b, int V, int P, const TileLayout& tl, void* tile_state) {
     memset(&b, 0, sizeof(b));
     b.P = P; b.nviews = V; b.ntiles = tl.ntiles; b.gx = tl.gx;
@@ -375,7 +391,7 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
                   void* scratch, int accumulate,
                   float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
                   float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
-                  int raw_activations) {
+                  int raw_activations, bool deterministic = false) {
     if (V <= 0 || P < 0 || image_height <= 0 || image_width <= 0) return fail("%s: bad sizes", fn);
     if (P == 0) return 0;
     if (!geom_state || !tile_state || !image_state || !scratch || !radii || !cams.bg)
@@ -391,7 +407,12 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
     const GeomLayout gl = geom_layout(P);
     const size_t gstride = ggrad_stride_bytes(P);
 
-    cudaError_t e = cudaMemsetAsync(scratch, 0, V > 1 ? gstride * (size_t)V : (size_t)P * SRF_GRAD_FLOATS * sizeof(float), stream);
+    // deterministic: the fixed-point records and the flag behind the fp32 records are zeroed, the fp32 records written
+    void* det = at<void>(scratch, gstride * (size_t)V);
+    const size_t dstride = det_stride_bytes(P);
+    uint32_t* overflow = at<uint32_t>(det, dstride * (size_t)V);
+    cudaError_t e = deterministic ? cudaMemsetAsync(det, 0, dstride * (size_t)V + sizeof(uint32_t), stream)
+                                  : cudaMemsetAsync(scratch, 0, V > 1 ? gstride * (size_t)V : (size_t)P * SRF_GRAD_FLOATS * sizeof(float), stream);
     if (e != cudaSuccess) return cuda_fail("memset gradient records", e);
 
     srf::RenderBwdArgs r;
@@ -414,7 +435,14 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
         r.image_stride = il.total; r.ggrad_stride = gstride;
     }
     r.cam_stride = cams.stride;
-    e = srf::launch_render_bwd(r, stream);
+    if (deterministic) {
+        srf::RenderBwdArgs rd = r;
+        rd.ggrad = static_cast<float*>(det);
+        rd.ggrad_stride = dstride;
+        e = srf::launch_render_bwd_det(rd, P, r.ggrad, V > 1 ? gstride : 0, overflow, stream);
+    } else {
+        e = srf::launch_render_bwd(r, stream);
+    }
     if (e != cudaSuccess) return cuda_fail("render_bwd launch", e);
 
     srf::PreprocessBwdArgs p;
@@ -441,7 +469,7 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
     p.dL_dscales = dL_dscales; p.dL_drotations = dL_drotations; p.dL_dtransMat = dL_dtransMat;
     e = srf::launch_preprocess_bwd(p, stream);
     if (e != cudaSuccess) return cuda_fail("preprocess_bwd launch", e);
-    return 0;
+    return deterministic ? check_overflow_flag(fn, overflow, stream) : 0;
 }
 
 Cams cams_of(const float* cams) {
@@ -580,6 +608,32 @@ int srf_views_backward(srf_stream_t stream_, int V, int P, int D, int M, int ima
                          dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drotations, dL_dtransMat, raw_activations);
 }
 
+int srf_views_backward_deterministic_scratch_bytes(int V, int P, size_t* bytes) {
+    if (V <= 0 || P < 0 || !bytes) return fail("srf_views_backward_deterministic_scratch_bytes: bad arguments");
+    *bytes = det_scratch_bytes(V, P);
+    return 0;
+}
+
+int srf_views_backward_deterministic(srf_stream_t stream_, int V, int P, int D, int M, int image_height, int image_width,
+                                     size_t capacity, const float* cams,
+                                     const float* means3D, const float* shs, int colors_were_precomputed,
+                                     const float* scales, const float* rotations, int transmat_was_precomputed,
+                                     float tan_fovx, float tan_fovy, const int* radii,
+                                     const void* geom_state, const void* tile_state, const uint32_t* point_list,
+                                     const void* image_state,
+                                     const float* dL_dout_color, const float* dL_dout_others,
+                                     void* scratch, int accumulate,
+                                     float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
+                                     float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
+                                     int raw_activations) {
+    if (!cams) return fail("srf_views_backward_deterministic: null camera records");
+    return backward_impl("srf_views_backward_deterministic", static_cast<cudaStream_t>(stream_), V, P, D, M, image_height,
+                         image_width, capacity, cams_of(cams), means3D, shs, colors_were_precomputed, scales, rotations,
+                         transmat_was_precomputed, tan_fovx, tan_fovy, radii, geom_state, tile_state, point_list,
+                         image_state, dL_dout_color, dL_dout_others, scratch, accumulate, dL_dmeans3D, dL_dmeans2D,
+                         dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drotations, dL_dtransMat, raw_activations, true);
+}
+
 static int epilogue_forward_impl(const char* fn, cudaStream_t stream, int V, int image_height, int image_width,
                                  float depth_ratio, const float* color, const float* allmap, const float* rays,
                                  const float* viewmatrix, size_t cam_stride, float* image, float* depth, float* acc_map,
@@ -672,6 +726,31 @@ int srf_loss_forward(srf_stream_t stream_, int V, int image_height, int image_wi
     a.image = image; a.target = target_hwc; a.rend_normal = rend_normal; a.depth_normal = depth_normal;
     a.acc = acc_map; a.dist = rend_dist; a.sums = sums;
     e = srf::launch_loss_fused(a, stream);
+    if (e != cudaSuccess) return cuda_fail("loss_sums launch", e);
+    return 0;
+}
+
+int srf_loss_deterministic_workspace_bytes(int V, int image_height, int image_width, size_t* bytes) {
+    if (V <= 0 || image_height <= 0 || image_width <= 0 || !bytes) return fail("srf_loss_deterministic_workspace_bytes: bad arguments");
+    *bytes = srf::loss_det_blocks((size_t)V * image_height * image_width) * 3 * sizeof(double);
+    return 0;
+}
+
+int srf_loss_forward_deterministic(srf_stream_t stream_, int V, int image_height, int image_width, int with_reg,
+                                   const float* image, const float* target_hwc, const float* rend_normal,
+                                   const float* depth_normal, const float* acc_map, const float* rend_dist, double* sums,
+                                   void* workspace) {
+    const char* fn = "srf_loss_forward_deterministic";
+    if (V <= 0 || image_height <= 0 || image_width <= 0) return fail("%s: bad sizes", fn);
+    if (!image || !target_hwc || !sums) return fail("%s: null pointer", fn);
+    if (with_reg && (!rend_normal || !depth_normal || !acc_map || !rend_dist)) return fail("%s: null regulariser input", fn);
+    if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 7)) return fail("%s: workspace must be 8-byte aligned", fn);
+    srf::LossArgs a;
+    memset(&a, 0, sizeof(a));
+    a.W = image_width; a.H = image_height; a.nviews = V; a.with_reg = with_reg ? 1 : 0;
+    a.image = image; a.target = target_hwc; a.rend_normal = rend_normal; a.depth_normal = depth_normal;
+    a.acc = acc_map; a.dist = rend_dist; a.sums = sums; a.partials = static_cast<double*>(workspace);
+    cudaError_t e = srf::launch_loss_fused(a, static_cast<cudaStream_t>(stream_));
     if (e != cudaSuccess) return cuda_fail("loss_sums launch", e);
     return 0;
 }
@@ -785,6 +864,47 @@ int srf_point_feats_backward(srf_stream_t stream_, int V, int n, int H, int W,
     e = srf::launch_point_feats(a, true, stream);
     if (e != cudaSuccess) return cuda_fail("point_feats_bwd launch", e);
     return 0;
+}
+
+// header (max |g_feats|, overflow flag), then the int64 planes g_image | g_acc | g_depth
+static size_t pf_det_planes_offset() { return 256; }
+
+int srf_point_feats_deterministic_workspace_bytes(int V, int H, int W, size_t* bytes) {
+    if (V <= 0 || H <= 0 || W <= 0 || !bytes) return fail("srf_point_feats_deterministic_workspace_bytes: bad arguments");
+    *bytes = pf_det_planes_offset() + 5 * (size_t)V * H * W * sizeof(long long);
+    return 0;
+}
+
+int srf_point_feats_backward_deterministic(srf_stream_t stream_, int V, int n, int H, int W,
+                                           const float* points, const float* w2cs, const float* ixts,
+                                           const float* img_ref, const float* image, const float* acc, const float* depth,
+                                           const float* g_feats, float* g_points, float* g_image, float* g_acc,
+                                           float* g_depth, void* workspace) {
+    const char* fn = "srf_point_feats_backward_deterministic";
+    if (point_feats_check(fn, V, n, H, W, points, w2cs, ixts, img_ref, image, acc, depth)) return 1;
+    if (n > 0 && !g_feats) return fail("%s: null upstream gradient", fn);
+    if (!workspace || misaligned(workspace)) return fail("%s: workspace must be 256-byte aligned", fn);
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    const size_t plane = (size_t)V * H * W * sizeof(float);
+    cudaError_t e = cudaSuccess;
+    if (n == 0 || (!g_points && !g_image && !g_acc && !g_depth)) {       // nothing to sum: cleared outputs, as the default
+        if (g_image && (e = cudaMemsetAsync(g_image, 0, 3 * plane, stream)) != cudaSuccess) return cuda_fail("memset g_image", e);
+        if (g_acc && (e = cudaMemsetAsync(g_acc, 0, plane, stream)) != cudaSuccess) return cuda_fail("memset g_acc", e);
+        if (g_depth && (e = cudaMemsetAsync(g_depth, 0, plane, stream)) != cudaSuccess) return cuda_fail("memset g_depth", e);
+        return 0;
+    }
+    e = cudaMemsetAsync(workspace, 0, pf_det_planes_offset() + 5 * (size_t)V * H * W * sizeof(long long), stream);
+    if (e != cudaSuccess) return cuda_fail("memset point_feats workspace", e);
+    srf::PointFeatsArgs a;
+    memset(&a, 0, sizeof(a));
+    a.V = V; a.n = n; a.H = H; a.W = W;
+    a.points = points; a.w2cs = w2cs; a.ixts = ixts; a.img_ref = img_ref; a.image = image; a.acc = acc; a.depth = depth;
+    a.g_feats = g_feats; a.g_points = g_points; a.g_image = g_image; a.g_acc = g_acc; a.g_depth = g_depth;
+    a.det = static_cast<uint32_t*>(workspace);
+    a.g_fixed = at<long long>(workspace, pf_det_planes_offset());
+    e = srf::launch_point_feats(a, true, stream);
+    if (e != cudaSuccess) return cuda_fail("point_feats_bwd launch", e);
+    return check_overflow_flag(fn, a.det + 1, stream);
 }
 
 static int ms_ssim_sizes(const char* fn, int B, int C, int H, int W) {

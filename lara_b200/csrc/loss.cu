@@ -17,6 +17,7 @@
 
 namespace srf {
 
+template <bool kDet>
 __global__ void __launch_bounds__(256) loss_sums_kernel(LossArgs a) {
     const size_t npix = (size_t)a.W * a.H, total = npix * (size_t)a.nviews;
     float s_mse = 0.f, s_dist = 0.f, s_norm = 0.f;
@@ -52,9 +53,22 @@ __global__ void __launch_bounds__(256) loss_sums_kernel(LossArgs a) {
         double t = 0.0;
 #pragma unroll
         for (int w = 0; w < 8; ++w) t += (double)s_part[threadIdx.x][w];
-        atomicAdd(a.sums + threadIdx.x, t);
+        if (kDet) a.partials[3 * blockIdx.x + threadIdx.x] = t;
+        else atomicAdd(a.sums + threadIdx.x, t);
     }
 }
+
+// deterministic path: the per-block partials of loss_sums_kernel<true> summed in a fixed order, warp w for term w
+__global__ void __launch_bounds__(96) loss_sums_finalize_kernel(const double* partials, int nblocks, double* sums) {
+    const int lane = threadIdx.x & 31, term = threadIdx.x >> 5;
+    double t = 0.0;
+    for (int b = lane; b < nblocks; b += 32) t += partials[3 * b + term];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+    if (lane == 0) sums[term] = t;
+}
+
+size_t loss_det_blocks(size_t total) { return min((size_t)kLossDetBlocks, (total + 255) / 256); }
 
 __global__ void __launch_bounds__(256) loss_grads_kernel(LossArgs a) {
     const size_t npix = (size_t)a.W * a.H, total = npix * (size_t)a.nviews;
@@ -91,9 +105,14 @@ __global__ void __launch_bounds__(256) loss_grads_kernel(LossArgs a) {
 cudaError_t launch_loss_fused(const LossArgs& a, cudaStream_t stream) {
     const size_t total = (size_t)a.W * a.H * (size_t)a.nviews;
     if (total == 0) return cudaSuccess;
-    if (a.sums != nullptr) {
+    if (a.sums != nullptr && a.partials != nullptr) {
+        // a grid that does not depend on the device: the same partials, and so the same bits, on every GPU
+        const int grid = (int)loss_det_blocks(total);
+        loss_sums_kernel<true><<<grid, 256, 0, stream>>>(a);
+        loss_sums_finalize_kernel<<<1, 96, 0, stream>>>(a.partials, grid, a.sums);
+    } else if (a.sums != nullptr) {
         const int grid = (int)min((size_t)sm_count() * 8, (total + 255) / 256);
-        loss_sums_kernel<<<grid, 256, 0, stream>>>(a);
+        loss_sums_kernel<false><<<grid, 256, 0, stream>>>(a);
     }
     if (a.g_image != nullptr) loss_grads_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(a);
     return cudaGetLastError();

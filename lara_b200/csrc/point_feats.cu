@@ -18,6 +18,7 @@
 // Backward: the upstream gradient g[V,8,n] is read coalesced; dL/dpoints[n,3] is summed over the views in registers
 // and written once; the gradients of the 5 differentiable channels go into planar g_image[V,3,H,W], g_acc[V,H,W]
 // and g_depth[V,H,W] with red.global.add.f32 (cleared by the caller).  No gradient is formed for img_ref.
+#include "det_sum.cuh"
 #include "surfel_kernels.h"
 
 namespace srf {
@@ -125,9 +126,44 @@ __global__ void __launch_bounds__(kPfThreads) point_feats_fwd_kernel(PointFeatsA
     }
 }
 
+__device__ __forceinline__ void pf_red_u64(long long* p, long long v) {
+    asm volatile("red.global.add.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+
+// Deterministic backward (DESIGN §3.13): every term a tap adds into a rendering gradient is w go with w <= 1 and
+// |go| <= max |g_feats|, and a pixel of a plane receives at most 4 V n of them.  The bound kernel takes that max
+// (det[0], fp32 bits); the backward adds the terms in 64-bit fixed point into planes laid out as g_image | g_acc |
+// g_depth; the convert kernel writes the fp32 results.  det[1] is set if a term was over its budget or not finite.
+__global__ void __launch_bounds__(kPfThreads) pf_bound_kernel(const float* g, size_t count, uint32_t* det) {
+    uint32_t m = 0;
+    for (size_t i = (size_t)blockIdx.x * kPfThreads + threadIdx.x; i < count; i += (size_t)gridDim.x * kPfThreads)
+        m = max(m, det::abs_bits(__ldg(g + i)));
+    m = __reduce_max_sync(0xffffffffu, m);
+    if ((threadIdx.x & 31) == 0 && m != 0u) atomicMax(det, m);
+}
+
+__global__ void __launch_bounds__(kPfThreads) pf_convert_kernel(PointFeatsArgs a) {
+    const size_t HW = (size_t)a.H * a.W, n_img = 3 * (size_t)a.V * HW, n_one = (size_t)a.V * HW;
+    const size_t j = (size_t)blockIdx.x * kPfThreads + threadIdx.x;
+    if (j >= n_img + 2 * n_one) return;
+    const int L = det::ceil_log2(4ull * (uint64_t)a.V * (uint64_t)a.n);
+    const int k = det::scale_exp(__ldg(a.det), L);
+    float* dst = j < n_img ? (a.g_image ? a.g_image + j : nullptr)
+               : j < n_img + n_one ? (a.g_acc ? a.g_acc + (j - n_img) : nullptr)
+                                   : (a.g_depth ? a.g_depth + (j - n_img - n_one) : nullptr);
+    if (dst) *dst = det::to_float(a.g_fixed[j], k);
+}
+
+template <bool kDet>
 __global__ void __launch_bounds__(kPfThreads) point_feats_bwd_kernel(PointFeatsArgs a) {
     const int i = blockIdx.x * kPfThreads + threadIdx.x;
     if (i >= a.n) return;
+    int L = 0, kq = 0;
+    bool ok = true;
+    if (kDet) {
+        L = det::ceil_log2(4ull * (uint64_t)a.V * (uint64_t)a.n);
+        kq = det::scale_exp(__ldg(a.det), L);
+    }
     const float x0 = a.points[3 * (size_t)i], x1 = a.points[3 * (size_t)i + 1], x2 = a.points[3 * (size_t)i + 2];
     const size_t HW = (size_t)a.H * a.W, n = (size_t)a.n;
     float gx0 = 0.0f, gx1 = 0.0f, gx2 = 0.0f;           // dL/dpoint, summed over the views
@@ -164,9 +200,21 @@ __global__ void __launch_bounds__(kPfThreads) point_feats_bwd_kernel(PointFeatsA
             else if (c == 6) dst = a.g_acc ? a.g_acc + (size_t)v * HW : nullptr;
             else if (c == 7) dst = a.g_depth ? a.g_depth + (size_t)v * HW : nullptr;
             if (dst && go != 0.0f) {
+                if (kDet) {
+                    const size_t plane = c < 6 ? (size_t)v * 3 + (c - 3) : (size_t)(c == 6 ? 3 : 4) * a.V + v;
+                    long long* qd = a.g_fixed + plane * HW;
 #pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    if (t.off[k] >= 0) pf_red(dst + t.off[k], __fmul_rn(t.w[k], go));
+                    for (int k = 0; k < 4; ++k) {
+                        if (t.off[k] < 0) continue;
+                        long long q;
+                        ok &= det::quantize(__fmul_rn(t.w[k], go), kq, L, q);
+                        if (q != 0) pf_red_u64(qd + t.off[k], q);
+                    }
+                } else {
+#pragma unroll
+                    for (int k = 0; k < 4; ++k)
+                        if (t.off[k] >= 0) pf_red(dst + t.off[k], __fmul_rn(t.w[k], go));
+                }
             }
         }
         if (!a.g_points) continue;
@@ -187,6 +235,7 @@ __global__ void __launch_bounds__(kPfThreads) point_feats_bwd_kernel(PointFeatsA
         for (int k = 0; k < 3; ++k) dx[k] = dq[0] * m[k] + dq[1] * m[4 + k] + dq[2] * m[8 + k];
         gx0 += dx[0]; gx1 += dx[1]; gx2 += dx[2];
     }
+    if (kDet && !ok) atomicOr(a.det + 1, 1u);
     if (a.g_points) {
         a.g_points[3 * (size_t)i] = gx0;
         a.g_points[3 * (size_t)i + 1] = gx1;
@@ -199,8 +248,18 @@ __global__ void __launch_bounds__(kPfThreads) point_feats_bwd_kernel(PointFeatsA
 cudaError_t launch_point_feats(const PointFeatsArgs& a, bool backward, cudaStream_t stream) {
     if (a.n <= 0) return cudaSuccess;
     const unsigned grid = (unsigned)((a.n + kPfThreads - 1) / kPfThreads);
-    if (backward) point_feats_bwd_kernel<<<grid, kPfThreads, 0, stream>>>(a);
-    else point_feats_fwd_kernel<<<grid, kPfThreads, 0, stream>>>(a);
+    if (!backward) {
+        point_feats_fwd_kernel<<<grid, kPfThreads, 0, stream>>>(a);
+    } else if (!a.g_fixed) {
+        point_feats_bwd_kernel<false><<<grid, kPfThreads, 0, stream>>>(a);
+    } else {
+        const size_t count = (size_t)a.V * 8 * a.n;
+        pf_bound_kernel<<<(unsigned)min((count + kPfThreads - 1) / kPfThreads, (size_t)sm_count() * 8), kPfThreads, 0, stream>>>(
+            a.g_feats, count, a.det);
+        point_feats_bwd_kernel<true><<<grid, kPfThreads, 0, stream>>>(a);
+        const size_t planes = 5 * (size_t)a.V * a.H * a.W;
+        pf_convert_kernel<<<(unsigned)((planes + kPfThreads - 1) / kPfThreads), kPfThreads, 0, stream>>>(a);
+    }
     return cudaGetLastError();
 }
 

@@ -27,6 +27,7 @@
 // narrow band around rho3d = rho2d (eval_pair_bwd below); which pairs were blended it takes from the record.
 // What is kept from round 1: tiles in LPT order (one 4-warp CTA per 16x8 half tile, five per SM), the list walked back
 // to front from the tile's deepest used entry in staged rounds, paired fp32 arithmetic, MUFU.RCP.
+#include "det_sum.cuh"
 #include "surfel_common.cuh"
 #include "surfel_kernels.h"
 
@@ -112,6 +113,58 @@ struct BwdSmem {
     static constexpr size_t total = wmax + sizeof(int) * kBwdWarps;
 };
 
+// What phase 2 does with a lane's 18 partial sums (its epilogue).  kEpiFloat is the default path: red.add into the fp32
+// gradient record, in whatever order the lanes arrive.  The deterministic path (DESIGN §3.13) runs the same kernel body
+// twice over DetRecords (a.ggrad): kEpiBound takes each channel's largest |partial| and counts the partials, kEpiFixed
+// adds them in 64-bit fixed point scaled by that bound; det_convert_kernel turns the sums into the fp32 record.
+enum BwdEpilogue { kEpiFloat = 0, kEpiBound = 1, kEpiFixed = 2 };
+
+// one (Gaussian, view) of the deterministic path: the 18 channels of the gradient record
+struct DetRecord {
+    long long sum[18];           // kEpiFixed: sum of round(partial 2^k)
+    uint32_t bound[18];          // kEpiBound: largest |partial| (fp32 bits)
+    uint32_t count;              // kEpiBound: number of lanes that sent partials
+    uint32_t overflow;           // kEpiFixed: a partial was over its budget or not finite
+};
+static_assert(sizeof(DetRecord) == 224 && sizeof(DetRecord) % 16 == 0, "DetRecord is read with vector loads");
+
+__device__ __forceinline__ void red_add_u64(long long* addr, long long v) {
+    asm volatile("red.global.add.u64 [%0], %1;" ::"l"(addr), "l"(v) : "memory");
+}
+
+template <int kEpi>
+__device__ __forceinline__ void det_epilogue(DetRecord* r, const float (&v)[18]) {
+    if (kEpi == kEpiBound) {
+        atomicAdd(&r->count, 1u);
+#pragma unroll
+        for (int c = 0; c < 18; ++c) {
+            const uint32_t b = det::abs_bits(v[c]);
+            if (b != 0u) atomicMax(&r->bound[c], b);
+        }
+    } else {
+        const int L = det::ceil_log2(__ldg(&r->count));
+        const uint4* bq = reinterpret_cast<const uint4*>(r->bound);
+        uint32_t bd[18];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const uint4 t = __ldg(bq + k);
+            bd[4 * k] = t.x; bd[4 * k + 1] = t.y; bd[4 * k + 2] = t.z; bd[4 * k + 3] = t.w;
+        }
+        const uint2 t2 = __ldg(reinterpret_cast<const uint2*>(r->bound + 16));
+        bd[16] = t2.x; bd[17] = t2.y;
+        bool ok = true;
+#pragma unroll
+        for (int c = 0; c < 18; ++c) {
+            if (v[c] == 0.0f) continue;
+            long long q;
+            ok &= det::quantize(v[c], det::scale_exp(bd[c], L), L, q);
+            if (q != 0) red_add_u64(&r->sum[c], q);
+        }
+        if (!ok) atomicOr(&r->overflow, 1u);
+    }
+}
+
+template <int kEpi>
 __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(RenderBwdArgs a) {
     static_assert(kBwdBatch <= 256, "hit lists are uint8");
     static_assert(kBwdBatch == kBwdThreads, "every thread stages one list entry per round");
@@ -485,14 +538,20 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
                         }
                     } while (--n_take != 0);
                     // the lane's partial sums
-                    float* dst = a.ggrad + (size_t)splat_id * SRF_GRAD_FLOATS;
                     const float2 a0 = up2(A0), a1 = up2(A1), a2 = up2(A2), a3 = up2(A3), a8 = up2(A8);
                     const float2 a4 = up2(A4), a5 = up2(A5), a6 = up2(A6), a7 = up2(A7);
-                    red_add_v4(dst + 0, a0.x, a0.y, a1.x, a1.y);
-                    red_add_v4(dst + 4, a2.x, a2.y, a3.x, a3.y);
-                    red_add_v4(dst + 8, a4.x, a4.y, a5.x, a5.y);
-                    red_add_v4(dst + 12, a6.x, a6.y, a7.x, a7.y);
-                    if (a8.x != 0.0f || a8.y != 0.0f) red_add_v4(dst + 16, a8.x, a8.y, 0.0f, 0.0f);
+                    if (kEpi == kEpiFloat) {
+                        float* dst = a.ggrad + (size_t)splat_id * SRF_GRAD_FLOATS;
+                        red_add_v4(dst + 0, a0.x, a0.y, a1.x, a1.y);
+                        red_add_v4(dst + 4, a2.x, a2.y, a3.x, a3.y);
+                        red_add_v4(dst + 8, a4.x, a4.y, a5.x, a5.y);
+                        red_add_v4(dst + 12, a6.x, a6.y, a7.x, a7.y);
+                        if (a8.x != 0.0f || a8.y != 0.0f) red_add_v4(dst + 16, a8.x, a8.y, 0.0f, 0.0f);
+                    } else {
+                        const float v[18] = {a0.x, a0.y, a1.x, a1.y, a2.x, a2.y, a3.x, a3.y, a4.x, a4.y,
+                                             a5.x, a5.y, a6.x, a6.y, a7.x, a7.y, a8.x, a8.y};
+                        det_epilogue<kEpi>(reinterpret_cast<DetRecord*>(a.ggrad) + splat_id, v);
+                    }
                 }
                 __syncwarp();     // phase 1 of the next group overwrites the X tile
             }
@@ -500,18 +559,57 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
     }
 }
 
+// one thread per (Gaussian, view): the fixed-point sums of a DetRecord -> the fp32 gradient record preprocess_bwd reads
+__global__ void __launch_bounds__(256) det_convert_kernel(const DetRecord* det, size_t det_stride, float* ggrad,
+                                                          size_t ggrad_stride, int P, int nviews, uint32_t* overflow) {
+    const size_t i = (size_t)blockIdx.x * 256 + threadIdx.x;
+    if (i >= (size_t)P * nviews) return;
+    const int view = (int)(i / (size_t)P), g = (int)(i - (size_t)view * P);
+    const DetRecord* r = view_ptr(det, view, det_stride) + g;
+    float4* out = reinterpret_cast<float4*>(view_ptr(ggrad, view, ggrad_stride) + (size_t)g * SRF_GRAD_FLOATS);
+    const int L = det::ceil_log2(r->count);
+    float f[20];
+#pragma unroll
+    for (int c = 0; c < 18; ++c) f[c] = det::to_float(r->sum[c], det::scale_exp(r->bound[c], L));
+    f[18] = f[19] = 0.0f;
+#pragma unroll
+    for (int k = 0; k < 5; ++k) out[k] = make_float4(f[4 * k], f[4 * k + 1], f[4 * k + 2], f[4 * k + 3]);
+    if (r->overflow) atomicOr(overflow, 1u);
+}
+
+template <int kEpi>
+cudaError_t launch_render_bwd_t(const RenderBwdArgs& a, cudaStream_t stream) {
+    const int ntiles = a.gx * a.gy;
+    prof_start(K_RENDER_BWD, stream);
+    // the opt-in is per device (and cheap): made on every call for the current device
+    cudaError_t e = cudaFuncSetAttribute(render_bwd_kernel<kEpi>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BwdSmem::total);
+    if (e == cudaSuccess)
+        render_bwd_kernel<kEpi><<<dim3(ntiles * 2, a.nviews), kBwdThreads, BwdSmem::total, stream>>>(a);   // two CTAs per tile
+    prof_stop(K_RENDER_BWD, stream);
+    return e != cudaSuccess ? e : cudaGetLastError();
+}
+
 }  // namespace
+
+size_t det_record_bytes() { return sizeof(DetRecord); }
 
 cudaError_t launch_render_bwd(const RenderBwdArgs& a, cudaStream_t stream) {
     const int ntiles = a.gx * a.gy;
     if (ntiles <= 0 || a.nviews <= 0) return cudaSuccess;
-    prof_start(K_RENDER_BWD, stream);
-    // the opt-in is per device (and cheap): made on every call for the current device
-    cudaError_t e = cudaFuncSetAttribute(render_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BwdSmem::total);
-    if (e == cudaSuccess)
-        render_bwd_kernel<<<dim3(ntiles * 2, a.nviews), kBwdThreads, BwdSmem::total, stream>>>(a);   // two CTAs per tile
-    prof_stop(K_RENDER_BWD, stream);
-    return e != cudaSuccess ? e : cudaGetLastError();
+    return launch_render_bwd_t<kEpiFloat>(a, stream);
+}
+
+cudaError_t launch_render_bwd_det(const RenderBwdArgs& a, int P, float* ggrad, size_t ggrad_stride, uint32_t* overflow,
+                                  cudaStream_t stream) {
+    const int ntiles = a.gx * a.gy;
+    if (ntiles <= 0 || a.nviews <= 0 || P <= 0) return cudaSuccess;
+    cudaError_t e = launch_render_bwd_t<kEpiBound>(a, stream);
+    if (e == cudaSuccess) e = launch_render_bwd_t<kEpiFixed>(a, stream);
+    if (e != cudaSuccess) return e;
+    const size_t n = (size_t)P * a.nviews;
+    det_convert_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const DetRecord*>(a.ggrad),
+                                                                        a.ggrad_stride, ggrad, ggrad_stride, P, a.nviews, overflow);
+    return cudaGetLastError();
 }
 
 }  // namespace srf

@@ -172,11 +172,14 @@ struct LossArgs {
     const float* acc;            // [V,H,W]
     const float* dist;           // [V,H,W]
     double* sums;                // [3]: sum (image-target)^2, sum dist, sum (1 - <rn,dn>) acc   (zeroed by the caller); null = skip
+    double* partials;            // [loss_det_blocks][3] or null: deterministic sums (written, then reduced in a fixed order)
     const float* gout;           // device scalar: upstream gradient of the loss (null = 1)
     float* g_image;              // [V,3,H,W] out (may be null: forward statistics only)
     float* g_rend_normal; float* g_depth_normal; float* g_dist;
 };
 cudaError_t launch_loss_fused(const LossArgs& a, cudaStream_t stream);
+constexpr int kLossDetBlocks = 1024;
+size_t loss_det_blocks(size_t total);            // blocks (= partial-sum triples) of the deterministic sums
 
 // Decoder epilogue (SURVEY 8f rank 4, lightning/network.py:261-278, 425-429): MLP output rows -> the five
 // contiguous parameter tensors, and the mirror-image backward.
@@ -207,6 +210,11 @@ struct PointFeatsArgs {
     const float* g_feats;        // [V,8,n] backward input
     float* g_points;             // [n,3] written (may be null)
     float* g_image; float* g_acc; float* g_depth;   // accumulated into, cleared by the caller (each may be null)
+    // deterministic backward (null = default): int64 planes [5V,H,W] in the layout g_image | g_acc | g_depth and a
+    // header det[0] = max |g_feats| (fp32 bits), det[1] = overflow; both zeroed by the caller.  The float outputs are
+    // then written, not accumulated into.
+    long long* g_fixed;
+    uint32_t* det;
 };
 cudaError_t launch_point_feats(const PointFeatsArgs& a, bool backward, cudaStream_t stream);
 
@@ -242,6 +250,12 @@ cudaError_t launch_tile_scan(const BinArgs& a, cudaStream_t stream);
 cudaError_t launch_bin_and_sort(const BinArgs& a, cudaStream_t stream);
 cudaError_t launch_render_fwd(const RenderFwdArgs& a, cudaStream_t stream);
 cudaError_t launch_render_bwd(const RenderBwdArgs& a, cudaStream_t stream);
+// Deterministic blend backward (DESIGN §3.13): a.ggrad / a.ggrad_stride point at zeroed det_record_bytes() records per
+// (Gaussian, view); the fp32 gradient records preprocess_bwd reads go to ggrad / ggrad_stride; *overflow (zeroed by the
+// caller) is set if a partial sum was over its fixed-point budget.
+size_t det_record_bytes();
+cudaError_t launch_render_bwd_det(const RenderBwdArgs& a, int P, float* ggrad, size_t ggrad_stride, uint32_t* overflow,
+                                  cudaStream_t stream);
 cudaError_t launch_preprocess_bwd(const PreprocessBwdArgs& a, cudaStream_t stream);
 
 }  // namespace srf

@@ -44,9 +44,14 @@ class _SceneLoss(torch.autograd.Function):
             raise RuntimeError(f"scene_loss: tar_rgb must be [V,H,W,3] = {(V, H, W, 3)}, got {tuple(target.shape)}")
         sums = torch.empty(3, dtype=torch.float64, device=dev)
         p = lambda t: 0 if t is None else t.data_ptr()      # noqa: E731
+        args = (_raw_stream(dev), V, H, W, 1 if with_reg else 0, image.data_ptr(), target.data_ptr(),
+                p(rend_normal), p(depth_normal), p(acc_map), p(rend_dist), sums.data_ptr())
         with _DeviceGuard(dev):
-            _lib.check(lib.srf_loss_forward(_raw_stream(dev), V, H, W, 1 if with_reg else 0, image.data_ptr(), target.data_ptr(),
-                                            p(rend_normal), p(depth_normal), p(acc_map), p(rend_dist), sums.data_ptr()), lib)
+            if _lib.deterministic():         # partial sums reduced in a fixed order instead of atomics
+                ws = torch.empty(_lib.det_loss_workspace_bytes(lib, V, H, W) // 8, dtype=torch.float64, device=dev)
+                _lib.check(lib.srf_loss_forward_deterministic(*args, ws.data_ptr()), lib)
+            else:
+                _lib.check(lib.srf_loss_forward(*args), lib)
         npx = float(batch_scenes) * V * H * W
         mse = sums[0] / (3.0 * npx)
         dist = sums[1] / npx

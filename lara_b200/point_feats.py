@@ -103,9 +103,15 @@ class _PointFeats(torch.autograd.Function):
             new(need[4], V, 1, H, W)
         g_feats = g_feats.contiguous()
         with _DeviceGuard(dev):
-            _lib.check(lib.srf_point_feats_backward(_raw_stream(dev), V, n, H, W, *[t.data_ptr() for t in ins],
-                                                    g_feats.data_ptr(), _p(g_points), _p(g_image), _p(g_acc),
-                                                    _p(g_depth)), lib)
+            if _lib.deterministic():
+                ws = torch.empty(_lib.det_point_feats_workspace_bytes(lib, V, H, W), dtype=torch.uint8, device=dev)
+                _lib.check(lib.srf_point_feats_backward_deterministic(
+                    _raw_stream(dev), V, n, H, W, *[t.data_ptr() for t in ins], g_feats.data_ptr(), _p(g_points),
+                    _p(g_image), _p(g_acc), _p(g_depth), ws.data_ptr()), lib)
+            else:
+                _lib.check(lib.srf_point_feats_backward(_raw_stream(dev), V, n, H, W, *[t.data_ptr() for t in ins],
+                                                        g_feats.data_ptr(), _p(g_points), _p(g_image), _p(g_acc),
+                                                        _p(g_depth)), lib)
         return g_points, None, g_image, g_acc, g_depth, None, None
 
 

@@ -466,22 +466,24 @@ def _grad_outputs(P, M, device, shs, colors_precomp, transMat_precomp, out, accu
 def backward_raw(state: ForwardState, radii, means3D, shs, colors_precomp, scales, rotations,
                  transMat_precomp, raster_settings, grad_color, grad_allmap, *,
                  out: Optional[dict] = None, accumulate: bool = False, need_means2D: bool = True,
-                 raw_activations: bool = False):
+                 raw_activations: bool = False, deterministic: Optional[bool] = None):
     """Enqueue one backward; returns a dict of gradient tensors.
 
     ``out`` may supply pre-allocated (possibly strided-into-a-flat-buffer but contiguous)
     tensors for 'means3D','sh','opacities','scales','rotations'; with ``accumulate`` the
     kernel adds into them (view-sharded accumulation).
+    ``deterministic``: bit-reproducible gradients (fixed-point sums of the blend backward, DESIGN §3.13; the call then
+    waits for the GPU); ``None`` follows ``torch.use_deterministic_algorithms``.
     """
     with _DeviceGuard(means3D.device):
         return _backward_raw(state, radii, means3D, shs, colors_precomp, scales, rotations, transMat_precomp,
                              raster_settings, grad_color, grad_allmap, out=out, accumulate=accumulate,
-                             need_means2D=need_means2D, raw_activations=raw_activations)
+                             need_means2D=need_means2D, raw_activations=raw_activations, deterministic=deterministic)
 
 
 def _backward_raw(state, radii, means3D, shs, colors_precomp, scales, rotations, transMat_precomp,
                   raster_settings, grad_color, grad_allmap, *, out=None, accumulate=False, need_means2D=True,
-                  raw_activations=False):
+                  raw_activations=False, deterministic=None):
     lib = _lib.load()
     H, W = int(raster_settings.image_height), int(raster_settings.image_width)
     P = int(means3D.shape[0])
@@ -491,6 +493,14 @@ def _backward_raw(state, radii, means3D, shs, colors_precomp, scales, rotations,
     if P == 0:
         return g
     state.resolve()                 # capacity verified (re-run if it overflowed) before the lists are walked again
+    if _lib.deterministic(deterministic):
+        # the views entry with V = 1: one camera record
+        cams = pack_cameras([raster_settings], device)
+        _views_backward(lib, lib.srf_views_backward_deterministic, _lib.det_backward_scratch_bytes(lib, 1, P), state,
+                        radii, means3D, shs, colors_precomp, scales, rotations, transMat_precomp, cams,
+                        raster_settings.tanfovx, raster_settings.tanfovy, H, W, raster_settings.sh_degree, grad_color,
+                        grad_allmap, g, accumulate, raw_activations)
+        return g
     _, _, _, scratch_b = _sizes(lib, P, H, W)
     scratch = _blob(scratch_b, device)
     sptr = _raw_stream(device)
@@ -515,9 +525,11 @@ def _backward_raw(state, radii, means3D, shs, colors_precomp, scales, rotations,
 def backward_views_raw(state: ForwardState, radii, means3D, shs, colors_precomp, scales, rotations, transMat_precomp,
                        cams: torch.Tensor, tanfovx: float, tanfovy: float, H: int, W: int, sh_degree: int,
                        grad_color, grad_allmap, *, out: Optional[dict] = None, accumulate: bool = False,
-                       need_means2D: bool = False, raw_activations: bool = False, debug: bool = False):
+                       need_means2D: bool = False, raw_activations: bool = False, debug: bool = False,
+                       deterministic: Optional[bool] = None):
     """Backward of forward_views_raw: grad_color [V,3,H,W], grad_allmap [V,8,H,W]; the per-Gaussian backward
-    sums the V views in registers and writes (accumulate: adds into) every parameter-gradient row once."""
+    sums the V views in registers and writes (accumulate: adds into) every parameter-gradient row once.
+    ``deterministic`` as in :func:`backward_raw`."""
     with _DeviceGuard(means3D.device):
         lib = _lib.load()
         device = means3D.device
@@ -527,21 +539,35 @@ def backward_views_raw(state: ForwardState, radii, means3D, shs, colors_precomp,
         if P == 0:
             return g
         state.resolve()
-        scratch_b = _lib.views_sizes(lib, V, P, H, W, 0)[5]
-        scratch = _blob(scratch_b, device)
-        _lib.check(lib.srf_views_backward(
-            _raw_stream(device), V, P, int(sh_degree), M, H, W, state.capacity, cams.data_ptr(),
-            _ptr(means3D), _ptr(shs), 1 if colors_precomp is not None else 0,
-            _ptr(scales), _ptr(rotations), 1 if transMat_precomp is not None else 0,
-            float(tanfovx), float(tanfovy), radii.data_ptr(),
-            state.geom.data_ptr(), state.tile.data_ptr(), state.point_list.data_ptr(), state.image.data_ptr(),
-            grad_color.data_ptr(), grad_allmap.data_ptr(), scratch.data_ptr(), 1 if accumulate else 0,
-            _ptr(g["means3D"]), _ptr(g["means2D"]), _ptr(g["sh"]), _ptr(g["colors_precomp"]),
-            _ptr(g["opacities"]), _ptr(g["scales"]), _ptr(g["rotations"]), _ptr(g["cov3Ds_precomp"]),
-            1 if raw_activations else 0), lib)
+        if _lib.deterministic(deterministic):
+            fn, scratch_b = lib.srf_views_backward_deterministic, _lib.det_backward_scratch_bytes(lib, V, P)
+        else:
+            fn, scratch_b = lib.srf_views_backward, _lib.views_sizes(lib, V, P, H, W, 0)[5]
+        _views_backward(lib, fn, scratch_b, state, radii, means3D, shs, colors_precomp, scales, rotations,
+                        transMat_precomp, cams, tanfovx, tanfovy, H, W, sh_degree, grad_color, grad_allmap, g,
+                        accumulate, raw_activations)
         if debug:
             torch.cuda.synchronize(device)
         return g
+
+
+def _views_backward(lib, fn, scratch_b, state, radii, means3D, shs, colors_precomp, scales, rotations, transMat_precomp,
+                    cams, tanfovx, tanfovy, H, W, sh_degree, grad_color, grad_allmap, g, accumulate, raw_activations):
+    """One call of srf_views_backward or srf_views_backward_deterministic (same arguments)."""
+    device = means3D.device
+    V, P = int(cams.shape[0]), int(means3D.shape[0])
+    M = int(shs.shape[1]) if shs is not None else 0
+    scratch = _blob(scratch_b, device)
+    _lib.check(fn(
+        _raw_stream(device), V, P, int(sh_degree), M, H, W, state.capacity, cams.data_ptr(),
+        _ptr(means3D), _ptr(shs), 1 if colors_precomp is not None else 0,
+        _ptr(scales), _ptr(rotations), 1 if transMat_precomp is not None else 0,
+        float(tanfovx), float(tanfovy), radii.data_ptr(),
+        state.geom.data_ptr(), state.tile.data_ptr(), state.point_list.data_ptr(), state.image.data_ptr(),
+        grad_color.data_ptr(), grad_allmap.data_ptr(), scratch.data_ptr(), 1 if accumulate else 0,
+        _ptr(g["means3D"]), _ptr(g["means2D"]), _ptr(g["sh"]), _ptr(g["colors_precomp"]),
+        _ptr(g["opacities"]), _ptr(g["scales"]), _ptr(g["rotations"]), _ptr(g["cov3Ds_precomp"]),
+        1 if raw_activations else 0), lib)
 
 
 def _dump_snapshot(path: str, items) -> None:
