@@ -179,7 +179,8 @@ __global__ void __launch_bounds__(256) epilogue_bwd_kernel(EpilogueArgs a) {
     float d_D = 0.f;
     if (q_ok) {
         d_D = g_exp / alpha;
-        d_alpha += -g_exp * D / (alpha * alpha);
+        // torch's div backward, -g * ((D / alpha) / alpha): alpha * alpha would underflow to 0 below alpha ~ 1e-19
+        d_alpha += -g_exp * (q / alpha);
     }
     a.dL_dallmap[pix] = d_D;
     a.dL_dallmap[pix + npix] = d_alpha;

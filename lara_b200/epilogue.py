@@ -12,7 +12,8 @@ switch ``Renderer.render_img`` to it with a two-line change::
     return render_img_epilogue(rendered_image, allmap, rays, cam.world_view_transform, depth_ratio, prex)
 
 One deliberate difference: where the reference's autograd produces NaN gradients (0/0 in the
-backward of ``D / alpha`` at pixels with alpha == 0) the fused backward produces 0.
+backward of ``D / alpha`` at pixels with alpha == 0, 0 * inf where fp32 ``D / alpha`` overflows, 0 * NaN at a
+non-finite median depth) the fused backward produces 0.
 """
 from __future__ import annotations
 
