@@ -14,7 +14,7 @@ from typing import Optional
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libsurfel_b200.so")
-ABI_VERSION = 7
+ABI_VERSION = 8
 CAM_FLOATS, CAM_VIEW, CAM_CAMPOS, CAM_BG = 24, 0, 16, 19      # include/surfel_rasterizer.h SRF_CAM_*
 
 
@@ -30,67 +30,17 @@ _P = c_void_p
 SIGNATURES = {
     "srf_abi_version": (c_int, []),
     "srf_last_error": (c_char_p, []),
-    "srf_geom_state_bytes": (c_int, [c_int, POINTER(c_size_t)]),
-    "srf_tile_state_bytes": (c_int, [c_int, c_int, POINTER(c_size_t)]),
-    "srf_image_state_bytes": (c_int, [c_int, c_int, POINTER(c_size_t)]),
-    "srf_binning_bytes": (c_int, [c_size_t, POINTER(c_size_t), POINTER(c_size_t)]),
-    "srf_backward_scratch_bytes": (c_int, [c_int, POINTER(c_size_t)]),
-    "srf_state_layout": (c_int, [c_int, c_int, c_int, POINTER(c_size_t), POINTER(c_size_t), POINTER(c_size_t)]),
-    "srf_forward_preprocess": (c_int, [
-        _P, c_int, c_int, c_int,            # stream, P, D, M
-        _P, _P, _P,                         # means3D, shs, colors_precomp
-        _P, _P, c_float,                    # opacities, scales, scale_modifier
-        _P, _P,                             # rotations, transMat_precomp
-        _P, _P, _P,                         # viewmatrix, projmatrix, campos
-        c_float, c_float, c_int, c_int,     # tan_fovx, tan_fovy, H, W
-        c_int,                              # prefiltered
-        _P, _P, _P,                         # radii, geom_state, tile_state
-        _P,                                 # num_rendered_host
-        c_int,                              # raw_activations
-    ]),
-    "srf_forward_render": (c_int, [
-        _P, c_int, c_int, c_int,            # stream, P, H, W
-        c_size_t, _P, _P,                   # capacity, geom_state, tile_state
-        _P, _P, _P,                         # entries, point_list, image_state
-        _P, _P, _P,                         # background, out_color, out_others
-    ]),
-    "srf_forward": (c_int, [
-        _P, c_int, c_int, c_int,            # stream, P, D, M
-        _P, _P, _P,                         # means3D, shs, colors_precomp
-        _P, _P, c_float,                    # opacities, scales, scale_modifier
-        _P, _P,                             # rotations, transMat_precomp
-        _P, _P, _P,                         # viewmatrix, projmatrix, campos
-        c_float, c_float, c_int, c_int,     # tan_fovx, tan_fovy, H, W
-        c_int,                              # prefiltered
-        _P, c_size_t,                       # background, capacity
-        _P, _P, _P, _P, _P, _P,             # radii, geom_state, tile_state, entries, point_list, image_state
-        _P, _P, _P, _P,                     # out_color, out_others, num_rendered_host, count_event
-        c_int,                              # raw_activations
-    ]),
-    "srf_backward": (c_int, [
-        _P, c_int, c_int, c_int, c_int, c_int,   # stream, P, D, M, H, W
-        c_size_t, _P,                            # capacity, background
-        _P, _P, c_int,                           # means3D, shs, colors_were_precomputed
-        _P, _P, c_int,                           # scales, rotations, transmat_was_precomputed
-        _P, _P, _P,                              # viewmatrix, projmatrix, campos
-        c_float, c_float, _P,                    # tan_fovx, tan_fovy, radii
-        _P, _P, _P, _P,                          # geom_state, tile_state, point_list, image_state
-        _P, _P,                                  # dL_dout_color, dL_dout_others
-        _P, c_int,                               # scratch, accumulate
-        _P, _P, _P, _P,                          # dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors
-        _P, _P, _P, _P,                          # dL_dopacity, dL_dscales, dL_drotations, dL_dtransMat
-        c_int,                                   # raw_activations
-    ]),
     "srf_views_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, c_size_t, POINTER(c_size_t)]),
-    "srf_views_forward_preprocess": (c_int, [
+    "srf_state_layout": (c_int, [c_int, c_int, c_int, POINTER(c_size_t), POINTER(c_size_t), POINTER(c_size_t)]),
+    "srf_views_forward": (c_int, [
         _P, c_int, c_int, c_int, c_int,     # stream, V, P, D, M
         _P, _P, _P,                         # means3D, shs, colors_precomp
         _P, _P, _P,                         # opacities, scales, rotations
         _P, _P,                             # transMat_precomp, cams
         c_float, c_float, c_int, c_int,     # tan_fovx, tan_fovy, H, W
-        c_int,                              # prefiltered
-        _P, _P, _P,                         # radii, geom_state, tile_state
-        _P,                                 # num_rendered_host
+        c_int, c_size_t,                    # prefiltered, capacity
+        _P, _P, _P, _P, _P, _P,             # radii, geom_state, tile_state, entries, point_list, image_state
+        _P, _P, _P, _P,                     # out_color, out_others, num_rendered_host, count_event
         c_int,                              # raw_activations
     ]),
     "srf_views_forward_render": (c_int, [
@@ -143,8 +93,6 @@ SIGNATURES = {
     "srf_ms_ssim_forward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _A, _P, _A, c_float, c_int, _P, _P]),
     "srf_ms_ssim_backward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _A, _P, _A, c_float, c_int, _P, _P, _P, _A]),
     "srf_mark_visible": (c_int, [_P, c_int, _P, _P, _P, _P]),
-    "srf_epilogue_forward": (c_int, [_P, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
-    "srf_epilogue_backward": (c_int, [_P, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "srf_profile_begin": (c_int, []),
     "srf_profile_end": (c_int, [POINTER(c_float), POINTER(c_int), c_int]),
 }
@@ -186,21 +134,6 @@ def check(status: int, lib=None) -> None:
         l = lib or _lib
         msg = l.srf_last_error().decode("utf-8", "replace") if l is not None else "unknown error"
         raise RuntimeError(msg)
-
-
-def sizes(lib, P: int, H: int, W: int):
-    g, t, i, s = c_size_t(), c_size_t(), c_size_t(), c_size_t()
-    check(lib.srf_geom_state_bytes(P, ctypes.byref(g)), lib)
-    check(lib.srf_tile_state_bytes(H, W, ctypes.byref(t)), lib)
-    check(lib.srf_image_state_bytes(H, W, ctypes.byref(i)), lib)
-    check(lib.srf_backward_scratch_bytes(P, ctypes.byref(s)), lib)
-    return g.value, t.value, i.value, s.value
-
-
-def binning_sizes(lib, capacity: int):
-    e, p = c_size_t(), c_size_t()
-    check(lib.srf_binning_bytes(capacity, ctypes.byref(e), ctypes.byref(p)), lib)
-    return e.value, p.value
 
 
 def views_sizes(lib, V: int, P: int, H: int, W: int, capacity: int):

@@ -85,6 +85,13 @@ size_t plist_masks_offset(size_t capacity) { return align_up(capacity * sizeof(u
 size_t plist_stride_bytes(size_t capacity) {
     return plist_masks_offset(capacity) + align_up(capacity * 8 * sizeof(uint32_t)) + 256;
 }
+size_t entries_stride_bytes(size_t capacity) { return align_up(capacity * sizeof(uint64_t)) + 256; }
+size_t ggrad_stride_bytes(int P) { return align_up((size_t)P * SRF_GRAD_FLOATS * sizeof(float)) + 256; }
+
+// Scratch of the deterministic backward: V fp32 gradient-record arrays (as srf_views_backward's scratch), then V arrays
+// of fixed-point records, then the overflow flag.
+size_t det_stride_bytes(int P) { return align_up((size_t)P * srf::det_record_bytes()); }
+size_t det_scratch_bytes(int V, int P) { return (ggrad_stride_bytes(P) + det_stride_bytes(P)) * (size_t)V + 256; }
 
 // ---- optional per-kernel timing --------------------------------------------------
 struct ProfSpan { int kernel; cudaEvent_t start, stop; };
@@ -164,34 +171,14 @@ int srf_profile_end(float* ms_out, int* launches_out, int n) {
 }
 const char* srf_last_error(void) { return g_err; }
 
-int srf_geom_state_bytes(int P, size_t* bytes) {
-    if (P < 0 || !bytes) return fail("srf_geom_state_bytes: bad arguments");
-    *bytes = geom_layout(P).total;
-    return 0;
-}
-
-int srf_tile_state_bytes(int H, int W, size_t* bytes) {
-    if (H <= 0 || W <= 0 || !bytes) return fail("srf_tile_state_bytes: bad arguments");
-    *bytes = tile_layout(H, W).total;
-    return 0;
-}
-
-int srf_image_state_bytes(int H, int W, size_t* bytes) {
-    if (H <= 0 || W <= 0 || !bytes) return fail("srf_image_state_bytes: bad arguments");
-    *bytes = image_layout(H, W).total;
-    return 0;
-}
-
-int srf_binning_bytes(size_t capacity, size_t* entries_bytes, size_t* point_list_bytes) {
-    if (!entries_bytes || !point_list_bytes) return fail("srf_binning_bytes: bad arguments");
-    *entries_bytes = align_up(capacity * sizeof(uint64_t)) + 256;
-    *point_list_bytes = plist_stride_bytes(capacity);
-    return 0;
-}
-
-int srf_backward_scratch_bytes(int P, size_t* bytes) {
-    if (P < 0 || !bytes) return fail("srf_backward_scratch_bytes: bad arguments");
-    *bytes = align_up((size_t)P * SRF_GRAD_FLOATS * sizeof(float)) + 256;
+int srf_views_workspace_bytes(int V, int P, int H, int W, size_t capacity, size_t bytes[6]) {
+    if (V <= 0 || P < 0 || H <= 0 || W <= 0 || !bytes) return fail("srf_views_workspace_bytes: bad arguments");
+    bytes[0] = geom_layout(P).total * (size_t)V;
+    bytes[1] = tile_layout(H, W).total * (size_t)V;
+    bytes[2] = image_layout(H, W).total * (size_t)V;
+    bytes[3] = entries_stride_bytes(capacity) * (size_t)V;
+    bytes[4] = plist_stride_bytes(capacity) * (size_t)V;
+    bytes[5] = ggrad_stride_bytes(P) * (size_t)V;
     return 0;
 }
 
@@ -209,25 +196,10 @@ int srf_state_layout(int P, int H, int W, size_t geom_off[3], size_t tile_off[5]
 }  // extern "C"
 
 // ---------------------------------------------------------------------------------------------
-// Implementation shared by the per-view entry points (the reference's interface, one view per call)
-// and the srf_views_* entry points (all V target views of one scene in one launch set).
+// Implementation of the srf_views_* entry points: V views of one scene in one launch set, each view's
+// camera a record of SRF_CAM_FLOATS floats in `cams`, each view's workspaces one layout stride apart.
 // ---------------------------------------------------------------------------------------------
 namespace {
-
-struct Cams {               // per-view camera data: three pointers into records `stride` floats apart
-    const float* view;
-    const float* campos;
-    const float* bg;
-    size_t stride;
-};
-
-size_t entries_stride_bytes(size_t capacity) { return align_up(capacity * sizeof(uint64_t)) + 256; }
-size_t ggrad_stride_bytes(int P) { return align_up((size_t)P * SRF_GRAD_FLOATS * sizeof(float)) + 256; }
-
-// Scratch of the deterministic backward: V fp32 gradient-record arrays (as srf_views_backward's scratch), then V arrays
-// of fixed-point records, then the overflow flag.
-size_t det_stride_bytes(int P) { return align_up((size_t)P * srf::det_record_bytes()); }
-size_t det_scratch_bytes(int V, int P) { return (ggrad_stride_bytes(P) + det_stride_bytes(P)) * (size_t)V + 256; }
 
 // reads a device flag that the work enqueued so far sets: waits for the stream
 int check_overflow_flag(const char* fn, const uint32_t* flag, cudaStream_t stream) {
@@ -248,13 +220,14 @@ void fill_bin_args(srf::BinArgs& b, int V, int P, const TileLayout& tl, void* ti
     b.ranges = at<uint2>(tile_state, tl.ranges);
     b.big_list = at<uint32_t>(tile_state, tl.big);
     b.tile_order = at<uint32_t>(tile_state, tl.order);
-    b.tile_stride = V > 1 ? tl.total : 0;
+    b.tile_stride = tl.total;
 }
 
+// stage 1: preprocess, per-tile counting, tile scan and the count read-back
 int forward_preprocess_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int M,
                             const float* means3D, const float* shs, const float* colors_precomp,
                             const float* opacities, const float* scales, const float* rotations,
-                            const float* transMat_precomp, Cams cams,
+                            const float* transMat_precomp, const float* cams,
                             float tan_fovx, float tan_fovy, int image_height, int image_width,
                             int prefiltered, int* radii, void* geom_state, void* tile_state,
                             uint32_t* num_rendered_host, int raw_activations) {
@@ -272,8 +245,7 @@ int forward_preprocess_impl(const char* fn, cudaStream_t stream, int V, int P, i
     fill_bin_args(b, V, P, tl, tile_state);
 
     if (P > 0) {
-        if (!means3D || !opacities || !cams.view || !cams.campos || !radii)
-            return fail("%s: null required pointer", fn);
+        if (!means3D || !opacities || !radii) return fail("%s: null required pointer", fn);
         if ((shs == nullptr) == (colors_precomp == nullptr))
             return fail("Please provide excatly one of either SHs or precomputed colors!");
         if (((scales == nullptr || rotations == nullptr) && transMat_precomp == nullptr) ||
@@ -289,7 +261,7 @@ int forward_preprocess_impl(const char* fn, cudaStream_t stream, int V, int P, i
         a.P = P; a.D = D; a.M = shs ? M : 0; a.nviews = V;
         a.means3D = means3D; a.scales = scales; a.rotations = rotations; a.opacities = opacities;
         a.shs = shs; a.transMat_precomp = transMat_precomp; a.colors_precomp = colors_precomp;
-        a.viewmatrix = cams.view; a.campos = cams.campos; a.cam_stride = cams.stride;
+        a.viewmatrix = cams + SRF_CAM_VIEW; a.campos = cams + SRF_CAM_CAMPOS; a.cam_stride = SRF_CAM_FLOATS;
         a.W = image_width; a.H = image_height;
         a.focal_y = image_height / (2.0f * tan_fovy);   // rasterizer_impl.cu:223-224
         a.focal_x = image_width / (2.0f * tan_fovx);
@@ -301,7 +273,7 @@ int forward_preprocess_impl(const char* fn, cudaStream_t stream, int V, int P, i
         a.depths = at<float>(geom_state, gl.depths);
         a.rects = at<uint2>(geom_state, gl.rects);
         a.tile_count = b.tile_count;
-        a.geom_stride = V > 1 ? gl.total : 0;
+        a.geom_stride = gl.total;
         a.tile_stride = b.tile_stride;
         e = srf::launch_preprocess_fwd(a, stream);
         if (e != cudaSuccess) return cuda_fail("preprocess_fwd launch", e);
@@ -329,13 +301,13 @@ int forward_preprocess_impl(const char* fn, cudaStream_t stream, int V, int P, i
     return 0;
 }
 
+// stage 2: scatter into tile buckets, per-tile depth sort, blend
 int forward_render_impl(const char* fn, cudaStream_t stream, int V, int P, int image_height, int image_width,
                         size_t capacity, const void* geom_state, void* tile_state,
                         void* entries, uint32_t* point_list, void* image_state,
-                        const float* background, size_t cam_stride, float* out_color, float* out_others) {
+                        const float* cams, float* out_color, float* out_others) {
     if (V <= 0 || P < 0 || image_height <= 0 || image_width <= 0) return fail("%s: bad sizes", fn);
-    if (!tile_state || !image_state || !background || !out_color || !out_others)
-        return fail("%s: null required pointer", fn);
+    if (!cams || !tile_state || !image_state || !out_color || !out_others) return fail("%s: null required pointer", fn);
     if (capacity > 0xfffffff0ull) return fail("%s: capacity exceeds 32-bit instance indices", fn);
     if (capacity > 0 && (!entries || !point_list)) return fail("%s: null binning buffers", fn);
     const TileLayout tl = tile_layout(image_height, image_width);
@@ -347,9 +319,9 @@ int forward_render_impl(const char* fn, cudaStream_t stream, int V, int P, int i
     b.capacity = (uint32_t)capacity;
     b.entries = static_cast<uint64_t*>(entries);
     b.point_list = point_list;
-    b.geom_stride = V > 1 ? gl.total : 0;
-    b.entries_stride = V > 1 ? entries_stride_bytes(capacity) : 0;
-    b.plist_stride = V > 1 ? plist_stride_bytes(capacity) : 0;
+    b.geom_stride = gl.total;
+    b.entries_stride = entries_stride_bytes(capacity);
+    b.plist_stride = plist_stride_bytes(capacity);
     cudaError_t e;
     if (P > 0) {
         if (!geom_state) return fail("%s: null geom_state", fn);
@@ -368,20 +340,20 @@ int forward_render_impl(const char* fn, cudaStream_t stream, int V, int P, int i
     r.point_list = point_list;
     r.masks = at<uint32_t>(point_list, plist_masks_offset(capacity));
     r.rec = P > 0 ? at<float4>(geom_state, gl.rec) : nullptr;
-    r.bg = background;
+    r.bg = cams + SRF_CAM_BG;
     r.out_color = out_color; r.out_others = out_others;
     r.accum = at<float>(image_state, il.accum);
     r.n_contrib = at<uint32_t>(image_state, il.ncontrib);
     r.geom_stride = b.geom_stride; r.tile_stride = b.tile_stride; r.plist_stride = b.plist_stride;
-    r.image_stride = V > 1 ? il.total : 0;
-    r.cam_stride = cam_stride;
+    r.image_stride = il.total;
+    r.cam_stride = SRF_CAM_FLOATS;
     e = srf::launch_render_fwd(r, stream);
     if (e != cudaSuccess) return cuda_fail("render_fwd launch", e);
     return 0;
 }
 
 int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int M, int image_height, int image_width,
-                  size_t capacity, Cams cams,
+                  size_t capacity, const float* cams,
                   const float* means3D, const float* shs, int colors_were_precomputed,
                   const float* scales, const float* rotations, int transmat_was_precomputed,
                   float tan_fovx, float tan_fovy, const int* radii,
@@ -391,15 +363,15 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
                   void* scratch, int accumulate,
                   float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
                   float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
-                  int raw_activations, bool deterministic = false) {
+                  int raw_activations, bool deterministic) {
+    if (!cams) return fail("%s: null camera records", fn);
     if (V <= 0 || P < 0 || image_height <= 0 || image_width <= 0) return fail("%s: bad sizes", fn);
     if (P == 0) return 0;
-    if (!geom_state || !tile_state || !image_state || !scratch || !radii || !cams.bg)
-        return fail("%s: null state pointer", fn);
+    if (!geom_state || !tile_state || !image_state || !scratch || !radii) return fail("%s: null state pointer", fn);
     if (!dL_dout_color || !dL_dout_others) return fail("%s: null upstream gradient", fn);
     if (!dL_dmeans3D || !dL_dopacity || !dL_dscales || !dL_drotations)
         return fail("%s: null required output gradient", fn);
-    if (!means3D || !cams.view || !cams.campos) return fail("%s: null input pointer", fn);
+    if (!means3D) return fail("%s: null input pointer", fn);
     if (!transmat_was_precomputed && (!scales || !rotations)) return fail("%s: scales/rotations required", fn);
     if (misaligned(scratch)) return fail("%s: scratch must be 256-byte aligned", fn);
     const TileLayout tl = tile_layout(image_height, image_width);
@@ -412,7 +384,7 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
     const size_t dstride = det_stride_bytes(P);
     uint32_t* overflow = at<uint32_t>(det, dstride * (size_t)V);
     cudaError_t e = deterministic ? cudaMemsetAsync(det, 0, dstride * (size_t)V + sizeof(uint32_t), stream)
-                                  : cudaMemsetAsync(scratch, 0, V > 1 ? gstride * (size_t)V : (size_t)P * SRF_GRAD_FLOATS * sizeof(float), stream);
+                                  : cudaMemsetAsync(scratch, 0, gstride * (size_t)V, stream);
     if (e != cudaSuccess) return cuda_fail("memset gradient records", e);
 
     srf::RenderBwdArgs r;
@@ -424,22 +396,20 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
     r.point_list = point_list;
     r.masks = at<const uint32_t>(point_list, plist_masks_offset(capacity));
     r.rec = at<float4>(geom_state, gl.rec);
-    r.bg = cams.bg;
+    r.bg = cams + SRF_CAM_BG;
     r.accum = at<float>(image_state, il.accum);
     r.n_contrib = at<uint32_t>(image_state, il.ncontrib);
     r.dL_dpix = dL_dout_color;
     r.dL_dothers = dL_dout_others;
     r.ggrad = static_cast<float*>(scratch);
-    if (V > 1) {
-        r.geom_stride = gl.total; r.tile_stride = tl.total; r.plist_stride = plist_stride_bytes(capacity);
-        r.image_stride = il.total; r.ggrad_stride = gstride;
-    }
-    r.cam_stride = cams.stride;
+    r.geom_stride = gl.total; r.tile_stride = tl.total; r.plist_stride = plist_stride_bytes(capacity);
+    r.image_stride = il.total; r.ggrad_stride = gstride;
+    r.cam_stride = SRF_CAM_FLOATS;
     if (deterministic) {
         srf::RenderBwdArgs rd = r;
         rd.ggrad = static_cast<float*>(det);
         rd.ggrad_stride = dstride;
-        e = srf::launch_render_bwd_det(rd, P, r.ggrad, V > 1 ? gstride : 0, overflow, stream);
+        e = srf::launch_render_bwd_det(rd, P, r.ggrad, gstride, overflow, stream);
     } else {
         e = srf::launch_render_bwd(r, stream);
     }
@@ -450,7 +420,7 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
     p.P = P; p.D = D; p.M = (shs && !colors_were_precomputed) ? M : 0; p.nviews = V;
     p.means3D = means3D; p.scales = scales; p.rotations = rotations;
     p.shs = colors_were_precomputed ? nullptr : shs;
-    p.viewmatrix = cams.view; p.campos = cams.campos; p.cam_stride = cams.stride;
+    p.viewmatrix = cams + SRF_CAM_VIEW; p.campos = cams + SRF_CAM_CAMPOS; p.cam_stride = SRF_CAM_FLOATS;
     p.W = image_width; p.H = image_height;
     p.focal_y = image_height / (2.0f * tan_fovy);
     p.focal_x = image_width / (2.0f * tan_fovx);
@@ -472,120 +442,40 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
     return deterministic ? check_overflow_flag(fn, overflow, stream) : 0;
 }
 
-Cams cams_of(const float* cams) {
-    Cams c;
-    c.view = cams; c.campos = cams ? cams + SRF_CAM_CAMPOS : nullptr; c.bg = cams ? cams + SRF_CAM_BG : nullptr;
-    c.stride = SRF_CAM_FLOATS;
-    return c;
-}
-
 }  // namespace
 
 extern "C" {
 
-int srf_forward_preprocess(srf_stream_t stream_, int P, int D, int M,
-                           const float* means3D, const float* shs, const float* colors_precomp,
-                           const float* opacities, const float* scales, float scale_modifier,
-                           const float* rotations, const float* transMat_precomp,
-                           const float* viewmatrix, const float* projmatrix, const float* campos,
-                           float tan_fovx, float tan_fovy, int image_height, int image_width,
-                           int prefiltered, int* radii, void* geom_state, void* tile_state,
-                           uint32_t* num_rendered_host, int raw_activations) {
-    (void)scale_modifier; (void)projmatrix;
-    Cams c; c.view = viewmatrix; c.campos = campos; c.bg = nullptr; c.stride = 0;
-    return forward_preprocess_impl("srf_forward_preprocess", static_cast<cudaStream_t>(stream_), 1, P, D, M, means3D, shs,
-                                   colors_precomp, opacities, scales, rotations, transMat_precomp, c, tan_fovx, tan_fovy,
-                                   image_height, image_width, prefiltered, radii, geom_state, tile_state,
-                                   num_rendered_host, raw_activations);
-}
-
-int srf_forward_render(srf_stream_t stream_, int P, int image_height, int image_width,
-                       size_t capacity, const void* geom_state, void* tile_state,
-                       void* entries, uint32_t* point_list, void* image_state,
-                       const float* background, float* out_color, float* out_others) {
-    return forward_render_impl("srf_forward_render", static_cast<cudaStream_t>(stream_), 1, P, image_height, image_width,
-                               capacity, geom_state, tile_state, entries, point_list, image_state, background, 0,
-                               out_color, out_others);
-}
-
-int srf_backward(srf_stream_t stream_, int P, int D, int M, int image_height, int image_width,
-                 size_t capacity, const float* background,
-                 const float* means3D, const float* shs, int colors_were_precomputed,
-                 const float* scales, const float* rotations, int transmat_was_precomputed,
-                 const float* viewmatrix, const float* projmatrix, const float* campos,
-                 float tan_fovx, float tan_fovy, const int* radii,
-                 const void* geom_state, const void* tile_state, const uint32_t* point_list,
-                 const void* image_state,
-                 const float* dL_dout_color, const float* dL_dout_others,
-                 void* scratch, int accumulate,
-                 float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
-                 float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
-                 int raw_activations) {
-    (void)projmatrix;
-    Cams c; c.view = viewmatrix; c.campos = campos; c.bg = background; c.stride = 0;
-    return backward_impl("srf_backward", static_cast<cudaStream_t>(stream_), 1, P, D, M, image_height, image_width, capacity, c,
-                         means3D, shs, colors_were_precomputed, scales, rotations, transmat_was_precomputed,
-                         tan_fovx, tan_fovy, radii, geom_state, tile_state, point_list, image_state,
-                         dL_dout_color, dL_dout_others, scratch, accumulate, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors,
-                         dL_dopacity, dL_dscales, dL_drotations, dL_dtransMat, raw_activations);
-}
-
-// both forward stages in one call (one host->library transition per view in the drop-in path)
-int srf_forward(srf_stream_t stream_, int P, int D, int M,
-                const float* means3D, const float* shs, const float* colors_precomp,
-                const float* opacities, const float* scales, float scale_modifier,
-                const float* rotations, const float* transMat_precomp,
-                const float* viewmatrix, const float* projmatrix, const float* campos,
-                float tan_fovx, float tan_fovy, int image_height, int image_width, int prefiltered,
-                const float* background, size_t capacity,
-                int* radii, void* geom_state, void* tile_state, void* entries, uint32_t* point_list, void* image_state,
-                float* out_color, float* out_others, uint32_t* num_rendered_host, void* count_event, int raw_activations) {
-    int rc = srf_forward_preprocess(stream_, P, D, M, means3D, shs, colors_precomp, opacities, scales, scale_modifier, rotations,
-                                    transMat_precomp, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, image_height,
-                                    image_width, prefiltered, radii, geom_state, tile_state, num_rendered_host, raw_activations);
+int srf_views_forward(srf_stream_t stream_, int V, int P, int D, int M,
+                      const float* means3D, const float* shs, const float* colors_precomp,
+                      const float* opacities, const float* scales, const float* rotations,
+                      const float* transMat_precomp, const float* cams,
+                      float tan_fovx, float tan_fovy, int image_height, int image_width, int prefiltered,
+                      size_t capacity, int* radii, void* geom_state, void* tile_state, void* entries,
+                      uint32_t* point_list, void* image_state, float* out_color, float* out_others,
+                      uint32_t* num_rendered_host, void* count_event, int raw_activations) {
+    const char* fn = "srf_views_forward";
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    if (!cams) return fail("%s: null camera records", fn);
+    int rc = forward_preprocess_impl(fn, stream, V, P, D, M, means3D, shs, colors_precomp, opacities, scales, rotations,
+                                     transMat_precomp, cams, tan_fovx, tan_fovy, image_height, image_width, prefiltered,
+                                     radii, geom_state, tile_state, num_rendered_host, raw_activations);
     if (rc != 0) return rc;
-    if (count_event) {      // lets the caller wait for the instance count without waiting for the blend
-        cudaError_t e = cudaEventRecord(static_cast<cudaEvent_t>(count_event), static_cast<cudaStream_t>(stream_));
+    if (count_event) {      // lets the caller wait for the instance counts without waiting for the blend
+        cudaError_t e = cudaEventRecord(static_cast<cudaEvent_t>(count_event), stream);
         if (e != cudaSuccess) return cuda_fail("count event record", e);
     }
-    return srf_forward_render(stream_, P, image_height, image_width, capacity, geom_state, tile_state, entries, point_list,
-                              image_state, background, out_color, out_others);
-}
-
-// ---- all V target views of one scene in one launch set (reference caller loop: lightning/network.py:484-497)
-int srf_views_workspace_bytes(int V, int P, int H, int W, size_t capacity, size_t bytes[6]) {
-    if (V <= 0 || P < 0 || H <= 0 || W <= 0 || !bytes) return fail("srf_views_workspace_bytes: bad arguments");
-    bytes[0] = geom_layout(P).total * (size_t)V;
-    bytes[1] = tile_layout(H, W).total * (size_t)V;
-    bytes[2] = image_layout(H, W).total * (size_t)V;
-    bytes[3] = entries_stride_bytes(capacity) * (size_t)V;
-    bytes[4] = plist_stride_bytes(capacity) * (size_t)V;
-    bytes[5] = ggrad_stride_bytes(P) * (size_t)V;
-    return 0;
-}
-
-int srf_views_forward_preprocess(srf_stream_t stream_, int V, int P, int D, int M,
-                                 const float* means3D, const float* shs, const float* colors_precomp,
-                                 const float* opacities, const float* scales, const float* rotations,
-                                 const float* transMat_precomp, const float* cams,
-                                 float tan_fovx, float tan_fovy, int image_height, int image_width,
-                                 int prefiltered, int* radii, void* geom_state, void* tile_state,
-                                 uint32_t* num_rendered_host, int raw_activations) {
-    if (!cams) return fail("srf_views_forward_preprocess: null camera records");
-    return forward_preprocess_impl("srf_views_forward_preprocess", static_cast<cudaStream_t>(stream_), V, P, D, M, means3D,
-                                   shs, colors_precomp, opacities, scales, rotations, transMat_precomp, cams_of(cams),
-                                   tan_fovx, tan_fovy, image_height, image_width, prefiltered, radii, geom_state,
-                                   tile_state, num_rendered_host, raw_activations);
+    return forward_render_impl(fn, stream, V, P, image_height, image_width, capacity, geom_state, tile_state, entries,
+                               point_list, image_state, cams, out_color, out_others);
 }
 
 int srf_views_forward_render(srf_stream_t stream_, int V, int P, int image_height, int image_width,
                              size_t capacity, const void* geom_state, void* tile_state,
                              void* entries, uint32_t* point_list, void* image_state,
                              const float* cams, float* out_color, float* out_others) {
-    if (!cams) return fail("srf_views_forward_render: null camera records");
     return forward_render_impl("srf_views_forward_render", static_cast<cudaStream_t>(stream_), V, P, image_height,
                                image_width, capacity, geom_state, tile_state, entries, point_list, image_state,
-                               cams + SRF_CAM_BG, SRF_CAM_FLOATS, out_color, out_others);
+                               cams, out_color, out_others);
 }
 
 int srf_views_backward(srf_stream_t stream_, int V, int P, int D, int M, int image_height, int image_width,
@@ -600,12 +490,12 @@ int srf_views_backward(srf_stream_t stream_, int V, int P, int D, int M, int ima
                        float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
                        float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
                        int raw_activations) {
-    if (!cams) return fail("srf_views_backward: null camera records");
     return backward_impl("srf_views_backward", static_cast<cudaStream_t>(stream_), V, P, D, M, image_height, image_width,
-                         capacity, cams_of(cams), means3D, shs, colors_were_precomputed, scales, rotations,
+                         capacity, cams, means3D, shs, colors_were_precomputed, scales, rotations,
                          transmat_was_precomputed, tan_fovx, tan_fovy, radii, geom_state, tile_state, point_list,
                          image_state, dL_dout_color, dL_dout_others, scratch, accumulate, dL_dmeans3D, dL_dmeans2D,
-                         dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drotations, dL_dtransMat, raw_activations);
+                         dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drotations, dL_dtransMat, raw_activations,
+                         false);
 }
 
 int srf_views_backward_deterministic_scratch_bytes(int V, int P, size_t* bytes) {
@@ -626,79 +516,30 @@ int srf_views_backward_deterministic(srf_stream_t stream_, int V, int P, int D, 
                                      float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
                                      float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
                                      int raw_activations) {
-    if (!cams) return fail("srf_views_backward_deterministic: null camera records");
     return backward_impl("srf_views_backward_deterministic", static_cast<cudaStream_t>(stream_), V, P, D, M, image_height,
-                         image_width, capacity, cams_of(cams), means3D, shs, colors_were_precomputed, scales, rotations,
+                         image_width, capacity, cams, means3D, shs, colors_were_precomputed, scales, rotations,
                          transmat_was_precomputed, tan_fovx, tan_fovy, radii, geom_state, tile_state, point_list,
                          image_state, dL_dout_color, dL_dout_others, scratch, accumulate, dL_dmeans3D, dL_dmeans2D,
                          dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drotations, dL_dtransMat, raw_activations, true);
-}
-
-static int epilogue_forward_impl(const char* fn, cudaStream_t stream, int V, int image_height, int image_width,
-                                 float depth_ratio, const float* color, const float* allmap, const float* rays,
-                                 const float* viewmatrix, size_t cam_stride, float* image, float* depth, float* acc_map,
-                                 float* rend_normal, float* depth_normal, float* rend_dist) {
-    if (V <= 0 || image_height <= 0 || image_width <= 0) return fail("%s: bad sizes", fn);
-    if (!color || !allmap || !viewmatrix || !image || !depth || !acc_map || !rend_normal || !depth_normal || !rend_dist)
-        return fail("%s: null pointer", fn);
-    srf::EpilogueArgs a;
-    memset(&a, 0, sizeof(a));
-    a.W = image_width; a.H = image_height; a.nviews = V; a.depth_ratio = depth_ratio;
-    a.color = color; a.allmap = allmap; a.rays = rays; a.viewmatrix = viewmatrix; a.cam_stride = cam_stride;
-    a.image = image; a.depth = depth; a.acc = acc_map; a.rend_normal = rend_normal; a.depth_normal = depth_normal;
-    a.dist = rend_dist;
-    cudaError_t e = srf::launch_epilogue_fwd(a, stream);
-    if (e != cudaSuccess) return cuda_fail("epilogue_fwd launch", e);
-    return 0;
-}
-
-static int epilogue_backward_impl(const char* fn, cudaStream_t stream, int V, int image_height, int image_width,
-                                  float depth_ratio, const float* color, const float* allmap, const float* rays,
-                                  const float* viewmatrix, size_t cam_stride,
-                                  const float* g_image, const float* g_depth, const float* g_acc_map,
-                                  const float* g_rend_normal, const float* g_depth_normal, const float* g_rend_dist,
-                                  float* scratch, float* dL_dcolor, float* dL_dallmap) {
-    if (V <= 0 || image_height <= 0 || image_width <= 0) return fail("%s: bad sizes", fn);
-    if (!color || !allmap || !viewmatrix || !dL_dcolor || !dL_dallmap) return fail("%s: null pointer", fn);
-    if (g_depth_normal && rays && !scratch) return fail("%s: scratch [V,3,H,W] required", fn);
-    srf::EpilogueArgs a;
-    memset(&a, 0, sizeof(a));
-    a.W = image_width; a.H = image_height; a.nviews = V; a.depth_ratio = depth_ratio;
-    a.color = color; a.allmap = allmap; a.rays = rays; a.viewmatrix = viewmatrix; a.cam_stride = cam_stride;
-    a.g_image = g_image; a.g_depth = g_depth; a.g_acc = g_acc_map; a.g_rend_normal = g_rend_normal;
-    a.g_depth_normal = g_depth_normal; a.g_dist = g_rend_dist;
-    a.scratch = scratch; a.dL_dcolor = dL_dcolor; a.dL_dallmap = dL_dallmap;
-    cudaError_t e = srf::launch_epilogue_bwd(a, stream);
-    if (e != cudaSuccess) return cuda_fail("epilogue_bwd launch", e);
-    return 0;
-}
-
-int srf_epilogue_forward(srf_stream_t stream_, int image_height, int image_width, float depth_ratio,
-                         const float* color, const float* allmap, const float* rays, const float* viewmatrix,
-                         float* image, float* depth, float* acc_map, float* rend_normal, float* depth_normal,
-                         float* rend_dist) {
-    return epilogue_forward_impl("srf_epilogue_forward", static_cast<cudaStream_t>(stream_), 1, image_height, image_width,
-                                 depth_ratio, color, allmap, rays, viewmatrix, 0, image, depth, acc_map, rend_normal,
-                                 depth_normal, rend_dist);
-}
-
-int srf_epilogue_backward(srf_stream_t stream_, int image_height, int image_width, float depth_ratio,
-                          const float* color, const float* allmap, const float* rays, const float* viewmatrix,
-                          const float* g_image, const float* g_depth, const float* g_acc_map,
-                          const float* g_rend_normal, const float* g_depth_normal, const float* g_rend_dist,
-                          float* scratch, float* dL_dcolor, float* dL_dallmap) {
-    return epilogue_backward_impl("srf_epilogue_backward", static_cast<cudaStream_t>(stream_), 1, image_height, image_width,
-                                  depth_ratio, color, allmap, rays, viewmatrix, 0, g_image, g_depth, g_acc_map,
-                                  g_rend_normal, g_depth_normal, g_rend_dist, scratch, dL_dcolor, dL_dallmap);
 }
 
 int srf_views_epilogue_forward(srf_stream_t stream_, int V, int image_height, int image_width, float depth_ratio,
                                const float* color, const float* allmap, const float* rays, const float* cams,
                                float* image, float* depth, float* acc_map, float* rend_normal, float* depth_normal,
                                float* rend_dist) {
-    return epilogue_forward_impl("srf_views_epilogue_forward", static_cast<cudaStream_t>(stream_), V, image_height,
-                                 image_width, depth_ratio, color, allmap, rays, cams, SRF_CAM_FLOATS, image, depth, acc_map,
-                                 rend_normal, depth_normal, rend_dist);
+    const char* fn = "srf_views_epilogue_forward";
+    if (V <= 0 || image_height <= 0 || image_width <= 0) return fail("%s: bad sizes", fn);
+    if (!color || !allmap || !cams || !image || !depth || !acc_map || !rend_normal || !depth_normal || !rend_dist)
+        return fail("%s: null pointer", fn);
+    srf::EpilogueArgs a;
+    memset(&a, 0, sizeof(a));
+    a.W = image_width; a.H = image_height; a.nviews = V; a.depth_ratio = depth_ratio;
+    a.color = color; a.allmap = allmap; a.rays = rays; a.viewmatrix = cams + SRF_CAM_VIEW; a.cam_stride = SRF_CAM_FLOATS;
+    a.image = image; a.depth = depth; a.acc = acc_map; a.rend_normal = rend_normal; a.depth_normal = depth_normal;
+    a.dist = rend_dist;
+    cudaError_t e = srf::launch_epilogue_fwd(a, static_cast<cudaStream_t>(stream_));
+    if (e != cudaSuccess) return cuda_fail("epilogue_fwd launch", e);
+    return 0;
 }
 
 int srf_views_epilogue_backward(srf_stream_t stream_, int V, int image_height, int image_width, float depth_ratio,
@@ -706,9 +547,20 @@ int srf_views_epilogue_backward(srf_stream_t stream_, int V, int image_height, i
                                 const float* g_image, const float* g_depth, const float* g_acc_map,
                                 const float* g_rend_normal, const float* g_depth_normal, const float* g_rend_dist,
                                 float* scratch, float* dL_dcolor, float* dL_dallmap) {
-    return epilogue_backward_impl("srf_views_epilogue_backward", static_cast<cudaStream_t>(stream_), V, image_height,
-                                  image_width, depth_ratio, color, allmap, rays, cams, SRF_CAM_FLOATS, g_image, g_depth,
-                                  g_acc_map, g_rend_normal, g_depth_normal, g_rend_dist, scratch, dL_dcolor, dL_dallmap);
+    const char* fn = "srf_views_epilogue_backward";
+    if (V <= 0 || image_height <= 0 || image_width <= 0) return fail("%s: bad sizes", fn);
+    if (!color || !allmap || !cams || !dL_dcolor || !dL_dallmap) return fail("%s: null pointer", fn);
+    if (g_depth_normal && rays && !scratch) return fail("%s: scratch [V,3,H,W] required", fn);
+    srf::EpilogueArgs a;
+    memset(&a, 0, sizeof(a));
+    a.W = image_width; a.H = image_height; a.nviews = V; a.depth_ratio = depth_ratio;
+    a.color = color; a.allmap = allmap; a.rays = rays; a.viewmatrix = cams + SRF_CAM_VIEW; a.cam_stride = SRF_CAM_FLOATS;
+    a.g_image = g_image; a.g_depth = g_depth; a.g_acc = g_acc_map; a.g_rend_normal = g_rend_normal;
+    a.g_depth_normal = g_depth_normal; a.g_dist = g_rend_dist;
+    a.scratch = scratch; a.dL_dcolor = dL_dcolor; a.dL_dallmap = dL_dallmap;
+    cudaError_t e = srf::launch_epilogue_bwd(a, static_cast<cudaStream_t>(stream_));
+    if (e != cudaSuccess) return cuda_fail("epilogue_bwd launch", e);
+    return 0;
 }
 
 int srf_loss_forward(srf_stream_t stream_, int V, int image_height, int image_width, int with_reg,

@@ -4,9 +4,9 @@
 // Every kernel takes a *view* dimension: the V target views of one scene share the Gaussian set
 // (reference caller loop lightning/network.py:484-497), so one launch covers all of them.  Per-view
 // arrays live in per-view workspaces of identical layout; the structs carry the base pointers of view 0
-// plus the byte stride from one view's workspace to the next (`*_stride`, 0 when nviews == 1).  Camera
-// data (view matrix, camera position, background) are three pointers into per-view camera records
-// `cam_stride` floats apart.  Images are stacked [V,C,H,W].
+// plus the byte stride from one view's workspace to the next (`*_stride`).  Camera data (view matrix,
+// camera position, background) are pointers into view 0's camera record (include/surfel_rasterizer.h
+// SRF_CAM_*), the records `cam_stride` floats apart.  Images are stacked [V,C,H,W].
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

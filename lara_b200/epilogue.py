@@ -33,37 +33,11 @@ def _c(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
     return None if t is None else t.contiguous()
 
 
-def epilogue_forward_raw(color, allmap, rays, viewmatrix, depth_ratio, image, depth, acc, rn, dn, dist):
-    """Enqueue the fused forward on the current stream; all tensors contiguous fp32 on one device,
-    outputs planar ([3,H,W], [1,H,W], [H,W], [3,H,W], [3,H,W], [H,W]; slices of stacked buffers are fine)."""
-    lib = _lib.load()
-    H, W = int(color.shape[1]), int(color.shape[2])
-    dev = color.device
-    with _DeviceGuard(dev):
-        _lib.check(lib.srf_epilogue_forward(
-            _raw_stream(dev), H, W, float(depth_ratio), color.data_ptr(), allmap.data_ptr(), _p(rays),
-            viewmatrix.data_ptr(), image.data_ptr(), depth.data_ptr(), acc.data_ptr(), rn.data_ptr(),
-            dn.data_ptr(), dist.data_ptr()), lib)
-
-
-def epilogue_backward_raw(color, allmap, rays, viewmatrix, depth_ratio, gi, gd, ga, grn, gdn, gds):
-    """Enqueue the fused backward; upstream gradients may be None.  Returns (dL_dcolor[3,H,W], dL_dallmap[8,H,W])."""
-    lib = _lib.load()
-    H, W = int(color.shape[1]), int(color.shape[2])
-    dev = color.device
-    buf = torch.empty((14, H, W), dtype=torch.float32, device=dev)
-    scratch, d_color, d_allmap = buf[0:3], buf[3:6], buf[6:14]
-    with _DeviceGuard(dev):
-        _lib.check(lib.srf_epilogue_backward(
-            _raw_stream(dev), H, W, float(depth_ratio), color.data_ptr(), allmap.data_ptr(), _p(rays),
-            viewmatrix.data_ptr(), _p(gi), _p(gd), _p(ga), _p(grn), _p(gdn), _p(gds),
-            scratch.data_ptr(), d_color.data_ptr(), d_allmap.data_ptr()), lib)
-    return d_color, d_allmap
-
-
 def epilogue_views_forward_raw(color, allmap, rays, cams, depth_ratio, image, depth, acc, rn, dn, dist):
-    """The fused forward over V stacked views in one launch: color [V,3,H,W], allmap [V,8,H,W], rays [V,H,W,6] or
-    None, cams [V,24] camera records (rasterizer.pack_cameras); outputs stacked [V,...] planar."""
+    """The fused forward over V stacked views in one launch, enqueued on the current stream: color [V,3,H,W],
+    allmap [V,8,H,W], rays [V,H,W,6] or None, cams [V,24] camera records (rasterizer.pack_cameras); outputs stacked
+    [V,...] planar.  All tensors contiguous fp32 on one device.  Only the view matrix of each record is read, so for
+    V = 1 a contiguous 16-float view matrix serves as `cams`."""
     lib = _lib.load()
     V, H, W = int(color.shape[0]), int(color.shape[2]), int(color.shape[3])
     dev = color.device
@@ -88,6 +62,20 @@ def epilogue_views_backward_raw(color, allmap, rays, cams, depth_ratio, gi, gd, 
             cams.data_ptr(), _p(gi), _p(gd), _p(ga), _p(grn), _p(gdn), _p(gds),
             scratch.data_ptr(), d_color.data_ptr(), d_allmap.data_ptr()), lib)
     return d_color, d_allmap
+
+
+def epilogue_forward_raw(color, allmap, rays, viewmatrix, depth_ratio, image, depth, acc, rn, dn, dist):
+    """One view ([3,H,W], [8,H,W], rays [H,W,6] or None, a contiguous 16-float view matrix): the V = 1 case of
+    :func:`epilogue_views_forward_raw`; outputs planar ([3,H,W], [1,H,W], [H,W], [3,H,W], [3,H,W], [H,W])."""
+    epilogue_views_forward_raw(color[None], allmap[None], None if rays is None else rays[None], viewmatrix,
+                               depth_ratio, image, depth, acc, rn, dn, dist)
+
+
+def epilogue_backward_raw(color, allmap, rays, viewmatrix, depth_ratio, gi, gd, ga, grn, gdn, gds):
+    """Backward of :func:`epilogue_forward_raw`; returns (dL_dcolor [3,H,W], dL_dallmap [8,H,W])."""
+    d_color, d_allmap = epilogue_views_backward_raw(color[None], allmap[None], None if rays is None else rays[None],
+                                                    viewmatrix, depth_ratio, gi, gd, ga, grn, gdn, gds)
+    return d_color[0], d_allmap[0]
 
 
 def _check_epilogue_inputs(color, allmap, rays, viewmatrix):

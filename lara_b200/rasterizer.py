@@ -47,7 +47,8 @@ class GaussianRasterizationSettings(NamedTuple):
 # small host-side helpers
 # ---------------------------------------------------------------------------------
 
-_size_cache: dict = {}
+_size_cache: dict = {}            # (V, P, H, W, capacity) -> srf_views_workspace_bytes
+_cam_pads: dict = {}              # device -> zero padding of a camera record
 _capacity_hwm: dict = {}          # device index -> largest num_rendered seen (instances per view)
 _lock = threading.Lock()          # autograd calls backward() from another host thread
 
@@ -71,11 +72,11 @@ def _f32c(t: torch.Tensor, name: str) -> torch.Tensor:
     return t.contiguous()
 
 
-def _sizes(lib, P: int, H: int, W: int):
-    key = (P, H, W)
+def _views_sizes(lib, V: int, P: int, H: int, W: int, capacity: int):
+    key = (V, P, H, W, capacity)
     v = _size_cache.get(key)
     if v is None:
-        v = _lib.sizes(lib, P, H, W)
+        v = _lib.views_sizes(lib, V, P, H, W, capacity)
         if len(_size_cache) > 64:
             _size_cache.clear()
         _size_cache[key] = v
@@ -239,13 +240,14 @@ class LazyCount:
 
 
 class ForwardState:
-    """What a forward leaves behind for the backward (the reference's three blobs).  For the batched
-    entry the workspaces hold V per-view workspaces back to back."""
-    __slots__ = ("geom", "tile", "image", "point_list", "capacity", "nviews", "_pending", "_counts")
+    """What a forward leaves behind for the backward (the reference's three blobs): V per-view workspaces back to
+    back, and the [V, SRF_CAM_FLOATS] camera records the forward ran on."""
+    __slots__ = ("geom", "tile", "image", "point_list", "capacity", "nviews", "cams", "_pending", "_counts")
 
-    def __init__(self, geom, tile, image, point_list, capacity, num_rendered=0, nviews: int = 1, pending=None):
+    def __init__(self, geom, tile, image, point_list, capacity, num_rendered=0, nviews: int = 1, pending=None,
+                 cams=None):
         self.geom, self.tile, self.image, self.point_list = geom, tile, image, point_list
-        self.capacity, self.nviews = capacity, nviews
+        self.capacity, self.nviews, self.cams = capacity, nviews, cams
         self._pending = pending
         self._counts = None if pending is not None else ([int(num_rendered)] * nviews
                                                          if not isinstance(num_rendered, (list, tuple)) else list(num_rendered))
@@ -262,127 +264,45 @@ class ForwardState:
         return c[0] if self.nviews == 1 else list(c)
 
 
-def _launch_forward(device, lib, nviews, P, capacity, debug, call_pre, call_render, state_blobs, alloc_binning,
-                    call_both=None):
-    """Common enqueue sequence of the per-view and the batched forward:
-    stage 1 (preprocess + tile scan + async count read-back) and stage 2 (binning + blend) with an optimistic
-    capacity, then an event for whoever eventually asks for the instance counts."""
-    _drain_ready(device)
-    rb = _take_readback(device, nviews)
-    slot, ev = rb
-    geom, tile, image = state_blobs
-    entries, point_list = alloc_binning(capacity)
-    # the event sits between stage 1 (which produces the counts) and stage 2: whoever resolves the counts later waits
-    # for the tile scan, never for the blend
-    if call_both is not None:
-        call_both(slot.data_ptr(), ev.cuda_event, capacity, entries, point_list)
-    else:
-        call_pre(slot.data_ptr())
-        ev.record()
-        call_render(capacity, entries, point_list)
-    state = ForwardState(geom, tile, image, point_list, capacity, nviews=nviews)
+def pack_cameras(settings_list: Sequence[GaussianRasterizationSettings], device) -> torch.Tensor:
+    """[V, SRF_CAM_FLOATS] device tensor of per-view camera records (viewmatrix | campos | bg | pad) built
+    from per-view settings with ONE cat kernel (the tensors are already on the device, as LaRa's MiniCam
+    produces them, lightning/utils.py:33-48; the zero padding is made once per device)."""
+    parts = []
+    pad = _cam_pad(device)
+    for rs in settings_list:
+        parts += [rs.viewmatrix.reshape(16), rs.campos.reshape(3), rs.bg.reshape(3), pad]
+    return torch.cat(parts).view(len(settings_list), _lib.CAM_FLOATS)
 
-    def rerun(new_capacity: int):
-        with _DeviceGuard(device):
-            e2, pl2 = alloc_binning(new_capacity)
-            call_render(new_capacity, e2, pl2)
-            state.point_list, state.capacity = pl2, new_capacity
 
-    pend = _Pending(device, rb, nviews, capacity, rerun)
-    state._pending, state._counts = pend, None
-    if _eager_sync(debug):
-        pend.resolve(stale_ok=True)      # nothing has consumed the outputs yet
-        state.resolve()
-    else:
-        with _lock:
-            _pending.setdefault(_dev_index(device), []).append(pend)
-    return state
+def _cam_pad(device) -> torch.Tensor:
+    pad = _cam_pads.get(device)
+    if pad is None:
+        device = torch.device(device)
+        if device.type == "cuda":
+            device = torch.device("cuda", _dev_index(device))
+        pad = _cam_pads.get(device)
+        if pad is None:
+            pad = torch.zeros(_lib.CAM_FLOATS - 22, dtype=torch.float32, device=device)
+            if device.type == "cuda":
+                torch.cuda.synchronize(device)      # filled before a record on any stream reads it
+            _cam_pads[device] = pad
+    return pad
 
 
 def forward_raw(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp,
                 raster_settings: GaussianRasterizationSettings, raw_activations: bool = False):
-    """Enqueue one forward on the current stream of the tensors' device.
+    """Enqueue one forward on the current stream of the tensors' device: :func:`forward_views_raw` with V = 1 on the
+    settings' camera record, which the returned state keeps for :func:`backward_raw`.
 
     Returns (color[3,H,W], allmap[8,H,W], radii[P], ForwardState).  Inputs must already be
     normalised (None for absent, fp32, contiguous, CUDA).
     """
+    rs = raster_settings
     with _DeviceGuard(means3D.device):
-        return _forward_raw(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp,
-                            raster_settings, raw_activations)
-
-
-def _forward_raw(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp, raster_settings,
-                 raw_activations=False):
-    lib = _lib.load()
-    H, W = int(raster_settings.image_height), int(raster_settings.image_width)
-    P = int(means3D.shape[0])
-    device = means3D.device
-    M = int(shs.shape[1]) if shs is not None else 0
-    geom_b, tile_b, image_b, _ = _sizes(lib, P, H, W)
-
-    # the three state workspaces share one byte blob (sub-blobs stay 256-byte aligned: the sizes are
-    # multiples of 256).  The two images stay separate tensors: outputs of an autograd.Function
-    # that are views of a common base cannot be modified in place by the caller.
-    color = torch.empty((3, H, W), dtype=torch.float32, device=device)
-    allmap = torch.empty((8, H, W), dtype=torch.float32, device=device)
-    radii = torch.empty((P,), dtype=torch.int32, device=device)
-    blob = _blob(geom_b + tile_b + image_b, device)
-    geom, tile, image = blob[:geom_b], blob[geom_b:geom_b + tile_b], blob[geom_b + tile_b:]
-    sptr = _raw_stream(device)
-
-    if P == 0:
-        # reference: zero-filled outputs, nothing rendered (rasterize_points.cu:92-94,105)
-        color.zero_(); allmap.zero_()
-        tile.zero_(); image.zero_()
-        pl = torch.empty((0,), dtype=torch.int32, device=device)
-        return color, allmap, radii, ForwardState(geom, tile, image, pl, 0, 0)
-
-    bg = raster_settings.bg
-    viewm = raster_settings.viewmatrix
-    projm = raster_settings.projmatrix
-    campos = raster_settings.campos
-
-    def call_both(slot_ptr, ev_handle, capacity, entries, point_list):
-        _lib.check(lib.srf_forward(
-            sptr, P, int(raster_settings.sh_degree), M,
-            _ptr(means3D), _ptr(shs), _ptr(colors_precomp),
-            _ptr(opacities), _ptr(scales), float(raster_settings.scale_modifier),
-            _ptr(rotations), _ptr(transMat_precomp),
-            _ptr(viewm), _ptr(projm), _ptr(campos),
-            float(raster_settings.tanfovx), float(raster_settings.tanfovy), H, W,
-            1 if raster_settings.prefiltered else 0, _ptr(bg), capacity,
-            radii.data_ptr(), geom.data_ptr(), tile.data_ptr(), entries.data_ptr(), point_list.data_ptr(), image.data_ptr(),
-            color.data_ptr(), allmap.data_ptr(), slot_ptr, ev_handle, 1 if raw_activations else 0), lib)
-
-    def alloc_binning(capacity):
-        ent_b, pl_b = _lib.binning_sizes(lib, capacity)
-        return _blob(ent_b, device), _blob(pl_b, device)
-
-    def call_render(capacity, entries, point_list):
-        # (re-)enqueued on whatever stream is current: a deferred re-run happens on the caller's stream
-        _lib.check(lib.srf_forward_render(
-            _raw_stream(device), P, H, W, capacity, geom.data_ptr(), tile.data_ptr(),
-            entries.data_ptr(), point_list.data_ptr(), image.data_ptr(),
-            _ptr(bg), color.data_ptr(), allmap.data_ptr()), lib)
-
-    # Optimistic capacity: stage 2 is enqueued before num_rendered is known on the host, so
-    # the GPU never idles behind the read-back; an overflow (rare) just re-runs stage 2.
-    state = _launch_forward(device, lib, 1, P, initial_capacity(P, device), raster_settings.debug,
-                            None, call_render, (geom, tile, image), alloc_binning, call_both=call_both)
-    if raster_settings.debug:
-        torch.cuda.synchronize(device)
-    return color, allmap, radii, state
-
-
-def pack_cameras(settings_list: Sequence[GaussianRasterizationSettings], device) -> torch.Tensor:
-    """[V, SRF_CAM_FLOATS] device tensor of per-view camera records (viewmatrix | campos | bg | pad) built
-    from per-view settings with ONE cat kernel (the tensors are already on the device, as LaRa's MiniCam
-    produces them, lightning/utils.py:33-48)."""
-    parts = []
-    pad = torch.zeros(_lib.CAM_FLOATS - 22, dtype=torch.float32, device=device)
-    for rs in settings_list:
-        parts += [rs.viewmatrix.reshape(16), rs.campos.reshape(3), rs.bg.reshape(3), pad]
-    return torch.cat(parts).view(len(settings_list), _lib.CAM_FLOATS)
+        return _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp,
+                        pack_cameras([rs], means3D.device), rs.tanfovx, rs.tanfovy, int(rs.image_height),
+                        int(rs.image_width), rs.sh_degree, rs.prefiltered, rs.debug, raw_activations, single=True)
 
 
 def forward_views_raw(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp,
@@ -392,45 +312,76 @@ def forward_views_raw(means3D, shs, colors_precomp, opacities, scales, rotations
     dimension.  `cams` is the [V, 24] device tensor of camera records (pack_cameras).
     Returns (color [V,3,H,W], allmap [V,8,H,W], radii [V,P], ForwardState with V back-to-back workspaces)."""
     with _DeviceGuard(means3D.device):
-        lib = _lib.load()
-        device = means3D.device
-        V, P = int(cams.shape[0]), int(means3D.shape[0])
-        M = int(shs.shape[1]) if shs is not None else 0
         if cams.dtype != torch.float32 or not cams.is_cuda or cams.shape[1] != _lib.CAM_FLOATS or not cams.is_contiguous():
             raise RuntimeError(f"cams must be a contiguous float32 CUDA tensor [V,{_lib.CAM_FLOATS}]")
-        color = torch.empty((V, 3, H, W), dtype=torch.float32, device=device)
-        allmap = torch.empty((V, 8, H, W), dtype=torch.float32, device=device)
-        radii = torch.empty((V, P), dtype=torch.int32, device=device)
-        geom_b, tile_b, image_b, _, _, _ = _lib.views_sizes(lib, V, P, H, W, 0)
-        blob = _blob(geom_b + tile_b + image_b, device)
-        geom, tile, image = blob[:geom_b], blob[geom_b:geom_b + tile_b], blob[geom_b + tile_b:]
-        if P == 0:
-            color.zero_(); allmap.zero_(); tile.zero_(); image.zero_()
-            pl = torch.empty((0,), dtype=torch.int32, device=device)
-            return color, allmap, radii, ForwardState(geom, tile, image, pl, 0, 0, nviews=V)
-        sptr = _raw_stream(device)
+        return _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp, cams, tanfovx,
+                        tanfovy, H, W, sh_degree, prefiltered, debug, raw_activations, single=False)
 
-        def call_pre(slot_ptr):
-            _lib.check(lib.srf_views_forward_preprocess(
-                sptr, V, P, int(sh_degree), M, _ptr(means3D), _ptr(shs), _ptr(colors_precomp), _ptr(opacities),
-                _ptr(scales), _ptr(rotations), _ptr(transMat_precomp), cams.data_ptr(), float(tanfovx), float(tanfovy),
-                H, W, 1 if prefiltered else 0, radii.data_ptr(), geom.data_ptr(), tile.data_ptr(), slot_ptr,
-                1 if raw_activations else 0), lib)
 
-        def alloc_binning(capacity):
-            _, _, _, ent_b, pl_b, _ = _lib.views_sizes(lib, V, P, H, W, capacity)
-            return _blob(ent_b, device), _blob(pl_b, device)
+def _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp, cams, tanfovx, tanfovy,
+             H, W, sh_degree, prefiltered, debug, raw_activations, single):
+    """srf_views_forward on the current stream: stage 1 (preprocess + tile scan + async count read-back) and stage 2
+    (binning + blend) with an optimistic capacity, then an event for whoever eventually asks for the instance counts.
+    `single`: one view, with the outputs in the reference's one-view shapes."""
+    lib = _lib.load()
+    device = means3D.device
+    V, P = int(cams.shape[0]), int(means3D.shape[0])
+    M = int(shs.shape[1]) if shs is not None else 0
+    # The outputs are separate tensors in the caller's shapes: outputs of an autograd.Function that are views (of a
+    # common base, or one view of a stacked buffer) cannot be modified in place by the caller.
+    lead = () if single else (V,)
+    color = torch.empty(lead + (3, H, W), dtype=torch.float32, device=device)
+    allmap = torch.empty(lead + (8, H, W), dtype=torch.float32, device=device)
+    radii = torch.empty(lead + (P,), dtype=torch.int32, device=device)
+    capacity = initial_capacity(P, device)
+    geom_b, tile_b, image_b, ent_b, pl_b, _ = _views_sizes(lib, V, P, H, W, capacity)
+    # the three state workspaces share one byte blob (sub-blobs stay 256-byte aligned: the sizes are multiples of 256)
+    blob = _blob(geom_b + tile_b + image_b, device)
+    geom, tile, image = blob[:geom_b], blob[geom_b:geom_b + tile_b], blob[geom_b + tile_b:]
+    if P == 0:
+        # reference: zero-filled outputs, nothing rendered (rasterize_points.cu:92-94,105)
+        color.zero_(); allmap.zero_(); tile.zero_(); image.zero_()
+        pl = torch.empty((0,), dtype=torch.int32, device=device)
+        return color, allmap, radii, ForwardState(geom, tile, image, pl, 0, 0, nviews=V, cams=cams)
 
-        def call_render(capacity, entries, point_list):
+    _drain_ready(device)
+    rb = _take_readback(device, V)
+    slot, ev = rb
+    point_list = _blob(pl_b, device)
+    # Stage 2 is enqueued before the counts are known on the host, so the GPU never idles behind the read-back; an
+    # overflow (rare) re-runs stage 2.  The event sits between the stages: whoever resolves the counts later waits for
+    # the tile scan, never for the blend.
+    _lib.check(lib.srf_views_forward(
+        _raw_stream(device), V, P, int(sh_degree), M, _ptr(means3D), _ptr(shs), _ptr(colors_precomp),
+        _ptr(opacities), _ptr(scales), _ptr(rotations), _ptr(transMat_precomp), cams.data_ptr(),
+        float(tanfovx), float(tanfovy), H, W, 1 if prefiltered else 0, capacity,
+        radii.data_ptr(), geom.data_ptr(), tile.data_ptr(), _blob(ent_b, device).data_ptr(), point_list.data_ptr(),
+        image.data_ptr(), color.data_ptr(), allmap.data_ptr(), slot.data_ptr(), ev.cuda_event,
+        1 if raw_activations else 0), lib)
+    state = ForwardState(geom, tile, image, point_list, capacity, nviews=V, cams=cams)
+
+    def rerun(new_capacity: int):
+        # enqueued on whatever stream is current: a deferred re-run happens on the caller's stream
+        with _DeviceGuard(device):
+            _, _, _, e_b, p_b, _ = _views_sizes(lib, V, P, H, W, new_capacity)
+            pl2 = _blob(p_b, device)
             _lib.check(lib.srf_views_forward_render(
-                _raw_stream(device), V, P, H, W, capacity, geom.data_ptr(), tile.data_ptr(), entries.data_ptr(),
-                point_list.data_ptr(), image.data_ptr(), cams.data_ptr(), color.data_ptr(), allmap.data_ptr()), lib)
+                _raw_stream(device), V, P, H, W, new_capacity, geom.data_ptr(), tile.data_ptr(),
+                _blob(e_b, device).data_ptr(), pl2.data_ptr(), image.data_ptr(), cams.data_ptr(), color.data_ptr(),
+                allmap.data_ptr()), lib)
+            state.point_list, state.capacity = pl2, new_capacity
 
-        state = _launch_forward(device, lib, V, P, initial_capacity(P, device), debug, call_pre, call_render,
-                                (geom, tile, image), alloc_binning)
-        if debug:
-            torch.cuda.synchronize(device)
-        return color, allmap, radii, state
+    pend = _Pending(device, rb, V, capacity, rerun)
+    state._pending, state._counts = pend, None
+    if _eager_sync(debug):
+        pend.resolve(stale_ok=True)      # nothing has consumed the outputs yet
+        state.resolve()
+    else:
+        with _lock:
+            _pending.setdefault(_dev_index(device), []).append(pend)
+    if debug:
+        torch.cuda.synchronize(device)
+    return color, allmap, radii, state
 
 
 def _grad_outputs(P, M, device, shs, colors_precomp, transMat_precomp, out, accumulate, need_means2D):
@@ -467,7 +418,8 @@ def backward_raw(state: ForwardState, radii, means3D, shs, colors_precomp, scale
                  transMat_precomp, raster_settings, grad_color, grad_allmap, *,
                  out: Optional[dict] = None, accumulate: bool = False, need_means2D: bool = True,
                  raw_activations: bool = False, deterministic: Optional[bool] = None):
-    """Enqueue one backward; returns a dict of gradient tensors.
+    """Enqueue the backward of :func:`forward_raw`: :func:`backward_views_raw` with V = 1 on the camera record the
+    forward kept in ``state``; returns a dict of gradient tensors.
 
     ``out`` may supply pre-allocated (possibly strided-into-a-flat-buffer but contiguous)
     tensors for 'means3D','sh','opacities','scales','rotations'; with ``accumulate`` the
@@ -475,51 +427,12 @@ def backward_raw(state: ForwardState, radii, means3D, shs, colors_precomp, scale
     ``deterministic``: bit-reproducible gradients (fixed-point sums of the blend backward, DESIGN §3.13; the call then
     waits for the GPU); ``None`` follows ``torch.use_deterministic_algorithms``.
     """
-    with _DeviceGuard(means3D.device):
-        return _backward_raw(state, radii, means3D, shs, colors_precomp, scales, rotations, transMat_precomp,
-                             raster_settings, grad_color, grad_allmap, out=out, accumulate=accumulate,
-                             need_means2D=need_means2D, raw_activations=raw_activations, deterministic=deterministic)
-
-
-def _backward_raw(state, radii, means3D, shs, colors_precomp, scales, rotations, transMat_precomp,
-                  raster_settings, grad_color, grad_allmap, *, out=None, accumulate=False, need_means2D=True,
-                  raw_activations=False, deterministic=None):
-    lib = _lib.load()
-    H, W = int(raster_settings.image_height), int(raster_settings.image_width)
-    P = int(means3D.shape[0])
-    device = means3D.device
-    M = int(shs.shape[1]) if shs is not None else 0
-    g = _grad_outputs(P, M, device, shs, colors_precomp, transMat_precomp, out or {}, accumulate, need_means2D)
-    if P == 0:
-        return g
-    state.resolve()                 # capacity verified (re-run if it overflowed) before the lists are walked again
-    if _lib.deterministic(deterministic):
-        # the views entry with V = 1: one camera record
-        cams = pack_cameras([raster_settings], device)
-        _views_backward(lib, lib.srf_views_backward_deterministic, _lib.det_backward_scratch_bytes(lib, 1, P), state,
-                        radii, means3D, shs, colors_precomp, scales, rotations, transMat_precomp, cams,
-                        raster_settings.tanfovx, raster_settings.tanfovy, H, W, raster_settings.sh_degree, grad_color,
-                        grad_allmap, g, accumulate, raw_activations)
-        return g
-    _, _, _, scratch_b = _sizes(lib, P, H, W)
-    scratch = _blob(scratch_b, device)
-    sptr = _raw_stream(device)
-    _lib.check(lib.srf_backward(
-        sptr, P, int(raster_settings.sh_degree), M, H, W,
-        state.capacity, _ptr(raster_settings.bg),
-        _ptr(means3D), _ptr(shs), 1 if colors_precomp is not None else 0,
-        _ptr(scales), _ptr(rotations), 1 if transMat_precomp is not None else 0,
-        _ptr(raster_settings.viewmatrix), _ptr(raster_settings.projmatrix), _ptr(raster_settings.campos),
-        float(raster_settings.tanfovx), float(raster_settings.tanfovy), radii.data_ptr(),
-        state.geom.data_ptr(), state.tile.data_ptr(), state.point_list.data_ptr(), state.image.data_ptr(),
-        grad_color.data_ptr(), grad_allmap.data_ptr(),
-        scratch.data_ptr(), 1 if accumulate else 0,
-        _ptr(g["means3D"]), _ptr(g["means2D"]), _ptr(g["sh"]), _ptr(g["colors_precomp"]),
-        _ptr(g["opacities"]), _ptr(g["scales"]), _ptr(g["rotations"]), _ptr(g["cov3Ds_precomp"]),
-        1 if raw_activations else 0), lib)
-    if raster_settings.debug:
-        torch.cuda.synchronize(device)
-    return g
+    rs = raster_settings
+    return backward_views_raw(state, radii, means3D, shs, colors_precomp, scales, rotations, transMat_precomp,
+                              state.cams, rs.tanfovx, rs.tanfovy, int(rs.image_height), int(rs.image_width),
+                              rs.sh_degree, grad_color, grad_allmap, out=out, accumulate=accumulate,
+                              need_means2D=need_means2D, raw_activations=raw_activations, debug=rs.debug,
+                              deterministic=deterministic)
 
 
 def backward_views_raw(state: ForwardState, radii, means3D, shs, colors_precomp, scales, rotations, transMat_precomp,
@@ -538,36 +451,24 @@ def backward_views_raw(state: ForwardState, radii, means3D, shs, colors_precomp,
         g = _grad_outputs(P, M, device, shs, colors_precomp, transMat_precomp, out or {}, accumulate, need_means2D)
         if P == 0:
             return g
-        state.resolve()
+        state.resolve()                 # capacity verified (re-run if it overflowed) before the lists are walked again
         if _lib.deterministic(deterministic):
             fn, scratch_b = lib.srf_views_backward_deterministic, _lib.det_backward_scratch_bytes(lib, V, P)
         else:
-            fn, scratch_b = lib.srf_views_backward, _lib.views_sizes(lib, V, P, H, W, 0)[5]
-        _views_backward(lib, fn, scratch_b, state, radii, means3D, shs, colors_precomp, scales, rotations,
-                        transMat_precomp, cams, tanfovx, tanfovy, H, W, sh_degree, grad_color, grad_allmap, g,
-                        accumulate, raw_activations)
+            fn, scratch_b = lib.srf_views_backward, _views_sizes(lib, V, P, H, W, state.capacity)[5]
+        _lib.check(fn(
+            _raw_stream(device), V, P, int(sh_degree), M, H, W, state.capacity, cams.data_ptr(),
+            _ptr(means3D), _ptr(shs), 1 if colors_precomp is not None else 0,
+            _ptr(scales), _ptr(rotations), 1 if transMat_precomp is not None else 0,
+            float(tanfovx), float(tanfovy), radii.data_ptr(),
+            state.geom.data_ptr(), state.tile.data_ptr(), state.point_list.data_ptr(), state.image.data_ptr(),
+            grad_color.data_ptr(), grad_allmap.data_ptr(), _blob(scratch_b, device).data_ptr(), 1 if accumulate else 0,
+            _ptr(g["means3D"]), _ptr(g["means2D"]), _ptr(g["sh"]), _ptr(g["colors_precomp"]),
+            _ptr(g["opacities"]), _ptr(g["scales"]), _ptr(g["rotations"]), _ptr(g["cov3Ds_precomp"]),
+            1 if raw_activations else 0), lib)
         if debug:
             torch.cuda.synchronize(device)
         return g
-
-
-def _views_backward(lib, fn, scratch_b, state, radii, means3D, shs, colors_precomp, scales, rotations, transMat_precomp,
-                    cams, tanfovx, tanfovy, H, W, sh_degree, grad_color, grad_allmap, g, accumulate, raw_activations):
-    """One call of srf_views_backward or srf_views_backward_deterministic (same arguments)."""
-    device = means3D.device
-    V, P = int(cams.shape[0]), int(means3D.shape[0])
-    M = int(shs.shape[1]) if shs is not None else 0
-    scratch = _blob(scratch_b, device)
-    _lib.check(fn(
-        _raw_stream(device), V, P, int(sh_degree), M, H, W, state.capacity, cams.data_ptr(),
-        _ptr(means3D), _ptr(shs), 1 if colors_precomp is not None else 0,
-        _ptr(scales), _ptr(rotations), 1 if transMat_precomp is not None else 0,
-        float(tanfovx), float(tanfovy), radii.data_ptr(),
-        state.geom.data_ptr(), state.tile.data_ptr(), state.point_list.data_ptr(), state.image.data_ptr(),
-        grad_color.data_ptr(), grad_allmap.data_ptr(), scratch.data_ptr(), 1 if accumulate else 0,
-        _ptr(g["means3D"]), _ptr(g["means2D"]), _ptr(g["sh"]), _ptr(g["colors_precomp"]),
-        _ptr(g["opacities"]), _ptr(g["scales"]), _ptr(g["rotations"]), _ptr(g["cov3Ds_precomp"]),
-        1 if raw_activations else 0), lib)
 
 
 def _dump_snapshot(path: str, items) -> None:

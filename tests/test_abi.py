@@ -18,10 +18,10 @@ def declared_symbols():
     return sorted(names)
 
 
-def test_header_declares_the_boundary():
+def test_header_declares_the_views_boundary():
     syms = declared_symbols()
-    for must in ("srf_forward_preprocess", "srf_forward_render", "srf_backward", "srf_mark_visible",
-                 "srf_geom_state_bytes", "srf_last_error"):
+    for must in ("srf_views_forward", "srf_views_forward_render", "srf_views_backward", "srf_mark_visible",
+                 "srf_views_workspace_bytes", "srf_last_error"):
         assert must in syms
 
 
@@ -40,30 +40,31 @@ def test_abi_version(lib):
     assert lib.srf_abi_version() == _lib.ABI_VERSION
 
 
-def test_workspace_sizes_host_only(lib):
+def test_views_workspace_sizes_host_only(lib):
     from lara_b200 import _lib
-    g, t, i, s = _lib.sizes(lib, 1000, 300, 500)
+    g, t, i, _, _, s = _lib.views_sizes(lib, 1, 1000, 300, 500, 0)
     assert g >= 1000 * (96 + 4 + 8) and i >= 300 * 500 * 20 and s >= 1000 * 80
     ntiles = ((500 + 15) // 16) * ((300 + 15) // 16)
     assert t >= ntiles * (256 + 8 + 4)
     goff, toff, ioff = _lib.layout(lib, 1000, 300, 500)
     assert goff[0] == 0 and goff[1] >= 96000 and goff[2] >= goff[1] + 4000
     assert all(o % 16 == 0 for o in goff + ioff)
-    e, p = _lib.binning_sizes(lib, 12345)
+    _, _, _, e, p, _ = _lib.views_sizes(lib, 1, 1000, 300, 500, 12345)
     assert e >= 12345 * 8 and p >= 12345 * 4
-    g0, _, _, s0 = _lib.sizes(lib, 0, 16, 16)
+    g0, _, _, _, _, s0 = _lib.views_sizes(lib, 1, 0, 16, 16, 0)
     assert g0 > 0 and s0 > 0
 
 
-def test_bad_arguments_return_status_and_message(lib):
-    n = ctypes.c_size_t()
-    assert lib.srf_geom_state_bytes(-1, ctypes.byref(n)) != 0
-    assert b"srf_geom_state_bytes" in lib.srf_last_error()
-    assert lib.srf_tile_state_bytes(0, 16, ctypes.byref(n)) != 0
+def test_views_entries_return_status_and_message_on_bad_arguments(lib):
+    n = (ctypes.c_size_t * 6)()
+    assert lib.srf_views_workspace_bytes(1, -1, 16, 16, 0, n) != 0
+    assert b"srf_views_workspace_bytes" in lib.srf_last_error()
+    assert lib.srf_views_workspace_bytes(1, 0, 0, 16, 0, n) != 0
     # null / misaligned workspaces are rejected before any CUDA call
-    args = [None, 4, 0, 1, None, None, None, None, None, 1.0, None, None, None, None, None,
-            1.0, 1.0, 16, 16, 0, None, None, None, None, 0]
-    assert lib.srf_forward_preprocess(*args) != 0
+    cams = (ctypes.c_float * 24)()
+    args = [None, 1, 4, 0, 1, None, None, None, None, None, None, None, ctypes.addressof(cams),
+            1.0, 1.0, 16, 16, 0, 0, None, None, None, None, None, None, None, None, None, None, 0]
+    assert lib.srf_views_forward(*args) != 0
     assert lib.srf_last_error() != b""
 
 

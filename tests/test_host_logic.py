@@ -210,13 +210,12 @@ def test_views_of_a_batched_call_must_share_size_fov_and_degree():
         shared_view_settings([a, _cpu_settings(deg=2)])
 
 
-def test_view_workspaces_are_the_single_view_ones_back_to_back():
+def test_view_workspaces_are_the_one_view_ones_back_to_back():
     """srf_views_workspace_bytes (host only): V per-view workspaces at a byte stride of the single-view size."""
     from lara_b200 import _lib
     lib = _lib.load()
     P, H, W, cap = 5000, 200, 136, 123456
-    g1, t1, i1, s1 = _lib.sizes(lib, P, H, W)
-    e1, p1 = _lib.binning_sizes(lib, cap)
+    g1, t1, i1, e1, p1, s1 = _lib.views_sizes(lib, 1, P, H, W, cap)
     for V in (1, 3, 8):
         g, t, i, e, pl, s = _lib.views_sizes(lib, V, P, H, W, cap)
         assert (g, t, i, e, pl) == (V * g1, V * t1, V * i1, V * e1, V * p1)
