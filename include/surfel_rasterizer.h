@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define SRF_ABI_VERSION 8
+#define SRF_ABI_VERSION 9
 
 /* cudaStream_t without pulling in cuda_runtime.h */
 typedef void* srf_stream_t;
@@ -262,6 +262,14 @@ int srf_point_feats_backward_deterministic(srf_stream_t stream, int V, int n, in
  * gradient through (b, c) is exactly 0.  Deterministic: no atomics.                                               */
 typedef struct srf_ms_ssim_addr { int64_t sb, sc, sy, sx, sv, wv; } srf_ms_ssim_addr;
 int srf_ms_ssim_workspace_bytes(int B, int C, int H, int W, size_t* bytes);
+/* Host only, for tests and tooling that read the workspace after a call (lara_b200.debug.unpack_ms_ssim).
+ *   regions[7]  : byte offsets of the pyramid, its gradient, the per-CTA partial sums (double), the means (double
+ *                 [5][B C]), the values (double [B C]), the coefficients (float [5][B C]); then the total size
+ *   levels[15]  : per level l, the element index of X_l in the pyramid (float; Y_l follows B C h_l w_l floats later),
+ *                 of dX_l in the gradient pyramid (float) and of the level's partial sums (double [B C][ntx ny]);
+ *                 the first two are unused at l = 0, whose X, Y and dX are the caller's tensors
+ *   dims[30]    : h[5], w[5], px[5], py[5] (pooling padding to the next level), ntx[5], nty[5] (forward tiles)  */
+int srf_ms_ssim_workspace_layout(int B, int C, int H, int W, size_t regions[7], size_t levels[15], int dims[30]);
 int srf_ms_ssim_forward(srf_stream_t stream, int B, int C, int H, int W,
                         const float* x, const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
                         float data_range, int size_average, void* workspace, float* out);

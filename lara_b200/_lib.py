@@ -14,7 +14,7 @@ from typing import Optional
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libsurfel_b200.so")
-ABI_VERSION = 8
+ABI_VERSION = 9
 CAM_FLOATS, CAM_VIEW, CAM_CAMPOS, CAM_BG = 24, 0, 16, 19      # include/surfel_rasterizer.h SRF_CAM_*
 
 
@@ -90,6 +90,8 @@ SIGNATURES = {
     "srf_point_feats_backward_deterministic": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P,
                                                        _P, _P, _P, _P, _P]),
     "srf_ms_ssim_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, POINTER(c_size_t)]),
+    "srf_ms_ssim_workspace_layout": (c_int, [c_int, c_int, c_int, c_int, POINTER(c_size_t), POINTER(c_size_t),
+                                             POINTER(c_int)]),
     "srf_ms_ssim_forward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _A, _P, _A, c_float, c_int, _P, _P]),
     "srf_ms_ssim_backward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _A, _P, _A, c_float, c_int, _P, _P, _P, _A]),
     "srf_mark_visible": (c_int, [_P, c_int, _P, _P, _P, _P]),
@@ -184,6 +186,20 @@ def layout(lib, P: int, H: int, W: int):
     i = (c_size_t * 2)()
     check(lib.srf_state_layout(P, H, W, g, t, i), lib)
     return list(g), list(t), list(i)
+
+
+def ms_ssim_layout(lib, B: int, C: int, H: int, W: int) -> dict:
+    """srf_ms_ssim_workspace_layout: the workspace's byte offsets ("pyr", "gpyr", "part", "mean", "val", "coef",
+    "total"), the per-level element indices ("pyr_l", "gpyr_l", "part_l") and geometry ("h", "w", "px", "py", "ntx",
+    "nty"), each a list over the 5 levels."""
+    r, lv, d = (c_size_t * 7)(), (c_size_t * 15)(), (c_int * 30)()
+    check(lib.srf_ms_ssim_workspace_layout(B, C, H, W, r, lv, d), lib)
+    out = dict(zip(("pyr", "gpyr", "part", "mean", "val", "coef", "total"), (int(x) for x in r)))
+    for i, k in enumerate(("pyr_l", "gpyr_l", "part_l")):
+        out[k] = [int(x) for x in lv[5 * i:5 * i + 5]]
+    for i, k in enumerate(("h", "w", "px", "py", "ntx", "nty")):
+        out[k] = [int(x) for x in d[5 * i:5 * i + 5]]
+    return out
 
 
 KERNEL_NAMES = ["preprocess_fwd", "tile_scan", "scatter", "sort_small", "sort_big", "render_fwd",

@@ -795,6 +795,13 @@ int srf_ms_ssim_workspace_bytes(int B, int C, int H, int W, size_t* bytes) {
     return 0;
 }
 
+int srf_ms_ssim_workspace_layout(int B, int C, int H, int W, size_t regions[7], size_t levels[15], int dims[30]) {
+    if (ms_ssim_sizes("srf_ms_ssim_workspace_layout", B, C, H, W)) return 1;
+    if (!regions || !levels || !dims) return fail("srf_ms_ssim_workspace_layout: null pointer");
+    srf::ms_ssim_workspace_layout(B, C, H, W, regions, levels, dims);
+    return 0;
+}
+
 int srf_ms_ssim_forward(srf_stream_t stream_, int B, int C, int H, int W,
                         const float* x, const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
                         float data_range, int size_average, void* workspace, float* out) {

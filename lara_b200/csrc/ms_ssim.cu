@@ -404,6 +404,17 @@ LevelArgs level_args(const MsSsimArgs& m, const Layout& L, char* ws, int l) {
 
 size_t ms_ssim_workspace_bytes(int B, int C, int H, int W) { return make_layout(B, C, H, W).total; }
 
+void ms_ssim_workspace_layout(int B, int C, int H, int W, size_t regions[7], size_t levels[15], int dims[30]) {
+    const Layout L = make_layout(B, C, H, W);
+    const size_t r[7] = {L.o_pyr, L.o_gpyr, L.o_part, L.o_mean, L.o_val, L.o_coef, L.total};
+    for (int i = 0; i < 7; ++i) regions[i] = r[i];
+    for (int l = 0; l < kLevels; ++l) {
+        levels[l] = L.pyr[l]; levels[kLevels + l] = L.gpyr[l]; levels[2 * kLevels + l] = L.part[l];
+        const int d[6] = {L.h[l], L.w[l], L.px[l], L.py[l], L.ntx[l], L.nty[l]};
+        for (int i = 0; i < 6; ++i) dims[i * kLevels + l] = d[i];
+    }
+}
+
 cudaError_t launch_ms_ssim(const MsSsimArgs& m, bool backward, cudaStream_t stream) {
     const Layout L = make_layout(m.B, m.C, m.H, m.W);
     char* ws = static_cast<char*>(m.workspace);

@@ -232,6 +232,8 @@ struct MsSsimArgs {
     float* gx; MsAddr ag;        // backward output, dL/dX
 };
 size_t ms_ssim_workspace_bytes(int B, int C, int H, int W);
+// host only: the workspace's regions and level geometry (srf_ms_ssim_workspace_layout in the C ABI)
+void ms_ssim_workspace_layout(int B, int C, int H, int W, size_t regions[7], size_t levels[15], int dims[30]);
 cudaError_t launch_ms_ssim(const MsSsimArgs& a, bool backward, cudaStream_t stream);
 
 // Optional per-kernel CUDA-event timing (srf_profile_begin/end in the C ABI); no-ops unless enabled.

@@ -64,3 +64,32 @@ def unpack_state(state: ForwardState, P: int, H: int, W: int, view: int = 0) -> 
     moff = (4 * cap + 255) // 256 * 256
     out["contrib_masks"] = state.point_list[moff:moff + 32 * cap].view(torch.int32).view(8, cap)[:, :R]
     return out
+
+
+def unpack_ms_ssim(ws: torch.Tensor, B: int, C: int, H: int, W: int) -> Dict[str, object]:
+    """Views into a fused MS-SSIM workspace (uint8, srf_ms_ssim_workspace_bytes) of the logical B x C x H x W image,
+    through ``srf_ms_ssim_workspace_layout``: ``X``, ``Y``, ``dX`` lists over the levels of [B,C,h_l,w_l] tensors
+    (None at level 0, which lives in the caller's tensors), ``part`` (list of [B*C, tiles] double), ``mean``
+    [5,B,C] double, ``val`` [B,C] double, ``coef`` [5,B,C] float, and the geometry under ``layout``."""
+    L = _lib.ms_ssim_layout(_lib.load(), B, C, H, W)
+    P = B * C
+
+    def f32(off, n):
+        return ws[off:off + 4 * n].view(torch.float32)
+
+    out: Dict[str, object] = {"layout": L, "X": [None], "Y": [None], "dX": [None], "part": []}
+    for l in range(5):
+        h, w = L["h"][l], L["w"][l]
+        n = P * h * w
+        if l:
+            xy = f32(L["pyr"] + 4 * L["pyr_l"][l], 2 * n).view(2, B, C, h, w)
+            out["X"].append(xy[0])
+            out["Y"].append(xy[1])
+            out["dX"].append(f32(L["gpyr"] + 4 * L["gpyr_l"][l], n).view(B, C, h, w))
+        nt = L["ntx"][l] * L["nty"][l]
+        off = L["part"] + 8 * L["part_l"][l]
+        out["part"].append(ws[off:off + 8 * P * nt].view(torch.float64).view(P, nt))
+    out["mean"] = ws[L["mean"]:L["mean"] + 8 * 5 * P].view(torch.float64).view(5, B, C)
+    out["val"] = ws[L["val"]:L["val"] + 8 * P].view(torch.float64).view(B, C)
+    out["coef"] = f32(L["coef"], 5 * P).view(5, B, C)
+    return out

@@ -514,6 +514,17 @@ def _chain(dev, det, ms_ssim):
     settings = [S.settings_for(c, torch.ones(3), 1, dev, R.GaussianRasterizationSettings) for c in cams]
     tar = torch.rand((V, H, W, 3), generator=g).to(dev)
     x = feats.to(dev).requires_grad_(True)
+    if ms_ssim:
+        # against uniform noise cs is about 0, so relu would leave the MS-SSIM term without a gradient or with
+        # planes whose sign is undecided: a target correlated with a first rendering instead
+        from test_ms_ssim import smooth_pair
+        with torch.no_grad():
+            dec = gaussians_from_decoder(x, grid.to(dev), K_, sh_dim, -2.1792, -4.2, 0.5 / 16)
+            centers, shs, scaling, rotation, opacity = (t.reshape((-1,) + tuple(t.shape[2:])) for t in dec)
+            img = render_scene_views(centers, shs, opacity, scaling, rotation, settings, rays=rays,
+                                     raw_activations=True)["image"]
+        _, pert = smooth_pair(V, 3, H, W, 78, dtype=torch.float32)
+        tar = (img + 0.1 * (pert.to(dev).permute(0, 2, 3, 1) - 0.5)).clamp(0, 1).contiguous()
     prev = torch.are_deterministic_algorithms_enabled()
     torch.use_deterministic_algorithms(det)
     try:
@@ -524,12 +535,12 @@ def _chain(dev, det, ms_ssim):
         out = render_scene_views(centers, shs, opacity, scaling, rotation, settings, rays=rays, raw_activations=True)
         for k in OUT_KEYS:
             out[k].retain_grad()
-        loss, _ = scene_loss(out, tar, 5000, ms_ssim=ms_ssim)
+        loss, stats = scene_loss(out, tar, 5000, ms_ssim=ms_ssim)
         (loss * 2.0).backward()
         torch.cuda.synchronize()
     finally:
         torch.use_deterministic_algorithms(prev)
-    return dict(feats=feats, grid=grid, x=x, dec=dec, out=out, loss=loss, tar=tar, cams=cams, rays=rays,
+    return dict(feats=feats, grid=grid, x=x, dec=dec, out=out, loss=loss, stats=stats, tar=tar, cams=cams, rays=rays,
                 settings=settings, params=(centers, shs, opacity, scaling, rotation), K=K_, sh_dim=sh_dim)
 
 
@@ -563,29 +574,44 @@ def test_lara_chain_link_by_link(cuda_device, det, ms_ssim):
     worst = {}
     # 1. decoder forward
     ref, _ = C.decoder64(ch["feats"], ch["grid"], ch["K"], ch["sh_dim"], -2.1792, -4.2, 0.5 / 16)
-    if not ms_ssim:
-        worst["decoder fwd"] = max(_compare(t.detach().cpu().numpy(), r, ctx="decoder fwd") for t, r in zip(ch["dec"], ref))
+    worst["decoder fwd"] = max(_compare(t.detach().cpu().numpy(), r, ctx="decoder fwd") for t, r in zip(ch["dec"], ref))
     # 2. epilogue forward and 3. the loss, given their actual fp32 inputs
     grads = {k: out[k].grad for k in OUT_KEYS}
     gpl = {k: (None if g is None else (g.permute(0, 3, 1, 2) if g.ndim == 4 else g).contiguous()) for k, g in grads.items()}
-    if not ms_ssim:
-        w = 0.0
-        for v in range(V):
-            st = C.EpilogueState(col[v], am[v], rays[v], vms[v], 0.0)
-            r, band, _ = C.epilogue64(None, None, None, None, None, state=st)
-            assert band.sum() == 0
-            for k, t in zip(OUT_KEYS, o):
-                w = max(w, _compare(t[v].cpu().numpy(), r[k], ctx=f"epilogue fwd view {v} {k}"))
-        worst["epilogue fwd"] = w
-        pl = {k: t.cpu() for k, t in zip(OUT_KEYS, o)}
-        n = V * H * W
-        blocks = min(1024, -(-n // 256)) if det else min(8 * _sm_count(), -(-n // 256))
-        vals, lg = C.loss64(pl["image"], ch["tar"].cpu(), pl["rend_normal"], pl["depth_normal"], pl["acc_map"],
-                            pl["rend_dist"], True, 1, 2.0, blocks)
-        v_, e_ = vals["loss"]
-        assert abs(float(ch["loss"]) - v_) <= e_
-        worst["loss"] = max(_compare(gpl[k].cpu().numpy(), g, ctx=f"loss {k}") for k, g in lg.items())
-        assert gpl["depth"] is None and gpl["acc_map"] is None
+    w = 0.0
+    for v in range(V):
+        st = C.EpilogueState(col[v], am[v], rays[v], vms[v], 0.0)
+        r, band, _ = C.epilogue64(None, None, None, None, None, state=st)
+        assert band.sum() == 0
+        for k, t in zip(OUT_KEYS, o):
+            w = max(w, _compare(t[v].cpu().numpy(), r[k], ctx=f"epilogue fwd view {v} {k}"))
+    worst["epilogue fwd"] = w
+    pl = {k: t.cpu() for k, t in zip(OUT_KEYS, o)}
+    n = V * H * W
+    blocks = min(1024, -(-n // 256)) if det else min(8 * _sm_count(), -(-n // 256))
+    vals, lg = C.loss64(pl["image"], ch["tar"].cpu(), pl["rend_normal"], pl["depth_normal"], pl["acc_map"],
+                        pl["rend_dist"], True, 1, 2.0, blocks)
+    loss_ref = EB(*vals["loss"])
+    w = 0.0
+    if ms_ssim:
+        # + (0.5 / B) (1 - s) in fp32 torch ops; the MS-SSIM gradient for autograd's upstream fp32(-0.5 * 2.0) on the
+        # views side by side, added to the MSE gradient in fp32
+        from oracle import ms_ssim64 as M
+        cat = lambda a: np.concatenate(list(a), axis=-1)[None]          # noqa: E731
+        ms = M.ms_ssim64(cat(pl["image"].numpy()), cat(ch["tar"].cpu().permute(0, 3, 1, 2).numpy()), 1.0, True,
+                         [float(np.float32(-0.5 * 2.0))])
+        assert all(p["state"] == "pos" for p in ms["planes"].values()), [p["m"] for p in ms["planes"].values()]
+        s = EB(*ms["out"][0])
+        w = max(w, _compare(float(ch["stats"]["ssim"]), s, ctx="ssim stat"))
+        loss_ref = M.Bound.add(loss_ref, M.Bound.scale(M.Bound.sub(1.0, s), 0.5))
+        gv = np.stack([ms["planes"][(0, c)]["dX"][0].v for c in range(3)]).reshape(3, H, V, W).transpose(2, 0, 1, 3)
+        ge = np.stack([ms["planes"][(0, c)]["dX"][0].e for c in range(3)]).reshape(3, H, V, W).transpose(2, 0, 1, 3)
+        lg["image"] = M.Bound.add(lg["image"], EB(gv, ge))
+    w = max(w, _compare(float(ch["loss"].detach()), loss_ref, ctx="loss value"))
+    worst["loss"] = max([w] + [_compare(gpl[k].cpu().numpy(), g, ctx=f"loss {k}") for k, g in lg.items()])
+    if ms_ssim:
+        worst["loss value, ssim stat and g_image with MS-SSIM"] = max(w, _compare(gpl["image"].cpu().numpy(), lg["image"]))
+    assert gpl["depth"] is None and gpl["acc_map"] is None
     # 4. epilogue vjp, given the node's upstream maps
     d_color, d_allmap = epilogue_views_backward_raw(color, allmap, ch["rays"], camt, 0.0, gpl["image"], gpl["depth"],
                                                     gpl["acc_map"], gpl["rend_normal"], gpl["depth_normal"],
