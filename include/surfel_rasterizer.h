@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define SRF_ABI_VERSION 9
+#define SRF_ABI_VERSION 10
 
 /* cudaStream_t without pulling in cuda_runtime.h */
 typedef void* srf_stream_t;
@@ -127,7 +127,13 @@ int srf_views_forward_render(srf_stream_t stream, int V, int P, int image_height
  *   dL_dtransMat[P,9] the gradient wrt the homography (cov3D_precomp slot).
  * raw_activations: the flag given to the forward; `scales` / `rotations` are then the raw
  * tensors and dL_dopacity / dL_dscales / dL_drotations are wrt the raw parameters (the
- * activated opacity is read back from geom_state).                                    */
+ * activated opacity is read back from geom_state).
+ * deterministic != 0 (also for V = 1): same results, but the blend backward's per-lane partial sums are added in
+ * 64-bit fixed point (two passes of the blend backward: per-channel bounds, then the sums), so two calls on the same
+ * inputs give bit-identical gradients.  `scratch` (256-byte aligned) is then
+ * srf_views_backward_deterministic_scratch_bytes(V, P) bytes, and the call waits for the stream before it returns: if a
+ * partial sum is not finite or beyond the fixed-point range it returns an error instead of a gradient (the output
+ * arrays then hold no meaningful values, and with accumulate != 0 they have been added to).                          */
 int srf_views_backward(srf_stream_t stream, int V, int P, int D, int M, int image_height, int image_width,
                        size_t capacity, const float* cams,
                        const float* means3D, const float* shs, int colors_were_precomputed,
@@ -139,26 +145,8 @@ int srf_views_backward(srf_stream_t stream, int V, int P, int D, int M, int imag
                        void* scratch, int accumulate,
                        float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
                        float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
-                       int raw_activations);
-/* Deterministic variant of srf_views_backward (also for V = 1): same arguments and results, but the blend
- * backward's per-lane partial sums are added in 64-bit fixed point (two passes of the blend backward: per-channel
- * bounds, then the sums), so two calls on the same inputs give bit-identical gradients.  `scratch` (256-byte aligned)
- * is srf_views_backward_deterministic_scratch_bytes(V, P) bytes.  Waits for the stream before it returns: if a partial
- * sum is not finite or beyond the fixed-point range it returns an error instead of a gradient (the output arrays then
- * hold no meaningful values, and with accumulate != 0 they have been added to).                                       */
+                       int raw_activations, int deterministic);
 int srf_views_backward_deterministic_scratch_bytes(int V, int P, size_t* bytes);
-int srf_views_backward_deterministic(srf_stream_t stream, int V, int P, int D, int M, int image_height, int image_width,
-                                     size_t capacity, const float* cams,
-                                     const float* means3D, const float* shs, int colors_were_precomputed,
-                                     const float* scales, const float* rotations, int transmat_was_precomputed,
-                                     float tan_fovx, float tan_fovy, const int* radii,
-                                     const void* geom_state, const void* tile_state, const uint32_t* point_list,
-                                     const void* image_state,
-                                     const float* dL_dout_color, const float* dL_dout_others,
-                                     void* scratch, int accumulate,
-                                     float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
-                                     float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
-                                     int raw_activations);
 
 /* ---- fused render_img epilogue (next-row: lightning/renderer_2dgs.py:220-268, :74-89) ---------
  * One pass over the rasterizer's outputs of V stacked views instead of ~12 torch ops (and ~20 autograd
@@ -189,17 +177,14 @@ int srf_views_epilogue_backward(srf_stream_t stream, int V, int image_height, in
  * them; `target_hwc` is the batch's own channel-last [V,H,W,3].  srf_loss_backward writes the four gradient maps
  * srf_views_epilogue_backward consumes, scaled by the device scalar `upstream` (NULL = 1):
  *   g_image = 2 w_mse (image - target), g_rend_dist = w_dist, g_rend_normal = -w_normal acc depth_normal,
- *   g_depth_normal = -w_normal acc rend_normal   (w_* = weight / element count).                          */
+ *   g_depth_normal = -w_normal acc rend_normal   (w_* = weight / element count).
+ * srf_loss_forward's `workspace`: NULL sums with atomics; otherwise (deterministic) the per-block partial sums go to
+ * `workspace` (8-byte aligned, srf_loss_deterministic_workspace_bytes) and are reduced in a fixed order, on a grid
+ * that does not depend on the device.                                                                       */
 int srf_loss_forward(srf_stream_t stream, int V, int image_height, int image_width, int with_reg,
                      const float* image, const float* target_hwc, const float* rend_normal, const float* depth_normal,
-                     const float* acc_map, const float* rend_dist, double* sums);
-/* Deterministic srf_loss_forward: the per-block partial sums go to `workspace` (8-byte aligned,
- * srf_loss_deterministic_workspace_bytes) and are reduced in a fixed order, on a grid that does not depend on the device. */
+                     const float* acc_map, const float* rend_dist, double* sums, void* workspace);
 int srf_loss_deterministic_workspace_bytes(int V, int image_height, int image_width, size_t* bytes);
-int srf_loss_forward_deterministic(srf_stream_t stream, int V, int image_height, int image_width, int with_reg,
-                                   const float* image, const float* target_hwc, const float* rend_normal,
-                                   const float* depth_normal, const float* acc_map, const float* rend_dist, double* sums,
-                                   void* workspace);
 int srf_loss_backward(srf_stream_t stream, int V, int image_height, int image_width, int with_reg,
                       float w_mse, float w_dist, float w_normal,
                       const float* image, const float* target_hwc, const float* rend_normal, const float* depth_normal,
@@ -229,7 +214,11 @@ int srf_decoder_layout_backward(srf_stream_t stream, size_t B, int N, int K, int
  * The backward writes g_points [n,3] (summed over views) and adds the gradients of image, acc and depth into
  * g_image / g_acc / g_depth, which it clears first; img_ref gets no gradient.  Each gradient output may be
  * NULL (not wanted).  n == 0 launches no kernel (the backward still clears the rendering gradients) and
- * points, feats and g_feats may then be NULL.                                                                      */
+ * points, feats and g_feats may then be NULL.
+ * The backward's `workspace`: NULL adds with atomics; otherwise (deterministic) the rendering gradients are summed in
+ * 64-bit fixed point in `workspace` (256-byte aligned, srf_point_feats_deterministic_workspace_bytes) and then written,
+ * so two calls give identical bits; the call then waits for the stream and returns an error instead of a gradient if
+ * g_feats holds a non-finite value.                                                                                 */
 int srf_point_feats_forward(srf_stream_t stream, int V, int n, int H, int W,
                             const float* points, const float* w2cs, const float* ixts,
                             const float* img_ref, const float* image, const float* acc, const float* depth,
@@ -237,16 +226,9 @@ int srf_point_feats_forward(srf_stream_t stream, int V, int n, int H, int W,
 int srf_point_feats_backward(srf_stream_t stream, int V, int n, int H, int W,
                              const float* points, const float* w2cs, const float* ixts,
                              const float* img_ref, const float* image, const float* acc, const float* depth,
-                             const float* g_feats, float* g_points, float* g_image, float* g_acc, float* g_depth);
-/* Deterministic srf_point_feats_backward: the rendering gradients are summed in 64-bit fixed point in `workspace`
- * (256-byte aligned, srf_point_feats_deterministic_workspace_bytes) and then written, so two calls give identical bits.
- * Waits for the stream; returns an error instead of a gradient if g_feats holds a non-finite value.                */
+                             const float* g_feats, float* g_points, float* g_image, float* g_acc, float* g_depth,
+                             void* workspace);
 int srf_point_feats_deterministic_workspace_bytes(int V, int H, int W, size_t* bytes);
-int srf_point_feats_backward_deterministic(srf_stream_t stream, int V, int n, int H, int W,
-                                           const float* points, const float* w2cs, const float* ixts,
-                                           const float* img_ref, const float* image, const float* acc, const float* depth,
-                                           const float* g_feats, float* g_points, float* g_image, float* g_acc,
-                                           float* g_depth, void* workspace);
 
 /* ---- fused MS-SSIM (next-row: lightning/loss.py:44-47, pytorch-msssim 1.0.0 MS_SSIM, channel = C) -------------
  * The 5-level MS-SSIM of X (rendering) and Y (target), logical images B x C x H x W, with the library's valid 11-tap

@@ -14,7 +14,7 @@ from typing import Optional
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libsurfel_b200.so")
-ABI_VERSION = 9
+ABI_VERSION = 10
 CAM_FLOATS, CAM_VIEW, CAM_CAMPOS, CAM_BG = 24, 0, 16, 19      # include/surfel_rasterizer.h SRF_CAM_*
 
 
@@ -60,35 +60,20 @@ SIGNATURES = {
         _P, c_int,                               # scratch, accumulate
         _P, _P, _P, _P,                          # dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors
         _P, _P, _P, _P,                          # dL_dopacity, dL_dscales, dL_drotations, dL_dtransMat
-        c_int,                                   # raw_activations
+        c_int, c_int,                            # raw_activations, deterministic
     ]),
     "srf_views_backward_deterministic_scratch_bytes": (c_int, [c_int, c_int, POINTER(c_size_t)]),
-    "srf_views_backward_deterministic": (c_int, [
-        _P, c_int, c_int, c_int, c_int, c_int, c_int,   # stream, V, P, D, M, H, W
-        c_size_t, _P,                            # capacity, cams
-        _P, _P, c_int,                           # means3D, shs, colors_were_precomputed
-        _P, _P, c_int,                           # scales, rotations, transmat_was_precomputed
-        c_float, c_float, _P,                    # tan_fovx, tan_fovy, radii
-        _P, _P, _P, _P,                          # geom_state, tile_state, point_list, image_state
-        _P, _P,                                  # dL_dout_color, dL_dout_others
-        _P, c_int,                               # scratch, accumulate
-        _P, _P, _P, _P,                          # dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors
-        _P, _P, _P, _P,                          # dL_dopacity, dL_dscales, dL_drotations, dL_dtransMat
-        c_int,                                   # raw_activations
-    ]),
     "srf_views_epilogue_forward": (c_int, [_P, c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "srf_views_epilogue_backward": (c_int, [_P, c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
-    "srf_loss_forward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P]),
+    "srf_loss_forward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P]),
     "srf_loss_deterministic_workspace_bytes": (c_int, [c_int, c_int, c_int, POINTER(c_size_t)]),
-    "srf_loss_forward_deterministic": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P]),
     "srf_loss_backward": (c_int, [_P, c_int, c_int, c_int, c_int, c_float, c_float, c_float, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "srf_decoder_layout_forward": (c_int, [_P, c_size_t, c_int, c_int, c_int, c_float, c_float, c_float, _P, _P, _P, _P, _P, _P, _P]),
     "srf_decoder_layout_backward": (c_int, [_P, c_size_t, c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P]),
     "srf_point_feats_forward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P]),
-    "srf_point_feats_backward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "srf_point_feats_backward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
+                                         _P]),
     "srf_point_feats_deterministic_workspace_bytes": (c_int, [c_int, c_int, c_int, POINTER(c_size_t)]),
-    "srf_point_feats_backward_deterministic": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P,
-                                                       _P, _P, _P, _P, _P]),
     "srf_ms_ssim_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, POINTER(c_size_t)]),
     "srf_ms_ssim_workspace_layout": (c_int, [c_int, c_int, c_int, c_int, POINTER(c_size_t), POINTER(c_size_t),
                                              POINTER(c_int)]),
@@ -152,7 +137,7 @@ def _size_query(fn, *args) -> int:
 
 
 def det_backward_scratch_bytes(lib, V: int, P: int) -> int:
-    """Scratch of srf_views_backward_deterministic."""
+    """Scratch of srf_views_backward(..., deterministic=1)."""
     return _size_query(lib.srf_views_backward_deterministic_scratch_bytes, V, P)
 
 

@@ -489,38 +489,19 @@ int srf_views_backward(srf_stream_t stream_, int V, int P, int D, int M, int ima
                        void* scratch, int accumulate,
                        float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
                        float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
-                       int raw_activations) {
+                       int raw_activations, int deterministic) {
     return backward_impl("srf_views_backward", static_cast<cudaStream_t>(stream_), V, P, D, M, image_height, image_width,
                          capacity, cams, means3D, shs, colors_were_precomputed, scales, rotations,
                          transmat_was_precomputed, tan_fovx, tan_fovy, radii, geom_state, tile_state, point_list,
                          image_state, dL_dout_color, dL_dout_others, scratch, accumulate, dL_dmeans3D, dL_dmeans2D,
                          dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drotations, dL_dtransMat, raw_activations,
-                         false);
+                         deterministic != 0);
 }
 
 int srf_views_backward_deterministic_scratch_bytes(int V, int P, size_t* bytes) {
     if (V <= 0 || P < 0 || !bytes) return fail("srf_views_backward_deterministic_scratch_bytes: bad arguments");
     *bytes = det_scratch_bytes(V, P);
     return 0;
-}
-
-int srf_views_backward_deterministic(srf_stream_t stream_, int V, int P, int D, int M, int image_height, int image_width,
-                                     size_t capacity, const float* cams,
-                                     const float* means3D, const float* shs, int colors_were_precomputed,
-                                     const float* scales, const float* rotations, int transmat_was_precomputed,
-                                     float tan_fovx, float tan_fovy, const int* radii,
-                                     const void* geom_state, const void* tile_state, const uint32_t* point_list,
-                                     const void* image_state,
-                                     const float* dL_dout_color, const float* dL_dout_others,
-                                     void* scratch, int accumulate,
-                                     float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
-                                     float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
-                                     int raw_activations) {
-    return backward_impl("srf_views_backward_deterministic", static_cast<cudaStream_t>(stream_), V, P, D, M, image_height,
-                         image_width, capacity, cams, means3D, shs, colors_were_precomputed, scales, rotations,
-                         transmat_was_precomputed, tan_fovx, tan_fovy, radii, geom_state, tile_state, point_list,
-                         image_state, dL_dout_color, dL_dout_others, scratch, accumulate, dL_dmeans3D, dL_dmeans2D,
-                         dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drotations, dL_dtransMat, raw_activations, true);
 }
 
 int srf_views_epilogue_forward(srf_stream_t stream_, int V, int image_height, int image_width, float depth_ratio,
@@ -565,18 +546,21 @@ int srf_views_epilogue_backward(srf_stream_t stream_, int V, int image_height, i
 
 int srf_loss_forward(srf_stream_t stream_, int V, int image_height, int image_width, int with_reg,
                      const float* image, const float* target_hwc, const float* rend_normal, const float* depth_normal,
-                     const float* acc_map, const float* rend_dist, double* sums) {
+                     const float* acc_map, const float* rend_dist, double* sums, void* workspace) {
     if (V <= 0 || image_height <= 0 || image_width <= 0) return fail("srf_loss_forward: bad sizes");
     if (!image || !target_hwc || !sums) return fail("srf_loss_forward: null pointer");
     if (with_reg && (!rend_normal || !depth_normal || !acc_map || !rend_dist)) return fail("srf_loss_forward: null regulariser input");
+    if (reinterpret_cast<uintptr_t>(workspace) & 7) return fail("srf_loss_forward: workspace must be 8-byte aligned");
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    cudaError_t e = cudaMemsetAsync(sums, 0, 3 * sizeof(double), stream);
-    if (e != cudaSuccess) return cuda_fail("memset loss sums", e);
+    cudaError_t e;
+    // the deterministic path writes every sum from its partials; the atomics need zeroed sums
+    if (!workspace && (e = cudaMemsetAsync(sums, 0, 3 * sizeof(double), stream)) != cudaSuccess)
+        return cuda_fail("memset loss sums", e);
     srf::LossArgs a;
     memset(&a, 0, sizeof(a));
     a.W = image_width; a.H = image_height; a.nviews = V; a.with_reg = with_reg ? 1 : 0;
     a.image = image; a.target = target_hwc; a.rend_normal = rend_normal; a.depth_normal = depth_normal;
-    a.acc = acc_map; a.dist = rend_dist; a.sums = sums;
+    a.acc = acc_map; a.dist = rend_dist; a.sums = sums; a.partials = static_cast<double*>(workspace);
     e = srf::launch_loss_fused(a, stream);
     if (e != cudaSuccess) return cuda_fail("loss_sums launch", e);
     return 0;
@@ -585,25 +569,6 @@ int srf_loss_forward(srf_stream_t stream_, int V, int image_height, int image_wi
 int srf_loss_deterministic_workspace_bytes(int V, int image_height, int image_width, size_t* bytes) {
     if (V <= 0 || image_height <= 0 || image_width <= 0 || !bytes) return fail("srf_loss_deterministic_workspace_bytes: bad arguments");
     *bytes = srf::loss_det_blocks((size_t)V * image_height * image_width) * 3 * sizeof(double);
-    return 0;
-}
-
-int srf_loss_forward_deterministic(srf_stream_t stream_, int V, int image_height, int image_width, int with_reg,
-                                   const float* image, const float* target_hwc, const float* rend_normal,
-                                   const float* depth_normal, const float* acc_map, const float* rend_dist, double* sums,
-                                   void* workspace) {
-    const char* fn = "srf_loss_forward_deterministic";
-    if (V <= 0 || image_height <= 0 || image_width <= 0) return fail("%s: bad sizes", fn);
-    if (!image || !target_hwc || !sums) return fail("%s: null pointer", fn);
-    if (with_reg && (!rend_normal || !depth_normal || !acc_map || !rend_dist)) return fail("%s: null regulariser input", fn);
-    if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 7)) return fail("%s: workspace must be 8-byte aligned", fn);
-    srf::LossArgs a;
-    memset(&a, 0, sizeof(a));
-    a.W = image_width; a.H = image_height; a.nviews = V; a.with_reg = with_reg ? 1 : 0;
-    a.image = image; a.target = target_hwc; a.rend_normal = rend_normal; a.depth_normal = depth_normal;
-    a.acc = acc_map; a.dist = rend_dist; a.sums = sums; a.partials = static_cast<double*>(workspace);
-    cudaError_t e = srf::launch_loss_fused(a, static_cast<cudaStream_t>(stream_));
-    if (e != cudaSuccess) return cuda_fail("loss_sums launch", e);
     return 0;
 }
 
@@ -694,69 +659,52 @@ int srf_point_feats_forward(srf_stream_t stream_, int V, int n, int H, int W,
     return 0;
 }
 
+// deterministic workspace: header (max |g_feats|, overflow flag), then the int64 planes g_image | g_acc | g_depth
+static size_t pf_det_planes_offset() { return 256; }
+static size_t pf_det_workspace_bytes(int V, int H, int W) {
+    return pf_det_planes_offset() + 5 * (size_t)V * H * W * sizeof(long long);
+}
+
 int srf_point_feats_backward(srf_stream_t stream_, int V, int n, int H, int W,
                              const float* points, const float* w2cs, const float* ixts,
                              const float* img_ref, const float* image, const float* acc, const float* depth,
-                             const float* g_feats, float* g_points, float* g_image, float* g_acc, float* g_depth) {
+                             const float* g_feats, float* g_points, float* g_image, float* g_acc, float* g_depth,
+                             void* workspace) {
     const char* fn = "srf_point_feats_backward";
     if (point_feats_check(fn, V, n, H, W, points, w2cs, ixts, img_ref, image, acc, depth)) return 1;
     if (n > 0 && !g_feats) return fail("%s: null upstream gradient", fn);
+    if (workspace && misaligned(workspace)) return fail("%s: workspace must be 256-byte aligned", fn);
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    const size_t plane = (size_t)V * H * W * sizeof(float);
-    cudaError_t e = cudaSuccess;
-    if (g_image && (e = cudaMemsetAsync(g_image, 0, 3 * plane, stream)) != cudaSuccess) return cuda_fail("memset g_image", e);
-    if (g_acc && (e = cudaMemsetAsync(g_acc, 0, plane, stream)) != cudaSuccess) return cuda_fail("memset g_acc", e);
-    if (g_depth && (e = cudaMemsetAsync(g_depth, 0, plane, stream)) != cudaSuccess) return cuda_fail("memset g_depth", e);
-    if (n == 0 || (!g_points && !g_image && !g_acc && !g_depth)) return 0;
-    srf::PointFeatsArgs a;
-    memset(&a, 0, sizeof(a));
-    a.V = V; a.n = n; a.H = H; a.W = W;
-    a.points = points; a.w2cs = w2cs; a.ixts = ixts; a.img_ref = img_ref; a.image = image; a.acc = acc; a.depth = depth;
-    a.g_feats = g_feats; a.g_points = g_points; a.g_image = g_image; a.g_acc = g_acc; a.g_depth = g_depth;
-    e = srf::launch_point_feats(a, true, stream);
-    if (e != cudaSuccess) return cuda_fail("point_feats_bwd launch", e);
-    return 0;
-}
-
-// header (max |g_feats|, overflow flag), then the int64 planes g_image | g_acc | g_depth
-static size_t pf_det_planes_offset() { return 256; }
-
-int srf_point_feats_deterministic_workspace_bytes(int V, int H, int W, size_t* bytes) {
-    if (V <= 0 || H <= 0 || W <= 0 || !bytes) return fail("srf_point_feats_deterministic_workspace_bytes: bad arguments");
-    *bytes = pf_det_planes_offset() + 5 * (size_t)V * H * W * sizeof(long long);
-    return 0;
-}
-
-int srf_point_feats_backward_deterministic(srf_stream_t stream_, int V, int n, int H, int W,
-                                           const float* points, const float* w2cs, const float* ixts,
-                                           const float* img_ref, const float* image, const float* acc, const float* depth,
-                                           const float* g_feats, float* g_points, float* g_image, float* g_acc,
-                                           float* g_depth, void* workspace) {
-    const char* fn = "srf_point_feats_backward_deterministic";
-    if (point_feats_check(fn, V, n, H, W, points, w2cs, ixts, img_ref, image, acc, depth)) return 1;
-    if (n > 0 && !g_feats) return fail("%s: null upstream gradient", fn);
-    if (!workspace || misaligned(workspace)) return fail("%s: workspace must be 256-byte aligned", fn);
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    const size_t plane = (size_t)V * H * W * sizeof(float);
-    cudaError_t e = cudaSuccess;
-    if (n == 0 || (!g_points && !g_image && !g_acc && !g_depth)) {       // nothing to sum: cleared outputs, as the default
+    const bool nothing = n == 0 || (!g_points && !g_image && !g_acc && !g_depth);
+    // the default path adds into cleared outputs; the deterministic one writes them from its fixed-point planes
+    if (!workspace || nothing) {
+        const size_t plane = (size_t)V * H * W * sizeof(float);
+        cudaError_t e = cudaSuccess;
         if (g_image && (e = cudaMemsetAsync(g_image, 0, 3 * plane, stream)) != cudaSuccess) return cuda_fail("memset g_image", e);
         if (g_acc && (e = cudaMemsetAsync(g_acc, 0, plane, stream)) != cudaSuccess) return cuda_fail("memset g_acc", e);
         if (g_depth && (e = cudaMemsetAsync(g_depth, 0, plane, stream)) != cudaSuccess) return cuda_fail("memset g_depth", e);
-        return 0;
     }
-    e = cudaMemsetAsync(workspace, 0, pf_det_planes_offset() + 5 * (size_t)V * H * W * sizeof(long long), stream);
-    if (e != cudaSuccess) return cuda_fail("memset point_feats workspace", e);
+    if (nothing) return 0;
     srf::PointFeatsArgs a;
     memset(&a, 0, sizeof(a));
     a.V = V; a.n = n; a.H = H; a.W = W;
     a.points = points; a.w2cs = w2cs; a.ixts = ixts; a.img_ref = img_ref; a.image = image; a.acc = acc; a.depth = depth;
     a.g_feats = g_feats; a.g_points = g_points; a.g_image = g_image; a.g_acc = g_acc; a.g_depth = g_depth;
-    a.det = static_cast<uint32_t*>(workspace);
-    a.g_fixed = at<long long>(workspace, pf_det_planes_offset());
-    e = srf::launch_point_feats(a, true, stream);
+    if (workspace) {
+        cudaError_t e = cudaMemsetAsync(workspace, 0, pf_det_workspace_bytes(V, H, W), stream);
+        if (e != cudaSuccess) return cuda_fail("memset point_feats workspace", e);
+        a.det = static_cast<uint32_t*>(workspace);
+        a.g_fixed = at<long long>(workspace, pf_det_planes_offset());
+    }
+    cudaError_t e = srf::launch_point_feats(a, true, stream);
     if (e != cudaSuccess) return cuda_fail("point_feats_bwd launch", e);
-    return check_overflow_flag(fn, a.det + 1, stream);
+    return workspace ? check_overflow_flag(fn, a.det + 1, stream) : 0;
+}
+
+int srf_point_feats_deterministic_workspace_bytes(int V, int H, int W, size_t* bytes) {
+    if (V <= 0 || H <= 0 || W <= 0 || !bytes) return fail("srf_point_feats_deterministic_workspace_bytes: bad arguments");
+    *bytes = pf_det_workspace_bytes(V, H, W);
+    return 0;
 }
 
 static int ms_ssim_sizes(const char* fn, int B, int C, int H, int W) {

@@ -17,7 +17,7 @@ from typing import Tuple
 import torch
 
 from . import _lib
-from .rasterizer import _DeviceGuard, _raw_stream
+from .rasterizer import _contig, _DeviceGuard, _ptr, _raw_stream
 
 
 class _DecoderLayout(torch.autograd.Function):
@@ -60,15 +60,13 @@ class _DecoderLayout(torch.autograd.Function):
         B, N, K, sh_dim, half_cell = ctx.meta
         dev = params.device
 
-        def c(t):
-            return None if t is None else t.contiguous()
-        g_centers, g_shs, g_scaling, g_rotation, g_opacity = c(g_centers), c(g_shs), c(g_scaling), c(g_rotation), c(g_opacity)
+        g_centers, g_shs, g_scaling, g_rotation, g_opacity = map(
+            _contig, (g_centers, g_shs, g_scaling, g_rotation, g_opacity))
         g_params = torch.empty_like(params)
-        p = lambda t: 0 if t is None else t.data_ptr()      # noqa: E731
         with _DeviceGuard(dev):
             _lib.check(lib.srf_decoder_layout_backward(
-                _raw_stream(dev), B, N, K, sh_dim, half_cell, params.data_ptr(), p(g_centers), p(g_shs), p(g_opacity),
-                p(g_scaling), p(g_rotation), g_params.data_ptr()), lib)
+                _raw_stream(dev), B, N, K, sh_dim, half_cell, params.data_ptr(), _ptr(g_centers), _ptr(g_shs),
+                _ptr(g_opacity), _ptr(g_scaling), _ptr(g_rotation), g_params.data_ptr()), lib)
         return g_params, None, None, None, None, None, None
 
 

@@ -22,15 +22,7 @@ from typing import Dict, Optional
 import torch
 
 from . import _lib
-from .rasterizer import _DeviceGuard, _raw_stream
-
-
-def _p(t: Optional[torch.Tensor]) -> int:
-    return 0 if t is None else t.data_ptr()
-
-
-def _c(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
-    return None if t is None else t.contiguous()
+from .rasterizer import _contig, _DeviceGuard, _ptr, _raw_stream
 
 
 def epilogue_views_forward_raw(color, allmap, rays, cams, depth_ratio, image, depth, acc, rn, dn, dist):
@@ -43,7 +35,7 @@ def epilogue_views_forward_raw(color, allmap, rays, cams, depth_ratio, image, de
     dev = color.device
     with _DeviceGuard(dev):
         _lib.check(lib.srf_views_epilogue_forward(
-            _raw_stream(dev), V, H, W, float(depth_ratio), color.data_ptr(), allmap.data_ptr(), _p(rays),
+            _raw_stream(dev), V, H, W, float(depth_ratio), color.data_ptr(), allmap.data_ptr(), _ptr(rays),
             cams.data_ptr(), image.data_ptr(), depth.data_ptr(), acc.data_ptr(), rn.data_ptr(),
             dn.data_ptr(), dist.data_ptr()), lib)
 
@@ -58,8 +50,8 @@ def epilogue_views_backward_raw(color, allmap, rays, cams, depth_ratio, gi, gd, 
     d_allmap = torch.empty((V, 8, H, W), dtype=torch.float32, device=dev)
     with _DeviceGuard(dev):
         _lib.check(lib.srf_views_epilogue_backward(
-            _raw_stream(dev), V, H, W, float(depth_ratio), color.data_ptr(), allmap.data_ptr(), _p(rays),
-            cams.data_ptr(), _p(gi), _p(gd), _p(ga), _p(grn), _p(gdn), _p(gds),
+            _raw_stream(dev), V, H, W, float(depth_ratio), color.data_ptr(), allmap.data_ptr(), _ptr(rays),
+            cams.data_ptr(), _ptr(gi), _ptr(gd), _ptr(ga), _ptr(grn), _ptr(gdn), _ptr(gds),
             scratch.data_ptr(), d_color.data_ptr(), d_allmap.data_ptr()), lib)
     return d_color, d_allmap
 
@@ -122,8 +114,9 @@ class _Epilogue(torch.autograd.Function):
     def backward(ctx, g_image, g_depth, g_acc, g_rn, g_dn, g_dist):
         color, allmap, rays, viewmatrix = ctx.saved_tensors
         rays = rays if ctx.has_rays else None
-        d_color, d_allmap = epilogue_backward_raw(color, allmap, rays, viewmatrix, ctx.depth_ratio, _c(g_image), _c(g_depth),
-                                                  _c(g_acc), _c(g_rn), _c(g_dn), _c(g_dist))
+        d_color, d_allmap = epilogue_backward_raw(color, allmap, rays, viewmatrix, ctx.depth_ratio, _contig(g_image),
+                                                  _contig(g_depth), _contig(g_acc), _contig(g_rn), _contig(g_dn),
+                                                  _contig(g_dist))
         return d_color, d_allmap, None, None, None
 
 

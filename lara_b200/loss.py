@@ -18,7 +18,7 @@ from typing import Callable, Dict, Optional, Tuple
 import torch
 
 from . import _lib
-from .rasterizer import _DeviceGuard, _raw_stream
+from .rasterizer import _DeviceGuard, _ptr, _raw_stream
 from .ssim import ms_ssim_views
 
 
@@ -43,15 +43,13 @@ class _SceneLoss(torch.autograd.Function):
         if tuple(target.shape) != (V, H, W, 3):
             raise RuntimeError(f"scene_loss: tar_rgb must be [V,H,W,3] = {(V, H, W, 3)}, got {tuple(target.shape)}")
         sums = torch.empty(3, dtype=torch.float64, device=dev)
-        p = lambda t: 0 if t is None else t.data_ptr()      # noqa: E731
-        args = (_raw_stream(dev), V, H, W, 1 if with_reg else 0, image.data_ptr(), target.data_ptr(),
-                p(rend_normal), p(depth_normal), p(acc_map), p(rend_dist), sums.data_ptr())
         with _DeviceGuard(dev):
-            if _lib.deterministic():         # partial sums reduced in a fixed order instead of atomics
-                ws = torch.empty(_lib.det_loss_workspace_bytes(lib, V, H, W) // 8, dtype=torch.float64, device=dev)
-                _lib.check(lib.srf_loss_forward_deterministic(*args, ws.data_ptr()), lib)
-            else:
-                _lib.check(lib.srf_loss_forward(*args), lib)
+            # partial sums reduced in a fixed order instead of atomics
+            ws = (torch.empty(_lib.det_loss_workspace_bytes(lib, V, H, W) // 8, dtype=torch.float64, device=dev)
+                  if _lib.deterministic() else None)
+            _lib.check(lib.srf_loss_forward(
+                _raw_stream(dev), V, H, W, 1 if with_reg else 0, image.data_ptr(), target.data_ptr(), _ptr(rend_normal),
+                _ptr(depth_normal), _ptr(acc_map), _ptr(rend_dist), sums.data_ptr(), _ptr(ws)), lib)
         npx = float(batch_scenes) * V * H * W
         mse = sums[0] / (3.0 * npx)
         dist = sums[1] / npx
@@ -75,12 +73,12 @@ class _SceneLoss(torch.autograd.Function):
             g_dist = torch.empty((V, H, W), dtype=torch.float32, device=dev)
         else:
             g_rn = g_dn = g_dist = None
-        p = lambda t: 0 if t is None else t.data_ptr()      # noqa: E731
         with _DeviceGuard(dev):
             _lib.check(lib.srf_loss_backward(
                 _raw_stream(dev), V, H, W, 1 if ctx.with_reg else 0, 1.0 / (3.0 * ctx.npx), 1000.0 / ctx.npx, 0.2 / ctx.npx,
-                image.data_ptr(), target.data_ptr(), p(rn if ctx.with_reg else None), p(dn if ctx.with_reg else None),
-                p(acc if ctx.with_reg else None), up.data_ptr(), g_image.data_ptr(), p(g_rn), p(g_dn), p(g_dist)), lib)
+                image.data_ptr(), target.data_ptr(), _ptr(rn if ctx.with_reg else None),
+                _ptr(dn if ctx.with_reg else None), _ptr(acc if ctx.with_reg else None), up.data_ptr(),
+                g_image.data_ptr(), _ptr(g_rn), _ptr(g_dn), _ptr(g_dist)), lib)
         return g_image, g_rn, g_dn, g_dist, None, None, None, None
 
 

@@ -88,9 +88,8 @@ class _RenderSceneViews(torch.autograd.Function):
         centers, shs, scales, rot, rays, cams, color, allmap, radii, _geom, _tile, _image = ctx.saved_tensors
         H, W, tfx, tfy, deg, debug = ctx.geometry
 
-        def c(t):
-            return None if t is None else t.contiguous()
         if ctx.has_rays:
+            c = R._contig
             d_color, d_allmap = epilogue_views_backward_raw(
                 color, allmap, rays, cams, ctx.depth_ratio, c(g_image), c(g_depth), c(g_acc), c(g_rn), c(g_dn), c(g_dist))
         else:

@@ -27,11 +27,7 @@ from typing import Dict
 import torch
 
 from . import _lib
-from .rasterizer import _DeviceGuard, _raw_stream
-
-
-def _p(t) -> int:
-    return 0 if t is None else t.data_ptr()
+from .rasterizer import _DeviceGuard, _ptr, _raw_stream
 
 
 _NAMES = ("points", "img_ref", "renderings['image']", "renderings['acc_map']", "renderings['depth']", "src_w2cs",
@@ -103,15 +99,12 @@ class _PointFeats(torch.autograd.Function):
             new(need[4], V, 1, H, W)
         g_feats = g_feats.contiguous()
         with _DeviceGuard(dev):
-            if _lib.deterministic():
-                ws = torch.empty(_lib.det_point_feats_workspace_bytes(lib, V, H, W), dtype=torch.uint8, device=dev)
-                _lib.check(lib.srf_point_feats_backward_deterministic(
-                    _raw_stream(dev), V, n, H, W, *[t.data_ptr() for t in ins], g_feats.data_ptr(), _p(g_points),
-                    _p(g_image), _p(g_acc), _p(g_depth), ws.data_ptr()), lib)
-            else:
-                _lib.check(lib.srf_point_feats_backward(_raw_stream(dev), V, n, H, W, *[t.data_ptr() for t in ins],
-                                                        g_feats.data_ptr(), _p(g_points), _p(g_image), _p(g_acc),
-                                                        _p(g_depth)), lib)
+            # fixed-point sums in a workspace instead of atomics
+            ws = (torch.empty(_lib.det_point_feats_workspace_bytes(lib, V, H, W), dtype=torch.uint8, device=dev)
+                  if _lib.deterministic() else None)
+            _lib.check(lib.srf_point_feats_backward(_raw_stream(dev), V, n, H, W, *[t.data_ptr() for t in ins],
+                                                    g_feats.data_ptr(), _ptr(g_points), _ptr(g_image), _ptr(g_acc),
+                                                    _ptr(g_depth), _ptr(ws)), lib)
         return g_points, None, g_image, g_acc, g_depth, None, None
 
 

@@ -57,6 +57,10 @@ def _ptr(t: Optional[torch.Tensor]) -> int:
     return 0 if t is None else t.data_ptr()
 
 
+def _contig(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
+    return None if t is None else t.contiguous()
+
+
 def _opt(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
     """The reference passes empty tensors for "not given"; normalise to None."""
     if t is None or t.numel() == 0:
@@ -452,11 +456,10 @@ def backward_views_raw(state: ForwardState, radii, means3D, shs, colors_precomp,
         if P == 0:
             return g
         state.resolve()                 # capacity verified (re-run if it overflowed) before the lists are walked again
-        if _lib.deterministic(deterministic):
-            fn, scratch_b = lib.srf_views_backward_deterministic, _lib.det_backward_scratch_bytes(lib, V, P)
-        else:
-            fn, scratch_b = lib.srf_views_backward, _views_sizes(lib, V, P, H, W, state.capacity)[5]
-        _lib.check(fn(
+        det = _lib.deterministic(deterministic)
+        scratch_b = (_lib.det_backward_scratch_bytes(lib, V, P) if det
+                     else _views_sizes(lib, V, P, H, W, state.capacity)[5])
+        _lib.check(lib.srf_views_backward(
             _raw_stream(device), V, P, int(sh_degree), M, H, W, state.capacity, cams.data_ptr(),
             _ptr(means3D), _ptr(shs), 1 if colors_precomp is not None else 0,
             _ptr(scales), _ptr(rotations), 1 if transMat_precomp is not None else 0,
@@ -465,7 +468,7 @@ def backward_views_raw(state: ForwardState, radii, means3D, shs, colors_precomp,
             grad_color.data_ptr(), grad_allmap.data_ptr(), _blob(scratch_b, device).data_ptr(), 1 if accumulate else 0,
             _ptr(g["means3D"]), _ptr(g["means2D"]), _ptr(g["sh"]), _ptr(g["colors_precomp"]),
             _ptr(g["opacities"]), _ptr(g["scales"]), _ptr(g["rotations"]), _ptr(g["cov3Ds_precomp"]),
-            1 if raw_activations else 0), lib)
+            1 if raw_activations else 0, 1 if det else 0), lib)
         if debug:
             torch.cuda.synchronize(device)
         return g
@@ -641,9 +644,9 @@ class GaussianRasterizer(nn.Module):
             P = int(pos.shape[0])
             present = torch.zeros((P,), dtype=torch.bool, device=pos.device)
             if P:
-                with torch.cuda.device(pos.device):
+                with _DeviceGuard(pos.device):
                     _lib.check(lib.srf_mark_visible(
-                        torch.cuda.current_stream(pos.device).cuda_stream, P, pos.data_ptr(),
+                        _raw_stream(pos.device), P, pos.data_ptr(),
                         rs.viewmatrix.data_ptr(), rs.projmatrix.data_ptr(), present.data_ptr()), lib)
         return present
 

@@ -63,9 +63,7 @@ class _MsSsim(torch.autograd.Function):
         if not X.is_cuda or Y.device != dev:
             raise RuntimeError(f"MS_SSIM: X and Y must be CUDA tensors on one device, got {X.device} and {Y.device}")
         B, C, H, W = _logical_shape(X, views)
-        nbytes = ctypes.c_size_t()
-        _lib.check(lib.srf_ms_ssim_workspace_bytes(B, C, H, W, ctypes.byref(nbytes)), lib)
-        ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+        ws = torch.empty(_lib._size_query(lib.srf_ms_ssim_workspace_bytes, B, C, H, W), dtype=torch.uint8, device=dev)
         out = torch.empty(() if size_average else (B,), dtype=torch.float32, device=dev)
         ax, ay = _addr(X, views), _addr(Y, views)
         with _DeviceGuard(dev):

@@ -177,15 +177,17 @@ def test_scratch_queries(lib):
     assert lib.srf_loss_deterministic_workspace_bytes(1, 4, -1, ctypes.byref(n)) != 0
 
 
-def test_bad_arguments_rejected_before_any_launch(lib):
-    # null cameras / workspace: status and message, no CUDA call
+def test_bad_arguments_and_misaligned_workspaces_rejected_before_any_launch(lib):
+    # null cameras / null input / misaligned workspace: status and message, no CUDA call
     args = [None, 1, 10, 0, 1, 16, 16, 0, None, None, None, 0, None, None, 0, 1.0, 1.0, None, None, None, None, None,
-            None, None, None, 0, None, None, None, None, None, None, None, None, 0]
-    assert lib.srf_views_backward_deterministic(*args) != 0
-    assert b"srf_views_backward_deterministic" in lib.srf_last_error()
-    assert lib.srf_loss_forward_deterministic(None, 1, 8, 8, 0, 1, 1, None, None, None, None, 1, None) != 0
-    assert lib.srf_point_feats_backward_deterministic(None, 1, 0, 8, 8, None, 1, 1, 1, 1, 1, 1, None, None, None,
-                                                      None, None, None) != 0
+            None, None, None, 0, None, None, None, None, None, None, None, None, 0, 1]
+    assert lib.srf_views_backward(*args) != 0
+    assert b"srf_views_backward" in lib.srf_last_error()
+    assert lib.srf_loss_forward(None, 1, 8, 8, 0, None, 1, None, None, None, None, 1, None) != 0
+    assert b"null pointer" in lib.srf_last_error()
+    assert lib.srf_loss_forward(None, 1, 8, 8, 0, 1, 1, None, None, None, None, 1, 1) != 0
+    assert b"workspace" in lib.srf_last_error()
+    assert lib.srf_point_feats_backward(None, 1, 0, 8, 8, None, 1, 1, 1, 1, 1, 1, None, None, None, None, None, 1) != 0
     assert b"workspace" in lib.srf_last_error()
 
 

@@ -165,28 +165,31 @@ def test_sample_point_feats_rejects_dtype_device_and_constants_requiring_grad():
             sample_point_feats(points, consts[0], rend, consts[1], consts[2])
 
 
-def test_point_feats_c_entries_reject_bad_arguments(lib):
+def test_point_feats_c_entries_reject_bad_arguments_before_any_launch(lib):
     P = ctypes.c_void_p(256)           # never dereferenced: the checks come before any CUDA call
     ins = [P] * 7
     for V, n, H, W in ((0, 4, 8, 8), (1, -1, 8, 8), (1, 4, 0, 8), (1, 4, 8, 0)):
         assert lib.srf_point_feats_forward(None, V, n, H, W, *ins, P) != 0
         assert b"srf_point_feats_forward: bad sizes" in lib.srf_last_error()
-        assert lib.srf_point_feats_backward(None, V, n, H, W, *ins, P, P, P, P, P) != 0
+        assert lib.srf_point_feats_backward(None, V, n, H, W, *ins, P, P, P, P, P, None) != 0
         assert b"srf_point_feats_backward: bad sizes" in lib.srf_last_error()
     for k in range(7):
         nulled = list(ins)
         nulled[k] = None
         assert lib.srf_point_feats_forward(None, 1, 4, 8, 8, *nulled, P) != 0
         assert b"null input pointer" in lib.srf_last_error()
-        assert lib.srf_point_feats_backward(None, 1, 4, 8, 8, *nulled, P, None, None, None, None) != 0
+        assert lib.srf_point_feats_backward(None, 1, 4, 8, 8, *nulled, P, None, None, None, None, None) != 0
         assert b"null input pointer" in lib.srf_last_error()
     assert lib.srf_point_feats_forward(None, 1, 4, 8, 8, *ins, None) != 0
     assert b"null output pointer" in lib.srf_last_error()
-    assert lib.srf_point_feats_backward(None, 1, 4, 8, 8, *ins, None, P, P, P, P) != 0
+    assert lib.srf_point_feats_backward(None, 1, 4, 8, 8, *ins, None, P, P, P, P, None) != 0
     assert b"null upstream gradient" in lib.srf_last_error()
+    # a deterministic workspace must be 256-byte aligned
+    assert lib.srf_point_feats_backward(None, 1, 4, 8, 8, *ins, P, P, P, P, P, 8) != 0
+    assert b"workspace must be 256-byte aligned" in lib.srf_last_error()
     # n == 0: nothing to read or write, so the empty point set's pointers may be NULL
     assert lib.srf_point_feats_forward(None, 1, 0, 8, 8, None, *ins[1:], None) == 0
-    assert lib.srf_point_feats_backward(None, 1, 0, 8, 8, None, *ins[1:], None, None, None, None, None) == 0
+    assert lib.srf_point_feats_backward(None, 1, 0, 8, 8, None, *ins[1:], None, None, None, None, None, None) == 0
 
 
 # ---- GPU: kernel vs restatement ----------------------------------------------------------------------------------
