@@ -8,6 +8,9 @@
  *     rasterize_gaussians_backward   -> srf_views_backward  (V = 1)
  *     mark_visible                   -> srf_mark_visible
  *
+ * A render no gradient flows through (no_grad / inference_mode) calls srf_views_forward_inference instead:
+ * the same outputs, bit for bit, without the state the backward needs (see "forward-only" below).
+ *
  * which in turn call CudaRasterizer::Rasterizer::{forward,backward,markVisible}
  * (DSR/cuda_rasterizer/rasterizer.h:24-86) with raw pointers.  This header is the
  * raw-pointer level: plain C, device pointers + sizes + a cudaStream_t, int status
@@ -32,7 +35,7 @@
 extern "C" {
 #endif
 
-#define SRF_ABI_VERSION 10
+#define SRF_ABI_VERSION 11
 
 /* cudaStream_t without pulling in cuda_runtime.h */
 typedef void* srf_stream_t;
@@ -112,6 +115,31 @@ int srf_views_forward_render(srf_stream_t stream, int V, int P, int image_height
                              size_t capacity, const void* geom_state, void* tile_state,
                              void* entries, uint32_t* point_list, void* image_state,
                              const float* cams, float* out_color, float* out_others);
+
+/* ---- forward-only --------------------------------------------------------------------
+ * The forward of a render that no backward will follow: same arguments, same stages, same deferred counts and
+ * bit-identical out_color / out_others / radii as srf_views_forward, but the blend keeps no contribution record and
+ * writes no per-pixel image state, so `point_list` holds only the sorted list and `image_state` is not used (may be
+ * NULL).  Size the workspaces with srf_views_inference_workspace_bytes:
+ *   bytes[0..4] = geom, tile, image (0: not needed), entries, point_list (4 B per instance of capacity,
+ *   rounded up to 256 B, per view) -- totals for V views, as srf_views_workspace_bytes.
+ * The state it leaves cannot feed srf_views_backward.  Null or misaligned workspaces are rejected before anything
+ * is enqueued; the other argument checks and their messages are those of srf_views_forward.
+ * srf_views_forward_inference_render is the stage-2 re-run for an overflowed capacity (as
+ * srf_views_forward_render).                                                                                      */
+int srf_views_inference_workspace_bytes(int V, int P, int H, int W, size_t capacity, size_t bytes[5]);
+int srf_views_forward_inference(srf_stream_t stream, int V, int P, int D, int M,
+                                const float* means3D, const float* shs, const float* colors_precomp,
+                                const float* opacities, const float* scales, const float* rotations,
+                                const float* transMat_precomp, const float* cams,
+                                float tan_fovx, float tan_fovy, int image_height, int image_width, int prefiltered,
+                                size_t capacity, int* radii, void* geom_state, void* tile_state, void* entries,
+                                uint32_t* point_list, void* image_state, float* out_color, float* out_others,
+                                uint32_t* num_rendered_host, void* count_event, int raw_activations);
+int srf_views_forward_inference_render(srf_stream_t stream, int V, int P, int image_height, int image_width,
+                                       size_t capacity, const void* geom_state, void* tile_state,
+                                       void* entries, uint32_t* point_list, void* image_state,
+                                       const float* cams, float* out_color, float* out_others);
 
 /* ---- backward ------------------------------------------------------------------
  * Replaces Rasterizer::backward (rasterizer_impl.cu:346-448): BACKWARD::render,
@@ -266,6 +294,7 @@ int srf_ms_ssim_backward(srf_stream_t stream, int B, int C, int H, int W,
  * them and returns, per kernel id, the summed device time in ms and the launch count.
  * Kernel ids: 0 preprocess_fwd, 1 tile_scan, 2 scatter, 3 sort_small, 4 sort_big,
  * 5 render_fwd, 6 render_bwd, 7 preprocess_bwd (SRF_NUM_KERNELS entries).  Not thread-safe.
+ * The forward-only blend counts as render_fwd.
  * The deterministic backward runs the blend backward twice: two render_bwd launches per call.            */
 #define SRF_NUM_KERNELS 8
 int srf_profile_begin(void);

@@ -85,6 +85,8 @@ size_t plist_masks_offset(size_t capacity) { return align_up(capacity * sizeof(u
 size_t plist_stride_bytes(size_t capacity) {
     return plist_masks_offset(capacity) + align_up(capacity * 8 * sizeof(uint32_t)) + 256;
 }
+// The forward-only entries' point_list workspace: the list alone.
+size_t inference_plist_stride_bytes(size_t capacity) { return align_up(capacity * sizeof(uint32_t)); }
 size_t entries_stride_bytes(size_t capacity) { return align_up(capacity * sizeof(uint64_t)) + 256; }
 size_t ggrad_stride_bytes(int P) { return align_up((size_t)P * SRF_GRAD_FLOATS * sizeof(float)) + 256; }
 
@@ -182,6 +184,16 @@ int srf_views_workspace_bytes(int V, int P, int H, int W, size_t capacity, size_
     return 0;
 }
 
+int srf_views_inference_workspace_bytes(int V, int P, int H, int W, size_t capacity, size_t bytes[5]) {
+    if (V <= 0 || P < 0 || H <= 0 || W <= 0 || !bytes) return fail("srf_views_inference_workspace_bytes: bad arguments");
+    bytes[0] = geom_layout(P).total * (size_t)V;
+    bytes[1] = tile_layout(H, W).total * (size_t)V;
+    bytes[2] = 0;
+    bytes[3] = entries_stride_bytes(capacity) * (size_t)V;
+    bytes[4] = inference_plist_stride_bytes(capacity) * (size_t)V;
+    return 0;
+}
+
 int srf_state_layout(int P, int H, int W, size_t geom_off[3], size_t tile_off[5], size_t image_off[2]) {
     if (P < 0 || H <= 0 || W <= 0) return fail("srf_state_layout: bad arguments");
     const GeomLayout g = geom_layout(P);
@@ -223,27 +235,16 @@ void fill_bin_args(srf::BinArgs& b, int V, int P, const TileLayout& tl, void* ti
     b.tile_stride = tl.total;
 }
 
-// stage 1: preprocess, per-tile counting, tile scan and the count read-back
-int forward_preprocess_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int M,
-                            const float* means3D, const float* shs, const float* colors_precomp,
-                            const float* opacities, const float* scales, const float* rotations,
-                            const float* transMat_precomp, const float* cams,
-                            float tan_fovx, float tan_fovy, int image_height, int image_width,
-                            int prefiltered, int* radii, void* geom_state, void* tile_state,
-                            uint32_t* num_rendered_host, int raw_activations) {
+// argument checks of stage 1, all made before it enqueues anything
+int forward_preprocess_check(const char* fn, int V, int P, int D, int M,
+                             const float* means3D, const float* shs, const float* colors_precomp,
+                             const float* opacities, const float* scales, const float* rotations,
+                             const float* transMat_precomp, int image_height, int image_width,
+                             const int* radii, const void* geom_state, const void* tile_state) {
     if (V <= 0 || P < 0 || image_height <= 0 || image_width <= 0) return fail("%s: bad sizes", fn);
     if (image_height > 16 * 65535 || image_width > 16 * 65535) return fail("%s: image too large", fn);
     if (!tile_state || misaligned(tile_state)) return fail("%s: tile_state must be 256-byte aligned", fn);
     if (D < 0 || D > 3) return fail("%s: sh degree must be in [0,3]", fn);
-    const TileLayout tl = tile_layout(image_height, image_width);
-    // tile blocks + counters of every view are zeroed by one 2-D memset
-    cudaError_t e = cudaMemset2DAsync(at<char>(tile_state, tl.count), tl.total, 0,
-                                      tl.counters + 4 * sizeof(uint32_t) - tl.count, (size_t)V, stream);
-    if (e != cudaSuccess) return cuda_fail("memset tile counters", e);
-
-    srf::BinArgs b;
-    fill_bin_args(b, V, P, tl, tile_state);
-
     if (P > 0) {
         if (!means3D || !opacities || !radii) return fail("%s: null required pointer", fn);
         if ((shs == nullptr) == (colors_precomp == nullptr))
@@ -255,6 +256,31 @@ int forward_preprocess_impl(const char* fn, cudaStream_t stream, int V, int P, i
         if (!geom_state || misaligned(geom_state)) return fail("%s: geom_state must be 256-byte aligned", fn);
         if ((reinterpret_cast<uintptr_t>(rotations) & 15) || (reinterpret_cast<uintptr_t>(scales) & 7))
             return fail("%s: rotations must be 16-byte and scales 8-byte aligned", fn);
+    }
+    return 0;
+}
+
+// stage 1: preprocess, per-tile counting, tile scan and the count read-back
+int forward_preprocess_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int M,
+                            const float* means3D, const float* shs, const float* colors_precomp,
+                            const float* opacities, const float* scales, const float* rotations,
+                            const float* transMat_precomp, const float* cams,
+                            float tan_fovx, float tan_fovy, int image_height, int image_width,
+                            int prefiltered, int* radii, void* geom_state, void* tile_state,
+                            uint32_t* num_rendered_host, int raw_activations) {
+    if (forward_preprocess_check(fn, V, P, D, M, means3D, shs, colors_precomp, opacities, scales, rotations,
+                                 transMat_precomp, image_height, image_width, radii, geom_state, tile_state))
+        return 1;
+    const TileLayout tl = tile_layout(image_height, image_width);
+    // tile blocks + counters of every view are zeroed by one 2-D memset
+    cudaError_t e = cudaMemset2DAsync(at<char>(tile_state, tl.count), tl.total, 0,
+                                      tl.counters + 4 * sizeof(uint32_t) - tl.count, (size_t)V, stream);
+    if (e != cudaSuccess) return cuda_fail("memset tile counters", e);
+
+    srf::BinArgs b;
+    fill_bin_args(b, V, P, tl, tile_state);
+
+    if (P > 0) {
         const GeomLayout gl = geom_layout(P);
         srf::PreprocessArgs a;
         memset(&a, 0, sizeof(a));
@@ -301,15 +327,33 @@ int forward_preprocess_impl(const char* fn, cudaStream_t stream, int V, int P, i
     return 0;
 }
 
-// stage 2: scatter into tile buckets, per-tile depth sort, blend
+// argument checks of stage 2; `record` = false (forward-only) needs no image_state
+int forward_render_check(const char* fn, int V, int P, int image_height, int image_width, size_t capacity,
+                         const void* geom_state, const void* tile_state, const void* entries, const uint32_t* point_list,
+                         const void* image_state, const float* cams, const float* out_color, const float* out_others, bool record) {
+    if (V <= 0 || P < 0 || image_height <= 0 || image_width <= 0) return fail("%s: bad sizes", fn);
+    if (!cams || !tile_state || (record && !image_state) || !out_color || !out_others)
+        return fail("%s: null required pointer", fn);
+    if (capacity > 0xfffffff0ull) return fail("%s: capacity exceeds 32-bit instance indices", fn);
+    if (capacity > 0 && (!entries || !point_list)) return fail("%s: null binning buffers", fn);
+    if (!record) {
+        if (P > 0 && (!geom_state || misaligned(geom_state))) return fail("%s: geom_state must be 256-byte aligned", fn);
+        if (misaligned(tile_state)) return fail("%s: tile_state must be 256-byte aligned", fn);
+        if (capacity > 0 && (misaligned(entries) || misaligned(point_list)))
+            return fail("%s: entries and point_list must be 256-byte aligned", fn);
+    }
+    return 0;
+}
+
+// stage 2: scatter into tile buckets, per-tile depth sort, blend (record = false: the forward-only blend, no
+// contribution record and no image state)
 int forward_render_impl(const char* fn, cudaStream_t stream, int V, int P, int image_height, int image_width,
                         size_t capacity, const void* geom_state, void* tile_state,
                         void* entries, uint32_t* point_list, void* image_state,
-                        const float* cams, float* out_color, float* out_others) {
-    if (V <= 0 || P < 0 || image_height <= 0 || image_width <= 0) return fail("%s: bad sizes", fn);
-    if (!cams || !tile_state || !image_state || !out_color || !out_others) return fail("%s: null required pointer", fn);
-    if (capacity > 0xfffffff0ull) return fail("%s: capacity exceeds 32-bit instance indices", fn);
-    if (capacity > 0 && (!entries || !point_list)) return fail("%s: null binning buffers", fn);
+                        const float* cams, float* out_color, float* out_others, bool record) {
+    if (forward_render_check(fn, V, P, image_height, image_width, capacity, geom_state, tile_state, entries, point_list,
+                             image_state, cams, out_color, out_others, record))
+        return 1;
     const TileLayout tl = tile_layout(image_height, image_width);
     const ImageLayout il = image_layout(image_height, image_width);
     const GeomLayout gl = geom_layout(P);
@@ -321,7 +365,7 @@ int forward_render_impl(const char* fn, cudaStream_t stream, int V, int P, int i
     b.point_list = point_list;
     b.geom_stride = gl.total;
     b.entries_stride = entries_stride_bytes(capacity);
-    b.plist_stride = plist_stride_bytes(capacity);
+    b.plist_stride = record ? plist_stride_bytes(capacity) : inference_plist_stride_bytes(capacity);
     cudaError_t e;
     if (P > 0) {
         if (!geom_state) return fail("%s: null geom_state", fn);
@@ -338,16 +382,18 @@ int forward_render_impl(const char* fn, cudaStream_t stream, int V, int P, int i
     r.ranges = b.ranges;
     r.tile_order = b.tile_order;
     r.point_list = point_list;
-    r.masks = at<uint32_t>(point_list, plist_masks_offset(capacity));
+    r.masks = record ? at<uint32_t>(point_list, plist_masks_offset(capacity)) : nullptr;
     r.rec = P > 0 ? at<float4>(geom_state, gl.rec) : nullptr;
     r.bg = cams + SRF_CAM_BG;
     r.out_color = out_color; r.out_others = out_others;
-    r.accum = at<float>(image_state, il.accum);
-    r.n_contrib = at<uint32_t>(image_state, il.ncontrib);
+    if (record) {
+        r.accum = at<float>(image_state, il.accum);
+        r.n_contrib = at<uint32_t>(image_state, il.ncontrib);
+        r.image_stride = il.total;
+    }
     r.geom_stride = b.geom_stride; r.tile_stride = b.tile_stride; r.plist_stride = b.plist_stride;
-    r.image_stride = il.total;
     r.cam_stride = SRF_CAM_FLOATS;
-    e = srf::launch_render_fwd(r, stream);
+    e = srf::launch_render_fwd(r, record, stream);
     if (e != cudaSuccess) return cuda_fail("render_fwd launch", e);
     return 0;
 }
@@ -466,7 +512,7 @@ int srf_views_forward(srf_stream_t stream_, int V, int P, int D, int M,
         if (e != cudaSuccess) return cuda_fail("count event record", e);
     }
     return forward_render_impl(fn, stream, V, P, image_height, image_width, capacity, geom_state, tile_state, entries,
-                               point_list, image_state, cams, out_color, out_others);
+                               point_list, image_state, cams, out_color, out_others, true);
 }
 
 int srf_views_forward_render(srf_stream_t stream_, int V, int P, int image_height, int image_width,
@@ -475,7 +521,45 @@ int srf_views_forward_render(srf_stream_t stream_, int V, int P, int image_heigh
                              const float* cams, float* out_color, float* out_others) {
     return forward_render_impl("srf_views_forward_render", static_cast<cudaStream_t>(stream_), V, P, image_height,
                                image_width, capacity, geom_state, tile_state, entries, point_list, image_state,
-                               cams, out_color, out_others);
+                               cams, out_color, out_others, true);
+}
+
+int srf_views_forward_inference(srf_stream_t stream_, int V, int P, int D, int M,
+                                const float* means3D, const float* shs, const float* colors_precomp,
+                                const float* opacities, const float* scales, const float* rotations,
+                                const float* transMat_precomp, const float* cams,
+                                float tan_fovx, float tan_fovy, int image_height, int image_width, int prefiltered,
+                                size_t capacity, int* radii, void* geom_state, void* tile_state, void* entries,
+                                uint32_t* point_list, void* image_state, float* out_color, float* out_others,
+                                uint32_t* num_rendered_host, void* count_event, int raw_activations) {
+    const char* fn = "srf_views_forward_inference";
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    if (!cams) return fail("%s: null camera records", fn);
+    // the checks of both stages (in the order srf_views_forward makes them) before stage 1 enqueues anything
+    if (forward_preprocess_check(fn, V, P, D, M, means3D, shs, colors_precomp, opacities, scales, rotations,
+                                 transMat_precomp, image_height, image_width, radii, geom_state, tile_state) ||
+        forward_render_check(fn, V, P, image_height, image_width, capacity, geom_state, tile_state, entries, point_list,
+                             image_state, cams, out_color, out_others, false))
+        return 1;
+    int rc = forward_preprocess_impl(fn, stream, V, P, D, M, means3D, shs, colors_precomp, opacities, scales, rotations,
+                                     transMat_precomp, cams, tan_fovx, tan_fovy, image_height, image_width, prefiltered,
+                                     radii, geom_state, tile_state, num_rendered_host, raw_activations);
+    if (rc != 0) return rc;
+    if (count_event) {
+        cudaError_t e = cudaEventRecord(static_cast<cudaEvent_t>(count_event), stream);
+        if (e != cudaSuccess) return cuda_fail("count event record", e);
+    }
+    return forward_render_impl(fn, stream, V, P, image_height, image_width, capacity, geom_state, tile_state, entries,
+                               point_list, nullptr, cams, out_color, out_others, false);
+}
+
+int srf_views_forward_inference_render(srf_stream_t stream_, int V, int P, int image_height, int image_width,
+                                       size_t capacity, const void* geom_state, void* tile_state,
+                                       void* entries, uint32_t* point_list, void* image_state,
+                                       const float* cams, float* out_color, float* out_others) {
+    return forward_render_impl("srf_views_forward_inference_render", static_cast<cudaStream_t>(stream_), V, P,
+                               image_height, image_width, capacity, geom_state, tile_state, entries, point_list,
+                               image_state, cams, out_color, out_others, false);
 }
 
 int srf_views_backward(srf_stream_t stream_, int V, int P, int D, int M, int image_height, int image_width,

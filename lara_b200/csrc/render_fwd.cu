@@ -13,16 +13,22 @@
 // Every warp also records, per list position, which pixels of its block the splat was blended into (one u32
 // per (position, 8x4 block), RenderFwdArgs::masks): the blend backward replays that record instead of culling,
 // masking and re-testing the pairs itself.
+// The forward-only instantiation (kRecord = false, for renders no gradient flows through) keeps the hit masks, the walk,
+// eval_pair, the saturation test and the output stores, and drops everything that serves only the backward: the record
+// (s_out, its clearing, the transposes back and the stores, the lanes' blended-bit write-backs into s_mask) and the
+// accum / n_contrib image state.  Its outputs are bit-identical to the training instantiation's.
 #include "surfel_common.cuh"
 #include "surfel_kernels.h"
 
 namespace srf {
 
+template <bool kRecord>
 __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) render_fwd_kernel(RenderFwdArgs a) {
     __shared__ float4 s_rec[SRF_REC_QUADS][SRF_BATCH];
     __shared__ uint32_t s_mask[SRF_CTA_WARPS][SRF_BATCH_CHUNKS][32];   // [warp][group of 32 hits][lane]: per-pixel hit words
     __shared__ uint8_t s_list[SRF_CTA_WARPS][SRF_BATCH];               // [warp]: batch slots of the splats that can touch the warp's block
     __shared__ __align__(16) uint32_t s_out[SRF_CTA_WARPS][SRF_BATCH];  // [warp][batch slot]: contribution masks of the batch
+                                                                        // (not referenced, so not allocated, without kRecord)
 
     const int tid = threadIdx.x;
     {   // view of this CTA: per-view workspaces of identical layout, images stacked [V,C,H,W]
@@ -97,8 +103,10 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
         // "which of these 32 splats can touch MY pixel".  A splat outside a pixel's word cannot reach
         // alpha >= 1/255 there, so skipping it changes no result.
         static_assert(SRF_BATCH == 256, "s_out is cleared with two 16-byte stores per lane");
-        reinterpret_cast<uint4*>(s_out[wid])[lane] = make_uint4(0u, 0u, 0u, 0u);
-        reinterpret_cast<uint4*>(s_out[wid])[lane + 32] = make_uint4(0u, 0u, 0u, 0u);
+        if constexpr (kRecord) {
+            reinterpret_cast<uint4*>(s_out[wid])[lane] = make_uint4(0u, 0u, 0u, 0u);
+            reinterpret_cast<uint4*>(s_out[wid])[lane + 32] = make_uint4(0u, 0u, 0u, 0u);
+        }
         int nh = 0;
         for (int c0 = 0; c0 < cnt; c0 += 32) {
             const int jt = c0 + lane;
@@ -127,13 +135,17 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
         int c = 0;
         uint32_t w = 0, cw = 0;
         if (done) {
-            for (int k = 0; k < nchunks; ++k) sts_u32(sa_mask + 128u * k, 0u);
+            if constexpr (kRecord)
+                for (int k = 0; k < nchunks; ++k) sts_u32(sa_mask + 128u * k, 0u);
             c = nchunks;
         } else if (nchunks > 0) {
             w = lds_u32(sa_mask);
         }
         for (;;) {
-            while (w == 0 && c < nchunks - 1) { sts_u32(sa_mask + 128u * c, cw); cw = 0; ++c; w = lds_u32(sa_mask + 128u * c); }
+            while (w == 0 && c < nchunks - 1) {
+                if constexpr (kRecord) { sts_u32(sa_mask + 128u * c, cw); cw = 0; }
+                ++c; w = lds_u32(sa_mask + 128u * c);
+            }
             const bool active = (w != 0);
             if (!__any_sync(0xffffffffu, active)) break;
             if (!active) continue;
@@ -149,12 +161,14 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
             const float test_T = fmul_(T, fadd_(1.0f, -alpha));
             if (!(test_T >= 0.0001f)) {
                 done = true;
-                sts_u32(sa_mask + 128u * c, cw);
-                for (int k = c + 1; k < nchunks; ++k) sts_u32(sa_mask + 128u * k, 0u);
+                if constexpr (kRecord) {
+                    sts_u32(sa_mask + 128u * c, cw);
+                    for (int k = c + 1; k < nchunks; ++k) sts_u32(sa_mask + 128u * k, 0u);
+                }
                 w = 0; c = nchunks;
                 continue;
             }
-            cw |= 1u << i;
+            if constexpr (kRecord) cw |= 1u << i;
             const float4 q3 = lds_f4(sa_j + 48u * SRF_BATCH);
             const float4 q4 = lds_f4(sa_j + 64u * SRF_BATCH);
             const float depth = e.depth;
@@ -179,21 +193,24 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
             T = test_T;
             last_contributor = contributor;
         }
-        if (c < nchunks) sts_u32(sa_mask + 128u * c, cw);
-        __syncwarp();
+        // without the record, the next batch's __syncthreads_count orders the reuse of the warp's shared arrays
+        if constexpr (kRecord) {
+            if (c < nchunks) sts_u32(sa_mask + 128u * c, cw);
+            __syncwarp();
 
-        // ---- contribution record of the batch: transposed back, lane l holds the pixel mask of hit 32 k + l, which
-        // goes to its batch slot (the slots the cull dropped stay 0); then 32 consecutive list positions per store
-        for (int k = 0; k < nchunks; ++k) {
-            const uint32_t m = transpose32(s_mask[wid][k][lane], lane);
-            if ((k << 5) + lane < nh) s_out[wid][s_list[wid][(k << 5) + lane]] = m;
+            // ---- contribution record of the batch: transposed back, lane l holds the pixel mask of hit 32 k + l, which
+            // goes to its batch slot (the slots the cull dropped stay 0); then 32 consecutive list positions per store
+            for (int k = 0; k < nchunks; ++k) {
+                const uint32_t m = transpose32(s_mask[wid][k][lane], lane);
+                if ((k << 5) + lane < nh) s_out[wid][s_list[wid][(k << 5) + lane]] = m;
+            }
+            // a warp that saturated in this batch stores only the positions before its block's deepest contributor
+            int lim = cnt;
+            if (__all_sync(0xffffffffu, done)) lim = min(cnt, (int)__reduce_max_sync(0xffffffffu, last_contributor) - b * SRF_BATCH);
+            __syncwarp();
+            uint32_t* dst = a.masks + (size_t)gw * a.capacity + range.x + b * SRF_BATCH;
+            for (int jt = lane; jt < lim; jt += 32) dst[jt] = s_out[wid][jt];
         }
-        // a warp that saturated in this batch stores only the positions before its block's deepest contributor
-        int lim = cnt;
-        if (__all_sync(0xffffffffu, done)) lim = min(cnt, (int)__reduce_max_sync(0xffffffffu, last_contributor) - b * SRF_BATCH);
-        __syncwarp();
-        uint32_t* dst = a.masks + (size_t)gw * a.capacity + range.x + b * SRF_BATCH;
-        for (int jt = lane; jt < lim; jt += 32) dst[jt] = s_out[wid][jt];
     }
 
     const float2 C01_ = up2(C01), C2r_ = up2(C2r), N01_ = up2(N01), N2D_ = up2(N2D), d12_f = up2(d12);
@@ -202,11 +219,13 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
     if (inside) {
         const size_t npix = (size_t)a.W * a.H;
         const size_t pix = (size_t)pyi * a.W + pxi;
-        a.accum[pix] = T;
-        a.accum[pix + npix] = dist1;
-        a.accum[pix + 2 * npix] = dist2;
-        a.n_contrib[pix] = last_contributor;
-        a.n_contrib[pix + npix] = median_contributor;
+        if constexpr (kRecord) {
+            a.accum[pix] = T;
+            a.accum[pix + npix] = dist1;
+            a.accum[pix + 2 * npix] = dist2;
+            a.n_contrib[pix] = last_contributor;
+            a.n_contrib[pix + npix] = median_contributor;
+        }
         a.out_color[pix] = fma_(__ldg(a.bg + 0), T, C0);
         a.out_color[pix + npix] = fma_(__ldg(a.bg + 1), T, C1);
         a.out_color[pix + 2 * npix] = fma_(__ldg(a.bg + 2), T, C2);
@@ -221,11 +240,15 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
     }
 }
 
-cudaError_t launch_render_fwd(const RenderFwdArgs& a, cudaStream_t stream) {
+cudaError_t launch_render_fwd(const RenderFwdArgs& a, bool record, cudaStream_t stream) {
     const int ntiles = a.gx * a.gy;
     if (ntiles <= 0 || a.nviews <= 0) return cudaSuccess;
     prof_start(K_RENDER_FWD, stream);
-    render_fwd_kernel<<<dim3(ntiles * SRF_CTAS_PER_TILE, a.nviews), SRF_CTA_THREADS, 0, stream>>>(a);
+    const dim3 grid(ntiles * SRF_CTAS_PER_TILE, a.nviews);
+    if (record)
+        render_fwd_kernel<true><<<grid, SRF_CTA_THREADS, 0, stream>>>(a);
+    else
+        render_fwd_kernel<false><<<grid, SRF_CTA_THREADS, 0, stream>>>(a);
     prof_stop(K_RENDER_FWD, stream);
     return cudaGetLastError();
 }

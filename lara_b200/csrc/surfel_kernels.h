@@ -250,7 +250,8 @@ cudaError_t launch_mark_visible(int P, const float* means3D, const float* viewma
                                 cudaStream_t stream);
 cudaError_t launch_tile_scan(const BinArgs& a, cudaStream_t stream);
 cudaError_t launch_bin_and_sort(const BinArgs& a, cudaStream_t stream);
-cudaError_t launch_render_fwd(const RenderFwdArgs& a, cudaStream_t stream);
+// record = false: the forward-only blend, which writes neither a.masks nor a.accum / a.n_contrib (they may be null)
+cudaError_t launch_render_fwd(const RenderFwdArgs& a, bool record, cudaStream_t stream);
 cudaError_t launch_render_bwd(const RenderBwdArgs& a, cudaStream_t stream);
 // Deterministic blend backward (DESIGN §3.13): a.ggrad / a.ggrad_stride point at zeroed det_record_bytes() records per
 // (Gaussian, view); the fp32 gradient records preprocess_bwd reads go to ggrad / ggrad_stride; *overflow (zeroed by the

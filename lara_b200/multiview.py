@@ -41,47 +41,58 @@ def shared_view_settings(settings_list: Sequence[R.GaussianRasterizationSettings
     return key + (any(bool(rs.prefiltered) for rs in settings_list), any(bool(rs.debug) for rs in settings_list))
 
 
+def _scene_views_forward(centers, shs, opacity, scales, rotations, rays, settings_list, depth_ratio, raw_activations,
+                         for_backward):
+    """Checks, the V-view rasterizer forward and the fused epilogue.  Returns the outputs (image, depth, acc, rn, dn,
+    dist, radii) and what the backward needs: (inputs, rays, cams, color, allmap, state, geometry)."""
+    dev = centers.device
+    V = len(settings_list)
+    centers_c, shs_c, _, opac_c, scales_c, rot_c, _ = R._normalise_inputs(
+        centers, shs, None, opacity, scales, rotations, None)
+    settings_list = [R._check_settings(rs, dev) for rs in settings_list]
+    H, W, tfx, tfy, deg, prefiltered, debug = shared_view_settings(settings_list)
+    rays_c = None
+    if rays is not None:
+        rays_c = rays.contiguous()
+        if rays_c.dtype != torch.float32 or tuple(rays_c.shape) != (V, H, W, 6):
+            raise RuntimeError(f"rays must be float32 [V,H,W,6] = {(V, H, W, 6)}, got {tuple(rays_c.shape)}")
+        if rays_c.device != dev:
+            raise RuntimeError(f"rays must live on {dev}, got {rays_c.device}")
+    cams = R.pack_cameras(settings_list, dev)
+    color, allmap, radii, state = R.forward_views_raw(
+        centers_c, shs_c, None, opac_c, scales_c, rot_c, None, cams, tfx, tfy, H, W, deg,
+        prefiltered=prefiltered, debug=debug, raw_activations=raw_activations, for_backward=for_backward)
+
+    def new(*shape):
+        return torch.empty(shape, dtype=torch.float32, device=dev)
+    if rays_c is not None:
+        image, depth, acc = new(V, 3, H, W), new(V, 1, H, W), new(V, H, W)
+        rn, dn, dist = new(V, 3, H, W), new(V, 3, H, W), new(V, H, W)
+        epilogue_views_forward_raw(color, allmap, rays_c, cams, depth_ratio, image, depth, acc, rn, dn, dist)
+    else:
+        image = color.clamp(0, 1)
+        depth = acc = rn = dn = dist = centers_c.new_empty(0)
+    return ((image, depth, acc, rn, dn, dist, radii),
+            ((centers_c, shs_c, scales_c, rot_c), rays_c, cams, color, allmap, state, (H, W, tfx, tfy, deg, debug)))
+
+
 class _RenderSceneViews(torch.autograd.Function):
     @staticmethod
     def forward(ctx, centers, shs, opacity, scales, rotations, rays, settings_list, depth_ratio, raw_activations):
-        dev = centers.device
-        V = len(settings_list)
-        centers_c, shs_c, _, opac_c, scales_c, rot_c, _ = R._normalise_inputs(
-            centers, shs, None, opacity, scales, rotations, None)
-        settings_list = [R._check_settings(rs, dev) for rs in settings_list]
-        H, W, tfx, tfy, deg, prefiltered, debug = shared_view_settings(settings_list)
-        rays_c = None
-        if rays is not None:
-            rays_c = rays.contiguous()
-            if rays_c.dtype != torch.float32 or tuple(rays_c.shape) != (V, H, W, 6):
-                raise RuntimeError(f"rays must be float32 [V,H,W,6] = {(V, H, W, 6)}, got {tuple(rays_c.shape)}")
-            if rays_c.device != dev:
-                raise RuntimeError(f"rays must live on {dev}, got {rays_c.device}")
-        cams = R.pack_cameras(settings_list, dev)
-        color, allmap, radii, state = R.forward_views_raw(
-            centers_c, shs_c, None, opac_c, scales_c, rot_c, None, cams, tfx, tfy, H, W, deg,
-            prefiltered=prefiltered, debug=debug, raw_activations=raw_activations)
-
-        def new(*shape):
-            return torch.empty(shape, dtype=torch.float32, device=dev)
-        if rays_c is not None:
-            image, depth, acc = new(V, 3, H, W), new(V, 1, H, W), new(V, H, W)
-            rn, dn, dist = new(V, 3, H, W), new(V, 3, H, W), new(V, H, W)
-            epilogue_views_forward_raw(color, allmap, rays_c, cams, depth_ratio, image, depth, acc, rn, dn, dist)
-        else:
-            image = color.clamp(0, 1)
-            depth = acc = rn = dn = dist = centers_c.new_empty(0)
-
+        outs, (inputs, rays_c, cams, color, allmap, state, geometry) = _scene_views_forward(
+            centers, shs, opacity, scales, rotations, rays, settings_list, depth_ratio, raw_activations, True)
+        centers_c, shs_c, scales_c, rot_c = inputs
+        radii = outs[-1]
         ctx.save_for_backward(centers_c, shs_c, scales_c, rot_c, rays_c if rays_c is not None else centers_c.new_empty(0),
                               cams, color, allmap, radii, state.geom, state.tile, state.image)
         ctx.state = state
-        ctx.geometry = (H, W, tfx, tfy, deg, debug)
+        ctx.geometry = geometry
         ctx.has_rays = rays_c is not None
         ctx.depth_ratio = float(depth_ratio)
         ctx.raw_activations = bool(raw_activations)
         ctx.opac_shape = tuple(opacity.shape)
         ctx.mark_non_differentiable(radii)
-        return image, depth, acc, rn, dn, dist, radii
+        return outs
 
     @staticmethod
     def backward(ctx, g_image, g_depth, g_acc, g_rn, g_dn, g_dist, _g_radii):
@@ -109,11 +120,16 @@ def render_scene_views(centers, shs, opacity, scales, rotations, settings_list: 
     the keys, channel-last layout and values of ``Renderer.render_img``'s dict (renderer_2dgs.py:256-268) plus
     ``radii+prex`` [V, P]; ``out[k][j]`` is what the j-th ``render_img`` call of network.py:486-495 returns.
     ``rays=None``: only ``image`` as [V,3,H,W] (render_img's early return is the clamped planar image).
-    ``streams`` is accepted for compatibility and ignored: the views share one launch set now."""
+    ``streams`` is accepted for compatibility and ignored: the views share one launch set now.
+    When no gradient can flow (``torch.no_grad()``, ``torch.inference_mode()``, no input requiring grad) the views
+    take the forward-only path: the same values, without the backward's state and without an autograd node."""
     if len(settings_list) == 0:
         raise ValueError("render_scene_views needs at least one view")
-    image, depth, acc, rn, dn, dist, radii = _RenderSceneViews.apply(
-        centers, shs, opacity, scales, rotations, rays, list(settings_list), float(depth_ratio), bool(raw_activations))
+    args = (centers, shs, opacity, scales, rotations, rays, list(settings_list), float(depth_ratio), bool(raw_activations))
+    if R.needs_backward(centers, shs, opacity, scales, rotations, rays):
+        image, depth, acc, rn, dn, dist, radii = _RenderSceneViews.apply(*args)
+    else:
+        (image, depth, acc, rn, dn, dist, radii), _ = _scene_views_forward(*args, False)
     if rays is None:          # render_img's early return hands back the clamped [3,H,W] image, not a dict
         return {f"image{prex}": image, f"radii{prex}": radii}
     return {

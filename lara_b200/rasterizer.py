@@ -47,7 +47,7 @@ class GaussianRasterizationSettings(NamedTuple):
 # small host-side helpers
 # ---------------------------------------------------------------------------------
 
-_size_cache: dict = {}            # (V, P, H, W, capacity) -> srf_views_workspace_bytes
+_size_cache: dict = {}            # (V, P, H, W, capacity, for_backward) -> workspace sizes
 _cam_pads: dict = {}              # device -> zero padding of a camera record
 _capacity_hwm: dict = {}          # device index -> largest num_rendered seen (instances per view)
 _lock = threading.Lock()          # autograd calls backward() from another host thread
@@ -76,11 +76,12 @@ def _f32c(t: torch.Tensor, name: str) -> torch.Tensor:
     return t.contiguous()
 
 
-def _views_sizes(lib, V: int, P: int, H: int, W: int, capacity: int):
-    key = (V, P, H, W, capacity)
+def _views_sizes(lib, V: int, P: int, H: int, W: int, capacity: int, for_backward: bool = True):
+    """srf_views_workspace_bytes (six sizes), or with for_backward=False srf_views_inference_workspace_bytes (five)."""
+    key = (V, P, H, W, capacity, for_backward)
     v = _size_cache.get(key)
     if v is None:
-        v = _lib.views_sizes(lib, V, P, H, W, capacity)
+        v = (_lib.views_sizes if for_backward else _lib.inference_sizes)(lib, V, P, H, W, capacity)
         if len(_size_cache) > 64:
             _size_cache.clear()
         _size_cache[key] = v
@@ -245,13 +246,15 @@ class LazyCount:
 
 class ForwardState:
     """What a forward leaves behind for the backward (the reference's three blobs): V per-view workspaces back to
-    back, and the [V, SRF_CAM_FLOATS] camera records the forward ran on."""
-    __slots__ = ("geom", "tile", "image", "point_list", "capacity", "nviews", "cams", "_pending", "_counts")
+    back, and the [V, SRF_CAM_FLOATS] camera records the forward ran on.  A forward-only state
+    (``for_backward=False``) keeps no image state and no point list: it cannot feed a backward."""
+    __slots__ = ("geom", "tile", "image", "point_list", "capacity", "nviews", "cams", "for_backward", "_pending",
+                 "_counts")
 
     def __init__(self, geom, tile, image, point_list, capacity, num_rendered=0, nviews: int = 1, pending=None,
-                 cams=None):
+                 cams=None, for_backward: bool = True):
         self.geom, self.tile, self.image, self.point_list = geom, tile, image, point_list
-        self.capacity, self.nviews, self.cams = capacity, nviews, cams
+        self.capacity, self.nviews, self.cams, self.for_backward = capacity, nviews, cams, for_backward
         self._pending = pending
         self._counts = None if pending is not None else ([int(num_rendered)] * nviews
                                                          if not isinstance(num_rendered, (list, tuple)) else list(num_rendered))
@@ -295,38 +298,46 @@ def _cam_pad(device) -> torch.Tensor:
 
 
 def forward_raw(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp,
-                raster_settings: GaussianRasterizationSettings, raw_activations: bool = False):
+                raster_settings: GaussianRasterizationSettings, raw_activations: bool = False, *,
+                for_backward: bool = True):
     """Enqueue one forward on the current stream of the tensors' device: :func:`forward_views_raw` with V = 1 on the
     settings' camera record, which the returned state keeps for :func:`backward_raw`.
 
     Returns (color[3,H,W], allmap[8,H,W], radii[P], ForwardState).  Inputs must already be
-    normalised (None for absent, fp32, contiguous, CUDA).
+    normalised (None for absent, fp32, contiguous, CUDA).  ``for_backward=False``: the forward-only path, as in
+    :func:`forward_views_raw`.
     """
     rs = raster_settings
     with _DeviceGuard(means3D.device):
         return _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp,
                         pack_cameras([rs], means3D.device), rs.tanfovx, rs.tanfovy, int(rs.image_height),
-                        int(rs.image_width), rs.sh_degree, rs.prefiltered, rs.debug, raw_activations, single=True)
+                        int(rs.image_width), rs.sh_degree, rs.prefiltered, rs.debug, raw_activations, single=True,
+                        for_backward=for_backward)
 
 
 def forward_views_raw(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp,
                       cams: torch.Tensor, tanfovx: float, tanfovy: float, H: int, W: int, sh_degree: int,
-                      prefiltered: bool = False, debug: bool = False, raw_activations: bool = False):
+                      prefiltered: bool = False, debug: bool = False, raw_activations: bool = False, *,
+                      for_backward: bool = True):
     """All V views of one Gaussian set in ONE launch set (srf_views_*): every kernel carries a view
     dimension.  `cams` is the [V, 24] device tensor of camera records (pack_cameras).
-    Returns (color [V,3,H,W], allmap [V,8,H,W], radii [V,P], ForwardState with V back-to-back workspaces)."""
+    Returns (color [V,3,H,W], allmap [V,8,H,W], radii [V,P], ForwardState with V back-to-back workspaces).
+    ``for_backward=False``: the forward-only entries (srf_views_forward_inference), bit-identical outputs without the
+    blend's contribution record and image state; the returned state cannot feed :func:`backward_views_raw`."""
     with _DeviceGuard(means3D.device):
         if cams.dtype != torch.float32 or not cams.is_cuda or cams.shape[1] != _lib.CAM_FLOATS or not cams.is_contiguous():
             raise RuntimeError(f"cams must be a contiguous float32 CUDA tensor [V,{_lib.CAM_FLOATS}]")
         return _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp, cams, tanfovx,
-                        tanfovy, H, W, sh_degree, prefiltered, debug, raw_activations, single=False)
+                        tanfovy, H, W, sh_degree, prefiltered, debug, raw_activations, single=False,
+                        for_backward=for_backward)
 
 
 def _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp, cams, tanfovx, tanfovy,
-             H, W, sh_degree, prefiltered, debug, raw_activations, single):
+             H, W, sh_degree, prefiltered, debug, raw_activations, single, for_backward):
     """srf_views_forward on the current stream: stage 1 (preprocess + tile scan + async count read-back) and stage 2
     (binning + blend) with an optimistic capacity, then an event for whoever eventually asks for the instance counts.
-    `single`: one view, with the outputs in the reference's one-view shapes."""
+    `single`: one view, with the outputs in the reference's one-view shapes.  `for_backward` False: the
+    srf_views_forward_inference pair of entries and their smaller workspaces, no image state or point list kept."""
     lib = _lib.load()
     device = means3D.device
     V, P = int(cams.shape[0]), int(means3D.shape[0])
@@ -338,13 +349,18 @@ def _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMa
     allmap = torch.empty(lead + (8, H, W), dtype=torch.float32, device=device)
     radii = torch.empty(lead + (P,), dtype=torch.int32, device=device)
     capacity = initial_capacity(P, device)
-    geom_b, tile_b, image_b, ent_b, pl_b, _ = _views_sizes(lib, V, P, H, W, capacity)
-    # the three state workspaces share one byte blob (sub-blobs stay 256-byte aligned: the sizes are multiples of 256)
+    geom_b, tile_b, image_b, ent_b, pl_b = _views_sizes(lib, V, P, H, W, capacity, for_backward)[:5]
+    # the state workspaces share one byte blob (sub-blobs stay 256-byte aligned: the sizes are multiples of 256)
     blob = _blob(geom_b + tile_b + image_b, device)
-    geom, tile, image = blob[:geom_b], blob[geom_b:geom_b + tile_b], blob[geom_b + tile_b:]
+    geom, tile = blob[:geom_b], blob[geom_b:geom_b + tile_b]
+    image = blob[geom_b + tile_b:] if for_backward else None
     if P == 0:
         # reference: zero-filled outputs, nothing rendered (rasterize_points.cu:92-94,105)
-        color.zero_(); allmap.zero_(); tile.zero_(); image.zero_()
+        color.zero_(); allmap.zero_(); tile.zero_()
+        if not for_backward:
+            return color, allmap, radii, ForwardState(geom, tile, None, None, 0, 0, nviews=V, cams=cams,
+                                                      for_backward=False)
+        image.zero_()
         pl = torch.empty((0,), dtype=torch.int32, device=device)
         return color, allmap, radii, ForwardState(geom, tile, image, pl, 0, 0, nviews=V, cams=cams)
 
@@ -355,25 +371,32 @@ def _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMa
     # Stage 2 is enqueued before the counts are known on the host, so the GPU never idles behind the read-back; an
     # overflow (rare) re-runs stage 2.  The event sits between the stages: whoever resolves the counts later waits for
     # the tile scan, never for the blend.
-    _lib.check(lib.srf_views_forward(
+    # the forward-only point list and entries are scratch of this call: they go back to the caching allocator when
+    # it returns, stream-ordered behind the kernels that use them
+    fwd, fwd_render = ((lib.srf_views_forward, lib.srf_views_forward_render) if for_backward else
+                       (lib.srf_views_forward_inference, lib.srf_views_forward_inference_render))
+    _lib.check(fwd(
         _raw_stream(device), V, P, int(sh_degree), M, _ptr(means3D), _ptr(shs), _ptr(colors_precomp),
         _ptr(opacities), _ptr(scales), _ptr(rotations), _ptr(transMat_precomp), cams.data_ptr(),
         float(tanfovx), float(tanfovy), H, W, 1 if prefiltered else 0, capacity,
         radii.data_ptr(), geom.data_ptr(), tile.data_ptr(), _blob(ent_b, device).data_ptr(), point_list.data_ptr(),
-        image.data_ptr(), color.data_ptr(), allmap.data_ptr(), slot.data_ptr(), ev.cuda_event,
+        _ptr(image), color.data_ptr(), allmap.data_ptr(), slot.data_ptr(), ev.cuda_event,
         1 if raw_activations else 0), lib)
-    state = ForwardState(geom, tile, image, point_list, capacity, nviews=V, cams=cams)
+    state = ForwardState(geom, tile, image, point_list if for_backward else None, capacity, nviews=V, cams=cams,
+                         for_backward=for_backward)
 
     def rerun(new_capacity: int):
         # enqueued on whatever stream is current: a deferred re-run happens on the caller's stream
         with _DeviceGuard(device):
-            _, _, _, e_b, p_b, _ = _views_sizes(lib, V, P, H, W, new_capacity)
+            e_b, p_b = _views_sizes(lib, V, P, H, W, new_capacity, for_backward)[3:5]
             pl2 = _blob(p_b, device)
-            _lib.check(lib.srf_views_forward_render(
+            _lib.check(fwd_render(
                 _raw_stream(device), V, P, H, W, new_capacity, geom.data_ptr(), tile.data_ptr(),
-                _blob(e_b, device).data_ptr(), pl2.data_ptr(), image.data_ptr(), cams.data_ptr(), color.data_ptr(),
+                _blob(e_b, device).data_ptr(), pl2.data_ptr(), _ptr(image), cams.data_ptr(), color.data_ptr(),
                 allmap.data_ptr()), lib)
-            state.point_list, state.capacity = pl2, new_capacity
+            state.capacity = new_capacity
+            if for_backward:
+                state.point_list = pl2
 
     pend = _Pending(device, rb, V, capacity, rerun)
     state._pending, state._counts = pend, None
@@ -447,6 +470,10 @@ def backward_views_raw(state: ForwardState, radii, means3D, shs, colors_precomp,
     """Backward of forward_views_raw: grad_color [V,3,H,W], grad_allmap [V,8,H,W]; the per-Gaussian backward
     sums the V views in registers and writes (accumulate: adds into) every parameter-gradient row once.
     ``deterministic`` as in :func:`backward_raw`."""
+    if not state.for_backward:
+        raise RuntimeError("backward of a forward-only render: this state comes from a forward with "
+                           "for_backward=False, which keeps no contribution record or image state; run the "
+                           "forward with for_backward=True to take its gradient")
     with _DeviceGuard(means3D.device):
         lib = _lib.load()
         device = means3D.device
@@ -548,10 +575,49 @@ def _normalise_inputs(means3D, sh, colors_precomp, opacities, scales, rotations,
 # the reference's public surface
 # ---------------------------------------------------------------------------------
 
+def needs_backward(*inputs) -> bool:
+    """Whether a render can have a gradient: grad mode is on and a tensor input requires grad.  Decided before any
+    ``autograd.Function`` runs: inside its forward grad mode is always off, and under ``torch.no_grad()``
+    ``ctx.needs_input_grad`` still reports inputs that require grad.  Renders for which this is False (``no_grad``,
+    ``inference_mode``, inputs that need no gradient) take the forward-only path."""
+    return torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in inputs)
+
+
+def _rasterize(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings,
+               raw_activations, for_backward):
+    """The checks of the reference's forward, then forward_raw; returns (settings, normalised inputs, color, allmap,
+    radii, state)."""
+    raster_settings = _check_settings(raster_settings, means3D.device)
+    inputs = _normalise_inputs(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp)
+    try:
+        color, allmap, radii, state = forward_raw(*inputs, raster_settings, raw_activations=raw_activations,
+                                                  for_backward=for_backward)
+    except Exception:
+        if raster_settings.debug:
+            # same debugging aid as the reference (DSR __init__.py:83-90)
+            _dump_snapshot("snapshot_fw.dump", (raster_settings, means3D, sh, colors_precomp, opacities,
+                                               scales, rotations, cov3Ds_precomp))
+            print("\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.")
+        raise
+    return raster_settings, inputs, color, allmap, radii, state
+
+
+def _rasterize_any(fn, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                   raster_settings):
+    """``fn.apply`` when a gradient can flow, else the forward-only path without an autograd node: the same
+    (color, radii, allmap)."""
+    if needs_backward(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp):
+        return fn.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                        raster_settings)
+    _, _, color, allmap, radii, _ = _rasterize(means3D, sh, colors_precomp, opacities, scales, rotations,
+                                               cov3Ds_precomp, raster_settings, fn.RAW_ACTIVATIONS, False)
+    return color, radii, allmap
+
+
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                         cov3Ds_precomp, raster_settings):
-    return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales,
-                                     rotations, cov3Ds_precomp, raster_settings)
+    return _rasterize_any(_RasterizeGaussians, means3D, means2D, sh, colors_precomp, opacities, scales,
+                          rotations, cov3Ds_precomp, raster_settings)
 
 
 class _RasterizeGaussians(torch.autograd.Function):
@@ -560,20 +626,10 @@ class _RasterizeGaussians(torch.autograd.Function):
     @classmethod
     def forward(cls, ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                 cov3Ds_precomp, raster_settings):
-        raster_settings = _check_settings(raster_settings, means3D.device)
-        (means3D_c, sh_c, colors_c, opac_c, scales_c, rot_c, cov_c) = _normalise_inputs(
-            means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp)
-        try:
-            color, allmap, radii, state = forward_raw(
-                means3D_c, sh_c, colors_c, opac_c, scales_c, rot_c, cov_c, raster_settings,
-                raw_activations=cls.RAW_ACTIVATIONS)
-        except Exception:
-            if raster_settings.debug:
-                # same debugging aid as the reference (DSR __init__.py:83-90)
-                _dump_snapshot("snapshot_fw.dump", (raster_settings, means3D, sh, colors_precomp, opacities,
-                                                   scales, rotations, cov3Ds_precomp))
-                print("\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.")
-            raise
+        raster_settings, inputs, color, allmap, radii, state = _rasterize(
+            means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings,
+            cls.RAW_ACTIVATIONS, True)
+        (means3D_c, sh_c, colors_c, opac_c, scales_c, rot_c, cov_c) = inputs
         ctx.raster_settings = raster_settings
         ctx.state = state
         # an int for an eager forward, else an int-like object that waits for the read-back when asked
@@ -626,8 +682,8 @@ class _RasterizeGaussiansRaw(_RasterizeGaussians):
 
 def rasterize_gaussians_raw(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                             cov3Ds_precomp, raster_settings):
-    return _RasterizeGaussiansRaw.apply(means3D, means2D, sh, colors_precomp, opacities, scales,
-                                        rotations, cov3Ds_precomp, raster_settings)
+    return _rasterize_any(_RasterizeGaussiansRaw, means3D, means2D, sh, colors_precomp, opacities, scales,
+                          rotations, cov3Ds_precomp, raster_settings)
 
 
 class GaussianRasterizer(nn.Module):

@@ -1,0 +1,246 @@
+"""Forward-only rendering, host side (no GPU needed): the srf_views_forward_inference entries and their workspace query,
+their argument checks, and the rule by which the public wrappers pick the forward-only path -- taken iff no gradient can
+flow (grad mode off, or no tensor input requires grad) -- driven with stand-ins for the raw forward functions."""
+import ctypes
+
+import pytest
+import torch
+
+from lara_b200 import _lib
+from lara_b200 import multiview as MV
+from lara_b200 import rasterizer as R
+
+from test_abi import declared_symbols
+
+NEW = ("srf_views_forward_inference", "srf_views_forward_inference_render", "srf_views_inference_workspace_bytes")
+
+
+def align256(x):
+    return (x + 255) // 256 * 256
+
+
+def test_new_entries_are_declared_exported_and_bound(lib):
+    syms = declared_symbols()
+    for name in NEW:
+        assert name in syms and name in _lib.SIGNATURES and hasattr(lib, name), name
+    # the forward-only twins take exactly the training entries' arguments
+    assert _lib.SIGNATURES["srf_views_forward_inference"] == _lib.SIGNATURES["srf_views_forward"]
+    assert _lib.SIGNATURES["srf_views_forward_inference_render"] == _lib.SIGNATURES["srf_views_forward_render"]
+    assert lib.srf_abi_version() == _lib.ABI_VERSION == 11
+
+
+@pytest.mark.parametrize("V,P,H,W,capacity", [(1, 1000, 300, 500, 12345), (8, 131072, 512, 512, 1 << 20),
+                                              (48, 524288, 512, 512, 8 * 524288), (3, 0, 16, 16, 0)])
+def test_inference_workspace_sizes(lib, V, P, H, W, capacity):
+    geom, tile, image, entries, plist = _lib.inference_sizes(lib, V, P, H, W, capacity)
+    tg, tt, ti, te, tp, _ = _lib.views_sizes(lib, V, P, H, W, capacity)
+    assert plist == align256(4 * capacity) * V
+    assert 8 * plist <= tp
+    assert tp - plist >= 32 * capacity * V              # the contribution record is what goes
+    assert image == 0 and ti > 0
+    assert (geom, tile, entries) == (tg, tt, te)
+
+
+def test_inference_workspace_query_rejects_bad_arguments(lib):
+    n = (ctypes.c_size_t * 5)()
+    for args in [(0, 1, 16, 16, 0), (1, -1, 16, 16, 0), (1, 0, 0, 16, 0), (1, 0, 16, -2, 0)]:
+        assert lib.srf_views_inference_workspace_bytes(*args, n) != 0
+        assert b"srf_views_inference_workspace_bytes: bad arguments" == lib.srf_last_error()
+    assert lib.srf_views_inference_workspace_bytes(1, 0, 16, 16, 0, None) != 0
+
+
+def _forward_args(V=1, P=4, D=0, H=16, W=16, capacity=0, geom=None, tile=None, entries=None, plist=None, out=None):
+    cams = (ctypes.c_float * 24)()
+    args = [None, V, P, D, 1, None, None, None, None, None, None, None, ctypes.addressof(cams),
+            1.0, 1.0, H, W, 0, capacity, None, geom, tile, entries, plist, None, out, out, None, None, 0]
+    return args, cams
+
+
+@pytest.mark.parametrize("case", [dict(V=0), dict(H=16 * 65535 + 1), dict(), dict(tile=0x1010),
+                                  dict(tile=0x1000, D=4)])
+def test_forward_inference_rejects_what_the_training_forward_rejects(lib, case):
+    """Same arguments, same message (but for the entry's name); every case fails before anything is enqueued."""
+    args, _cams = _forward_args(**case)
+    assert lib.srf_views_forward(*args) != 0
+    train = lib.srf_last_error().decode()
+    assert lib.srf_views_forward_inference(*args) != 0
+    inf = lib.srf_last_error().decode()
+    assert train.startswith("srf_views_forward: ") and inf == train.replace("srf_views_forward", "srf_views_forward_inference")
+
+
+def test_forward_inference_rejects_null_or_misaligned_workspaces_before_any_cuda_call(lib):
+    """Without a device any CUDA call would fail with a CUDA error; these fail with the argument check's message."""
+    x = 0x10000          # a 256-byte aligned address that is never dereferenced: every call below fails its checks
+    cases = [
+        (dict(P=0, tile=x, capacity=64, entries=x, plist=None, out=x), "null binning buffers"),
+        (dict(P=0, tile=x, capacity=64, entries=x, plist=x + 4, out=x), "entries and point_list must be 256-byte aligned"),
+        (dict(P=0, tile=x, capacity=64, entries=x + 8, plist=x, out=x), "entries and point_list must be 256-byte aligned"),
+        (dict(P=0, tile=x, capacity=64, entries=x, plist=x, out=None), "null required pointer"),
+    ]
+    for kw, msg in cases:
+        args, _cams = _forward_args(**kw)
+        assert lib.srf_views_forward_inference(*args) != 0
+        assert lib.srf_last_error().decode() == f"srf_views_forward_inference: {msg}", kw
+    cams = (ctypes.c_float * 24)()
+    # stage 2 alone: image_state may be NULL, a misaligned geom_state or point_list is rejected
+    render = [None, 1, 4, 16, 16, 64, x + 16, x, x, x, None, ctypes.addressof(cams), x, x]
+    assert lib.srf_views_forward_inference_render(*render) != 0
+    assert lib.srf_last_error() == b"srf_views_forward_inference_render: geom_state must be 256-byte aligned"
+    render[6], render[9] = x, x + 4
+    assert lib.srf_views_forward_inference_render(*render) != 0
+    assert lib.srf_last_error() == b"srf_views_forward_inference_render: entries and point_list must be 256-byte aligned"
+    render[1] = 0
+    assert lib.srf_views_forward_inference_render(*render) != 0
+    assert lib.srf_last_error() == b"srf_views_forward_inference_render: bad sizes"
+    render[1], render[2], render[10], render[11] = 1, 0, None, None
+    assert lib.srf_views_forward_inference_render(*render) != 0
+    assert lib.srf_last_error() == b"srf_views_forward_inference_render: null required pointer"
+
+
+# ---------------------------------------------------------------------------------------------- selection rule
+
+P, H, W = 5, 4, 6
+
+
+def _settings():
+    return R.GaussianRasterizationSettings(
+        image_height=H, image_width=W, tanfovx=0.5, tanfovy=0.5, bg=torch.zeros(3), scale_modifier=1.0,
+        viewmatrix=torch.eye(4), projmatrix=torch.eye(4), sh_degree=0, campos=torch.zeros(3), prefiltered=False,
+        debug=False)
+
+
+def _fake_outputs(V, for_backward, single):
+    lead = () if single else (V,)
+    color = torch.arange(V * 3 * H * W, dtype=torch.float32).reshape(lead + (3, H, W)) / 100.0
+    allmap = torch.full(lead + (8, H, W), 0.25)
+    radii = torch.arange(V * P, dtype=torch.int32).reshape(lead + (P,))
+    blob = torch.zeros(16, dtype=torch.uint8)
+    state = R.ForwardState(blob, blob, blob if for_backward else None, blob if for_backward else None, 0, 0,
+                           nviews=V, for_backward=for_backward)
+    return color, allmap, radii, state
+
+
+@pytest.fixture
+def stand_ins(monkeypatch):
+    """forward_raw / forward_views_raw record which path was asked for; the CUDA-only input checks pass CPU tensors."""
+    calls = []
+
+    def forward_raw(*a, raw_activations=False, for_backward=True):
+        calls.append(("forward_raw", for_backward, raw_activations))
+        return _fake_outputs(1, for_backward, True)
+
+    def forward_views_raw(*a, raw_activations=False, for_backward=True, **kw):
+        V = int(a[7].shape[0])
+        calls.append(("forward_views_raw", for_backward, raw_activations))
+        return _fake_outputs(V, for_backward, False)
+
+    monkeypatch.setattr(R, "forward_raw", forward_raw)
+    monkeypatch.setattr(R, "forward_views_raw", forward_views_raw)
+    monkeypatch.setattr(R, "_f32c", lambda t, name: t.contiguous())
+    monkeypatch.setattr(R, "_check_settings", lambda rs, device: rs)
+    return calls
+
+
+def _inputs(requires=()):
+    g = torch.Generator().manual_seed(0)
+    t = {"means3D": torch.randn((P, 3), generator=g), "means2D": torch.zeros((P, 3)),
+         "shs": torch.randn((P, 1, 3), generator=g), "opacities": torch.rand((P, 1), generator=g),
+         "scales": torch.rand((P, 2), generator=g), "rotations": torch.randn((P, 4), generator=g)}
+    for k in requires:
+        t[k].requires_grad_(True)
+    return t
+
+
+ALL = ("means3D", "means2D", "shs", "opacities", "scales", "rotations")
+MATRIX = [  # (grad mode, inputs requiring grad, training path expected)
+    ("grad", ALL, True),
+    ("grad", ("means2D",), True),
+    ("grad", ("opacities",), True),
+    ("grad", (), False),
+    ("no_grad", ALL, False),
+    ("no_grad", (), False),
+    ("inference_mode", ALL, False),
+]
+
+
+def _mode(name):
+    return {"grad": torch.enable_grad, "no_grad": torch.no_grad, "inference_mode": torch.inference_mode}[name]()
+
+
+@pytest.mark.parametrize("mode,requires,training", MATRIX)
+@pytest.mark.parametrize("entry", ["rasterize_gaussians", "rasterize_gaussians_raw", "module", "module_raw"])
+def test_dropin_selection_rule(stand_ins, entry, mode, requires, training):
+    t = _inputs(requires)
+    rs = _settings()
+    with _mode(mode):
+        if entry == "rasterize_gaussians":
+            out = R.rasterize_gaussians(t["means3D"], t["means2D"], t["shs"], None, t["opacities"], t["scales"],
+                                        t["rotations"], None, rs)
+        elif entry == "rasterize_gaussians_raw":
+            out = R.rasterize_gaussians_raw(t["means3D"], t["means2D"], t["shs"], None, t["opacities"], t["scales"],
+                                            t["rotations"], None, rs)
+        elif entry == "module":
+            out = R.GaussianRasterizer(rs)(means3D=t["means3D"], means2D=t["means2D"], shs=t["shs"],
+                                           opacities=t["opacities"], scales=t["scales"], rotations=t["rotations"])
+        else:
+            out = R.GaussianRasterizer(rs).forward_raw_activations(t["means3D"], t["means2D"], t["opacities"],
+                                                                   t["scales"], t["rotations"], shs=t["shs"])
+    assert stand_ins == [("forward_raw", training, entry.endswith("raw"))]
+    color, radii, allmap = out
+    ref_c, ref_a, ref_r, _ = _fake_outputs(1, True, True)
+    assert torch.equal(color.detach(), ref_c) and torch.equal(allmap.detach(), ref_a) and torch.equal(radii, ref_r)
+    assert radii.dtype == torch.int32 and not radii.requires_grad
+    assert color.requires_grad == training and (color.grad_fn is not None) == training
+
+
+@pytest.mark.parametrize("mode,requires,training", [m for m in MATRIX if "means2D" not in m[1] or len(m[1]) > 1])
+def test_scene_views_selection_rule(stand_ins, mode, requires, training):
+    t = _inputs(requires)
+    V = 3
+    sets = [_settings() for _ in range(V)]
+    with _mode(mode):
+        out = MV.render_scene_views(t["means3D"], t["shs"], t["opacities"], t["scales"], t["rotations"], sets,
+                                    raw_activations=True)
+    assert stand_ins == [("forward_views_raw", training, True)]
+    ref_c, _, ref_r, _ = _fake_outputs(V, True, False)
+    assert torch.equal(out["image"].detach(), ref_c.clamp(0, 1)) and torch.equal(out["radii"], ref_r)
+    assert out["image"].requires_grad == training
+
+
+def test_scene_views_rays_requiring_grad_keep_the_training_path(stand_ins, monkeypatch):
+    """rays get no gradient, but a call whose only grad-requiring input is rays built an autograd node before; it
+    still does."""
+    monkeypatch.setattr(MV, "epilogue_views_forward_raw", lambda *a: None)
+    t = _inputs()
+    rays = torch.zeros((1, H, W, 6), requires_grad=True)
+    out = MV.render_scene_views(t["means3D"], t["shs"], t["opacities"], t["scales"], t["rotations"], [_settings()],
+                                rays=rays)
+    assert stand_ins == [("forward_views_raw", True, False)]
+    assert out["image"].requires_grad
+
+
+def test_backward_of_a_forward_only_state_raises():
+    t = _inputs()
+    st = R.ForwardState(None, None, None, None, 0, 0, nviews=1, for_backward=False)
+    grad = torch.zeros((3, H, W)), torch.zeros((8, H, W))
+    with pytest.raises(RuntimeError, match="forward-only"):
+        R.backward_raw(st, torch.zeros(P, dtype=torch.int32), t["means3D"], t["shs"], None, t["scales"], t["rotations"],
+                       None, _settings(), *grad)
+    with pytest.raises(RuntimeError, match="for_backward=True"):
+        R.backward_views_raw(st, torch.zeros((1, P), dtype=torch.int32), t["means3D"], t["shs"], None, t["scales"],
+                             t["rotations"], None, torch.zeros((1, 24)), 0.5, 0.5, H, W, 0, *grad)
+
+
+def test_empty_forward_only_keeps_no_backward_state(monkeypatch):
+    """P = 0 returns before any CUDA call: zero outputs, and a state without image state or point list."""
+    monkeypatch.setattr(R, "_dev_index", lambda device: 0)
+    monkeypatch.setattr(R, "_capacity_hwm", {})
+    e = torch.empty((0, 3))
+    color, allmap, radii, st = R.forward_raw(e, torch.empty((0, 1, 3)), None, torch.empty((0, 1)), torch.empty((0, 2)),
+                                             torch.empty((0, 4)), None, _settings(), for_backward=False)
+    assert color.shape == (3, H, W) and allmap.shape == (8, H, W) and radii.shape == (0,)
+    assert not color.any() and not allmap.any()
+    assert st.image is None and st.point_list is None and not st.for_backward and st.num_rendered == 0
+    _, _, _, st_train = R.forward_raw(e, torch.empty((0, 1, 3)), None, torch.empty((0, 1)), torch.empty((0, 2)),
+                                      torch.empty((0, 4)), None, _settings())
+    assert st_train.for_backward and st_train.image is not None and st_train.geom.numel() == st.geom.numel()
