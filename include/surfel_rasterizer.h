@@ -8,9 +8,6 @@
  *     rasterize_gaussians_backward   -> srf_views_backward  (V = 1)
  *     mark_visible                   -> srf_mark_visible
  *
- * A render no gradient flows through (no_grad / inference_mode) calls srf_views_forward_inference instead:
- * the same outputs, bit for bit, without the state the backward needs (see "forward-only" below).
- *
  * which in turn call CudaRasterizer::Rasterizer::{forward,backward,markVisible}
  * (DSR/cuda_rasterizer/rasterizer.h:24-86) with raw pointers.  This header is the
  * raw-pointer level: plain C, device pointers + sizes + a cudaStream_t, int status
@@ -18,7 +15,9 @@
  * types, no allocation inside the library: the caller owns every buffer (the
  * reference's three growable byte blobs become caller-allocated workspaces whose
  * sizes srf_views_workspace_bytes reports).  All entry points only enqueue work on
- * `stream`; none of them synchronises.
+ * `stream`; none of them synchronises.  A render no gradient flows through
+ * (no_grad / inference_mode) passes for_backward = 0 to the forward: the same
+ * outputs, bit for bit, without the state the backward needs.
  *
  * Pointer conventions: every pointer is a CUDA device pointer unless it says "host".
  * Workspaces must be 256-byte aligned.  Matrices follow the reference:
@@ -35,7 +34,7 @@
 extern "C" {
 #endif
 
-#define SRF_ABI_VERSION 11
+#define SRF_ABI_VERSION 12
 
 /* cudaStream_t without pulling in cuda_runtime.h */
 typedef void* srf_stream_t;
@@ -71,8 +70,10 @@ const char* srf_last_error(void);
  *                    4*capacity rounded up to 256), the forward's contribution masks,
  *                    u32 [8][capacity] (36 B per instance of capacity in all); keep it from
  *                    forward to backward.
- *   [5] scratch    : srf_views_backward's scratch, one 80-byte gradient record per Gaussian and view. */
-int srf_views_workspace_bytes(int V, int P, int H, int W, size_t capacity, size_t bytes[6]);
+ *   [5] scratch    : srf_views_backward's scratch, one 80-byte gradient record per Gaussian and view.
+ * for_backward = 0 sizes the workspaces of a forward-only srf_views_forward (below): image and scratch are 0
+ * (not needed) and point_list is the list alone, 4 B per instance of capacity rounded up to 256 B per view. */
+int srf_views_workspace_bytes(int V, int P, int H, int W, size_t capacity, int for_backward, size_t bytes[6]);
 
 /* Byte offsets of the sub-arrays inside one view's workspaces (for tests / tooling that
  * inspect state the way the reference's blobs can be parsed).
@@ -101,7 +102,13 @@ int srf_state_layout(int P, int H, int W, size_t geom_off[3], size_t tile_off[5]
  * raw_activations != 0 (next-row extension, no reference counterpart): `opacities`, `scales`,
  * `rotations` are LaRa's raw network outputs and the kernel applies the activations of
  * lightning/renderer_2dgs.py:183-188 itself (sigmoid, exp, F.normalize); pass the same flag and the same
- * raw tensors to the backward, whose gradients are then wrt the raw parameters. */
+ * raw tensors to the backward, whose gradients are then wrt the raw parameters.
+ * for_backward = 0 (forward-only): the forward of a render that no backward will follow.  Same stages, same deferred
+ * counts and bit-identical out_color / out_others / radii, but the blend keeps no contribution record and writes no
+ * per-pixel image state, so `point_list` holds only the sorted list and `image_state` is not used (may be NULL); size
+ * the workspaces with srf_views_workspace_bytes(..., for_backward = 0, ...).  The state it leaves cannot feed
+ * srf_views_backward.
+ * Every argument check of both stages, including null or misaligned workspaces, is made before anything is enqueued. */
 int srf_views_forward(srf_stream_t stream, int V, int P, int D, int M,
                       const float* means3D, const float* shs, const float* colors_precomp,
                       const float* opacities, const float* scales, const float* rotations,
@@ -109,37 +116,13 @@ int srf_views_forward(srf_stream_t stream, int V, int P, int D, int M,
                       float tan_fovx, float tan_fovy, int image_height, int image_width, int prefiltered,
                       size_t capacity, int* radii, void* geom_state, void* tile_state, void* entries,
                       uint32_t* point_list, void* image_state, float* out_color, float* out_others,
-                      uint32_t* num_rendered_host, void* count_event, int raw_activations);
-/* stage 2 alone, on the state stage 1 left: the re-run with larger binning buffers */
+                      uint32_t* num_rendered_host, void* count_event, int raw_activations, int for_backward);
+/* stage 2 alone, on the state stage 1 left: the re-run with larger binning buffers; for_backward as given to the
+ * forward */
 int srf_views_forward_render(srf_stream_t stream, int V, int P, int image_height, int image_width,
                              size_t capacity, const void* geom_state, void* tile_state,
                              void* entries, uint32_t* point_list, void* image_state,
-                             const float* cams, float* out_color, float* out_others);
-
-/* ---- forward-only --------------------------------------------------------------------
- * The forward of a render that no backward will follow: same arguments, same stages, same deferred counts and
- * bit-identical out_color / out_others / radii as srf_views_forward, but the blend keeps no contribution record and
- * writes no per-pixel image state, so `point_list` holds only the sorted list and `image_state` is not used (may be
- * NULL).  Size the workspaces with srf_views_inference_workspace_bytes:
- *   bytes[0..4] = geom, tile, image (0: not needed), entries, point_list (4 B per instance of capacity,
- *   rounded up to 256 B, per view) -- totals for V views, as srf_views_workspace_bytes.
- * The state it leaves cannot feed srf_views_backward.  Null or misaligned workspaces are rejected before anything
- * is enqueued; the other argument checks and their messages are those of srf_views_forward.
- * srf_views_forward_inference_render is the stage-2 re-run for an overflowed capacity (as
- * srf_views_forward_render).                                                                                      */
-int srf_views_inference_workspace_bytes(int V, int P, int H, int W, size_t capacity, size_t bytes[5]);
-int srf_views_forward_inference(srf_stream_t stream, int V, int P, int D, int M,
-                                const float* means3D, const float* shs, const float* colors_precomp,
-                                const float* opacities, const float* scales, const float* rotations,
-                                const float* transMat_precomp, const float* cams,
-                                float tan_fovx, float tan_fovy, int image_height, int image_width, int prefiltered,
-                                size_t capacity, int* radii, void* geom_state, void* tile_state, void* entries,
-                                uint32_t* point_list, void* image_state, float* out_color, float* out_others,
-                                uint32_t* num_rendered_host, void* count_event, int raw_activations);
-int srf_views_forward_inference_render(srf_stream_t stream, int V, int P, int image_height, int image_width,
-                                       size_t capacity, const void* geom_state, void* tile_state,
-                                       void* entries, uint32_t* point_list, void* image_state,
-                                       const float* cams, float* out_color, float* out_others);
+                             const float* cams, float* out_color, float* out_others, int for_backward);
 
 /* ---- backward ------------------------------------------------------------------
  * Replaces Rasterizer::backward (rasterizer_impl.cu:346-448): BACKWARD::render,

@@ -14,7 +14,7 @@ from typing import Optional
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libsurfel_b200.so")
-ABI_VERSION = 11
+ABI_VERSION = 12
 CAM_FLOATS, CAM_VIEW, CAM_CAMPOS, CAM_BG = 24, 0, 16, 19      # include/surfel_rasterizer.h SRF_CAM_*
 
 
@@ -27,35 +27,29 @@ _A = POINTER(MsSsimAddr)
 
 # name -> (restype, argtypes); mirrors include/surfel_rasterizer.h one to one
 _P = c_void_p
-# srf_views_forward and srf_views_forward_inference
-_FORWARD = (c_int, [
-    _P, c_int, c_int, c_int, c_int,     # stream, V, P, D, M
-    _P, _P, _P,                         # means3D, shs, colors_precomp
-    _P, _P, _P,                         # opacities, scales, rotations
-    _P, _P,                             # transMat_precomp, cams
-    c_float, c_float, c_int, c_int,     # tan_fovx, tan_fovy, H, W
-    c_int, c_size_t,                    # prefiltered, capacity
-    _P, _P, _P, _P, _P, _P,             # radii, geom_state, tile_state, entries, point_list, image_state
-    _P, _P, _P, _P,                     # out_color, out_others, num_rendered_host, count_event
-    c_int,                              # raw_activations
-])
-# srf_views_forward_render and srf_views_forward_inference_render
-_FORWARD_RENDER = (c_int, [
-    _P, c_int, c_int, c_int, c_int,     # stream, V, P, H, W
-    c_size_t, _P, _P,                   # capacity, geom_state, tile_state
-    _P, _P, _P,                         # entries, point_list, image_state
-    _P, _P, _P,                         # cams, out_color, out_others
-])
 SIGNATURES = {
     "srf_abi_version": (c_int, []),
     "srf_last_error": (c_char_p, []),
-    "srf_views_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, c_size_t, POINTER(c_size_t)]),
+    "srf_views_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, c_size_t, c_int, POINTER(c_size_t)]),
     "srf_state_layout": (c_int, [c_int, c_int, c_int, POINTER(c_size_t), POINTER(c_size_t), POINTER(c_size_t)]),
-    "srf_views_forward": _FORWARD,
-    "srf_views_forward_render": _FORWARD_RENDER,
-    "srf_views_forward_inference": _FORWARD,
-    "srf_views_forward_inference_render": _FORWARD_RENDER,
-    "srf_views_inference_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, c_size_t, POINTER(c_size_t)]),
+    "srf_views_forward": (c_int, [
+        _P, c_int, c_int, c_int, c_int,     # stream, V, P, D, M
+        _P, _P, _P,                         # means3D, shs, colors_precomp
+        _P, _P, _P,                         # opacities, scales, rotations
+        _P, _P,                             # transMat_precomp, cams
+        c_float, c_float, c_int, c_int,     # tan_fovx, tan_fovy, H, W
+        c_int, c_size_t,                    # prefiltered, capacity
+        _P, _P, _P, _P, _P, _P,             # radii, geom_state, tile_state, entries, point_list, image_state
+        _P, _P, _P, _P,                     # out_color, out_others, num_rendered_host, count_event
+        c_int, c_int,                       # raw_activations, for_backward
+    ]),
+    "srf_views_forward_render": (c_int, [
+        _P, c_int, c_int, c_int, c_int,     # stream, V, P, H, W
+        c_size_t, _P, _P,                   # capacity, geom_state, tile_state
+        _P, _P, _P,                         # entries, point_list, image_state
+        _P, _P, _P,                         # cams, out_color, out_others
+        c_int,                              # for_backward
+    ]),
     "srf_views_backward": (c_int, [
         _P, c_int, c_int, c_int, c_int, c_int, c_int,   # stream, V, P, D, M, H, W
         c_size_t, _P,                            # capacity, cams
@@ -130,18 +124,11 @@ def check(status: int, lib=None) -> None:
         raise RuntimeError(msg)
 
 
-def views_sizes(lib, V: int, P: int, H: int, W: int, capacity: int):
-    """(geom, tile, image, entries, point_list, backward scratch) bytes for V back-to-back per-view workspaces."""
+def views_sizes(lib, V: int, P: int, H: int, W: int, capacity: int, for_backward: bool = True):
+    """(geom, tile, image, entries, point_list, backward scratch) bytes for V back-to-back per-view workspaces; with
+    ``for_backward=False`` those of a forward-only forward (image and scratch 0, a list-only point_list)."""
     b = (c_size_t * 6)()
-    check(lib.srf_views_workspace_bytes(V, P, H, W, capacity, b), lib)
-    return tuple(int(x) for x in b)
-
-
-def inference_sizes(lib, V: int, P: int, H: int, W: int, capacity: int):
-    """(geom, tile, image, entries, point_list) bytes of the forward-only entries' V back-to-back workspaces; image is
-    0 (not needed)."""
-    b = (c_size_t * 5)()
-    check(lib.srf_views_inference_workspace_bytes(V, P, H, W, capacity, b), lib)
+    check(lib.srf_views_workspace_bytes(V, P, H, W, capacity, 1 if for_backward else 0, b), lib)
     return tuple(int(x) for x in b)
 
 

@@ -79,14 +79,14 @@ T* at(const void* base, size_t off) {
 
 bool misaligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 255) != 0; }
 
-// One view's point_list workspace: the depth-sorted list (u32 [capacity]), then the blend forward's contribution
-// masks (u32 [8 warp blocks][capacity], indexed by list position), which the blend backward replays.
+// One view's point_list workspace: the depth-sorted list (u32 [capacity]), then, for a forward a backward follows, the
+// blend forward's contribution masks (u32 [8 warp blocks][capacity], indexed by list position), which the blend
+// backward replays.
 size_t plist_masks_offset(size_t capacity) { return align_up(capacity * sizeof(uint32_t)); }
-size_t plist_stride_bytes(size_t capacity) {
+size_t plist_stride_bytes(size_t capacity, bool for_backward) {
+    if (!for_backward) return plist_masks_offset(capacity);
     return plist_masks_offset(capacity) + align_up(capacity * 8 * sizeof(uint32_t)) + 256;
 }
-// The forward-only entries' point_list workspace: the list alone.
-size_t inference_plist_stride_bytes(size_t capacity) { return align_up(capacity * sizeof(uint32_t)); }
 size_t entries_stride_bytes(size_t capacity) { return align_up(capacity * sizeof(uint64_t)) + 256; }
 size_t ggrad_stride_bytes(int P) { return align_up((size_t)P * SRF_GRAD_FLOATS * sizeof(float)) + 256; }
 
@@ -173,24 +173,14 @@ int srf_profile_end(float* ms_out, int* launches_out, int n) {
 }
 const char* srf_last_error(void) { return g_err; }
 
-int srf_views_workspace_bytes(int V, int P, int H, int W, size_t capacity, size_t bytes[6]) {
+int srf_views_workspace_bytes(int V, int P, int H, int W, size_t capacity, int for_backward, size_t bytes[6]) {
     if (V <= 0 || P < 0 || H <= 0 || W <= 0 || !bytes) return fail("srf_views_workspace_bytes: bad arguments");
     bytes[0] = geom_layout(P).total * (size_t)V;
     bytes[1] = tile_layout(H, W).total * (size_t)V;
-    bytes[2] = image_layout(H, W).total * (size_t)V;
+    bytes[2] = for_backward ? image_layout(H, W).total * (size_t)V : 0;
     bytes[3] = entries_stride_bytes(capacity) * (size_t)V;
-    bytes[4] = plist_stride_bytes(capacity) * (size_t)V;
-    bytes[5] = ggrad_stride_bytes(P) * (size_t)V;
-    return 0;
-}
-
-int srf_views_inference_workspace_bytes(int V, int P, int H, int W, size_t capacity, size_t bytes[5]) {
-    if (V <= 0 || P < 0 || H <= 0 || W <= 0 || !bytes) return fail("srf_views_inference_workspace_bytes: bad arguments");
-    bytes[0] = geom_layout(P).total * (size_t)V;
-    bytes[1] = tile_layout(H, W).total * (size_t)V;
-    bytes[2] = 0;
-    bytes[3] = entries_stride_bytes(capacity) * (size_t)V;
-    bytes[4] = inference_plist_stride_bytes(capacity) * (size_t)V;
+    bytes[4] = plist_stride_bytes(capacity, for_backward != 0) * (size_t)V;
+    bytes[5] = for_backward ? ggrad_stride_bytes(P) * (size_t)V : 0;
     return 0;
 }
 
@@ -260,17 +250,14 @@ int forward_preprocess_check(const char* fn, int V, int P, int D, int M,
     return 0;
 }
 
-// stage 1: preprocess, per-tile counting, tile scan and the count read-back
-int forward_preprocess_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int M,
+// stage 1: preprocess, per-tile counting, tile scan and the count read-back (arguments checked by the caller)
+int forward_preprocess_impl(cudaStream_t stream, int V, int P, int D, int M,
                             const float* means3D, const float* shs, const float* colors_precomp,
                             const float* opacities, const float* scales, const float* rotations,
                             const float* transMat_precomp, const float* cams,
                             float tan_fovx, float tan_fovy, int image_height, int image_width,
                             int prefiltered, int* radii, void* geom_state, void* tile_state,
                             uint32_t* num_rendered_host, int raw_activations) {
-    if (forward_preprocess_check(fn, V, P, D, M, means3D, shs, colors_precomp, opacities, scales, rotations,
-                                 transMat_precomp, image_height, image_width, radii, geom_state, tile_state))
-        return 1;
     const TileLayout tl = tile_layout(image_height, image_width);
     // tile blocks + counters of every view are zeroed by one 2-D memset
     cudaError_t e = cudaMemset2DAsync(at<char>(tile_state, tl.count), tl.total, 0,
@@ -327,7 +314,7 @@ int forward_preprocess_impl(const char* fn, cudaStream_t stream, int V, int P, i
     return 0;
 }
 
-// argument checks of stage 2; `record` = false (forward-only) needs no image_state
+// argument checks of stage 2, all made before anything is enqueued; `record` = false (forward-only) needs no image_state
 int forward_render_check(const char* fn, int V, int P, int image_height, int image_width, size_t capacity,
                          const void* geom_state, const void* tile_state, const void* entries, const uint32_t* point_list,
                          const void* image_state, const float* cams, const float* out_color, const float* out_others, bool record) {
@@ -336,24 +323,19 @@ int forward_render_check(const char* fn, int V, int P, int image_height, int ima
         return fail("%s: null required pointer", fn);
     if (capacity > 0xfffffff0ull) return fail("%s: capacity exceeds 32-bit instance indices", fn);
     if (capacity > 0 && (!entries || !point_list)) return fail("%s: null binning buffers", fn);
-    if (!record) {
-        if (P > 0 && (!geom_state || misaligned(geom_state))) return fail("%s: geom_state must be 256-byte aligned", fn);
-        if (misaligned(tile_state)) return fail("%s: tile_state must be 256-byte aligned", fn);
-        if (capacity > 0 && (misaligned(entries) || misaligned(point_list)))
-            return fail("%s: entries and point_list must be 256-byte aligned", fn);
-    }
+    if (P > 0 && (!geom_state || misaligned(geom_state))) return fail("%s: geom_state must be 256-byte aligned", fn);
+    if (misaligned(tile_state)) return fail("%s: tile_state must be 256-byte aligned", fn);
+    if (capacity > 0 && (misaligned(entries) || misaligned(point_list)))
+        return fail("%s: entries and point_list must be 256-byte aligned", fn);
     return 0;
 }
 
-// stage 2: scatter into tile buckets, per-tile depth sort, blend (record = false: the forward-only blend, no
-// contribution record and no image state)
-int forward_render_impl(const char* fn, cudaStream_t stream, int V, int P, int image_height, int image_width,
+// stage 2: scatter into tile buckets, per-tile depth sort, blend (arguments checked by the caller; record = false: the
+// forward-only blend, no contribution record and no image state)
+int forward_render_impl(cudaStream_t stream, int V, int P, int image_height, int image_width,
                         size_t capacity, const void* geom_state, void* tile_state,
                         void* entries, uint32_t* point_list, void* image_state,
                         const float* cams, float* out_color, float* out_others, bool record) {
-    if (forward_render_check(fn, V, P, image_height, image_width, capacity, geom_state, tile_state, entries, point_list,
-                             image_state, cams, out_color, out_others, record))
-        return 1;
     const TileLayout tl = tile_layout(image_height, image_width);
     const ImageLayout il = image_layout(image_height, image_width);
     const GeomLayout gl = geom_layout(P);
@@ -365,10 +347,9 @@ int forward_render_impl(const char* fn, cudaStream_t stream, int V, int P, int i
     b.point_list = point_list;
     b.geom_stride = gl.total;
     b.entries_stride = entries_stride_bytes(capacity);
-    b.plist_stride = record ? plist_stride_bytes(capacity) : inference_plist_stride_bytes(capacity);
+    b.plist_stride = plist_stride_bytes(capacity, record);
     cudaError_t e;
     if (P > 0) {
-        if (!geom_state) return fail("%s: null geom_state", fn);
         // culled Gaussians carry an empty rect, so the radii array is not needed here
         b.depths = at<float>(geom_state, gl.depths);
         b.rects = at<uint2>(geom_state, gl.rects);
@@ -448,7 +429,7 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
     r.dL_dpix = dL_dout_color;
     r.dL_dothers = dL_dout_others;
     r.ggrad = static_cast<float*>(scratch);
-    r.geom_stride = gl.total; r.tile_stride = tl.total; r.plist_stride = plist_stride_bytes(capacity);
+    r.geom_stride = gl.total; r.tile_stride = tl.total; r.plist_stride = plist_stride_bytes(capacity, true);
     r.image_stride = il.total; r.ggrad_stride = gstride;
     r.cam_stride = SRF_CAM_FLOATS;
     if (deterministic) {
@@ -499,11 +480,16 @@ int srf_views_forward(srf_stream_t stream_, int V, int P, int D, int M,
                       float tan_fovx, float tan_fovy, int image_height, int image_width, int prefiltered,
                       size_t capacity, int* radii, void* geom_state, void* tile_state, void* entries,
                       uint32_t* point_list, void* image_state, float* out_color, float* out_others,
-                      uint32_t* num_rendered_host, void* count_event, int raw_activations) {
+                      uint32_t* num_rendered_host, void* count_event, int raw_activations, int for_backward) {
     const char* fn = "srf_views_forward";
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    if (!cams) return fail("%s: null camera records", fn);
-    int rc = forward_preprocess_impl(fn, stream, V, P, D, M, means3D, shs, colors_precomp, opacities, scales, rotations,
+    // the checks of both stages before stage 1 enqueues anything
+    if (forward_preprocess_check(fn, V, P, D, M, means3D, shs, colors_precomp, opacities, scales, rotations,
+                                 transMat_precomp, image_height, image_width, radii, geom_state, tile_state) ||
+        forward_render_check(fn, V, P, image_height, image_width, capacity, geom_state, tile_state, entries, point_list,
+                             image_state, cams, out_color, out_others, for_backward != 0))
+        return 1;
+    int rc = forward_preprocess_impl(stream, V, P, D, M, means3D, shs, colors_precomp, opacities, scales, rotations,
                                      transMat_precomp, cams, tan_fovx, tan_fovy, image_height, image_width, prefiltered,
                                      radii, geom_state, tile_state, num_rendered_host, raw_activations);
     if (rc != 0) return rc;
@@ -511,55 +497,20 @@ int srf_views_forward(srf_stream_t stream_, int V, int P, int D, int M,
         cudaError_t e = cudaEventRecord(static_cast<cudaEvent_t>(count_event), stream);
         if (e != cudaSuccess) return cuda_fail("count event record", e);
     }
-    return forward_render_impl(fn, stream, V, P, image_height, image_width, capacity, geom_state, tile_state, entries,
-                               point_list, image_state, cams, out_color, out_others, true);
+    return forward_render_impl(stream, V, P, image_height, image_width, capacity, geom_state, tile_state, entries,
+                               point_list, image_state, cams, out_color, out_others, for_backward != 0);
 }
 
 int srf_views_forward_render(srf_stream_t stream_, int V, int P, int image_height, int image_width,
                              size_t capacity, const void* geom_state, void* tile_state,
                              void* entries, uint32_t* point_list, void* image_state,
-                             const float* cams, float* out_color, float* out_others) {
-    return forward_render_impl("srf_views_forward_render", static_cast<cudaStream_t>(stream_), V, P, image_height,
-                               image_width, capacity, geom_state, tile_state, entries, point_list, image_state,
-                               cams, out_color, out_others, true);
-}
-
-int srf_views_forward_inference(srf_stream_t stream_, int V, int P, int D, int M,
-                                const float* means3D, const float* shs, const float* colors_precomp,
-                                const float* opacities, const float* scales, const float* rotations,
-                                const float* transMat_precomp, const float* cams,
-                                float tan_fovx, float tan_fovy, int image_height, int image_width, int prefiltered,
-                                size_t capacity, int* radii, void* geom_state, void* tile_state, void* entries,
-                                uint32_t* point_list, void* image_state, float* out_color, float* out_others,
-                                uint32_t* num_rendered_host, void* count_event, int raw_activations) {
-    const char* fn = "srf_views_forward_inference";
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    if (!cams) return fail("%s: null camera records", fn);
-    // the checks of both stages (in the order srf_views_forward makes them) before stage 1 enqueues anything
-    if (forward_preprocess_check(fn, V, P, D, M, means3D, shs, colors_precomp, opacities, scales, rotations,
-                                 transMat_precomp, image_height, image_width, radii, geom_state, tile_state) ||
-        forward_render_check(fn, V, P, image_height, image_width, capacity, geom_state, tile_state, entries, point_list,
-                             image_state, cams, out_color, out_others, false))
+                             const float* cams, float* out_color, float* out_others, int for_backward) {
+    if (forward_render_check("srf_views_forward_render", V, P, image_height, image_width, capacity, geom_state,
+                             tile_state, entries, point_list, image_state, cams, out_color, out_others, for_backward != 0))
         return 1;
-    int rc = forward_preprocess_impl(fn, stream, V, P, D, M, means3D, shs, colors_precomp, opacities, scales, rotations,
-                                     transMat_precomp, cams, tan_fovx, tan_fovy, image_height, image_width, prefiltered,
-                                     radii, geom_state, tile_state, num_rendered_host, raw_activations);
-    if (rc != 0) return rc;
-    if (count_event) {
-        cudaError_t e = cudaEventRecord(static_cast<cudaEvent_t>(count_event), stream);
-        if (e != cudaSuccess) return cuda_fail("count event record", e);
-    }
-    return forward_render_impl(fn, stream, V, P, image_height, image_width, capacity, geom_state, tile_state, entries,
-                               point_list, nullptr, cams, out_color, out_others, false);
-}
-
-int srf_views_forward_inference_render(srf_stream_t stream_, int V, int P, int image_height, int image_width,
-                                       size_t capacity, const void* geom_state, void* tile_state,
-                                       void* entries, uint32_t* point_list, void* image_state,
-                                       const float* cams, float* out_color, float* out_others) {
-    return forward_render_impl("srf_views_forward_inference_render", static_cast<cudaStream_t>(stream_), V, P,
-                               image_height, image_width, capacity, geom_state, tile_state, entries, point_list,
-                               image_state, cams, out_color, out_others, false);
+    return forward_render_impl(static_cast<cudaStream_t>(stream_), V, P, image_height, image_width, capacity, geom_state,
+                               tile_state, entries, point_list, image_state, cams, out_color, out_others,
+                               for_backward != 0);
 }
 
 int srf_views_backward(srf_stream_t stream_, int V, int P, int D, int M, int image_height, int image_width,

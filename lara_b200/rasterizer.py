@@ -77,11 +77,11 @@ def _f32c(t: torch.Tensor, name: str) -> torch.Tensor:
 
 
 def _views_sizes(lib, V: int, P: int, H: int, W: int, capacity: int, for_backward: bool = True):
-    """srf_views_workspace_bytes (six sizes), or with for_backward=False srf_views_inference_workspace_bytes (five)."""
+    """srf_views_workspace_bytes: the six sizes, those of a forward-only forward with for_backward=False."""
     key = (V, P, H, W, capacity, for_backward)
     v = _size_cache.get(key)
     if v is None:
-        v = (_lib.views_sizes if for_backward else _lib.inference_sizes)(lib, V, P, H, W, capacity)
+        v = _lib.views_sizes(lib, V, P, H, W, capacity, for_backward)
         if len(_size_cache) > 64:
             _size_cache.clear()
         _size_cache[key] = v
@@ -322,8 +322,8 @@ def forward_views_raw(means3D, shs, colors_precomp, opacities, scales, rotations
     """All V views of one Gaussian set in ONE launch set (srf_views_*): every kernel carries a view
     dimension.  `cams` is the [V, 24] device tensor of camera records (pack_cameras).
     Returns (color [V,3,H,W], allmap [V,8,H,W], radii [V,P], ForwardState with V back-to-back workspaces).
-    ``for_backward=False``: the forward-only entries (srf_views_forward_inference), bit-identical outputs without the
-    blend's contribution record and image state; the returned state cannot feed :func:`backward_views_raw`."""
+    ``for_backward=False``: the forward-only forward (srf_views_forward with for_backward = 0), bit-identical outputs
+    without the blend's contribution record and image state; the returned state cannot feed :func:`backward_views_raw`."""
     with _DeviceGuard(means3D.device):
         if cams.dtype != torch.float32 or not cams.is_cuda or cams.shape[1] != _lib.CAM_FLOATS or not cams.is_contiguous():
             raise RuntimeError(f"cams must be a contiguous float32 CUDA tensor [V,{_lib.CAM_FLOATS}]")
@@ -336,8 +336,8 @@ def _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMa
              H, W, sh_degree, prefiltered, debug, raw_activations, single, for_backward):
     """srf_views_forward on the current stream: stage 1 (preprocess + tile scan + async count read-back) and stage 2
     (binning + blend) with an optimistic capacity, then an event for whoever eventually asks for the instance counts.
-    `single`: one view, with the outputs in the reference's one-view shapes.  `for_backward` False: the
-    srf_views_forward_inference pair of entries and their smaller workspaces, no image state or point list kept."""
+    `single`: one view, with the outputs in the reference's one-view shapes.  `for_backward` False: the forward-only
+    forward and its smaller workspaces, no image state or point list kept."""
     lib = _lib.load()
     device = means3D.device
     V, P = int(cams.shape[0]), int(means3D.shape[0])
@@ -373,15 +373,13 @@ def _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMa
     # the tile scan, never for the blend.
     # the forward-only point list and entries are scratch of this call: they go back to the caching allocator when
     # it returns, stream-ordered behind the kernels that use them
-    fwd, fwd_render = ((lib.srf_views_forward, lib.srf_views_forward_render) if for_backward else
-                       (lib.srf_views_forward_inference, lib.srf_views_forward_inference_render))
-    _lib.check(fwd(
+    _lib.check(lib.srf_views_forward(
         _raw_stream(device), V, P, int(sh_degree), M, _ptr(means3D), _ptr(shs), _ptr(colors_precomp),
         _ptr(opacities), _ptr(scales), _ptr(rotations), _ptr(transMat_precomp), cams.data_ptr(),
         float(tanfovx), float(tanfovy), H, W, 1 if prefiltered else 0, capacity,
         radii.data_ptr(), geom.data_ptr(), tile.data_ptr(), _blob(ent_b, device).data_ptr(), point_list.data_ptr(),
         _ptr(image), color.data_ptr(), allmap.data_ptr(), slot.data_ptr(), ev.cuda_event,
-        1 if raw_activations else 0), lib)
+        1 if raw_activations else 0, 1 if for_backward else 0), lib)
     state = ForwardState(geom, tile, image, point_list if for_backward else None, capacity, nviews=V, cams=cams,
                          for_backward=for_backward)
 
@@ -390,10 +388,10 @@ def _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMa
         with _DeviceGuard(device):
             e_b, p_b = _views_sizes(lib, V, P, H, W, new_capacity, for_backward)[3:5]
             pl2 = _blob(p_b, device)
-            _lib.check(fwd_render(
+            _lib.check(lib.srf_views_forward_render(
                 _raw_stream(device), V, P, H, W, new_capacity, geom.data_ptr(), tile.data_ptr(),
                 _blob(e_b, device).data_ptr(), pl2.data_ptr(), _ptr(image), cams.data_ptr(), color.data_ptr(),
-                allmap.data_ptr()), lib)
+                allmap.data_ptr(), 1 if for_backward else 0), lib)
             state.capacity = new_capacity
             if for_backward:
                 state.point_list = pl2

@@ -1,7 +1,10 @@
-"""Forward-only rendering, host side (no GPU needed): the srf_views_forward_inference entries and their workspace query,
-their argument checks, and the rule by which the public wrappers pick the forward-only path -- taken iff no gradient can
-flow (grad mode off, or no tensor input requires grad) -- driven with stand-ins for the raw forward functions."""
+"""Forward-only rendering, host side (no GPU needed): the for_backward flag of srf_views_forward, its stage-2 re-run and
+the workspace query, their argument checks, and the rule by which the public wrappers pick the forward-only path --
+taken iff no gradient can flow (grad mode off, or no tensor input requires grad) -- driven with stand-ins for the raw
+forward functions."""
 import ctypes
+import os
+import re
 
 import pytest
 import torch
@@ -10,66 +13,76 @@ from lara_b200 import _lib
 from lara_b200 import multiview as MV
 from lara_b200 import rasterizer as R
 
-from test_abi import declared_symbols
+from test_abi import ROOT, declared_symbols
 
-NEW = ("srf_views_forward_inference", "srf_views_forward_inference_render", "srf_views_inference_workspace_bytes")
+# the forward-only twins of ABI 11, folded into the flag
+REMOVED = ("srf_views_forward_inference", "srf_views_forward_inference_render", "srf_views_inference_workspace_bytes")
 
 
 def align256(x):
     return (x + 255) // 256 * 256
 
 
-def test_new_entries_are_declared_exported_and_bound(lib):
+def test_forward_only_is_a_flag_of_the_forward_entries(lib):
     syms = declared_symbols()
-    for name in NEW:
-        assert name in syms and name in _lib.SIGNATURES and hasattr(lib, name), name
-    # the forward-only twins take exactly the training entries' arguments
-    assert _lib.SIGNATURES["srf_views_forward_inference"] == _lib.SIGNATURES["srf_views_forward"]
-    assert _lib.SIGNATURES["srf_views_forward_inference_render"] == _lib.SIGNATURES["srf_views_forward_render"]
-    assert lib.srf_abi_version() == _lib.ABI_VERSION == 11
+    for name in REMOVED:
+        assert name not in syms and name not in _lib.SIGNATURES and not hasattr(lib, name), name
+    assert lib.srf_abi_version() == _lib.ABI_VERSION == 12
+    header = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "surfel_rasterizer.h")).read(), flags=re.S)
+    header = re.sub(r"\s+", " ", header)
+    for name in ("srf_views_forward", "srf_views_forward_render"):
+        assert re.search(rf"\b{name}\([^;]*, int for_backward\);", header), name
+        assert _lib.SIGNATURES[name][1][-1] is ctypes.c_int, name
+    assert "srf_views_workspace_bytes(int V, int P, int H, int W, size_t capacity, int for_backward, size_t bytes[6]);" \
+        in header
 
 
 @pytest.mark.parametrize("V,P,H,W,capacity", [(1, 1000, 300, 500, 12345), (8, 131072, 512, 512, 1 << 20),
                                               (48, 524288, 512, 512, 8 * 524288), (3, 0, 16, 16, 0)])
-def test_inference_workspace_sizes(lib, V, P, H, W, capacity):
-    geom, tile, image, entries, plist = _lib.inference_sizes(lib, V, P, H, W, capacity)
-    tg, tt, ti, te, tp, _ = _lib.views_sizes(lib, V, P, H, W, capacity)
+def test_forward_only_workspace_sizes(lib, V, P, H, W, capacity):
+    geom, tile, image, entries, plist, scratch = _lib.views_sizes(lib, V, P, H, W, capacity, for_backward=False)
+    tg, tt, ti, te, tp, _ = _lib.views_sizes(lib, V, P, H, W, capacity, for_backward=True)
     assert plist == align256(4 * capacity) * V
     assert 8 * plist <= tp
     assert tp - plist >= 32 * capacity * V              # the contribution record is what goes
     assert image == 0 and ti > 0
+    assert scratch == 0
     assert (geom, tile, entries) == (tg, tt, te)
 
 
-def test_inference_workspace_query_rejects_bad_arguments(lib):
-    n = (ctypes.c_size_t * 5)()
-    for args in [(0, 1, 16, 16, 0), (1, -1, 16, 16, 0), (1, 0, 0, 16, 0), (1, 0, 16, -2, 0)]:
-        assert lib.srf_views_inference_workspace_bytes(*args, n) != 0
-        assert b"srf_views_inference_workspace_bytes: bad arguments" == lib.srf_last_error()
-    assert lib.srf_views_inference_workspace_bytes(1, 0, 16, 16, 0, None) != 0
+def test_workspace_query_rejects_bad_arguments_with_either_flag(lib):
+    n = (ctypes.c_size_t * 6)()
+    for for_backward in (0, 1):
+        for args in [(0, 1, 16, 16, 0), (1, -1, 16, 16, 0), (1, 0, 0, 16, 0), (1, 0, 16, -2, 0)]:
+            assert lib.srf_views_workspace_bytes(*args, for_backward, n) != 0
+            assert b"srf_views_workspace_bytes: bad arguments" == lib.srf_last_error()
+        assert lib.srf_views_workspace_bytes(1, 0, 16, 16, 0, for_backward, None) != 0
 
 
-def _forward_args(V=1, P=4, D=0, H=16, W=16, capacity=0, geom=None, tile=None, entries=None, plist=None, out=None):
+def _forward_args(V=1, P=4, D=0, H=16, W=16, capacity=0, geom=None, tile=None, entries=None, plist=None, image=None,
+                  out=None, for_backward=0):
     cams = (ctypes.c_float * 24)()
     args = [None, V, P, D, 1, None, None, None, None, None, None, None, ctypes.addressof(cams),
-            1.0, 1.0, H, W, 0, capacity, None, geom, tile, entries, plist, None, out, out, None, None, 0]
+            1.0, 1.0, H, W, 0, capacity, None, geom, tile, entries, plist, image, out, out, None, None, 0, for_backward]
     return args, cams
 
 
 @pytest.mark.parametrize("case", [dict(V=0), dict(H=16 * 65535 + 1), dict(), dict(tile=0x1010),
                                   dict(tile=0x1000, D=4)])
-def test_forward_inference_rejects_what_the_training_forward_rejects(lib, case):
-    """Same arguments, same message (but for the entry's name); every case fails before anything is enqueued."""
-    args, _cams = _forward_args(**case)
-    assert lib.srf_views_forward(*args) != 0
-    train = lib.srf_last_error().decode()
-    assert lib.srf_views_forward_inference(*args) != 0
-    inf = lib.srf_last_error().decode()
-    assert train.startswith("srf_views_forward: ") and inf == train.replace("srf_views_forward", "srf_views_forward_inference")
+def test_forward_only_rejects_what_the_training_forward_rejects(lib, case):
+    """Same arguments, the same message byte for byte with either flag; every case fails before anything is
+    enqueued."""
+    msgs = []
+    for for_backward in (0, 1):
+        args, _cams = _forward_args(**case, for_backward=for_backward)
+        assert lib.srf_views_forward(*args) != 0
+        msgs.append(lib.srf_last_error())
+    assert msgs[0].startswith(b"srf_views_forward: ") and msgs[0] == msgs[1]
 
 
-def test_forward_inference_rejects_null_or_misaligned_workspaces_before_any_cuda_call(lib):
-    """Without a device any CUDA call would fail with a CUDA error; these fail with the argument check's message."""
+def test_forward_rejects_null_or_misaligned_workspaces_before_any_cuda_call(lib):
+    """Without a device any CUDA call would fail with a CUDA error; these fail with the argument check's message, with
+    either flag: the checks of both stages come before stage 1 enqueues anything."""
     x = 0x10000          # a 256-byte aligned address that is never dereferenced: every call below fails its checks
     cases = [
         (dict(P=0, tile=x, capacity=64, entries=x, plist=None, out=x), "null binning buffers"),
@@ -77,24 +90,33 @@ def test_forward_inference_rejects_null_or_misaligned_workspaces_before_any_cuda
         (dict(P=0, tile=x, capacity=64, entries=x + 8, plist=x, out=x), "entries and point_list must be 256-byte aligned"),
         (dict(P=0, tile=x, capacity=64, entries=x, plist=x, out=None), "null required pointer"),
     ]
-    for kw, msg in cases:
-        args, _cams = _forward_args(**kw)
-        assert lib.srf_views_forward_inference(*args) != 0
-        assert lib.srf_last_error().decode() == f"srf_views_forward_inference: {msg}", kw
+    for for_backward in (0, 1):
+        # the training forward needs an image_state; the forward-only one does not use it
+        image = x if for_backward else None
+        for kw, msg in cases:
+            args, _cams = _forward_args(**kw, image=image, for_backward=for_backward)
+            assert lib.srf_views_forward(*args) != 0
+            assert lib.srf_last_error().decode() == f"srf_views_forward: {msg}", (kw, for_backward)
+    args, _cams = _forward_args(P=0, tile=x, capacity=64, entries=x, plist=x, out=x, image=None, for_backward=1)
+    assert lib.srf_views_forward(*args) != 0
+    assert lib.srf_last_error() == b"srf_views_forward: null required pointer"
+
+    # stage 2 alone: a misaligned geom_state or point_list is rejected; image_state may be NULL when forward-only
     cams = (ctypes.c_float * 24)()
-    # stage 2 alone: image_state may be NULL, a misaligned geom_state or point_list is rejected
-    render = [None, 1, 4, 16, 16, 64, x + 16, x, x, x, None, ctypes.addressof(cams), x, x]
-    assert lib.srf_views_forward_inference_render(*render) != 0
-    assert lib.srf_last_error() == b"srf_views_forward_inference_render: geom_state must be 256-byte aligned"
-    render[6], render[9] = x, x + 4
-    assert lib.srf_views_forward_inference_render(*render) != 0
-    assert lib.srf_last_error() == b"srf_views_forward_inference_render: entries and point_list must be 256-byte aligned"
-    render[1] = 0
-    assert lib.srf_views_forward_inference_render(*render) != 0
-    assert lib.srf_last_error() == b"srf_views_forward_inference_render: bad sizes"
-    render[1], render[2], render[10], render[11] = 1, 0, None, None
-    assert lib.srf_views_forward_inference_render(*render) != 0
-    assert lib.srf_last_error() == b"srf_views_forward_inference_render: null required pointer"
+    for for_backward in (0, 1):
+        image = x if for_backward else None
+        render = [None, 1, 4, 16, 16, 64, x + 16, x, x, x, image, ctypes.addressof(cams), x, x, for_backward]
+        assert lib.srf_views_forward_render(*render) != 0
+        assert lib.srf_last_error() == b"srf_views_forward_render: geom_state must be 256-byte aligned"
+        render[6], render[9] = x, x + 4
+        assert lib.srf_views_forward_render(*render) != 0
+        assert lib.srf_last_error() == b"srf_views_forward_render: entries and point_list must be 256-byte aligned"
+        render[1] = 0
+        assert lib.srf_views_forward_render(*render) != 0
+        assert lib.srf_last_error() == b"srf_views_forward_render: bad sizes"
+        render[1], render[2], render[10], render[11] = 1, 0, None, None
+        assert lib.srf_views_forward_render(*render) != 0
+        assert lib.srf_last_error() == b"srf_views_forward_render: null required pointer"
 
 
 # ---------------------------------------------------------------------------------------------- selection rule

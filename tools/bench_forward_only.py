@@ -1,6 +1,6 @@
-"""What the forward-only path saves (DESIGN §3.14): the training forward (srf_views_forward, with the contribution
-record and the image state the backward reads) against the forward-only one (srf_views_forward_inference) on the same
-inputs, alternated in one process.
+"""What the forward-only path saves (DESIGN §3.14): the training forward (srf_views_forward with for_backward = 1, with
+the contribution record and the image state the backward reads) against the forward-only one (for_backward = 0) on the
+same inputs, alternated in one process.
 
 Per point: the whole call (forward_views_raw, enqueue to completion) timed with CUDA events, the mean of --iters calls
 in each of --rounds alternations, the blend forward's device time per view (srf_profile_*, render_fwd), and the peak of
