@@ -24,6 +24,8 @@ class MsSsimAddr(Structure):
 
 
 _A = POINTER(MsSsimAddr)
+_I3 = POINTER(c_int)            # host int[3]
+MESH_CAM_FLOATS = 24            # include/surfel_mesh.h SRF_MESH_CAM_FLOATS
 
 # name -> (restype, argtypes); mirrors include/surfel_rasterizer.h one to one
 _P = c_void_p
@@ -81,6 +83,12 @@ SIGNATURES = {
     "srf_ms_ssim_forward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _A, _P, _A, c_float, c_int, _P, _P]),
     "srf_ms_ssim_backward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _A, _P, _A, c_float, c_int, _P, _P, _P, _A]),
     "srf_mark_visible": (c_int, [_P, c_int, _P, _P, _P, _P]),
+    # include/surfel_mesh.h
+    "srf_tsdf_integrate": (c_int, [_P, _I3, _I3, c_float, c_float, _P, _P, _P, c_int, c_int, c_int, _P, _P, _P, _P,
+                                   c_float]),
+    "srf_mesh_workspace_bytes": (c_int, [_I3, POINTER(c_size_t)]),
+    "srf_mesh_count": (c_int, [_P, _I3, _P, _P, _P, _P]),
+    "srf_mesh_emit": (c_int, [_P, _I3, _I3, c_float, _P, _P, _P, c_int, c_int, _P, _P, _P]),
     "srf_profile_begin": (c_int, []),
     "srf_profile_end": (c_int, [POINTER(c_float), POINTER(c_int), c_int]),
 }
@@ -165,6 +173,15 @@ def deterministic(requested: Optional[bool] = None) -> bool:
     import torch
     return use_deterministic(requested, torch.are_deterministic_algorithms_enabled(),
                              torch.is_deterministic_algorithms_warn_only_enabled())
+
+
+def int3(v) -> ctypes.Array:
+    """A host int[3] (the mesh entries' n0 / dims)."""
+    return (c_int * 3)(*(int(x) for x in v))
+
+
+def mesh_workspace_bytes(lib, dims) -> int:
+    return _size_query(lib.srf_mesh_workspace_bytes, int3(dims))
 
 
 def layout(lib, P: int, H: int, W: int):

@@ -9,10 +9,24 @@
 // SRF_CAM_*), the records `cam_stride` floats apart.  Images are stacked [V,C,H,W].
 #pragma once
 #include <cuda_runtime.h>
+#include <stdarg.h>
 #include <stdint.h>
 #include <stdio.h>
 
+extern "C" const char* srf_last_error(void);
+
 namespace srf {
+
+// Report a failure from a translation unit other than api.cu: the text goes to the thread-local buffer srf_last_error()
+// returns (api.cu's, kErrorBytes long).  Returns 1, the C ABI's failure status.
+constexpr size_t kErrorBytes = 512;
+inline int set_error(const char* fmt, ...) {
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(const_cast<char*>(srf_last_error()), kErrorBytes, fmt, ap);
+    va_end(ap);
+    return 1;
+}
 
 // pointer of view `v` given the pointer of view 0 and a byte stride
 template <typename T>

@@ -113,3 +113,39 @@ def settings_for(cam: Camera, bg: torch.Tensor, sh_degree: int, device, settings
         tanfovx=cam.tanfovx, tanfovy=cam.tanfovy, bg=bg.to(device),
         scale_modifier=1.0, viewmatrix=cam.viewmatrix.to(device), projmatrix=cam.projmatrix.to(device),
         sh_degree=sh_degree, campos=cam.campos.to(device), prefiltered=False, debug=debug)
+
+
+class PathCamera:
+    """A camera with the attributes and ``get_rays`` of LaRa's ``tools/camera.MiniCam`` (tools/camera.py:21-56), which
+    ``MeshExtractor`` and ``Renderer.render_views`` read; ``c2w`` in OpenCV axes."""
+
+    def __init__(self, c2w: torch.Tensor, H: int, W: int, fov: float, znear: float = 0.5, zfar: float = 2.5):
+        cam = camera_from_c2w(c2w, H, W, fov, fov, znear, zfar)
+        self.image_width, self.image_height, self.FoVx, self.FoVy = W, H, fov, fov
+        self.world_view_transform = cam.viewmatrix
+        self.full_proj_transform = cam.projmatrix
+        self.camera_center = cam.campos
+        self.c2w = c2w
+
+    def to_device(self, device):
+        self.world_view_transform = self.world_view_transform.to(device)
+        self.full_proj_transform = self.full_proj_transform.to(device)
+        self.camera_center = self.camera_center.to(device)
+
+    def get_rays(self) -> torch.Tensor:
+        """[1,H,W,6] origins | directions through pixel centres, as LaRa's build_rays (dataLoader/utils.py:21-34)."""
+        H, W = self.image_height, self.image_width
+        f = 0.5 * W / math.tan(0.5 * self.FoVx), 0.5 * H / math.tan(0.5 * self.FoVy)
+        y, x = torch.meshgrid(torch.arange(H, dtype=torch.float64), torch.arange(W, dtype=torch.float64), indexing="ij")
+        d = torch.stack(((x + 0.5 - W / 2) / f[0], (y + 0.5 - H / 2) / f[1], torch.ones_like(x)), -1)
+        d = d @ self.c2w[:3, :3].to(torch.float64).T
+        o = self.c2w[:3, 3].to(torch.float64).expand(H, W, 3)
+        return torch.cat((o, d), -1).to(torch.float32)[None]
+
+
+def mesh_path(n: int = 16, H: int = 512, W: int = 512, fov: float = 0.75, radius: float = 1.905,
+              elevations=(0.0, -30.0, 30.0)):
+    """LaRa's mesh camera path (tools/gen_video_path.py:117-129): n azimuths at each elevation (degrees), looking at
+    the origin from ``radius``; 48 cameras by default."""
+    return [PathCamera(look_at_c2w(2.0 * math.pi * a / n, math.radians(e), radius), H, W, fov)
+            for e in elevations for a in range(n)]
