@@ -89,6 +89,18 @@ SIGNATURES = {
     "srf_mesh_workspace_bytes": (c_int, [_I3, POINTER(c_size_t)]),
     "srf_mesh_count": (c_int, [_P, _I3, _P, _P, _P, _P]),
     "srf_mesh_emit": (c_int, [_P, _I3, _I3, c_float, _P, _P, _P, c_int, c_int, _P, _P, _P]),
+    # include/surfel_fine_head.h
+    "srf_fine_head_forward": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int,   # stream, n, V, D, sh_dim, K, N
+                                      _P, _P, _P, _P,                               # volume_feat, idx, point_feats, shs
+                                      _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,       # norm w, b, wq, wk, wv, wo, w1, b1, w2, b2
+                                      _P]),                                         # sh_out
+    "srf_fine_head_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, c_int, POINTER(c_size_t)]),
+    "srf_fine_head_backward": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int,  # stream, n, V, D, sh_dim, K, N
+                                       _P, _P, _P,                                    # volume_feat, idx, point_feats
+                                       _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,        # the ten parameters
+                                       _P, _P,                                        # dL_dsh, workspace
+                                       _P, _P, _P,                                    # dL_dvolume_feat, _dpoint_feats, _dshs
+                                       _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),      # the ten parameter gradients
     "srf_profile_begin": (c_int, []),
     "srf_profile_end": (c_int, [POINTER(c_float), POINTER(c_int), c_int]),
 }
@@ -173,6 +185,11 @@ def deterministic(requested: Optional[bool] = None) -> bool:
     import torch
     return use_deterministic(requested, torch.are_deterministic_algorithms_enabled(),
                              torch.is_deterministic_algorithms_warn_only_enabled())
+
+
+def fine_head_workspace_bytes(lib, n: int, V: int, D: int, sh_dim: int, gather: bool) -> int:
+    """Workspace of srf_fine_head_backward on the current device."""
+    return _size_query(lib.srf_fine_head_workspace_bytes, n, V, D, sh_dim, 1 if gather else 0)
 
 
 def int3(v) -> ctypes.Array:
