@@ -4,6 +4,8 @@ There is no fallback path: if the shared library is missing or does not export
 the expected ABI the import of :mod:`lara_b200` still succeeds (so that LaRa's
 CPU-only plumbing can import ``diff_surfel_rasterization``), but the first use of
 the rasterizer raises ``RuntimeError`` loudly.
+
+Every entry that enqueues work is called through :func:`launch`, which passes torch's current stream.
 """
 from __future__ import annotations
 
@@ -11,6 +13,8 @@ import ctypes
 import os
 from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int64, c_size_t, c_void_p
 from typing import Optional
+
+import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libsurfel_b200.so")
@@ -144,6 +148,49 @@ def check(status: int, lib=None) -> None:
         raise RuntimeError(msg)
 
 
+def _ptr(t: Optional[torch.Tensor]) -> int:
+    return 0 if t is None else t.data_ptr()
+
+
+def _contig(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
+    return None if t is None else t.contiguous()
+
+
+def _dev_index(device: torch.device) -> int:
+    return device.index if device.index is not None else torch.cuda.current_device()
+
+
+def _raw_stream(device: torch.device) -> int:
+    return torch._C._cuda_getCurrentRawStream(_dev_index(device))
+
+
+class _DeviceGuard:
+    """`with torch.cuda.device(d)` only when d is not already current (the common case)."""
+
+    def __init__(self, device: torch.device):
+        self.idx = device.index
+        self.ctx = None
+
+    def __enter__(self):
+        if self.idx is not None and self.idx != torch.cuda.current_device():
+            self.ctx = torch.cuda.device(self.idx)
+            self.ctx.__enter__()
+
+    def __exit__(self, *exc):
+        if self.ctx is not None:
+            self.ctx.__exit__(*exc)
+        return False
+
+
+def launch(name: str, device: torch.device, *args) -> None:
+    """Call the enqueuing entry ``name`` with torch's current stream of ``device`` as its first argument and ``args``
+    after it, ``device`` current during the call.  The stream is read now, so work is enqueued on whatever stream is
+    current when this runs.  A non-zero status raises ``RuntimeError`` with the library's message."""
+    lib = load()
+    with _DeviceGuard(device):
+        check(getattr(lib, name)(_raw_stream(device), *args), lib)
+
+
 def views_sizes(lib, V: int, P: int, H: int, W: int, capacity: int, for_backward: bool = True):
     """(geom, tile, image, entries, point_list, backward scratch) bytes for V back-to-back per-view workspaces; with
     ``for_backward=False`` those of a forward-only forward (image and scratch 0, a list-only point_list)."""
@@ -161,6 +208,10 @@ def _size_query(fn, *args) -> int:
 def det_backward_scratch_bytes(lib, V: int, P: int) -> int:
     """Scratch of srf_views_backward(..., deterministic=1)."""
     return _size_query(lib.srf_views_backward_deterministic_scratch_bytes, V, P)
+
+
+def ms_ssim_workspace_bytes(lib, B: int, C: int, H: int, W: int) -> int:
+    return _size_query(lib.srf_ms_ssim_workspace_bytes, B, C, H, W)
 
 
 def det_point_feats_workspace_bytes(lib, V: int, H: int, W: int) -> int:
@@ -182,7 +233,6 @@ def use_deterministic(requested: Optional[bool], enabled: bool, warn_only: bool)
 
 def deterministic(requested: Optional[bool] = None) -> bool:
     """:func:`use_deterministic` with torch's current setting, read when the op runs."""
-    import torch
     return use_deterministic(requested, torch.are_deterministic_algorithms_enabled(),
                              torch.is_deterministic_algorithms_warn_only_enabled())
 

@@ -1,4 +1,6 @@
-// api.cu -- the extern "C" boundary declared in include/surfel_rasterizer.h.
+// api.cu -- the library-wide part of the extern "C" boundary declared in include/surfel_rasterizer.h: the ABI version,
+// the last-error buffer, per-kernel profiling, the workspace layouts and the rasterizer's entries (forward, its
+// stage-2 re-run, backward, srf_mark_visible).  The fused ops' entries are defined next to their kernels.
 // Plain pointers and sizes in, int status out; only enqueues work on the given stream.
 #include <cuda_runtime.h>
 #include <stdarg.h>
@@ -13,23 +15,14 @@
 #include "surfel_common.cuh"
 #include "surfel_kernels.h"
 
+using srf::align_up;
+using srf::cuda_error;
+using srf::misaligned;
+using srf::set_error;
+
 namespace {
 
 thread_local char g_err[512] = "";
-
-int fail(const char* fmt, ...) {
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(g_err, sizeof(g_err), fmt, ap);
-    va_end(ap);
-    return 1;
-}
-
-int cuda_fail(const char* what, cudaError_t e) {
-    return fail("%s: %s", what, cudaGetErrorString(e));
-}
-
-inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
 
 struct GeomLayout { size_t rec, depths, rects, total; };
 struct TileLayout { size_t count, counters, ranges, big, order, total; int gx, gy, ntiles; };
@@ -77,8 +70,6 @@ T* at(const void* base, size_t off) {
     return reinterpret_cast<T*>(reinterpret_cast<uintptr_t>(base) + off);
 }
 
-bool misaligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 255) != 0; }
-
 // One view's point_list workspace: the depth-sorted list (u32 [capacity]), then, for a forward a backward follows, the
 // blend forward's contribution masks (u32 [8 warp blocks][capacity], indexed by list position), which the blend
 // backward replays.
@@ -113,6 +104,24 @@ cudaEvent_t take_event() {
 }  // namespace
 
 namespace srf {
+int set_error(const char* fmt, ...) {
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(g_err, sizeof(g_err), fmt, ap);
+    va_end(ap);
+    return 1;
+}
+
+int check_overflow_flag(const char* fn, const uint32_t* flag, cudaStream_t stream) {
+    uint32_t h = 0;
+    cudaError_t e = cudaMemcpyAsync(&h, flag, sizeof(h), cudaMemcpyDeviceToHost, stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+    if (e != cudaSuccess) return cuda_error("deterministic overflow flag read-back", e);
+    if (h) return set_error("%s: a gradient term is not finite or beyond the range of the deterministic fixed-point sum; "
+                            "no gradient was produced", fn);
+    return 0;
+}
+
 void prof_start(int kernel, cudaStream_t stream) {
     if (!g_prof_on) return;
     std::lock_guard<std::mutex> lk(g_prof_mu);
@@ -156,14 +165,14 @@ int srf_profile_begin(void) {
 int srf_profile_end(float* ms_out, int* launches_out, int n) {
     g_prof_on = false;
     std::lock_guard<std::mutex> lk(g_prof_mu);
-    if (n < srf::K_COUNT || !ms_out || !launches_out) return fail("srf_profile_end: need arrays of %d entries", (int)srf::K_COUNT);
+    if (n < srf::K_COUNT || !ms_out || !launches_out) return set_error("srf_profile_end: need arrays of %d entries", (int)srf::K_COUNT);
     for (int k = 0; k < n; ++k) { ms_out[k] = 0.f; launches_out[k] = 0; }
     for (auto& s : g_spans) {
         cudaError_t e = cudaEventSynchronize(s.stop);
-        if (e != cudaSuccess) return cuda_fail("profile event sync", e);
+        if (e != cudaSuccess) return cuda_error("profile event sync", e);
         float ms = 0.f;
         e = cudaEventElapsedTime(&ms, s.start, s.stop);
-        if (e != cudaSuccess) return cuda_fail("profile elapsed", e);
+        if (e != cudaSuccess) return cuda_error("profile elapsed", e);
         ms_out[s.kernel] += ms;
         launches_out[s.kernel] += 1;
         g_event_pool.push_back(s.start); g_event_pool.push_back(s.stop);
@@ -174,7 +183,7 @@ int srf_profile_end(float* ms_out, int* launches_out, int n) {
 const char* srf_last_error(void) { return g_err; }
 
 int srf_views_workspace_bytes(int V, int P, int H, int W, size_t capacity, int for_backward, size_t bytes[6]) {
-    if (V <= 0 || P < 0 || H <= 0 || W <= 0 || !bytes) return fail("srf_views_workspace_bytes: bad arguments");
+    if (V <= 0 || P < 0 || H <= 0 || W <= 0 || !bytes) return set_error("srf_views_workspace_bytes: bad arguments");
     bytes[0] = geom_layout(P).total * (size_t)V;
     bytes[1] = tile_layout(H, W).total * (size_t)V;
     bytes[2] = for_backward ? image_layout(H, W).total * (size_t)V : 0;
@@ -185,7 +194,7 @@ int srf_views_workspace_bytes(int V, int P, int H, int W, size_t capacity, int f
 }
 
 int srf_state_layout(int P, int H, int W, size_t geom_off[3], size_t tile_off[5], size_t image_off[2]) {
-    if (P < 0 || H <= 0 || W <= 0) return fail("srf_state_layout: bad arguments");
+    if (P < 0 || H <= 0 || W <= 0) return set_error("srf_state_layout: bad arguments");
     const GeomLayout g = geom_layout(P);
     const TileLayout t = tile_layout(H, W);
     const ImageLayout i = image_layout(H, W);
@@ -202,17 +211,6 @@ int srf_state_layout(int P, int H, int W, size_t geom_off[3], size_t tile_off[5]
 // camera a record of SRF_CAM_FLOATS floats in `cams`, each view's workspaces one layout stride apart.
 // ---------------------------------------------------------------------------------------------
 namespace {
-
-// reads a device flag that the work enqueued so far sets: waits for the stream
-int check_overflow_flag(const char* fn, const uint32_t* flag, cudaStream_t stream) {
-    uint32_t h = 0;
-    cudaError_t e = cudaMemcpyAsync(&h, flag, sizeof(h), cudaMemcpyDeviceToHost, stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-    if (e != cudaSuccess) return cuda_fail("deterministic overflow flag read-back", e);
-    if (h) return fail("%s: a gradient term is not finite or beyond the range of the deterministic fixed-point sum; "
-                       "no gradient was produced", fn);
-    return 0;
-}
 
 void fill_bin_args(srf::BinArgs& b, int V, int P, const TileLayout& tl, void* tile_state) {
     memset(&b, 0, sizeof(b));
@@ -231,21 +229,21 @@ int forward_preprocess_check(const char* fn, int V, int P, int D, int M,
                              const float* opacities, const float* scales, const float* rotations,
                              const float* transMat_precomp, int image_height, int image_width,
                              const int* radii, const void* geom_state, const void* tile_state) {
-    if (V <= 0 || P < 0 || image_height <= 0 || image_width <= 0) return fail("%s: bad sizes", fn);
-    if (image_height > 16 * 65535 || image_width > 16 * 65535) return fail("%s: image too large", fn);
-    if (!tile_state || misaligned(tile_state)) return fail("%s: tile_state must be 256-byte aligned", fn);
-    if (D < 0 || D > 3) return fail("%s: sh degree must be in [0,3]", fn);
+    if (V <= 0 || P < 0 || image_height <= 0 || image_width <= 0) return set_error("%s: bad sizes", fn);
+    if (image_height > 16 * 65535 || image_width > 16 * 65535) return set_error("%s: image too large", fn);
+    if (!tile_state || misaligned(tile_state)) return set_error("%s: tile_state must be 256-byte aligned", fn);
+    if (D < 0 || D > 3) return set_error("%s: sh degree must be in [0,3]", fn);
     if (P > 0) {
-        if (!means3D || !opacities || !radii) return fail("%s: null required pointer", fn);
+        if (!means3D || !opacities || !radii) return set_error("%s: null required pointer", fn);
         if ((shs == nullptr) == (colors_precomp == nullptr))
-            return fail("Please provide excatly one of either SHs or precomputed colors!");
+            return set_error("Please provide excatly one of either SHs or precomputed colors!");
         if (((scales == nullptr || rotations == nullptr) && transMat_precomp == nullptr) ||
             ((scales != nullptr || rotations != nullptr) && transMat_precomp != nullptr))
-            return fail("Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!");
-        if (shs && M < (D + 1) * (D + 1)) return fail("%s: M=%d SH coefficients < (D+1)^2 for D=%d", fn, M, D);
-        if (!geom_state || misaligned(geom_state)) return fail("%s: geom_state must be 256-byte aligned", fn);
+            return set_error("Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!");
+        if (shs && M < (D + 1) * (D + 1)) return set_error("%s: M=%d SH coefficients < (D+1)^2 for D=%d", fn, M, D);
+        if (!geom_state || misaligned(geom_state)) return set_error("%s: geom_state must be 256-byte aligned", fn);
         if ((reinterpret_cast<uintptr_t>(rotations) & 15) || (reinterpret_cast<uintptr_t>(scales) & 7))
-            return fail("%s: rotations must be 16-byte and scales 8-byte aligned", fn);
+            return set_error("%s: rotations must be 16-byte and scales 8-byte aligned", fn);
     }
     return 0;
 }
@@ -262,7 +260,7 @@ int forward_preprocess_impl(cudaStream_t stream, int V, int P, int D, int M,
     // tile blocks + counters of every view are zeroed by one 2-D memset
     cudaError_t e = cudaMemset2DAsync(at<char>(tile_state, tl.count), tl.total, 0,
                                       tl.counters + 4 * sizeof(uint32_t) - tl.count, (size_t)V, stream);
-    if (e != cudaSuccess) return cuda_fail("memset tile counters", e);
+    if (e != cudaSuccess) return cuda_error("memset tile counters", e);
 
     srf::BinArgs b;
     fill_bin_args(b, V, P, tl, tile_state);
@@ -289,7 +287,7 @@ int forward_preprocess_impl(cudaStream_t stream, int V, int P, int D, int M,
         a.geom_stride = gl.total;
         a.tile_stride = b.tile_stride;
         e = srf::launch_preprocess_fwd(a, stream);
-        if (e != cudaSuccess) return cuda_fail("preprocess_fwd launch", e);
+        if (e != cudaSuccess) return cuda_error("preprocess_fwd launch", e);
     }
     // num_rendered read-back: pinned host memory is device-visible under UVA, so the scan kernel stores the counts there
     // itself (no copy-engine operation between the kernels of the stream); pageable memory falls back to an async copy
@@ -305,11 +303,11 @@ int forward_preprocess_impl(cudaStream_t stream, int V, int P, int D, int M,
         }
     }
     e = srf::launch_tile_scan(b, stream);
-    if (e != cudaSuccess) return cuda_fail("tile_scan launch", e);
+    if (e != cudaSuccess) return cuda_error("tile_scan launch", e);
     if (num_rendered_host && !zero_copy) {
         e = cudaMemcpy2DAsync(num_rendered_host, sizeof(uint32_t), b.counters, tl.total, sizeof(uint32_t), (size_t)V,
                               cudaMemcpyDeviceToHost, stream);
-        if (e != cudaSuccess) return cuda_fail("num_rendered copy", e);
+        if (e != cudaSuccess) return cuda_error("num_rendered copy", e);
     }
     return 0;
 }
@@ -318,15 +316,15 @@ int forward_preprocess_impl(cudaStream_t stream, int V, int P, int D, int M,
 int forward_render_check(const char* fn, int V, int P, int image_height, int image_width, size_t capacity,
                          const void* geom_state, const void* tile_state, const void* entries, const uint32_t* point_list,
                          const void* image_state, const float* cams, const float* out_color, const float* out_others, bool record) {
-    if (V <= 0 || P < 0 || image_height <= 0 || image_width <= 0) return fail("%s: bad sizes", fn);
+    if (V <= 0 || P < 0 || image_height <= 0 || image_width <= 0) return set_error("%s: bad sizes", fn);
     if (!cams || !tile_state || (record && !image_state) || !out_color || !out_others)
-        return fail("%s: null required pointer", fn);
-    if (capacity > 0xfffffff0ull) return fail("%s: capacity exceeds 32-bit instance indices", fn);
-    if (capacity > 0 && (!entries || !point_list)) return fail("%s: null binning buffers", fn);
-    if (P > 0 && (!geom_state || misaligned(geom_state))) return fail("%s: geom_state must be 256-byte aligned", fn);
-    if (misaligned(tile_state)) return fail("%s: tile_state must be 256-byte aligned", fn);
+        return set_error("%s: null required pointer", fn);
+    if (capacity > 0xfffffff0ull) return set_error("%s: capacity exceeds 32-bit instance indices", fn);
+    if (capacity > 0 && (!entries || !point_list)) return set_error("%s: null binning buffers", fn);
+    if (P > 0 && (!geom_state || misaligned(geom_state))) return set_error("%s: geom_state must be 256-byte aligned", fn);
+    if (misaligned(tile_state)) return set_error("%s: tile_state must be 256-byte aligned", fn);
     if (capacity > 0 && (misaligned(entries) || misaligned(point_list)))
-        return fail("%s: entries and point_list must be 256-byte aligned", fn);
+        return set_error("%s: entries and point_list must be 256-byte aligned", fn);
     return 0;
 }
 
@@ -354,7 +352,7 @@ int forward_render_impl(cudaStream_t stream, int V, int P, int image_height, int
         b.depths = at<float>(geom_state, gl.depths);
         b.rects = at<uint2>(geom_state, gl.rects);
         e = srf::launch_bin_and_sort(b, stream);
-        if (e != cudaSuccess) return cuda_fail("binning launch", e);
+        if (e != cudaSuccess) return cuda_error("binning launch", e);
     }
     srf::RenderFwdArgs r;
     memset(&r, 0, sizeof(r));
@@ -375,7 +373,7 @@ int forward_render_impl(cudaStream_t stream, int V, int P, int image_height, int
     r.geom_stride = b.geom_stride; r.tile_stride = b.tile_stride; r.plist_stride = b.plist_stride;
     r.cam_stride = SRF_CAM_FLOATS;
     e = srf::launch_render_fwd(r, record, stream);
-    if (e != cudaSuccess) return cuda_fail("render_fwd launch", e);
+    if (e != cudaSuccess) return cuda_error("render_fwd launch", e);
     return 0;
 }
 
@@ -391,16 +389,16 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
                   float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
                   float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
                   int raw_activations, bool deterministic) {
-    if (!cams) return fail("%s: null camera records", fn);
-    if (V <= 0 || P < 0 || image_height <= 0 || image_width <= 0) return fail("%s: bad sizes", fn);
+    if (!cams) return set_error("%s: null camera records", fn);
+    if (V <= 0 || P < 0 || image_height <= 0 || image_width <= 0) return set_error("%s: bad sizes", fn);
     if (P == 0) return 0;
-    if (!geom_state || !tile_state || !image_state || !scratch || !radii) return fail("%s: null state pointer", fn);
-    if (!dL_dout_color || !dL_dout_others) return fail("%s: null upstream gradient", fn);
+    if (!geom_state || !tile_state || !image_state || !scratch || !radii) return set_error("%s: null state pointer", fn);
+    if (!dL_dout_color || !dL_dout_others) return set_error("%s: null upstream gradient", fn);
     if (!dL_dmeans3D || !dL_dopacity || !dL_dscales || !dL_drotations)
-        return fail("%s: null required output gradient", fn);
-    if (!means3D) return fail("%s: null input pointer", fn);
-    if (!transmat_was_precomputed && (!scales || !rotations)) return fail("%s: scales/rotations required", fn);
-    if (misaligned(scratch)) return fail("%s: scratch must be 256-byte aligned", fn);
+        return set_error("%s: null required output gradient", fn);
+    if (!means3D) return set_error("%s: null input pointer", fn);
+    if (!transmat_was_precomputed && (!scales || !rotations)) return set_error("%s: scales/rotations required", fn);
+    if (misaligned(scratch)) return set_error("%s: scratch must be 256-byte aligned", fn);
     const TileLayout tl = tile_layout(image_height, image_width);
     const ImageLayout il = image_layout(image_height, image_width);
     const GeomLayout gl = geom_layout(P);
@@ -412,7 +410,7 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
     uint32_t* overflow = at<uint32_t>(det, dstride * (size_t)V);
     cudaError_t e = deterministic ? cudaMemsetAsync(det, 0, dstride * (size_t)V + sizeof(uint32_t), stream)
                                   : cudaMemsetAsync(scratch, 0, gstride * (size_t)V, stream);
-    if (e != cudaSuccess) return cuda_fail("memset gradient records", e);
+    if (e != cudaSuccess) return cuda_error("memset gradient records", e);
 
     srf::RenderBwdArgs r;
     memset(&r, 0, sizeof(r));
@@ -440,7 +438,7 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
     } else {
         e = srf::launch_render_bwd(r, stream);
     }
-    if (e != cudaSuccess) return cuda_fail("render_bwd launch", e);
+    if (e != cudaSuccess) return cuda_error("render_bwd launch", e);
 
     srf::PreprocessBwdArgs p;
     memset(&p, 0, sizeof(p));
@@ -465,8 +463,8 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
     p.dL_dcolors = dL_dcolors; p.dL_dopacity = dL_dopacity;
     p.dL_dscales = dL_dscales; p.dL_drotations = dL_drotations; p.dL_dtransMat = dL_dtransMat;
     e = srf::launch_preprocess_bwd(p, stream);
-    if (e != cudaSuccess) return cuda_fail("preprocess_bwd launch", e);
-    return deterministic ? check_overflow_flag(fn, overflow, stream) : 0;
+    if (e != cudaSuccess) return cuda_error("preprocess_bwd launch", e);
+    return deterministic ? srf::check_overflow_flag(fn, overflow, stream) : 0;
 }
 
 }  // namespace
@@ -495,7 +493,7 @@ int srf_views_forward(srf_stream_t stream_, int V, int P, int D, int M,
     if (rc != 0) return rc;
     if (count_event) {      // lets the caller wait for the instance counts without waiting for the blend
         cudaError_t e = cudaEventRecord(static_cast<cudaEvent_t>(count_event), stream);
-        if (e != cudaSuccess) return cuda_fail("count event record", e);
+        if (e != cudaSuccess) return cuda_error("count event record", e);
     }
     return forward_render_impl(stream, V, P, image_height, image_width, capacity, geom_state, tile_state, entries,
                                point_list, image_state, cams, out_color, out_others, for_backward != 0);
@@ -534,282 +532,8 @@ int srf_views_backward(srf_stream_t stream_, int V, int P, int D, int M, int ima
 }
 
 int srf_views_backward_deterministic_scratch_bytes(int V, int P, size_t* bytes) {
-    if (V <= 0 || P < 0 || !bytes) return fail("srf_views_backward_deterministic_scratch_bytes: bad arguments");
+    if (V <= 0 || P < 0 || !bytes) return set_error("srf_views_backward_deterministic_scratch_bytes: bad arguments");
     *bytes = det_scratch_bytes(V, P);
-    return 0;
-}
-
-int srf_views_epilogue_forward(srf_stream_t stream_, int V, int image_height, int image_width, float depth_ratio,
-                               const float* color, const float* allmap, const float* rays, const float* cams,
-                               float* image, float* depth, float* acc_map, float* rend_normal, float* depth_normal,
-                               float* rend_dist) {
-    const char* fn = "srf_views_epilogue_forward";
-    if (V <= 0 || image_height <= 0 || image_width <= 0) return fail("%s: bad sizes", fn);
-    if (!color || !allmap || !cams || !image || !depth || !acc_map || !rend_normal || !depth_normal || !rend_dist)
-        return fail("%s: null pointer", fn);
-    srf::EpilogueArgs a;
-    memset(&a, 0, sizeof(a));
-    a.W = image_width; a.H = image_height; a.nviews = V; a.depth_ratio = depth_ratio;
-    a.color = color; a.allmap = allmap; a.rays = rays; a.viewmatrix = cams + SRF_CAM_VIEW; a.cam_stride = SRF_CAM_FLOATS;
-    a.image = image; a.depth = depth; a.acc = acc_map; a.rend_normal = rend_normal; a.depth_normal = depth_normal;
-    a.dist = rend_dist;
-    cudaError_t e = srf::launch_epilogue_fwd(a, static_cast<cudaStream_t>(stream_));
-    if (e != cudaSuccess) return cuda_fail("epilogue_fwd launch", e);
-    return 0;
-}
-
-int srf_views_epilogue_backward(srf_stream_t stream_, int V, int image_height, int image_width, float depth_ratio,
-                                const float* color, const float* allmap, const float* rays, const float* cams,
-                                const float* g_image, const float* g_depth, const float* g_acc_map,
-                                const float* g_rend_normal, const float* g_depth_normal, const float* g_rend_dist,
-                                float* scratch, float* dL_dcolor, float* dL_dallmap) {
-    const char* fn = "srf_views_epilogue_backward";
-    if (V <= 0 || image_height <= 0 || image_width <= 0) return fail("%s: bad sizes", fn);
-    if (!color || !allmap || !cams || !dL_dcolor || !dL_dallmap) return fail("%s: null pointer", fn);
-    if (g_depth_normal && rays && !scratch) return fail("%s: scratch [V,3,H,W] required", fn);
-    srf::EpilogueArgs a;
-    memset(&a, 0, sizeof(a));
-    a.W = image_width; a.H = image_height; a.nviews = V; a.depth_ratio = depth_ratio;
-    a.color = color; a.allmap = allmap; a.rays = rays; a.viewmatrix = cams + SRF_CAM_VIEW; a.cam_stride = SRF_CAM_FLOATS;
-    a.g_image = g_image; a.g_depth = g_depth; a.g_acc = g_acc_map; a.g_rend_normal = g_rend_normal;
-    a.g_depth_normal = g_depth_normal; a.g_dist = g_rend_dist;
-    a.scratch = scratch; a.dL_dcolor = dL_dcolor; a.dL_dallmap = dL_dallmap;
-    cudaError_t e = srf::launch_epilogue_bwd(a, static_cast<cudaStream_t>(stream_));
-    if (e != cudaSuccess) return cuda_fail("epilogue_bwd launch", e);
-    return 0;
-}
-
-int srf_loss_forward(srf_stream_t stream_, int V, int image_height, int image_width, int with_reg,
-                     const float* image, const float* target_hwc, const float* rend_normal, const float* depth_normal,
-                     const float* acc_map, const float* rend_dist, double* sums, void* workspace) {
-    if (V <= 0 || image_height <= 0 || image_width <= 0) return fail("srf_loss_forward: bad sizes");
-    if (!image || !target_hwc || !sums) return fail("srf_loss_forward: null pointer");
-    if (with_reg && (!rend_normal || !depth_normal || !acc_map || !rend_dist)) return fail("srf_loss_forward: null regulariser input");
-    if (reinterpret_cast<uintptr_t>(workspace) & 7) return fail("srf_loss_forward: workspace must be 8-byte aligned");
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    cudaError_t e;
-    // the deterministic path writes every sum from its partials; the atomics need zeroed sums
-    if (!workspace && (e = cudaMemsetAsync(sums, 0, 3 * sizeof(double), stream)) != cudaSuccess)
-        return cuda_fail("memset loss sums", e);
-    srf::LossArgs a;
-    memset(&a, 0, sizeof(a));
-    a.W = image_width; a.H = image_height; a.nviews = V; a.with_reg = with_reg ? 1 : 0;
-    a.image = image; a.target = target_hwc; a.rend_normal = rend_normal; a.depth_normal = depth_normal;
-    a.acc = acc_map; a.dist = rend_dist; a.sums = sums; a.partials = static_cast<double*>(workspace);
-    e = srf::launch_loss_fused(a, stream);
-    if (e != cudaSuccess) return cuda_fail("loss_sums launch", e);
-    return 0;
-}
-
-int srf_loss_deterministic_workspace_bytes(int V, int image_height, int image_width, size_t* bytes) {
-    if (V <= 0 || image_height <= 0 || image_width <= 0 || !bytes) return fail("srf_loss_deterministic_workspace_bytes: bad arguments");
-    *bytes = srf::loss_det_blocks((size_t)V * image_height * image_width) * 3 * sizeof(double);
-    return 0;
-}
-
-int srf_loss_backward(srf_stream_t stream_, int V, int image_height, int image_width, int with_reg,
-                      float w_mse, float w_dist, float w_normal,
-                      const float* image, const float* target_hwc, const float* rend_normal, const float* depth_normal,
-                      const float* acc_map, const float* upstream,
-                      float* g_image, float* g_rend_normal, float* g_depth_normal, float* g_rend_dist) {
-    if (V <= 0 || image_height <= 0 || image_width <= 0) return fail("srf_loss_backward: bad sizes");
-    if (!image || !target_hwc || !g_image) return fail("srf_loss_backward: null pointer");
-    if (with_reg && (!rend_normal || !depth_normal || !acc_map || !g_rend_normal || !g_depth_normal || !g_rend_dist))
-        return fail("srf_loss_backward: null regulariser pointer");
-    srf::LossArgs a;
-    memset(&a, 0, sizeof(a));
-    a.W = image_width; a.H = image_height; a.nviews = V; a.with_reg = with_reg ? 1 : 0;
-    a.w_mse = w_mse; a.w_dist = w_dist; a.w_normal = w_normal;
-    a.image = image; a.target = target_hwc; a.rend_normal = rend_normal; a.depth_normal = depth_normal; a.acc = acc_map;
-    a.gout = upstream;
-    a.g_image = g_image; a.g_rend_normal = g_rend_normal; a.g_depth_normal = g_depth_normal; a.g_dist = g_rend_dist;
-    cudaError_t e = srf::launch_loss_fused(a, static_cast<cudaStream_t>(stream_));
-    if (e != cudaSuccess) return cuda_fail("loss_grads launch", e);
-    return 0;
-}
-
-int srf_decoder_layout_forward(srf_stream_t stream_, size_t B, int N, int K, int sh_dim,
-                               float opacity_shift, float scaling_shift, float half_cell_size,
-                               const float* params, const float* group_centers,
-                               float* centers, float* shs, float* opacity, float* scaling, float* rotation) {
-    if (N <= 0 || K <= 0 || sh_dim < 3 || sh_dim % 3 != 0) return fail("srf_decoder_layout_forward: bad sizes");
-    if (!params || !group_centers || !centers || !shs || !opacity || !scaling || !rotation)
-        return fail("srf_decoder_layout_forward: null pointer");
-    if ((reinterpret_cast<uintptr_t>(rotation) & 15) || (reinterpret_cast<uintptr_t>(scaling) & 7) ||
-        ((sh_dim & 3) == 0 && (reinterpret_cast<uintptr_t>(shs) & 15)))
-        return fail("srf_decoder_layout_forward: outputs must be 16-byte aligned");
-    srf::DecoderArgs a;
-    memset(&a, 0, sizeof(a));
-    a.total = B * (size_t)N * (size_t)K; a.N = N; a.K = K; a.C = 10 + sh_dim; a.sh_dim = sh_dim;
-    a.opacity_shift = opacity_shift; a.scaling_shift = scaling_shift; a.half_cell = half_cell_size;
-    a.params = params; a.group_centers = group_centers;
-    a.centers = centers; a.shs = shs; a.opacity = opacity; a.scaling = scaling; a.rotation = rotation;
-    cudaError_t e = srf::launch_decoder_layout(a, false, static_cast<cudaStream_t>(stream_));
-    if (e != cudaSuccess) return cuda_fail("decoder_layout launch", e);
-    return 0;
-}
-
-int srf_decoder_layout_backward(srf_stream_t stream_, size_t B, int N, int K, int sh_dim, float half_cell_size,
-                                const float* params, const float* g_centers, const float* g_shs, const float* g_opacity,
-                                const float* g_scaling, const float* g_rotation, float* g_params) {
-    if (N <= 0 || K <= 0 || sh_dim < 3 || sh_dim % 3 != 0) return fail("srf_decoder_layout_backward: bad sizes");
-    if (!params || !g_params) return fail("srf_decoder_layout_backward: null pointer");
-    srf::DecoderArgs a;
-    memset(&a, 0, sizeof(a));
-    a.total = B * (size_t)N * (size_t)K; a.N = N; a.K = K; a.C = 10 + sh_dim; a.sh_dim = sh_dim;
-    a.half_cell = half_cell_size;
-    a.params = params;
-    a.g_centers = g_centers; a.g_shs = g_shs; a.g_opacity = g_opacity; a.g_scaling = g_scaling; a.g_rotation = g_rotation;
-    a.g_params = g_params;
-    cudaError_t e = srf::launch_decoder_layout(a, true, static_cast<cudaStream_t>(stream_));
-    if (e != cudaSuccess) return cuda_fail("decoder_layout backward launch", e);
-    return 0;
-}
-
-static int point_feats_check(const char* fn, int V, int n, int H, int W, const float* points, const float* w2cs,
-                             const float* ixts, const float* img_ref, const float* image, const float* acc,
-                             const float* depth) {
-    if (V <= 0 || n < 0 || H <= 0 || W <= 0) return fail("%s: bad sizes (V=%d, n=%d, H=%d, W=%d)", fn, V, n, H, W);
-    if (H > (1 << 24) || W > (1 << 24)) return fail("%s: image too large", fn);    // pixel indices exact in fp32
-    // an empty point set has no storage: points (and feats / g_feats) are only needed when n > 0
-    if ((n > 0 && !points) || !w2cs || !ixts || !img_ref || !image || !acc || !depth) return fail("%s: null input pointer", fn);
-    return 0;
-}
-
-int srf_point_feats_forward(srf_stream_t stream_, int V, int n, int H, int W,
-                            const float* points, const float* w2cs, const float* ixts,
-                            const float* img_ref, const float* image, const float* acc, const float* depth,
-                            float* feats) {
-    const char* fn = "srf_point_feats_forward";
-    if (point_feats_check(fn, V, n, H, W, points, w2cs, ixts, img_ref, image, acc, depth)) return 1;
-    if (n > 0 && !feats) return fail("%s: null output pointer", fn);
-    if (n == 0) return 0;
-    srf::PointFeatsArgs a;
-    memset(&a, 0, sizeof(a));
-    a.V = V; a.n = n; a.H = H; a.W = W;
-    a.points = points; a.w2cs = w2cs; a.ixts = ixts; a.img_ref = img_ref; a.image = image; a.acc = acc; a.depth = depth;
-    a.feats = feats;
-    cudaError_t e = srf::launch_point_feats(a, false, static_cast<cudaStream_t>(stream_));
-    if (e != cudaSuccess) return cuda_fail("point_feats_fwd launch", e);
-    return 0;
-}
-
-// deterministic workspace: header (max |g_feats|, overflow flag), then the int64 planes g_image | g_acc | g_depth
-static size_t pf_det_planes_offset() { return 256; }
-static size_t pf_det_workspace_bytes(int V, int H, int W) {
-    return pf_det_planes_offset() + 5 * (size_t)V * H * W * sizeof(long long);
-}
-
-int srf_point_feats_backward(srf_stream_t stream_, int V, int n, int H, int W,
-                             const float* points, const float* w2cs, const float* ixts,
-                             const float* img_ref, const float* image, const float* acc, const float* depth,
-                             const float* g_feats, float* g_points, float* g_image, float* g_acc, float* g_depth,
-                             void* workspace) {
-    const char* fn = "srf_point_feats_backward";
-    if (point_feats_check(fn, V, n, H, W, points, w2cs, ixts, img_ref, image, acc, depth)) return 1;
-    if (n > 0 && !g_feats) return fail("%s: null upstream gradient", fn);
-    if (workspace && misaligned(workspace)) return fail("%s: workspace must be 256-byte aligned", fn);
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    const bool nothing = n == 0 || (!g_points && !g_image && !g_acc && !g_depth);
-    // the default path adds into cleared outputs; the deterministic one writes them from its fixed-point planes
-    if (!workspace || nothing) {
-        const size_t plane = (size_t)V * H * W * sizeof(float);
-        cudaError_t e = cudaSuccess;
-        if (g_image && (e = cudaMemsetAsync(g_image, 0, 3 * plane, stream)) != cudaSuccess) return cuda_fail("memset g_image", e);
-        if (g_acc && (e = cudaMemsetAsync(g_acc, 0, plane, stream)) != cudaSuccess) return cuda_fail("memset g_acc", e);
-        if (g_depth && (e = cudaMemsetAsync(g_depth, 0, plane, stream)) != cudaSuccess) return cuda_fail("memset g_depth", e);
-    }
-    if (nothing) return 0;
-    srf::PointFeatsArgs a;
-    memset(&a, 0, sizeof(a));
-    a.V = V; a.n = n; a.H = H; a.W = W;
-    a.points = points; a.w2cs = w2cs; a.ixts = ixts; a.img_ref = img_ref; a.image = image; a.acc = acc; a.depth = depth;
-    a.g_feats = g_feats; a.g_points = g_points; a.g_image = g_image; a.g_acc = g_acc; a.g_depth = g_depth;
-    if (workspace) {
-        cudaError_t e = cudaMemsetAsync(workspace, 0, pf_det_workspace_bytes(V, H, W), stream);
-        if (e != cudaSuccess) return cuda_fail("memset point_feats workspace", e);
-        a.det = static_cast<uint32_t*>(workspace);
-        a.g_fixed = at<long long>(workspace, pf_det_planes_offset());
-    }
-    cudaError_t e = srf::launch_point_feats(a, true, stream);
-    if (e != cudaSuccess) return cuda_fail("point_feats_bwd launch", e);
-    return workspace ? check_overflow_flag(fn, a.det + 1, stream) : 0;
-}
-
-int srf_point_feats_deterministic_workspace_bytes(int V, int H, int W, size_t* bytes) {
-    if (V <= 0 || H <= 0 || W <= 0 || !bytes) return fail("srf_point_feats_deterministic_workspace_bytes: bad arguments");
-    *bytes = pf_det_workspace_bytes(V, H, W);
-    return 0;
-}
-
-static int ms_ssim_sizes(const char* fn, int B, int C, int H, int W) {
-    if (B <= 0 || C <= 0 || H <= 0 || W <= 0) return fail("%s: bad sizes (B=%d, C=%d, H=%d, W=%d)", fn, B, C, H, W);
-    if ((H < W ? H : W) <= 160)
-        return fail("%s: Image size should be larger than 160 due to the 4 downsamplings in ms-ssim (H=%d, W=%d)", fn, H, W);
-    if ((long long)B * C > 65535) return fail("%s: B*C=%lld planes exceeds 65535", fn, (long long)B * C);
-    return 0;
-}
-
-static int ms_ssim_addr(const char* fn, const char* what, const float* p, const srf_ms_ssim_addr* a, srf::MsAddr* out) {
-    if (!p || !a) return fail("%s: null %s pointer", fn, what);
-    if (reinterpret_cast<uintptr_t>(p) & 3) return fail("%s: %s must be 4-byte aligned", fn, what);
-    if (a->wv <= 0 || a->wv > 0x7fffffff) return fail("%s: %s view width %lld out of range", fn, what, (long long)a->wv);
-    out->sb = a->sb; out->sc = a->sc; out->sy = a->sy; out->sx = a->sx; out->sv = a->sv; out->wv = (int)a->wv;
-    return 0;
-}
-
-static int ms_ssim_prepare(const char* fn, int B, int C, int H, int W, const float* x, const srf_ms_ssim_addr* x_addr,
-                           const float* y, const srf_ms_ssim_addr* y_addr, float data_range, int size_average,
-                           void* workspace, srf::MsSsimArgs* a) {
-    memset(a, 0, sizeof(*a));
-    if (ms_ssim_sizes(fn, B, C, H, W)) return 1;
-    if (ms_ssim_addr(fn, "x", x, x_addr, &a->ax) || ms_ssim_addr(fn, "y", y, y_addr, &a->ay)) return 1;
-    if (!(data_range > 0.f) || !(data_range < 3.0e38f)) return fail("%s: data_range must be positive and finite", fn);
-    if (!workspace || misaligned(workspace)) return fail("%s: workspace must be 256-byte aligned", fn);
-    a->B = B; a->C = C; a->H = H; a->W = W; a->size_average = size_average ? 1 : 0; a->data_range = data_range;
-    a->x = x; a->y = y; a->workspace = workspace;
-    return 0;
-}
-
-int srf_ms_ssim_workspace_bytes(int B, int C, int H, int W, size_t* bytes) {
-    if (ms_ssim_sizes("srf_ms_ssim_workspace_bytes", B, C, H, W)) return 1;
-    if (!bytes) return fail("srf_ms_ssim_workspace_bytes: null pointer");
-    *bytes = srf::ms_ssim_workspace_bytes(B, C, H, W);
-    return 0;
-}
-
-int srf_ms_ssim_workspace_layout(int B, int C, int H, int W, size_t regions[7], size_t levels[15], int dims[30]) {
-    if (ms_ssim_sizes("srf_ms_ssim_workspace_layout", B, C, H, W)) return 1;
-    if (!regions || !levels || !dims) return fail("srf_ms_ssim_workspace_layout: null pointer");
-    srf::ms_ssim_workspace_layout(B, C, H, W, regions, levels, dims);
-    return 0;
-}
-
-int srf_ms_ssim_forward(srf_stream_t stream_, int B, int C, int H, int W,
-                        const float* x, const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
-                        float data_range, int size_average, void* workspace, float* out) {
-    const char* fn = "srf_ms_ssim_forward";
-    srf::MsSsimArgs a;
-    if (ms_ssim_prepare(fn, B, C, H, W, x, x_addr, y, y_addr, data_range, size_average, workspace, &a)) return 1;
-    if (!out) return fail("%s: null output pointer", fn);
-    a.out = out;
-    cudaError_t e = srf::launch_ms_ssim(a, false, static_cast<cudaStream_t>(stream_));
-    if (e != cudaSuccess) return cuda_fail("ms_ssim_fwd launch", e);
-    return 0;
-}
-
-int srf_ms_ssim_backward(srf_stream_t stream_, int B, int C, int H, int W,
-                         const float* x, const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
-                         float data_range, int size_average, void* workspace, const float* upstream,
-                         float* dx, const srf_ms_ssim_addr* dx_addr) {
-    const char* fn = "srf_ms_ssim_backward";
-    srf::MsSsimArgs a;
-    if (ms_ssim_prepare(fn, B, C, H, W, x, x_addr, y, y_addr, data_range, size_average, workspace, &a)) return 1;
-    if (!upstream) return fail("%s: null upstream gradient", fn);
-    if (ms_ssim_addr(fn, "dx", dx, dx_addr, &a.ag)) return 1;
-    a.gout = upstream; a.gx = dx;
-    cudaError_t e = srf::launch_ms_ssim(a, true, static_cast<cudaStream_t>(stream_));
-    if (e != cudaSuccess) return cuda_fail("ms_ssim_bwd launch", e);
     return 0;
 }
 
@@ -817,11 +541,11 @@ int srf_mark_visible(srf_stream_t stream_, int P, const float* means3D,
                      const float* viewmatrix, const float* projmatrix, uint8_t* present) {
     (void)projmatrix;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    if (P < 0) return fail("srf_mark_visible: bad P");
+    if (P < 0) return set_error("srf_mark_visible: bad P");
     if (P == 0) return 0;
-    if (!means3D || !viewmatrix || !present) return fail("srf_mark_visible: null pointer");
+    if (!means3D || !viewmatrix || !present) return set_error("srf_mark_visible: null pointer");
     cudaError_t e = srf::launch_mark_visible(P, means3D, viewmatrix, present, stream);
-    if (e != cudaSuccess) return cuda_fail("mark_visible launch", e);
+    if (e != cudaSuccess) return cuda_error("mark_visible launch", e);
     return 0;
 }
 

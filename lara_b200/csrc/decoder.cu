@@ -12,10 +12,25 @@
 // Gaussian once (rows staged through shared memory with 128-bit loads) and writes the five tensors in the
 // 16/8-byte aligned row layout preprocess_fwd_kernel loads with vector instructions; the backward is the
 // mirror image (five gradient tensors in, one [B,N,K*C] gradient out, sigmoid vjp applied in registers).
+// The C entries srf_decoder_layout_forward / _backward (include/surfel_rasterizer.h) are defined here.
+#include <string.h>
+
+#include "../../include/surfel_rasterizer.h"
 #include "surfel_common.cuh"
 #include "surfel_kernels.h"
 
 namespace srf {
+
+struct DecoderArgs {
+    size_t total;                // B * N * K Gaussians
+    int N, K, C, sh_dim;         // voxels per scene, Gaussians per voxel, floats per row (10 + sh_dim), SH floats
+    float opacity_shift, scaling_shift, half_cell;
+    const float* params;         // [B,N,K*C] MLP output (fp32)
+    const float* group_centers;  // [N,3]
+    float* centers; float* shs; float* opacity; float* scaling; float* rotation;     // forward outputs
+    const float* g_centers; const float* g_shs; const float* g_opacity; const float* g_scaling; const float* g_rotation;
+    float* g_params;             // [B,N,K*C] backward output
+};
 
 __device__ __forceinline__ float dec_sigmoid(float x) { return __fdiv_rn(1.0f, 1.0f + expf(-x)); }   // torch's CUDA sigmoid
 
@@ -95,21 +110,58 @@ __global__ void __launch_bounds__(256) decoder_layout_kernel(DecoderArgs a) {
     }
 }
 
-cudaError_t launch_decoder_layout(const DecoderArgs& a, bool backward, cudaStream_t stream) {
-    if (a.total == 0) return cudaSuccess;
+}  // namespace srf
+
+using srf::cuda_error;
+using srf::set_error;
+
+extern "C" int srf_decoder_layout_forward(srf_stream_t stream, size_t B, int N, int K, int sh_dim,
+                                          float opacity_shift, float scaling_shift, float half_cell_size,
+                                          const float* params, const float* group_centers, float* centers, float* shs,
+                                          float* opacity, float* scaling, float* rotation) {
+    if (N <= 0 || K <= 0 || sh_dim < 3 || sh_dim % 3 != 0) return set_error("srf_decoder_layout_forward: bad sizes");
+    if (!params || !group_centers || !centers || !shs || !opacity || !scaling || !rotation)
+        return set_error("srf_decoder_layout_forward: null pointer");
+    if ((reinterpret_cast<uintptr_t>(rotation) & 15) || (reinterpret_cast<uintptr_t>(scaling) & 7) ||
+        ((sh_dim & 3) == 0 && (reinterpret_cast<uintptr_t>(shs) & 15)))
+        return set_error("srf_decoder_layout_forward: outputs must be 16-byte aligned");
+    srf::DecoderArgs a;
+    memset(&a, 0, sizeof(a));
+    a.total = B * (size_t)N * (size_t)K; a.N = N; a.K = K; a.C = 10 + sh_dim; a.sh_dim = sh_dim;
+    a.opacity_shift = opacity_shift; a.scaling_shift = scaling_shift; a.half_cell = half_cell_size;
+    a.params = params; a.group_centers = group_centers;
+    a.centers = centers; a.shs = shs; a.opacity = opacity; a.scaling = scaling; a.rotation = rotation;
+    if (a.total == 0) return 0;
     const size_t smem = (size_t)256 * a.C * sizeof(float);
-    const unsigned grid = (unsigned)((a.total + 255) / 256);
-    cudaError_t e;
-    if (backward) {
-        e = cudaFuncSetAttribute(decoder_layout_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        decoder_layout_kernel<true><<<grid, 256, smem, stream>>>(a);
-    } else {
-        e = cudaFuncSetAttribute(decoder_layout_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        decoder_layout_kernel<false><<<grid, 256, smem, stream>>>(a);
+    cudaError_t e = cudaFuncSetAttribute(srf::decoder_layout_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem);
+    if (e == cudaSuccess) {
+        srf::decoder_layout_kernel<false><<<(unsigned)((a.total + 255) / 256), 256, smem, (cudaStream_t)stream>>>(a);
+        e = cudaGetLastError();
     }
-    return cudaGetLastError();
+    return e == cudaSuccess ? 0 : cuda_error("decoder_layout launch", e);
 }
 
-}  // namespace srf
+extern "C" int srf_decoder_layout_backward(srf_stream_t stream, size_t B, int N, int K, int sh_dim,
+                                           float half_cell_size, const float* params, const float* g_centers,
+                                           const float* g_shs, const float* g_opacity, const float* g_scaling,
+                                           const float* g_rotation, float* g_params) {
+    if (N <= 0 || K <= 0 || sh_dim < 3 || sh_dim % 3 != 0) return set_error("srf_decoder_layout_backward: bad sizes");
+    if (!params || !g_params) return set_error("srf_decoder_layout_backward: null pointer");
+    srf::DecoderArgs a;
+    memset(&a, 0, sizeof(a));
+    a.total = B * (size_t)N * (size_t)K; a.N = N; a.K = K; a.C = 10 + sh_dim; a.sh_dim = sh_dim;
+    a.half_cell = half_cell_size;
+    a.params = params;
+    a.g_centers = g_centers; a.g_shs = g_shs; a.g_opacity = g_opacity; a.g_scaling = g_scaling; a.g_rotation = g_rotation;
+    a.g_params = g_params;
+    if (a.total == 0) return 0;
+    const size_t smem = (size_t)256 * a.C * sizeof(float);
+    cudaError_t e = cudaFuncSetAttribute(srf::decoder_layout_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem);
+    if (e == cudaSuccess) {
+        srf::decoder_layout_kernel<true><<<(unsigned)((a.total + 255) / 256), 256, smem, (cudaStream_t)stream>>>(a);
+        e = cudaGetLastError();
+    }
+    return e == cudaSuccess ? 0 : cuda_error("decoder_layout backward launch", e);
+}

@@ -10,11 +10,40 @@
 //
 // Layouts: color [3,H,W], allmap [8,H,W], rays [H,W,6] (origin xyz, direction xyz),
 // viewmatrix [16] (row-major memory of world_view_transform = w2c^T).  Outputs are planar
-// [C,H,W]; the Python layer returns the .permute(1,2,0) views the reference returns.
+// [C,H,W]; the Python layer returns the .permute(1,2,0) views the reference returns.  The C entries
+// srf_views_epilogue_forward / _backward (include/surfel_rasterizer.h) are defined here.
+#include <string.h>
+
+#include "../../include/surfel_rasterizer.h"
 #include "surfel_common.cuh"
 #include "surfel_kernels.h"
 
 namespace srf {
+
+// all images planar [V,C,H,W] fp32
+struct EpilogueArgs {
+    int W, H;
+    int nviews;
+    float depth_ratio;
+    const float* color;          // [V,3,H,W] rasterizer colour
+    const float* allmap;         // [V,8,H,W] rasterizer aux maps
+    const float* rays;           // [V,H,W,6] or null (then no pseudo normals)
+    const float* viewmatrix;     // [16] per view, cam_stride floats apart
+    size_t cam_stride;
+    // forward outputs
+    float* image;                // [V,3,H,W]
+    float* depth;                // [V,1,H,W]
+    float* acc;                  // [V,H,W]
+    float* rend_normal;          // [V,3,H,W]
+    float* depth_normal;         // [V,3,H,W]
+    float* dist;                 // [V,H,W]
+    // backward inputs (any may be null = zero) and outputs
+    const float* g_image; const float* g_depth; const float* g_acc;
+    const float* g_rend_normal; const float* g_depth_normal; const float* g_dist;
+    float* scratch;              // [V,3,H,W]
+    float* dL_dcolor;            // [V,3,H,W]
+    float* dL_dallmap;           // [V,8,H,W]
+};
 
 __device__ __forceinline__ float nan_to_num0(float v) {
     // torch.nan_to_num(v, nan=0, posinf=0): NaN and +inf -> 0, -inf -> lowest finite
@@ -194,17 +223,53 @@ __global__ void __launch_bounds__(256) epilogue_bwd_kernel(EpilogueArgs a) {
     a.dL_dallmap[pix + 7 * npix] = 0.0f;
 }
 
-cudaError_t launch_epilogue_fwd(const EpilogueArgs& a, cudaStream_t stream) {
-    const dim3 grid((a.W + 31) / 32, (a.H + 7) / 8, a.nviews > 0 ? a.nviews : 1);
-    epilogue_fwd_kernel<<<grid, 256, 0, stream>>>(a);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_epilogue_bwd(const EpilogueArgs& a, cudaStream_t stream) {
-    const dim3 grid((a.W + 31) / 32, (a.H + 7) / 8, a.nviews > 0 ? a.nviews : 1);
-    if (a.g_depth_normal != nullptr && a.rays != nullptr) epilogue_bwd_cross_kernel<<<grid, 256, 0, stream>>>(a);
-    epilogue_bwd_kernel<<<grid, 256, 0, stream>>>(a);
-    return cudaGetLastError();
-}
-
 }  // namespace srf
+
+using srf::cuda_error;
+using srf::set_error;
+
+extern "C" int srf_views_epilogue_forward(srf_stream_t stream, int V, int image_height, int image_width,
+                                          float depth_ratio, const float* color, const float* allmap, const float* rays,
+                                          const float* cams, float* image, float* depth, float* acc_map,
+                                          float* rend_normal, float* depth_normal, float* rend_dist) {
+    const char* fn = "srf_views_epilogue_forward";
+    if (V <= 0 || image_height <= 0 || image_width <= 0) return set_error("%s: bad sizes", fn);
+    if (!color || !allmap || !cams || !image || !depth || !acc_map || !rend_normal || !depth_normal || !rend_dist)
+        return set_error("%s: null pointer", fn);
+    srf::EpilogueArgs a;
+    memset(&a, 0, sizeof(a));
+    a.W = image_width; a.H = image_height; a.nviews = V; a.depth_ratio = depth_ratio;
+    a.color = color; a.allmap = allmap; a.rays = rays; a.viewmatrix = cams + SRF_CAM_VIEW; a.cam_stride = SRF_CAM_FLOATS;
+    a.image = image; a.depth = depth; a.acc = acc_map; a.rend_normal = rend_normal; a.depth_normal = depth_normal;
+    a.dist = rend_dist;
+    const dim3 grid((a.W + 31) / 32, (a.H + 7) / 8, V);
+    srf::epilogue_fwd_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : cuda_error("epilogue_fwd launch", e);
+}
+
+extern "C" int srf_views_epilogue_backward(srf_stream_t stream_, int V, int image_height, int image_width,
+                                           float depth_ratio, const float* color, const float* allmap,
+                                           const float* rays, const float* cams, const float* g_image,
+                                           const float* g_depth, const float* g_acc_map, const float* g_rend_normal,
+                                           const float* g_depth_normal, const float* g_rend_dist, float* scratch,
+                                           float* dL_dcolor, float* dL_dallmap) {
+    const char* fn = "srf_views_epilogue_backward";
+    if (V <= 0 || image_height <= 0 || image_width <= 0) return set_error("%s: bad sizes", fn);
+    if (!color || !allmap || !cams || !dL_dcolor || !dL_dallmap) return set_error("%s: null pointer", fn);
+    if (g_depth_normal && rays && !scratch) return set_error("%s: scratch [V,3,H,W] required", fn);
+    srf::EpilogueArgs a;
+    memset(&a, 0, sizeof(a));
+    a.W = image_width; a.H = image_height; a.nviews = V; a.depth_ratio = depth_ratio;
+    a.color = color; a.allmap = allmap; a.rays = rays; a.viewmatrix = cams + SRF_CAM_VIEW; a.cam_stride = SRF_CAM_FLOATS;
+    a.g_image = g_image; a.g_depth = g_depth; a.g_acc = g_acc_map; a.g_rend_normal = g_rend_normal;
+    a.g_depth_normal = g_depth_normal; a.g_dist = g_rend_dist;
+    a.scratch = scratch; a.dL_dcolor = dL_dcolor; a.dL_dallmap = dL_dallmap;
+    const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    const dim3 grid((a.W + 31) / 32, (a.H + 7) / 8, V);
+    // pass 1 (the pseudo normals' cross-product gradients) only when they have a gradient
+    if (g_depth_normal && rays) srf::epilogue_bwd_cross_kernel<<<grid, 256, 0, stream>>>(a);
+    srf::epilogue_bwd_kernel<<<grid, 256, 0, stream>>>(a);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : cuda_error("epilogue_bwd launch", e);
+}

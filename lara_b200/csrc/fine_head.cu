@@ -545,15 +545,14 @@ int grid_for(int n) {
 }
 
 WsLayout ws_layout(int n, int D, int Sp, bool gather) {
-    auto up = [](size_t x) { return (x + 255) / 256 * 256; };
     const Layout l = layout(D, Sp);
     WsLayout w;
     w.parts = 0;
-    w.tot = up(w.parts + sizeof(float) * (size_t)grid_for(n) * l.nacc);
-    w.B = up(w.tot + sizeof(double) * l.nacc);
-    w.dB = up(w.B + sizeof(double) * D * kHK);
-    w.rows = up(w.dB + sizeof(double) * D * kHK);
-    w.total = up(w.rows + (gather ? sizeof(float) * (size_t)n * D : 0));
+    w.tot = align_up(w.parts + sizeof(float) * (size_t)grid_for(n) * l.nacc);
+    w.B = align_up(w.tot + sizeof(double) * l.nacc);
+    w.dB = align_up(w.B + sizeof(double) * D * kHK);
+    w.rows = align_up(w.dB + sizeof(double) * D * kHK);
+    w.total = align_up(w.rows + (gather ? sizeof(float) * (size_t)n * D : 0));
     return w;
 }
 
@@ -569,8 +568,6 @@ int check_sizes(const char* fn, int n, int V, int D, int sh_dim, int K, int N, b
     return 0;
 }
 
-bool misaligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 255) != 0; }
-
 void fill_common(Args& a, int n, int V, int D, int sh_dim, int K, int N, const float* vf, const int* idx,
                  const float* pf, const float* ln_w, const float* ln_b, const float* wq, const float* wk,
                  const float* wv, const float* wo, const float* w1, const float* b1, const float* w2, const float* b2) {
@@ -583,6 +580,7 @@ void fill_common(Args& a, int n, int V, int D, int sh_dim, int K, int N, const f
 }  // namespace
 }  // namespace srf
 
+using srf::cuda_error;
 using srf::set_error;
 
 extern "C" int srf_fine_head_workspace_bytes(int n, int V, int D, int sh_dim, int gather, size_t* bytes) {
@@ -614,10 +612,10 @@ extern "C" int srf_fine_head_forward(void* stream, int n, int V, int D, int sh_d
     a.out = sh_out;
     const size_t smem = sizeof(float) * srf::layout(D, a.Sp).fwd_floats;
     cudaError_t e = cudaFuncSetAttribute(srf::fine_head_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return set_error("fine_head_fwd shared memory: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return cuda_error("fine_head_fwd shared memory", e);
     srf::fine_head_fwd_kernel<<<srf::grid_for(n), srf::kThreads, smem, (cudaStream_t)stream>>>(a);
     e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : set_error("fine_head_fwd launch: %s", cudaGetErrorString(e));
+    return e == cudaSuccess ? 0 : cuda_error("fine_head_fwd launch", e);
 }
 
 extern "C" int srf_fine_head_backward(void* stream_, int n, int V, int D, int sh_dim, int K, int N,
@@ -657,15 +655,15 @@ extern "C" int srf_fine_head_backward(void* stream_, int n, int V, int D, int sh
     cudaError_t e;
     if (dL_dshs_coarse && N > 0) {
         e = cudaMemsetAsync(dL_dshs_coarse, 0, sizeof(float) * (size_t)N * K * sh_dim, stream);
-        if (e != cudaSuccess) return set_error("memset dL_dshs_coarse: %s", cudaGetErrorString(e));
+        if (e != cudaSuccess) return cuda_error("memset dL_dshs_coarse", e);
     }
     const int grid = srf::grid_for(n);
     if (grid > 0) {
         const size_t smem = sizeof(float) * l.bwd_floats;
         e = cudaFuncSetAttribute(srf::fine_head_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return set_error("fine_head_bwd shared memory: %s", cudaGetErrorString(e));
+        if (e != cudaSuccess) return cuda_error("fine_head_bwd shared memory", e);
         srf::fine_head_bwd_kernel<<<grid, srf::kThreads, smem, stream>>>(a);
-        if ((e = cudaGetLastError()) != cudaSuccess) return set_error("fine_head_bwd launch: %s", cudaGetErrorString(e));
+        if ((e = cudaGetLastError()) != cudaSuccess) return cuda_error("fine_head_bwd launch", e);
     }
     double* tot = reinterpret_cast<double*>(ws + w.tot);
     srf::fine_head_reduce_kernel<<<(l.nacc + 255) / 256, 256, 0, stream>>>(a.partials, grid, l.nacc, tot);
@@ -680,5 +678,5 @@ extern "C" int srf_fine_head_backward(void* stream_, int n, int V, int D, int sh
                                                                                              dL_dvolume_feat);
     }
     e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : set_error("fine_head backward launch: %s", cudaGetErrorString(e));
+    return e == cudaSuccess ? 0 : cuda_error("fine_head backward launch", e);
 }

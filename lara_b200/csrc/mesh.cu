@@ -109,17 +109,16 @@ __global__ void __launch_bounds__(kMeshThreads) tsdf_integrate_kernel(IntegrateA
 struct Workspace { size_t edge, tri, cases, sums, total; size_t n_edge, n_cube, nb_edge, nb_cube; };
 
 Workspace workspace_layout(size_t N) {
-    auto up = [](size_t x) { return (x + 255) / 256 * 256; };
     Workspace l;
     l.n_edge = 3 * N;
     l.n_cube = N;
     l.nb_edge = (l.n_edge + kScanTile - 1) / kScanTile;
     l.nb_cube = (l.n_cube + kScanTile - 1) / kScanTile;
-    l.edge = 0;                                           // u32 [3N + 1]: crossing flags, then vertex ids; [3N] = Nv
-    l.tri = up(l.edge + 4 * (l.n_edge + 1));              // u32 [N + 1]: triangle counts, then offsets;  [N] = Nt
-    l.cases = up(l.tri + 4 * (l.n_cube + 1));             // u8 [N]: sign case of each valid cube, 0 otherwise
-    l.sums = up(l.cases + l.n_cube);                      // u32 [nb_edge + nb_cube]: per-tile sums of the scans
-    l.total = up(l.sums + 4 * (l.nb_edge + l.nb_cube));
+    l.edge = 0;                                             // u32 [3N + 1]: crossing flags, then vertex ids; [3N] = Nv
+    l.tri = align_up(l.edge + 4 * (l.n_edge + 1));          // u32 [N + 1]: triangle counts, then offsets;  [N] = Nt
+    l.cases = align_up(l.tri + 4 * (l.n_cube + 1));         // u8 [N]: sign case of each valid cube, 0 otherwise
+    l.sums = align_up(l.cases + l.n_cube);                  // u32 [nb_edge + nb_cube]: per-tile sums of the scans
+    l.total = align_up(l.sums + 4 * (l.nb_edge + l.nb_cube));
     return l;
 }
 
@@ -314,11 +313,10 @@ int check_grid(const char* fn, const int* n0, const int* dims, Grid& g) {
     return 0;
 }
 
-bool misaligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 255) != 0; }
-
 }  // namespace
 }  // namespace srf
 
+using srf::cuda_error;
 using srf::set_error;
 
 extern "C" int srf_tsdf_integrate(void* stream, const int* n0, const int* dims, float voxel_size, float sdf_trunc,
@@ -342,7 +340,7 @@ extern "C" int srf_tsdf_integrate(void* stream, const int* n0, const int* dims, 
     const size_t blocks = (a.g.N + srf::kMeshThreads - 1) / srf::kMeshThreads;
     srf::tsdf_integrate_kernel<<<(unsigned)blocks, srf::kMeshThreads, 0, (cudaStream_t)stream>>>(a);
     const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : set_error("tsdf_integrate launch: %s", cudaGetErrorString(e));
+    return e == cudaSuccess ? 0 : cuda_error("tsdf_integrate launch", e);
 }
 
 extern "C" int srf_mesh_workspace_bytes(const int* dims, size_t* bytes) {
@@ -369,13 +367,13 @@ extern "C" int srf_mesh_count(void* stream_, const int* dims, const float* tsdf,
     a.cases = reinterpret_cast<uint8_t*>(ws + l.cases);
     uint32_t* sums = reinterpret_cast<uint32_t*>(ws + l.sums);
     cudaError_t e = cudaMemsetAsync(a.edge, 0, 4 * l.n_edge, stream);
-    if (e != cudaSuccess) return set_error("memset mesh edge flags: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return cuda_error("memset mesh edge flags", e);
     const size_t blocks = (a.g.N + srf::kMeshThreads - 1) / srf::kMeshThreads;
     srf::mesh_classify_kernel<<<(unsigned)blocks, srf::kMeshThreads, 0, stream>>>(a);
-    if ((e = cudaGetLastError()) != cudaSuccess) return set_error("mesh_classify launch: %s", cudaGetErrorString(e));
+    if ((e = cudaGetLastError()) != cudaSuccess) return cuda_error("mesh_classify launch", e);
     if ((e = srf::exclusive_scan(a.edge, l.n_edge, sums, l.nb_edge, totals, stream)) != cudaSuccess ||
         (e = srf::exclusive_scan(a.tri, l.n_cube, sums + l.nb_edge, l.nb_cube, totals + 1, stream)) != cudaSuccess)
-        return set_error("mesh scan launch: %s", cudaGetErrorString(e));
+        return cuda_error("mesh scan launch", e);
     return 0;
 }
 
@@ -403,5 +401,5 @@ extern "C" int srf_mesh_emit(void* stream, const int* n0, const int* dims, float
     const size_t blocks = (a.g.N + srf::kMeshThreads - 1) / srf::kMeshThreads;
     srf::mesh_emit_kernel<<<(unsigned)blocks, srf::kMeshThreads, 0, (cudaStream_t)stream>>>(a);
     const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : set_error("mesh_emit launch: %s", cudaGetErrorString(e));
+    return e == cudaSuccess ? 0 : cuda_error("mesh_emit launch", e);
 }

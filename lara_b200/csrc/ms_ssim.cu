@@ -17,13 +17,29 @@
 //                        and adds the pooling backward: dX_l = G^T A + 2 X G^T B + Y G^T C + dX_{l+1}(parent) / 4.
 // No atomics anywhere: two identical calls give identical bits.  The level-0 image is read (and its gradient
 // written) through MsAddr, so a channel-last tensor and V planar views side by side are read in place.
+// The C entries srf_ms_ssim_* (include/surfel_rasterizer.h) are defined here.
 #include <math.h>
 #include <string.h>
 
+#include "../../include/surfel_rasterizer.h"
 #include "surfel_common.cuh"
 #include "surfel_kernels.h"
 
 namespace srf {
+
+// A logical B x C x H x W image read through element strides; column x of the logical image lies in view x / wv at
+// column x % wv.
+struct MsAddr { long long sb, sc, sy, sx, sv; int wv; };
+struct MsSsimArgs {
+    int B, C, H, W;
+    int size_average;            // out[0] = mean over (b, c); else out[b] = mean over c
+    float data_range;
+    const float* x; const float* y; MsAddr ax, ay;
+    void* workspace;             // srf_ms_ssim_workspace_bytes: pyramid, its gradient, partial sums, coefficients
+    float* out;                  // forward output
+    const float* gout;           // backward: upstream gradient of out (device)
+    float* gx; MsAddr ag;        // backward output, dL/dX
+};
 
 namespace {
 
@@ -31,8 +47,6 @@ constexpr int kTW = 32, kTH = 16;          // tile of output pixels (forward) / 
 constexpr int kR = 10;                     // window size - 1
 constexpr int kThreads = 256;
 constexpr int kLevels = 5;
-
-inline size_t align_up(size_t x) { return (x + 255) / 256 * 256; }
 
 struct Layout {
     int h[kLevels], w[kLevels];
@@ -402,50 +416,118 @@ LevelArgs level_args(const MsSsimArgs& m, const Layout& L, char* ws, int l) {
 
 }  // namespace
 
-size_t ms_ssim_workspace_bytes(int B, int C, int H, int W) { return make_layout(B, C, H, W).total; }
+}  // namespace srf
 
-void ms_ssim_workspace_layout(int B, int C, int H, int W, size_t regions[7], size_t levels[15], int dims[30]) {
-    const Layout L = make_layout(B, C, H, W);
-    const size_t r[7] = {L.o_pyr, L.o_gpyr, L.o_part, L.o_mean, L.o_val, L.o_coef, L.total};
-    for (int i = 0; i < 7; ++i) regions[i] = r[i];
-    for (int l = 0; l < kLevels; ++l) {
-        levels[l] = L.pyr[l]; levels[kLevels + l] = L.gpyr[l]; levels[2 * kLevels + l] = L.part[l];
-        const int d[6] = {L.h[l], L.w[l], L.px[l], L.py[l], L.ntx[l], L.nty[l]};
-        for (int i = 0; i < 6; ++i) dims[i * kLevels + l] = d[i];
-    }
+using srf::cuda_error;
+using srf::set_error;
+
+static int ms_ssim_sizes(const char* fn, int B, int C, int H, int W) {
+    if (B <= 0 || C <= 0 || H <= 0 || W <= 0) return set_error("%s: bad sizes (B=%d, C=%d, H=%d, W=%d)", fn, B, C, H, W);
+    if ((H < W ? H : W) <= 160)
+        return set_error("%s: Image size should be larger than 160 due to the 4 downsamplings in ms-ssim (H=%d, W=%d)", fn, H, W);
+    if ((long long)B * C > 65535) return set_error("%s: B*C=%lld planes exceeds 65535", fn, (long long)B * C);
+    return 0;
 }
 
-cudaError_t launch_ms_ssim(const MsSsimArgs& m, bool backward, cudaStream_t stream) {
-    const Layout L = make_layout(m.B, m.C, m.H, m.W);
-    char* ws = static_cast<char*>(m.workspace);
-    const int planes = m.B * m.C;
+static int ms_ssim_addr(const char* fn, const char* what, const float* p, const srf_ms_ssim_addr* a, srf::MsAddr* out) {
+    if (!p || !a) return set_error("%s: null %s pointer", fn, what);
+    if (reinterpret_cast<uintptr_t>(p) & 3) return set_error("%s: %s must be 4-byte aligned", fn, what);
+    if (a->wv <= 0 || a->wv > 0x7fffffff) return set_error("%s: %s view width %lld out of range", fn, what, (long long)a->wv);
+    out->sb = a->sb; out->sc = a->sc; out->sy = a->sy; out->sx = a->sx; out->sv = a->sv; out->wv = (int)a->wv;
+    return 0;
+}
+
+static int ms_ssim_prepare(const char* fn, int B, int C, int H, int W, const float* x, const srf_ms_ssim_addr* x_addr,
+                           const float* y, const srf_ms_ssim_addr* y_addr, float data_range, int size_average,
+                           void* workspace, srf::MsSsimArgs* a) {
+    memset(a, 0, sizeof(*a));
+    if (ms_ssim_sizes(fn, B, C, H, W)) return 1;
+    if (ms_ssim_addr(fn, "x", x, x_addr, &a->ax) || ms_ssim_addr(fn, "y", y, y_addr, &a->ay)) return 1;
+    if (!(data_range > 0.f) || !(data_range < 3.0e38f)) return set_error("%s: data_range must be positive and finite", fn);
+    if (!workspace || srf::misaligned(workspace)) return set_error("%s: workspace must be 256-byte aligned", fn);
+    a->B = B; a->C = C; a->H = H; a->W = W; a->size_average = size_average ? 1 : 0; a->data_range = data_range;
+    a->x = x; a->y = y; a->workspace = workspace;
+    return 0;
+}
+
+extern "C" int srf_ms_ssim_workspace_bytes(int B, int C, int H, int W, size_t* bytes) {
+    if (ms_ssim_sizes("srf_ms_ssim_workspace_bytes", B, C, H, W)) return 1;
+    if (!bytes) return set_error("srf_ms_ssim_workspace_bytes: null pointer");
+    *bytes = srf::make_layout(B, C, H, W).total;
+    return 0;
+}
+
+extern "C" int srf_ms_ssim_workspace_layout(int B, int C, int H, int W, size_t regions[7], size_t levels[15],
+                                            int dims[30]) {
+    if (ms_ssim_sizes("srf_ms_ssim_workspace_layout", B, C, H, W)) return 1;
+    if (!regions || !levels || !dims) return set_error("srf_ms_ssim_workspace_layout: null pointer");
+    const srf::Layout L = srf::make_layout(B, C, H, W);
+    const size_t r[7] = {L.o_pyr, L.o_gpyr, L.o_part, L.o_mean, L.o_val, L.o_coef, L.total};
+    for (int i = 0; i < 7; ++i) regions[i] = r[i];
+    for (int l = 0; l < srf::kLevels; ++l) {
+        levels[l] = L.pyr[l]; levels[srf::kLevels + l] = L.gpyr[l]; levels[2 * srf::kLevels + l] = L.part[l];
+        const int d[6] = {L.h[l], L.w[l], L.px[l], L.py[l], L.ntx[l], L.nty[l]};
+        for (int i = 0; i < 6; ++i) dims[i * srf::kLevels + l] = d[i];
+    }
+    return 0;
+}
+
+extern "C" int srf_ms_ssim_forward(srf_stream_t stream_, int B, int C, int H, int W, const float* x,
+                                   const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
+                                   float data_range, int size_average, void* workspace, float* out) {
+    using namespace srf;
+    const char* fn = "srf_ms_ssim_forward";
+    MsSsimArgs m;
+    if (ms_ssim_prepare(fn, B, C, H, W, x, x_addr, y, y_addr, data_range, size_average, workspace, &m)) return 1;
+    if (!out) return set_error("%s: null output pointer", fn);
+    m.out = out;
+    const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    const Layout L = make_layout(B, C, H, W);
+    char* ws = static_cast<char*>(workspace);
+    const int planes = B * C;
+    for (int l = 0; l < kLevels; ++l) {
+        LevelArgs a = level_args(m, L, ws, l);
+        a.ntx = L.ntx[l];
+        a.part = reinterpret_cast<double*>(ws + L.o_part) + L.part[l];
+        const dim3 grid((unsigned)(L.ntx[l] * L.nty[l]), (unsigned)planes);
+        if (l + 1 < kLevels) ms_ssim_fwd_kernel<false><<<grid, kThreads, 0, stream>>>(a);
+        else ms_ssim_fwd_kernel<true><<<grid, kThreads, 0, stream>>>(a);
+    }
+    FinalArgs f;
+    memset(&f, 0, sizeof(f));
+    f.B = B; f.C = C; f.planes = planes; f.size_average = m.size_average;
+    for (int l = 0; l < kLevels; ++l) {
+        f.ntiles[l] = L.ntx[l] * L.nty[l];
+        f.part_off[l] = L.part[l];
+        f.count[l] = (double)(L.h[l] - kR) * (double)(L.w[l] - kR);
+    }
+    f.part = reinterpret_cast<const double*>(ws + L.o_part);
+    f.mean = reinterpret_cast<double*>(ws + L.o_mean);
+    f.val = reinterpret_cast<double*>(ws + L.o_val);
+    f.coef = reinterpret_cast<float*>(ws + L.o_coef);
+    f.out = out;
+    ms_ssim_finalize_kernel<<<1, kThreads, 0, stream>>>(f);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : cuda_error("ms_ssim_fwd launch", e);
+}
+
+extern "C" int srf_ms_ssim_backward(srf_stream_t stream_, int B, int C, int H, int W, const float* x,
+                                    const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
+                                    float data_range, int size_average, void* workspace, const float* upstream,
+                                    float* dx, const srf_ms_ssim_addr* dx_addr) {
+    using namespace srf;
+    const char* fn = "srf_ms_ssim_backward";
+    MsSsimArgs m;
+    if (ms_ssim_prepare(fn, B, C, H, W, x, x_addr, y, y_addr, data_range, size_average, workspace, &m)) return 1;
+    if (!upstream) return set_error("%s: null upstream gradient", fn);
+    if (ms_ssim_addr(fn, "dx", dx, dx_addr, &m.ag)) return 1;
+    m.gout = upstream; m.gx = dx;
+    const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    const Layout L = make_layout(B, C, H, W);
+    char* ws = static_cast<char*>(workspace);
+    const int planes = B * C;
     float* coef = reinterpret_cast<float*>(ws + L.o_coef);
     float* gpyr = reinterpret_cast<float*>(ws + L.o_gpyr);
-    if (!backward) {
-        for (int l = 0; l < kLevels; ++l) {
-            LevelArgs a = level_args(m, L, ws, l);
-            a.ntx = L.ntx[l];
-            a.part = reinterpret_cast<double*>(ws + L.o_part) + L.part[l];
-            const dim3 grid((unsigned)(L.ntx[l] * L.nty[l]), (unsigned)planes);
-            if (l + 1 < kLevels) ms_ssim_fwd_kernel<false><<<grid, kThreads, 0, stream>>>(a);
-            else ms_ssim_fwd_kernel<true><<<grid, kThreads, 0, stream>>>(a);
-        }
-        FinalArgs f;
-        memset(&f, 0, sizeof(f));
-        f.B = m.B; f.C = m.C; f.planes = planes; f.size_average = m.size_average;
-        for (int l = 0; l < kLevels; ++l) {
-            f.ntiles[l] = L.ntx[l] * L.nty[l];
-            f.part_off[l] = L.part[l];
-            f.count[l] = (double)(L.h[l] - kR) * (double)(L.w[l] - kR);
-        }
-        f.part = reinterpret_cast<const double*>(ws + L.o_part);
-        f.mean = reinterpret_cast<double*>(ws + L.o_mean);
-        f.val = reinterpret_cast<double*>(ws + L.o_val);
-        f.coef = coef;
-        f.out = m.out;
-        ms_ssim_finalize_kernel<<<1, kThreads, 0, stream>>>(f);
-        return cudaGetLastError();
-    }
     for (int l = kLevels - 1; l >= 0; --l) {
         LevelArgs a = level_args(m, L, ws, l);
         a.ntx = (L.w[l] + kTW - 1) / kTW;
@@ -459,7 +541,6 @@ cudaError_t launch_ms_ssim(const MsSsimArgs& m, bool backward, cudaStream_t stre
         if (l + 1 < kLevels) ms_ssim_bwd_kernel<false><<<grid, kThreads, 0, stream>>>(a);
         else ms_ssim_bwd_kernel<true><<<grid, kThreads, 0, stream>>>(a);
     }
-    return cudaGetLastError();
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : cuda_error("ms_ssim_bwd launch", e);
 }
-
-}  // namespace srf

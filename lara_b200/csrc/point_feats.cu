@@ -17,11 +17,37 @@
 //
 // Backward: the upstream gradient g[V,8,n] is read coalesced; dL/dpoints[n,3] is summed over the views in registers
 // and written once; the gradients of the 5 differentiable channels go into planar g_image[V,3,H,W], g_acc[V,H,W]
-// and g_depth[V,H,W] with red.global.add.f32 (cleared by the caller).  No gradient is formed for img_ref.
+// and g_depth[V,H,W] with red.global.add.f32 (cleared by the entry).  No gradient is formed for img_ref.
+// The C entries srf_point_feats_* (include/surfel_rasterizer.h) are defined here.
+#include <string.h>
+
+#include "../../include/surfel_rasterizer.h"
 #include "det_sum.cuh"
 #include "surfel_kernels.h"
 
 namespace srf {
+
+// n points sampled in V source views from the 8-channel stack img_ref | image | acc | depth; all images planar fp32
+struct PointFeatsArgs {
+    int V, n, H, W;
+    const float* points;         // [n,3]
+    const float* w2cs;           // [V,4,4] row-major
+    const float* ixts;           // [V,3,3] row-major
+    const float* img_ref;        // [V,3,H,W]
+    const float* image;          // [V,3,H,W]
+    const float* acc;            // [V,H,W]
+    const float* depth;          // [V,H,W]
+    float* feats;                // [V,8,n] forward output
+    const float* g_feats;        // [V,8,n] backward input
+    float* g_points;             // [n,3] written (may be null)
+    float* g_image; float* g_acc; float* g_depth;   // accumulated into, cleared by the entry (each may be null)
+    // deterministic backward (null = default): int64 planes [5V,H,W] in the layout g_image | g_acc | g_depth and a
+    // header det[0] = max |g_feats| (fp32 bits), det[1] = overflow; both zeroed by the entry.  The float outputs are
+    // then written, not accumulated into.
+    long long* g_fixed;
+    uint32_t* det;
+};
+
 namespace {
 
 constexpr int kPfThreads = 256;
@@ -245,22 +271,90 @@ __global__ void __launch_bounds__(kPfThreads) point_feats_bwd_kernel(PointFeatsA
 
 }  // namespace
 
-cudaError_t launch_point_feats(const PointFeatsArgs& a, bool backward, cudaStream_t stream) {
-    if (a.n <= 0) return cudaSuccess;
-    const unsigned grid = (unsigned)((a.n + kPfThreads - 1) / kPfThreads);
-    if (!backward) {
-        point_feats_fwd_kernel<<<grid, kPfThreads, 0, stream>>>(a);
-    } else if (!a.g_fixed) {
-        point_feats_bwd_kernel<false><<<grid, kPfThreads, 0, stream>>>(a);
-    } else {
-        const size_t count = (size_t)a.V * 8 * a.n;
-        pf_bound_kernel<<<(unsigned)min((count + kPfThreads - 1) / kPfThreads, (size_t)sm_count() * 8), kPfThreads, 0, stream>>>(
-            a.g_feats, count, a.det);
-        point_feats_bwd_kernel<true><<<grid, kPfThreads, 0, stream>>>(a);
-        const size_t planes = 5 * (size_t)a.V * a.H * a.W;
-        pf_convert_kernel<<<(unsigned)((planes + kPfThreads - 1) / kPfThreads), kPfThreads, 0, stream>>>(a);
-    }
-    return cudaGetLastError();
+}  // namespace srf
+
+using srf::cuda_error;
+using srf::set_error;
+
+static int point_feats_check(const char* fn, int V, int n, int H, int W, const float* points, const float* w2cs,
+                             const float* ixts, const float* img_ref, const float* image, const float* acc,
+                             const float* depth) {
+    if (V <= 0 || n < 0 || H <= 0 || W <= 0) return set_error("%s: bad sizes (V=%d, n=%d, H=%d, W=%d)", fn, V, n, H, W);
+    if (H > (1 << 24) || W > (1 << 24)) return set_error("%s: image too large", fn);    // pixel indices exact in fp32
+    // an empty point set has no storage: points (and feats / g_feats) are only needed when n > 0
+    if ((n > 0 && !points) || !w2cs || !ixts || !img_ref || !image || !acc || !depth) return set_error("%s: null input pointer", fn);
+    return 0;
 }
 
-}  // namespace srf
+extern "C" int srf_point_feats_forward(srf_stream_t stream, int V, int n, int H, int W, const float* points,
+                                       const float* w2cs, const float* ixts, const float* img_ref, const float* image,
+                                       const float* acc, const float* depth, float* feats) {
+    const char* fn = "srf_point_feats_forward";
+    if (point_feats_check(fn, V, n, H, W, points, w2cs, ixts, img_ref, image, acc, depth)) return 1;
+    if (n > 0 && !feats) return set_error("%s: null output pointer", fn);
+    if (n == 0) return 0;
+    srf::PointFeatsArgs a;
+    memset(&a, 0, sizeof(a));
+    a.V = V; a.n = n; a.H = H; a.W = W;
+    a.points = points; a.w2cs = w2cs; a.ixts = ixts; a.img_ref = img_ref; a.image = image; a.acc = acc; a.depth = depth;
+    a.feats = feats;
+    const unsigned grid = (unsigned)((n + srf::kPfThreads - 1) / srf::kPfThreads);
+    srf::point_feats_fwd_kernel<<<grid, srf::kPfThreads, 0, static_cast<cudaStream_t>(stream)>>>(a);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : cuda_error("point_feats_fwd launch", e);
+}
+
+// deterministic workspace: header (max |g_feats|, overflow flag), then the int64 planes g_image | g_acc | g_depth
+static size_t pf_det_planes_offset() { return 256; }
+static size_t pf_det_workspace_bytes(int V, int H, int W) {
+    return pf_det_planes_offset() + 5 * (size_t)V * H * W * sizeof(long long);
+}
+
+extern "C" int srf_point_feats_backward(srf_stream_t stream_, int V, int n, int H, int W, const float* points,
+                                        const float* w2cs, const float* ixts, const float* img_ref, const float* image,
+                                        const float* acc, const float* depth, const float* g_feats, float* g_points,
+                                        float* g_image, float* g_acc, float* g_depth, void* workspace) {
+    const char* fn = "srf_point_feats_backward";
+    if (point_feats_check(fn, V, n, H, W, points, w2cs, ixts, img_ref, image, acc, depth)) return 1;
+    if (n > 0 && !g_feats) return set_error("%s: null upstream gradient", fn);
+    if (workspace && srf::misaligned(workspace)) return set_error("%s: workspace must be 256-byte aligned", fn);
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    const bool nothing = n == 0 || (!g_points && !g_image && !g_acc && !g_depth);
+    // the default path adds into cleared outputs; the deterministic one writes them from its fixed-point planes
+    if (!workspace || nothing) {
+        const size_t plane = (size_t)V * H * W * sizeof(float);
+        cudaError_t e = cudaSuccess;
+        if (g_image && (e = cudaMemsetAsync(g_image, 0, 3 * plane, stream)) != cudaSuccess) return cuda_error("memset g_image", e);
+        if (g_acc && (e = cudaMemsetAsync(g_acc, 0, plane, stream)) != cudaSuccess) return cuda_error("memset g_acc", e);
+        if (g_depth && (e = cudaMemsetAsync(g_depth, 0, plane, stream)) != cudaSuccess) return cuda_error("memset g_depth", e);
+    }
+    if (nothing) return 0;
+    srf::PointFeatsArgs a;
+    memset(&a, 0, sizeof(a));
+    a.V = V; a.n = n; a.H = H; a.W = W;
+    a.points = points; a.w2cs = w2cs; a.ixts = ixts; a.img_ref = img_ref; a.image = image; a.acc = acc; a.depth = depth;
+    a.g_feats = g_feats; a.g_points = g_points; a.g_image = g_image; a.g_acc = g_acc; a.g_depth = g_depth;
+    const unsigned grid = (unsigned)((n + srf::kPfThreads - 1) / srf::kPfThreads);
+    cudaError_t e;
+    if (!workspace) {
+        srf::point_feats_bwd_kernel<false><<<grid, srf::kPfThreads, 0, stream>>>(a);
+    } else {
+        e = cudaMemsetAsync(workspace, 0, pf_det_workspace_bytes(V, H, W), stream);
+        if (e != cudaSuccess) return cuda_error("memset point_feats workspace", e);
+        a.det = static_cast<uint32_t*>(workspace);
+        a.g_fixed = reinterpret_cast<long long*>(static_cast<char*>(workspace) + pf_det_planes_offset());
+        const size_t count = (size_t)V * 8 * n, planes = 5 * (size_t)V * H * W;
+        srf::pf_bound_kernel<<<(unsigned)min((count + srf::kPfThreads - 1) / srf::kPfThreads, (size_t)srf::sm_count() * 8),
+                               srf::kPfThreads, 0, stream>>>(a.g_feats, count, a.det);
+        srf::point_feats_bwd_kernel<true><<<grid, srf::kPfThreads, 0, stream>>>(a);
+        srf::pf_convert_kernel<<<(unsigned)((planes + srf::kPfThreads - 1) / srf::kPfThreads), srf::kPfThreads, 0, stream>>>(a);
+    }
+    if ((e = cudaGetLastError()) != cudaSuccess) return cuda_error("point_feats_bwd launch", e);
+    return workspace ? srf::check_overflow_flag(fn, a.det + 1, stream) : 0;
+}
+
+extern "C" int srf_point_feats_deterministic_workspace_bytes(int V, int H, int W, size_t* bytes) {
+    if (V <= 0 || H <= 0 || W <= 0 || !bytes) return set_error("srf_point_feats_deterministic_workspace_bytes: bad arguments");
+    *bytes = pf_det_workspace_bytes(V, H, W);
+    return 0;
+}

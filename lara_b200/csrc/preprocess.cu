@@ -12,6 +12,7 @@
 // directly counts instances per tile (tile_count[]), the first half of the
 // tile-bucketed binning that replaces the reference's global 64-bit radix sort.
 #include <cuda_fp16.h>
+#include <stdio.h>
 
 #include "surfel_common.cuh"
 #include "surfel_kernels.h"

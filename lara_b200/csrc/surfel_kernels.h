@@ -1,7 +1,9 @@
-// surfel_kernels.h -- internal (non-ABI) interface between the C-ABI layer (api.cu)
-// and the kernel translation units.  The public boundary is include/surfel_rasterizer.h.
+// surfel_kernels.h -- internal (non-ABI) interface of the library: the rasterizer's kernel launchers, which api.cu's
+// srf_views_* entries call, and the host helpers every translation unit's extern "C" entries share.  The public
+// boundary is include/surfel_rasterizer.h (and surfel_mesh.h, surfel_fine_head.h); each fused op (epilogue, loss,
+// decoder layout, point features, MS-SSIM, mesh, fine head) keeps its argument structs and entries in its own .cu.
 //
-// Every kernel takes a *view* dimension: the V target views of one scene share the Gaussian set
+// Every rasterizer kernel takes a *view* dimension: the V target views of one scene share the Gaussian set
 // (reference caller loop lightning/network.py:484-497), so one launch covers all of them.  Per-view
 // arrays live in per-view workspaces of identical layout; the structs carry the base pointers of view 0
 // plus the byte stride from one view's workspace to the next (`*_stride`).  Camera data (view matrix,
@@ -9,24 +11,23 @@
 // SRF_CAM_*), the records `cam_stride` floats apart.  Images are stacked [V,C,H,W].
 #pragma once
 #include <cuda_runtime.h>
-#include <stdarg.h>
+#include <stddef.h>
 #include <stdint.h>
-#include <stdio.h>
-
-extern "C" const char* srf_last_error(void);
 
 namespace srf {
 
-// Report a failure from a translation unit other than api.cu: the text goes to the thread-local buffer srf_last_error()
-// returns (api.cu's, kErrorBytes long).  Returns 1, the C ABI's failure status.
-constexpr size_t kErrorBytes = 512;
-inline int set_error(const char* fmt, ...) {
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(const_cast<char*>(srf_last_error()), kErrorBytes, fmt, ap);
-    va_end(ap);
-    return 1;
-}
+// ---- host helpers of the extern "C" entries ----
+// Record a failure: the text goes to the thread-local buffer srf_last_error() returns.  Returns 1, the C ABI's
+// failure status.
+int set_error(const char* fmt, ...) __attribute__((format(printf, 1, 2)));
+// a CUDA call's failure as "<what>: <CUDA error string>"
+inline int cuda_error(const char* what, cudaError_t e) { return set_error("%s: %s", what, cudaGetErrorString(e)); }
+// workspaces are 256-byte aligned, and so are the regions inside them
+inline bool misaligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 255) != 0; }
+inline size_t align_up(size_t x) { return (x + 255) / 256 * 256; }
+// Reads a device flag that the work enqueued so far sets (waits for the stream); set means a deterministic
+// fixed-point sum overflowed, reported as a failure of `fn`.
+int check_overflow_flag(const char* fn, const uint32_t* flag, cudaStream_t stream);
 
 // pointer of view `v` given the pointer of view 0 and a byte stride
 template <typename T>
@@ -146,109 +147,6 @@ struct PreprocessBwdArgs {
     float* dL_drotations;        // [P,4]
     float* dL_dtransMat;         // [P,9] or null
 };
-
-// Fused render_img epilogue (SURVEY 8f rank 2); all images planar [V,C,H,W] fp32.
-struct EpilogueArgs {
-    int W, H;
-    int nviews;
-    float depth_ratio;
-    const float* color;          // [V,3,H,W] rasterizer colour
-    const float* allmap;         // [V,8,H,W] rasterizer aux maps
-    const float* rays;           // [V,H,W,6] or null (then no pseudo normals)
-    const float* viewmatrix;     // [16] per view, cam_stride floats apart
-    size_t cam_stride;
-    // forward outputs
-    float* image;                // [V,3,H,W]
-    float* depth;                // [V,1,H,W]
-    float* acc;                  // [V,H,W]
-    float* rend_normal;          // [V,3,H,W]
-    float* depth_normal;         // [V,3,H,W]
-    float* dist;                 // [V,H,W]
-    // backward inputs (any may be null = zero) and outputs
-    const float* g_image; const float* g_depth; const float* g_acc;
-    const float* g_rend_normal; const float* g_depth_normal; const float* g_dist;
-    float* scratch;              // [V,3,H,W]
-    float* dL_dcolor;            // [V,3,H,W]
-    float* dL_dallmap;           // [V,8,H,W]
-};
-cudaError_t launch_epilogue_fwd(const EpilogueArgs& a, cudaStream_t stream);
-cudaError_t launch_epilogue_bwd(const EpilogueArgs& a, cudaStream_t stream);
-
-// Fused loss -> dL/d(render_img outputs) producer (SURVEY 8f rank 3, lightning/loss.py:33-60).
-struct LossArgs {
-    int W, H, nviews;
-    int with_reg;                // iter > 1000: distortion and normal-consistency terms are on
-    float w_mse, w_dist, w_normal;   // weights already divided by the reference's mean() denominators
-    const float* image;          // [V,3,H,W]
-    const float* target;         // [V,H,W,3] channel-last, the batch's own layout
-    const float* rend_normal;    // [V,3,H,W]
-    const float* depth_normal;   // [V,3,H,W]
-    const float* acc;            // [V,H,W]
-    const float* dist;           // [V,H,W]
-    double* sums;                // [3]: sum (image-target)^2, sum dist, sum (1 - <rn,dn>) acc   (zeroed by the caller); null = skip
-    double* partials;            // [loss_det_blocks][3] or null: deterministic sums (written, then reduced in a fixed order)
-    const float* gout;           // device scalar: upstream gradient of the loss (null = 1)
-    float* g_image;              // [V,3,H,W] out (may be null: forward statistics only)
-    float* g_rend_normal; float* g_depth_normal; float* g_dist;
-};
-cudaError_t launch_loss_fused(const LossArgs& a, cudaStream_t stream);
-constexpr int kLossDetBlocks = 1024;
-size_t loss_det_blocks(size_t total);            // blocks (= partial-sum triples) of the deterministic sums
-
-// Decoder epilogue (SURVEY 8f rank 4, lightning/network.py:261-278, 425-429): MLP output rows -> the five
-// contiguous parameter tensors, and the mirror-image backward.
-struct DecoderArgs {
-    size_t total;                // B * N * K Gaussians
-    int N, K, C, sh_dim;         // voxels per scene, Gaussians per voxel, floats per row (10 + sh_dim), SH floats
-    float opacity_shift, scaling_shift, half_cell;
-    const float* params;         // [B,N,K*C] MLP output (fp32)
-    const float* group_centers;  // [N,3]
-    float* centers; float* shs; float* opacity; float* scaling; float* rotation;     // forward outputs
-    const float* g_centers; const float* g_shs; const float* g_opacity; const float* g_scaling; const float* g_rotation;
-    float* g_params;             // [B,N,K*C] backward output
-};
-cudaError_t launch_decoder_layout(const DecoderArgs& a, bool backward, cudaStream_t stream);
-
-// Fine-pass point-feature sampler (lightning/network.py:390-411, projection :182-187): n points sampled in V source
-// views from the 8-channel stack img_ref | image | acc | depth; all images planar fp32.
-struct PointFeatsArgs {
-    int V, n, H, W;
-    const float* points;         // [n,3]
-    const float* w2cs;           // [V,4,4] row-major
-    const float* ixts;           // [V,3,3] row-major
-    const float* img_ref;        // [V,3,H,W]
-    const float* image;          // [V,3,H,W]
-    const float* acc;            // [V,H,W]
-    const float* depth;          // [V,H,W]
-    float* feats;                // [V,8,n] forward output
-    const float* g_feats;        // [V,8,n] backward input
-    float* g_points;             // [n,3] written (may be null)
-    float* g_image; float* g_acc; float* g_depth;   // accumulated into, cleared by the caller (each may be null)
-    // deterministic backward (null = default): int64 planes [5V,H,W] in the layout g_image | g_acc | g_depth and a
-    // header det[0] = max |g_feats| (fp32 bits), det[1] = overflow; both zeroed by the caller.  The float outputs are
-    // then written, not accumulated into.
-    long long* g_fixed;
-    uint32_t* det;
-};
-cudaError_t launch_point_feats(const PointFeatsArgs& a, bool backward, cudaStream_t stream);
-
-// Fused MS-SSIM (lightning/loss.py:44-47, pytorch-msssim MS_SSIM): a logical B x C x H x W image read through
-// element strides; column x of the logical image lies in view x / wv at column x % wv.
-struct MsAddr { long long sb, sc, sy, sx, sv; int wv; };
-struct MsSsimArgs {
-    int B, C, H, W;
-    int size_average;            // out[0] = mean over (b, c); else out[b] = mean over c
-    float data_range;
-    const float* x; const float* y; MsAddr ax, ay;
-    void* workspace;             // ms_ssim_workspace_bytes: pyramid, its gradient, partial sums, coefficients
-    float* out;                  // forward output
-    const float* gout;           // backward: upstream gradient of out (device)
-    float* gx; MsAddr ag;        // backward output, dL/dX
-};
-size_t ms_ssim_workspace_bytes(int B, int C, int H, int W);
-// host only: the workspace's regions and level geometry (srf_ms_ssim_workspace_layout in the C ABI)
-void ms_ssim_workspace_layout(int B, int C, int H, int W, size_t regions[7], size_t levels[15], int dims[30]);
-cudaError_t launch_ms_ssim(const MsSsimArgs& a, bool backward, cudaStream_t stream);
 
 // Optional per-kernel CUDA-event timing (srf_profile_begin/end in the C ABI); no-ops unless enabled.
 enum KernelId { K_PREPROCESS_FWD = 0, K_TILE_SCAN, K_SCATTER, K_SORT_SMALL, K_SORT_BIG, K_RENDER_FWD,

@@ -17,13 +17,12 @@ from typing import Tuple
 import torch
 
 from . import _lib
-from .rasterizer import _contig, _DeviceGuard, _ptr, _raw_stream
+from ._lib import _contig, _ptr
 
 
 class _DecoderLayout(torch.autograd.Function):
     @staticmethod
     def forward(ctx, params, group_centers, K, sh_dim, opacity_shift, scaling_shift, half_cell):
-        lib = _lib.load()
         if params.ndim != 3:
             raise RuntimeError("gaussians_from_decoder: parameters must be [B, N, K*C]")
         B, N, KC = params.shape
@@ -44,29 +43,23 @@ class _DecoderLayout(torch.autograd.Function):
             return torch.empty(shape, dtype=torch.float32, device=dev)
         centers, shs, opacity = new(B, G, 3), new(B, G, sh_dim // 3, 3), new(B, G, 1)
         scaling, rotation = new(B, G, 2), new(B, G, 4)
-        with _DeviceGuard(dev):
-            _lib.check(lib.srf_decoder_layout_forward(
-                _raw_stream(dev), B, N, int(K), int(sh_dim), float(opacity_shift), float(scaling_shift), float(half_cell),
-                params_c.data_ptr(), gc.data_ptr(), centers.data_ptr(), shs.data_ptr(), opacity.data_ptr(),
-                scaling.data_ptr(), rotation.data_ptr()), lib)
+        _lib.launch("srf_decoder_layout_forward", dev, B, N, int(K), int(sh_dim), float(opacity_shift),
+                    float(scaling_shift), float(half_cell), params_c.data_ptr(), gc.data_ptr(), centers.data_ptr(),
+                    shs.data_ptr(), opacity.data_ptr(), scaling.data_ptr(), rotation.data_ptr())
         ctx.save_for_backward(params_c)
         ctx.meta = (B, N, int(K), int(sh_dim), float(half_cell))
         return centers, shs, scaling, rotation, opacity
 
     @staticmethod
     def backward(ctx, g_centers, g_shs, g_scaling, g_rotation, g_opacity):
-        lib = _lib.load()
         (params,) = ctx.saved_tensors
         B, N, K, sh_dim, half_cell = ctx.meta
-        dev = params.device
-
         g_centers, g_shs, g_scaling, g_rotation, g_opacity = map(
             _contig, (g_centers, g_shs, g_scaling, g_rotation, g_opacity))
         g_params = torch.empty_like(params)
-        with _DeviceGuard(dev):
-            _lib.check(lib.srf_decoder_layout_backward(
-                _raw_stream(dev), B, N, K, sh_dim, half_cell, params.data_ptr(), _ptr(g_centers), _ptr(g_shs),
-                _ptr(g_opacity), _ptr(g_scaling), _ptr(g_rotation), g_params.data_ptr()), lib)
+        _lib.launch("srf_decoder_layout_backward", params.device, B, N, K, sh_dim, half_cell, params.data_ptr(),
+                    _ptr(g_centers), _ptr(g_shs), _ptr(g_opacity), _ptr(g_scaling), _ptr(g_rotation),
+                    g_params.data_ptr())
         return g_params, None, None, None, None, None, None
 
 

@@ -22,7 +22,7 @@ from typing import Dict, Optional
 import torch
 
 from . import _lib
-from .rasterizer import _contig, _DeviceGuard, _ptr, _raw_stream
+from ._lib import _contig, _ptr
 
 
 def epilogue_views_forward_raw(color, allmap, rays, cams, depth_ratio, image, depth, acc, rn, dn, dist):
@@ -30,29 +30,22 @@ def epilogue_views_forward_raw(color, allmap, rays, cams, depth_ratio, image, de
     allmap [V,8,H,W], rays [V,H,W,6] or None, cams [V,24] camera records (rasterizer.pack_cameras); outputs stacked
     [V,...] planar.  All tensors contiguous fp32 on one device.  Only the view matrix of each record is read, so for
     V = 1 a contiguous 16-float view matrix serves as `cams`."""
-    lib = _lib.load()
     V, H, W = int(color.shape[0]), int(color.shape[2]), int(color.shape[3])
-    dev = color.device
-    with _DeviceGuard(dev):
-        _lib.check(lib.srf_views_epilogue_forward(
-            _raw_stream(dev), V, H, W, float(depth_ratio), color.data_ptr(), allmap.data_ptr(), _ptr(rays),
-            cams.data_ptr(), image.data_ptr(), depth.data_ptr(), acc.data_ptr(), rn.data_ptr(),
-            dn.data_ptr(), dist.data_ptr()), lib)
+    _lib.launch("srf_views_epilogue_forward", color.device, V, H, W, float(depth_ratio), color.data_ptr(),
+                allmap.data_ptr(), _ptr(rays), cams.data_ptr(), image.data_ptr(), depth.data_ptr(), acc.data_ptr(),
+                rn.data_ptr(), dn.data_ptr(), dist.data_ptr())
 
 
 def epilogue_views_backward_raw(color, allmap, rays, cams, depth_ratio, gi, gd, ga, grn, gdn, gds):
     """Fused backward over V stacked views; returns (dL_dcolor [V,3,H,W], dL_dallmap [V,8,H,W])."""
-    lib = _lib.load()
     V, H, W = int(color.shape[0]), int(color.shape[2]), int(color.shape[3])
     dev = color.device
     scratch = torch.empty((V, 3, H, W), dtype=torch.float32, device=dev)
     d_color = torch.empty((V, 3, H, W), dtype=torch.float32, device=dev)
     d_allmap = torch.empty((V, 8, H, W), dtype=torch.float32, device=dev)
-    with _DeviceGuard(dev):
-        _lib.check(lib.srf_views_epilogue_backward(
-            _raw_stream(dev), V, H, W, float(depth_ratio), color.data_ptr(), allmap.data_ptr(), _ptr(rays),
-            cams.data_ptr(), _ptr(gi), _ptr(gd), _ptr(ga), _ptr(grn), _ptr(gdn), _ptr(gds),
-            scratch.data_ptr(), d_color.data_ptr(), d_allmap.data_ptr()), lib)
+    _lib.launch("srf_views_epilogue_backward", dev, V, H, W, float(depth_ratio), color.data_ptr(), allmap.data_ptr(),
+                _ptr(rays), cams.data_ptr(), _ptr(gi), _ptr(gd), _ptr(ga), _ptr(grn), _ptr(gdn), _ptr(gds),
+                scratch.data_ptr(), d_color.data_ptr(), d_allmap.data_ptr())
     return d_color, d_allmap
 
 

@@ -22,7 +22,6 @@ import torch
 from torch import nn
 
 from . import _lib
-from .rasterizer import _DeviceGuard, _raw_stream
 
 HEADS, COND, HIDDEN = 8, 8, 64
 SH_DIMS = (3, 12, 27, 48)
@@ -54,13 +53,10 @@ class _FineHead(torch.autograd.Function):
         V, _, n = (int(s) for s in pf.shape)
         D, S = int(vf.shape[1]), int(params[8].shape[0])
         N = int(vf.shape[0])
-        lib = _lib.load()
         out = torch.empty((n, S), dtype=torch.float32, device=vf.device)
-        with _DeviceGuard(vf.device):
-            _lib.check(lib.srf_fine_head_forward(
-                _raw_stream(vf.device), n, V, D, S, K, N, vf.data_ptr(), idx.data_ptr() if idx is not None else None,
-                pf.data_ptr(), shs.data_ptr() if shs is not None else None, *[p.data_ptr() for p in params],
-                out.data_ptr()), lib)
+        _lib.launch("srf_fine_head_forward", vf.device, n, V, D, S, K, N, vf.data_ptr(),
+                    idx.data_ptr() if idx is not None else None, pf.data_ptr(),
+                    shs.data_ptr() if shs is not None else None, *[p.data_ptr() for p in params], out.data_ptr())
         ctx.save_for_backward(vf, pf, idx, *params)
         ctx.dims = (n, V, D, S, K, N, shs is not None, None if shs is None else shs.shape)
         return out
@@ -70,19 +66,18 @@ class _FineHead(torch.autograd.Function):
     def backward(ctx, g):
         vf, pf, idx, *params = ctx.saved_tensors
         n, V, D, S, K, N, has_shs, shs_shape = ctx.dims
-        lib = _lib.load()
         dev = vf.device
         g = g.contiguous()
         g_vf, g_pf = torch.empty_like(vf), torch.empty_like(pf)
         g_shs = torch.empty(shs_shape, dtype=torch.float32, device=dev) if has_shs else None
         g_params = [torch.empty_like(p) for p in params]
         gather = idx is not None
-        with _DeviceGuard(dev):
-            ws = torch.empty(_lib.fine_head_workspace_bytes(lib, n, V, D, S, gather), dtype=torch.uint8, device=dev)
-            _lib.check(lib.srf_fine_head_backward(
-                _raw_stream(dev), n, V, D, S, K, N, vf.data_ptr(), idx.data_ptr() if gather else None, pf.data_ptr(),
-                *[p.data_ptr() for p in params], g.data_ptr(), ws.data_ptr(), g_vf.data_ptr(), g_pf.data_ptr(),
-                g_shs.data_ptr() if has_shs else None, *[p.data_ptr() for p in g_params]), lib)
+        with _lib._DeviceGuard(dev):        # the workspace size depends on the device's SM count
+            ws = torch.empty(_lib.fine_head_workspace_bytes(_lib.load(), n, V, D, S, gather), dtype=torch.uint8,
+                             device=dev)
+        _lib.launch("srf_fine_head_backward", dev, n, V, D, S, K, N, vf.data_ptr(), idx.data_ptr() if gather else None,
+                    pf.data_ptr(), *[p.data_ptr() for p in params], g.data_ptr(), ws.data_ptr(), g_vf.data_ptr(),
+                    g_pf.data_ptr(), g_shs.data_ptr() if has_shs else None, *[p.data_ptr() for p in g_params])
         return (g_vf, g_pf, g_shs, None, None, *g_params)
 
 

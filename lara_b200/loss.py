@@ -18,7 +18,7 @@ from typing import Callable, Dict, Optional, Tuple
 import torch
 
 from . import _lib
-from .rasterizer import _DeviceGuard, _ptr, _raw_stream
+from ._lib import _ptr
 from .ssim import ms_ssim_views
 
 
@@ -31,7 +31,6 @@ def _planar(t: torch.Tensor) -> torch.Tensor:
 class _SceneLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, image, rend_normal, depth_normal, rend_dist, acc_map, target, with_reg, batch_scenes):
-        lib = _lib.load()
         dev = image.device
         V, _, H, W = image.shape
         for name, t in (("image", image), ("target", target), ("rend_normal", rend_normal), ("depth_normal", depth_normal),
@@ -43,13 +42,11 @@ class _SceneLoss(torch.autograd.Function):
         if tuple(target.shape) != (V, H, W, 3):
             raise RuntimeError(f"scene_loss: tar_rgb must be [V,H,W,3] = {(V, H, W, 3)}, got {tuple(target.shape)}")
         sums = torch.empty(3, dtype=torch.float64, device=dev)
-        with _DeviceGuard(dev):
-            # partial sums reduced in a fixed order instead of atomics
-            ws = (torch.empty(_lib.det_loss_workspace_bytes(lib, V, H, W) // 8, dtype=torch.float64, device=dev)
-                  if _lib.deterministic() else None)
-            _lib.check(lib.srf_loss_forward(
-                _raw_stream(dev), V, H, W, 1 if with_reg else 0, image.data_ptr(), target.data_ptr(), _ptr(rend_normal),
-                _ptr(depth_normal), _ptr(acc_map), _ptr(rend_dist), sums.data_ptr(), _ptr(ws)), lib)
+        # partial sums reduced in a fixed order instead of atomics
+        ws = (torch.empty(_lib.det_loss_workspace_bytes(_lib.load(), V, H, W) // 8, dtype=torch.float64, device=dev)
+              if _lib.deterministic() else None)
+        _lib.launch("srf_loss_forward", dev, V, H, W, 1 if with_reg else 0, image.data_ptr(), target.data_ptr(),
+                    _ptr(rend_normal), _ptr(depth_normal), _ptr(acc_map), _ptr(rend_dist), sums.data_ptr(), _ptr(ws))
         npx = float(batch_scenes) * V * H * W
         mse = sums[0] / (3.0 * npx)
         dist = sums[1] / npx
@@ -62,7 +59,6 @@ class _SceneLoss(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_loss, _g_mse, _g_dist, _g_nerr):
-        lib = _lib.load()
         image, target, rn, dn, acc = ctx.saved_tensors
         dev = image.device
         V, _, H, W = image.shape
@@ -73,12 +69,11 @@ class _SceneLoss(torch.autograd.Function):
             g_dist = torch.empty((V, H, W), dtype=torch.float32, device=dev)
         else:
             g_rn = g_dn = g_dist = None
-        with _DeviceGuard(dev):
-            _lib.check(lib.srf_loss_backward(
-                _raw_stream(dev), V, H, W, 1 if ctx.with_reg else 0, 1.0 / (3.0 * ctx.npx), 1000.0 / ctx.npx, 0.2 / ctx.npx,
-                image.data_ptr(), target.data_ptr(), _ptr(rn if ctx.with_reg else None),
-                _ptr(dn if ctx.with_reg else None), _ptr(acc if ctx.with_reg else None), up.data_ptr(),
-                g_image.data_ptr(), _ptr(g_rn), _ptr(g_dn), _ptr(g_dist)), lib)
+        _lib.launch("srf_loss_backward", dev, V, H, W, 1 if ctx.with_reg else 0, 1.0 / (3.0 * ctx.npx),
+                    1000.0 / ctx.npx, 0.2 / ctx.npx, image.data_ptr(), target.data_ptr(),
+                    _ptr(rn if ctx.with_reg else None), _ptr(dn if ctx.with_reg else None),
+                    _ptr(acc if ctx.with_reg else None), up.data_ptr(), g_image.data_ptr(), _ptr(g_rn), _ptr(g_dn),
+                    _ptr(g_dist))
         return g_image, g_rn, g_dn, g_dist, None, None, None, None
 
 

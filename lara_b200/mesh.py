@@ -23,7 +23,6 @@ import numpy as np
 import torch
 
 from . import _lib
-from .rasterizer import _DeviceGuard, _raw_stream
 
 CAM_FX, CAM_FY, CAM_CX, CAM_CY, CAM_DEPTH_TRUNC = 16, 17, 18, 19, 20      # include/surfel_mesh.h SRF_MESH_CAM_*
 
@@ -156,13 +155,9 @@ def integrate(volume: TSDFVolume, depth: torch.Tensor, acc: torch.Tensor, image:
     V, H, W = _check_views(depth, acc, image, cams)
     if volume.empty or V == 0:
         return
-    lib = _lib.load()
-    with _DeviceGuard(depth.device):
-        _lib.check(lib.srf_tsdf_integrate(_raw_stream(depth.device), _lib.int3(volume.n0), _lib.int3(volume.dims),
-                                          volume.voxel_size, volume.sdf_trunc, volume.tsdf.data_ptr(),
-                                          volume.weight.data_ptr(), volume.color.data_ptr(), V, H, W,
-                                          depth.data_ptr(), acc.data_ptr(), image.data_ptr(), cams.data_ptr(),
-                                          float(alpha_thres)), lib)
+    _lib.launch("srf_tsdf_integrate", depth.device, _lib.int3(volume.n0), _lib.int3(volume.dims), volume.voxel_size,
+                volume.sdf_trunc, volume.tsdf.data_ptr(), volume.weight.data_ptr(), volume.color.data_ptr(), V, H, W,
+                depth.data_ptr(), acc.data_ptr(), image.data_ptr(), cams.data_ptr(), float(alpha_thres))
 
 
 def extract_triangle_mesh(volume: TSDFVolume):
@@ -172,21 +167,18 @@ def extract_triangle_mesh(volume: TSDFVolume):
     if volume.empty:
         return (torch.empty((0, 3), dtype=torch.float32, device=dev), torch.empty((0, 3), dtype=torch.int32, device=dev),
                 torch.empty((0, 3), dtype=torch.float32, device=dev))
-    lib = _lib.load()
     dims = _lib.int3(volume.dims)
-    ws = torch.empty(_lib.mesh_workspace_bytes(lib, volume.dims), dtype=torch.uint8, device=dev)
+    ws = torch.empty(_lib.mesh_workspace_bytes(_lib.load(), volume.dims), dtype=torch.uint8, device=dev)
     totals = torch.empty(2, dtype=torch.int32, device=dev)
-    with _DeviceGuard(dev):
-        stream = _raw_stream(dev)
-        _lib.check(lib.srf_mesh_count(stream, dims, volume.tsdf.data_ptr(), volume.weight.data_ptr(), ws.data_ptr(),
-                                      totals.data_ptr()), lib)
-        Nv, Nt = (int(x) for x in totals.cpu())
-        vertices = torch.empty((Nv, 3), dtype=torch.float32, device=dev)
-        colors = torch.empty((Nv, 3), dtype=torch.float32, device=dev)
-        triangles = torch.empty((Nt, 3), dtype=torch.int32, device=dev)
-        _lib.check(lib.srf_mesh_emit(stream, _lib.int3(volume.n0), dims, volume.voxel_size, volume.tsdf.data_ptr(),
-                                     volume.color.data_ptr(), ws.data_ptr(), Nv, Nt, vertices.data_ptr(),
-                                     colors.data_ptr(), triangles.data_ptr()), lib)
+    _lib.launch("srf_mesh_count", dev, dims, volume.tsdf.data_ptr(), volume.weight.data_ptr(), ws.data_ptr(),
+                totals.data_ptr())
+    Nv, Nt = (int(x) for x in totals.cpu())
+    vertices = torch.empty((Nv, 3), dtype=torch.float32, device=dev)
+    colors = torch.empty((Nv, 3), dtype=torch.float32, device=dev)
+    triangles = torch.empty((Nt, 3), dtype=torch.int32, device=dev)
+    _lib.launch("srf_mesh_emit", dev, _lib.int3(volume.n0), dims, volume.voxel_size, volume.tsdf.data_ptr(),
+                volume.color.data_ptr(), ws.data_ptr(), Nv, Nt, vertices.data_ptr(), colors.data_ptr(),
+                triangles.data_ptr())
     return vertices, triangles, colors
 
 

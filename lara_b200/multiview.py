@@ -23,6 +23,7 @@ from typing import Dict, Optional, Sequence
 
 import torch
 
+from . import _lib
 from . import rasterizer as R
 from .epilogue import epilogue_views_backward_raw, epilogue_views_forward_raw
 
@@ -100,7 +101,7 @@ class _RenderSceneViews(torch.autograd.Function):
         H, W, tfx, tfy, deg, debug = ctx.geometry
 
         if ctx.has_rays:
-            c = R._contig
+            c = _lib._contig
             d_color, d_allmap = epilogue_views_backward_raw(
                 color, allmap, rays, cams, ctx.depth_ratio, c(g_image), c(g_depth), c(g_acc), c(g_rn), c(g_dn), c(g_dist))
         else:

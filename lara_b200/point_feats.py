@@ -27,7 +27,7 @@ from typing import Dict
 import torch
 
 from . import _lib
-from .rasterizer import _DeviceGuard, _ptr, _raw_stream
+from ._lib import _ptr
 
 
 _NAMES = ("points", "img_ref", "renderings['image']", "renderings['acc_map']", "renderings['depth']", "src_w2cs",
@@ -72,14 +72,11 @@ class _PointFeats(torch.autograd.Function):
     def forward(ctx, points, img_ref, image, acc, depth, w2cs, ixts):
         _check_tensors((points, img_ref, image, acc, depth, w2cs, ixts))
         V, _, H, W = (int(s) for s in img_ref.shape)
-        lib = _lib.load()
         ins = [t.contiguous() for t in (points, w2cs, ixts, img_ref, image, acc, depth)]
         n = int(points.shape[0])
-        dev = points.device
-        feats = torch.empty((V, 8, n), dtype=torch.float32, device=dev)
-        with _DeviceGuard(dev):
-            _lib.check(lib.srf_point_feats_forward(_raw_stream(dev), V, n, H, W, *[t.data_ptr() for t in ins],
-                                                   feats.data_ptr()), lib)
+        feats = torch.empty((V, 8, n), dtype=torch.float32, device=points.device)
+        _lib.launch("srf_point_feats_forward", points.device, V, n, H, W, *[t.data_ptr() for t in ins],
+                    feats.data_ptr())
         ctx.save_for_backward(*ins)
         ctx.dims = (V, n, H, W)
         return feats
@@ -87,7 +84,6 @@ class _PointFeats(torch.autograd.Function):
     @staticmethod
     @torch.amp.custom_bwd(device_type="cuda")
     def backward(ctx, g_feats):
-        lib = _lib.load()
         ins = ctx.saved_tensors
         V, n, H, W = ctx.dims
         dev = g_feats.device
@@ -98,13 +94,11 @@ class _PointFeats(torch.autograd.Function):
         g_points, g_image, g_acc, g_depth = new(need[0], n, 3), new(need[2], V, 3, H, W), new(need[3], V, H, W), \
             new(need[4], V, 1, H, W)
         g_feats = g_feats.contiguous()
-        with _DeviceGuard(dev):
-            # fixed-point sums in a workspace instead of atomics
-            ws = (torch.empty(_lib.det_point_feats_workspace_bytes(lib, V, H, W), dtype=torch.uint8, device=dev)
-                  if _lib.deterministic() else None)
-            _lib.check(lib.srf_point_feats_backward(_raw_stream(dev), V, n, H, W, *[t.data_ptr() for t in ins],
-                                                    g_feats.data_ptr(), _ptr(g_points), _ptr(g_image), _ptr(g_acc),
-                                                    _ptr(g_depth), _ptr(ws)), lib)
+        # fixed-point sums in a workspace instead of atomics
+        ws = (torch.empty(_lib.det_point_feats_workspace_bytes(_lib.load(), V, H, W), dtype=torch.uint8, device=dev)
+              if _lib.deterministic() else None)
+        _lib.launch("srf_point_feats_backward", dev, V, n, H, W, *[t.data_ptr() for t in ins], g_feats.data_ptr(),
+                    _ptr(g_points), _ptr(g_image), _ptr(g_acc), _ptr(g_depth), _ptr(ws))
         return g_points, None, g_image, g_acc, g_depth, None, None
 
 

@@ -26,6 +26,8 @@ import torch
 import torch.nn as nn
 
 from . import _lib
+from ._lib import _DeviceGuard, _dev_index, _ptr
+from ._lib import _raw_stream  # noqa: F401  (still importable from here: callers of the raw entries use it)
 
 
 class GaussianRasterizationSettings(NamedTuple):
@@ -51,14 +53,6 @@ _size_cache: dict = {}            # (V, P, H, W, capacity, for_backward) -> work
 _cam_pads: dict = {}              # device -> zero padding of a camera record
 _capacity_hwm: dict = {}          # device index -> largest num_rendered seen (instances per view)
 _lock = threading.Lock()          # autograd calls backward() from another host thread
-
-
-def _ptr(t: Optional[torch.Tensor]) -> int:
-    return 0 if t is None else t.data_ptr()
-
-
-def _contig(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
-    return None if t is None else t.contiguous()
 
 
 def _opt(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
@@ -90,32 +84,6 @@ def _views_sizes(lib, V: int, P: int, H: int, W: int, capacity: int, for_backwar
 
 def _blob(nbytes: int, device) -> torch.Tensor:
     return torch.empty(nbytes, dtype=torch.uint8, device=device)
-
-
-def _dev_index(device: torch.device) -> int:
-    return device.index if device.index is not None else torch.cuda.current_device()
-
-
-def _raw_stream(device: torch.device) -> int:
-    return torch._C._cuda_getCurrentRawStream(_dev_index(device))
-
-
-class _DeviceGuard:
-    """`with torch.cuda.device(d)` only when d is not already current (the common case)."""
-
-    def __init__(self, device: torch.device):
-        self.idx = device.index
-        self.ctx = None
-
-    def __enter__(self):
-        if self.idx is not None and self.idx != torch.cuda.current_device():
-            self.ctx = torch.cuda.device(self.idx)
-            self.ctx.__enter__()
-
-    def __exit__(self, *exc):
-        if self.ctx is not None:
-            self.ctx.__exit__(*exc)
-        return False
 
 
 def initial_capacity(P: int, device: torch.device) -> int:
@@ -373,28 +341,26 @@ def _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMa
     # the tile scan, never for the blend.
     # the forward-only point list and entries are scratch of this call: they go back to the caching allocator when
     # it returns, stream-ordered behind the kernels that use them
-    _lib.check(lib.srf_views_forward(
-        _raw_stream(device), V, P, int(sh_degree), M, _ptr(means3D), _ptr(shs), _ptr(colors_precomp),
+    _lib.launch(
+        "srf_views_forward", device, V, P, int(sh_degree), M, _ptr(means3D), _ptr(shs), _ptr(colors_precomp),
         _ptr(opacities), _ptr(scales), _ptr(rotations), _ptr(transMat_precomp), cams.data_ptr(),
         float(tanfovx), float(tanfovy), H, W, 1 if prefiltered else 0, capacity,
         radii.data_ptr(), geom.data_ptr(), tile.data_ptr(), _blob(ent_b, device).data_ptr(), point_list.data_ptr(),
         _ptr(image), color.data_ptr(), allmap.data_ptr(), slot.data_ptr(), ev.cuda_event,
-        1 if raw_activations else 0, 1 if for_backward else 0), lib)
+        1 if raw_activations else 0, 1 if for_backward else 0)
     state = ForwardState(geom, tile, image, point_list if for_backward else None, capacity, nviews=V, cams=cams,
                          for_backward=for_backward)
 
     def rerun(new_capacity: int):
         # enqueued on whatever stream is current: a deferred re-run happens on the caller's stream
-        with _DeviceGuard(device):
-            e_b, p_b = _views_sizes(lib, V, P, H, W, new_capacity, for_backward)[3:5]
-            pl2 = _blob(p_b, device)
-            _lib.check(lib.srf_views_forward_render(
-                _raw_stream(device), V, P, H, W, new_capacity, geom.data_ptr(), tile.data_ptr(),
-                _blob(e_b, device).data_ptr(), pl2.data_ptr(), _ptr(image), cams.data_ptr(), color.data_ptr(),
-                allmap.data_ptr(), 1 if for_backward else 0), lib)
-            state.capacity = new_capacity
-            if for_backward:
-                state.point_list = pl2
+        e_b, p_b = _views_sizes(lib, V, P, H, W, new_capacity, for_backward)[3:5]
+        pl2 = _blob(p_b, device)
+        _lib.launch("srf_views_forward_render", device, V, P, H, W, new_capacity, geom.data_ptr(), tile.data_ptr(),
+                    _blob(e_b, device).data_ptr(), pl2.data_ptr(), _ptr(image), cams.data_ptr(), color.data_ptr(),
+                    allmap.data_ptr(), 1 if for_backward else 0)
+        state.capacity = new_capacity
+        if for_backward:
+            state.point_list = pl2
 
     pend = _Pending(device, rb, V, capacity, rerun)
     state._pending, state._counts = pend, None
@@ -472,31 +438,30 @@ def backward_views_raw(state: ForwardState, radii, means3D, shs, colors_precomp,
         raise RuntimeError("backward of a forward-only render: this state comes from a forward with "
                            "for_backward=False, which keeps no contribution record or image state; run the "
                            "forward with for_backward=True to take its gradient")
-    with _DeviceGuard(means3D.device):
-        lib = _lib.load()
-        device = means3D.device
-        V, P = int(cams.shape[0]), int(means3D.shape[0])
-        M = int(shs.shape[1]) if shs is not None else 0
-        g = _grad_outputs(P, M, device, shs, colors_precomp, transMat_precomp, out or {}, accumulate, need_means2D)
-        if P == 0:
-            return g
-        state.resolve()                 # capacity verified (re-run if it overflowed) before the lists are walked again
-        det = _lib.deterministic(deterministic)
-        scratch_b = (_lib.det_backward_scratch_bytes(lib, V, P) if det
-                     else _views_sizes(lib, V, P, H, W, state.capacity)[5])
-        _lib.check(lib.srf_views_backward(
-            _raw_stream(device), V, P, int(sh_degree), M, H, W, state.capacity, cams.data_ptr(),
-            _ptr(means3D), _ptr(shs), 1 if colors_precomp is not None else 0,
-            _ptr(scales), _ptr(rotations), 1 if transMat_precomp is not None else 0,
-            float(tanfovx), float(tanfovy), radii.data_ptr(),
-            state.geom.data_ptr(), state.tile.data_ptr(), state.point_list.data_ptr(), state.image.data_ptr(),
-            grad_color.data_ptr(), grad_allmap.data_ptr(), _blob(scratch_b, device).data_ptr(), 1 if accumulate else 0,
-            _ptr(g["means3D"]), _ptr(g["means2D"]), _ptr(g["sh"]), _ptr(g["colors_precomp"]),
-            _ptr(g["opacities"]), _ptr(g["scales"]), _ptr(g["rotations"]), _ptr(g["cov3Ds_precomp"]),
-            1 if raw_activations else 0, 1 if det else 0), lib)
-        if debug:
-            torch.cuda.synchronize(device)
+    lib = _lib.load()
+    device = means3D.device
+    V, P = int(cams.shape[0]), int(means3D.shape[0])
+    M = int(shs.shape[1]) if shs is not None else 0
+    g = _grad_outputs(P, M, device, shs, colors_precomp, transMat_precomp, out or {}, accumulate, need_means2D)
+    if P == 0:
         return g
+    state.resolve()                 # capacity verified (re-run if it overflowed) before the lists are walked again
+    det = _lib.deterministic(deterministic)
+    scratch_b = (_lib.det_backward_scratch_bytes(lib, V, P) if det
+                 else _views_sizes(lib, V, P, H, W, state.capacity)[5])
+    _lib.launch(
+        "srf_views_backward", device, V, P, int(sh_degree), M, H, W, state.capacity, cams.data_ptr(),
+        _ptr(means3D), _ptr(shs), 1 if colors_precomp is not None else 0,
+        _ptr(scales), _ptr(rotations), 1 if transMat_precomp is not None else 0,
+        float(tanfovx), float(tanfovy), radii.data_ptr(),
+        state.geom.data_ptr(), state.tile.data_ptr(), state.point_list.data_ptr(), state.image.data_ptr(),
+        grad_color.data_ptr(), grad_allmap.data_ptr(), _blob(scratch_b, device).data_ptr(), 1 if accumulate else 0,
+        _ptr(g["means3D"]), _ptr(g["means2D"]), _ptr(g["sh"]), _ptr(g["colors_precomp"]),
+        _ptr(g["opacities"]), _ptr(g["scales"]), _ptr(g["rotations"]), _ptr(g["cov3Ds_precomp"]),
+        1 if raw_activations else 0, 1 if det else 0)
+    if debug:
+        torch.cuda.synchronize(device)
+    return g
 
 
 def _dump_snapshot(path: str, items) -> None:
@@ -692,16 +657,13 @@ class GaussianRasterizer(nn.Module):
     def markVisible(self, positions):
         """Boolean mask of points in front of the near plane (DSR __init__.py:177-186)."""
         with torch.no_grad():
-            lib = _lib.load()
             pos = _f32c(positions, "means3D")
             rs = _check_settings(self.raster_settings, pos.device)
             P = int(pos.shape[0])
             present = torch.zeros((P,), dtype=torch.bool, device=pos.device)
             if P:
-                with _DeviceGuard(pos.device):
-                    _lib.check(lib.srf_mark_visible(
-                        _raw_stream(pos.device), P, pos.data_ptr(),
-                        rs.viewmatrix.data_ptr(), rs.projmatrix.data_ptr(), present.data_ptr()), lib)
+                _lib.launch("srf_mark_visible", pos.device, P, pos.data_ptr(), rs.viewmatrix.data_ptr(),
+                            rs.projmatrix.data_ptr(), present.data_ptr())
         return present
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None,

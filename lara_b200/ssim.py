@@ -20,7 +20,6 @@ import ctypes
 import torch
 
 from . import _lib
-from .rasterizer import _DeviceGuard, _raw_stream
 
 _MIN_SIDE = (11 - 1) * 2 ** 4
 
@@ -58,35 +57,29 @@ def check_inputs(fn: str, X: torch.Tensor, Y: torch.Tensor) -> None:
 class _MsSsim(torch.autograd.Function):
     @staticmethod
     def forward(ctx, X, Y, views, data_range, size_average):
-        lib = _lib.load()
         dev = X.device
         if not X.is_cuda or Y.device != dev:
             raise RuntimeError(f"MS_SSIM: X and Y must be CUDA tensors on one device, got {X.device} and {Y.device}")
         B, C, H, W = _logical_shape(X, views)
-        ws = torch.empty(_lib._size_query(lib.srf_ms_ssim_workspace_bytes, B, C, H, W), dtype=torch.uint8, device=dev)
+        ws = torch.empty(_lib.ms_ssim_workspace_bytes(_lib.load(), B, C, H, W), dtype=torch.uint8, device=dev)
         out = torch.empty(() if size_average else (B,), dtype=torch.float32, device=dev)
         ax, ay = _addr(X, views), _addr(Y, views)
-        with _DeviceGuard(dev):
-            _lib.check(lib.srf_ms_ssim_forward(_raw_stream(dev), B, C, H, W, X.data_ptr(), ctypes.byref(ax),
-                                               Y.data_ptr(), ctypes.byref(ay), float(data_range),
-                                               1 if size_average else 0, ws.data_ptr(), out.data_ptr()), lib)
+        _lib.launch("srf_ms_ssim_forward", dev, B, C, H, W, X.data_ptr(), ctypes.byref(ax), Y.data_ptr(),
+                    ctypes.byref(ay), float(data_range), 1 if size_average else 0, ws.data_ptr(), out.data_ptr())
         ctx.save_for_backward(X, Y, ws)
         ctx.cfg = (views, float(data_range), bool(size_average), (B, C, H, W))
         return out
 
     @staticmethod
     def backward(ctx, g_out):
-        lib = _lib.load()
         X, Y, ws = ctx.saved_tensors
         views, data_range, size_average, (B, C, H, W) = ctx.cfg
-        dev = X.device
         up = g_out.to(torch.float32).reshape(-1).contiguous()
         gX = torch.empty_like(X)
         ax, ay, ag = _addr(X, views), _addr(Y, views), _addr(gX, views)
-        with _DeviceGuard(dev):
-            _lib.check(lib.srf_ms_ssim_backward(_raw_stream(dev), B, C, H, W, X.data_ptr(), ctypes.byref(ax),
-                                                Y.data_ptr(), ctypes.byref(ay), data_range, 1 if size_average else 0,
-                                                ws.data_ptr(), up.data_ptr(), gX.data_ptr(), ctypes.byref(ag)), lib)
+        _lib.launch("srf_ms_ssim_backward", X.device, B, C, H, W, X.data_ptr(), ctypes.byref(ax), Y.data_ptr(),
+                    ctypes.byref(ay), data_range, 1 if size_average else 0, ws.data_ptr(), up.data_ptr(),
+                    gX.data_ptr(), ctypes.byref(ag))
         return gX, None, None, None, None
 
 

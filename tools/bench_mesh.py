@@ -33,7 +33,6 @@ def run_point(P: int, rounds: int) -> dict:
     from lara_b200 import _lib, mesh as MS, scene as S
     from lara_b200.renderer import Renderer
     dev = torch.device("cuda:0")
-    lib = _lib.load()
     sc = S.scene(P, 0)
     cams = S.mesh_path(16, 512, 512, 0.75)
     for c in cams:
@@ -64,12 +63,11 @@ def run_point(P: int, rounds: int) -> dict:
         MS.integrate(vol, depth, acc, image, rec, 0.08)
         e[3].record()
         dims = _lib.int3(vol.dims)
-        ws = torch.empty(_lib.mesh_workspace_bytes(lib, vol.dims), dtype=torch.uint8, device=dev)
+        ws = torch.empty(_lib.mesh_workspace_bytes(_lib.load(), vol.dims), dtype=torch.uint8, device=dev)
         totals = torch.empty(2, dtype=torch.int32, device=dev)
         e[4].record()
-        stream = torch.cuda.current_stream().cuda_stream
-        _lib.check(lib.srf_mesh_count(stream, dims, vol.tsdf.data_ptr(), vol.weight.data_ptr(), ws.data_ptr(),
-                                      totals.data_ptr()), lib)
+        _lib.launch("srf_mesh_count", dev, dims, vol.tsdf.data_ptr(), vol.weight.data_ptr(), ws.data_ptr(),
+                    totals.data_ptr())
         e[5].record()
         e[5].synchronize()
         h0 = time.perf_counter()
@@ -80,9 +78,8 @@ def run_point(P: int, rounds: int) -> dict:
         tris = torch.empty((Nt, 3), dtype=torch.int32, device=dev)
         f = [ev(), ev()]
         f[0].record()
-        _lib.check(lib.srf_mesh_emit(stream, _lib.int3(vol.n0), dims, vol.voxel_size, vol.tsdf.data_ptr(),
-                                     vol.color.data_ptr(), ws.data_ptr(), Nv, Nt, verts.data_ptr(), cols.data_ptr(),
-                                     tris.data_ptr()), lib)
+        _lib.launch("srf_mesh_emit", dev, _lib.int3(vol.n0), dims, vol.voxel_size, vol.tsdf.data_ptr(),
+                    vol.color.data_ptr(), ws.data_ptr(), Nv, Nt, verts.data_ptr(), cols.data_ptr(), tris.data_ptr())
         f[1].record()
         torch.cuda.synchronize()
         peak = torch.cuda.max_memory_allocated() - base
