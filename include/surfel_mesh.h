@@ -57,6 +57,26 @@ int srf_mesh_emit(void* stream, const int* n0, const int* dims, float voxel_size
                   const float* color, const void* workspace, int Nv, int Nt,
                   float* vertices, float* colors, int32_t* triangles);
 
+/* LaRa's mesh postprocess (tools/meshExtractor.py:116-134) on the device, for vertices [Nv,3], colors [Nv,3] and
+ * triangles [Nt,3] (int32).  With aabb (host double[6]: lo xyz, hi xyz; NULL = no crop) a triangle with a vertex outside
+ * the inclusive box is dropped (each float coordinate compared as a double, a NaN is outside).  Two surviving triangles
+ * are adjacent if they share an undirected vertex pair among their edges (a, b), (b, c), (c, a); the clusters are the
+ * connected components.  With C clusters, every triangle whose cluster holds at least the min(C, keep)-th largest count
+ * is kept (ties keep more), and a vertex is kept if a kept triangle references it.  Kept vertices, colours and triangles
+ * stay in input order, the triangles' indices remapped.
+ * srf_mesh_filter_count writes to totals (device int32[4]) the kept vertex count, the kept triangle count, the cluster
+ * count after the crop and the number of triangles with an index outside [0, Nv), and keeps in the workspace (256-byte
+ * aligned, srf_mesh_filter_workspace_bytes) what srf_mesh_filter_emit reads.  If the last count is not 0 the mesh is
+ * invalid: such triangles are treated as cropped, and the caller should not emit.  srf_mesh_filter_emit then writes
+ * out_vertices, out_colors [Nv_out,3] and out_triangles [Nt_out,3]; pass both the same inputs and workspace, and the
+ * first two totals as Nv_out, Nt_out.  Integer atomics only: the output is bit-reproducible. */
+int srf_mesh_filter_workspace_bytes(int Nv, int Nt, size_t* bytes);
+int srf_mesh_filter_count(void* stream, int Nv, int Nt, const float* vertices, const int32_t* triangles,
+                          const double* aabb, int keep, void* workspace, int32_t* totals);
+int srf_mesh_filter_emit(void* stream, int Nv, int Nt, const float* vertices, const float* colors,
+                         const int32_t* triangles, const void* workspace, int Nv_out, int Nt_out,
+                         float* out_vertices, float* out_colors, int32_t* out_triangles);
+
 #ifdef __cplusplus
 }
 #endif

@@ -11,7 +11,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int64, c_size_t, c_void_p
+from ctypes import POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int64, c_size_t, c_void_p
 from typing import Optional
 
 import torch
@@ -93,6 +93,9 @@ SIGNATURES = {
     "srf_mesh_workspace_bytes": (c_int, [_I3, POINTER(c_size_t)]),
     "srf_mesh_count": (c_int, [_P, _I3, _P, _P, _P, _P]),
     "srf_mesh_emit": (c_int, [_P, _I3, _I3, c_float, _P, _P, _P, c_int, c_int, _P, _P, _P]),
+    "srf_mesh_filter_workspace_bytes": (c_int, [c_int, c_int, POINTER(c_size_t)]),
+    "srf_mesh_filter_count": (c_int, [_P, c_int, c_int, _P, _P, POINTER(c_double), c_int, _P, _P]),
+    "srf_mesh_filter_emit": (c_int, [_P, c_int, c_int, _P, _P, _P, _P, c_int, c_int, _P, _P, _P]),
     # include/surfel_fine_head.h
     "srf_fine_head_forward": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int,   # stream, n, V, D, sh_dim, K, N
                                       _P, _P, _P, _P,                               # volume_feat, idx, point_feats, shs
@@ -249,6 +252,11 @@ def int3(v) -> ctypes.Array:
 
 def mesh_workspace_bytes(lib, dims) -> int:
     return _size_query(lib.srf_mesh_workspace_bytes, int3(dims))
+
+
+def mesh_filter_workspace_bytes(lib, Nv: int, Nt: int) -> int:
+    """Workspace of srf_mesh_filter_count / _emit for a mesh of Nv vertices and Nt triangles."""
+    return _size_query(lib.srf_mesh_filter_workspace_bytes, Nv, Nt)
 
 
 def layout(lib, P: int, H: int, W: int):

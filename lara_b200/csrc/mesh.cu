@@ -17,6 +17,12 @@
 // Marching cubes: count (classify + idempotent edge marks, then two exclusive scans over edges and cubes, totals to
 // device memory) and emit (one thread per voxel writes the vertices of its three edges and the triangles of its
 // cube).  Integer scans and stores only; every output lands at an index the scans fixed.
+//
+// Cluster filter (LaRa's postprocess): crop flags, an open-addressing hash table of the live triangles' undirected edges
+// whose slots keep the smallest triangle on the edge, a union-find over "shares an edge" (larger root hooked under the
+// smaller), component sizes, an exact radix select of the min(C, keep)-th largest size, then keep / used flags, the two
+// scans and emit.  Integer atomics only, and every step's result is independent of scheduling: each component's
+// root is its smallest triangle.
 #include "../../include/surfel_mesh.h"
 #include "mc_table.cuh"
 #include "surfel_kernels.h"
@@ -245,10 +251,11 @@ __global__ void __launch_bounds__(kScanThreads) scan_apply_kernel(uint32_t* data
     }
 }
 
+// n = 0 (nb = 0) only writes the total 0
 cudaError_t exclusive_scan(uint32_t* data, size_t n, uint32_t* sums, size_t nb, int32_t* total, cudaStream_t stream) {
-    scan_tile_sums_kernel<<<(unsigned)nb, kScanThreads, 0, stream>>>(data, n, sums);
+    if (nb) scan_tile_sums_kernel<<<(unsigned)nb, kScanThreads, 0, stream>>>(data, n, sums);
     scan_sums_kernel<<<1, kScanThreads, 0, stream>>>(sums, nb, data + n, total);
-    scan_apply_kernel<<<(unsigned)nb, kScanThreads, 0, stream>>>(data, n, sums);
+    if (nb) scan_apply_kernel<<<(unsigned)nb, kScanThreads, 0, stream>>>(data, n, sums);
     return cudaGetLastError();
 }
 
@@ -293,6 +300,235 @@ __global__ void __launch_bounds__(kMeshThreads) mesh_emit_kernel(EmitArgs a) {
         int c, axis;
         edge_start(kMcTris[cs][t], c, axis);
         out[t] = (int32_t)a.edge[3 * corner_index(a.g, idx, c) + axis];
+    }
+}
+
+// ---- cluster filter ----
+
+constexpr unsigned long long kEmptyKey = ~0ull;    // no edge key: indices are < 2^31
+constexpr uint32_t kDead = ~0u;                    // label of a cropped (or invalid) triangle
+constexpr int kSelectPasses = 4;                   // 8-bit digits of a u32 cluster size
+
+struct FilterWorkspace {
+    size_t keys, owner, parent, size, label, used, hist, sel, sums, total;
+    size_t slots, nb_tri, nb_vert;
+};
+
+FilterWorkspace filter_layout(size_t Nv, size_t Nt) {
+    FilterWorkspace l;
+    l.slots = 1;
+    while (l.slots < 6 * Nt) l.slots <<= 1;                // load factor <= 1/2 over the 3 Nt edges
+    l.nb_tri = (Nt + kScanTile - 1) / kScanTile;
+    l.nb_vert = (Nv + kScanTile - 1) / kScanTile;
+    l.keys = 0;                                             // u64 [slots]: edge keys min << 32 | max, ~0 = empty
+    l.owner = align_up(l.keys + 8 * l.slots);               // u32 [slots]: smallest live triangle on the edge
+    l.parent = align_up(l.owner + 4 * l.slots);             // i32 [Nt]: union-find forest, -1 = dropped by the crop
+    l.size = align_up(l.parent + 4 * Nt);                   // u32 [Nt]: triangle count of each root
+    l.label = align_up(l.size + 4 * Nt);                    // u32 [Nt + 1]: root, then keep flags, then offsets
+    l.used = align_up(l.label + 4 * (Nt + 1));              // u32 [Nv + 1]: used flags, then offsets
+    l.hist = align_up(l.used + 4 * (Nv + 1));               // u32 [4][256]: radix-select histograms
+    l.sel = align_up(l.hist + 4 * 256 * kSelectPasses);     // u32 [2]: size prefix found so far, rank left in it
+    l.sums = align_up(l.sel + 8);                           // u32 [nb_tri + nb_vert]: per-tile sums of the scans
+    l.total = align_up(l.sums + 4 * (l.nb_tri + l.nb_vert));
+    return l;
+}
+
+struct FilterArgs {
+    int Nv, Nt, keep, crop;
+    double lo[3], hi[3];
+    size_t mask;                                            // slots - 1
+    const float* vertices; const int32_t* triangles;
+    unsigned long long* keys; uint32_t* owner; int32_t* parent; uint32_t* size; uint32_t* label; uint32_t* used;
+    uint32_t* hist; uint32_t* sel; int32_t* totals;
+};
+
+__device__ __forceinline__ unsigned long long edge_key(int32_t x, int32_t y) {
+    return x < y ? ((unsigned long long)x << 32) | (uint32_t)y : ((unsigned long long)y << 32) | (uint32_t)x;
+}
+
+__device__ __forceinline__ size_t edge_slot(unsigned long long k, size_t mask) {   // murmur3's 64-bit finaliser
+    k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
+    return (size_t)k & mask;
+}
+
+__device__ __forceinline__ bool in_box(const FilterArgs& a, int32_t v) {
+    const float* p = a.vertices + 3 * (size_t)v;
+    bool in = true;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+        const double x = (double)__ldg(p + r);
+        in &= x >= a.lo[r] && x <= a.hi[r];                 // false for NaN
+    }
+    return in;
+}
+
+__global__ void __launch_bounds__(kMeshThreads) filter_crop_kernel(FilterArgs a) {
+    const long long t = (long long)blockIdx.x * kMeshThreads + threadIdx.x;
+    if (t >= a.Nt) return;
+    const int32_t* tri = a.triangles + 3 * (size_t)t;
+    const int32_t x = __ldg(tri), y = __ldg(tri + 1), z = __ldg(tri + 2);
+    bool live;
+    if ((uint32_t)x >= (uint32_t)a.Nv || (uint32_t)y >= (uint32_t)a.Nv || (uint32_t)z >= (uint32_t)a.Nv) {
+        atomicAdd(a.totals + 3, 1);
+        live = false;
+    } else {
+        live = !a.crop || (in_box(a, x) && in_box(a, y) && in_box(a, z));
+    }
+    a.parent[t] = live ? (int32_t)t : -1;
+}
+
+// pass one: every live triangle's three edges into the table; a slot's owner ends as the smallest triangle on its edge
+__global__ void __launch_bounds__(kMeshThreads) filter_insert_kernel(FilterArgs a) {
+    const long long t = (long long)blockIdx.x * kMeshThreads + threadIdx.x;
+    if (t >= a.Nt || a.parent[t] < 0) return;
+    const int32_t* tri = a.triangles + 3 * (size_t)t;
+    const int32_t v[3] = {__ldg(tri), __ldg(tri + 1), __ldg(tri + 2)};
+#pragma unroll
+    for (int e = 0; e < 3; ++e) {
+        const unsigned long long key = edge_key(v[e], v[e == 2 ? 0 : e + 1]);
+        for (size_t h = edge_slot(key, a.mask);; h = (h + 1) & a.mask) {
+            const unsigned long long prev = atomicCAS(a.keys + h, kEmptyKey, key);
+            if (prev == kEmptyKey || prev == key) {
+                atomicMin(a.owner + h, (uint32_t)t);
+                break;
+            }
+        }
+    }
+}
+
+// root of x with path splitting (ECL-CC): every parent is <= its child, so a root is its component's smallest triangle
+__device__ __forceinline__ int32_t find_root(volatile int32_t* parent, int32_t x) {
+    int32_t cur = parent[x];
+    if (cur != x) {
+        int32_t next, prev = x;
+        while (cur > (next = parent[cur])) {
+            parent[prev] = next;
+            prev = cur;
+            cur = next;
+        }
+    }
+    return cur;
+}
+
+// pass two: each live triangle joins the owners of its edges, hooking the larger root under the smaller
+__global__ void __launch_bounds__(kMeshThreads) filter_union_kernel(FilterArgs a) {
+    const long long t = (long long)blockIdx.x * kMeshThreads + threadIdx.x;
+    if (t >= a.Nt || a.parent[t] < 0) return;
+    const int32_t* tri = a.triangles + 3 * (size_t)t;
+    const int32_t v[3] = {__ldg(tri), __ldg(tri + 1), __ldg(tri + 2)};
+#pragma unroll
+    for (int e = 0; e < 3; ++e) {
+        const unsigned long long key = edge_key(v[e], v[e == 2 ? 0 : e + 1]);
+        size_t h = edge_slot(key, a.mask);
+        while (a.keys[h] != key) h = (h + 1) & a.mask;
+        const int32_t o = (int32_t)a.owner[h];
+        if (o == t) continue;
+        int32_t ra = find_root(a.parent, (int32_t)t), rb = find_root(a.parent, o);
+        while (ra != rb) {
+            if (ra > rb) { const int32_t s = ra; ra = rb; rb = s; }
+            const int32_t prev = atomicCAS(a.parent + rb, rb, ra);
+            if (prev == rb) break;
+            rb = prev;                                      // rb was hooked meanwhile: retry from its new parent
+        }
+    }
+}
+
+// every live triangle's root into label, the roots' sizes and the cluster count
+__global__ void __launch_bounds__(kMeshThreads) filter_label_kernel(FilterArgs a) {
+    const long long t = (long long)blockIdx.x * kMeshThreads + threadIdx.x;
+    if (t >= a.Nt) return;
+    if (a.parent[t] < 0) {
+        a.label[t] = kDead;
+        return;
+    }
+    const int32_t r = find_root(a.parent, (int32_t)t);
+    a.label[t] = (uint32_t)r;
+    const unsigned peers = __match_any_sync(__activemask(), r);     // neighbours are mostly in one cluster
+    if ((threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(a.size + r, (uint32_t)__popc(peers));
+    if (r == t) atomicAdd(a.totals + 2, 1);
+}
+
+// one thread: pass < 0 sets the rank min(C, keep); pass p fixes digit p (most significant first) of that rank's size
+__global__ void filter_select_kernel(FilterArgs a, int pass) {
+    if (pass < 0) {
+        a.sel[0] = 0;
+        a.sel[1] = min((uint32_t)a.totals[2], (uint32_t)a.keep);
+        return;
+    }
+    const uint32_t k = a.sel[1];
+    if (!k) return;
+    const uint32_t* h = a.hist + 256 * pass;
+    uint32_t cum = 0;
+    for (int d = 255; d >= 0; --d) {
+        if (cum + h[d] >= k) {
+            a.sel[0] |= (uint32_t)d << (24 - 8 * pass);
+            a.sel[1] = k - cum;
+            return;
+        }
+        cum += h[d];
+    }
+}
+
+// histogram of digit `pass` over the roots whose higher digits equal the prefix found so far
+__global__ void __launch_bounds__(kMeshThreads) filter_hist_kernel(FilterArgs a, int pass) {
+    __shared__ uint32_t h[256];
+    static_assert(kMeshThreads == 256, "one bin per thread");
+    h[threadIdx.x] = 0;
+    __syncthreads();
+    const long long t = (long long)blockIdx.x * kMeshThreads + threadIdx.x;
+    if (t < a.Nt && a.sel[1] && a.label[t] == (uint32_t)t) {
+        const int shift = 24 - 8 * pass;
+        const uint32_t s = a.size[t], high = pass ? ~0u << (shift + 8) : 0u;
+        if ((s & high) == (a.sel[0] & high)) atomicAdd(h + ((s >> shift) & 255), 1u);
+    }
+    __syncthreads();
+    if (h[threadIdx.x]) atomicAdd(a.hist + 256 * pass + threadIdx.x, h[threadIdx.x]);
+}
+
+// keep flags over the labels, and idempotent used marks of the kept triangles' vertices
+__global__ void __launch_bounds__(kMeshThreads) filter_keep_kernel(FilterArgs a) {
+    const long long t = (long long)blockIdx.x * kMeshThreads + threadIdx.x;
+    if (t >= a.Nt) return;
+    const uint32_t r = a.label[t];
+    const bool kept = r != kDead && a.size[r] >= a.sel[0];
+    a.label[t] = kept ? 1u : 0u;
+    if (kept) {
+        const int32_t* tri = a.triangles + 3 * (size_t)t;
+        a.used[__ldg(tri)] = 1u;
+        a.used[__ldg(tri + 1)] = 1u;
+        a.used[__ldg(tri + 2)] = 1u;
+    }
+}
+
+struct FilterEmitArgs {
+    int Nv, Nt, Nv_out, Nt_out;
+    const float* vertices; const float* colors; const int32_t* triangles;
+    const uint32_t* label; const uint32_t* used;
+    float* out_vertices; float* out_colors; int32_t* out_triangles;
+};
+
+// one thread per vertex and per triangle (the same index), each written at its scanned offset
+__global__ void __launch_bounds__(kMeshThreads) filter_emit_kernel(FilterEmitArgs a) {
+    const long long i = (long long)blockIdx.x * kMeshThreads + threadIdx.x;
+    if (i < a.Nv) {
+        const uint32_t o = a.used[i];
+        if (a.used[i + 1] != o && o < (uint32_t)a.Nv_out) {
+#pragma unroll
+            for (int r = 0; r < 3; ++r) {
+                a.out_vertices[3 * (size_t)o + r] = __ldg(a.vertices + 3 * (size_t)i + r);
+                a.out_colors[3 * (size_t)o + r] = __ldg(a.colors + 3 * (size_t)i + r);
+            }
+        }
+    }
+    if (i < a.Nt) {
+        const uint32_t o = a.label[i];
+        if (a.label[i + 1] != o && o < (uint32_t)a.Nt_out) {
+#pragma unroll
+            for (int m = 0; m < 3; ++m) {
+                const int32_t v = __ldg(a.triangles + 3 * (size_t)i + m);
+                a.out_triangles[3 * (size_t)o + m] = (uint32_t)v < (uint32_t)a.Nv ? (int32_t)a.used[v] : -1;
+            }
+        }
     }
 }
 
@@ -402,4 +638,96 @@ extern "C" int srf_mesh_emit(void* stream, const int* n0, const int* dims, float
     srf::mesh_emit_kernel<<<(unsigned)blocks, srf::kMeshThreads, 0, (cudaStream_t)stream>>>(a);
     const cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? 0 : cuda_error("mesh_emit launch", e);
+}
+
+extern "C" int srf_mesh_filter_workspace_bytes(int Nv, int Nt, size_t* bytes) {
+    if (Nv < 0 || Nt < 0) return set_error("srf_mesh_filter_workspace_bytes: bad sizes (Nv=%d, Nt=%d)", Nv, Nt);
+    if (!bytes) return set_error("srf_mesh_filter_workspace_bytes: null output");
+    *bytes = srf::filter_layout((size_t)Nv, (size_t)Nt).total;
+    return 0;
+}
+
+extern "C" int srf_mesh_filter_count(void* stream_, int Nv, int Nt, const float* vertices, const int32_t* triangles,
+                                     const double* aabb, int keep, void* workspace, int32_t* totals) {
+    const char* fn = "srf_mesh_filter_count";
+    if (Nv < 0 || Nt < 0) return set_error("%s: bad sizes (Nv=%d, Nt=%d)", fn, Nv, Nt);
+    if (keep < 1) return set_error("%s: keep must be >= 1, got %d", fn, keep);
+    if ((Nv > 0 && !vertices) || (Nt > 0 && !triangles) || !totals) return set_error("%s: null pointer", fn);
+    if (!workspace || srf::misaligned(workspace)) return set_error("%s: workspace must be 256-byte aligned", fn);
+    const cudaStream_t stream = (cudaStream_t)stream_;
+    const srf::FilterWorkspace l = srf::filter_layout((size_t)Nv, (size_t)Nt);
+    char* ws = static_cast<char*>(workspace);
+    srf::FilterArgs a;
+    a.Nv = Nv; a.Nt = Nt; a.keep = keep; a.crop = aabb != nullptr;
+    for (int r = 0; r < 3; ++r) {
+        a.lo[r] = aabb ? aabb[r] : 0.0;
+        a.hi[r] = aabb ? aabb[3 + r] : 0.0;
+    }
+    a.mask = l.slots - 1;
+    a.vertices = vertices; a.triangles = triangles;
+    a.keys = reinterpret_cast<unsigned long long*>(ws + l.keys);
+    a.owner = reinterpret_cast<uint32_t*>(ws + l.owner);
+    a.parent = reinterpret_cast<int32_t*>(ws + l.parent);
+    a.size = reinterpret_cast<uint32_t*>(ws + l.size);
+    a.label = reinterpret_cast<uint32_t*>(ws + l.label);
+    a.used = reinterpret_cast<uint32_t*>(ws + l.used);
+    a.hist = reinterpret_cast<uint32_t*>(ws + l.hist);
+    a.sel = reinterpret_cast<uint32_t*>(ws + l.sel);
+    a.totals = totals;
+    uint32_t* sums = reinterpret_cast<uint32_t*>(ws + l.sums);
+    cudaError_t e;
+    if ((e = cudaMemsetAsync(totals, 0, 4 * sizeof(int32_t), stream)) != cudaSuccess ||
+        (e = cudaMemsetAsync(a.used, 0, 4 * (size_t)Nv, stream)) != cudaSuccess)
+        return cuda_error("memset mesh filter totals", e);
+    if (Nt > 0) {
+        if ((e = cudaMemsetAsync(a.keys, 0xff, 8 * l.slots, stream)) != cudaSuccess ||
+            (e = cudaMemsetAsync(a.owner, 0xff, 4 * l.slots, stream)) != cudaSuccess ||
+            (e = cudaMemsetAsync(a.size, 0, 4 * (size_t)Nt, stream)) != cudaSuccess ||
+            (e = cudaMemsetAsync(a.hist, 0, 4 * 256 * srf::kSelectPasses, stream)) != cudaSuccess)
+            return cuda_error("memset mesh filter workspace", e);
+        const unsigned blocks = (unsigned)(((size_t)Nt + srf::kMeshThreads - 1) / srf::kMeshThreads);
+        srf::filter_crop_kernel<<<blocks, srf::kMeshThreads, 0, stream>>>(a);
+        srf::filter_insert_kernel<<<blocks, srf::kMeshThreads, 0, stream>>>(a);
+        srf::filter_union_kernel<<<blocks, srf::kMeshThreads, 0, stream>>>(a);
+        srf::filter_label_kernel<<<blocks, srf::kMeshThreads, 0, stream>>>(a);
+        srf::filter_select_kernel<<<1, 1, 0, stream>>>(a, -1);
+        for (int pass = 0; pass < srf::kSelectPasses; ++pass) {
+            srf::filter_hist_kernel<<<blocks, srf::kMeshThreads, 0, stream>>>(a, pass);
+            srf::filter_select_kernel<<<1, 1, 0, stream>>>(a, pass);
+        }
+        srf::filter_keep_kernel<<<blocks, srf::kMeshThreads, 0, stream>>>(a);
+        if ((e = cudaGetLastError()) != cudaSuccess) return cuda_error("mesh filter launch", e);
+    }
+    // with Nt = 0 the label flags are empty and the used flags all 0: the scans write the totals 0
+    if ((e = srf::exclusive_scan(a.used, (size_t)Nv, sums + l.nb_tri, l.nb_vert, totals, stream)) != cudaSuccess ||
+        (e = srf::exclusive_scan(a.label, (size_t)Nt, sums, l.nb_tri, totals + 1, stream)) != cudaSuccess)
+        return cuda_error("mesh filter scan launch", e);
+    return 0;
+}
+
+extern "C" int srf_mesh_filter_emit(void* stream, int Nv, int Nt, const float* vertices, const float* colors,
+                                    const int32_t* triangles, const void* workspace, int Nv_out, int Nt_out,
+                                    float* out_vertices, float* out_colors, int32_t* out_triangles) {
+    const char* fn = "srf_mesh_filter_emit";
+    if (Nv < 0 || Nt < 0) return set_error("%s: bad sizes (Nv=%d, Nt=%d)", fn, Nv, Nt);
+    if (Nv_out < 0 || Nt_out < 0 || Nv_out > Nv || Nt_out > Nt)
+        return set_error("%s: bad totals (Nv_out=%d, Nt_out=%d for Nv=%d, Nt=%d)", fn, Nv_out, Nt_out, Nv, Nt);
+    if ((Nv > 0 && (!vertices || !colors)) || (Nt > 0 && !triangles)) return set_error("%s: null input pointer", fn);
+    if (!workspace || srf::misaligned(workspace)) return set_error("%s: workspace must be 256-byte aligned", fn);
+    if ((Nv_out > 0 && (!out_vertices || !out_colors)) || (Nt_out > 0 && !out_triangles))
+        return set_error("%s: null output pointer", fn);
+    if (Nv_out == 0 && Nt_out == 0) return 0;
+    const srf::FilterWorkspace l = srf::filter_layout((size_t)Nv, (size_t)Nt);
+    const char* ws = static_cast<const char*>(workspace);
+    srf::FilterEmitArgs a;
+    a.Nv = Nv; a.Nt = Nt; a.Nv_out = Nv_out; a.Nt_out = Nt_out;
+    a.vertices = vertices; a.colors = colors; a.triangles = triangles;
+    a.label = reinterpret_cast<const uint32_t*>(ws + l.label);
+    a.used = reinterpret_cast<const uint32_t*>(ws + l.used);
+    a.out_vertices = out_vertices; a.out_colors = out_colors; a.out_triangles = out_triangles;
+    const size_t n = (size_t)(Nv > Nt ? Nv : Nt);
+    const unsigned blocks = (unsigned)((n + srf::kMeshThreads - 1) / srf::kMeshThreads);
+    srf::filter_emit_kernel<<<blocks, srf::kMeshThreads, 0, (cudaStream_t)stream>>>(a);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : cuda_error("mesh_filter_emit launch", e);
 }

@@ -3,18 +3,21 @@ and marching cubes in CUDA (``csrc/mesh.cu``, C ABI ``include/surfel_mesh.h``), 
 
 LaRa's ``MeshExtractor.extract`` renders 48 views, copies each to the host and fuses it into open3d's CPU
 ``ScalableTSDFVolume``, then runs open3d's marching cubes and a cluster filter.  Here the forward-only renders are fused
-on the device as the fused epilogue leaves them, the mesh is extracted on the device and only the filter (connected
-components, as LaRa runs them) and the file write are on the host:
+on the device as the fused epilogue leaves them, the mesh is extracted and filtered (edge-connected clusters, as LaRa
+filters them) on the device, and only the filtered mesh is copied to the host for the file write:
 
     vol = tsdf_volume(depth, acc, records, voxel_size, sdf_trunc, alpha_thres, aabb)
     integrate(vol, depth, acc, image, records, alpha_thres)
-    vertices, triangles, colors = filter_mesh(extract_triangle_mesh(vol), aabb)
+    vertices, triangles, colors = filter_mesh_device(extract_triangle_mesh(vol), aabb)
     write_obj(path, vertices, triangles, colors)
+
+``filter_mesh`` is the same filter on the host (numpy and scipy), equal to ``filter_mesh_device`` element for element.
 
 ``MeshExtractor`` wraps these behind LaRa's class, with the camera list in place of ``uni_mesh_path``'s arguments.
 """
 from __future__ import annotations
 
+import ctypes
 import math
 from dataclasses import dataclass
 from typing import Optional, Sequence, Tuple
@@ -220,6 +223,52 @@ def filter_mesh(mesh, aabb: Optional[np.ndarray], keep: int = 10):
             np.ascontiguousarray(colors[used]))
 
 
+def _check_mesh(vertices, triangles, colors):
+    for name, t, dtype in (("vertices", vertices, torch.float32), ("triangles", triangles, torch.int32),
+                           ("colors", colors, torch.float32)):
+        if not isinstance(t, torch.Tensor) or t.dtype != dtype or not t.is_cuda:
+            raise RuntimeError(f"filter_mesh_device: {name} must be a {dtype} CUDA tensor")
+        if t.device != vertices.device:
+            raise RuntimeError(f"filter_mesh_device: {name} must be on {vertices.device}, got {t.device}")
+        if t.ndim != 2 or t.shape[1] != 3:
+            raise RuntimeError(f"filter_mesh_device: {name} must be [N,3], got {tuple(t.shape)}")
+        if not t.is_contiguous():
+            raise RuntimeError(f"filter_mesh_device: {name} must be contiguous")
+    if colors.shape[0] != vertices.shape[0]:
+        raise RuntimeError(f"filter_mesh_device: colors must be {tuple(vertices.shape)}, got {tuple(colors.shape)}")
+    return int(vertices.shape[0]), int(triangles.shape[0])
+
+
+def filter_mesh_device(mesh, aabb: Optional[np.ndarray] = None, keep: int = 10):
+    """:func:`filter_mesh` on the device (``srf_mesh_filter_count`` / ``_emit``): the same crop to ``aabb`` ([2,3]
+    float64, inclusive, each float32 coordinate compared as a float64), edge-connected clusters, the cut at the
+    min(#clusters, keep)-th largest count and the compaction, equal to it element for element.  ``mesh`` is
+    (vertices [Nv,3] float32, triangles [Nt,3] int32, colors [Nv,3] float32) on one CUDA device, e.g. the output of
+    :func:`extract_triangle_mesh`; returns the filtered three as CUDA tensors on that device.  Runs on torch's current
+    stream with one host read of the counts; an index outside [0, Nv) raises ``RuntimeError`` before any output is
+    written."""
+    vertices, triangles, colors = mesh
+    Nv, Nt = _check_mesh(vertices, triangles, colors)
+    dev = vertices.device
+    box = None
+    if aabb is not None:
+        box = (ctypes.c_double * 6)(*np.asarray(aabb, dtype=np.float64).reshape(6).tolist())
+    lib = _lib.load()
+    ws = torch.empty(_lib.mesh_filter_workspace_bytes(lib, Nv, Nt), dtype=torch.uint8, device=dev)
+    totals = torch.empty(4, dtype=torch.int32, device=dev)
+    _lib.launch("srf_mesh_filter_count", dev, Nv, Nt, vertices.data_ptr(), triangles.data_ptr(), box,
+                min(int(keep), 2**31 - 1), ws.data_ptr(), totals.data_ptr())
+    nv, nt, _clusters, invalid = (int(x) for x in totals.cpu())
+    if invalid:
+        raise RuntimeError(f"filter_mesh_device: {invalid} triangles have an index outside [0, {Nv})")
+    out_v = torch.empty((nv, 3), dtype=torch.float32, device=dev)
+    out_c = torch.empty((nv, 3), dtype=torch.float32, device=dev)
+    out_t = torch.empty((nt, 3), dtype=torch.int32, device=dev)
+    _lib.launch("srf_mesh_filter_emit", dev, Nv, Nt, vertices.data_ptr(), colors.data_ptr(), triangles.data_ptr(),
+                ws.data_ptr(), nv, nt, out_v.data_ptr(), out_c.data_ptr(), out_t.data_ptr())
+    return out_v, out_t, out_c
+
+
 def write_obj(path: str, vertices, triangles, colors) -> None:
     """``v x y z r g b`` lines (9 significant digits: float32 values read back exactly) and 1-based ``f a b c``."""
     v, t, c = _numpy(vertices), _numpy(triangles), _numpy(colors)
@@ -260,15 +309,15 @@ class MeshExtractor:
     @torch.no_grad()
     def extract(self, save_mesh_path: Optional[str], cams: Sequence, voxel_size: float = 2 / 256,
                 sdf_trunc: float = 0.08, alpha_thres: float = 0.08, depth_trunc: float = 10, device="cuda"):
-        """Render ``cams``, fuse, extract, filter and write the mesh to ``save_mesh_path`` (OBJ; None writes nothing).
-        Returns (vertices [Nv,3], triangles [Nt,3] int32, colors [Nv,3]) as CPU tensors."""
+        """Render ``cams``, fuse, extract and filter on the device, and write the mesh to ``save_mesh_path`` (OBJ; None
+        writes nothing).  Returns (vertices [Nv,3], triangles [Nt,3] int32, colors [Nv,3]) as CPU tensors."""
         voxel_size, sdf_trunc, center, radius = mesh_settings(self.aabb, voxel_size, sdf_trunc)
         device = torch.device(device)
         depth, acc, image = self._render(cams, device)
         records = camera_records(cams, device, center, radius, depth_trunc)
         vol = tsdf_volume(depth, acc, records, voxel_size, sdf_trunc, alpha_thres, self.aabb)
         integrate(vol, depth, acc, image, records, alpha_thres)
-        vertices, triangles, colors = filter_mesh(extract_triangle_mesh(vol), self.aabb)
+        vertices, triangles, colors = (x.cpu() for x in filter_mesh_device(extract_triangle_mesh(vol), self.aabb))
         if save_mesh_path is not None:
             write_obj(save_mesh_path, vertices, triangles, colors)
-        return torch.from_numpy(vertices), torch.from_numpy(triangles), torch.from_numpy(colors)
+        return vertices, triangles, colors

@@ -1,10 +1,13 @@
 """LaRa's mesh path on the GPU (DESIGN §3.15), stage by stage: the forward-only render of the 48 cameras (16 azimuths x
 {0, -30, 30} deg, radius 1.905, fov 0.75, 512 x 512), TSDF integration, marching-cubes count, the host read of the
-two totals, emit, the host filter and the OBJ write, for scene(524288) and for an almost empty scene (the fixed
-costs), with LaRa's aabb config.  Device stages are timed with CUDA events, host stages with a host clock after a
-synchronise; each stage's median and range over --rounds rounds after one warm-up round.  Also the peak memory, Nv / Nt
-and the integrate kernel against its floor computed from the shapes.  open3d's CPU integration is not measured (it is
-not installed in any environment of this project).  Prints the card name and power limit, then one JSON line per scene.
+two totals, emit, the device filter (filter_mesh_device, its one host read of the counts included), the host copy of
+the filtered mesh and the OBJ write, for scene(524288) and for an almost empty scene (the fixed costs), with LaRa's
+aabb config.  The host filter (filter_mesh, with its copy of the unfiltered mesh) is timed in the same rounds for
+comparison, and its output is checked equal to the device filter's.  Device stages are timed with CUDA events, host
+stages with a host clock after a synchronise; each stage's median and range over --rounds rounds after one warm-up
+round.  Also the peak memory, Nv / Nt before and after the filter and the integrate kernel against its floor computed
+from the shapes.  open3d's CPU integration is not measured (it is not installed in any environment of this project).
+Prints the card name and power limit, then one JSON line per scene.
 
     python tools/bench_mesh.py [--rounds 5] [--points 524288,64]
 """
@@ -45,7 +48,8 @@ def run_point(P: int, rounds: int) -> dict:
     vs, st, center, radius = MS.mesh_settings(aabb, 2 / 256, 0.08)
     rec = MS.camera_records(cams, dev, center, radius)
     ev = lambda: torch.cuda.Event(enable_timing=True)      # noqa: E731
-    times = {k: [] for k in ("render", "integrate", "count", "readback", "emit", "filter", "obj_write")}
+    times = {k: [] for k in ("render", "integrate", "count", "readback", "emit", "filter_device", "filtered_copy",
+                             "host_filter", "obj_write")}
     tmp = tempfile.mkdtemp()
     out = {}
     for rnd in range(rounds + 1):
@@ -81,13 +85,21 @@ def run_point(P: int, rounds: int) -> dict:
         _lib.launch("srf_mesh_emit", dev, _lib.int3(vol.n0), dims, vol.voxel_size, vol.tsdf.data_ptr(),
                     vol.color.data_ptr(), ws.data_ptr(), Nv, Nt, verts.data_ptr(), cols.data_ptr(), tris.data_ptr())
         f[1].record()
+        g = [ev(), ev()]
+        g[0].record()
+        dv = MS.filter_mesh_device((verts, tris, cols), aabb)
+        g[1].record()
         torch.cuda.synchronize()
         peak = torch.cuda.max_memory_allocated() - base
         h2 = time.perf_counter()
-        fv, ft, fc = MS.filter_mesh((verts, tris, cols), aabb)
+        fv, ft, fc = (x.cpu().numpy() for x in dv)
         h3 = time.perf_counter()
         MS.write_obj(os.path.join(tmp, "mesh.obj"), fv, ft, fc)
         h4 = time.perf_counter()
+        hv, ht, hc = MS.filter_mesh((verts, tris, cols), aabb)
+        h5 = time.perf_counter()
+        if not (np.array_equal(fv, hv) and np.array_equal(ft, ht) and np.array_equal(fc, hc)):
+            raise SystemExit("bench_mesh: the device filter's output differs from the host filter's")
         if rnd == 0:      # warm-up round
             continue
         times["render"].append(e[0].elapsed_time(e[1]))
@@ -95,11 +107,13 @@ def run_point(P: int, rounds: int) -> dict:
         times["count"].append(e[4].elapsed_time(e[5]))
         times["readback"].append(1e3 * (h1 - h0))
         times["emit"].append(f[0].elapsed_time(f[1]))
-        times["filter"].append(1e3 * (h3 - h2))
+        times["filter_device"].append(g[0].elapsed_time(g[1]))
+        times["filtered_copy"].append(1e3 * (h3 - h2))
+        times["host_filter"].append(1e3 * (h5 - h4))
         times["obj_write"].append(1e3 * (h4 - h3))
         out = {"dims": list(vol.dims), "voxels": int(np.prod(vol.dims)), "Nv": Nv, "Nt": Nt,
                "Nv_filtered": len(fv), "Nt_filtered": len(ft), "peak_bytes": int(peak)}
-        del o, depth, acc, image, vol, ws, verts, cols, tris
+        del o, depth, acc, image, vol, ws, verts, cols, tris, dv
     N = out["voxels"]
     V, HW = len(cams), 512 * 512
     floor_bytes = 40 * N + V * HW * 4 * 5           # state read + written once; depth, acc, image read once
