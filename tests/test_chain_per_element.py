@@ -492,9 +492,12 @@ def test_decoder_per_element(cuda_device, B, N, K_, sh_dim):
 
 # -------------------------------------------------------------------------------------- GPU: the chain, link by link
 
-def _chain(dev, det, ms_ssim):
+def _chain(dev, det, ms_ssim, fine=False):
     """decoder output -> gaussians_from_decoder -> render_scene_views (raw activations, LaRa rays, V = 3) ->
-    scene_loss(iter=5000) -> backward, with every boundary's maps kept."""
+    scene_loss(iter=5000) -> backward, with every boundary's maps kept.  `fine`: LaRa's fine pass as well -- a seeded
+    mask with voxels of 0, 1 and 2 masked Gaussians, sample_point_feats on the first n_sel = 2 coarse views,
+    FineHead(80, 12).fine_shs on a volume_feat_up leaf, the masked render and scene_loss(prex="_fine") added to the
+    coarse loss."""
     from lara_b200 import rasterizer as R
     from lara_b200 import scene as S
     from lara_b200.decoder_layout import gaussians_from_decoder
@@ -536,39 +539,169 @@ def _chain(dev, det, ms_ssim):
         for k in OUT_KEYS:
             out[k].retain_grad()
         loss, stats = scene_loss(out, tar, 5000, ms_ssim=ms_ssim)
-        (loss * 2.0).backward()
+        extra = _fine_pass(dev, out, centers, shs, opacity, scaling, rotation, cams, settings, rays, tar, N, K_,
+                           sh_dim) if fine else {}
+        total = loss + extra["loss_fine"] if fine else loss
+        (total * 2.0).backward()
         torch.cuda.synchronize()
     finally:
         torch.use_deterministic_algorithms(prev)
     return dict(feats=feats, grid=grid, x=x, dec=dec, out=out, loss=loss, stats=stats, tar=tar, cams=cams, rays=rays,
-                settings=settings, params=(centers, shs, opacity, scaling, rotation), K=K_, sh_dim=sh_dim)
+                settings=settings, params=(centers, shs, opacity, scaling, rotation), K=K_, sh_dim=sh_dim, **extra)
+
+
+N_SEL = 2
+
+
+def _pinhole(cams):
+    """w2c [V,4,4] and the pinhole ixt [V,3,3] of the cameras (principal point at the image centre)."""
+    w2c = torch.stack([c.viewmatrix.T for c in cams]).contiguous()
+    ixt = torch.zeros((len(cams), 3, 3))
+    for v, c in enumerate(cams):
+        W, H = c.image_width, c.image_height
+        ixt[v, 0, 0], ixt[v, 1, 1] = W / (2 * c.tanfovx), H / (2 * c.tanfovy)
+        ixt[v, 0, 2], ixt[v, 1, 2], ixt[v, 2, 2] = W / 2, H / 2, 1.0
+    return w2c, ixt
+
+
+def _fine_pass(dev, out, centers, shs, opacity, scaling, rotation, cams, settings, rays, tar, N, K_, sh_dim):
+    from lara_b200.loss import scene_loss
+    from lara_b200.multiview import render_scene_views
+    from lara_b200.point_feats import sample_point_feats
+    from test_fine_head import _head
+    V, H, W = len(cams), cams[0].image_height, cams[0].image_width
+    g = torch.Generator().manual_seed(79)
+    mask = (torch.rand((N * K_,), generator=g) < 0.5).to(dev)
+    per_voxel = mask.view(N, K_).sum(1)
+    assert all(bool((per_voxel == c).any()) for c in range(K_ + 1))
+    img_ref = torch.rand((N_SEL, 3, H, W), generator=g).to(dev)
+    vf = (torch.randn((N, 80), generator=g) * 0.5 + 0.3).to(dev).requires_grad_(True)
+    head = _head(80, sh_dim, 13, dev)
+    w2c, ixt = (t.to(dev) for t in _pinhole(cams))
+    pts = centers[mask]
+    pts.retain_grad()
+    pf = sample_point_feats(pts, img_ref, {k: out[k][:N_SEL] for k in ("image", "acc_map", "depth")}, w2c[:N_SEL],
+                            ixt[:N_SEL])
+    pf.retain_grad()
+    shs_fine = head.fine_shs(vf, K_, mask, pf, shs)
+    fp = [centers[mask], shs_fine, opacity[mask], scaling[mask], rotation[mask]]
+    for t in fp:
+        t.retain_grad()
+    fine = render_scene_views(fp[0], fp[1], fp[2], fp[3], fp[4], settings, rays=rays, raw_activations=True,
+                              prex="_fine")
+    for k in OUT_KEYS:
+        fine[k + "_fine"].retain_grad()
+    loss_fine, _ = scene_loss(fine, tar, 5000, prex="_fine")
+    return dict(mask=mask, img_ref=img_ref, vf=vf, head=head, w2c=w2c, ixt=ixt, pts=pts, pf=pf, fine_params=fp,
+                fine=fine, loss_fine=loss_fine)
+
+
+def _render_link(prm, camt, cams, rays, dev):
+    """The renderer's forward again on the node's parameters (deterministic, so its state is the node's) and the
+    epilogue forward on its maps.  Returns (color, allmap, radii, state, [six epilogue outputs])."""
+    from lara_b200 import rasterizer as R
+    from lara_b200.epilogue import epilogue_views_forward_raw
+    centers, shs, opacity, scaling, rotation = prm
+    V, H, W = len(cams), cams[0].image_height, cams[0].image_width
+    color, allmap, radii, state = R.forward_views_raw(centers, shs, None, opacity, scaling, rotation, None, camt,
+                                                      cams[0].tanfovx, cams[0].tanfovy, H, W, 1, raw_activations=True)
+    new = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)     # noqa: E731
+    o = [new(V, 3, H, W), new(V, 1, H, W), new(V, H, W), new(V, 3, H, W), new(V, 3, H, W), new(V, H, W)]
+    epilogue_views_forward_raw(color, allmap, rays, camt, 0.0, *o)
+    return color, allmap, radii, state, o
+
+
+def _node_planar(out, prex=""):
+    """The node's six outputs and their gradients, planar."""
+    pl = lambda t: None if t is None else (t.permute(0, 3, 1, 2) if t.ndim == 4 else t).contiguous()    # noqa: E731
+    return ({k: pl(out[k + prex].detach()) for k in OUT_KEYS}, {k: pl(out[k + prex].grad) for k in OUT_KEYS})
+
+
+def _epilogue_fwd_link(o, out_nodes, col, am, rays, vms, ctx):
+    """The re-run epilogue equals the node bit for bit, and every view's outputs lie within epilogue64's bound."""
+    for k, t in zip(OUT_KEYS, o):
+        assert torch.equal(t, out_nodes[k]), f"{ctx} {k}"
+    w = 0.0
+    for v in range(col.shape[0]):
+        st = C.EpilogueState(col[v], am[v], rays[v], vms[v], 0.0)
+        r, band, _ = C.epilogue64(None, None, None, None, None, state=st)
+        assert band.sum() == 0
+        for k, t in zip(OUT_KEYS, o):
+            w = max(w, _compare(t[v].cpu().numpy(), r[k], ctx=f"{ctx} epilogue fwd view {v} {k}"))
+    return w
+
+
+def _epilogue_vjp_link(color, allmap, rays_t, camt, col, am, rays, vms, gpl, ctx):
+    """The epilogue backward given the node's upstream maps, every element within epilogue_vjp64's bound.  Returns
+    (d_color, d_allmap, worst)."""
+    from lara_b200.epilogue import epilogue_views_backward_raw
+    d_color, d_allmap = epilogue_views_backward_raw(color, allmap, rays_t, camt, 0.0, gpl["image"], gpl["depth"],
+                                                    gpl["acc_map"], gpl["rend_normal"], gpl["depth_normal"],
+                                                    gpl["rend_dist"])
+    dc, da = d_color.cpu().numpy(), d_allmap.cpu().numpy()
+    w = 0.0
+    for v in range(col.shape[0]):
+        st = C.EpilogueState(col[v], am[v], rays[v], vms[v], 0.0)
+        up = {k: (None if g is None else g[v].cpu().numpy()) for k, g in gpl.items()}
+        rc, ra, excl = _vjp(st, up)
+        assert excl.sum() == 0
+        w = max(w, _compare(dc[v], rc, ctx=f"{ctx} epilogue vjp view {v} d_color"),
+                _compare(da[v], ra, ctx=f"{ctx} view {v} d_allmap"))
+    return d_color, d_allmap, w
+
+
+GAUSS_KEYS = ("means3D", "sh", "opacities", "scales", "rotations")
+
+
+def _replay_link(state, radii, prm, camt, cams, d_color, d_allmap, det, ctx):
+    """The per-Gaussian backward given d_color / d_allmap, against the float64 replay of every view.  Returns
+    (kernel gradients, replay {key: (value, bound)}, band mask, worst)."""
+    from lara_b200 import rasterizer as R
+    from lara_b200.debug import unpack_state
+    from oracle import oracle as O
+    from test_grad_per_gaussian import _cam_dict
+    centers, shs, opacity, scaling, rotation = prm
+    V, H, W = len(cams), cams[0].image_height, cams[0].image_width
+    P = centers.shape[0]
+    g = R.backward_views_raw(state, radii, centers, shs, None, scaling, rotation, None, camt, cams[0].tanfovx,
+                             cams[0].tanfovy, H, W, 1, d_color, d_allmap, raw_activations=True, deterministic=det)
+    torch.cuda.synchronize()
+    dc, da = d_color.cpu().numpy(), d_allmap.cpu().numpy()
+    p = dict(means3D=centers.cpu().numpy(), shs=shs.cpu().numpy(), sh_degree=1, opacities=opacity.cpu().numpy(),
+             scales=scaling.cpu().numpy(), rotations=rotation.cpu().numpy(), raw_activations=True)
+    views, band = [], np.zeros(P, bool)
+    for v in range(V):
+        u = {k: x.cpu().numpy() for k, x in unpack_state(state, P, H, W, view=v).items()}
+        u["visible"] = radii[v].cpu().numpy() > 0
+        r = O.replay(u, np.ones(3, np.float32), dc[v], da[v])
+        views.append(O.view_vjp(u, r["g"], r["g_e"], p, _cam_dict(cams[v])))
+        band |= r["band"] != 0
+    ref = O.gaussian_grads(views, p, u["opacity"])
+    assert band.sum() < 1e-4 * P + 1, f"{ctx}: {int(band.sum())} band Gaussians"
+    w = 0.0
+    for k in GAUSS_KEYS:
+        v_, e_ = ref[k]
+        w = max(w, _compare(g[k].cpu().numpy().reshape(v_.shape), EB(v_, e_), _band(band, v_), f"{ctx} per-Gaussian {k}"))
+    return g, ref, band, w
+
+
+def _band(band, v_):
+    return band.reshape((-1,) + (1,) * (v_.ndim - 1))
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("det,ms_ssim", [(False, False), (True, False), (False, True)])
 def test_lara_chain_link_by_link(cuda_device, det, ms_ssim):
     from lara_b200 import rasterizer as R
-    from lara_b200.debug import unpack_state
-    from lara_b200.epilogue import epilogue_views_backward_raw, epilogue_views_forward_raw
-    from oracle import oracle as O
-    from test_grad_per_gaussian import _cam_dict
     dev = cuda_device
     ch = _chain(dev, det, ms_ssim)
     cams, settings, out = ch["cams"], ch["settings"], ch["out"]
     V, H, W = len(cams), cams[0].image_height, cams[0].image_width
-    centers, shs, opacity, scaling, rotation = (t.detach().contiguous() for t in ch["params"])
-    P = centers.shape[0]
+    prm = tuple(t.detach().contiguous() for t in ch["params"])
     camt = R.pack_cameras(settings, dev)
     # the node's state, repeated: the forward is deterministic, so its epilogue outputs equal the node's bit for bit
-    color, allmap, radii, state = R.forward_views_raw(centers, shs, None, opacity, scaling, rotation, None, camt,
-                                                      cams[0].tanfovx, cams[0].tanfovy, H, W, 1, raw_activations=True)
-    new = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)     # noqa: E731
-    o = [new(V, 3, H, W), new(V, 1, H, W), new(V, H, W), new(V, 3, H, W), new(V, 3, H, W), new(V, H, W)]
-    epilogue_views_forward_raw(color, allmap, ch["rays"], camt, 0.0, *o)
-    for k, t in zip(OUT_KEYS, o):
-        node = out[k].detach()
-        node = node.permute(0, 3, 1, 2) if node.ndim == 4 else node
-        assert torch.equal(t, node.contiguous()), k
+    color, allmap, radii, state, o = _render_link(prm, camt, cams, ch["rays"], dev)
+    nodes, gpl = _node_planar(out)
     col, am, rays = color.cpu().numpy(), allmap.cpu().numpy(), ch["rays"].cpu().numpy()
     vms = [c.viewmatrix.numpy().reshape(16) for c in cams]
     worst = {}
@@ -576,16 +709,7 @@ def test_lara_chain_link_by_link(cuda_device, det, ms_ssim):
     ref, _ = C.decoder64(ch["feats"], ch["grid"], ch["K"], ch["sh_dim"], -2.1792, -4.2, 0.5 / 16)
     worst["decoder fwd"] = max(_compare(t.detach().cpu().numpy(), r, ctx="decoder fwd") for t, r in zip(ch["dec"], ref))
     # 2. epilogue forward and 3. the loss, given their actual fp32 inputs
-    grads = {k: out[k].grad for k in OUT_KEYS}
-    gpl = {k: (None if g is None else (g.permute(0, 3, 1, 2) if g.ndim == 4 else g).contiguous()) for k, g in grads.items()}
-    w = 0.0
-    for v in range(V):
-        st = C.EpilogueState(col[v], am[v], rays[v], vms[v], 0.0)
-        r, band, _ = C.epilogue64(None, None, None, None, None, state=st)
-        assert band.sum() == 0
-        for k, t in zip(OUT_KEYS, o):
-            w = max(w, _compare(t[v].cpu().numpy(), r[k], ctx=f"epilogue fwd view {v} {k}"))
-    worst["epilogue fwd"] = w
+    worst["epilogue fwd"] = _epilogue_fwd_link(o, nodes, col, am, rays, vms, "coarse")
     pl = {k: t.cpu() for k, t in zip(OUT_KEYS, o)}
     n = V * H * W
     blocks = min(1024, -(-n // 256)) if det else min(8 * _sm_count(), -(-n // 256))
@@ -613,46 +737,17 @@ def test_lara_chain_link_by_link(cuda_device, det, ms_ssim):
         worst["loss value, ssim stat and g_image with MS-SSIM"] = max(w, _compare(gpl["image"].cpu().numpy(), lg["image"]))
     assert gpl["depth"] is None and gpl["acc_map"] is None
     # 4. epilogue vjp, given the node's upstream maps
-    d_color, d_allmap = epilogue_views_backward_raw(color, allmap, ch["rays"], camt, 0.0, gpl["image"], gpl["depth"],
-                                                    gpl["acc_map"], gpl["rend_normal"], gpl["depth_normal"],
-                                                    gpl["rend_dist"])
-    dc, da = d_color.cpu().numpy(), d_allmap.cpu().numpy()
-    w = 0.0
-    for v in range(V):
-        st = C.EpilogueState(col[v], am[v], rays[v], vms[v], 0.0)
-        up = {k: (None if g is None else g[v].cpu().numpy()) for k, g in gpl.items()}
-        rc, ra, excl = _vjp(st, up)
-        assert excl.sum() == 0
-        w = max(w, _compare(dc[v], rc, ctx=f"epilogue vjp view {v} d_color"), _compare(da[v], ra, ctx=f"view {v} d_allmap"))
-    worst["epilogue vjp"] = w
+    d_color, d_allmap, worst["epilogue vjp"] = _epilogue_vjp_link(color, allmap, ch["rays"], camt, col, am, rays, vms,
+                                                                  gpl, "coarse")
     # 5. per-Gaussian gradients: the replay of every view with the kernel's d_color / d_allmap
-    g = R.backward_views_raw(state, radii, centers, shs, None, scaling, rotation, None, camt, cams[0].tanfovx,
-                             cams[0].tanfovy, H, W, 1, d_color, d_allmap, raw_activations=True, deterministic=det)
-    torch.cuda.synchronize()
+    g, ref, band, w = _replay_link(state, radii, prm, camt, cams, d_color, d_allmap, det, "coarse")
     node = {"means3D": ch["dec"][0].grad, "sh": ch["dec"][1].grad, "scales": ch["dec"][2].grad,
             "rotations": ch["dec"][3].grad, "opacities": ch["dec"][4].grad}
-    for k, t in node.items():
-        a, b = g[k].reshape(-1), t.reshape(-1)
-        if det:
-            assert torch.equal(a, b), k            # the decomposition is the node's, bit for bit
-    p = dict(means3D=centers.cpu().numpy(), shs=shs.cpu().numpy(), sh_degree=1, opacities=opacity.cpu().numpy(),
-             scales=scaling.cpu().numpy(), rotations=rotation.cpu().numpy(), raw_activations=True)
-    views, band = [], np.zeros(P, bool)
-    for v in range(V):
-        u = {k: x.cpu().numpy() for k, x in unpack_state(state, P, H, W, view=v).items()}
-        u["visible"] = radii[v].cpu().numpy() > 0
-        r = O.replay(u, np.ones(3, np.float32), dc[v], da[v])
-        views.append(O.view_vjp(u, r["g"], r["g_e"], p, _cam_dict(cams[v])))
-        band |= r["band"] != 0
-    ref = O.gaussian_grads(views, p, u["opacity"])
-    assert band.sum() < 1e-4 * P + 1, f"{int(band.sum())} band Gaussians"
-    w = 0.0
-    for k in ("means3D", "sh", "opacities", "scales", "rotations"):
+    for k in GAUSS_KEYS:
         v_, e_ = ref[k]
-        got = g[k].cpu().numpy().reshape(v_.shape)
-        w = max(w, _compare(got, EB(v_, e_), band.reshape((-1,) + (1,) * (v_.ndim - 1)), f"per-Gaussian {k}"))
-        w = max(w, _compare(node[k].cpu().numpy().reshape(v_.shape), EB(v_, e_),
-                            band.reshape((-1,) + (1,) * (v_.ndim - 1)), f"node {k}"))
+        if det:
+            assert torch.equal(g[k].reshape(-1), node[k].reshape(-1)), k     # the decomposition is the node's
+        w = max(w, _compare(node[k].cpu().numpy().reshape(v_.shape), EB(v_, e_), _band(band, v_), f"node {k}"))
     worst["per-Gaussian"] = w
     # 6. decoder backward, given the node's parameter gradients
     _, gref = C.decoder64(ch["feats"], ch["grid"], ch["K"], ch["sh_dim"], -2.1792, -4.2, 0.5 / 16,
@@ -660,3 +755,129 @@ def test_lara_chain_link_by_link(cuda_device, det, ms_ssim):
     worst["decoder bwd"] = _compare(ch["x"].grad.cpu().numpy(), gref, ctx="decoder bwd")
     print(f"\n  chain det={det} ms_ssim={ms_ssim}: " + ", ".join(f"{k} {v:.3g}" for k, v in worst.items()) +
           f"; band-excluded Gaussians {int(band.sum())}")
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("det", [False, True])
+def test_lara_fine_chain_link_by_link(cuda_device, det):
+    """The coarse chain with LaRa's fine pass, link by link on each link's actual fp32 inputs: the sampler against
+    point_feats64, the head against fine_head_torch in float64 (1e-5 of each tensor's maximum), the fine render's
+    epilogue, loss and per-Gaussian replay through the coarse chain's helpers, and where the passes meet: the coarse
+    image / acc_map / depth node gradients (loss part + sampler part on views < n_sel), the Gaussians' node gradients
+    (coarse + mask-scattered fine + sampler point part) with the head's residual into shs, then the decoder backward."""
+    from lara_b200 import rasterizer as R
+    from oracle import point_feats64 as P
+    from oracle.fine_head_torch import fine_shs_torch
+    from test_fine_head import TOL, _err
+    from test_point_feats_per_element import _kernels
+    dev = cuda_device
+    ch = _chain(dev, det, False, fine=True)
+    cams, settings, out, fine = ch["cams"], ch["settings"], ch["out"], ch["fine"]
+    V, H, W = len(cams), cams[0].image_height, cams[0].image_width
+    prm = tuple(t.detach().contiguous() for t in ch["params"])
+    camt = R.pack_cameras(settings, dev)
+    rays, rays_t = ch["rays"].cpu().numpy(), ch["rays"]
+    vms = [c.viewmatrix.numpy().reshape(16) for c in cams]
+    n = V * H * W
+    blocks = min(1024, -(-n // 256)) if det else min(8 * _sm_count(), -(-n // 256))
+    mask = ch["mask"]
+    sfx = "_det" if det else ""
+    worst = {}
+    # coarse forward: render, epilogue and the loss value on their inputs
+    color, allmap, radii, state, o = _render_link(prm, camt, cams, rays_t, dev)
+    nodes, gpl = _node_planar(out)
+    col, am = color.cpu().numpy(), allmap.cpu().numpy()
+    worst["coarse epilogue fwd"] = _epilogue_fwd_link(o, nodes, col, am, rays, vms, "coarse")
+    pl = {k: t.cpu() for k, t in zip(OUT_KEYS, o)}
+    vals, lg = C.loss64(pl["image"], ch["tar"].cpu(), pl["rend_normal"], pl["depth_normal"], pl["acc_map"],
+                        pl["rend_dist"], True, 1, 2.0, blocks)
+    worst["coarse loss value"] = _compare(float(ch["loss"].detach()), EB(*vals["loss"]), ctx="coarse loss value")
+    # the sampler on its actual inputs: forward and the node's vjp; its rendering gradients from a re-run
+    pts = prm[0][mask]
+    rend = {k: out[k][:N_SEL].detach() for k in ("image", "acc_map", "depth")}
+    case = (pts, ch["img_ref"], rend, ch["w2c"][:N_SEL], ch["ixt"][:N_SEL])
+    up = ch["pf"].grad
+    st = P.point_feats64(pts, case[3], case[4], ch["img_ref"], rend["image"].permute(0, 3, 1, 2), rend["acc_map"],
+                         rend["depth"][..., 0], up)
+    assert not st["inf_pairs"].any()
+    rerun = _kernels(case, up, det, dev)
+    worst["sampler"] = max(_compare(ch["pf"].detach().cpu().numpy(), st["feats"], ctx="sampler feats"),
+                           _compare(ch["pts"].grad.cpu().numpy(), st["g_points"], ctx="sampler g_points (node)"),
+                           _compare(rerun["g_points"], st["g_points"], ctx="sampler g_points"),
+                           *[_compare(rerun[k], st[k + sfx], ctx=f"sampler {k}") for k in ("g_image", "g_acc", "g_depth")])
+    # the head against float64, on the node's inputs and upstream
+    params = [p.detach().double() for p in ch["head"]._params()]
+    vf64 = ch["vf"].detach().double().requires_grad_(True)
+    pf64 = ch["pf"].detach().double().requires_grad_(True)
+    shs64 = prm[1].double().requires_grad_(True)
+    shs_fine = ch["fine_params"][1]
+    o64 = fine_shs_torch(vf64, ch["K"], mask, pf64, shs64, params)
+    o64.backward(shs_fine.grad.double())
+    head = {"out": _err(shs_fine.detach(), o64.detach()), "g_volume_feat": _err(ch["vf"].grad, vf64.grad),
+            "g_point_feats": _err(ch["pf"].grad, pf64.grad)}
+    assert all(e <= TOL for e in head.values()), head
+    # the fine render: epilogue, loss (no regularisers under prex="_fine") and per-Gaussian replay
+    fprm = tuple(t.detach().contiguous() for t in ch["fine_params"])
+    colorf, allmapf, radiif, statef, of = _render_link(fprm, camt, cams, rays_t, dev)
+    nodesf, gplf = _node_planar(fine, "_fine")
+    colf, amf = colorf.cpu().numpy(), allmapf.cpu().numpy()
+    worst["fine epilogue fwd"] = _epilogue_fwd_link(of, nodesf, colf, amf, rays, vms, "fine")
+    plf = {k: t.cpu() for k, t in zip(OUT_KEYS, of)}
+    valsf, lgf = C.loss64(plf["image"], ch["tar"].cpu(), plf["rend_normal"], plf["depth_normal"], plf["acc_map"],
+                          plf["rend_dist"], False, 1, 2.0, blocks)
+    w = _compare(float(ch["loss_fine"].detach()), EB(*valsf["loss"]), ctx="fine loss value")
+    worst["fine loss"] = max(w, _compare(gplf["image"].cpu().numpy(), lgf["image"], ctx="fine loss image"))
+    assert all(gplf[k] is None or not bool(gplf[k].any()) for k in OUT_KEYS if k != "image")
+    dcf, daf, worst["fine epilogue vjp"] = _epilogue_vjp_link(colorf, allmapf, rays_t, camt, colf, amf, rays, vms,
+                                                              gplf, "fine")
+    _, reff, bandf, worst["fine per-Gaussian"] = _replay_link(statef, radiif, fprm, camt, cams, dcf, daf, det, "fine")
+    fnode = dict(zip(GAUSS_KEYS, (ch["fine_params"][0].grad, shs_fine.grad, ch["fine_params"][2].grad,
+                                  ch["fine_params"][3].grad, ch["fine_params"][4].grad)))
+    for k in GAUSS_KEYS:
+        v_, e_ = reff[k]
+        worst["fine per-Gaussian"] = max(worst["fine per-Gaussian"], _compare(
+            fnode[k].cpu().numpy().reshape(v_.shape), EB(v_, e_), _band(bandf, v_), f"fine node {k}"))
+    # where the passes meet (1): the coarse nodes' gradients, loss part + sampler part on the first n_sel views
+    samp = {"image": st["g_image" + sfx], "acc_map": st["g_acc" + sfx], "depth": st["g_depth" + sfx]}
+    w = 0.0
+    for k in ("image", "acc_map", "depth"):
+        shape = gpl[k].shape
+        base = lg[k] if k == "image" else EB(np.zeros(shape))
+        part = EB(np.zeros(shape), np.zeros(shape))
+        part.v[:N_SEL] = samp[k].v.reshape((N_SEL,) + shape[1:])
+        part.e[:N_SEL] = samp[k].e.reshape((N_SEL,) + shape[1:])
+        w = max(w, _compare(gpl[k].cpu().numpy(), P.add(EB(base.v, base.e), part), ctx=f"coarse node {k}"))
+    worst["coarse nodes: loss + sampler"] = w
+    # the coarse epilogue vjp and replay, given those node gradients
+    d_color, d_allmap, worst["coarse epilogue vjp"] = _epilogue_vjp_link(color, allmap, rays_t, camt, col, am, rays,
+                                                                         vms, gpl, "coarse")
+    _, ref, band, worst["coarse per-Gaussian"] = _replay_link(state, radii, prm, camt, cams, d_color, d_allmap, det,
+                                                              "coarse")
+    # where the passes meet (2): the Gaussians' node gradients, coarse + mask-scattered fine (+ the sampler's point
+    # gradient into the means, the head's residual into shs), in any order of autograd's additions
+    m = mask.cpu().numpy()
+    node = {"means3D": ch["dec"][0].grad, "sh": ch["dec"][1].grad, "scales": ch["dec"][2].grad,
+            "rotations": ch["dec"][3].grad, "opacities": ch["dec"][4].grad}
+    w = 0.0
+    for k in GAUSS_KEYS:
+        v_, e_ = ref[k]
+        fv, fe = np.zeros_like(v_), np.zeros_like(e_)
+        fv[m], fe[m] = reff[k][0], reff[k][1]
+        terms = [EB(v_, e_), EB(fv, fe)]
+        if k == "means3D":
+            sv, se = np.zeros_like(v_), np.zeros_like(e_)
+            sv[m], se[m] = st["g_points"].v, st["g_points"].e
+            terms.append(EB(sv, se))
+        excl = _band(band, v_).copy()
+        excl[m] |= _band(bandf, reff[k][0])
+        w = max(w, _compare(node[k].cpu().numpy().reshape(v_.shape), P.sum_any_order(terms), excl, f"node {k}"))
+    worst["Gaussian nodes: coarse + fine + sampler"] = w
+    # the decoder backward, given the node's parameter gradients
+    _, gref = C.decoder64(ch["feats"], ch["grid"], ch["K"], ch["sh_dim"], -2.1792, -4.2, 0.5 / 16,
+                          [t.grad.cpu().numpy() for t in ch["dec"]])
+    worst["decoder bwd"] = _compare(ch["x"].grad.cpu().numpy(), gref, ctx="decoder bwd")
+    print(f"\n  fine chain det={det}: " + ", ".join(f"{k} {v:.3g}" for k, v in worst.items()) +
+          f"; head (err / max) " + ", ".join(f"{k} {v:.2g}" for k, v in head.items()) +
+          f"; masked Gaussians {int(m.sum())}, widened sampler pairs {int(st['wide_pairs'].sum())}, band-excluded "
+          f"Gaussians {int(band.sum())} coarse, {int(bandf.sum())} fine")
+    _tightness("sampler g_points", st["g_points"])

@@ -17,7 +17,25 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 from helpers import rel_err  # noqa: E402
 from lara_b200.point_feats import sample_point_feats  # noqa: E402
-from test_point_feats import make_case, near_jump, point_feats_torch, restated_coords  # noqa: E402
+from test_point_feats import make_case, point_feats_torch  # noqa: E402
+
+
+def restated_coords(points, w2c, ixt, H, W):
+    """[V,n,2] grid_sample source coordinates (ix, iy) along the restatement's own chain of fp32 operations."""
+    cam = points.reshape(1, -1, 3) @ w2c[:, :3, :3].permute(0, 2, 1) + w2c[:, :3, 3][:, None]
+    cam = cam @ ixt.permute(0, 2, 1)
+    wh = torch.tensor([W, H], device=points.device)
+    g = (cam[..., :2] / cam[..., -1:] + 0.5) / wh * 2 - 1.0
+    return ((g + 1) * wh - 1) / 2
+
+
+def near_jump(coords, H, W, eps=1e-3):
+    """[V,n] bool: a coordinate of the point that reaches the image lies within eps px of a pixel-centre line, where
+    the point gradient jumps; the agreement of the point gradients is reported over the other points."""
+    size = torch.tensor([W, H], dtype=coords.dtype, device=coords.device)
+    c = coords.double()
+    reaches = torch.isfinite(c) & (c > -1 - eps) & (c < size + eps)
+    return (reaches & ((c - c.round()).abs() <= eps)).any(-1)
 
 
 def main():
