@@ -40,6 +40,11 @@ constexpr int kBwdWarps = 4;                  // warps per CTA: one CTA per 16x8
 constexpr int kBwdThreads = kBwdWarps * 32;
 constexpr int kBwdBatch = 128;                // splats staged per round, one per thread
 constexpr int kBwdCtasPerSM = 5;             // resident CTAs per SM that __launch_bounds__ sizes the registers for
+// The staged record of a splat, five float4 planes: the first three as in the geometry record (q0 q1 q2), then
+//   plane 3 = n.x n.y n.z r        plane 4 = g b splat-id (unused)
+// so that phase 1 reads the normal and colour it needs with one 16-byte and one 8-byte load instead of two 16-byte
+// ones.  The record's depth and clamp bits (q3.w, q4.w) and its cull octagon (q5) are not used here.
+constexpr int kBwdRecQuads = 5;
 
 __device__ __forceinline__ float rcp_fast(float x) {
     float r;
@@ -52,10 +57,22 @@ __device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float 
 }
 
 __device__ __forceinline__ void sts_f(uint32_t a, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(a), "f"(v) : "memory"); }
+__device__ __forceinline__ float2 lds_f2(uint32_t a) {
+    float2 v;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(a) : "memory");
+    return v;
+}
 __device__ __forceinline__ float lds_f(uint32_t a) {
     float v;
     asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a) : "memory");
     return v;
+}
+
+// (1 << n) - 1 for n in [0, 32], in one BMSK and without a constant in a register
+__device__ __forceinline__ uint32_t bits_below(int n) {
+    uint32_t m;
+    asm("bmsk.clamp.b32 %0, 0, %1;" : "=r"(m) : "r"(n));
+    return m;
 }
 
 __device__ __forceinline__ float ex2_fast(float x) {
@@ -103,8 +120,8 @@ __device__ __forceinline__ void eval_pair_bwd(const float4 q0, const float4 q1, 
 }
 
 struct BwdSmem {
-    static constexpr size_t rec = 0;                                                         // float4 [6][kBwdBatch]
-    static constexpr size_t x = rec + sizeof(float4) * SRF_REC_QUADS * kBwdBatch;            // float [warps][3][16][32]
+    static constexpr size_t rec = 0;                                                         // float4 [kBwdRecQuads][kBwdBatch]
+    static constexpr size_t x = rec + sizeof(float4) * kBwdRecQuads * kBwdBatch;             // float [warps][3][16][32]
     static constexpr size_t pixA = x + sizeof(float) * kBwdWarps * 3 * kBwdGroup * 32;       // float4 [threads] dn0 dn1 dn2 dpix0
     static constexpr size_t pixB = pixA + sizeof(float4) * kBwdThreads;                      // float4 [threads] dpix1 dpix2 pixel centre x y
     static constexpr size_t hm = pixB + sizeof(float4) * kBwdThreads;                        // u32 [warps][kBwdBatch]
@@ -255,22 +272,30 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
     for (int w = 0; w < kBwdWarps; ++w) n_eff = max(n_eff, s_wmax[w]);
     const int rounds = (n_eff + kBwdBatch - 1) / kBwdBatch;
 
-    // accum_rec / last_* recursions of backward.cu:331-385, two channels per f32x2 pair:
-    // (c0,c1) (c2,depth) (n0,n1) (n2,alpha); the matching upstream gradients are paired the same way
+    // accum_rec / last_* recursions of backward.cu:331-385.  Of the eight accum_rec channels (colour, depth, normal,
+    // alpha) dL_dalpha only ever needs sum_k (c_k - accum_rec_k) g_k, g_k the channel's upstream gradient, so the
+    // recursion is carried as the one scalar acc_g = sum_k accum_rec_k g_k:
+    //     sum_k (c_k - accum_rec_k) g_k = sum_k c_k g_k - acc_g,
+    //     accum_rec_k <- accum_rec_k + alpha (c_k - accum_rec_k)   gives   acc_g <- acc_g + alpha * (that sum)
     // (the reference keeps the previous splat in last_* and folds it in at the top of the next iteration;
     //  folding it in at the bottom of its own iteration is the same arithmetic and needs no such state)
-    f32x2 acc_c01 = zero2(), acc_c2d = zero2(), acc_n01 = zero2(), acc_n2a = zero2();
-    const f32x2 r_dpix01 = pk2(dpix0, dpix1), r_dpix2d = pk2(dpix2, dL_ddepth);
-    const f32x2 r_dn01 = pk2(dn0, dn1), r_dn2a = pk2(dn2, dL_daccum);
+    float acc_g = 0.f;
     float last_dL_dT = 0.f;
     const float nTfinal_bg = -T_final * bg_dot_dpixel;
     // the distortion terms of a pair with mapped depth m (backward.cu:350-368), per pixel constants folded in:
-    //   dL_dweight = (D2 + m^2 A - 2 m D) dL_dreg = m (m A_r + nD_r) + D2_r,
-    //   dL_dmd     = 2 w (m A - D) dL_dreg         = w (m A2_r + nD_r)
-    // (A_r = A dL_dreg, A2_r = 2 A_r, nD_r = -2 D dL_dreg, D2_r = D2 dL_dreg); dL_dmd * dm/dd = dL_dmd c2 / d^2 with the
-    // factor c2 = 20 / 99.8 taken into kA2_r, knD_r
-    const float A_r = final_A * dL_dreg, nD_r = -2.0f * final_D * dL_dreg, D2_r = final_D2 * dL_dreg;
-    const float kA2_r = (float)(2.0 * 20.0 / 99.8) * A_r, knD_r = (float)(20.0 / 99.8) * nD_r;
+    //   dL_dweight = (D2 + m^2 A - 2 m D) dL_dreg,   dL_dmd = 2 w (m A - D) dL_dreg,   dm/dd = c2 / d^2,
+    // with m = c1 - c2 r, r = 1/d (c1 = 100 / 99.8, c2 = 20 / 99.8).  As polynomials in r, with the per-pixel
+    // coefficients taken once here (in double, rounded once):
+    //   dL_dweight = (W2 r - Z0) r + W0,   dL_dmd * dm/dd = w (Z1 r + Z0) r^2
+    float W2, W0, Z1, Z0;
+    {
+        const double c1 = 100.0 / 99.8, c2 = 20.0 / 99.8;
+        const double Ar = (double)final_A * dL_dreg, nDr = -2.0 * (double)final_D * dL_dreg, D2r = (double)final_D2 * dL_dreg;
+        W2 = (float)(Ar * c2 * c2);
+        W0 = (float)((c1 * Ar + nDr) * c1 + D2r);
+        Z1 = (float)(-2.0 * c2 * c2 * Ar);
+        Z0 = (float)(c2 * (2.0 * c1 * Ar + nDr));
+    }
 
     // phase-2 identity of this lane: its candidate chunk size C = (lane & 15) + 1 and the multiplier that turns
     // n / C into a multiply ((n * M) >> 16 == n / C exactly while n * C < 65536; n <= 47, C <= 16 here)
@@ -305,9 +330,10 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
                 const uint32_t id = next_id;
                 const float4* r = a.rec + (size_t)id * SRF_REC_QUADS;
 #pragma unroll
-                for (int k = 0; k < SRF_REC_QUADS; ++k) s_rec[k][jt] = ldg4(r + k);
-                // the splat id rides in the (otherwise unused by the blend) clamp-bits word of q4
-                s_rec[4][jt].w = __uint_as_float(id);
+                for (int k = 0; k < 3; ++k) s_rec[k][jt] = ldg4(r + k);
+                const float4 q3 = ldg4(r + 3), q4 = ldg4(r + 4);
+                s_rec[3][jt] = make_float4(q3.x, q3.y, q3.z, q4.x);
+                s_rec[4][jt] = make_float4(q4.y, q4.z, __uint_as_float(id), 0.0f);
             }
         }
         const int npos = n_eff - 1 - ((b + 1) * kBwdBatch + tid);
@@ -330,7 +356,8 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
         }
         __syncwarp();
         // the batch slot of the pixel's median contributor: slot j holds list position n_eff - 1 - (b kBwdBatch + j)
-        const int j_median = n_eff - median_contributor - b * kBwdBatch;
+        int j_median = n_eff - median_contributor - b * kBwdBatch;
+        asm volatile("" : "+r"(j_median));               // kept in a register, not rebuilt at every phase-1 trip
 
         for (int g0 = 0; g0 < nh; g0 += 32) {
             // pixel mask of chunk entry g0 + lane (0 past the end of the list); the 32x32 bit transpose of the chunk's
@@ -370,65 +397,64 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
                 if (gbase >= nh) break;
 
                 // ================= phase 1: lane = pixel =================
-                uint32_t bits = (colword >> (sub * kBwdGroup)) & 0xffffu;
-                const int iters1 = (int)__reduce_max_sync(0xffffffffu, (unsigned)__popc(bits));
-                for (int it = 0; it < iters1; ++it) {
-                    if (bits == 0) continue;
-                    const int i = __ffs(bits) - 1;
-                    bits &= bits - 1;
-                    const int j = (int)lds_u8(sa_list + gbase + i);
+                // The lane's contributing entries of the group, bit-reversed: entry i is bit 31 - i, so the next one
+                // back to front is the highest set bit (one FLO) and dropping it keeps the bits below (BMSK, LOP3).
+                // Each lane loops over its own pairs and leaves when it has none left; the warp reconverges once,
+                // after the loop, not at every trip.
+                uint32_t rbits = __brev(colword >> (sub * kBwdGroup)) & 0xffff0000u;
+                const uint32_t sa_list_g = sa_list + (uint32_t)(gbase + 31);
+                while (rbits != 0u) {
+                    const int p = 31 - __clz(rbits);             // entry i = 31 - p of the group
+                    rbits &= bits_below(p);
+                    const int j = (int)lds_u8(sa_list_g - (uint32_t)p);
                     PairBwd e;
                     const uint32_t sa_j = sa_rec + 16u * j;
-                    eval_pair_bwd(lds_f4(sa_j), lds_f4(sa_j + 16u * kBwdBatch), lds_f4(sa_j + 32u * kBwdBatch), pixx, pixy, e);
+                    // all five loads go out before the pair evaluation, so that their latency overlaps it
+                    const float4 q0 = lds_f4(sa_j), q1 = lds_f4(sa_j + 16u * kBwdBatch), q2 = lds_f4(sa_j + 32u * kBwdBatch);
+                    const float4 q3 = lds_f4(sa_j + 48u * kBwdBatch);   // n.x n.y n.z r
+                    const float2 q4 = lds_f2(sa_j + 64u * kBwdBatch);   // g b
+                    eval_pair_bwd(q0, q1, q2, pixx, pixy, e);
                     const bool lowpass = e.lowpass;
-                    const float4 q3 = lds_f4(sa_j + 48u * kBwdBatch);
-                    const float4 q4 = lds_f4(sa_j + 64u * kBwdBatch);
                     const float alpha = e.alpha, c_d = e.depth;
 
                     // one reciprocal serves T / (1-alpha) and the background term's T_final / (1-alpha)
                     const float r1ma = rcp_fast(1.0f - alpha);   // 1 - alpha >= 0.01
                     T = T * r1ma;
                     const float w = alpha * T;
-                    const f32x2 cur_c01 = pk2(q4.x, q4.y), cur_c2d = pk2(q4.z, c_d);
-                    const f32x2 cur_n01 = pk2(q3.x, q3.y), cur_n2a = pk2(q3.z, 1.0f);
-                    // dL_dalpha += (channel - accum_rec) * dL_dchannel over colour, depth, normal, alpha
-                    const f32x2 d_c01 = sub2(cur_c01, acc_c01), d_c2d = sub2(cur_c2d, acc_c2d);
-                    const f32x2 d_n01 = sub2(cur_n01, acc_n01), d_n2a = sub2(cur_n2a, acc_n2a);
-                    f32x2 dsum = mul2(d_c01, r_dpix01);
-                    dsum = fma2(d_c2d, r_dpix2d, dsum);
-                    dsum = fma2(d_n01, r_dn01, dsum);
-                    dsum = fma2(d_n2a, r_dn2a, dsum);
-                    const float2 dsum_ = up2(dsum);
-                    // accum_rec <- alpha * channel + (1 - alpha) * accum_rec = accum_rec + alpha * (channel - accum_rec)
-                    // (all eight channels), for the next splat: one fma on the differences dL_dalpha already took
-                    const f32x2 la2 = bc2(alpha);
-                    acc_c01 = fma2(d_c01, la2, acc_c01);
-                    acc_c2d = fma2(d_c2d, la2, acc_c2d);
-                    acc_n01 = fma2(d_n01, la2, acc_n01);
-                    acc_n2a = fma2(d_n2a, la2, acc_n2a);
+                    // dL_dalpha += (channel - accum_rec) * dL_dchannel over colour, depth, normal, alpha (alpha's
+                    // channel value is 1), then accum_rec <- accum_rec + alpha * (channel - accum_rec), as acc_g
+                    float cg = fmaf(q3.w, dpix0, dL_daccum);
+                    cg = fmaf(q4.x, dpix1, cg);
+                    cg = fmaf(q4.y, dpix2, cg);
+                    cg = fmaf(q3.x, dn0, cg);
+                    cg = fmaf(q3.y, dn1, cg);
+                    cg = fmaf(q3.z, dn2, cg);
+                    cg = fmaf(c_d, dL_ddepth, cg);
+                    const float dsum = cg - acc_g;
+                    acc_g = fmaf(alpha, dsum, acc_g);
 
-                    float dL_dz = w * up2(r_dpix2d).y;
+                    float dL_dz = w * dL_ddepth;
                     // distortion / median terms (backward.cu:350-368).  m_d = (FAR d - FAR NEAR)/((FAR-NEAR) d)
                     // = c1 - c2/d and d m_d/dd = c2/d^2; the reference evaluates both in double.  fp32 is
                     // enough here: the weight term is stationary in m_d (its derivative is
                     // 2 (m_d A - D) ~ 0), and the gradients carry 1e-6 atomic-order noise anyway.
                     const float rcd = rcp_fast(c_d);             // depth >= 0.2
-                    const float m_d = fmaf(-(float)(20.0 / 99.8), rcd, (float)(100.0 / 99.8));
-                    float dL_dweight = fmaf(m_d, fmaf(m_d, A_r, nD_r), D2_r);
+                    float dL_dweight = fmaf(fmaf(W2, rcd, -Z0), rcd, W0);
                     if (j == j_median) {
                         dL_dz += dL_dmedian_depth;
                         dL_dweight += dL_dmax_dweight;
                     }
                     const float ddw = dL_dweight - last_dL_dT;
-                    float dL_dalpha = (dsum_.x + dsum_.y) + ddw;
+                    float dL_dalpha = dsum + ddw;
                     last_dL_dT = fmaf(alpha, ddw, last_dL_dT);   // dL_dweight * alpha + (1 - alpha) * last_dL_dT
-                    dL_dz = fmaf(w * fmaf(m_d, kA2_r, knD_r), rcd * rcd, dL_dz);   // += dL_dmd * dm_d/dd
+                    dL_dz = fmaf(w * fmaf(Z1, rcd, Z0), rcd * rcd, dL_dz);       // += dL_dmd * dm_d/dd
                     dL_dalpha *= T;
                     // background term (backward.cu:391-396)
                     dL_dalpha = fmaf(nTfinal_bg, r1ma, dL_dalpha);
 
                     // park the three scalars phase 2 needs; the sign of w carries the branch (w > 0 always)
-                    const uint32_t xa = sa_x + 4u * (uint32_t)(i * 32 + (lane ^ i));
+                    // at row i, column lane ^ i; with i = 31 - p that is word 31*32 + ((lane ^ 31) ^ p) - 32 p
+                    const uint32_t xa = sa_x + 4u * (31 * 32) + 4u * (uint32_t)(((lane ^ 31) ^ p) - 32 * p);
                     sts_f(xa, lowpass ? -w : w);
                     sts_f(xa + 4u * kBwdGroup * 32, e.G * dL_dalpha);
                     sts_f(xa + 8u * kBwdGroup * 32, dL_dz);
@@ -474,25 +500,27 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
                 if (mybits != 0) {
                     const uint32_t sa_j2 = sa_rec + 16u * lds_u8(sa_list + gbase + own);
                     const float4 q0 = lds_f4(sa_j2), q1 = lds_f4(sa_j2 + 16u * kBwdBatch), q2 = lds_f4(sa_j2 + 32u * kBwdBatch);
-                    const uint32_t splat_id = lds_u32(sa_j2 + 64u * kBwdBatch + 12u);
+                    const uint32_t splat_id = lds_u32(sa_j2 + 64u * kBwdBatch + 8u);
                     const f32x2 nTu_x = pk2(-q0.x, -q0.y), nTu_y = pk2(-q0.z, -q0.w), nTu_z = pk2(-q1.x, -q1.y);
                     const float Twx = q1.z, Twy = q1.w, Twz = q2.x;
                     const f32x2 Twxy = pk2(Twx, Twy), cen = pk2(q2.y, q2.z);
-                    const float nopac = -q2.w;
+                    const float nopac = -q2.w, n2opac = 2.0f * nopac;
                     // accumulators, laid out as the gradient record: (DT0,DT1) (DT2,DT3) (DT4,DT5) (DT6,DT7) (DT8,DOPAC)
                     // (DN0,DN1) (DN2,DC0) (DC1,DC2) (DM0,DM1)
                     f32x2 A0 = zero2(), A1 = zero2(), A2 = zero2(), A3 = zero2(), A4 = zero2(), A5 = zero2(), A6 = zero2(), A7 = zero2(), A8 = zero2();
                     const uint32_t sa_xrow = sa_x + 128u * (uint32_t)own;   // the splat's row of the X tile
                     // every lane walks its own contributing pixels, C of them (fewer in a splat's last lane); the warp makes
                     // max-over-lanes trips
+                    // (bit-reversed as in phase 1: pixel t is bit 31 - t, the next one is the highest set bit)
                     int n_take = min(C, __popc(mybits));
+                    uint32_t rbits = __brev(mybits);
                     do {
-                        const int t = __ffs(mybits) - 1;
-                        mybits &= mybits - 1;
-                        const uint32_t xa = sa_xrow + 4u * (uint32_t)(t ^ own);
+                        const int p = 31 - __clz(rbits);             // pixel t = 31 - p
+                        rbits &= bits_below(p);
+                        const uint32_t xa = sa_xrow + 4u * (uint32_t)((own ^ 31) ^ p);   // column t ^ own
                         const float ws = lds_f(xa), GdA = lds_f(xa + 4u * kBwdGroup * 32), dL_dz = lds_f(xa + 8u * kBwdGroup * 32);
-                        const float4 pa = lds_f4(sa_pixA + 16u * t);
-                        const float4 pb = lds_f4(sa_pixB + 16u * t);
+                        const float4 pa = lds_f4(sa_pixA + 16u * 31 - 16u * (uint32_t)p);
+                        const float4 pb = lds_f4(sa_pixB + 16u * 31 - 16u * (uint32_t)p);
                         const float ppx = pb.z, ppy = pb.w;
                         const float w = fabsf(ws);
                         const f32x2 w2 = bc2(w);
@@ -501,6 +529,7 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
                         fma2_acc(A7, w2, pk2(pb.x, pb.y));      // dL/dcolor.gb
                         const f32x2 pix2 = pk2(ppx, ppy);
                         A4.y = __fadd_rn(A4.y, GdA);            // dL/dopacity, both branches
+                        float tw8;                              // dL/dTw.z of the pair: A4.x's term in both branches
                         if (ws > 0.0f) {
                             // ray-splat branch: vjp through s = p.xy / p.z, p = k x l (backward.cu:405-435)
                             const float2 klx = up2(fma2(pix2, bc2(Twx), nTu_x));
@@ -528,14 +557,14 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
                             tw67 = fma2(bc2(ppx), pk2(Dx_.x, Dy_.x), tw67);
                             tw67 = fma2(bc2(-ppy), pk2(Dx_.y, Dy_.y), tw67);
                             add2_acc(A3, tw67);
-                            const float tw8 = fmaf(ppx, Dz_.x, fmaf(-ppy, Dz_.y, dL_dz));
-                            A4.x = __fadd_rn(A4.x, tw8);
+                            tw8 = fmaf(ppx, Dz_.x, fmaf(-ppy, Dz_.y, dL_dz));
                         } else {
                             // low-pass branch (backward.cu:436-443); FilterInvSquare == 2 after fp32 rounding
                             const f32x2 d = sub2(cen, pix2);
-                            fma2_acc(A8, d, bc2(2.0f * nopac * GdA));
-                            A4.x = __fadd_rn(A4.x, dL_dz);
+                            fma2_acc(A8, d, bc2(n2opac * GdA));
+                            tw8 = dL_dz;
                         }
+                        A4.x = __fadd_rn(A4.x, tw8);
                     } while (--n_take != 0);
                     // the lane's partial sums
                     const float2 a0 = up2(A0), a1 = up2(A1), a2 = up2(A2), a3 = up2(A3), a8 = up2(A8);

@@ -4,7 +4,8 @@
     python tools/sass_budget.py FILE.cubin      # or an existing cubin
     python tools/sass_budget.py FILE.sass       # or the text of `cuobjdump -sass`
 
-Prints the static instruction counts of the four parts of render_bwd_kernel that a group runs through:
+Prints the static instruction counts of the four parts of render_bwd_kernel<kEpiFloat> (the default epilogue; the
+deterministic instantiations in the same cubin are not counted) that a group runs through:
 
   phase-1 trip     the per-pixel pair loop (from its head to its back-branch), without the exact re-evaluation of
                    eval_pair_bwd (the smallest forward branch in the loop that jumps over every CALL of it: the IEEE
@@ -13,9 +14,9 @@ Prints the static instruction counts of the four parts of render_bwd_kernel that
   phase-2 trip     the phase-2 pixel loop, head to back-branch (both branches of the body: ray-splat and low-pass)
   partial sums     from the phase-2 back-branch to the last RED (red.global.add.v4.f32) of the kernel
 
-The ranges are found by their anchors -- the REDUX.MAX that starts phase 1 (the warp's trip count), the loops'
-back-branches and the REDs -- not by addresses, so the script keeps working when the code moves.  Counts are static
-(instructions in the range), not dynamic issue counts.
+The ranges are found by their anchors -- the phase-1 loop (the first loop whose body has a MUFU.EX2: the pair's
+exp), the loops' back-branches and the REDs -- not by addresses, so the script keeps working when the code moves.
+Counts are static (instructions in the range), not dynamic issue counts.
 """
 from __future__ import annotations
 
@@ -50,18 +51,22 @@ def sass_of(path: str | None) -> str:
 
 
 def kernel_insns(sass: str) -> list[tuple[int, str]]:
-    """(address, text) of every instruction of render_bwd_kernel."""
+    """(address, text) of every instruction of the default-epilogue render_bwd_kernel.
+
+    The cubin holds one instantiation of the kernel per epilogue (render_bwd_kernel<kEpi>); each starts its addresses
+    at 0, so only one of them may be read.  The one counted is kEpiFloat (= 0), the path every non-deterministic
+    backward runs: its mangled name carries the template argument as ILi0E."""
     out, inside = [], False
     for line in sass.splitlines():
         if "Function :" in line:
-            inside = KERNEL in line
+            inside = KERNEL + "ILi0E" in line
             continue
         if inside:
             m = _INSN.match(line)
             if m:
                 out.append((int(m.group(1), 16), m.group(2)))
     if not out:
-        raise SystemExit(f"no {KERNEL} in the SASS")
+        raise SystemExit(f"no {KERNEL}<kEpiFloat> in the SASS")
     return out
 
 
@@ -79,8 +84,17 @@ def budget(insns: list[tuple[int, str]]) -> dict[str, int]:
                     return tgt, i
         raise SystemExit("loop not found")
 
-    redux = next(i for i, (_, t) in enumerate(insns) if "REDUX.MAX" in t)
-    h1, b1 = back_branch_after(redux)
+    # phase 1: the first loop, by its back-branch, with a MUFU.EX2 in its body
+    h1 = b1 = -1
+    for i, (a, t) in enumerate(insns):
+        m = _BRA.search(t)
+        if m and int(m.group(1), 16) <= a:
+            head = idx[int(m.group(1), 16)]
+            if any("MUFU.EX2" in insns[k][1] for k in range(head, i)):
+                h1, b1 = head, i
+                break
+    if h1 < 0:
+        raise SystemExit("phase-1 loop not found")
     # the exact re-evaluation: the smallest forward branch of the loop that skips every CALL in it
     calls = [i for i in range(h1, b1 + 1) if "CALL" in insns[i][1]]
     exact = 0
@@ -101,12 +115,12 @@ def budget(insns: list[tuple[int, str]]) -> dict[str, int]:
     outer = []
     for i in range(last_red, len(insns)):
         m = _BRA.search(insns[i][1])
-        if m and int(m.group(1), 16) < insns[redux][0]:
+        if m and int(m.group(1), 16) < insns[h1][0]:
             outer.append((idx[int(m.group(1), 16)], i))
     (gh, gb), (ch, _) = outer[0], outer[1]
     return {
         "chunk set-up (per 32 entries)": gh - ch,
-        "group head (to REDUX.MAX)": redux - gh + 1,
+        "group head (to the phase-1 loop)": h1 - gh,
         "phase-1 trip (fast path)": (b1 - h1 + 1) - exact,
         "phase-1 exact re-evaluation": exact,
         "between phases": h2 - (b1 + 1),
