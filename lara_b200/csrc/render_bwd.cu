@@ -57,22 +57,10 @@ __device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float 
 }
 
 __device__ __forceinline__ void sts_f(uint32_t a, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(a), "f"(v) : "memory"); }
-__device__ __forceinline__ float2 lds_f2(uint32_t a) {
-    float2 v;
-    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(a) : "memory");
-    return v;
-}
 __device__ __forceinline__ float lds_f(uint32_t a) {
     float v;
     asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a) : "memory");
     return v;
-}
-
-// (1 << n) - 1 for n in [0, 32], in one BMSK and without a constant in a register
-__device__ __forceinline__ uint32_t bits_below(int n) {
-    uint32_t m;
-    asm("bmsk.clamp.b32 %0, 0, %1;" : "=r"(m) : "r"(n));
-    return m;
 }
 
 __device__ __forceinline__ float ex2_fast(float x) {

@@ -3,13 +3,14 @@
 //
 // One CTA (SRF_CTA_WARPS = 8 warps) per 16x16 tile, one thread per pixel (each warp owns an
 // 8x4 pixel block).  The tile's depth-sorted Gaussian list is consumed in rounds of SRF_BATCH
-// = 256: every thread gathers one 96 B GeomRecord with six 128-bit loads and stages it in
-// shared memory as six float4 planes, so the inner loop never touches global memory --
-// including the colour, which the reference fetches from global memory per contributing pixel.
-// Per round each warp builds per-pixel hit masks (the splat's conservative alpha >= 1/255
-// octagon rasterised over the warp's block, transposed across the warp) and every lane then
-// walks its own hits in list order, reading the records at per-lane indices (phases A / B
-// below).  Arithmetic and predicates follow the reference exactly (see eval_pair()).
+// = 256: every thread gathers one 96 B GeomRecord with six 128-bit loads, stages what the blend
+// reads in shared memory, so the inner loop never touches global memory -- including the colour,
+// which the reference fetches from global memory per contributing pixel -- and culls the splat
+// against the tile's eight 8x4 blocks once (one byte per batch slot).  Per round each warp then
+// builds per-pixel hit masks (the splat's conservative alpha >= 1/255 octagon rasterised over the
+// warp's block, transposed across the warp) and every lane walks its own hits in list order,
+// reading the records at per-lane indices (phases A / B below).  Arithmetic and predicates follow
+// the reference exactly (see eval_pair()).
 // Every warp also records, per list position, which pixels of its block the splat was blended into (one u32
 // per (position, 8x4 block), RenderFwdArgs::masks): the blend backward replays that record instead of culling,
 // masking and re-testing the pairs itself.
@@ -22,13 +23,25 @@
 
 namespace srf {
 
+// The staged record in shared memory, as phase B reads it: four float4 planes q0, q1, q2 and (n.x, n.y, n.z, r), the
+// colour's (g, b) as one float2 plane, and the cull octagon q5, which only the pixel masks read.  A contributing trip reads
+// normal and colour with one 16-byte and one 8-byte load; the view-space depth q3.w and the clamp bits q4.w, which the
+// blend never reads, are not staged.  Byte offsets of the planes:
+constexpr uint32_t kFwdQ3 = 16u * 3 * SRF_BATCH;          // (n.x, n.y, n.z, r)
+constexpr uint32_t kFwdGB = 16u * 4 * SRF_BATCH;          // (g, b)
+constexpr uint32_t kFwdOct = kFwdGB + 8u * SRF_BATCH;     // q5
+constexpr uint32_t kFwdRecBytes = kFwdOct + 16u * SRF_BATCH;
+
 template <bool kRecord>
 __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) render_fwd_kernel(RenderFwdArgs a) {
-    __shared__ float4 s_rec[SRF_REC_QUADS][SRF_BATCH];
+    __shared__ __align__(16) uint8_t s_rec[kFwdRecBytes];
+    __shared__ uint8_t s_blk[SRF_BATCH];                               // [batch slot]: bit b = may touch the tile's block b
     __shared__ uint32_t s_mask[SRF_CTA_WARPS][SRF_BATCH_CHUNKS][32];   // [warp][group of 32 hits][lane]: per-pixel hit words
     __shared__ uint8_t s_list[SRF_CTA_WARPS][SRF_BATCH];               // [warp]: batch slots of the splats that can touch the warp's block
     __shared__ __align__(16) uint32_t s_out[SRF_CTA_WARPS][SRF_BATCH];  // [warp][batch slot]: contribution masks of the batch
                                                                         // (not referenced, so not allocated, without kRecord)
+    float4* const s_q = reinterpret_cast<float4*>(s_rec);               // s_q[k * SRF_BATCH + slot]: float4 plane k
+    const float4* const s_q5 = reinterpret_cast<const float4*>(s_rec + kFwdOct);
 
     const int tid = threadIdx.x;
     {   // view of this CTA: per-view workspaces of identical layout, images stacked [V,C,H,W]
@@ -53,7 +66,7 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
     const int pxi = txi * SRF_TILE + lx, pyi = tyi * SRF_TILE + ly;
     const bool inside = pxi < a.W && pyi < a.H;
     const float pixx = (float)pxi + 0.5f, pixy = (float)pyi + 0.5f;
-    // pixel-centre rectangle of this warp's 8x4 block, for the warp-level cull
+    // pixel-centre rectangle of this warp's 8x4 block, for the pixel masks
     const int lane = tid & 31, wid = tid >> 5;
     const WarpRect wrect = make_warp_rect(txi, tyi, gw);
 
@@ -64,7 +77,7 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
 
     bool done = !inside;
     float T = 1.0f;
-    uint32_t contributor = 0, last_contributor = 0;
+    uint32_t last_contributor = 0;
     // accumulators, two per f32x2 pair: (C0,C1) (C2,distortion) (N0,N1) (N2,D) (dist1,dist2)
     f32x2 C01 = zero2(), C2r = zero2(), N01 = zero2(), N2D = zero2(), d12 = zero2();
     float median_depth = 0.f, median_weight = 0.f;
@@ -75,7 +88,7 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
 
     // phase B addresses its shared arrays explicitly (smem_addr): the staged records, the warp's hit list and the lane's
     // hit words
-    uint32_t sa_rec = smem_addr(&s_rec[0][0]), sa_list = smem_addr(&s_list[wid][0]), sa_mask = smem_addr(&s_mask[wid][0][lane]);
+    uint32_t sa_rec = smem_addr(s_rec), sa_list = smem_addr(&s_list[wid][0]), sa_mask = smem_addr(&s_mask[wid][0][lane]);
     asm volatile("" : "+r"(sa_rec), "+r"(sa_list), "+r"(sa_mask));   // opaque: kept in registers, not rebuilt at every use
     // ptxas still rematerialises the record base (S2R SR_CgaCtaId + LEA) at both of its uses in the pair loop; a shuffled
     // copy is a value it cannot recompute
@@ -85,23 +98,38 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
     for (int b = 0; b < rounds; ++b, todo -= SRF_BATCH) {
         // whole tile saturated -> stop (reference forward.cu:334-336)
         if (__syncthreads_count(done) == SRF_CTA_THREADS) break;
+        // ---- staging and the cull: the thread of batch slot tid stages its splat and tests the splat's conservative
+        // alpha >= 1/255 octagon against all eight 8x4 blocks of the tile (octagon_block_bits: bit b is exactly
+        // octagon_hits against block b), so each staged splat is culled once for the whole tile.  Slots past the list's
+        // end get no bits.
         const int progress = b * SRF_BATCH + tid;
+        uint32_t blk = 0;
         if (progress < n) {
             const uint32_t id = __ldg(a.point_list + range.x + progress);
             const float4* r = a.rec + (size_t)id * SRF_REC_QUADS;
-#pragma unroll
-            for (int k = 0; k < SRF_REC_QUADS; ++k) s_rec[k][tid] = ldg4(r + k);
+            const float4 q2 = ldg4(r + 2), q3 = ldg4(r + 3), q4 = ldg4(r + 4), q5 = ldg4(r + 5);
+            s_q[0 * SRF_BATCH + tid] = ldg4(r + 0);
+            s_q[1 * SRF_BATCH + tid] = ldg4(r + 1);
+            s_q[2 * SRF_BATCH + tid] = q2;
+            s_q[3 * SRF_BATCH + tid] = make_float4(q3.x, q3.y, q3.z, q4.x);
+            reinterpret_cast<float2*>(s_rec + kFwdGB)[tid] = make_float2(q4.y, q4.z);
+            reinterpret_cast<float4*>(s_rec + kFwdOct)[tid] = q5;
+            // the tile's block bounds are rebuilt here per batch: hoisted out of the batch loop, their 44 floats
+            // do not fit in the registers
+            int tx = txi, ty = tyi;
+            asm volatile("" : "+r"(tx), "+r"(ty));
+            blk = octagon_block_bits(q2, q5, tx, ty);
         }
+        s_blk[tid] = (uint8_t)blk;
         __syncthreads();
         const int cnt = min(SRF_BATCH, todo);
         // warp-uniform skip: a fully saturated warp only helps with staging
         if (__all_sync(0xffffffffu, done)) continue;
-        // ---- phase A: per-pixel hit masks.  First a warp-level cull: the staged splats whose conservative
-        // alpha >= 1/255 octagon can touch this warp's 8x4 block at all (~1 in 5) are compacted into a list, in list
-        // order.  Then, 32 hits at a time, lane l rasterises the octagon of hit g*32+l over the block into a 32-bit
-        // mask (bit = lane that owns the pixel) and a 32x32 bit transpose over the warp hands every lane the word
-        // "which of these 32 splats can touch MY pixel".  A splat outside a pixel's word cannot reach
-        // alpha >= 1/255 there, so skipping it changes no result.
+        // ---- phase A: per-pixel hit masks.  The staged splats whose octagon can touch this warp's 8x4 block at all
+        // (~1 in 5: bit gw of their block byte) are compacted into a list, in list order.  Then, 32 hits at a time, lane
+        // l rasterises the octagon of hit g*32+l over the block into a 32-bit mask (bit = lane that owns the pixel) and a
+        // 32x32 bit transpose over the warp hands every lane the word "which of these 32 splats can touch MY pixel".  A
+        // splat outside a pixel's word cannot reach alpha >= 1/255 there, so skipping it changes no result.
         static_assert(SRF_BATCH == 256, "s_out is cleared with two 16-byte stores per lane");
         if constexpr (kRecord) {
             reinterpret_cast<uint4*>(s_out[wid])[lane] = make_uint4(0u, 0u, 0u, 0u);
@@ -110,7 +138,7 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
         int nh = 0;
         for (int c0 = 0; c0 < cnt; c0 += 32) {
             const int jt = c0 + lane;
-            const bool hit = (jt < cnt) && octagon_hits(s_rec[2][jt], s_rec[5][jt], wrect);
+            const bool hit = (s_blk[jt] >> gw) & 1u;   // 0 for slots at or past cnt
             const unsigned hits = __ballot_sync(0xffffffffu, hit);
             if (hit) s_list[wid][nh + __popc(hits & ((1u << lane) - 1u))] = (uint8_t)jt;
             nh += __popc(hits);
@@ -122,16 +150,18 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
             uint32_t m = 0;
             if (h < nh) {
                 const int jt = s_list[wid][h];
-                m = octagon_pixel_mask(s_rec[2][jt], s_rec[5][jt], wrect);
+                m = octagon_pixel_mask(s_q[2 * SRF_BATCH + jt], s_q5[jt], wrect);
             }
             s_mask[wid][c][lane] = transpose32(m, lane);
         }
         __syncwarp();
 
-        // ---- phase B: every lane walks its own hits in list order.  The warp iterates max-over-lanes
-        // times instead of once per splat that touches the block anywhere (lane utilisation there was ~30 %).
-        // Each lane also records which of its hits it blended: cw collects the bits of chunk c and replaces the
-        // lane's (already read) hit word s_mask[wid][c][lane] when the lane leaves the chunk.
+        // ---- phase B: every lane walks its own hits in list order and leaves the loop when it has none left; the warp
+        // reconverges once, after the loop.  The lane's hit word is bit-reversed: hit i of the chunk is bit 31 - i, the
+        // next one is the highest set bit p (hit 31 - p), and w & bits_below(p) drops it.
+        // Each lane also records which of its hits it blended: cw collects the (bit-reversed) bits of chunk c and replaces
+        // the lane's (already read) hit word s_mask[wid][c][lane], in list order again, when the lane leaves the chunk.
+        const uint32_t cbase = (uint32_t)(b * SRF_BATCH + 1);   // contributor = cbase + batch slot (1-based list position)
         int c = 0;
         uint32_t w = 0, cw = 0;
         if (done) {
@@ -139,38 +169,37 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
                 for (int k = 0; k < nchunks; ++k) sts_u32(sa_mask + 128u * k, 0u);
             c = nchunks;
         } else if (nchunks > 0) {
-            w = lds_u32(sa_mask);
+            w = __brev(lds_u32(sa_mask));
         }
+        uint32_t sa_lc = sa_list + 31u;   // hit 31 - p of chunk c is list entry sa_lc - p
         for (;;) {
             while (w == 0 && c < nchunks - 1) {
-                if constexpr (kRecord) { sts_u32(sa_mask + 128u * c, cw); cw = 0; }
-                ++c; w = lds_u32(sa_mask + 128u * c);
+                if constexpr (kRecord) { sts_u32(sa_mask + 128u * c, __brev(cw)); cw = 0; }
+                ++c; sa_lc += 32u; w = __brev(lds_u32(sa_mask + 128u * c));
             }
-            const bool active = (w != 0);
-            if (!__any_sync(0xffffffffu, active)) break;
-            if (!active) continue;
-            const int i = __ffs(w) - 1;
-            const int j = (int)lds_u8(sa_list + (c << 5) + i);
+            if (w == 0) break;
+            const int p = 31 - __clz(w);
+            w &= bits_below(p);
+            const uint32_t j = lds_u8(sa_lc - (uint32_t)p);
             const uint32_t sa_j = sa_rec + 16u * j;
-            w &= w - 1;
-            contributor = (uint32_t)(b * SRF_BATCH + j + 1);
+            const float4 q0 = lds_f4(sa_j), q1 = lds_f4(sa_j + 16u * SRF_BATCH), q2 = lds_f4(sa_j + 32u * SRF_BATCH);
+            const float4 q3 = lds_f4(sa_j + kFwdQ3);
+            const float2 gb = lds_f2(sa_rec + kFwdGB + 8u * j);
             PairEval e;
-            eval_pair(lds_f4(sa_j), lds_f4(sa_j + 16u * SRF_BATCH), lds_f4(sa_j + 32u * SRF_BATCH), pixx, pixy, e);
+            eval_pair(q0, q1, q2, pixx, pixy, e);
             if (!e.valid) continue;
             const float alpha = e.alpha;
             const float test_T = fmul_(T, fadd_(1.0f, -alpha));
             if (!(test_T >= 0.0001f)) {
                 done = true;
                 if constexpr (kRecord) {
-                    sts_u32(sa_mask + 128u * c, cw);
+                    sts_u32(sa_mask + 128u * c, __brev(cw));
                     for (int k = c + 1; k < nchunks; ++k) sts_u32(sa_mask + 128u * k, 0u);
                 }
-                w = 0; c = nchunks;
-                continue;
+                c = nchunks;
+                break;
             }
-            if constexpr (kRecord) cw |= 1u << i;
-            const float4 q3 = lds_f4(sa_j + 48u * SRF_BATCH);
-            const float4 q4 = lds_f4(sa_j + 64u * SRF_BATCH);
+            if constexpr (kRecord) cw |= 1u << p;
             const float depth = e.depth;
             const float A = fadd_(1.0f, -T);
             const float m = mapped_depth_fast(depth);
@@ -180,22 +209,22 @@ __global__ void __launch_bounds__(SRF_CTA_THREADS, 1024 / SRF_CTA_THREADS) rende
             if (T > 0.5f) {
                 median_depth = depth;
                 median_weight = fmul_(T, alpha);
-                median_contributor = contributor;
+                median_contributor = cbase + j;
             }
             // every channel: acc = fma(T, channel * alpha, acc) -- the reference's rounding sequence,
             // two channels per mul2 / fma2 pair
             const f32x2 a2 = bc2(alpha), T2 = bc2(T);
-            fma2_acc(C01, T2, mul2(pk2(q4.x, q4.y), a2));
-            fma2_acc(C2r, T2, mul2(pk2(q4.z, err), a2));
+            fma2_acc(C01, T2, mul2(pk2(q3.w, gb.x), a2));
+            fma2_acc(C2r, T2, mul2(pk2(gb.y, err), a2));
             fma2_acc(N01, T2, mul2(pk2(q3.x, q3.y), a2));
             fma2_acc(N2D, T2, mul2(pk2(q3.z, depth), a2));
             fma2_acc(d12, T2, mul2(pk2(m, mm), a2));
             T = test_T;
-            last_contributor = contributor;
+            last_contributor = cbase + j;
         }
         // without the record, the next batch's __syncthreads_count orders the reuse of the warp's shared arrays
         if constexpr (kRecord) {
-            if (c < nchunks) sts_u32(sa_mask + 128u * c, cw);
+            if (c < nchunks) sts_u32(sa_mask + 128u * c, __brev(cw));
             __syncwarp();
 
             // ---- contribution record of the batch: transposed back, lane l holds the pixel mask of hit 32 k + l, which

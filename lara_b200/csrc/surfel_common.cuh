@@ -22,6 +22,7 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
 
 #define SRF_TILE 16
 #define SRF_TILE_PIX 256
@@ -216,7 +217,20 @@ __device__ __forceinline__ uint32_t lds_u32(uint32_t a) {
     asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
     return v;
 }
+__device__ __forceinline__ float2 lds_f2(uint32_t a) {
+    float2 v;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(a) : "memory");
+    return v;
+}
 __device__ __forceinline__ void sts_u32(uint32_t a, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
+
+// (1 << n) - 1 for n in [0, 32], in one BMSK and without a constant in a register.  The blend loops walk bit-reversed
+// words: the next entry is the highest set bit p = 31 - clz, and w & bits_below(p) drops it.
+__device__ __forceinline__ uint32_t bits_below(int n) {
+    uint32_t m;
+    asm("bmsk.clamp.b32 %0, 0, %1;" : "=r"(m) : "r"(n));
+    return m;
+}
 
 // pixel owned by thread `tid` of a 256-thread tile CTA: each warp covers an 8x4 block.
 __device__ __forceinline__ void tile_pixel(int tid, int& lx, int& ly) {
@@ -242,7 +256,7 @@ __device__ __forceinline__ float act_quat_norm(float4 q) {
 struct WarpRect {
     float xmin, xmax, ymin, ymax, umin, umax, vmin, vmax;
 };
-__device__ __forceinline__ WarpRect make_warp_rect(int tile_x, int tile_y, int wid) {
+__host__ __device__ __forceinline__ WarpRect make_warp_rect(int tile_x, int tile_y, int wid) {
     WarpRect w;
     w.xmin = (float)(tile_x * SRF_TILE + ((wid & 1) << 3)) + 0.5f; w.xmax = w.xmin + 7.0f;
     w.ymin = (float)(tile_y * SRF_TILE + ((wid >> 1) << 2)) + 0.5f; w.ymax = w.ymin + 3.0f;
@@ -259,18 +273,55 @@ __device__ __forceinline__ WarpRect warp_rect_at(float xmin, float ymin) {
     w.vmin = w.xmin - w.ymax; w.vmax = w.xmax - w.ymin;
     return w;
 }
-// true if the splat's conservative octagon (q5, centred at q2.yz) may touch the warp's block
-__device__ __forceinline__ bool octagon_hits(const float4 q2, const float4 q5, const WarpRect& w) {
+// The two fp16 offsets packed in one float of q5, as floats (host and device)
+__host__ __device__ __forceinline__ float2 unpack_half2(float f) {
+    __half2 h;
+    memcpy(&h, &f, sizeof(h));
+    return __half22float2(h);
+}
+// true if the splat's conservative octagon (q5, centred at q2.yz) may touch the warp's block (the blend forward culls
+// with octagon_block_bits, which is this test for all eight blocks of a tile; this form is kept as its definition)
+__host__ __device__ __forceinline__ bool octagon_hits(const float4 q2, const float4 q5, const WarpRect& w) {
     const float cx = q2.y, cy = q2.z;
-    const unsigned ux = __float_as_uint(q5.x), uy = __float_as_uint(q5.y), uu = __float_as_uint(q5.z), uv = __float_as_uint(q5.w);
-    const float2 ex = __half22float2(*reinterpret_cast<const __half2*>(&ux));
-    const float2 ey = __half22float2(*reinterpret_cast<const __half2*>(&uy));
-    const float2 eu = __half22float2(*reinterpret_cast<const __half2*>(&uu));
-    const float2 ev = __half22float2(*reinterpret_cast<const __half2*>(&uv));
+    const float2 ex = unpack_half2(q5.x), ey = unpack_half2(q5.y), eu = unpack_half2(q5.z), ev = unpack_half2(q5.w);
     const float cu = cx + cy, cv = cx - cy;
     const bool out = (cx + ex.x > w.xmax) || (cx + ex.y < w.xmin) || (cy + ey.x > w.ymax) || (cy + ey.y < w.ymin) ||
                      (cu + eu.x > w.umax) || (cu + eu.y < w.umin) || (cv + ev.x > w.vmax) || (cv + ev.y < w.vmin);
     return !out;
+}
+
+// octagon_hits() against all eight 8x4 blocks of tile (tile_x, tile_y) at once: bit b is
+// octagon_hits(q2, q5, make_warp_rect(tile_x, tile_y, b)), with the same float operations and comparisons, so the bits
+// are exactly that test's.  The x bounds depend only on the block's column (b & 1), the y bounds only on its row (b >> 1),
+// and the offsets of the splat's octagon are decoded once for all eight blocks.  The blend forward runs it once per
+// staged splat, in the thread that staged it.
+__host__ __device__ __forceinline__ uint32_t octagon_block_bits(const float4 q2, const float4 q5, int tile_x, int tile_y) {
+    const float cx = q2.y, cy = q2.z;
+    const float2 ex = unpack_half2(q5.x), ey = unpack_half2(q5.y), eu = unpack_half2(q5.z), ev = unpack_half2(q5.w);
+    const float cu = cx + cy, cv = cx - cy;
+    const float xlo = cx + ex.x, xhi = cx + ex.y, ylo = cy + ey.x, yhi = cy + ey.y;
+    const float ulo = cu + eu.x, uhi = cu + eu.y, vlo = cv + ev.x, vhi = cv + ev.y;
+    float xmin[2], xmax[2];
+    bool xin[2];
+#pragma unroll
+    for (int col = 0; col < 2; ++col) {
+        xmin[col] = (float)(tile_x * SRF_TILE + (col << 3)) + 0.5f; xmax[col] = xmin[col] + 7.0f;
+        xin[col] = !(xlo > xmax[col]) && !(xhi < xmin[col]);
+    }
+    uint32_t bits = 0;
+#pragma unroll
+    for (int row = 0; row < 4; ++row) {
+        const float ymin = (float)(tile_y * SRF_TILE + (row << 2)) + 0.5f, ymax = ymin + 3.0f;
+        const bool yin = !(ylo > ymax) && !(yhi < ymin);
+#pragma unroll
+        for (int col = 0; col < 2; ++col) {
+            const float umin = xmin[col] + ymin, umax = xmax[col] + ymax;
+            const float vmin = xmin[col] - ymax, vmax = xmax[col] - ymin;
+            const bool in = xin[col] && yin && !(ulo > umax) && !(uhi < umin) && !(vlo > vmax) && !(vhi < vmin);
+            bits |= (uint32_t)in << (2 * row + col);
+        }
+    }
+    return bits;
 }
 
 // Which pixels of the warp's 8x4 block (bit = lane owning the pixel, tile_pixel()) can the splat's

@@ -17,6 +17,26 @@ deterministic instantiations in the same cubin are not counted) that a group run
 The ranges are found by their anchors -- the phase-1 loop (the first loop whose body has a MUFU.EX2: the pair's
 exp), the loops' back-branches and the REDs -- not by addresses, so the script keeps working when the code moves.
 Counts are static (instructions in the range), not dynamic issue counts.
+
+    python tools/sass_budget.py --fwd [FILE]    # the blend forward: lara_b200/csrc/render_fwd.cu
+
+counts render_fwd_kernel<true> (the training instantiation, with the contribution record) by the same kind of anchors:
+
+  staging             from the batch's __syncthreads_count (BAR.RED.POPC) to the barrier after staging (BAR.SYNC):
+                      the gathers, the shared stores and, since the cull moved there, the per-tile octagon test
+  cull, per 32 slots  the warp's compaction loop after that barrier (the loop with a VOTE.ANY), per ballot: its body
+                      over the ballots ptxas unrolled into it
+  batch set-up        the rest up to the pixel-mask loop (s_out clearing, loop control)
+  phase A, per chunk  the pixel-mask loop (the loop with an F2I: the mask's row bounds), head to back-branch
+  trip: loop head     the pair loop (the first loop after phase A whose body has a MUFU.EX2) from its head to its
+                      first LDS.U8 (the hit's list entry)
+  trip: body          from there to the back-branch: a contributing trip's fast path
+  chunk advance       the spans of the pair loop that a trip inside a chunk branches over and that hold a shared store
+                      (the write-back of a finished chunk's blended bits): once per 32 hits
+  exact paths         the spans that hold a CALL or a double-precision instruction (the IEEE divisions' slow paths and
+                      mapped_depth's DP sequence, which runs only where the fp32 estimate cannot settle the rounding)
+  record, per batch   from the pair loop's back-branch to the batch loop's back-branch: the saturation exit, the
+                      transposes back, the scatter into s_out and the stores
 """
 from __future__ import annotations
 
@@ -29,8 +49,11 @@ import tempfile
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CUDA = os.environ.get("CUDA_HOME", "/usr/local/cuda")
 KERNEL = "render_bwd_kernel"
+SOURCE = "render_bwd.cu"
+INSTANTIATION = "ILi0E"   # the default epilogue, kEpiFloat
 
 _INSN = re.compile(r"^\s*/\*([0-9a-f]{4,})\*/\s+(.*?)\s*;")
+_F64 = re.compile(r"\bD(?:FMA|MUL|ADD)\b|F64|RCP64H")
 _BRA = re.compile(r"\bBRA\b(?:\s+!?U?P\d,)?\s+0x([0-9a-f]+)")
 
 
@@ -41,11 +64,11 @@ def sass_of(path: str | None) -> str:
     with tempfile.TemporaryDirectory() as tmp:
         cubin = path
         if cubin is None:
-            cubin = os.path.join(tmp, "render_bwd.cubin")
+            cubin = os.path.join(tmp, "kernel.cubin")
             csrc = os.path.join(ROOT, "lara_b200", "csrc")
             subprocess.run([os.path.join(CUDA, "bin", "nvcc"), "-gencode", "arch=compute_90a,code=sm_90a", "-O3",
                             "-std=c++17", "-I", csrc, "-I", os.path.join(ROOT, "include"), "-cubin", "-o", cubin,
-                            os.path.join(csrc, "render_bwd.cu")], check=True)
+                            os.path.join(csrc, SOURCE)], check=True)
         return subprocess.run([os.path.join(CUDA, "bin", "cuobjdump"), "-sass", cubin], check=True,
                               capture_output=True, text=True).stdout
 
@@ -59,14 +82,14 @@ def kernel_insns(sass: str) -> list[tuple[int, str]]:
     out, inside = [], False
     for line in sass.splitlines():
         if "Function :" in line:
-            inside = KERNEL + "ILi0E" in line
+            inside = KERNEL + INSTANTIATION in line
             continue
         if inside:
             m = _INSN.match(line)
             if m:
                 out.append((int(m.group(1), 16), m.group(2)))
     if not out:
-        raise SystemExit(f"no {KERNEL}<kEpiFloat> in the SASS")
+        raise SystemExit(f"no {KERNEL} {INSTANTIATION} in the SASS")
     return out
 
 
@@ -131,10 +154,73 @@ def budget(insns: list[tuple[int, str]]) -> dict[str, int]:
     }
 
 
+def _is_back(insn: tuple[int, str]) -> int | None:
+    m = _BRA.search(insn[1])
+    return int(m.group(1), 16) if m and int(m.group(1), 16) <= insn[0] else None
+
+
+def fwd_budget(insns: list[tuple[int, str]]) -> dict[str, int]:
+    addr = [a for a, _ in insns]
+    idx = {a: i for i, a in enumerate(addr)}
+
+    def loop_with(anchor: str, i0: int) -> tuple[int, int]:
+        """(head, back-branch) of the first loop after index i0 whose body holds `anchor`."""
+        for i in range(i0, len(insns)):
+            t = _is_back(insns[i])
+            if t is not None and idx[t] >= i0 and any(anchor in insns[k][1] for k in range(idx[t], i)):
+                return idx[t], i
+        raise SystemExit(f"no loop with {anchor} after {i0}")
+
+    def spans(h: int, b: int, inner: list[int]) -> set[int]:
+        """Indices inside the smallest forward branch of [h, b] that jumps over each index of `inner`."""
+        out: set[int] = set()
+        for k in inner:
+            best = None
+            for i in range(h, k):
+                m = _BRA.search(insns[i][1])
+                if m and int(m.group(1), 16) > insns[i][0]:
+                    tgt = idx[int(m.group(1), 16)]
+                    if tgt > k and tgt <= b and (best is None or tgt - i < best[1] - best[0]):
+                        best = (i, tgt)
+            if best:
+                out.update(range(best[0] + 1, best[1]))
+        return out
+
+    bh = next(i for i, (_, t) in enumerate(insns) if "BAR.RED.POPC" in t)
+    bs = next(i for i in range(bh, len(insns)) if "BAR.SYNC" in insns[i][1])
+    mh, mb = loop_with("F2I", bs)
+    ch, cb = loop_with("VOTE.ANY", bs)
+    ballots = sum(1 for k in range(ch, cb) if "VOTE.ANY" in insns[k][1])
+    ph, pb = loop_with("MUFU.EX2", mb)
+    exact = spans(ph, pb, [i for i in range(ph, pb) if "CALL" in insns[i][1] or _F64.search(insns[i][1])])
+    advance = spans(ph, pb, [i for i in range(ph, pb) if insns[i][1].lstrip("@!P0123456789 ").startswith("STS")]) - exact
+    lu8 = next(i for i in range(ph, pb) if "LDS.U8" in insns[i][1])
+    rare = exact | advance
+    batch_end = next(i for i in range(pb + 1, len(insns)) if (t := _is_back(insns[i])) is not None and idx[t] <= bh)
+    return {
+        "staging (per batch)": bs - bh + 1,
+        "cull, per 32 slots": round((cb - ch + 1) / max(ballots, 1)),
+        "batch set-up (rest, to phase A)": (mh - bs - 1) - (cb - ch + 1),
+        "phase A, per chunk": mb - mh + 1,
+        "trip: loop head": sum(1 for i in range(ph, lu8) if i not in rare),
+        "trip: body (fast path)": sum(1 for i in range(lu8, pb + 1) if i not in rare),
+        "chunk advance (per 32 hits)": len(advance),
+        "exact paths": len(exact),
+        "record (per batch)": batch_end - pb,
+    }
+
+
 def main() -> None:
-    path = sys.argv[1] if len(sys.argv) > 1 else None
-    for k, v in budget(kernel_insns(sass_of(path))).items():
-        print(f"{k:30s} {v:5d}")
+    args = sys.argv[1:]
+    fwd = "--fwd" in args
+    args = [a for a in args if a != "--fwd"]
+    path = args[0] if args else None
+    if fwd:
+        global KERNEL, SOURCE, INSTANTIATION
+        KERNEL, SOURCE, INSTANTIATION = "render_fwd_kernel", "render_fwd.cu", "ILb1E"
+    res = fwd_budget(kernel_insns(sass_of(path))) if fwd else budget(kernel_insns(sass_of(path)))
+    for k, v in res.items():
+        print(f"{k:34s} {v:5d}")
 
 
 if __name__ == "__main__":
