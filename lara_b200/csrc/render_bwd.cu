@@ -25,8 +25,9 @@
 //            sums go out as 4 (5) red.global.add.v4.f32 per lane.
 // Phase 1 evaluates pairs with MUFU.RCP / MUFU.EX2 and re-evaluates with the forward's exact sequence only within a
 // narrow band around rho3d = rho2d (eval_pair_bwd below); which pairs were blended it takes from the record.
-// What is kept from round 1: tiles in LPT order (one 4-warp CTA per 16x8 half tile, five per SM), the list walked back
-// to front from the tile's deepest used entry in staged rounds, paired fp32 arithmetic, MUFU.RCP.
+// Each warp walks its own block's entries of the tile list back to front from its own deepest contributor, gathers their
+// records into its own ring and meets the CTA's other warps at no barrier.  What is kept from round 1: tiles in LPT
+// order (one 4-warp CTA per 16x8 half tile, five per SM), paired fp32 arithmetic, MUFU.RCP.
 #include "det_sum.cuh"
 #include "surfel_common.cuh"
 #include "surfel_kernels.h"
@@ -38,7 +39,9 @@ namespace {
 constexpr int kBwdGroup = 16;                 // splats per phase-1 / phase-2 group (X tile = 16 splats x 32 pixels)
 constexpr int kBwdWarps = 4;                  // warps per CTA: one CTA per 16x8 half tile, two CTAs walk a tile's list
 constexpr int kBwdThreads = kBwdWarps * 32;
-constexpr int kBwdBatch = 128;                // splats staged per round, one per thread
+constexpr int kBwdWindow = 128;               // list positions a warp reads masks of per step of its walk, 4 per lane
+constexpr int kBwdChunk = 32;                 // compacted entries per chunk: two groups, one record gather
+constexpr int kBwdQueue = kBwdChunk - 1 + kBwdWindow;   // a step's new entries behind those carried from the last
 constexpr int kBwdCtasPerSM = 5;             // resident CTAs per SM that __launch_bounds__ sizes the registers for
 // The staged record of a splat, five float4 planes: the first three as in the geometry record (q0 q1 q2), then
 //   plane 3 = n.x n.y n.z r        plane 4 = g b splat-id (unused)
@@ -107,15 +110,15 @@ __device__ __forceinline__ void eval_pair_bwd(const float4 q0, const float4 q1, 
     }
 }
 
+// Every region is per warp: after the prologue the warps share nothing and meet at no barrier.
 struct BwdSmem {
-    static constexpr size_t rec = 0;                                                         // float4 [kBwdRecQuads][kBwdBatch]
-    static constexpr size_t x = rec + sizeof(float4) * kBwdRecQuads * kBwdBatch;             // float [warps][3][16][32]
+    static constexpr size_t rec = 0;                                                         // float4 [warps][kBwdRecQuads][kBwdChunk]
+    static constexpr size_t x = rec + sizeof(float4) * kBwdWarps * kBwdRecQuads * kBwdChunk; // float [warps][3][16][32]
     static constexpr size_t pixA = x + sizeof(float) * kBwdWarps * 3 * kBwdGroup * 32;       // float4 [threads] dn0 dn1 dn2 dpix0
     static constexpr size_t pixB = pixA + sizeof(float4) * kBwdThreads;                      // float4 [threads] dpix1 dpix2 pixel centre x y
-    static constexpr size_t hm = pixB + sizeof(float4) * kBwdThreads;                        // u32 [warps][kBwdBatch]
-    static constexpr size_t list = hm + sizeof(uint32_t) * kBwdWarps * kBwdBatch;            // uint8 [warps][kBwdBatch]
-    static constexpr size_t wmax = list + (size_t)kBwdWarps * kBwdBatch;                     // int [warps]
-    static constexpr size_t total = wmax + sizeof(int) * kBwdWarps;
+    static constexpr size_t qmask = pixB + sizeof(float4) * kBwdThreads;                     // u32 [warps][kBwdQueue + 1]
+    static constexpr size_t qpos = qmask + sizeof(uint32_t) * kBwdWarps * (kBwdQueue + 1);   // int [warps][kBwdQueue + 1]
+    static constexpr size_t total = qpos + sizeof(int) * kBwdWarps * (kBwdQueue + 1);
 };
 
 // What phase 2 does with a lane's 18 partial sums (its epilogue).  kEpiFloat is the default path: red.add into the fp32
@@ -171,22 +174,22 @@ __device__ __forceinline__ void det_epilogue(DetRecord* r, const float (&v)[18])
 
 template <int kEpi>
 __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(RenderBwdArgs a) {
-    static_assert(kBwdBatch <= 256, "hit lists are uint8");
-    static_assert(kBwdBatch == kBwdThreads, "every thread stages one list entry per round");
+    static_assert(kBwdWindow == 4 * 32, "a walk step reads four mask words per lane");
     extern __shared__ __align__(16) unsigned char smem[];
     typedef BwdSmem L;
-    float4 (*s_rec)[kBwdBatch] = reinterpret_cast<float4 (*)[kBwdBatch]>(smem + L::rec);
     float4* s_pixA = reinterpret_cast<float4*>(smem + L::pixA);
     float4* s_pixB = reinterpret_cast<float4*>(smem + L::pixB);
-    int* s_wmax = reinterpret_cast<int*>(smem + L::wmax);
 
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    uint8_t* s_listw = reinterpret_cast<uint8_t*>(smem + L::list) + wid * kBwdBatch;
-    uint32_t* s_hmw = reinterpret_cast<uint32_t*>(smem + L::hm) + wid * kBwdBatch;
+    // this warp's queue of compacted list entries: pixel mask and list position
+    uint32_t* s_qmask = reinterpret_cast<uint32_t*>(smem + L::qmask) + wid * (kBwdQueue + 1);
+    int* s_qpos = reinterpret_cast<int*>(smem + L::qpos) + wid * (kBwdQueue + 1);
+    float4* s_recw = reinterpret_cast<float4*>(smem + L::rec) + wid * (kBwdRecQuads * kBwdChunk);
     uint32_t sa_base = smem_addr(smem);
     asm volatile("" : "+r"(sa_base));                     // opaque: kept in a register, not rebuilt at every use
-    const uint32_t sa_rec = sa_base + (uint32_t)L::rec, sa_x = sa_base + (uint32_t)(L::x + wid * (3 * kBwdGroup * 32 * sizeof(float))),
-                   sa_list = sa_base + (uint32_t)(L::list + wid * kBwdBatch);
+    const uint32_t sa_rec = sa_base + (uint32_t)(L::rec + wid * (kBwdRecQuads * kBwdChunk * sizeof(float4))),
+                   sa_x = sa_base + (uint32_t)(L::x + wid * (3 * kBwdGroup * 32 * sizeof(float))),
+                   sa_qpos = sa_base + (uint32_t)(L::qpos + wid * (kBwdQueue + 1) * sizeof(int));
 
     const int view = blockIdx.y;
     const size_t npix = (size_t)a.W * a.H;
@@ -249,16 +252,14 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
     s_pixB[tid] = make_float4(dpix1, dpix2, pixx, pixy);
     asm volatile("" : "+f"(pixx), "+f"(pixy));
 
-    // deepest list entry any pixel of the warp / of the tile blended
+    // deepest list entry any pixel of the warp blended: the warp walks from there, whatever the other warps do
     int wmax = last_contributor;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) wmax = max(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
-    if (lane == 0) s_wmax[wid] = wmax;
-    __syncthreads();
-    int n_eff = 0;
-#pragma unroll
-    for (int w = 0; w < kBwdWarps; ++w) n_eff = max(n_eff, s_wmax[w]);
-    const int rounds = (n_eff + kBwdBatch - 1) / kBwdBatch;
+    const int steps = (wmax + kBwdWindow - 1) / kBwdWindow;
+    // the list position of the pixel's median contributor (-1: none)
+    int pos_median = median_contributor - 1;
+    asm volatile("" : "+r"(pos_median));             // kept in a register, not rebuilt at every phase-1 trip
 
     // accum_rec / last_* recursions of backward.cu:331-385.  Of the eight accum_rec channels (colour, depth, normal,
     // alpha) dL_dalpha only ever needs sum_k (c_k - accum_rec_k) g_k, g_k the channel's upstream gradient, so the
@@ -289,65 +290,59 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
     // n / C into a multiply ((n * M) >> 16 == n / C exactly while n * C < 65536; n <= 47, C <= 16 here)
     const uint32_t candM = 65536u / (uint32_t)((lane & (kBwdGroup - 1)) + 1) + 1u;
     const uint32_t hshift = (uint32_t)lane & 16u;          // 16 * (which half of a 32-entry chunk this lane stands for)
-    const uint32_t sa_hm = sa_base + (uint32_t)(L::hm + wid * kBwdBatch * sizeof(uint32_t));
+    const uint32_t sa_hm = sa_base + (uint32_t)(L::qmask + wid * (kBwdQueue + 1) * sizeof(uint32_t));
     const uint32_t sa_pixA = sa_base + (uint32_t)(L::pixA + wid * 32 * sizeof(float4));
     const uint32_t sa_pixB = sa_base + (uint32_t)(L::pixB + wid * 32 * sizeof(float4));
 
-    // every thread fetches the list entry it will stage in the NEXT round while the current round is being
-    // processed, so that a round's staging waits for one global load, not two dependent ones
-    uint32_t next_id = 0;
-    if (n_eff - 1 - tid >= 0) next_id = __ldg(a.point_list + range.x + (n_eff - 1 - tid));
-
     // this warp's row of the forward's contribution record, by list position
     const uint32_t* wmasks = a.masks + (size_t)gw * a.capacity + range.x;
+    const uint32_t* plist = a.point_list + range.x;
 
-    for (int b = 0; b < rounds; ++b) {
-        // ---- the warp's contribution masks of batch b, requested first so that they arrive with the records (lane
-        // takes slots lane + 32 k); positions at or behind the warp's deepest contributor were not recorded: 0
-        uint32_t mk[kBwdBatch / 32];
+    // The warp walks its own block's list positions back to front from its own deepest contributor, kBwdWindow per
+    // step, and appends the entries the forward blended into some pixel of the block to its queue.  Every full 32-entry
+    // chunk of the queue is processed at once; the rest waits for the next step, so that every group but the warp's
+    // last is full.  Nothing here depends on the other warps of the CTA.
+    int nq = 0;                                           // entries in the queue, carried from the last step
+    for (int b = 0; b < steps; ++b) {
+        // ---- the block's contribution masks of positions wmax-1-(b kBwdWindow + 32 k + lane), k = 0..3, all requested
+        // before the first is used
+        uint32_t mk[kBwdWindow / 32];
 #pragma unroll
-        for (int k = 0; k < kBwdBatch / 32; ++k) {
-            const int pos = n_eff - 1 - (b * kBwdBatch + k * 32 + lane);
-            mk[k] = (pos >= 0 && pos < wmax) ? __ldg(wmasks + pos) : 0u;
+        for (int k = 0; k < kBwdWindow / 32; ++k) {
+            const int pos = wmax - 1 - (b * kBwdWindow + k * 32 + lane);
+            mk[k] = pos >= 0 ? __ldg(wmasks + pos) : 0u;
         }
-        // ---- stage batch b (back to front: slot j holds list position n_eff-1-(b*kBwdBatch+j))
-        __syncthreads();                                  // every warp is done with the previous batch's records
-        for (int jt = tid; jt < kBwdBatch; jt += kBwdThreads) {
-            const int pos = n_eff - 1 - (b * kBwdBatch + jt);
-            if (pos >= 0) {
-                const uint32_t id = next_id;
-                const float4* r = a.rec + (size_t)id * SRF_REC_QUADS;
+        // ---- appended to the queue, in walk order, with their list positions
 #pragma unroll
-                for (int k = 0; k < 3; ++k) s_rec[k][jt] = ldg4(r + k);
-                const float4 q3 = ldg4(r + 3), q4 = ldg4(r + 4);
-                s_rec[3][jt] = make_float4(q3.x, q3.y, q3.z, q4.x);
-                s_rec[4][jt] = make_float4(q4.y, q4.z, __uint_as_float(id), 0.0f);
-            }
-        }
-        const int npos = n_eff - 1 - ((b + 1) * kBwdBatch + tid);
-        if (npos >= 0) next_id = __ldg(a.point_list + range.x + npos);
-        __syncthreads();
-
-        // ---- compacted list of the staged splats the forward blended into some pixel of this warp's block, with
-        // their pixel masks
-        int nh = 0;
-#pragma unroll
-        for (int k = 0; k < kBwdBatch / 32; ++k) {
+        for (int k = 0; k < kBwdWindow / 32; ++k) {
             const bool hit = mk[k] != 0u;
             const unsigned hits = __ballot_sync(0xffffffffu, hit);
             if (hit) {
-                const int h = nh + __popc(hits & ((1u << lane) - 1u));
-                s_listw[h] = (uint8_t)(k * 32 + lane);
-                s_hmw[h] = mk[k];
+                const int h = nq + __popc(hits & ((1u << lane) - 1u));
+                s_qpos[h] = wmax - 1 - (b * kBwdWindow + k * 32 + lane);
+                s_qmask[h] = mk[k];
             }
-            nh += __popc(hits);
+            nq += __popc(hits);
         }
+        // the full chunks of the queue; at the warp's last step, all of it
+        const int nh = b == steps - 1 ? nq : (nq & ~(kBwdChunk - 1));
         __syncwarp();
-        // the batch slot of the pixel's median contributor: slot j holds list position n_eff - 1 - (b kBwdBatch + j)
-        int j_median = n_eff - median_contributor - b * kBwdBatch;
-        asm volatile("" : "+r"(j_median));               // kept in a register, not rebuilt at every phase-1 trip
 
-        for (int g0 = 0; g0 < nh; g0 += 32) {
+        for (int g0 = 0; g0 < nh; g0 += kBwdChunk) {
+            // ---- gather the chunk's records into the warp's ring (slot i = chunk entry i), five planes:
+            //   q0 q1 q2, (n.x n.y n.z r), (g b splat-id)
+            // The previous chunk's last group ended with a __syncwarp, so its records are no longer read.
+            if (g0 + lane < nh) {
+                const uint32_t id = __ldg(plist + s_qpos[g0 + lane]);
+                const float4* r = a.rec + (size_t)id * SRF_REC_QUADS;
+                const float4 q0 = ldg4(r), q1 = ldg4(r + 1), q2 = ldg4(r + 2), q3 = ldg4(r + 3), q4 = ldg4(r + 4);
+                s_recw[lane] = q0;
+                s_recw[kBwdChunk + lane] = q1;
+                s_recw[2 * kBwdChunk + lane] = q2;
+                s_recw[3 * kBwdChunk + lane] = make_float4(q3.x, q3.y, q3.z, q4.x);
+                s_recw[4 * kBwdChunk + lane] = make_float4(q4.y, q4.z, __uint_as_float(id), 0.0f);
+            }
+            __syncwarp();
             // pixel mask of chunk entry g0 + lane (0 past the end of the list); the 32x32 bit transpose of the chunk's
             // masks hands lane p the word "which of these 32 splats were blended into MY pixel"
             const uint32_t ew = g0 + lane < nh ? lds_u32(sa_hm + 4u * (uint32_t)(g0 + lane)) : 0u;
@@ -390,17 +385,19 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
                 // Each lane loops over its own pairs and leaves when it has none left; the warp reconverges once,
                 // after the loop, not at every trip.
                 uint32_t rbits = __brev(colword >> (sub * kBwdGroup)) & 0xffff0000u;
-                const uint32_t sa_list_g = sa_list + (uint32_t)(gbase + 31);
+                // entry i of the group is queue entry gbase + i and ring slot sub * 16 + i
+                const uint32_t sa_pos_g = sa_qpos + 4u * (uint32_t)(gbase + 31);
+                const uint32_t sa_rec_g = sa_rec + 16u * (uint32_t)(sub * kBwdGroup + 31);
                 while (rbits != 0u) {
                     const int p = 31 - __clz(rbits);             // entry i = 31 - p of the group
                     rbits &= bits_below(p);
-                    const int j = (int)lds_u8(sa_list_g - (uint32_t)p);
+                    const int pos = (int)lds_u32(sa_pos_g - 4u * (uint32_t)p);
                     PairBwd e;
-                    const uint32_t sa_j = sa_rec + 16u * j;
+                    const uint32_t sa_j = sa_rec_g - 16u * (uint32_t)p;
                     // all five loads go out before the pair evaluation, so that their latency overlaps it
-                    const float4 q0 = lds_f4(sa_j), q1 = lds_f4(sa_j + 16u * kBwdBatch), q2 = lds_f4(sa_j + 32u * kBwdBatch);
-                    const float4 q3 = lds_f4(sa_j + 48u * kBwdBatch);   // n.x n.y n.z r
-                    const float2 q4 = lds_f2(sa_j + 64u * kBwdBatch);   // g b
+                    const float4 q0 = lds_f4(sa_j), q1 = lds_f4(sa_j + 16u * kBwdChunk), q2 = lds_f4(sa_j + 32u * kBwdChunk);
+                    const float4 q3 = lds_f4(sa_j + 48u * kBwdChunk);   // n.x n.y n.z r
+                    const float2 q4 = lds_f2(sa_j + 64u * kBwdChunk);   // g b
                     eval_pair_bwd(q0, q1, q2, pixx, pixy, e);
                     const bool lowpass = e.lowpass;
                     const float alpha = e.alpha, c_d = e.depth;
@@ -428,7 +425,7 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
                     // 2 (m_d A - D) ~ 0), and the gradients carry 1e-6 atomic-order noise anyway.
                     const float rcd = rcp_fast(c_d);             // depth >= 0.2
                     float dL_dweight = fmaf(fmaf(W2, rcd, -Z0), rcd, W0);
-                    if (j == j_median) {
+                    if (pos == pos_median) {
                         dL_dz += dL_dmedian_depth;
                         dL_dweight += dL_dmax_dweight;
                     }
@@ -470,7 +467,7 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
                 const uint32_t own_s = __shfl_sync(0xffffffffu, sched, hb + own);
                 const int own_end = (int)(own_s & 0xffu), own_n = (int)((own_s >> 8) & 0xffu), C = (int)(own_s >> 16) + 1;
                 // Every compacted entry has a non-zero mask, so every group has work.  The pixel mask of entry gbase + i
-                // is the word "which pixels contributed to splat i": the very word s_hmw holds, which the chunk's
+                // is the word "which pixels contributed to splat i": the very word the queue holds, which the chunk's
                 // transpose was made from and which transposing phase 1's words back would rebuild.
                 const uint32_t word = lds_u32(sa_hm + 4u * (uint32_t)(gbase + own));
                 const bool have = lane < lanes_used;
@@ -486,9 +483,9 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
                 uint32_t mybits = have ? (word & (0xffffffffu << pos)) : 0u;
                 // only a lane in use (it has at least one pair) loads the record, accumulates and sends partial sums
                 if (mybits != 0) {
-                    const uint32_t sa_j2 = sa_rec + 16u * lds_u8(sa_list + gbase + own);
-                    const float4 q0 = lds_f4(sa_j2), q1 = lds_f4(sa_j2 + 16u * kBwdBatch), q2 = lds_f4(sa_j2 + 32u * kBwdBatch);
-                    const uint32_t splat_id = lds_u32(sa_j2 + 64u * kBwdBatch + 8u);
+                    const uint32_t sa_j2 = sa_rec + 16u * (uint32_t)(sub * kBwdGroup + own);
+                    const float4 q0 = lds_f4(sa_j2), q1 = lds_f4(sa_j2 + 16u * kBwdChunk), q2 = lds_f4(sa_j2 + 32u * kBwdChunk);
+                    const uint32_t splat_id = lds_u32(sa_j2 + 64u * kBwdChunk + 8u);
                     const f32x2 nTu_x = pk2(-q0.x, -q0.y), nTu_y = pk2(-q0.z, -q0.w), nTu_z = pk2(-q1.x, -q1.y);
                     const float Twx = q1.z, Twy = q1.w, Twz = q2.x;
                     const f32x2 Twxy = pk2(Twx, Twy), cen = pk2(q2.y, q2.z);
@@ -573,6 +570,17 @@ __global__ void __launch_bounds__(kBwdThreads, kBwdCtasPerSM) render_bwd_kernel(
                 __syncwarp();     // phase 1 of the next group overwrites the X tile
             }
         }
+        // ---- the entries of a partial chunk move to the front of the queue and wait for the next step
+        const int rest = nq - nh;
+        if (nh > 0 && rest > 0) {
+            uint32_t m = 0u;
+            int p = 0;
+            if (lane < rest) { m = s_qmask[nh + lane]; p = s_qpos[nh + lane]; }
+            __syncwarp();
+            if (lane < rest) { s_qmask[lane] = m; s_qpos[lane] = p; }
+            __syncwarp();
+        }
+        nq = rest;
     }
 }
 

@@ -4,8 +4,13 @@
     python tools/sass_budget.py FILE.cubin      # or an existing cubin
     python tools/sass_budget.py FILE.sass       # or the text of `cuobjdump -sass`
 
-Prints the static instruction counts of the four parts of render_bwd_kernel<kEpiFloat> (the default epilogue; the
-deterministic instantiations in the same cubin are not counted) that a group runs through:
+Prints the static instruction counts of the parts of render_bwd_kernel<kEpiFloat> (the default epilogue; the
+deterministic instantiations in the same cubin are not counted):
+
+  walk step        the warp's step of 128 list positions outside its chunks: mask loads, compaction into the queue,
+                   the carry of a partial chunk (the outermost of the three loops around the groups)
+  record gather    the chunk's point_list and record loads into the warp's ring, per 32 entries
+  chunk set-up     the rest of the chunk loop before its first group: mask transpose and phase-2 schedule
 
   phase-1 trip     the per-pixel pair loop (from its head to its back-branch), without the exact re-evaluation of
                    eval_pair_bwd (the smallest forward branch in the loop that jumps over every CALL of it: the IEEE
@@ -131,18 +136,28 @@ def budget(insns: list[tuple[int, str]]) -> dict[str, int]:
                     spans.append(tgt - i - 1)
         exact = min(spans) if spans else 0
     h2, b2 = back_branch_after(b1 + 1)
-    reds = [i for i, (_, t) in enumerate(insns) if t.lstrip("@!P0123456789 ").startswith("RED")]
-    last_red = max(r for r in reds if r > b2)
-    # the two loops around the groups, by their back-branches to before phase 1: the 16-entry groups of a chunk,
-    # then the 32-entry chunks of a batch
+    # the partial sums' REDs (not the REDUX of the warp reductions): the run of them right after phase 2; ptxas may
+    # place copies of the group body for divergent warps after the kernel's end, which are not counted
+    reds = [i for i, (_, t) in enumerate(insns)
+            if t.lstrip("@!P0123456789 ").startswith("RED") and not t.lstrip("@!P0123456789 ").startswith("REDUX")]
+    last_red = next(r for r in reds if r > b2)
+    while any(last_red < r <= last_red + 8 for r in reds):
+        last_red = next(r for r in reds if last_red < r <= last_red + 8)
+    # the three loops around the groups, by their back-branches to before phase 1: the 16-entry groups of a chunk,
+    # the 32-entry chunks of a walk step, then the warp's walk steps of 128 list positions
     outer = []
     for i in range(last_red, len(insns)):
         m = _BRA.search(insns[i][1])
         if m and int(m.group(1), 16) < insns[h1][0]:
             outer.append((idx[int(m.group(1), 16)], i))
-    (gh, gb), (ch, _) = outer[0], outer[1]
+    (gh, gb), (ch, cb), (sh, sb) = outer[0], outer[1], outer[2]
+    # the chunk's record gather: from the chunk loop's head to its last 16-byte shared store before the groups (none
+    # where the records are staged per step, for the whole CTA)
+    gather = max((i for i in range(ch, gh) if "STS.128" in insns[i][1]), default=ch - 1) - ch + 1
     return {
-        "chunk set-up (per 32 entries)": gh - ch,
+        "walk step (per 128 positions)": (sb - sh + 1) - (cb - ch + 1),
+        "record gather (per 32 entries)": gather,
+        "chunk set-up (per 32 entries)": gh - ch - gather,
         "group head (to the phase-1 loop)": h1 - gh,
         "phase-1 trip (fast path)": (b1 - h1 + 1) - exact,
         "phase-1 exact re-evaluation": exact,
@@ -150,7 +165,7 @@ def budget(insns: list[tuple[int, str]]) -> dict[str, int]:
         "phase-2 trip": b2 - h2 + 1,
         "partial sums": last_red - b2,
         "group tail (after the REDs)": gb - last_red,
-        "REDs": sum(1 for r in reds if r > b2),
+        "REDs": sum(1 for r in reds if b2 < r <= last_red),
     }
 
 
