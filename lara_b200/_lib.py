@@ -108,6 +108,19 @@ SIGNATURES = {
                                        _P, _P,                                        # dL_dsh, workspace
                                        _P, _P, _P,                                    # dL_dvolume_feat, _dpoint_feats, _dshs
                                        _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),      # the ten parameter gradients
+    # include/surfel_feat_volume.h
+    "srf_feat_volume_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_size_t)]),
+    "srf_feat_volume_forward": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, c_int,   # stream, B, V, C, h, w, R, E
+                                        c_int, c_int, c_int, c_int,                  # Vmax, H_img, W_img, n_group
+                                        _P, _P, _P, _P, _P,                          # img_feats, rays, w2c, ixt, grid
+                                        _P, _P, _P, _P, _P,                          # norm w, b, mlp w, b, view_embed
+                                        _P, _P]),                                    # workspace, out
+    "srf_feat_volume_backward": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                         c_int, c_int, c_int, c_int,
+                                         _P, _P, _P, _P, _P,
+                                         _P, _P, _P, _P,                             # norm w, b, mlp w, b
+                                         _P, _P,                                     # dL_dout, workspace
+                                         _P, _P, _P, _P, _P, _P]),                   # the six gradients
     "srf_profile_begin": (c_int, []),
     "srf_profile_end": (c_int, [POINTER(c_float), POINTER(c_int), c_int]),
 }
@@ -243,6 +256,11 @@ def deterministic(requested: Optional[bool] = None) -> bool:
 def fine_head_workspace_bytes(lib, n: int, V: int, D: int, sh_dim: int, gather: bool) -> int:
     """Workspace of srf_fine_head_backward on the current device."""
     return _size_query(lib.srf_fine_head_workspace_bytes, n, V, D, sh_dim, 1 if gather else 0)
+
+
+def feat_volume_workspace_bytes(lib, B: int, V: int, C: int, h: int, w: int, R: int, E: int) -> int:
+    """Workspace of srf_feat_volume_forward / _backward."""
+    return _size_query(lib.srf_feat_volume_workspace_bytes, B, V, C, h, w, R, E)
 
 
 def int3(v) -> ctypes.Array:

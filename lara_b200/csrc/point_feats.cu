@@ -9,7 +9,8 @@
 //                    img_ref(3) | image(3) | acc_map(1) | depth(1),   channel 7 replaced by |s_depth - z|
 // The chain of roundings is kept as written: folding it to ix = x moves points across pixel-centre lines at the
 // ulp level, and those lines are where the point gradient jumps.  The projection sums in the order of a k-ordered
-// FMA loop, the tap weights are grid_sampler_2d's.
+// FMA loop, the tap weights are grid_sampler_2d's.  Projection, coordinate chain and taps are in sample_taps.cuh,
+// shared with feat_volume.cu.
 //
 // A tap is used only if its sample coordinate is finite and its integer index lies in the image: the bounds are
 // tested on the floored float before any conversion, so no input can make the kernels read outside the images.
@@ -23,6 +24,7 @@
 
 #include "../../include/surfel_rasterizer.h"
 #include "det_sum.cuh"
+#include "sample_taps.cuh"
 #include "surfel_kernels.h"
 
 namespace srf {
@@ -52,63 +54,6 @@ namespace {
 
 constexpr int kPfThreads = 256;
 
-struct PfTaps {
-    float tx0, tx1, ty0, ty1;    // ix - floor(ix), floor(ix) + 1 - ix, same for y
-    float w[4];                  // nw, ne, sw, se
-    int off[4];                  // y * W + x of each tap, -1 = not used
-    bool any;
-};
-
-// p = K (R x + t) for view v; returns xy / z in xy, z in z
-__device__ __forceinline__ void pf_project(const PointFeatsArgs& a, int v, float x0, float x1, float x2,
-                                           float& px, float& py, float& pz, float m[21]) {
-    const float* E = a.w2cs + 16 * (size_t)v;
-    const float* K = a.ixts + 9 * (size_t)v;
-#pragma unroll
-    for (int r = 0; r < 3; ++r) {
-#pragma unroll
-        for (int k = 0; k < 4; ++k) m[4 * r + k] = __ldg(E + 4 * r + k);
-    }
-#pragma unroll
-    for (int k = 0; k < 9; ++k) m[12 + k] = __ldg(K + k);
-    float q[3];
-#pragma unroll
-    for (int r = 0; r < 3; ++r)      // points @ R^T, then + t (two torch ops)
-        q[r] = __fadd_rn(__fmaf_rn(x2, m[4 * r + 2], __fmaf_rn(x1, m[4 * r + 1], __fmul_rn(x0, m[4 * r]))), m[4 * r + 3]);
-    float p[3];
-#pragma unroll
-    for (int r = 0; r < 3; ++r)      // @ K^T
-        p[r] = __fmaf_rn(q[2], m[12 + 3 * r + 2], __fmaf_rn(q[1], m[12 + 3 * r + 1], __fmul_rn(q[0], m[12 + 3 * r])));
-    px = p[0]; py = p[1]; pz = p[2];
-}
-
-// network.py:401 followed by grid_sample's unnormalisation, one rounding per torch operation
-__device__ __forceinline__ float pf_source_coord(float xy, float size) {
-    const float g = __fadd_rn(__fmul_rn(__fdiv_rn(__fadd_rn(xy, 0.5f), size), 2.0f), -1.0f);
-    return __fdiv_rn(__fadd_rn(__fmul_rn(__fadd_rn(g, 1.0f), size), -1.0f), 2.0f);
-}
-
-__device__ __forceinline__ PfTaps pf_taps(float ix, float iy, int W, int H) {
-    PfTaps t;
-    const float fx = floorf(ix), fy = floorf(iy);
-    t.tx1 = __fsub_rn(__fadd_rn(fx, 1.0f), ix); t.tx0 = __fsub_rn(ix, fx);
-    t.ty1 = __fsub_rn(__fadd_rn(fy, 1.0f), iy); t.ty0 = __fsub_rn(iy, fy);
-    t.w[0] = __fmul_rn(t.tx1, t.ty1);    // nw = (ix_se - ix) * (iy_se - iy)
-    t.w[1] = __fmul_rn(t.tx0, t.ty1);    // ne = (ix - ix_sw) * (iy_sw - iy)
-    t.w[2] = __fmul_rn(t.tx1, t.ty0);    // sw = (ix_ne - ix) * (iy - iy_ne)
-    t.w[3] = __fmul_rn(t.tx0, t.ty0);    // se = (ix - ix_nw) * (iy - iy_nw)
-    // comparisons with NaN are false and +-inf fails one side: non-finite coordinates use no tap
-    const bool x0 = fx >= 0.0f && fx <= (float)(W - 1), x1 = fx >= -1.0f && fx <= (float)(W - 2);
-    const bool y0 = fy >= 0.0f && fy <= (float)(H - 1), y1 = fy >= -1.0f && fy <= (float)(H - 2);
-    const int xi = (x0 || x1) ? (int)fx : 0, yi = (y0 || y1) ? (int)fy : 0;
-    t.off[0] = (x0 && y0) ? yi * W + xi : -1;
-    t.off[1] = (x1 && y0) ? yi * W + xi + 1 : -1;
-    t.off[2] = (x0 && y1) ? (yi + 1) * W + xi : -1;
-    t.off[3] = (x1 && y1) ? (yi + 1) * W + xi + 1 : -1;
-    t.any = (x0 || x1) && (y0 || y1);
-    return t;
-}
-
 // plane of channel c (0..7) of view v in the stack img_ref | image | acc | depth
 __device__ __forceinline__ const float* pf_plane(const PointFeatsArgs& a, int v, int c, size_t HW) {
     if (c < 3) return a.img_ref + ((size_t)v * 3 + c) * HW;
@@ -137,9 +82,9 @@ __global__ void __launch_bounds__(kPfThreads) point_feats_fwd_kernel(PointFeatsA
     const size_t HW = (size_t)a.H * a.W, n = (size_t)a.n;
     for (int v = 0; v < a.V; ++v) {
         float px, py, pz, m[21];
-        pf_project(a, v, x0, x1, x2, px, py, pz, m);
-        const float ix = pf_source_coord(__fdiv_rn(px, pz), (float)a.W);
-        const float iy = pf_source_coord(__fdiv_rn(py, pz), (float)a.H);
+        pf_project(a.w2cs + 16 * (size_t)v, a.ixts + 9 * (size_t)v, x0, x1, x2, px, py, pz, m);
+        const float ix = pf_source_coord(__fdiv_rn(px, pz), (float)a.W, (float)a.W);
+        const float iy = pf_source_coord(__fdiv_rn(py, pz), (float)a.H, (float)a.H);
         const PfTaps t = pf_taps(ix, iy, a.W, a.H);
         float* out = a.feats + (size_t)v * 8 * n + i;
 #pragma unroll
@@ -195,9 +140,10 @@ __global__ void __launch_bounds__(kPfThreads) point_feats_bwd_kernel(PointFeatsA
     float gx0 = 0.0f, gx1 = 0.0f, gx2 = 0.0f;           // dL/dpoint, summed over the views
     for (int v = 0; v < a.V; ++v) {
         float px, py, pz, m[21];
-        pf_project(a, v, x0, x1, x2, px, py, pz, m);
+        pf_project(a.w2cs + 16 * (size_t)v, a.ixts + 9 * (size_t)v, x0, x1, x2, px, py, pz, m);
         const float xs = __fdiv_rn(px, pz), ys = __fdiv_rn(py, pz);
-        const PfTaps t = pf_taps(pf_source_coord(xs, (float)a.W), pf_source_coord(ys, (float)a.H), a.W, a.H);
+        const PfTaps t = pf_taps(pf_source_coord(xs, (float)a.W, (float)a.W),
+                                 pf_source_coord(ys, (float)a.H, (float)a.H), a.W, a.H);
         const float* g = a.g_feats + (size_t)v * 8 * n + i;
         // z_diff = |s_depth - z|: vjp with sign(0) = 0
         float dvals[4];
