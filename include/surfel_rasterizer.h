@@ -124,6 +124,31 @@ int srf_views_forward_render(srf_stream_t stream, int V, int P, int image_height
                              void* entries, uint32_t* point_list, void* image_state,
                              const float* cams, float* out_color, float* out_others, int for_backward);
 
+/* ---- subset forward (LaRa's fine pass, lightning/network.py:486-525; DESIGN §3.18) ----------------------------
+ * Renders the n Gaussians idx[0..n) (strictly ascending indices into the P of a coarse srf_views_forward) of the same V
+ * cameras and image size with new SH coefficients shs [n,M,3], from the coarse forward's state instead of a preprocess
+ * and a binning: the records, depths, rects and radii of the subset are the coarse ones of Gaussian idx[j], with the
+ * colour word recomputed from shs[j]; each tile's list is the coarse list with the other Gaussians removed.  The
+ * outputs are bit-identical to srf_views_forward on the gathered subset (means3D[idx], opacities[idx], ...) with the
+ * same raw_activations flag, and the state it leaves feeds srf_views_backward with P = n (for_backward != 0) exactly
+ * as that forward's would.  The kept entries stay at the coarse tile's list offsets, so the subset's `point_list`
+ * workspace is sized, like the coarse one, by `capacity`, which must equal the coarse forward's capacity
+ * (`coarse_capacity`, whose counts must have fit it: re-run the coarse stage 2 first if they did not).
+ * Inputs: the coarse state (radii [V,P], geom / tile workspaces, point_list, and whether the coarse forward was
+ * for_backward), means3D [P,3] (the coarse centers), cams as given to the coarse forward.  Outputs: radii [V,n], the
+ * subset's geom / tile / image workspaces and point_list (sizes from srf_views_workspace_bytes(V, n, H, W, capacity,
+ * for_backward); entries are not used), out_color / out_others as srf_views_forward.  `workspace`: 256-byte aligned,
+ * srf_views_subset_workspace_bytes(P).  colors_precomp is not supported (must be NULL).  n == 0 renders the
+ * background.  Every argument check is made before anything is enqueued; nothing waits for the stream. */
+int srf_views_subset_forward(srf_stream_t stream, int V, int P, int n, int D, int M,
+                             const int64_t* idx, const float* means3D, const float* shs, const float* colors_precomp,
+                             const float* cams, int image_height, int image_width, size_t capacity,
+                             const int* coarse_radii, const void* coarse_geom_state, const void* coarse_tile_state,
+                             const uint32_t* coarse_point_list, size_t coarse_capacity, int coarse_for_backward,
+                             int* radii, void* geom_state, void* tile_state, uint32_t* point_list, void* image_state,
+                             float* out_color, float* out_others, void* workspace, int for_backward);
+int srf_views_subset_workspace_bytes(int P, size_t* bytes);
+
 /* ---- backward ------------------------------------------------------------------
  * Replaces Rasterizer::backward (rasterizer_impl.cu:346-448): BACKWARD::render,
  * computeAABB backward, BACKWARD::preprocess.  Consumes the state the forward left in the

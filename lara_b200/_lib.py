@@ -69,6 +69,15 @@ SIGNATURES = {
         _P, _P, _P, _P,                          # dL_dopacity, dL_dscales, dL_drotations, dL_dtransMat
         c_int, c_int,                            # raw_activations, deterministic
     ]),
+    "srf_views_subset_forward": (c_int, [
+        _P, c_int, c_int, c_int, c_int, c_int,  # stream, V, P, n, D, M
+        _P, _P, _P, _P, _P,                 # idx, means3D, shs, colors_precomp, cams
+        c_int, c_int, c_size_t,             # H, W, capacity
+        _P, _P, _P, _P, c_size_t, c_int,    # coarse radii, geom_state, tile_state, point_list, capacity, for_backward
+        _P, _P, _P, _P, _P,                 # radii, geom_state, tile_state, point_list, image_state
+        _P, _P, _P, c_int,                  # out_color, out_others, workspace, for_backward
+    ]),
+    "srf_views_subset_workspace_bytes": (c_int, [c_int, POINTER(c_size_t)]),
     "srf_views_backward_deterministic_scratch_bytes": (c_int, [c_int, c_int, POINTER(c_size_t)]),
     "srf_views_epilogue_forward": (c_int, [_P, c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "srf_views_epilogue_backward": (c_int, [_P, c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
@@ -224,6 +233,11 @@ def _size_query(fn, *args) -> int:
 def det_backward_scratch_bytes(lib, V: int, P: int) -> int:
     """Scratch of srf_views_backward(..., deterministic=1)."""
     return _size_query(lib.srf_views_backward_deterministic_scratch_bytes, V, P)
+
+
+def subset_workspace_bytes(lib, P: int) -> int:
+    """Workspace of srf_views_subset_forward for a coarse forward of P Gaussians."""
+    return _size_query(lib.srf_views_subset_workspace_bytes, P)
 
 
 def ms_ssim_workspace_bytes(lib, B: int, C: int, H: int, W: int) -> int:

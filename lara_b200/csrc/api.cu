@@ -148,6 +148,47 @@ int sm_count() {
     }
     return cache[dev];
 }
+
+StateLayout state_layout(int P, int H, int W) {
+    const GeomLayout g = geom_layout(P);
+    const TileLayout t = tile_layout(H, W);
+    StateLayout s;
+    s.rec = g.rec; s.depths = g.depths; s.rects = g.rects; s.geom_stride = g.total;
+    s.tile_count = t.count; s.counters = t.counters; s.ranges = t.ranges; s.order = t.order; s.tile_stride = t.total;
+    s.gx = t.gx; s.gy = t.gy; s.ntiles = t.ntiles;
+    return s;
+}
+
+size_t plist_stride(size_t capacity, bool for_backward) { return plist_stride_bytes(capacity, for_backward); }
+
+int views_blend(cudaStream_t stream, int V, int P, int image_height, int image_width, size_t capacity,
+                const void* geom_state, const void* tile_state, const uint32_t* point_list, void* image_state,
+                const float* cams, float* out_color, float* out_others, bool record) {
+    const TileLayout tl = tile_layout(image_height, image_width);
+    const ImageLayout il = image_layout(image_height, image_width);
+    const GeomLayout gl = geom_layout(P);
+    RenderFwdArgs r;
+    memset(&r, 0, sizeof(r));
+    r.W = image_width; r.H = image_height; r.gx = tl.gx; r.gy = tl.gy; r.nviews = V;
+    r.capacity = (uint32_t)capacity;
+    r.ranges = at<uint2>(tile_state, tl.ranges);
+    r.tile_order = at<uint32_t>(tile_state, tl.order);
+    r.point_list = point_list;
+    r.masks = record ? at<uint32_t>(point_list, plist_masks_offset(capacity)) : nullptr;
+    r.rec = P > 0 ? at<float4>(geom_state, gl.rec) : nullptr;
+    r.bg = cams + SRF_CAM_BG;
+    r.out_color = out_color; r.out_others = out_others;
+    if (record) {
+        r.accum = at<float>(image_state, il.accum);
+        r.n_contrib = at<uint32_t>(image_state, il.ncontrib);
+        r.image_stride = il.total;
+    }
+    r.geom_stride = gl.total; r.tile_stride = tl.total; r.plist_stride = plist_stride_bytes(capacity, record);
+    r.cam_stride = SRF_CAM_FLOATS;
+    const cudaError_t e = launch_render_fwd(r, record, stream);
+    if (e != cudaSuccess) return cuda_error("render_fwd launch", e);
+    return 0;
+}
 }  // namespace srf
 
 extern "C" {
@@ -335,7 +376,6 @@ int forward_render_impl(cudaStream_t stream, int V, int P, int image_height, int
                         void* entries, uint32_t* point_list, void* image_state,
                         const float* cams, float* out_color, float* out_others, bool record) {
     const TileLayout tl = tile_layout(image_height, image_width);
-    const ImageLayout il = image_layout(image_height, image_width);
     const GeomLayout gl = geom_layout(P);
 
     srf::BinArgs b;
@@ -354,27 +394,8 @@ int forward_render_impl(cudaStream_t stream, int V, int P, int image_height, int
         e = srf::launch_bin_and_sort(b, stream);
         if (e != cudaSuccess) return cuda_error("binning launch", e);
     }
-    srf::RenderFwdArgs r;
-    memset(&r, 0, sizeof(r));
-    r.W = image_width; r.H = image_height; r.gx = tl.gx; r.gy = tl.gy; r.nviews = V;
-    r.capacity = (uint32_t)capacity;
-    r.ranges = b.ranges;
-    r.tile_order = b.tile_order;
-    r.point_list = point_list;
-    r.masks = record ? at<uint32_t>(point_list, plist_masks_offset(capacity)) : nullptr;
-    r.rec = P > 0 ? at<float4>(geom_state, gl.rec) : nullptr;
-    r.bg = cams + SRF_CAM_BG;
-    r.out_color = out_color; r.out_others = out_others;
-    if (record) {
-        r.accum = at<float>(image_state, il.accum);
-        r.n_contrib = at<uint32_t>(image_state, il.ncontrib);
-        r.image_stride = il.total;
-    }
-    r.geom_stride = b.geom_stride; r.tile_stride = b.tile_stride; r.plist_stride = b.plist_stride;
-    r.cam_stride = SRF_CAM_FLOATS;
-    e = srf::launch_render_fwd(r, record, stream);
-    if (e != cudaSuccess) return cuda_error("render_fwd launch", e);
-    return 0;
+    return srf::views_blend(stream, V, P, image_height, image_width, capacity, geom_state, tile_state, point_list,
+                            image_state, cams, out_color, out_others, record);
 }
 
 int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int M, int image_height, int image_width,

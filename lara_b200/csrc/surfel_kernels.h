@@ -157,6 +157,22 @@ void prof_stop(int kernel, cudaStream_t stream);
 // number of SMs of the current device (cached per device)
 int sm_count();
 
+// Byte offsets inside one view's geom / tile workspaces and their per-view strides (the layout srf_state_layout
+// reports), for the entries outside api.cu that read or write the forward's state.
+struct StateLayout {
+    size_t rec, depths, rects, geom_stride;
+    size_t tile_count, counters, ranges, order, tile_stride;
+    int gx, gy, ntiles;
+};
+StateLayout state_layout(int P, int H, int W);
+// bytes from one view's point_list workspace to the next (the list, then for_backward the contribution record)
+size_t plist_stride(size_t capacity, bool for_backward);
+// The blend forward of V views on the state stage 1 and the binning left (ranges, launch order, point_list, records):
+// the render_fwd launch of srf_views_forward, arguments checked by the caller.  record = false: forward-only.
+int views_blend(cudaStream_t stream, int V, int P, int image_height, int image_width, size_t capacity,
+                const void* geom_state, const void* tile_state, const uint32_t* point_list, void* image_state,
+                const float* cams, float* out_color, float* out_others, bool record);
+
 cudaError_t launch_preprocess_fwd(const PreprocessArgs& a, cudaStream_t stream);
 cudaError_t launch_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present,
                                 cudaStream_t stream);

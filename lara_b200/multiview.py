@@ -24,6 +24,7 @@ from typing import Dict, Optional, Sequence
 import torch
 
 from . import _lib
+from ._lib import _DeviceGuard, _ptr
 from . import rasterizer as R
 from .epilogue import epilogue_views_backward_raw, epilogue_views_forward_raw
 
@@ -43,7 +44,7 @@ def shared_view_settings(settings_list: Sequence[R.GaussianRasterizationSettings
 
 
 def _scene_views_forward(centers, shs, opacity, scales, rotations, rays, settings_list, depth_ratio, raw_activations,
-                         for_backward):
+                         for_backward, keep_list=False):
     """Checks, the V-view rasterizer forward and the fused epilogue.  Returns the outputs (image, depth, acc, rn, dn,
     dist, radii) and what the backward needs: (inputs, rays, cams, color, allmap, state, geometry)."""
     dev = centers.device
@@ -62,26 +63,47 @@ def _scene_views_forward(centers, shs, opacity, scales, rotations, rays, setting
     cams = R.pack_cameras(settings_list, dev)
     color, allmap, radii, state = R.forward_views_raw(
         centers_c, shs_c, None, opac_c, scales_c, rot_c, None, cams, tfx, tfy, H, W, deg,
-        prefiltered=prefiltered, debug=debug, raw_activations=raw_activations, for_backward=for_backward)
+        prefiltered=prefiltered, debug=debug, raw_activations=raw_activations, for_backward=for_backward,
+        keep_list=keep_list)
+    return ((*_epilogue_forward(color, allmap, rays_c, cams, depth_ratio), radii),
+            ((centers_c, shs_c, scales_c, rot_c), rays_c, cams, color, allmap, state, (H, W, tfx, tfy, deg, debug)))
+
+
+def _epilogue_forward(color, allmap, rays_c, cams, depth_ratio):
+    """The six render_img outputs of the rasterizer's stacked color / allmap (only the clamped image without rays)."""
+    V, _, H, W = color.shape
 
     def new(*shape):
-        return torch.empty(shape, dtype=torch.float32, device=dev)
+        return torch.empty(shape, dtype=torch.float32, device=color.device)
     if rays_c is not None:
         image, depth, acc = new(V, 3, H, W), new(V, 1, H, W), new(V, H, W)
         rn, dn, dist = new(V, 3, H, W), new(V, 3, H, W), new(V, H, W)
         epilogue_views_forward_raw(color, allmap, rays_c, cams, depth_ratio, image, depth, acc, rn, dn, dist)
     else:
         image = color.clamp(0, 1)
-        depth = acc = rn = dn = dist = centers_c.new_empty(0)
-    return ((image, depth, acc, rn, dn, dist, radii),
-            ((centers_c, shs_c, scales_c, rot_c), rays_c, cams, color, allmap, state, (H, W, tfx, tfy, deg, debug)))
+        depth = acc = rn = dn = dist = color.new_empty(0)
+    return image, depth, acc, rn, dn, dist
+
+
+def _epilogue_backward(color, allmap, rays, cams, depth_ratio, has_rays, g_image, g_depth, g_acc, g_rn, g_dn, g_dist):
+    """dL/dcolor and dL/dallmap from the gradients of the six outputs of :func:`_epilogue_forward`."""
+    if has_rays:
+        c = _lib._contig
+        return epilogue_views_backward_raw(color, allmap, rays, cams, depth_ratio, c(g_image), c(g_depth), c(g_acc),
+                                           c(g_rn), c(g_dn), c(g_dist))
+    gi = g_image if g_image is not None else torch.zeros_like(color)
+    d_color = (gi * ((color >= 0) & (color <= 1))).contiguous()      # vjp of clamp(0, 1)
+    return d_color, torch.zeros_like(allmap)
 
 
 class _RenderSceneViews(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, centers, shs, opacity, scales, rotations, rays, settings_list, depth_ratio, raw_activations):
+    def forward(ctx, centers, shs, opacity, scales, rotations, rays, settings_list, depth_ratio, raw_activations,
+                keep=None):
         outs, (inputs, rays_c, cams, color, allmap, state, geometry) = _scene_views_forward(
             centers, shs, opacity, scales, rotations, rays, settings_list, depth_ratio, raw_activations, True)
+        if keep is not None:
+            keep.append((inputs[0], rays_c, cams, state, geometry))
         centers_c, shs_c, scales_c, rot_c = inputs
         radii = outs[-1]
         ctx.save_for_backward(centers_c, shs_c, scales_c, rot_c, rays_c if rays_c is not None else centers_c.new_empty(0),
@@ -100,38 +122,47 @@ class _RenderSceneViews(torch.autograd.Function):
         centers, shs, scales, rot, rays, cams, color, allmap, radii, _geom, _tile, _image = ctx.saved_tensors
         H, W, tfx, tfy, deg, debug = ctx.geometry
 
-        if ctx.has_rays:
-            c = _lib._contig
-            d_color, d_allmap = epilogue_views_backward_raw(
-                color, allmap, rays, cams, ctx.depth_ratio, c(g_image), c(g_depth), c(g_acc), c(g_rn), c(g_dn), c(g_dist))
-        else:
-            gi = g_image if g_image is not None else torch.zeros_like(color)
-            d_color = (gi * ((color >= 0) & (color <= 1))).contiguous()      # vjp of clamp(0, 1)
-            d_allmap = torch.zeros_like(allmap)
+        d_color, d_allmap = _epilogue_backward(color, allmap, rays, cams, ctx.depth_ratio, ctx.has_rays, g_image, g_depth,
+                                               g_acc, g_rn, g_dn, g_dist)
         g = R.backward_views_raw(ctx.state, radii, centers, shs, None, scales, rot, None, cams, tfx, tfy, H, W, deg,
                                  d_color, d_allmap, need_means2D=False, raw_activations=ctx.raw_activations, debug=debug)
         return (g["means3D"], g["sh"], g["opacities"].view(ctx.opac_shape), g["scales"], g["rotations"],
-                None, None, None, None)
+                None, None, None, None, None)
 
 
 def render_scene_views(centers, shs, opacity, scales, rotations, settings_list: Sequence[R.GaussianRasterizationSettings],
                        rays: Optional[torch.Tensor] = None, depth_ratio: float = 0.0, raw_activations: bool = False,
-                       streams: int = 1, prex: str = "") -> Dict[str, torch.Tensor]:
+                       streams: int = 1, prex: str = "", keep_binning: bool = False) -> Dict[str, object]:
     """All views of one scene: returns stacked per-view results, ``{key+prex: [V, H, W, C] or [V, H, W]}`` with
     the keys, channel-last layout and values of ``Renderer.render_img``'s dict (renderer_2dgs.py:256-268) plus
     ``radii+prex`` [V, P]; ``out[k][j]`` is what the j-th ``render_img`` call of network.py:486-495 returns.
     ``rays=None``: only ``image`` as [V,3,H,W] (render_img's early return is the clamped planar image).
     ``streams`` is accepted for compatibility and ignored: the views share one launch set now.
     When no gradient can flow (``torch.no_grad()``, ``torch.inference_mode()``, no input requiring grad) the views
-    take the forward-only path: the same values, without the backward's state and without an autograd node."""
+    take the forward-only path: the same values, without the backward's state and without an autograd node.
+    ``keep_binning=True`` adds ``out["binning"+prex]``, an opaque :class:`SceneBinning` that
+    :func:`render_subset_views` renders a masked subset of these Gaussians from."""
     if len(settings_list) == 0:
         raise ValueError("render_scene_views needs at least one view")
     args = (centers, shs, opacity, scales, rotations, rays, list(settings_list), float(depth_ratio), bool(raw_activations))
+    keep = [] if keep_binning else None
     if R.needs_backward(centers, shs, opacity, scales, rotations, rays):
-        image, depth, acc, rn, dn, dist, radii = _RenderSceneViews.apply(*args)
+        image, depth, acc, rn, dn, dist, radii = _RenderSceneViews.apply(*args, keep)
     else:
-        (image, depth, acc, rn, dn, dist, radii), _ = _scene_views_forward(*args, False)
-    if rays is None:          # render_img's early return hands back the clamped [3,H,W] image, not a dict
+        (image, depth, acc, rn, dn, dist, radii), (inputs, rays_c, cams, _, _, state, geometry) = _scene_views_forward(
+            *args, False, keep_list=keep_binning)
+        if keep is not None:
+            keep.append((inputs[0], rays_c, cams, state, geometry))
+    out = _out_dict(image, depth, acc, rn, dn, dist, radii, rays is not None, prex)
+    if keep_binning:
+        means, rays_c, cams, state, geometry = keep[0]
+        out["binning" + prex] = SceneBinning(state, radii, means, cams, geometry, rays_c, float(depth_ratio),
+                                             bool(raw_activations), (centers, shs, opacity, scales, rotations))
+    return out
+
+
+def _out_dict(image, depth, acc, rn, dn, dist, radii, has_rays, prex):
+    if not has_rays:          # render_img's early return hands back the clamped [3,H,W] image, not a dict
         return {f"image{prex}": image, f"radii{prex}": radii}
     return {
         f"image{prex}": image.permute(0, 2, 3, 1), f"depth{prex}": depth.permute(0, 2, 3, 1), f"acc_map{prex}": acc,
@@ -140,12 +171,146 @@ def render_scene_views(centers, shs, opacity, scales, rotations, settings_list: 
     }
 
 
+class SceneBinning:
+    """What a ``render_scene_views(..., keep_binning=True)`` call leaves for :func:`render_subset_views`: the coarse
+    forward's state (records, depths, tile rectangles, radii and depth-sorted tile lists of every view), its cameras,
+    settings, rays, ``depth_ratio`` and ``raw_activations`` flag, and the five Gaussian tensors with their
+    ``_version`` at the call.  Opaque: hand it to :func:`render_subset_views` as it is."""
+    __slots__ = ("state", "radii", "means", "cams", "geometry", "rays", "depth_ratio", "raw_activations", "tensors",
+                 "versions")
+
+    def __init__(self, state, radii, means, cams, geometry, rays, depth_ratio, raw_activations, tensors):
+        self.state, self.radii, self.means, self.cams, self.geometry = state, radii, means, cams, geometry
+        self.rays, self.depth_ratio, self.raw_activations, self.tensors = rays, depth_ratio, raw_activations, tensors
+        # inference tensors keep no version counter (None: not checked)
+        self.versions = tuple(None if t.is_inference() else t._version for t in tensors + (radii,))
+
+    def check_unchanged(self):
+        for name, t, v in zip(("centers", "shs", "opacity", "scales", "rotations", "radii"), self.tensors + (self.radii,),
+                              self.versions):
+            if v is not None and t._version != v:
+                raise RuntimeError(f"render_subset_views: the coarse {name} was modified in place after the coarse "
+                                   "render_scene_views call, so its binning no longer describes these Gaussians")
+
+
+def _subset_forward(b: SceneBinning, idx, shs_c, for_backward):
+    """srf_views_subset_forward on the coarse state and the fused epilogue.  Returns the outputs (image, depth, acc, rn,
+    dn, dist, radii) and (color, allmap, state) for the backward."""
+    lib = _lib.load()
+    st = b.state
+    dev = b.means.device
+    H, W, _, _, deg, debug = b.geometry
+    V, P, n, M = st.nviews, int(b.means.shape[0]), int(idx.numel()), int(shs_c.shape[1])
+    color = torch.empty((V, 3, H, W), dtype=torch.float32, device=dev)
+    allmap = torch.empty((V, 8, H, W), dtype=torch.float32, device=dev)
+    radii = torch.empty((V, n), dtype=torch.int32, device=dev)
+    if n == 0:
+        # what a forward of zero Gaussians returns (rasterizer._forward): zero-filled outputs, nothing rendered
+        color.zero_(); allmap.zero_()
+        geom_b, tile_b, image_b = R._views_sizes(lib, V, 0, H, W, 0, for_backward)[:3]
+        image = torch.zeros(image_b, dtype=torch.uint8, device=dev) if for_backward else None
+        pl = torch.empty((0,), dtype=torch.int32, device=dev)
+        state = R.ForwardState(R._blob(geom_b, dev), torch.zeros(tile_b, dtype=torch.uint8, device=dev), image,
+                               pl if for_backward else None, 0, 0, nviews=V, cams=b.cams, for_backward=for_backward)
+    else:
+        counts = st.resolve()       # capacity verified (stage 2 re-run if it overflowed) before the lists are read
+        capacity = st.capacity
+        geom_b, tile_b, image_b, _, pl_b = R._views_sizes(lib, V, n, H, W, capacity, for_backward)[:5]
+        blob = R._blob(geom_b + tile_b + image_b, dev)
+        geom, tile = blob[:geom_b], blob[geom_b:geom_b + tile_b]
+        image = blob[geom_b + tile_b:] if for_backward else None
+        point_list = R._blob(pl_b, dev)
+        _lib.launch(
+            "srf_views_subset_forward", dev, V, P, n, int(deg), M, idx.data_ptr(), b.means.data_ptr(), shs_c.data_ptr(),
+            None, b.cams.data_ptr(), H, W, capacity, b.radii.data_ptr(), st.geom.data_ptr(), st.tile.data_ptr(),
+            st.point_list.data_ptr(), capacity, 1 if st.for_backward else 0, radii.data_ptr(), geom.data_ptr(),
+            tile.data_ptr(), point_list.data_ptr(), _ptr(image), color.data_ptr(), allmap.data_ptr(),
+            R._blob(_lib.subset_workspace_bytes(lib, P), dev).data_ptr(), 1 if for_backward else 0)
+        # the kept entries sit at the coarse list positions: the list's extent is the coarse one
+        state = R.ForwardState(geom, tile, image, point_list if for_backward else None, capacity, counts, nviews=V,
+                               cams=b.cams, for_backward=for_backward)
+        if debug:
+            torch.cuda.synchronize(dev)
+    return ((*_epilogue_forward(color, allmap, b.rays, b.cams, b.depth_ratio), radii), (color, allmap, state))
+
+
+class _RenderSubsetViews(torch.autograd.Function):
+    """Inputs: the full-size coarse centers, opacity, scales and rotations and ``shs_fine``; the gradients of the coarse
+    tensors are the subset's in rows ``idx`` and zero elsewhere."""
+
+    @staticmethod
+    def forward(ctx, binning, idx, shs_c, centers, opacity, scales, rotations):
+        outs, (color, allmap, state) = _subset_forward(binning, idx, shs_c, True)
+        radii = outs[-1]
+        ctx.save_for_backward(idx, shs_c, centers, scales, rotations, color, allmap, radii, state.geom, state.tile,
+                              state.image)
+        ctx.binning, ctx.state, ctx.opac_shape = binning, state, tuple(opacity.shape)
+        ctx.mark_non_differentiable(radii)
+        return outs
+
+    @staticmethod
+    def backward(ctx, g_image, g_depth, g_acc, g_rn, g_dn, g_dist, _g_radii):
+        idx, shs, centers, scales, rotations, color, allmap, radii, _geom, _tile, _image = ctx.saved_tensors
+        b = ctx.binning
+        H, W, tfx, tfy, deg, debug = b.geometry
+        d_color, d_allmap = _epilogue_backward(color, allmap, b.rays, b.cams, b.depth_ratio, b.rays is not None,
+                                               g_image, g_depth, g_acc, g_rn, g_dn, g_dist)
+        # the per-Gaussian backward reads the n rows of the subset (a gather, exact); its gradients go to rows idx
+        rows = [t.index_select(0, idx).contiguous() for t in (centers, scales, rotations)]
+        g = R.backward_views_raw(ctx.state, radii, rows[0], shs, None, rows[1], rows[2], None, b.cams, tfx, tfy, H, W,
+                                 deg, d_color, d_allmap, need_means2D=False, raw_activations=b.raw_activations,
+                                 debug=debug)
+
+        def scatter(gn, shape):
+            full = torch.zeros(shape, dtype=torch.float32, device=idx.device)
+            if idx.numel():
+                full.view(shape[0], -1)[idx] = gn.view(idx.numel(), -1)      # idx is unique: an exact copy per row
+            return full
+        return (None, None, g["sh"], scatter(g["means3D"], tuple(centers.shape)), scatter(g["opacities"], ctx.opac_shape),
+                scatter(g["scales"], tuple(scales.shape)), scatter(g["rotations"], tuple(rotations.shape)))
+
+
+def render_subset_views(binning: SceneBinning, mask: torch.Tensor, shs_fine: torch.Tensor,
+                        prex: str = "_fine") -> Dict[str, torch.Tensor]:
+    """LaRa's fine-pass render (network.py:486-525 with ``_centers[mask]``, ``_opacity_coarse[i][mask]``, ...) from the
+    coarse pass's binning: ``binning`` is ``out["binning"]`` of ``render_scene_views(..., keep_binning=True)``, ``mask``
+    a bool tensor [P] on the Gaussians' device, ``shs_fine`` the subset's SH coefficients [n, M, 3].  Returns the dict
+    ``render_scene_views`` returns for the gathered subset (same keys, layout and bits, ``radii`` [V, n]) without a
+    preprocess, scatter or sort: the coarse records are copied with a new colour and the coarse tile lists filtered to
+    the mask.  One host sync (the ``nonzero`` of the mask).  The gradients of the coarse centers, opacity, scales and
+    rotations are those of the gathered path; under ``no_grad`` / ``inference_mode`` the forward-only path is taken."""
+    if not isinstance(binning, SceneBinning):
+        raise TypeError("render_subset_views: binning must be out['binning'] of render_scene_views(..., keep_binning=True)")
+    binning.check_unchanged()
+    centers, _, opacity, scales, rotations = binning.tensors
+    P, dev = int(binning.means.shape[0]), binning.means.device
+    if not isinstance(mask, torch.Tensor) or mask.dtype != torch.bool or tuple(mask.shape) != (P,) or mask.device != dev:
+        raise RuntimeError(f"render_subset_views: mask must be a bool tensor [{P}] on {dev}, got "
+                           f"{getattr(mask, 'dtype', type(mask))} {tuple(getattr(mask, 'shape', ()))} on "
+                           f"{getattr(mask, 'device', None)}")
+    deg = binning.geometry[4]
+    if not isinstance(shs_fine, torch.Tensor) or shs_fine.dtype != torch.float32 or shs_fine.device != dev or \
+            shs_fine.ndim != 3 or shs_fine.shape[2] != 3 or shs_fine.shape[1] < (deg + 1) ** 2:
+        raise RuntimeError(f"render_subset_views: shs_fine must be float32 [n, M >= {(deg + 1) ** 2}, 3] on {dev}, got "
+                           f"{getattr(shs_fine, 'dtype', type(shs_fine))} {tuple(getattr(shs_fine, 'shape', ()))}")
+    idx = mask.nonzero().view(-1)
+    if shs_fine.shape[0] != idx.numel():
+        raise RuntimeError(f"render_subset_views: shs_fine has {shs_fine.shape[0]} rows, the mask selects {idx.numel()}")
+    shs_c = shs_fine.contiguous()
+    with _DeviceGuard(dev):
+        if R.needs_backward(centers, shs_fine, opacity, scales, rotations):
+            outs = _RenderSubsetViews.apply(binning, idx, shs_c, centers, opacity, scales, rotations)
+        else:
+            outs = _subset_forward(binning, idx, shs_c, False)[0]
+    return _out_dict(*outs, binning.rays is not None, prex)
+
+
 def concat_views(out: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
     """The layout LaRa's step hands to the loss: ``torch.cat([frame[k] for frame in views], dim=1)``
     (network.py:525), i.e. the views side by side along the width."""
     res = {}
     for k, t in out.items():
-        if k.startswith("radii"):
+        if k.startswith("radii") or not isinstance(t, torch.Tensor):     # radii, the kept binning
             continue
         if t.ndim == 4:      # [V,H,W,C] -> [H, V*W, C]
             V, H, W, C = t.shape

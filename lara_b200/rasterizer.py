@@ -286,26 +286,27 @@ def forward_raw(means3D, shs, colors_precomp, opacities, scales, rotations, tran
 def forward_views_raw(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp,
                       cams: torch.Tensor, tanfovx: float, tanfovy: float, H: int, W: int, sh_degree: int,
                       prefiltered: bool = False, debug: bool = False, raw_activations: bool = False, *,
-                      for_backward: bool = True):
+                      for_backward: bool = True, keep_list: bool = False):
     """All V views of one Gaussian set in ONE launch set (srf_views_*): every kernel carries a view
     dimension.  `cams` is the [V, 24] device tensor of camera records (pack_cameras).
     Returns (color [V,3,H,W], allmap [V,8,H,W], radii [V,P], ForwardState with V back-to-back workspaces).
     ``for_backward=False``: the forward-only forward (srf_views_forward with for_backward = 0), bit-identical outputs
-    without the blend's contribution record and image state; the returned state cannot feed :func:`backward_views_raw`."""
+    without the blend's contribution record and image state; the returned state cannot feed :func:`backward_views_raw`.
+    ``keep_list``: a forward-only state keeps its point list too (the tile lists a subset render filters)."""
     with _DeviceGuard(means3D.device):
         if cams.dtype != torch.float32 or not cams.is_cuda or cams.shape[1] != _lib.CAM_FLOATS or not cams.is_contiguous():
             raise RuntimeError(f"cams must be a contiguous float32 CUDA tensor [V,{_lib.CAM_FLOATS}]")
         return _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp, cams, tanfovx,
                         tanfovy, H, W, sh_degree, prefiltered, debug, raw_activations, single=False,
-                        for_backward=for_backward)
+                        for_backward=for_backward, keep_list=keep_list)
 
 
 def _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp, cams, tanfovx, tanfovy,
-             H, W, sh_degree, prefiltered, debug, raw_activations, single, for_backward):
+             H, W, sh_degree, prefiltered, debug, raw_activations, single, for_backward, keep_list=False):
     """srf_views_forward on the current stream: stage 1 (preprocess + tile scan + async count read-back) and stage 2
     (binning + blend) with an optimistic capacity, then an event for whoever eventually asks for the instance counts.
     `single`: one view, with the outputs in the reference's one-view shapes.  `for_backward` False: the forward-only
-    forward and its smaller workspaces, no image state or point list kept."""
+    forward and its smaller workspaces, no image state and, unless `keep_list`, no point list kept."""
     lib = _lib.load()
     device = means3D.device
     V, P = int(cams.shape[0]), int(means3D.shape[0])
@@ -326,7 +327,8 @@ def _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMa
         # reference: zero-filled outputs, nothing rendered (rasterize_points.cu:92-94,105)
         color.zero_(); allmap.zero_(); tile.zero_()
         if not for_backward:
-            return color, allmap, radii, ForwardState(geom, tile, None, None, 0, 0, nviews=V, cams=cams,
+            pl = torch.empty((0,), dtype=torch.int32, device=device) if keep_list else None
+            return color, allmap, radii, ForwardState(geom, tile, None, pl, 0, 0, nviews=V, cams=cams,
                                                       for_backward=False)
         image.zero_()
         pl = torch.empty((0,), dtype=torch.int32, device=device)
@@ -348,8 +350,8 @@ def _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMa
         radii.data_ptr(), geom.data_ptr(), tile.data_ptr(), _blob(ent_b, device).data_ptr(), point_list.data_ptr(),
         _ptr(image), color.data_ptr(), allmap.data_ptr(), slot.data_ptr(), ev.cuda_event,
         1 if raw_activations else 0, 1 if for_backward else 0)
-    state = ForwardState(geom, tile, image, point_list if for_backward else None, capacity, nviews=V, cams=cams,
-                         for_backward=for_backward)
+    state = ForwardState(geom, tile, image, point_list if for_backward or keep_list else None, capacity, nviews=V,
+                         cams=cams, for_backward=for_backward)
 
     def rerun(new_capacity: int):
         # enqueued on whatever stream is current: a deferred re-run happens on the caller's stream
@@ -359,7 +361,7 @@ def _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMa
                     _blob(e_b, device).data_ptr(), pl2.data_ptr(), _ptr(image), cams.data_ptr(), color.data_ptr(),
                     allmap.data_ptr(), 1 if for_backward else 0)
         state.capacity = new_capacity
-        if for_backward:
+        if for_backward or keep_list:
             state.point_list = pl2
 
     pend = _Pending(device, rb, V, capacity, rerun)

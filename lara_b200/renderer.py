@@ -83,11 +83,12 @@ class Renderer(nn.Module):
         return render_img_epilogue(rendered_image, allmap, rays, cam.world_view_transform, depth_ratio, prex)
 
     def render_views(self, cams, rays, centers, shs, opacity, scales, rotations, device, bg_colors=None,
-                     prex: str = "", depth_ratio: float = 0.0, streams: int = 3):
+                     prex: str = "", depth_ratio: float = 0.0, streams: int = 3, keep_binning: bool = False):
         """All target views of one scene in one autograd node (the loop of network.py:486-495):
         ``cams`` a sequence of MiniCam-like objects, ``rays`` [V,H,W,6] (or None), ``bg_colors`` an
         optional [V,3] / sequence of per-view backgrounds (network.py:489-490), default ``self.bg_color``.
-        Returns stacked ``{key: [V,H,W,C]}``; ``lara_b200.multiview.concat_views`` gives network.py:525's layout."""
+        Returns stacked ``{key: [V,H,W,C]}``; ``lara_b200.multiview.concat_views`` gives network.py:525's layout.
+        ``keep_binning``: also ``out["binning"+prex]``, from which :meth:`render_subset_views` renders the fine pass."""
         from .multiview import render_scene_views
         settings = []
         for j, cam in enumerate(cams):
@@ -100,4 +101,10 @@ class Renderer(nn.Module):
             scales = self.scaling_activation(scales)
             rotations = self.rotation_activation(rotations)
         return render_scene_views(centers, shs, opacity, scales, rotations, settings, rays=rays, depth_ratio=depth_ratio,
-                                  raw_activations=fuse, streams=streams, prex=prex)
+                                  raw_activations=fuse, streams=streams, prex=prex, keep_binning=keep_binning)
+
+    def render_subset_views(self, binning, mask, shs_fine, prex: str = "_fine"):
+        """The fine pass over ``mask`` of the Gaussians a ``render_views(..., keep_binning=True)`` call rendered, with
+        the SH coefficients ``shs_fine``: ``lara_b200.multiview.render_subset_views``."""
+        from .multiview import render_subset_views
+        return render_subset_views(binning, mask, shs_fine, prex=prex)
