@@ -130,6 +130,18 @@ SIGNATURES = {
                                          _P, _P, _P, _P,                             # norm w, b, mlp w, b
                                          _P, _P,                                     # dL_dout, workspace
                                          _P, _P, _P, _P, _P, _P]),                   # the six gradients
+    # include/surfel_vol_transformer.h
+    "srf_group_attn_forward": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int,   # stream, B, R, g, S, C, H
+                                       _P, _P, _P, _P]),                             # q, k, v, o
+    "srf_group_attn_backward": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int,
+                                        _P, _P, _P, _P,                              # q, k, v, dL_do
+                                        _P, _P, _P]),                                # dL_dq, dL_dk, dL_dv
+    "srf_add_layernorm_forward": (c_int, [_P, c_int, c_int, c_float,                 # stream, rows, C, eps
+                                          _P, _P, _P, _P, _P, _P]),                  # a, b, gamma, beta, y, n
+    "srf_add_layernorm_workspace_bytes": (c_int, [c_int, c_int, POINTER(c_size_t)]),
+    "srf_add_layernorm_backward": (c_int, [_P, c_int, c_int, c_float,
+                                           _P, _P, _P, _P, _P,                       # y, gamma, dL_dn, dL_dy, workspace
+                                           _P, _P, _P]),                             # dL_da, d_gamma, d_beta
     "srf_profile_begin": (c_int, []),
     "srf_profile_end": (c_int, [POINTER(c_float), POINTER(c_int), c_int]),
 }
@@ -275,6 +287,11 @@ def fine_head_workspace_bytes(lib, n: int, V: int, D: int, sh_dim: int, gather: 
 def feat_volume_workspace_bytes(lib, B: int, V: int, C: int, h: int, w: int, R: int, E: int) -> int:
     """Workspace of srf_feat_volume_forward / _backward."""
     return _size_query(lib.srf_feat_volume_workspace_bytes, B, V, C, h, w, R, E)
+
+
+def add_layernorm_workspace_bytes(lib, rows: int, C: int) -> int:
+    """Workspace of srf_add_layernorm_backward."""
+    return _size_query(lib.srf_add_layernorm_workspace_bytes, rows, C)
 
 
 def int3(v) -> ctypes.Array:
