@@ -7,6 +7,7 @@ from .rasterizer import (  # noqa: F401
     rasterize_gaussians,
     _RasterizeGaussians,
 )
+from .coarse_head import CoarseHead  # noqa: F401
 
-__all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians"]
+__all__ = ["GaussianRasterizationSettings", "GaussianRasterizer", "rasterize_gaussians", "CoarseHead"]
 __version__ = "0.1.0"

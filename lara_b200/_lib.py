@@ -117,6 +117,16 @@ SIGNATURES = {
                                        _P, _P,                                        # dL_dsh, workspace
                                        _P, _P, _P,                                    # dL_dvolume_feat, _dpoint_feats, _dshs
                                        _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),      # the ten parameter gradients
+    # include/surfel_coarse_head.h
+    "srf_coarse_head_forward": (c_int, [_P, c_int, c_int, c_int, c_int, c_int,      # stream, rows, N, D, K, sh_dim
+                                        c_float, c_float, c_float,                  # opacity / scaling shift, half_cell
+                                        _P, _P, _P, _P, _P, _P, _P, _P,             # feats, group_centers, w0 .. b2
+                                        _P, _P, _P, _P, _P]),                       # the five outputs
+    "srf_coarse_head_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, POINTER(c_size_t)]),
+    "srf_coarse_head_backward": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_float,   # stream .. sh_dim, half_cell
+                                         _P, _P, _P, _P, _P, _P, _P, _P,            # feats, group_centers, w0 .. b2
+                                         _P, _P, _P, _P, _P, _P,                    # the five upstreams, workspace
+                                         _P, _P, _P, _P, _P, _P, _P]),              # dL_dfeats, the six gradients
     # include/surfel_feat_volume.h
     "srf_feat_volume_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_size_t)]),
     "srf_feat_volume_forward": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, c_int,   # stream, B, V, C, h, w, R, E
@@ -282,6 +292,11 @@ def deterministic(requested: Optional[bool] = None) -> bool:
 def fine_head_workspace_bytes(lib, n: int, V: int, D: int, sh_dim: int, gather: bool) -> int:
     """Workspace of srf_fine_head_backward on the current device."""
     return _size_query(lib.srf_fine_head_workspace_bytes, n, V, D, sh_dim, 1 if gather else 0)
+
+
+def coarse_head_workspace_bytes(lib, rows: int, D: int, K: int, sh_dim: int) -> int:
+    """Workspace of srf_coarse_head_backward on the current device."""
+    return _size_query(lib.srf_coarse_head_workspace_bytes, rows, D, K, sh_dim)
 
 
 def feat_volume_workspace_bytes(lib, B: int, V: int, C: int, h: int, w: int, R: int, E: int) -> int:
