@@ -184,6 +184,63 @@ int srf_views_backward(srf_stream_t stream, int V, int P, int D, int M, int imag
                        int raw_activations, int deterministic);
 int srf_views_backward_deterministic_scratch_bytes(int V, int P, size_t* bytes);
 
+/* ---- S scenes in one launch set (a training batch; DESIGN §3.21) -------------------------------------------------
+ * S scenes of Vs views each, every scene its own Gaussians, are laid out as one srf_views_* call of V = S*Vs views:
+ * view v (camera record v of `cams` [S*Vs, SRF_CAM_FLOATS], workspace slot v, output image v) belongs to scene v / Vs.
+ * The views of one scene share its field of view, tan_fov[2s] (x) and tan_fov[2s+1] (y), a host array [S,2] of finite
+ * positive values; all views share the image size and the SH degree.  Each view's outputs and state are bit-identical
+ * to those of srf_views_forward / srf_views_subset_forward on that scene alone, and each scene's gradient rows to those
+ * of srf_views_backward on that scene alone (with deterministic != 0; otherwise up to the order of float atomics).
+ * 0 < S <= SRF_MAX_SCENES, Vs > 0, S*Vs <= 65535.  Every argument check is made before anything is enqueued.
+ *
+ * srf_scenes_forward: srf_views_forward on S scenes.  Gaussian inputs [S,P,...] (means3D [S,P,3], shs [S,P,M,3], ...);
+ * radii [S*Vs,P]; workspaces sized by srf_views_workspace_bytes(S*Vs, P, ...); num_rendered_host holds S*Vs counts.
+ * Its stage-2 re-run is srf_views_forward_render with V = S*Vs, which reads no Gaussian input.
+ *
+ * srf_scenes_subset_forward: srf_views_subset_forward on S scenes with ragged subsets.  `offsets` (device int64 [S+1],
+ * from 0, non-decreasing, ending at n) splits `idx` [n], the concatenation of the S strictly ascending index lists,
+ * into scene s's idx[offsets[s] .. offsets[s+1]) (indices into that scene's P Gaussians); shs [n,M,3] is concatenated
+ * the same way; means3D [S,P,3] are the coarse centers.  The subset state is laid out as S*Vs views of n_max Gaussians
+ * each (n_max >= every scene's count, <= P): radii [S*Vs,n_max], workspaces srf_views_workspace_bytes(S*Vs, n_max,
+ * ...), `workspace` srf_views_subset_workspace_bytes(S*P); view v holds scene v / Vs's subset in its first slots.  The
+ * entry reads `offsets` back to check it, so it waits for the stream.
+ *
+ * srf_scenes_backward: srf_views_backward on the state of either forward.  It takes `P` (Gaussians per view slot) and
+ * `offsets`: NULL for srf_scenes_forward's state (scene s's inputs and gradient rows are [s*P, (s+1)*P) of [S,P,...]
+ * arrays), or the subset forward's offsets with P = n_max (scene s's rows are [offsets[s], offsets[s+1]) of the
+ * concatenated [n,...] arrays: the gathered subset inputs, as for srf_views_backward on a subset).  Each scene's rows
+ * sum that scene's Vs views only, in view order.  With offsets it reads them back to check them (waits for the
+ * stream).  Scratch sizes are those of V = S*Vs views of P Gaussians.                                                */
+#define SRF_MAX_SCENES 128
+int srf_scenes_forward(srf_stream_t stream, int S, int Vs, int P, int D, int M,
+                       const float* means3D, const float* shs, const float* colors_precomp,
+                       const float* opacities, const float* scales, const float* rotations,
+                       const float* transMat_precomp, const float* cams, const float* tan_fov,
+                       int image_height, int image_width, int prefiltered,
+                       size_t capacity, int* radii, void* geom_state, void* tile_state, void* entries,
+                       uint32_t* point_list, void* image_state, float* out_color, float* out_others,
+                       uint32_t* num_rendered_host, void* count_event, int raw_activations, int for_backward);
+int srf_scenes_subset_forward(srf_stream_t stream, int S, int Vs, int P, int n, int n_max, int D, int M,
+                              const int64_t* idx, const int64_t* offsets, const float* means3D, const float* shs,
+                              const float* colors_precomp, const float* cams, int image_height, int image_width,
+                              size_t capacity, const int* coarse_radii, const void* coarse_geom_state,
+                              const void* coarse_tile_state, const uint32_t* coarse_point_list, size_t coarse_capacity,
+                              int coarse_for_backward, int* radii, void* geom_state, void* tile_state,
+                              uint32_t* point_list, void* image_state, float* out_color, float* out_others,
+                              void* workspace, int for_backward);
+int srf_scenes_backward(srf_stream_t stream, int S, int Vs, int P, const int64_t* offsets, int D, int M,
+                        int image_height, int image_width, size_t capacity, const float* cams,
+                        const float* means3D, const float* shs, int colors_were_precomputed,
+                        const float* scales, const float* rotations, int transmat_was_precomputed,
+                        const float* tan_fov, const int* radii,
+                        const void* geom_state, const void* tile_state, const uint32_t* point_list,
+                        const void* image_state,
+                        const float* dL_dout_color, const float* dL_dout_others,
+                        void* scratch, int accumulate,
+                        float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
+                        float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
+                        int raw_activations, int deterministic);
+
 /* ---- fused render_img epilogue (next-row: lightning/renderer_2dgs.py:220-268, :74-89) ---------
  * One pass over the rasterizer's outputs of V stacked views instead of ~12 torch ops (and ~20 autograd
  * ops) per view: image = clamp(color,0,1); acc_map = alpha; rend_normal = viewmatrix[:3,:3] . normal;

@@ -78,6 +78,37 @@ SIGNATURES = {
         _P, _P, _P, c_int,                  # out_color, out_others, workspace, for_backward
     ]),
     "srf_views_subset_workspace_bytes": (c_int, [c_int, POINTER(c_size_t)]),
+    "srf_scenes_forward": (c_int, [
+        _P, c_int, c_int, c_int, c_int, c_int,  # stream, S, Vs, P, D, M
+        _P, _P, _P,                         # means3D, shs, colors_precomp
+        _P, _P, _P,                         # opacities, scales, rotations
+        _P, _P, _P,                         # transMat_precomp, cams, tan_fov (host float [S,2])
+        c_int, c_int, c_int, c_size_t,      # H, W, prefiltered, capacity
+        _P, _P, _P, _P, _P, _P,             # radii, geom_state, tile_state, entries, point_list, image_state
+        _P, _P, _P, _P,                     # out_color, out_others, num_rendered_host, count_event
+        c_int, c_int,                       # raw_activations, for_backward
+    ]),
+    "srf_scenes_subset_forward": (c_int, [
+        _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int,  # stream, S, Vs, P, n, n_max, D, M
+        _P, _P, _P, _P, _P, _P,             # idx, offsets, means3D, shs, colors_precomp, cams
+        c_int, c_int, c_size_t,             # H, W, capacity
+        _P, _P, _P, _P, c_size_t, c_int,    # coarse radii, geom_state, tile_state, point_list, capacity, for_backward
+        _P, _P, _P, _P, _P,                 # radii, geom_state, tile_state, point_list, image_state
+        _P, _P, _P, c_int,                  # out_color, out_others, workspace, for_backward
+    ]),
+    "srf_scenes_backward": (c_int, [
+        _P, c_int, c_int, c_int, _P, c_int, c_int,   # stream, S, Vs, P, offsets, D, M
+        c_int, c_int, c_size_t, _P,              # H, W, capacity, cams
+        _P, _P, c_int,                           # means3D, shs, colors_were_precomputed
+        _P, _P, c_int,                           # scales, rotations, transmat_was_precomputed
+        _P, _P,                                  # tan_fov (host float [S,2]), radii
+        _P, _P, _P, _P,                          # geom_state, tile_state, point_list, image_state
+        _P, _P,                                  # dL_dout_color, dL_dout_others
+        _P, c_int,                               # scratch, accumulate
+        _P, _P, _P, _P,                          # dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors
+        _P, _P, _P, _P,                          # dL_dopacity, dL_dscales, dL_drotations, dL_dtransMat
+        c_int, c_int,                            # raw_activations, deterministic
+    ]),
     "srf_views_backward_deterministic_scratch_bytes": (c_int, [c_int, c_int, POINTER(c_size_t)]),
     "srf_views_epilogue_forward": (c_int, [_P, c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "srf_views_epilogue_backward": (c_int, [_P, c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
@@ -255,6 +286,11 @@ def _size_query(fn, *args) -> int:
 def det_backward_scratch_bytes(lib, V: int, P: int) -> int:
     """Scratch of srf_views_backward(..., deterministic=1)."""
     return _size_query(lib.srf_views_backward_deterministic_scratch_bytes, V, P)
+
+
+def tan_fov_array(tan_fov) -> ctypes.Array:
+    """The host float [S,2] tan_fov of the srf_scenes_* entries from a sequence of (tan_fovx, tan_fovy)."""
+    return (c_float * (2 * len(tan_fov)))(*(float(v) for xy in tan_fov for v in xy))
 
 
 def subset_workspace_bytes(lib, P: int) -> int:

@@ -3,6 +3,7 @@
 // stage-2 re-run, backward, srf_mark_visible).  The fused ops' entries are defined next to their kernels.
 // Plain pointers and sizes in, int status out; only enqueues work on the given stream.
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdarg.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -161,6 +162,41 @@ StateLayout state_layout(int P, int H, int W) {
 
 size_t plist_stride(size_t capacity, bool for_backward) { return plist_stride_bytes(capacity, for_backward); }
 
+int check_scenes(const char* fn, int S, int Vs) {
+    if (S <= 0 || Vs <= 0) return set_error("%s: need S > 0 scenes of Vs > 0 views, got S = %d, Vs = %d", fn, S, Vs);
+    if (S > SRF_MAX_SCENES) return set_error("%s: S = %d scenes exceeds SRF_MAX_SCENES = %d", fn, S, SRF_MAX_SCENES);
+    if ((int64_t)S * Vs > 65535) return set_error("%s: S * Vs = %lld views exceeds 65535", fn, (long long)S * Vs);
+    return 0;
+}
+
+int scene_fov(const char* fn, int S, const float* tan_fov, int image_height, int image_width, SceneArgs& s) {
+    if (!tan_fov) return set_error("%s: null tan_fov", fn);
+    for (int i = 0; i < S; ++i) {
+        const float tx = tan_fov[2 * i], ty = tan_fov[2 * i + 1];
+        if (!isfinite(tx) || !isfinite(ty) || !(tx > 0.f) || !(ty > 0.f))
+            return set_error("%s: tan_fov of scene %d is (%g, %g), not finite and positive", fn, i, tx, ty);
+        // the focal lengths of srf_views_forward / _backward, rasterizer_impl.cu:223-224
+        s.fov[i] = make_float4(image_width / (2.0f * tx), image_height / (2.0f * ty), tx, ty);
+    }
+    return 0;
+}
+
+int check_offsets(const char* fn, cudaStream_t stream, int S, const int64_t* offsets, int n_max, int n) {
+    if (!offsets) return set_error("%s: null offsets", fn);
+    int64_t h[SRF_MAX_SCENES + 1];
+    cudaError_t e = cudaMemcpyAsync(h, offsets, (size_t)(S + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+    if (e != cudaSuccess) return cuda_error("offsets read-back", e);
+    if (h[0] != 0) return set_error("%s: offsets[0] = %lld, not 0", fn, (long long)h[0]);
+    for (int i = 0; i < S; ++i) {
+        if (h[i + 1] < h[i]) return set_error("%s: offsets decrease at scene %d", fn, i);
+        if (h[i + 1] - h[i] > n_max)
+            return set_error("%s: scene %d has %lld Gaussians, more than %d", fn, i, (long long)(h[i + 1] - h[i]), n_max);
+    }
+    if (n >= 0 && h[S] != n) return set_error("%s: offsets end at %lld, not at n = %d", fn, (long long)h[S], n);
+    return 0;
+}
+
 int views_blend(cudaStream_t stream, int V, int P, int image_height, int image_width, size_t capacity,
                 const void* geom_state, const void* tile_state, const uint32_t* point_list, void* image_state,
                 const float* cams, float* out_color, float* out_others, bool record) {
@@ -296,7 +332,7 @@ int forward_preprocess_impl(cudaStream_t stream, int V, int P, int D, int M,
                             const float* transMat_precomp, const float* cams,
                             float tan_fovx, float tan_fovy, int image_height, int image_width,
                             int prefiltered, int* radii, void* geom_state, void* tile_state,
-                            uint32_t* num_rendered_host, int raw_activations) {
+                            uint32_t* num_rendered_host, int raw_activations, const srf::SceneArgs* scenes) {
     const TileLayout tl = tile_layout(image_height, image_width);
     // tile blocks + counters of every view are zeroed by one 2-D memset
     cudaError_t e = cudaMemset2DAsync(at<char>(tile_state, tl.count), tl.total, 0,
@@ -327,7 +363,7 @@ int forward_preprocess_impl(cudaStream_t stream, int V, int P, int D, int M,
         a.tile_count = b.tile_count;
         a.geom_stride = gl.total;
         a.tile_stride = b.tile_stride;
-        e = srf::launch_preprocess_fwd(a, stream);
+        e = scenes ? srf::launch_preprocess_fwd_scenes(a, *scenes, stream) : srf::launch_preprocess_fwd(a, stream);
         if (e != cudaSuccess) return cuda_error("preprocess_fwd launch", e);
     }
     // num_rendered read-back: pinned host memory is device-visible under UVA, so the scan kernel stores the counts there
@@ -409,7 +445,7 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
                   void* scratch, int accumulate,
                   float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
                   float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
-                  int raw_activations, bool deterministic) {
+                  int raw_activations, bool deterministic, const srf::SceneArgs* scenes = nullptr, int S = 1) {
     if (!cams) return set_error("%s: null camera records", fn);
     if (V <= 0 || P < 0 || image_height <= 0 || image_width <= 0) return set_error("%s: bad sizes", fn);
     if (P == 0) return 0;
@@ -483,7 +519,7 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
     p.dL_dsh = p.M > 0 ? dL_dsh : nullptr;
     p.dL_dcolors = dL_dcolors; p.dL_dopacity = dL_dopacity;
     p.dL_dscales = dL_dscales; p.dL_drotations = dL_drotations; p.dL_dtransMat = dL_dtransMat;
-    e = srf::launch_preprocess_bwd(p, stream);
+    e = scenes ? srf::launch_preprocess_bwd_scenes(p, *scenes, S, stream) : srf::launch_preprocess_bwd(p, stream);
     if (e != cudaSuccess) return cuda_error("preprocess_bwd launch", e);
     return deterministic ? srf::check_overflow_flag(fn, overflow, stream) : 0;
 }
@@ -510,7 +546,7 @@ int srf_views_forward(srf_stream_t stream_, int V, int P, int D, int M,
         return 1;
     int rc = forward_preprocess_impl(stream, V, P, D, M, means3D, shs, colors_precomp, opacities, scales, rotations,
                                      transMat_precomp, cams, tan_fovx, tan_fovy, image_height, image_width, prefiltered,
-                                     radii, geom_state, tile_state, num_rendered_host, raw_activations);
+                                     radii, geom_state, tile_state, num_rendered_host, raw_activations, nullptr);
     if (rc != 0) return rc;
     if (count_event) {      // lets the caller wait for the instance counts without waiting for the blend
         cudaError_t e = cudaEventRecord(static_cast<cudaEvent_t>(count_event), stream);
@@ -550,6 +586,68 @@ int srf_views_backward(srf_stream_t stream_, int V, int P, int D, int M, int ima
                          image_state, dL_dout_color, dL_dout_others, scratch, accumulate, dL_dmeans3D, dL_dmeans2D,
                          dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drotations, dL_dtransMat, raw_activations,
                          deterministic != 0);
+}
+
+int srf_scenes_forward(srf_stream_t stream_, int S, int Vs, int P, int D, int M,
+                       const float* means3D, const float* shs, const float* colors_precomp,
+                       const float* opacities, const float* scales, const float* rotations,
+                       const float* transMat_precomp, const float* cams, const float* tan_fov,
+                       int image_height, int image_width, int prefiltered,
+                       size_t capacity, int* radii, void* geom_state, void* tile_state, void* entries,
+                       uint32_t* point_list, void* image_state, float* out_color, float* out_others,
+                       uint32_t* num_rendered_host, void* count_event, int raw_activations, int for_backward) {
+    const char* fn = "srf_scenes_forward";
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    srf::SceneArgs scenes;
+    if (srf::check_scenes(fn, S, Vs) || srf::scene_fov(fn, S, tan_fov, image_height, image_width, scenes)) return 1;
+    scenes.views_per_scene = Vs;
+    scenes.offsets = nullptr;
+    const int V = S * Vs;
+    if (forward_preprocess_check(fn, V, P, D, M, means3D, shs, colors_precomp, opacities, scales, rotations,
+                                 transMat_precomp, image_height, image_width, radii, geom_state, tile_state) ||
+        forward_render_check(fn, V, P, image_height, image_width, capacity, geom_state, tile_state, entries, point_list,
+                             image_state, cams, out_color, out_others, for_backward != 0))
+        return 1;
+    if ((size_t)S * P > 0x7fffffffull) return set_error("%s: S * P exceeds 32-bit Gaussian indices", fn);
+    int rc = forward_preprocess_impl(stream, V, P, D, M, means3D, shs, colors_precomp, opacities, scales, rotations,
+                                     transMat_precomp, cams, scenes.fov[0].z, scenes.fov[0].w, image_height, image_width,
+                                     prefiltered, radii, geom_state, tile_state, num_rendered_host, raw_activations,
+                                     &scenes);
+    if (rc != 0) return rc;
+    if (count_event) {
+        cudaError_t e = cudaEventRecord(static_cast<cudaEvent_t>(count_event), stream);
+        if (e != cudaSuccess) return cuda_error("count event record", e);
+    }
+    return forward_render_impl(stream, V, P, image_height, image_width, capacity, geom_state, tile_state, entries,
+                               point_list, image_state, cams, out_color, out_others, for_backward != 0);
+}
+
+int srf_scenes_backward(srf_stream_t stream_, int S, int Vs, int P, const int64_t* offsets, int D, int M,
+                        int image_height, int image_width, size_t capacity, const float* cams,
+                        const float* means3D, const float* shs, int colors_were_precomputed,
+                        const float* scales, const float* rotations, int transmat_was_precomputed,
+                        const float* tan_fov, const int* radii,
+                        const void* geom_state, const void* tile_state, const uint32_t* point_list,
+                        const void* image_state,
+                        const float* dL_dout_color, const float* dL_dout_others,
+                        void* scratch, int accumulate,
+                        float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
+                        float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
+                        int raw_activations, int deterministic) {
+    const char* fn = "srf_scenes_backward";
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    srf::SceneArgs scenes;
+    if (srf::check_scenes(fn, S, Vs) || srf::scene_fov(fn, S, tan_fov, image_height, image_width, scenes)) return 1;
+    if (P < 0) return set_error("%s: bad sizes", fn);
+    if (!offsets && (size_t)S * P > 0x7fffffffull) return set_error("%s: S * P exceeds 32-bit Gaussian indices", fn);
+    if (offsets && P > 0 && srf::check_offsets(fn, stream, S, offsets, P, -1)) return 1;
+    scenes.views_per_scene = Vs;
+    scenes.offsets = offsets;
+    return backward_impl(fn, stream, S * Vs, P, D, M, image_height, image_width, capacity, cams, means3D, shs,
+                         colors_were_precomputed, scales, rotations, transmat_was_precomputed, scenes.fov[0].z,
+                         scenes.fov[0].w, radii, geom_state, tile_state, point_list, image_state, dL_dout_color,
+                         dL_dout_others, scratch, accumulate, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity,
+                         dL_dscales, dL_drotations, dL_dtransMat, raw_activations, deterministic != 0, &scenes, S);
 }
 
 int srf_views_backward_deterministic_scratch_bytes(int V, int P, size_t* bytes) {

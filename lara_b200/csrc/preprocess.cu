@@ -14,6 +14,8 @@
 #include <cuda_fp16.h>
 #include <stdio.h>
 
+#include <type_traits>
+
 #include "surfel_common.cuh"
 #include "surfel_kernels.h"
 #include "sh_eval.cuh"
@@ -35,13 +37,23 @@ __device__ __forceinline__ void stage_rows(float* __restrict__ dst, const float*
     }
 }
 
+template <typename T>
+__device__ __forceinline__ const T* rows_at(const T* p, size_t row, int width) {
+    return p ? p + row * width : p;
+}
+
 // Adds one instance to every tile of rect [x0,x1) x [y0,y1).
 __device__ __forceinline__ void count_tiles_serial(uint32_t* tile_count, int gx, int x0, int y0, int x1, int y1) {
     for (int y = y0; y < y1; ++y)
         for (int x = x0; x < x1; ++x) atomicAdd(&tile_count[(size_t)(y * gx + x) * SRF_TILE_CTR_STRIDE], 1u);
 }
 
-__global__ void __launch_bounds__(256) preprocess_fwd_kernel(PreprocessArgs a) {
+// Without scenes (srf_views_forward) the kernel takes an empty second argument; with scenes (srf_scenes_forward) the
+// view's scene gives the Gaussian rows and the field of view.
+struct NoScenes {};
+
+template <typename Scenes>
+__global__ void __launch_bounds__(256) preprocess_fwd_kernel(PreprocessArgs a, const __grid_constant__ Scenes s) {
     __shared__ __align__(16) float s_means[256 * 3];
     __shared__ float s_view[16];
     __shared__ float s_cam[3];
@@ -61,6 +73,19 @@ __global__ void __launch_bounds__(256) preprocess_fwd_kernel(PreprocessArgs a) {
         a.depths = view_ptr(a.depths, view, a.geom_stride);
         a.rects = view_ptr(a.rects, view, a.geom_stride);
         a.tile_count = view_ptr(a.tile_count, view, a.tile_stride);
+        if constexpr (!std::is_same<Scenes, NoScenes>::value) {
+            const int scene = view / s.views_per_scene;
+            const size_t row = (size_t)scene * a.P;
+            a.means3D = rows_at(a.means3D, row, 3);
+            a.scales = rows_at(a.scales, row, 2);
+            a.rotations = rows_at(a.rotations, row, 4);
+            a.opacities = rows_at(a.opacities, row, 1);
+            a.shs = rows_at(a.shs, row, 3 * a.M);
+            a.transMat_precomp = rows_at(a.transMat_precomp, row, 9);
+            a.colors_precomp = rows_at(a.colors_precomp, row, 3);
+            a.focal_x = s.fov[scene].x;
+            a.focal_y = s.fov[scene].y;
+        }
     }
 
     stage_rows(s_means, a.means3D + (size_t)base * 3, nrows * 3, tid, 256);
@@ -320,7 +345,8 @@ __global__ void __launch_bounds__(256) mark_visible_kernel(int P, const float* _
     present[idx] = (pvz <= 0.2f) ? 0 : 1;
 }
 
-cudaError_t launch_preprocess_fwd(const PreprocessArgs& a, cudaStream_t stream) {
+template <typename Scenes>
+static cudaError_t launch_preprocess(const PreprocessArgs& a, const Scenes& s, cudaStream_t stream) {
     if (a.P <= 0 || a.nviews <= 0) return cudaSuccess;
     PreprocessArgs args = a;
     const size_t sh_bytes = (size_t)256 * 3 * a.M * sizeof(float);
@@ -332,9 +358,17 @@ cudaError_t launch_preprocess_fwd(const PreprocessArgs& a, cudaStream_t stream) 
     const size_t dyn = args.stage_sh ? sh_bytes : 0;
     const int grid = (a.P + 255) / 256;
     prof_start(K_PREPROCESS_FWD, stream);
-    preprocess_fwd_kernel<<<dim3(grid, a.nviews), 256, dyn, stream>>>(args);
+    preprocess_fwd_kernel<Scenes><<<dim3(grid, a.nviews), 256, dyn, stream>>>(args, s);
     prof_stop(K_PREPROCESS_FWD, stream);
     return cudaGetLastError();
+}
+
+cudaError_t launch_preprocess_fwd(const PreprocessArgs& a, cudaStream_t stream) {
+    return launch_preprocess(a, NoScenes(), stream);
+}
+
+cudaError_t launch_preprocess_fwd_scenes(const PreprocessArgs& a, const SceneArgs& s, cudaStream_t stream) {
+    return launch_preprocess(a, s, stream);
 }
 
 cudaError_t launch_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present,

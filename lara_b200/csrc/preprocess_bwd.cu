@@ -8,6 +8,8 @@
 // zeros for culled Gaussians -- so the host never pre-fills nine zero tensors as the
 // reference does (rasterize_points.cu:194-202).  With accumulate=1 the kernel adds into
 // the outputs instead (view-sharded accumulation before the NCCL all-reduce).
+#include <type_traits>
+
 #include "surfel_common.cuh"
 #include "surfel_kernels.h"
 
@@ -44,10 +46,52 @@ __device__ __forceinline__ void put2(float* p, float2 v) {   // p must be 8-byte
     *q = v;
 }
 
-template <bool ACC>
-__global__ void __launch_bounds__(256) preprocess_bwd_kernel(PreprocessBwdArgs a) {
+template <typename T>
+__device__ __forceinline__ T* rows_at(T* p, size_t row, int width) {
+    return p ? p + row * width : p;
+}
+
+// Without scenes (srf_views_backward) the kernel takes an empty second argument.  With scenes (srf_scenes_backward) it
+// runs one thread per (Gaussian, scene = blockIdx.y) and sums that scene's Vs views: the scene gives the rows of the
+// inputs and outputs, the first view and the field of view.
+struct NoScenes {};
+
+template <bool ACC, typename Scenes>
+__global__ void __launch_bounds__(256) preprocess_bwd_kernel(PreprocessBwdArgs a, const __grid_constant__ Scenes s) {
     const int idx = blockIdx.x * 256 + threadIdx.x;
-    if (idx >= a.P) return;
+    if constexpr (std::is_same<Scenes, NoScenes>::value) {
+        if (idx >= a.P) return;
+    } else {
+        const int scene = blockIdx.y;
+        size_t row = (size_t)scene * a.P;
+        int n = a.P;
+        if (s.offsets) {
+            row = (size_t)s.offsets[scene];
+            n = (int)(s.offsets[scene + 1] - s.offsets[scene]);
+        }
+        const int v0 = scene * s.views_per_scene;
+        a.nviews = s.views_per_scene;
+        a.radii += (size_t)v0 * a.P;
+        a.rec = view_ptr(a.rec, v0, a.geom_stride);
+        a.ggrad = view_ptr(a.ggrad, v0, a.ggrad_stride);
+        a.viewmatrix += (size_t)v0 * a.cam_stride;
+        a.campos += (size_t)v0 * a.cam_stride;
+        a.focal_x = s.fov[scene].x; a.focal_y = s.fov[scene].y;
+        a.tan_fovx = s.fov[scene].z; a.tan_fovy = s.fov[scene].w;
+        a.means3D = rows_at(a.means3D, row, 3);
+        a.scales = rows_at(a.scales, row, 2);
+        a.rotations = rows_at(a.rotations, row, 4);
+        a.shs = rows_at(a.shs, row, 3 * a.M);
+        a.dL_dmeans3D = rows_at(a.dL_dmeans3D, row, 3);
+        a.dL_dmeans2D = rows_at(a.dL_dmeans2D, row, 3);
+        a.dL_dsh = rows_at(a.dL_dsh, row, 3 * a.M);
+        a.dL_dcolors = rows_at(a.dL_dcolors, row, 3);
+        a.dL_dopacity = rows_at(a.dL_dopacity, row, 1);
+        a.dL_dscales = rows_at(a.dL_dscales, row, 2);
+        a.dL_drotations = rows_at(a.dL_drotations, row, 4);
+        a.dL_dtransMat = rows_at(a.dL_dtransMat, row, 9);
+        if (idx >= n) return;
+    }
     const int M3 = 3 * a.M;
 
     // sums over the views of the call (one view in the drop-in path)
@@ -333,19 +377,29 @@ __global__ void __launch_bounds__(256) preprocess_bwd_kernel(PreprocessBwdArgs a
     }
 }
 
-cudaError_t launch_preprocess_bwd(const PreprocessBwdArgs& a, cudaStream_t stream) {
+template <typename Scenes>
+static cudaError_t launch(const PreprocessBwdArgs& a, const Scenes& s, int S, cudaStream_t stream) {
     if (a.P <= 0 || a.nviews <= 0) return cudaSuccess;
-    const int grid = (a.P + 255) / 256;
+    const dim3 grid((a.P + 255) / 256, S);
     PreprocessBwdArgs args = a;
+    // every row is a whole number of 16-byte rotation / 8-byte scale / (M = 4) 48-byte SH rows from the base
     auto al = [](const void* p, uintptr_t n) { return (reinterpret_cast<uintptr_t>(p) & (n - 1)) == 0; };
     args.vec_ok = (al(a.dL_drotations, 16) && al(a.dL_dscales, 8) && (a.dL_dsh == nullptr || al(a.dL_dsh, 16))) ? 1 : 0;
     prof_start(K_PREPROCESS_BWD, stream);
     if (a.accumulate)
-        preprocess_bwd_kernel<true><<<grid, 256, 0, stream>>>(args);
+        preprocess_bwd_kernel<true, Scenes><<<grid, 256, 0, stream>>>(args, s);
     else
-        preprocess_bwd_kernel<false><<<grid, 256, 0, stream>>>(args);
+        preprocess_bwd_kernel<false, Scenes><<<grid, 256, 0, stream>>>(args, s);
     prof_stop(K_PREPROCESS_BWD, stream);
     return cudaGetLastError();
+}
+
+cudaError_t launch_preprocess_bwd(const PreprocessBwdArgs& a, cudaStream_t stream) {
+    return launch(a, NoScenes(), 1, stream);
+}
+
+cudaError_t launch_preprocess_bwd_scenes(const PreprocessBwdArgs& a, const SceneArgs& s, int S, cudaStream_t stream) {
+    return launch(a, s, S, stream);
 }
 
 }  // namespace srf

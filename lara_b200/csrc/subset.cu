@@ -34,8 +34,10 @@ T* at(const void* base, size_t off) {
 
 struct RecordsArgs {
     int P, n, D, M;
-    const int64_t* idx;            // [n] ascending coarse indices
-    const float* means3D;          // [P,3] coarse centers
+    int n_slot, views_per_scene;   // Gaussians per view of the subset state; views per scene
+    const int64_t* offsets;        // [S+1]: scene s's subset is idx[offsets[s] .. offsets[s+1]); null: one scene
+    const int64_t* idx;            // [n] ascending coarse indices per scene
+    const float* means3D;          // [S,P,3] coarse centers
     const float* shs;              // [n,M,3]
     const float* cams;             // [V, SRF_CAM_FLOATS]
     const int* c_radii;            // [V,P]
@@ -43,22 +45,24 @@ struct RecordsArgs {
     const float* c_depths;
     const uint2* c_rects;
     size_t c_geom_stride;
-    int* radii;                    // [V,n] out
+    int* radii;                    // [V,n_slot] out
     float4* rec;
     float* depths;
     uint2* rects;
     size_t geom_stride;
-    uint32_t* rank;                // [P], kNoRank outside the subset
+    uint32_t* rank;                // [S,P], kNoRank outside the subset
 };
 
 __global__ void __launch_bounds__(256) subset_records_kernel(RecordsArgs a) {
     const int j = blockIdx.x * 256 + threadIdx.x;
     const int view = blockIdx.y;
-    if (j >= a.n) return;
-    const int64_t g = a.idx[j];
-    if (view == 0) a.rank[g] = (uint32_t)j;
+    const int scene = view / a.views_per_scene;
+    const int64_t first = a.offsets ? a.offsets[scene] : 0;
+    if (j >= (a.offsets ? a.offsets[scene + 1] - first : a.n)) return;
+    const int64_t g = a.idx[first + j];
+    if (view == scene * a.views_per_scene) a.rank[(size_t)scene * a.P + g] = (uint32_t)j;
     const int radius = a.c_radii[(size_t)view * a.P + g];
-    a.radii[(size_t)view * a.n + j] = radius;
+    a.radii[(size_t)view * a.n_slot + j] = radius;
     view_ptr(a.rects, view, a.geom_stride)[j] = view_ptr(a.c_rects, view, a.c_geom_stride)[g];
     if (radius == 0) return;      // culled: the preprocess writes no record and no depth either
     const float4* cq = view_ptr(a.c_rec, view, a.c_geom_stride) + (size_t)g * SRF_REC_QUADS;
@@ -67,12 +71,13 @@ __global__ void __launch_bounds__(256) subset_records_kernel(RecordsArgs a) {
     view_ptr(a.depths, view, a.geom_stride)[j] = view_ptr(a.c_depths, view, a.c_geom_stride)[g];
     // q4 exactly as preprocess_fwd_kernel writes it: normalised view direction, SH -> RGB, clamp bits
     const float* campos = a.cams + (size_t)view * SRF_CAM_FLOATS + SRF_CAM_CAMPOS;
-    const float px = a.means3D[3 * g + 0], py = a.means3D[3 * g + 1], pz = a.means3D[3 * g + 2];
+    const float* mean = a.means3D + 3 * ((size_t)scene * a.P + g);
+    const float px = mean[0], py = mean[1], pz = mean[2];
     float dx = fadd_(px, -campos[0]), dy = fadd_(py, -campos[1]), dz = fadd_(pz, -campos[2]);
     const float len = __fsqrt_rn(fma_(dz, dz, fma_(dx, dx, fmul_(dy, dy))));
     dx = __fdiv_rn(dx, len); dy = __fdiv_rn(dy, len); dz = __fdiv_rn(dz, len);
     float rgb[3];
-    sh_to_rgb(a.D, a.shs + (size_t)j * 3 * a.M, dx, dy, dz, rgb);
+    sh_to_rgb(a.D, a.shs + (size_t)(first + j) * 3 * a.M, dx, dy, dz, rgb);
     int clampbits = 0;
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
@@ -84,8 +89,9 @@ __global__ void __launch_bounds__(256) subset_records_kernel(RecordsArgs a) {
 
 struct FilterArgs {
     int n, ntiles;
+    int P, views_per_scene;
     uint32_t capacity;
-    const uint32_t* rank;
+    const uint32_t* rank;          // [S,P]
     const uint2* c_ranges;
     const uint32_t* c_order;
     const uint32_t* c_counters;
@@ -106,6 +112,7 @@ __global__ void __launch_bounds__(256) subset_filter_kernel(FilterArgs a) {
     if (t >= a.ntiles) return;
     const uint2 cr = view_ptr(a.c_ranges, view, a.c_tile_stride)[t];
     const uint32_t* src = view_ptr(a.c_plist, view, a.c_plist_stride);
+    const uint32_t* rank = a.rank + (size_t)(view / a.views_per_scene) * a.P;
     uint32_t* dst = view_ptr(a.plist, view, a.plist_stride) + cr.x;
     const uint32_t below = (1u << lane) - 1u;
     uint32_t kept = 0;
@@ -121,7 +128,7 @@ __global__ void __launch_bounds__(256) subset_filter_kernel(FilterArgs a) {
             r[k] = i < end ? src[i] : kNoRank;
         }
 #pragma unroll
-        for (int k = 0; k < kFilterChunks; ++k) r[k] = r[k] != kNoRank ? a.rank[r[k]] : kNoRank;
+        for (int k = 0; k < kFilterChunks; ++k) r[k] = r[k] != kNoRank ? rank[r[k]] : kNoRank;
 #pragma unroll
         for (int k = 0; k < kFilterChunks; ++k) {
             const uint32_t keep = __ballot_sync(0xffffffffu, r[k] != kNoRank);
@@ -142,32 +149,21 @@ __global__ void __launch_bounds__(256) subset_filter_kernel(FilterArgs a) {
 size_t rank_bytes(int P) { return align_up((size_t)(P > 0 ? P : 1) * sizeof(uint32_t)); }
 
 }  // namespace
-}  // namespace srf
 
-using srf::misaligned;
-using srf::set_error;
-
-extern "C" {
-
-int srf_views_subset_workspace_bytes(int P, size_t* bytes) {
-    if (P < 0 || !bytes) return set_error("srf_views_subset_workspace_bytes: bad arguments");
-    *bytes = srf::rank_bytes(P);
-    return 0;
-}
-
-int srf_views_subset_forward(srf_stream_t stream_, int V, int P, int n, int D, int M,
-                             const int64_t* idx, const float* means3D, const float* shs, const float* colors_precomp,
-                             const float* cams, int image_height, int image_width, size_t capacity,
-                             const int* coarse_radii, const void* coarse_geom_state, const void* coarse_tile_state,
-                             const uint32_t* coarse_point_list, size_t coarse_capacity, int coarse_for_backward,
-                             int* radii, void* geom_state, void* tile_state, uint32_t* point_list, void* image_state,
-                             float* out_color, float* out_others, void* workspace, int for_backward) {
-    const char* fn = "srf_views_subset_forward";
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+// srf_views_subset_forward and srf_scenes_subset_forward: S scenes of Vs views, scene s's subset idx[offsets[s] ..
+// offsets[s+1]) of its P coarse Gaussians (offsets null: S = 1, the n Gaussians idx[0..n)), n_slot Gaussians per view of
+// the subset state.  The caller has checked S, Vs, the offsets and n_slot.
+int subset_forward(const char* fn, cudaStream_t stream, int S, int Vs, int P, int n, int n_slot, const int64_t* offsets,
+                   int D, int M, const int64_t* idx, const float* means3D, const float* shs, const float* colors_precomp,
+                   const float* cams, int image_height, int image_width, size_t capacity,
+                   const int* coarse_radii, const void* coarse_geom_state, const void* coarse_tile_state,
+                   const uint32_t* coarse_point_list, size_t coarse_capacity, int coarse_for_backward,
+                   int* radii, void* geom_state, void* tile_state, uint32_t* point_list, void* image_state,
+                   float* out_color, float* out_others, void* workspace, int for_backward) {
+    const int V = S * Vs;
     // every check before anything is enqueued
-    if (V <= 0 || P < 0 || n < 0 || image_height <= 0 || image_width <= 0) return set_error("%s: bad sizes", fn);
+    if (P < 0 || n < 0 || image_height <= 0 || image_width <= 0) return set_error("%s: bad sizes", fn);
     if (image_height > 16 * 65535 || image_width > 16 * 65535) return set_error("%s: image too large", fn);
-    if (n > P) return set_error("%s: the subset has n = %d > P = %d Gaussians", fn, n, P);
     if (D < 0 || D > 3) return set_error("%s: sh degree must be in [0,3]", fn);
     if (colors_precomp) return set_error("%s: colors_precomp is not supported: the subset's colour comes from shs", fn);
     if (capacity != coarse_capacity)
@@ -190,15 +186,16 @@ int srf_views_subset_forward(srf_stream_t stream_, int V, int P, int n, int D, i
         return set_error("%s: tile_state, point_list and image_state (and the coarse ones) must be 256-byte aligned", fn);
 
     const srf::StateLayout cl = srf::state_layout(P, image_height, image_width);
-    const srf::StateLayout sl = srf::state_layout(n, image_height, image_width);
+    const srf::StateLayout sl = srf::state_layout(n_slot, image_height, image_width);
     uint32_t* rank = static_cast<uint32_t*>(workspace);
     cudaError_t e;
     if (n > 0) {
-        e = cudaMemsetAsync(rank, 0xff, (size_t)P * sizeof(uint32_t), stream);
+        e = cudaMemsetAsync(rank, 0xff, (size_t)S * P * sizeof(uint32_t), stream);
         if (e != cudaSuccess) return srf::cuda_error("memset rank", e);
         srf::RecordsArgs r;
         memset(&r, 0, sizeof(r));
         r.P = P; r.n = n; r.D = D; r.M = M;
+        r.n_slot = n_slot; r.views_per_scene = Vs; r.offsets = offsets;
         r.idx = idx; r.means3D = means3D; r.shs = shs; r.cams = cams;
         r.c_radii = coarse_radii;
         r.c_rec = srf::at<const float4>(coarse_geom_state, cl.rec);
@@ -211,13 +208,14 @@ int srf_views_subset_forward(srf_stream_t stream_, int V, int P, int n, int D, i
         r.rects = srf::at<uint2>(geom_state, sl.rects);
         r.geom_stride = sl.geom_stride;
         r.rank = rank;
-        srf::subset_records_kernel<<<dim3((n + 255) / 256, V), 256, 0, stream>>>(r);
+        srf::subset_records_kernel<<<dim3((n_slot + 255) / 256, V), 256, 0, stream>>>(r);
         e = cudaGetLastError();
         if (e != cudaSuccess) return srf::cuda_error("subset_records launch", e);
     }
     srf::FilterArgs f;
     memset(&f, 0, sizeof(f));
     f.n = n; f.ntiles = cl.ntiles; f.capacity = (uint32_t)capacity;
+    f.P = P; f.views_per_scene = Vs;
     f.rank = rank;
     f.c_ranges = srf::at<const uint2>(coarse_tile_state, cl.ranges);
     f.c_order = srf::at<const uint32_t>(coarse_tile_state, cl.order);
@@ -235,8 +233,58 @@ int srf_views_subset_forward(srf_stream_t stream_, int V, int P, int n, int D, i
     srf::subset_filter_kernel<<<dim3((cl.ntiles + 7) / 8, V), 256, 0, stream>>>(f);
     e = cudaGetLastError();
     if (e != cudaSuccess) return srf::cuda_error("subset_filter launch", e);
-    return srf::views_blend(stream, V, n, image_height, image_width, capacity, geom_state, tile_state, point_list,
+    return srf::views_blend(stream, V, n_slot, image_height, image_width, capacity, geom_state, tile_state, point_list,
                             image_state, cams, out_color, out_others, for_backward != 0);
+}
+
+}  // namespace srf
+
+using srf::misaligned;
+using srf::set_error;
+
+extern "C" {
+
+int srf_views_subset_workspace_bytes(int P, size_t* bytes) {
+    if (P < 0 || !bytes) return set_error("srf_views_subset_workspace_bytes: bad arguments");
+    *bytes = srf::rank_bytes(P);
+    return 0;
+}
+
+int srf_views_subset_forward(srf_stream_t stream_, int V, int P, int n, int D, int M,
+                             const int64_t* idx, const float* means3D, const float* shs, const float* colors_precomp,
+                             const float* cams, int image_height, int image_width, size_t capacity,
+                             const int* coarse_radii, const void* coarse_geom_state, const void* coarse_tile_state,
+                             const uint32_t* coarse_point_list, size_t coarse_capacity, int coarse_for_backward,
+                             int* radii, void* geom_state, void* tile_state, uint32_t* point_list, void* image_state,
+                             float* out_color, float* out_others, void* workspace, int for_backward) {
+    const char* fn = "srf_views_subset_forward";
+    if (V <= 0 || P < 0 || n < 0 || image_height <= 0 || image_width <= 0) return set_error("%s: bad sizes", fn);
+    if (n > P) return set_error("%s: the subset has n = %d > P = %d Gaussians", fn, n, P);
+    return srf::subset_forward(fn, static_cast<cudaStream_t>(stream_), 1, V, P, n, n, nullptr, D, M, idx, means3D, shs,
+                               colors_precomp, cams, image_height, image_width, capacity, coarse_radii,
+                               coarse_geom_state, coarse_tile_state, coarse_point_list, coarse_capacity,
+                               coarse_for_backward, radii, geom_state, tile_state, point_list, image_state, out_color,
+                               out_others, workspace, for_backward);
+}
+
+int srf_scenes_subset_forward(srf_stream_t stream_, int S, int Vs, int P, int n, int n_max, int D, int M,
+                              const int64_t* idx, const int64_t* offsets, const float* means3D, const float* shs,
+                              const float* colors_precomp, const float* cams, int image_height, int image_width,
+                              size_t capacity, const int* coarse_radii, const void* coarse_geom_state,
+                              const void* coarse_tile_state, const uint32_t* coarse_point_list, size_t coarse_capacity,
+                              int coarse_for_backward, int* radii, void* geom_state, void* tile_state,
+                              uint32_t* point_list, void* image_state, float* out_color, float* out_others,
+                              void* workspace, int for_backward) {
+    const char* fn = "srf_scenes_subset_forward";
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    if (srf::check_scenes(fn, S, Vs)) return 1;
+    if (P < 0 || n < 0 || n_max < 0 || n_max > P) return set_error("%s: bad sizes", fn);
+    if ((size_t)S * P > 0x7fffffffull) return set_error("%s: S * P exceeds 32-bit Gaussian indices", fn);
+    if (srf::check_offsets(fn, stream, S, offsets, n_max, n)) return 1;
+    return srf::subset_forward(fn, stream, S, Vs, P, n, n_max, offsets, D, M, idx, means3D, shs, colors_precomp, cams,
+                               image_height, image_width, capacity, coarse_radii, coarse_geom_state, coarse_tile_state,
+                               coarse_point_list, coarse_capacity, coarse_for_backward, radii, geom_state, tile_state,
+                               point_list, image_state, out_color, out_others, workspace, for_backward);
 }
 
 }  // extern "C"

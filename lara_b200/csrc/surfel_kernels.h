@@ -14,6 +14,8 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include "../../include/surfel_rasterizer.h"
+
 namespace srf {
 
 // ---- host helpers of the extern "C" entries ----
@@ -148,6 +150,16 @@ struct PreprocessBwdArgs {
     float* dL_dtransMat;         // [P,9] or null
 };
 
+// The scenes of an srf_scenes_* call (include/surfel_rasterizer.h): S scenes of Vs views each, laid out as V = S*Vs
+// views; view v belongs to scene v / Vs.  Passed as a __grid_constant__ kernel parameter (the kernels index `fov` by
+// the scene without a local copy) next to the per-view arguments, whose Gaussian pointers are those of scene 0.
+struct SceneArgs {
+    int views_per_scene;         // Vs
+    const int64_t* offsets;      // [S+1] device: scene s's Gaussians are rows [offsets[s], offsets[s+1]) of the inputs
+                                 //   and gradients; null: rows [s*P, (s+1)*P)
+    float4 fov[SRF_MAX_SCENES];  // per scene: focal_x, focal_y, tan_fovx, tan_fovy
+};
+
 // Optional per-kernel CUDA-event timing (srf_profile_begin/end in the C ABI); no-ops unless enabled.
 enum KernelId { K_PREPROCESS_FWD = 0, K_TILE_SCAN, K_SCATTER, K_SORT_SMALL, K_SORT_BIG, K_RENDER_FWD,
                 K_RENDER_BWD, K_PREPROCESS_BWD, K_COUNT };
@@ -173,6 +185,14 @@ int views_blend(cudaStream_t stream, int V, int P, int image_height, int image_w
                 const void* geom_state, const void* tile_state, const uint32_t* point_list, void* image_state,
                 const float* cams, float* out_color, float* out_others, bool record);
 
+// Argument checks of the srf_scenes_* entries, made before they enqueue anything.  check_scenes: 0 < S <=
+// SRF_MAX_SCENES, Vs > 0, S * Vs <= 65535 (views are a grid dimension).  scene_fov: finite positive tan_fov [S,2]
+// (host) into s.fov.  check_offsets: reads the device array offsets [S+1] (waits for the stream) and checks that it
+// starts at 0, never decreases, puts at most n_max Gaussians in a scene and, if n >= 0, ends at n.
+int check_scenes(const char* fn, int S, int Vs);
+int scene_fov(const char* fn, int S, const float* tan_fov, int image_height, int image_width, SceneArgs& s);
+int check_offsets(const char* fn, cudaStream_t stream, int S, const int64_t* offsets, int n_max, int n);
+
 cudaError_t launch_preprocess_fwd(const PreprocessArgs& a, cudaStream_t stream);
 cudaError_t launch_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present,
                                 cudaStream_t stream);
@@ -188,5 +208,9 @@ size_t det_record_bytes();
 cudaError_t launch_render_bwd_det(const RenderBwdArgs& a, int P, float* ggrad, size_t ggrad_stride, uint32_t* overflow,
                                   cudaStream_t stream);
 cudaError_t launch_preprocess_bwd(const PreprocessBwdArgs& a, cudaStream_t stream);
+// The same kernels over the scenes of `s`: a.nviews = S * Vs views whose Gaussian inputs are those of their scene.  The
+// backward runs one thread per (Gaussian, scene) and sums that scene's Vs views only.
+cudaError_t launch_preprocess_fwd_scenes(const PreprocessArgs& a, const SceneArgs& s, cudaStream_t stream);
+cudaError_t launch_preprocess_bwd_scenes(const PreprocessBwdArgs& a, const SceneArgs& s, int S, cudaStream_t stream);
 
 }  // namespace srf

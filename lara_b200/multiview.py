@@ -319,3 +319,272 @@ def concat_views(out: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
             V, H, W = t.shape
             res[k] = t.permute(1, 0, 2).reshape(H, V * W)
     return res
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# B scenes in one launch set (srf_scenes_*, DESIGN §3.21): the B*V views of a batch are rendered as one V-view call
+# whose preprocess and per-Gaussian backward read each view's Gaussians from its own scene.
+# ---------------------------------------------------------------------------------------------------------------------
+
+def batch_view_settings(settings: Sequence[Sequence[R.GaussianRasterizationSettings]]):
+    """(H, W, [(tanfovx, tanfovy)] per scene, sh_degree, prefiltered, debug) of a batch: each scene's views share what
+    :func:`shared_view_settings` requires, and all scenes share V, the image size and the SH degree."""
+    if len(settings) == 0 or any(len(s) == 0 for s in settings):
+        raise ValueError("render_batch_views needs at least one scene of at least one view")
+    V = len(settings[0])
+    keys = [shared_view_settings(list(s)) for s in settings]
+    for s, k in zip(settings, keys):
+        if len(s) != V:
+            raise RuntimeError("render_batch_views: all scenes of a batch must have the same number of views")
+        if (k[0], k[1], k[4]) != (keys[0][0], keys[0][1], keys[0][4]):
+            raise RuntimeError("render_batch_views: all scenes of a batch must share the image size and the SH degree")
+    return (keys[0][0], keys[0][1], [(k[2], k[3]) for k in keys], keys[0][4], any(k[5] for k in keys),
+            any(k[6] for k in keys))
+
+
+def _batch_inputs(centers, shs, opacity, scales, rotations):
+    """Shape checks of the [B,P,...] Gaussian tensors; returns them fp32 contiguous, opacity as [B,P]."""
+    if not isinstance(centers, torch.Tensor) or centers.ndim != 3 or centers.shape[2] != 3:
+        raise RuntimeError("render_batch_views: centers must be [B,P,3]")
+    B, P = int(centers.shape[0]), int(centers.shape[1])
+    want = {"shs": (shs, 4), "scales": (scales, 3), "rotations": (rotations, 3)}
+    for name, (t, nd) in want.items():
+        if not isinstance(t, torch.Tensor) or t.ndim != nd or tuple(t.shape[:2]) != (B, P):
+            raise RuntimeError(f"render_batch_views: {name} must be [B,P,...] = [{B},{P},...]")
+    if shs.shape[3] != 3 or scales.shape[2] != 2 or rotations.shape[2] != 4:
+        raise RuntimeError("render_batch_views: shs must be [B,P,M,3], scales [B,P,2] and rotations [B,P,4]")
+    if not isinstance(opacity, torch.Tensor) or opacity.numel() != B * P or tuple(opacity.shape[:2]) != (B, P):
+        raise RuntimeError(f"render_batch_views: opacity must be [B,P] or [B,P,1] = [{B},{P}]")
+    return tuple(R._f32c(t, n) for t, n in ((centers, "centers"), (shs, "shs"), (opacity.reshape(B, P), "opacity"),
+                                            (scales, "scales"), (rotations, "rotations")))
+
+
+def _batch_forward(centers, shs, opacity, scales, rotations, rays, settings, depth_ratio, raw_activations, for_backward,
+                   keep_list=False):
+    """Checks, the batched rasterizer forward and the fused epilogue over the B*V views.  Returns the outputs (image,
+    depth, acc, rn, dn, dist, radii), stacked [B*V, ...], and (inputs, rays, cams, color, allmap, state, geometry)."""
+    dev = centers.device
+    inputs = _batch_inputs(centers, shs, opacity, scales, rotations)
+    settings = [[R._check_settings(rs, dev) for rs in s] for s in settings]
+    H, W, tan_fov, deg, prefiltered, debug = batch_view_settings(settings)
+    B, V = len(settings), len(settings[0])
+    rays_c = None
+    if rays is not None:
+        rays_c = rays.contiguous()
+        if rays_c.dtype != torch.float32 or tuple(rays_c.shape) != (B, V, H, W, 6) or rays_c.device != dev:
+            raise RuntimeError(f"rays must be float32 [B,V,H,W,6] = {(B, V, H, W, 6)} on {dev}, got "
+                               f"{rays_c.dtype} {tuple(rays_c.shape)} on {rays_c.device}")
+        rays_c = rays_c.view(B * V, H, W, 6)
+    cams = R.pack_cameras([rs for s in settings for rs in s], dev)
+    centers_c, shs_c, opac_c, scales_c, rot_c = inputs
+    with _DeviceGuard(dev):
+        color, allmap, radii, state = R.forward_batch_raw(
+            centers_c, shs_c, None, opac_c, scales_c, rot_c, None, cams, tan_fov, H, W, deg, prefiltered=prefiltered,
+            debug=debug, raw_activations=raw_activations, for_backward=for_backward, keep_list=keep_list)
+        outs = (*_epilogue_forward(color, allmap, rays_c, cams, depth_ratio), radii)
+    return outs, ((centers_c, shs_c, scales_c, rot_c), rays_c, cams, color, allmap, state, (H, W, tan_fov, deg, debug))
+
+
+class _RenderBatchViews(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, centers, shs, opacity, scales, rotations, rays, settings, depth_ratio, raw_activations, keep=None):
+        outs, (inputs, rays_c, cams, color, allmap, state, geometry) = _batch_forward(
+            centers, shs, opacity, scales, rotations, rays, settings, depth_ratio, raw_activations, True)
+        if keep is not None:
+            keep.append((inputs[0], rays_c, cams, state, geometry))
+        radii = outs[-1]
+        ctx.save_for_backward(*inputs, rays_c if rays_c is not None else color.new_empty(0), cams, color, allmap, radii,
+                              state.geom, state.tile, state.image)
+        ctx.state, ctx.geometry, ctx.has_rays = state, geometry, rays_c is not None
+        ctx.depth_ratio, ctx.raw_activations, ctx.opac_shape = float(depth_ratio), bool(raw_activations), tuple(opacity.shape)
+        ctx.mark_non_differentiable(radii)
+        return outs
+
+    @staticmethod
+    def backward(ctx, g_image, g_depth, g_acc, g_rn, g_dn, g_dist, _g_radii):
+        centers, shs, scales, rot, rays, cams, color, allmap, radii, _geom, _tile, _image = ctx.saved_tensors
+        H, W, tan_fov, deg, debug = ctx.geometry
+        d_color, d_allmap = _epilogue_backward(color, allmap, rays, cams, ctx.depth_ratio, ctx.has_rays, g_image, g_depth,
+                                               g_acc, g_rn, g_dn, g_dist)
+        g = R.backward_batch_raw(ctx.state, radii, centers, shs, scales, rot, cams, tan_fov, H, W, deg, d_color, d_allmap,
+                                 raw_activations=ctx.raw_activations, debug=debug)
+        return (g["means3D"], g["sh"], g["opacities"].view(ctx.opac_shape), g["scales"], g["rotations"],
+                None, None, None, None, None)
+
+
+def _batch_out_dict(outs, B, has_rays, prex):
+    """{key: [B,V,...]} of the [B*V,...] outputs, the layout of :func:`render_scene_views` per scene."""
+    out = _out_dict(*outs, has_rays, prex)
+    return {k: t.view((B, t.shape[0] // B) + tuple(t.shape[1:])) for k, t in out.items()}
+
+
+def render_batch_views(centers, shs, opacity, scales, rotations,
+                       settings: Sequence[Sequence[R.GaussianRasterizationSettings]],
+                       rays: Optional[torch.Tensor] = None, depth_ratio: float = 0.0, raw_activations: bool = False,
+                       prex: str = "", keep_binning: bool = False) -> Dict[str, object]:
+    """All views of all B scenes of a batch in one autograd node and one launch set: ``centers`` [B,P,3], ``shs``
+    [B,P,M,3], ``opacity`` [B,P] or [B,P,1], ``scales`` [B,P,2], ``rotations`` [B,P,4], ``settings[b]`` scene b's V
+    view settings, ``rays`` [B,V,H,W,6] or None.  Returns ``{key+prex: [B,V,...]}``, where ``out[k][b]`` is what
+    :func:`render_scene_views` returns for scene b alone (bit for bit), and ``radii+prex`` [B,V,P].  Scenes may differ
+    in field of view and background; they must share V, the image size and the SH degree.  No-grad renders take the
+    forward-only path.  ``keep_binning=True`` adds ``out["binning"+prex]``, a :class:`BatchBinning` for
+    :func:`render_batch_subset_views`."""
+    settings = [list(s) for s in settings]
+    args = (centers, shs, opacity, scales, rotations, rays, settings, float(depth_ratio), bool(raw_activations))
+    keep = [] if keep_binning else None
+    if R.needs_backward(centers, shs, opacity, scales, rotations, rays):
+        outs = _RenderBatchViews.apply(*args, keep)
+    else:
+        outs, (inputs, rays_c, cams, _, _, state, geometry) = _batch_forward(*args, False, keep_list=keep_binning)
+        if keep is not None:
+            keep.append((inputs[0], rays_c, cams, state, geometry))
+    B = len(settings)
+    out = _batch_out_dict(outs, B, rays is not None, prex)
+    if keep_binning:
+        means, rays_c, cams, state, geometry = keep[0]
+        out["binning" + prex] = BatchBinning(state, outs[-1], means, cams, geometry, rays_c, float(depth_ratio),
+                                             bool(raw_activations), (centers, shs, opacity, scales, rotations))
+    return out
+
+
+class BatchBinning(SceneBinning):
+    """What ``render_batch_views(..., keep_binning=True)`` leaves for :func:`render_batch_subset_views`: a
+    :class:`SceneBinning` of the batch's B*V views, whose ``means`` are [B,P,3] and whose ``geometry`` holds the
+    per-scene fields of view.  Opaque."""
+    __slots__ = ()
+
+
+def _batch_subset_forward(b: BatchBinning, idx, offsets, counts, shs_c, for_backward):
+    """srf_scenes_subset_forward on the coarse state and the fused epilogue.  Returns the outputs (image, depth, acc, rn,
+    dn, dist, radii [B*V, n_max]) and (color, allmap, state, n_max) for the backward."""
+    lib = _lib.load()
+    st = b.state
+    dev = b.means.device
+    H, W, _, deg, debug = b.geometry
+    B, P = int(b.means.shape[0]), int(b.means.shape[1])
+    V, n, M, n_max = st.nviews, int(idx.numel()), int(shs_c.shape[1]), max(counts)
+    color = torch.empty((V, 3, H, W), dtype=torch.float32, device=dev)
+    allmap = torch.empty((V, 8, H, W), dtype=torch.float32, device=dev)
+    radii = torch.empty((V, n_max), dtype=torch.int32, device=dev)
+    st.resolve()       # capacity verified (stage 2 re-run if it overflowed) before the lists are read
+    capacity = st.capacity
+    geom_b, tile_b, image_b, _, pl_b = R._views_sizes(lib, V, n_max, H, W, capacity, for_backward)[:5]
+    blob = R._blob(geom_b + tile_b + image_b, dev)
+    geom, tile = blob[:geom_b], blob[geom_b:geom_b + tile_b]
+    image = blob[geom_b + tile_b:] if for_backward else None
+    point_list = R._blob(pl_b, dev)
+    _lib.launch(
+        "srf_scenes_subset_forward", dev, B, V // B, P, n, n_max, int(deg), M, idx.data_ptr(), offsets.data_ptr(),
+        b.means.data_ptr(), shs_c.data_ptr(), None, b.cams.data_ptr(), H, W, capacity, b.radii.data_ptr(),
+        st.geom.data_ptr(), st.tile.data_ptr(), st.point_list.data_ptr(), capacity, 1 if st.for_backward else 0,
+        radii.data_ptr(), geom.data_ptr(), tile.data_ptr(), point_list.data_ptr(), _ptr(image), color.data_ptr(),
+        allmap.data_ptr(), R._blob(_lib.subset_workspace_bytes(lib, B * P), dev).data_ptr(), 1 if for_backward else 0)
+    Vs = V // B
+    for s, c in enumerate(counts):
+        if c == 0:      # a scene with an empty mask renders what a forward of zero Gaussians renders: zeros
+            color[s * Vs:(s + 1) * Vs].zero_()
+            allmap[s * Vs:(s + 1) * Vs].zero_()
+    state = R.ForwardState(geom, tile, image, point_list if for_backward else None, capacity, st.resolve(), nviews=V,
+                           cams=b.cams, for_backward=for_backward)
+    if debug:
+        torch.cuda.synchronize(dev)
+    return ((*_epilogue_forward(color, allmap, b.rays, b.cams, b.depth_ratio), radii), (color, allmap, state, n_max))
+
+
+class _RenderBatchSubsetViews(torch.autograd.Function):
+    """Inputs: the full-size [B,P,...] coarse centers, opacity, scales and rotations and the concatenated ``shs_fine``;
+    the gradients of the coarse tensors are the subsets' in their rows and zero elsewhere."""
+
+    @staticmethod
+    def forward(ctx, binning, idx, offsets, counts, shs_c, centers, opacity, scales, rotations):
+        outs, (color, allmap, state, n_max) = _batch_subset_forward(binning, idx, offsets, counts, shs_c, True)
+        radii = outs[-1]
+        ctx.save_for_backward(idx, offsets, shs_c, centers, scales, rotations, color, allmap, radii, state.geom,
+                              state.tile, state.image)
+        ctx.binning, ctx.state, ctx.n_max, ctx.counts, ctx.opac_shape = binning, state, n_max, counts, tuple(opacity.shape)
+        ctx.mark_non_differentiable(radii)
+        return outs
+
+    @staticmethod
+    def backward(ctx, g_image, g_depth, g_acc, g_rn, g_dn, g_dist, _g_radii):
+        idx, offsets, shs, centers, scales, rotations, color, allmap, radii, _geom, _tile, _image = ctx.saved_tensors
+        b = ctx.binning
+        H, W, tan_fov, deg, debug = b.geometry
+        B, P = int(centers.shape[0]), int(centers.shape[1])
+        d_color, d_allmap = _epilogue_backward(color, allmap, b.rays, b.cams, b.depth_ratio, b.rays is not None,
+                                               g_image, g_depth, g_acc, g_rn, g_dn, g_dist)
+        # rows of the flattened [B*P] coarse tensors: scene s's local index + s*P
+        scene = torch.repeat_interleave(torch.arange(B, device=idx.device),
+                                        torch.tensor(ctx.counts, device=idx.device), output_size=int(idx.numel()))
+        rows_idx = idx + scene * P
+        rows = [t.reshape(B * P, -1).index_select(0, rows_idx).contiguous() for t in (centers, scales, rotations)]
+        g = R.backward_batch_raw(ctx.state, radii, rows[0], shs, rows[1], rows[2], b.cams, tan_fov, H, W, deg, d_color,
+                                 d_allmap, offsets=offsets, P=ctx.n_max, raw_activations=b.raw_activations, debug=debug)
+
+        def scatter(gn, shape):
+            full = torch.zeros(shape, dtype=torch.float32, device=idx.device)
+            if idx.numel():
+                full.view(B * P, -1)[rows_idx] = gn.reshape(idx.numel(), -1)     # unique rows: an exact copy per row
+            return full
+        return (None, None, None, None, g["sh"], scatter(g["means3D"], tuple(centers.shape)),
+                scatter(g["opacities"], ctx.opac_shape), scatter(g["scales"], tuple(scales.shape)),
+                scatter(g["rotations"], tuple(rotations.shape)))
+
+
+def render_batch_subset_views(binning: BatchBinning, masks: torch.Tensor, shs_fine: torch.Tensor,
+                              prex: str = "_fine") -> Dict[str, object]:
+    """LaRa's fine pass for all B scenes of a batch from the coarse pass's binning: ``binning`` is ``out["binning"]`` of
+    ``render_batch_views(..., keep_binning=True)``, ``masks`` a bool tensor [B,P], ``shs_fine`` [n,M,3] the subsets' SH
+    coefficients concatenated in scene order (B calls of ``FineHead.fine_shs`` concatenated).  Returns ``{key+prex:
+    [B,V,...]}`` where ``out[k][b]`` is what :func:`render_subset_views` returns for scene b alone, bit for bit, and
+    ``radii+prex`` a list of B tensors [V, n_b].  One host sync for the mask counts (and the C entry's check of the
+    offsets, which waits for the stream).  Gradients go to the [B,P,...] coarse tensors and to ``shs_fine``."""
+    if not isinstance(binning, BatchBinning):
+        raise TypeError("render_batch_subset_views: binning must be out['binning'] of render_batch_views(..., "
+                        "keep_binning=True)")
+    binning.check_unchanged()
+    centers, _, opacity, scales, rotations = binning.tensors
+    B, P, dev = int(binning.means.shape[0]), int(binning.means.shape[1]), binning.means.device
+    if not isinstance(masks, torch.Tensor) or masks.dtype != torch.bool or tuple(masks.shape) != (B, P) or \
+            masks.device != dev:
+        raise RuntimeError(f"render_batch_subset_views: masks must be a bool tensor [{B},{P}] on {dev}, got "
+                           f"{getattr(masks, 'dtype', type(masks))} {tuple(getattr(masks, 'shape', ()))} on "
+                           f"{getattr(masks, 'device', None)}")
+    deg = binning.geometry[3]
+    if not isinstance(shs_fine, torch.Tensor) or shs_fine.dtype != torch.float32 or shs_fine.device != dev or \
+            shs_fine.ndim != 3 or shs_fine.shape[2] != 3 or shs_fine.shape[1] < (deg + 1) ** 2:
+        raise RuntimeError(f"render_batch_subset_views: shs_fine must be float32 [n, M >= {(deg + 1) ** 2}, 3] on {dev}, "
+                           f"got {getattr(shs_fine, 'dtype', type(shs_fine))} {tuple(getattr(shs_fine, 'shape', ()))}")
+    counts_d = masks.sum(1)
+    counts = [int(c) for c in counts_d.tolist()]        # the host sync
+    n = sum(counts)
+    if shs_fine.shape[0] != n:
+        raise RuntimeError(f"render_batch_subset_views: shs_fine has {shs_fine.shape[0]} rows, the masks select {n}")
+    idx = torch.nonzero_static(masks, size=n)[:, 1].contiguous()      # scene-major, ascending within a scene
+    offsets = torch.zeros(B + 1, dtype=torch.int64, device=dev)
+    torch.cumsum(counts_d, 0, out=offsets[1:])
+    shs_c = shs_fine.contiguous()
+    with _DeviceGuard(dev):
+        if n == 0:
+            # every mask empty: B*V renders of zero Gaussians, as render_subset_views gives them
+            outs = _empty_subset(binning, B, shs_c)
+        elif R.needs_backward(centers, shs_fine, opacity, scales, rotations):
+            outs = _RenderBatchSubsetViews.apply(binning, idx, offsets, counts, shs_c, centers, opacity, scales, rotations)
+        else:
+            outs = _batch_subset_forward(binning, idx, offsets, counts, shs_c, False)[0]
+    radii = outs[-1]
+    out = _batch_out_dict(outs[:-1] + (radii,), B, binning.rays is not None, prex)
+    V = radii.shape[0] // B
+    out["radii" + prex] = [radii[b * V:(b + 1) * V, :counts[b]] for b in range(B)]
+    return out
+
+
+def _empty_subset(b: BatchBinning, B, shs_c):
+    """The outputs of a batch subset render of zero Gaussians: the backgrounds (what a forward of zero Gaussians
+    renders, rasterizer._forward), through the epilogue; the autograd graph still reaches ``shs_fine``."""
+    V = b.state.nviews
+    H, W = b.geometry[0], b.geometry[1]
+    color = torch.zeros((V, 3, H, W), dtype=torch.float32, device=shs_c.device)
+    allmap = torch.zeros((V, 8, H, W), dtype=torch.float32, device=shs_c.device)
+    return (*_epilogue_forward(color, allmap, b.rays, b.cams, b.depth_ratio),
+            torch.empty((V, 0), dtype=torch.int32, device=shs_c.device))

@@ -108,3 +108,31 @@ class Renderer(nn.Module):
         the SH coefficients ``shs_fine``: ``lara_b200.multiview.render_subset_views``."""
         from .multiview import render_subset_views
         return render_subset_views(binning, mask, shs_fine, prex=prex)
+
+    def render_batch_views(self, cams, rays, centers, shs, opacity, scales, rotations, device, bg_colors=None,
+                           prex: str = "", depth_ratio: float = 0.0, keep_binning: bool = False):
+        """:meth:`render_views` for all B scenes of a batch in one launch set: ``cams[b]`` scene b's V cameras,
+        ``rays`` [B,V,H,W,6] (or None), Gaussian tensors [B,P,...], ``bg_colors[b][j]`` optional per-view backgrounds.
+        Returns ``{key: [B,V,H,W,C]}`` (``lara_b200.multiview.render_batch_views``)."""
+        from .multiview import render_batch_views
+        settings = []
+        for b, scene_cams in enumerate(cams):
+            row = []
+            for j, cam in enumerate(scene_cams):
+                if bg_colors is not None:
+                    self.set_bg_color(bg_colors[b][j])
+                row.append(self.set_rasterizer(cam, device=device).raster_settings)
+            settings.append(row)
+        fuse = self.fused_activations
+        if not fuse:
+            opacity = self.opacity_activation(opacity)
+            scales = self.scaling_activation(scales)
+            rotations = self.rotation_activation(rotations)
+        return render_batch_views(centers, shs, opacity, scales, rotations, settings, rays=rays, depth_ratio=depth_ratio,
+                                  raw_activations=fuse, prex=prex, keep_binning=keep_binning)
+
+    def render_batch_subset_views(self, binning, masks, shs_fine, prex: str = "_fine"):
+        """The fine pass of all scenes of a :meth:`render_batch_views` call with ``keep_binning=True``:
+        ``lara_b200.multiview.render_batch_subset_views``."""
+        from .multiview import render_batch_subset_views
+        return render_batch_subset_views(binning, masks, shs_fine, prex=prex)
