@@ -4,8 +4,8 @@
  * reference crosses Python -> native at three pybind entry points
  * (DSR/ext.cpp:15-19, DSR/rasterize_points.h:18-68):
  *
- *     rasterize_gaussians            -> srf_views_forward   (V = 1)
- *     rasterize_gaussians_backward   -> srf_views_backward  (V = 1)
+ *     rasterize_gaussians            -> srf_scenes_forward   (S = 1, Vs = 1)
+ *     rasterize_gaussians_backward   -> srf_scenes_backward  (S = 1, Vs = 1)
  *     mark_visible                   -> srf_mark_visible
  *
  * which in turn call CudaRasterizer::Rasterizer::{forward,backward,markVisible}
@@ -34,7 +34,7 @@
 extern "C" {
 #endif
 
-#define SRF_ABI_VERSION 12
+#define SRF_ABI_VERSION 13
 
 /* cudaStream_t without pulling in cuda_runtime.h */
 typedef void* srf_stream_t;
@@ -49,8 +49,8 @@ const char* srf_last_error(void);
  * SRF_CAM_FLOATS floats each:
  *   [SRF_CAM_VIEW, +16)   viewmatrix (as above), [SRF_CAM_CAMPOS, +3) campos,
  *   [SRF_CAM_BG, +3)      background colour, the rest padding.
- * The views of one call share tan_fovx/tan_fovy, the image size and the SH degree.  One view of the
- * reference's interface is V = 1: one record. */
+ * The views of one call share the image size and the SH degree, and the views of one scene its field of view
+ * (below).  One view of the reference's interface is V = 1: one record. */
 #define SRF_CAM_FLOATS 24
 #define SRF_CAM_VIEW 0
 #define SRF_CAM_CAMPOS 16
@@ -70,8 +70,8 @@ const char* srf_last_error(void);
  *                    4*capacity rounded up to 256), the forward's contribution masks,
  *                    u32 [8][capacity] (36 B per instance of capacity in all); keep it from
  *                    forward to backward.
- *   [5] scratch    : srf_views_backward's scratch, one 80-byte gradient record per Gaussian and view.
- * for_backward = 0 sizes the workspaces of a forward-only srf_views_forward (below): image and scratch are 0
+ *   [5] scratch    : srf_scenes_backward's scratch, one 80-byte gradient record per Gaussian and view.
+ * for_backward = 0 sizes the workspaces of a forward-only srf_scenes_forward (below): image and scratch are 0
  * (not needed) and point_list is the list alone, 4 B per instance of capacity rounded up to 256 B per view. */
 int srf_views_workspace_bytes(int V, int P, int H, int W, size_t capacity, int for_backward, size_t bytes[6]);
 
@@ -83,17 +83,29 @@ int srf_views_workspace_bytes(int V, int P, int H, int W, size_t capacity, int f
  *   image_off[2] : accum(3 float planes), n_contrib(2 u32 planes)                    */
 int srf_state_layout(int P, int H, int W, size_t geom_off[3], size_t tile_off[5], size_t image_off[2]);
 
+/* ---- scenes -------------------------------------------------------------------------------------------------------
+ * The forward, subset forward and backward take S scenes of Vs views each, every scene its own Gaussians, laid out as
+ * one call of V = S*Vs views: view v (camera record v of `cams` [S*Vs, SRF_CAM_FLOATS], workspace slot v, output image
+ * v) belongs to scene v / Vs.  The views of one scene share its field of view, tan_fov[2s] (x) and tan_fov[2s+1] (y), a
+ * host array [S,2] of finite positive values; all views share the image size and the SH degree.  One scene of V views
+ * (the reference's interface: V = 1) is S = 1, Vs = V.  Each view's outputs and state are bit-identical to those of
+ * the same call on its scene alone, and each scene's gradient rows too (with deterministic != 0; otherwise up to the
+ * order of float atomics).  0 < S <= SRF_MAX_SCENES, Vs > 0, S*Vs <= 65535.  The per-view entries below
+ * (srf_views_forward_render, the workspace and scratch queries) take V = S*Vs.                                        */
+#define SRF_MAX_SCENES 128
+
 /* ---- forward ------------------------------------------------------------------------
  * Stage 1 replaces FORWARD::preprocess, cub::DeviceScan::InclusiveSum and the blocking cudaMemcpy of
  * num_rendered (rasterizer_impl.cu:241-282); stage 2 replaces duplicateWithKeys,
  * cub::DeviceRadixSort::SortPairs, identifyTileRanges and FORWARD::render (rasterizer_impl.cu:290-341).
- * srf_views_forward runs both stages.  Stage 1 writes radii [V,P] and the geom/tile workspaces and
+ * srf_scenes_forward runs both stages.  Gaussian inputs are [S,P,...] (means3D [S,P,3], shs [S,P,M,3], ...).
+ * Stage 1 writes radii [V,P] and the geom/tile workspaces (sized by srf_views_workspace_bytes(V, P, ...)) and
  * stores each view's instance count (uint32) in `num_rendered_host` (pinned host array of V, may be
  * NULL) asynchronously -- wait on the stream or on `count_event` (a cudaEvent_t, may be NULL), which is
  * recorded between the two stages: waiting on it waits for the counts, not for the blend.
  * `capacity` is the per-view number of instances `entries` / `point_list` can hold.  If a count exceeds
  * it nothing is written out of bounds, the outputs are unspecified, and the caller runs stage 2 again
- * with srf_views_forward_render and larger buffers (stage 1 need not be repeated).
+ * with srf_views_forward_render and larger buffers (stage 1 need not be repeated; stage 2 reads no Gaussian input).
  * Outputs: out_color [V,3,H,W], out_others [V,8,H,W] (depth, alpha, normal xyz, median depth,
  * distortion, median weight -- auxiliary.h:25-30).
  * `shs` XOR `colors_precomp`, (`scales`,`rotations`) XOR `transMat_precomp` as in the reference
@@ -107,16 +119,16 @@ int srf_state_layout(int P, int H, int W, size_t geom_off[3], size_t tile_off[5]
  * counts and bit-identical out_color / out_others / radii, but the blend keeps no contribution record and writes no
  * per-pixel image state, so `point_list` holds only the sorted list and `image_state` is not used (may be NULL); size
  * the workspaces with srf_views_workspace_bytes(..., for_backward = 0, ...).  The state it leaves cannot feed
- * srf_views_backward.
+ * srf_scenes_backward.
  * Every argument check of both stages, including null or misaligned workspaces, is made before anything is enqueued. */
-int srf_views_forward(srf_stream_t stream, int V, int P, int D, int M,
-                      const float* means3D, const float* shs, const float* colors_precomp,
-                      const float* opacities, const float* scales, const float* rotations,
-                      const float* transMat_precomp, const float* cams,
-                      float tan_fovx, float tan_fovy, int image_height, int image_width, int prefiltered,
-                      size_t capacity, int* radii, void* geom_state, void* tile_state, void* entries,
-                      uint32_t* point_list, void* image_state, float* out_color, float* out_others,
-                      uint32_t* num_rendered_host, void* count_event, int raw_activations, int for_backward);
+int srf_scenes_forward(srf_stream_t stream, int S, int Vs, int P, int D, int M,
+                       const float* means3D, const float* shs, const float* colors_precomp,
+                       const float* opacities, const float* scales, const float* rotations,
+                       const float* transMat_precomp, const float* cams, const float* tan_fov,
+                       int image_height, int image_width, int prefiltered,
+                       size_t capacity, int* radii, void* geom_state, void* tile_state, void* entries,
+                       uint32_t* point_list, void* image_state, float* out_color, float* out_others,
+                       uint32_t* num_rendered_host, void* count_event, int raw_activations, int for_backward);
 /* stage 2 alone, on the state stage 1 left: the re-run with larger binning buffers; for_backward as given to the
  * forward */
 int srf_views_forward_render(srf_stream_t stream, int V, int P, int image_height, int image_width,
@@ -125,36 +137,49 @@ int srf_views_forward_render(srf_stream_t stream, int V, int P, int image_height
                              const float* cams, float* out_color, float* out_others, int for_backward);
 
 /* ---- subset forward (LaRa's fine pass, lightning/network.py:486-525; DESIGN §3.18) ----------------------------
- * Renders the n Gaussians idx[0..n) (strictly ascending indices into the P of a coarse srf_views_forward) of the same V
- * cameras and image size with new SH coefficients shs [n,M,3], from the coarse forward's state instead of a preprocess
- * and a binning: the records, depths, rects and radii of the subset are the coarse ones of Gaussian idx[j], with the
- * colour word recomputed from shs[j]; each tile's list is the coarse list with the other Gaussians removed.  The
- * outputs are bit-identical to srf_views_forward on the gathered subset (means3D[idx], opacities[idx], ...) with the
- * same raw_activations flag, and the state it leaves feeds srf_views_backward with P = n (for_backward != 0) exactly
- * as that forward's would.  The kept entries stay at the coarse tile's list offsets, so the subset's `point_list`
- * workspace is sized, like the coarse one, by `capacity`, which must equal the coarse forward's capacity
- * (`coarse_capacity`, whose counts must have fit it: re-run the coarse stage 2 first if they did not).
- * Inputs: the coarse state (radii [V,P], geom / tile workspaces, point_list, and whether the coarse forward was
- * for_backward), means3D [P,3] (the coarse centers), cams as given to the coarse forward.  Outputs: radii [V,n], the
- * subset's geom / tile / image workspaces and point_list (sizes from srf_views_workspace_bytes(V, n, H, W, capacity,
- * for_backward); entries are not used), out_color / out_others as srf_views_forward.  `workspace`: 256-byte aligned,
- * srf_views_subset_workspace_bytes(P).  colors_precomp is not supported (must be NULL).  n == 0 renders the
- * background.  Every argument check is made before anything is enqueued; nothing waits for the stream. */
-int srf_views_subset_forward(srf_stream_t stream, int V, int P, int n, int D, int M,
-                             const int64_t* idx, const float* means3D, const float* shs, const float* colors_precomp,
-                             const float* cams, int image_height, int image_width, size_t capacity,
-                             const int* coarse_radii, const void* coarse_geom_state, const void* coarse_tile_state,
-                             const uint32_t* coarse_point_list, size_t coarse_capacity, int coarse_for_backward,
-                             int* radii, void* geom_state, void* tile_state, uint32_t* point_list, void* image_state,
-                             float* out_color, float* out_others, void* workspace, int for_backward);
+ * Renders a subset of each scene's Gaussians of a coarse srf_scenes_forward with the same cameras and image size and
+ * new SH coefficients, from the coarse forward's state instead of a preprocess and a binning: the records, depths,
+ * rects and radii of the subset are the coarse ones of its Gaussians, with the colour word recomputed from the new
+ * SH; each tile's list is the coarse list with the other Gaussians removed.  The outputs are bit-identical to
+ * srf_scenes_forward on the gathered subsets (means3D[idx], opacities[idx], ...) with the same raw_activations flag,
+ * and the state it leaves feeds srf_scenes_backward with P = n_max and the same `offsets` (for_backward != 0) exactly
+ * as that forward's would.
+ * `idx` [n] is the concatenation of the S strictly ascending index lists, each into its scene's P coarse Gaussians;
+ * `offsets` (device int64 [S+1], from 0, non-decreasing, ending at n) splits it: scene s's subset is
+ * idx[offsets[s] .. offsets[s+1]).  shs [n,M,3] is concatenated the same way; means3D [S,P,3] are the coarse centers.
+ * The entry reads `offsets` back to check it, so it waits for the stream.  offsets == NULL is one scene (S = 1), whose
+ * subset is idx[0..n) with n_max == n: nothing is read back and nothing waits for the stream.
+ * The subset state is laid out as V views of n_max Gaussians each (n_max >= every scene's count, <= P): radii
+ * [V,n_max], workspaces srf_views_workspace_bytes(V, n_max, H, W, capacity, for_backward) (entries are not used);
+ * view v holds scene v / Vs's subset in its first slots.  The kept entries stay at the coarse tile's list offsets, so
+ * the subset's `point_list` workspace is sized, like the coarse one, by `capacity`, which must equal the coarse
+ * forward's capacity (`coarse_capacity`, whose counts must have fit it: re-run the coarse stage 2 first if they did
+ * not).  Inputs: the coarse state (radii [V,P], geom / tile workspaces, point_list, and whether the coarse forward was
+ * for_backward) and cams as given to the coarse forward.  out_color / out_others as srf_scenes_forward.
+ * `workspace`: 256-byte aligned, srf_views_subset_workspace_bytes(S*P).  colors_precomp is not supported (must be
+ * NULL).  A scene with an empty subset (n == 0 included) renders the background.  Every argument check is made before
+ * anything is enqueued. */
+int srf_scenes_subset_forward(srf_stream_t stream, int S, int Vs, int P, int n, int n_max, int D, int M,
+                              const int64_t* idx, const int64_t* offsets, const float* means3D, const float* shs,
+                              const float* colors_precomp, const float* cams, int image_height, int image_width,
+                              size_t capacity, const int* coarse_radii, const void* coarse_geom_state,
+                              const void* coarse_tile_state, const uint32_t* coarse_point_list, size_t coarse_capacity,
+                              int coarse_for_backward, int* radii, void* geom_state, void* tile_state,
+                              uint32_t* point_list, void* image_state, float* out_color, float* out_others,
+                              void* workspace, int for_backward);
 int srf_views_subset_workspace_bytes(int P, size_t* bytes);
 
 /* ---- backward ------------------------------------------------------------------
  * Replaces Rasterizer::backward (rasterizer_impl.cu:346-448): BACKWARD::render,
  * computeAABB backward, BACKWARD::preprocess.  Consumes the state the forward left in the
  * geom/tile/image workspaces and point_list; upstream gradients dL_dout_color [V,3,H,W],
- * dL_dout_others [V,8,H,W].  The per-Gaussian backward sums the gradients of all V views in
- * registers and writes every output row once (zeros for culled Gaussians), so the outputs need
+ * dL_dout_others [V,8,H,W].  `P` is the number of Gaussians per view slot and `offsets` says where each scene's
+ * inputs and gradient rows are:
+ *   NULL for srf_scenes_forward's state: scene s's rows are [s*P, (s+1)*P) of [S,P,...] arrays;
+ *   the subset forward's offsets, with P = n_max: scene s's rows are [offsets[s], offsets[s+1]) of the concatenated
+ *   [n,...] arrays (the gathered subset inputs).  The entry reads them back to check them (waits for the stream).
+ * The per-Gaussian backward sums the gradients of a scene's Vs views in registers, in view order, and writes every
+ * output row once (zeros for culled Gaussians), so the outputs need
  * no initialisation -- unless accumulate != 0, in which case the kernel adds into them (used to
  * sum several calls before one all-reduce).  Output pointers may be NULL when that gradient is
  * not wanted (dL_dmeans3D, dL_dopacity, dL_dscales, dL_drotations are required).
@@ -170,64 +195,6 @@ int srf_views_subset_workspace_bytes(int P, size_t* bytes);
  * srf_views_backward_deterministic_scratch_bytes(V, P) bytes, and the call waits for the stream before it returns: if a
  * partial sum is not finite or beyond the fixed-point range it returns an error instead of a gradient (the output
  * arrays then hold no meaningful values, and with accumulate != 0 they have been added to).                          */
-int srf_views_backward(srf_stream_t stream, int V, int P, int D, int M, int image_height, int image_width,
-                       size_t capacity, const float* cams,
-                       const float* means3D, const float* shs, int colors_were_precomputed,
-                       const float* scales, const float* rotations, int transmat_was_precomputed,
-                       float tan_fovx, float tan_fovy, const int* radii,
-                       const void* geom_state, const void* tile_state, const uint32_t* point_list,
-                       const void* image_state,
-                       const float* dL_dout_color, const float* dL_dout_others,
-                       void* scratch, int accumulate,
-                       float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
-                       float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
-                       int raw_activations, int deterministic);
-int srf_views_backward_deterministic_scratch_bytes(int V, int P, size_t* bytes);
-
-/* ---- S scenes in one launch set (a training batch; DESIGN §3.21) -------------------------------------------------
- * S scenes of Vs views each, every scene its own Gaussians, are laid out as one srf_views_* call of V = S*Vs views:
- * view v (camera record v of `cams` [S*Vs, SRF_CAM_FLOATS], workspace slot v, output image v) belongs to scene v / Vs.
- * The views of one scene share its field of view, tan_fov[2s] (x) and tan_fov[2s+1] (y), a host array [S,2] of finite
- * positive values; all views share the image size and the SH degree.  Each view's outputs and state are bit-identical
- * to those of srf_views_forward / srf_views_subset_forward on that scene alone, and each scene's gradient rows to those
- * of srf_views_backward on that scene alone (with deterministic != 0; otherwise up to the order of float atomics).
- * 0 < S <= SRF_MAX_SCENES, Vs > 0, S*Vs <= 65535.  Every argument check is made before anything is enqueued.
- *
- * srf_scenes_forward: srf_views_forward on S scenes.  Gaussian inputs [S,P,...] (means3D [S,P,3], shs [S,P,M,3], ...);
- * radii [S*Vs,P]; workspaces sized by srf_views_workspace_bytes(S*Vs, P, ...); num_rendered_host holds S*Vs counts.
- * Its stage-2 re-run is srf_views_forward_render with V = S*Vs, which reads no Gaussian input.
- *
- * srf_scenes_subset_forward: srf_views_subset_forward on S scenes with ragged subsets.  `offsets` (device int64 [S+1],
- * from 0, non-decreasing, ending at n) splits `idx` [n], the concatenation of the S strictly ascending index lists,
- * into scene s's idx[offsets[s] .. offsets[s+1]) (indices into that scene's P Gaussians); shs [n,M,3] is concatenated
- * the same way; means3D [S,P,3] are the coarse centers.  The subset state is laid out as S*Vs views of n_max Gaussians
- * each (n_max >= every scene's count, <= P): radii [S*Vs,n_max], workspaces srf_views_workspace_bytes(S*Vs, n_max,
- * ...), `workspace` srf_views_subset_workspace_bytes(S*P); view v holds scene v / Vs's subset in its first slots.  The
- * entry reads `offsets` back to check it, so it waits for the stream.
- *
- * srf_scenes_backward: srf_views_backward on the state of either forward.  It takes `P` (Gaussians per view slot) and
- * `offsets`: NULL for srf_scenes_forward's state (scene s's inputs and gradient rows are [s*P, (s+1)*P) of [S,P,...]
- * arrays), or the subset forward's offsets with P = n_max (scene s's rows are [offsets[s], offsets[s+1]) of the
- * concatenated [n,...] arrays: the gathered subset inputs, as for srf_views_backward on a subset).  Each scene's rows
- * sum that scene's Vs views only, in view order.  With offsets it reads them back to check them (waits for the
- * stream).  Scratch sizes are those of V = S*Vs views of P Gaussians.                                                */
-#define SRF_MAX_SCENES 128
-int srf_scenes_forward(srf_stream_t stream, int S, int Vs, int P, int D, int M,
-                       const float* means3D, const float* shs, const float* colors_precomp,
-                       const float* opacities, const float* scales, const float* rotations,
-                       const float* transMat_precomp, const float* cams, const float* tan_fov,
-                       int image_height, int image_width, int prefiltered,
-                       size_t capacity, int* radii, void* geom_state, void* tile_state, void* entries,
-                       uint32_t* point_list, void* image_state, float* out_color, float* out_others,
-                       uint32_t* num_rendered_host, void* count_event, int raw_activations, int for_backward);
-int srf_scenes_subset_forward(srf_stream_t stream, int S, int Vs, int P, int n, int n_max, int D, int M,
-                              const int64_t* idx, const int64_t* offsets, const float* means3D, const float* shs,
-                              const float* colors_precomp, const float* cams, int image_height, int image_width,
-                              size_t capacity, const int* coarse_radii, const void* coarse_geom_state,
-                              const void* coarse_tile_state, const uint32_t* coarse_point_list, size_t coarse_capacity,
-                              int coarse_for_backward, int* radii, void* geom_state, void* tile_state,
-                              uint32_t* point_list, void* image_state, float* out_color, float* out_others,
-                              void* workspace, int for_backward);
 int srf_scenes_backward(srf_stream_t stream, int S, int Vs, int P, const int64_t* offsets, int D, int M,
                         int image_height, int image_width, size_t capacity, const float* cams,
                         const float* means3D, const float* shs, int colors_were_precomputed,
@@ -240,6 +207,7 @@ int srf_scenes_backward(srf_stream_t stream, int S, int Vs, int P, const int64_t
                         float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
                         float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
                         int raw_activations, int deterministic);
+int srf_views_backward_deterministic_scratch_bytes(int V, int P, size_t* bytes);
 
 /* ---- fused render_img epilogue (next-row: lightning/renderer_2dgs.py:220-268, :74-89) ---------
  * One pass over the rasterizer's outputs of V stacked views instead of ~12 torch ops (and ~20 autograd
@@ -250,7 +218,7 @@ int srf_scenes_backward(srf_stream_t stream, int S, int Vs, int P, const int64_t
  * pseudo normals).  Of each camera record the epilogue reads only the view matrix, floats
  * [SRF_CAM_VIEW, SRF_CAM_VIEW + 16): for V = 1 a bare 16-float view matrix is a valid `cams`.
  * The backward takes the gradients of the six outputs (NULL = zero) and writes dL_dcolor [V,3,H,W] and
- * dL_dallmap [V,8,H,W], ready for srf_views_backward; where the reference's autograd produces NaN
+ * dL_dallmap [V,8,H,W], ready for srf_scenes_backward; where the reference's autograd produces NaN
  * (0/0 at alpha == 0) this writes 0.  scratch: [V,3,H,W] floats.                                      */
 int srf_views_epilogue_forward(srf_stream_t stream, int V, int image_height, int image_width, float depth_ratio,
                                const float* color, const float* allmap, const float* rays, const float* cams,

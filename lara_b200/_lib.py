@@ -18,7 +18,7 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libsurfel_b200.so")
-ABI_VERSION = 12
+ABI_VERSION = 13
 CAM_FLOATS, CAM_VIEW, CAM_CAMPOS, CAM_BG = 24, 0, 16, 19      # include/surfel_rasterizer.h SRF_CAM_*
 
 
@@ -38,44 +38,12 @@ SIGNATURES = {
     "srf_last_error": (c_char_p, []),
     "srf_views_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, c_size_t, c_int, POINTER(c_size_t)]),
     "srf_state_layout": (c_int, [c_int, c_int, c_int, POINTER(c_size_t), POINTER(c_size_t), POINTER(c_size_t)]),
-    "srf_views_forward": (c_int, [
-        _P, c_int, c_int, c_int, c_int,     # stream, V, P, D, M
-        _P, _P, _P,                         # means3D, shs, colors_precomp
-        _P, _P, _P,                         # opacities, scales, rotations
-        _P, _P,                             # transMat_precomp, cams
-        c_float, c_float, c_int, c_int,     # tan_fovx, tan_fovy, H, W
-        c_int, c_size_t,                    # prefiltered, capacity
-        _P, _P, _P, _P, _P, _P,             # radii, geom_state, tile_state, entries, point_list, image_state
-        _P, _P, _P, _P,                     # out_color, out_others, num_rendered_host, count_event
-        c_int, c_int,                       # raw_activations, for_backward
-    ]),
     "srf_views_forward_render": (c_int, [
         _P, c_int, c_int, c_int, c_int,     # stream, V, P, H, W
         c_size_t, _P, _P,                   # capacity, geom_state, tile_state
         _P, _P, _P,                         # entries, point_list, image_state
         _P, _P, _P,                         # cams, out_color, out_others
         c_int,                              # for_backward
-    ]),
-    "srf_views_backward": (c_int, [
-        _P, c_int, c_int, c_int, c_int, c_int, c_int,   # stream, V, P, D, M, H, W
-        c_size_t, _P,                            # capacity, cams
-        _P, _P, c_int,                           # means3D, shs, colors_were_precomputed
-        _P, _P, c_int,                           # scales, rotations, transmat_was_precomputed
-        c_float, c_float, _P,                    # tan_fovx, tan_fovy, radii
-        _P, _P, _P, _P,                          # geom_state, tile_state, point_list, image_state
-        _P, _P,                                  # dL_dout_color, dL_dout_others
-        _P, c_int,                               # scratch, accumulate
-        _P, _P, _P, _P,                          # dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors
-        _P, _P, _P, _P,                          # dL_dopacity, dL_dscales, dL_drotations, dL_dtransMat
-        c_int, c_int,                            # raw_activations, deterministic
-    ]),
-    "srf_views_subset_forward": (c_int, [
-        _P, c_int, c_int, c_int, c_int, c_int,  # stream, V, P, n, D, M
-        _P, _P, _P, _P, _P,                 # idx, means3D, shs, colors_precomp, cams
-        c_int, c_int, c_size_t,             # H, W, capacity
-        _P, _P, _P, _P, c_size_t, c_int,    # coarse radii, geom_state, tile_state, point_list, capacity, for_backward
-        _P, _P, _P, _P, _P,                 # radii, geom_state, tile_state, point_list, image_state
-        _P, _P, _P, c_int,                  # out_color, out_others, workspace, for_backward
     ]),
     "srf_views_subset_workspace_bytes": (c_int, [c_int, POINTER(c_size_t)]),
     "srf_scenes_forward": (c_int, [
@@ -284,7 +252,7 @@ def _size_query(fn, *args) -> int:
 
 
 def det_backward_scratch_bytes(lib, V: int, P: int) -> int:
-    """Scratch of srf_views_backward(..., deterministic=1)."""
+    """Scratch of srf_scenes_backward(..., deterministic=1) for V views of P Gaussians."""
     return _size_query(lib.srf_views_backward_deterministic_scratch_bytes, V, P)
 
 
@@ -294,7 +262,7 @@ def tan_fov_array(tan_fov) -> ctypes.Array:
 
 
 def subset_workspace_bytes(lib, P: int) -> int:
-    """Workspace of srf_views_subset_forward for a coarse forward of P Gaussians."""
+    """Workspace of srf_scenes_subset_forward for a coarse forward of P Gaussians over all its scenes."""
     return _size_query(lib.srf_views_subset_workspace_bytes, P)
 
 

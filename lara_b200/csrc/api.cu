@@ -82,7 +82,7 @@ size_t plist_stride_bytes(size_t capacity, bool for_backward) {
 size_t entries_stride_bytes(size_t capacity) { return align_up(capacity * sizeof(uint64_t)) + 256; }
 size_t ggrad_stride_bytes(int P) { return align_up((size_t)P * SRF_GRAD_FLOATS * sizeof(float)) + 256; }
 
-// Scratch of the deterministic backward: V fp32 gradient-record arrays (as srf_views_backward's scratch), then V arrays
+// Scratch of the deterministic backward: V fp32 gradient-record arrays (as srf_scenes_backward's scratch), then V arrays
 // of fixed-point records, then the overflow flag.
 size_t det_stride_bytes(int P) { return align_up((size_t)P * srf::det_record_bytes()); }
 size_t det_scratch_bytes(int V, int P) { return (ggrad_stride_bytes(P) + det_stride_bytes(P)) * (size_t)V + 256; }
@@ -175,7 +175,7 @@ int scene_fov(const char* fn, int S, const float* tan_fov, int image_height, int
         const float tx = tan_fov[2 * i], ty = tan_fov[2 * i + 1];
         if (!isfinite(tx) || !isfinite(ty) || !(tx > 0.f) || !(ty > 0.f))
             return set_error("%s: tan_fov of scene %d is (%g, %g), not finite and positive", fn, i, tx, ty);
-        // the focal lengths of srf_views_forward / _backward, rasterizer_impl.cu:223-224
+        // the focal lengths of forward_preprocess_impl / backward_impl, rasterizer_impl.cu:223-224
         s.fov[i] = make_float4(image_width / (2.0f * tx), image_height / (2.0f * ty), tx, ty);
     }
     return 0;
@@ -284,7 +284,7 @@ int srf_state_layout(int P, int H, int W, size_t geom_off[3], size_t tile_off[5]
 }  // extern "C"
 
 // ---------------------------------------------------------------------------------------------
-// Implementation of the srf_views_* entry points: V views of one scene in one launch set, each view's
+// Implementation of the rasterizer's entry points: V views in one launch set, each view's
 // camera a record of SRF_CAM_FLOATS floats in `cams`, each view's workspaces one layout stride apart.
 // ---------------------------------------------------------------------------------------------
 namespace {
@@ -445,7 +445,7 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
                   void* scratch, int accumulate,
                   float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
                   float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
-                  int raw_activations, bool deterministic, const srf::SceneArgs* scenes = nullptr, int S = 1) {
+                  int raw_activations, bool deterministic, const srf::SceneArgs* scenes, int S) {
     if (!cams) return set_error("%s: null camera records", fn);
     if (V <= 0 || P < 0 || image_height <= 0 || image_width <= 0) return set_error("%s: bad sizes", fn);
     if (P == 0) return 0;
@@ -528,34 +528,6 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
 
 extern "C" {
 
-int srf_views_forward(srf_stream_t stream_, int V, int P, int D, int M,
-                      const float* means3D, const float* shs, const float* colors_precomp,
-                      const float* opacities, const float* scales, const float* rotations,
-                      const float* transMat_precomp, const float* cams,
-                      float tan_fovx, float tan_fovy, int image_height, int image_width, int prefiltered,
-                      size_t capacity, int* radii, void* geom_state, void* tile_state, void* entries,
-                      uint32_t* point_list, void* image_state, float* out_color, float* out_others,
-                      uint32_t* num_rendered_host, void* count_event, int raw_activations, int for_backward) {
-    const char* fn = "srf_views_forward";
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    // the checks of both stages before stage 1 enqueues anything
-    if (forward_preprocess_check(fn, V, P, D, M, means3D, shs, colors_precomp, opacities, scales, rotations,
-                                 transMat_precomp, image_height, image_width, radii, geom_state, tile_state) ||
-        forward_render_check(fn, V, P, image_height, image_width, capacity, geom_state, tile_state, entries, point_list,
-                             image_state, cams, out_color, out_others, for_backward != 0))
-        return 1;
-    int rc = forward_preprocess_impl(stream, V, P, D, M, means3D, shs, colors_precomp, opacities, scales, rotations,
-                                     transMat_precomp, cams, tan_fovx, tan_fovy, image_height, image_width, prefiltered,
-                                     radii, geom_state, tile_state, num_rendered_host, raw_activations, nullptr);
-    if (rc != 0) return rc;
-    if (count_event) {      // lets the caller wait for the instance counts without waiting for the blend
-        cudaError_t e = cudaEventRecord(static_cast<cudaEvent_t>(count_event), stream);
-        if (e != cudaSuccess) return cuda_error("count event record", e);
-    }
-    return forward_render_impl(stream, V, P, image_height, image_width, capacity, geom_state, tile_state, entries,
-                               point_list, image_state, cams, out_color, out_others, for_backward != 0);
-}
-
 int srf_views_forward_render(srf_stream_t stream_, int V, int P, int image_height, int image_width,
                              size_t capacity, const void* geom_state, void* tile_state,
                              void* entries, uint32_t* point_list, void* image_state,
@@ -566,26 +538,6 @@ int srf_views_forward_render(srf_stream_t stream_, int V, int P, int image_heigh
     return forward_render_impl(static_cast<cudaStream_t>(stream_), V, P, image_height, image_width, capacity, geom_state,
                                tile_state, entries, point_list, image_state, cams, out_color, out_others,
                                for_backward != 0);
-}
-
-int srf_views_backward(srf_stream_t stream_, int V, int P, int D, int M, int image_height, int image_width,
-                       size_t capacity, const float* cams,
-                       const float* means3D, const float* shs, int colors_were_precomputed,
-                       const float* scales, const float* rotations, int transmat_was_precomputed,
-                       float tan_fovx, float tan_fovy, const int* radii,
-                       const void* geom_state, const void* tile_state, const uint32_t* point_list,
-                       const void* image_state,
-                       const float* dL_dout_color, const float* dL_dout_others,
-                       void* scratch, int accumulate,
-                       float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
-                       float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
-                       int raw_activations, int deterministic) {
-    return backward_impl("srf_views_backward", static_cast<cudaStream_t>(stream_), V, P, D, M, image_height, image_width,
-                         capacity, cams, means3D, shs, colors_were_precomputed, scales, rotations,
-                         transmat_was_precomputed, tan_fovx, tan_fovy, radii, geom_state, tile_state, point_list,
-                         image_state, dL_dout_color, dL_dout_others, scratch, accumulate, dL_dmeans3D, dL_dmeans2D,
-                         dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drotations, dL_dtransMat, raw_activations,
-                         deterministic != 0);
 }
 
 int srf_scenes_forward(srf_stream_t stream_, int S, int Vs, int P, int D, int M,
@@ -609,12 +561,14 @@ int srf_scenes_forward(srf_stream_t stream_, int S, int Vs, int P, int D, int M,
                              image_state, cams, out_color, out_others, for_backward != 0))
         return 1;
     if ((size_t)S * P > 0x7fffffffull) return set_error("%s: S * P exceeds 32-bit Gaussian indices", fn);
+    // one scene runs the preprocess instantiation without scene arguments (NoScenes): it reads the focal lengths
+    // scene_fov computed from the same tan_fov, and it is the lighter kernel (DESIGN §3.21)
     int rc = forward_preprocess_impl(stream, V, P, D, M, means3D, shs, colors_precomp, opacities, scales, rotations,
                                      transMat_precomp, cams, scenes.fov[0].z, scenes.fov[0].w, image_height, image_width,
                                      prefiltered, radii, geom_state, tile_state, num_rendered_host, raw_activations,
-                                     &scenes);
+                                     S == 1 ? nullptr : &scenes);
     if (rc != 0) return rc;
-    if (count_event) {
+    if (count_event) {      // lets the caller wait for the instance counts without waiting for the blend
         cudaError_t e = cudaEventRecord(static_cast<cudaEvent_t>(count_event), stream);
         if (e != cudaSuccess) return cuda_error("count event record", e);
     }
@@ -647,7 +601,8 @@ int srf_scenes_backward(srf_stream_t stream_, int S, int Vs, int P, const int64_
                          colors_were_precomputed, scales, rotations, transmat_was_precomputed, scenes.fov[0].z,
                          scenes.fov[0].w, radii, geom_state, tile_state, point_list, image_state, dL_dout_color,
                          dL_dout_others, scratch, accumulate, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity,
-                         dL_dscales, dL_drotations, dL_dtransMat, raw_activations, deterministic != 0, &scenes, S);
+                         dL_dscales, dL_drotations, dL_dtransMat, raw_activations, deterministic != 0,
+                         S == 1 && !offsets ? nullptr : &scenes, S);
 }
 
 int srf_views_backward_deterministic_scratch_bytes(int V, int P, size_t* bytes) {

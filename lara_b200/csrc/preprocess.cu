@@ -48,7 +48,7 @@ __device__ __forceinline__ void count_tiles_serial(uint32_t* tile_count, int gx,
         for (int x = x0; x < x1; ++x) atomicAdd(&tile_count[(size_t)(y * gx + x) * SRF_TILE_CTR_STRIDE], 1u);
 }
 
-// Without scenes (srf_views_forward) the kernel takes an empty second argument; with scenes (srf_scenes_forward) the
+// For one scene (srf_scenes_forward with S = 1) the kernel takes an empty second argument; with S > 1 scenes the
 // view's scene gives the Gaussian rows and the field of view.
 struct NoScenes {};
 

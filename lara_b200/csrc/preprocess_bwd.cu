@@ -51,7 +51,7 @@ __device__ __forceinline__ T* rows_at(T* p, size_t row, int width) {
     return p ? p + row * width : p;
 }
 
-// Without scenes (srf_views_backward) the kernel takes an empty second argument.  With scenes (srf_scenes_backward) it
+// For one scene without offsets (srf_scenes_backward with S = 1) the kernel takes an empty second argument.  Else it
 // runs one thread per (Gaussian, scene = blockIdx.y) and sums that scene's Vs views: the scene gives the rows of the
 // inputs and outputs, the first view and the field of view.
 struct NoScenes {};

@@ -11,7 +11,7 @@
 //             rank[idx[j]] = j;
 //   filter  : one warp per (tile, view) walks the coarse list in order and keeps, ballot-compacted, the entries whose
 //             rank is set, writing ranks (subset indices) at the coarse tile's start offset.
-// Then the unchanged blend forward runs on that state (views_blend), and srf_views_backward with P = n takes its
+// Then the unchanged blend forward runs on that state (views_blend), and srf_scenes_backward with P = n_max takes its
 // gradient.  Nothing is counted, sorted or read back.
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -150,9 +150,9 @@ size_t rank_bytes(int P) { return align_up((size_t)(P > 0 ? P : 1) * sizeof(uint
 
 }  // namespace
 
-// srf_views_subset_forward and srf_scenes_subset_forward: S scenes of Vs views, scene s's subset idx[offsets[s] ..
-// offsets[s+1]) of its P coarse Gaussians (offsets null: S = 1, the n Gaussians idx[0..n)), n_slot Gaussians per view of
-// the subset state.  The caller has checked S, Vs, the offsets and n_slot.
+// srf_scenes_subset_forward: S scenes of Vs views, scene s's subset idx[offsets[s] .. offsets[s+1]) of its P coarse
+// Gaussians (offsets null: S = 1, the n Gaussians idx[0..n)), n_slot Gaussians per view of the subset state.  The caller
+// has checked S, Vs, the offsets and n_slot.
 int subset_forward(const char* fn, cudaStream_t stream, int S, int Vs, int P, int n, int n_slot, const int64_t* offsets,
                    int D, int M, const int64_t* idx, const float* means3D, const float* shs, const float* colors_precomp,
                    const float* cams, int image_height, int image_width, size_t capacity,
@@ -250,23 +250,6 @@ int srf_views_subset_workspace_bytes(int P, size_t* bytes) {
     return 0;
 }
 
-int srf_views_subset_forward(srf_stream_t stream_, int V, int P, int n, int D, int M,
-                             const int64_t* idx, const float* means3D, const float* shs, const float* colors_precomp,
-                             const float* cams, int image_height, int image_width, size_t capacity,
-                             const int* coarse_radii, const void* coarse_geom_state, const void* coarse_tile_state,
-                             const uint32_t* coarse_point_list, size_t coarse_capacity, int coarse_for_backward,
-                             int* radii, void* geom_state, void* tile_state, uint32_t* point_list, void* image_state,
-                             float* out_color, float* out_others, void* workspace, int for_backward) {
-    const char* fn = "srf_views_subset_forward";
-    if (V <= 0 || P < 0 || n < 0 || image_height <= 0 || image_width <= 0) return set_error("%s: bad sizes", fn);
-    if (n > P) return set_error("%s: the subset has n = %d > P = %d Gaussians", fn, n, P);
-    return srf::subset_forward(fn, static_cast<cudaStream_t>(stream_), 1, V, P, n, n, nullptr, D, M, idx, means3D, shs,
-                               colors_precomp, cams, image_height, image_width, capacity, coarse_radii,
-                               coarse_geom_state, coarse_tile_state, coarse_point_list, coarse_capacity,
-                               coarse_for_backward, radii, geom_state, tile_state, point_list, image_state, out_color,
-                               out_others, workspace, for_backward);
-}
-
 int srf_scenes_subset_forward(srf_stream_t stream_, int S, int Vs, int P, int n, int n_max, int D, int M,
                               const int64_t* idx, const int64_t* offsets, const float* means3D, const float* shs,
                               const float* colors_precomp, const float* cams, int image_height, int image_width,
@@ -278,9 +261,16 @@ int srf_scenes_subset_forward(srf_stream_t stream_, int S, int Vs, int P, int n,
     const char* fn = "srf_scenes_subset_forward";
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     if (srf::check_scenes(fn, S, Vs)) return 1;
-    if (P < 0 || n < 0 || n_max < 0 || n_max > P) return set_error("%s: bad sizes", fn);
+    if (P < 0 || n < 0 || n_max < 0) return set_error("%s: bad sizes", fn);
+    if (n_max > P) return set_error("%s: bad sizes: a subset of n_max = %d > P = %d Gaussians", fn, n_max, P);
     if ((size_t)S * P > 0x7fffffffull) return set_error("%s: S * P exceeds 32-bit Gaussian indices", fn);
-    if (srf::check_offsets(fn, stream, S, offsets, n_max, n)) return 1;
+    if (!offsets) {         // one scene, idx[0..n): nothing to read back, no wait for the stream
+        if (S != 1 || n_max != n)
+            return set_error("%s: null offsets need one scene and n_max == n, got S = %d, n = %d, n_max = %d", fn, S, n,
+                             n_max);
+    } else if (srf::check_offsets(fn, stream, S, offsets, n_max, n)) {
+        return 1;
+    }
     return srf::subset_forward(fn, stream, S, Vs, P, n, n_max, offsets, D, M, idx, means3D, shs, colors_precomp, cams,
                                image_height, image_width, capacity, coarse_radii, coarse_geom_state, coarse_tile_state,
                                coarse_point_list, coarse_capacity, coarse_for_backward, radii, geom_state, tile_state,

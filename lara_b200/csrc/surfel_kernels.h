@@ -1,5 +1,5 @@
 // surfel_kernels.h -- internal (non-ABI) interface of the library: the rasterizer's kernel launchers, which api.cu's
-// srf_views_* entries call, and the host helpers every translation unit's extern "C" entries share.  The public
+// entries call, and the host helpers every translation unit's extern "C" entries share.  The public
 // boundary is include/surfel_rasterizer.h (and surfel_mesh.h, surfel_fine_head.h); each fused op (epilogue, loss,
 // decoder layout, point features, MS-SSIM, mesh, fine head) keeps its argument structs and entries in its own .cu.
 //
@@ -180,7 +180,7 @@ StateLayout state_layout(int P, int H, int W);
 // bytes from one view's point_list workspace to the next (the list, then for_backward the contribution record)
 size_t plist_stride(size_t capacity, bool for_backward);
 // The blend forward of V views on the state stage 1 and the binning left (ranges, launch order, point_list, records):
-// the render_fwd launch of srf_views_forward, arguments checked by the caller.  record = false: forward-only.
+// the render_fwd launch of srf_scenes_forward, arguments checked by the caller.  record = false: forward-only.
 int views_blend(cudaStream_t stream, int V, int P, int image_height, int image_width, size_t capacity,
                 const void* geom_state, const void* tile_state, const uint32_t* point_list, void* image_state,
                 const float* cams, float* out_color, float* out_others, bool record);

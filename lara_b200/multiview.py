@@ -4,8 +4,8 @@ AND one launch set.
 LaRa's step renders the V target views of a scene one after the other (``lightning/network.py:486-495``:
 ``for j, c2w in enumerate(tar_c2ws): frame = self.gs_render.render_img(cam, rays_d, _centers, ...)``) and
 then concatenates the frames (``:525``): V autograd nodes, V launch sets of ~8 kernels, V host round trips.
-``render_scene_views`` is the same computation as one ``torch.autograd.Function`` over the ``srf_views_*``
-entry points, whose kernels all carry a view dimension:
+``render_scene_views`` is the same computation as one ``torch.autograd.Function`` over the ``srf_scenes_*``
+entry points (one scene), whose kernels all carry a view dimension:
 
 * forward : preprocess (grid.y = view) -> tile scan (one CTA per view) -> scatter -> per-tile sorts -> blend
             (one CTA per (tile, view), heaviest tiles first) -> fused epilogue (grid.z = view); outputs are
@@ -43,32 +43,6 @@ def shared_view_settings(settings_list: Sequence[R.GaussianRasterizationSettings
     return key + (any(bool(rs.prefiltered) for rs in settings_list), any(bool(rs.debug) for rs in settings_list))
 
 
-def _scene_views_forward(centers, shs, opacity, scales, rotations, rays, settings_list, depth_ratio, raw_activations,
-                         for_backward, keep_list=False):
-    """Checks, the V-view rasterizer forward and the fused epilogue.  Returns the outputs (image, depth, acc, rn, dn,
-    dist, radii) and what the backward needs: (inputs, rays, cams, color, allmap, state, geometry)."""
-    dev = centers.device
-    V = len(settings_list)
-    centers_c, shs_c, _, opac_c, scales_c, rot_c, _ = R._normalise_inputs(
-        centers, shs, None, opacity, scales, rotations, None)
-    settings_list = [R._check_settings(rs, dev) for rs in settings_list]
-    H, W, tfx, tfy, deg, prefiltered, debug = shared_view_settings(settings_list)
-    rays_c = None
-    if rays is not None:
-        rays_c = rays.contiguous()
-        if rays_c.dtype != torch.float32 or tuple(rays_c.shape) != (V, H, W, 6):
-            raise RuntimeError(f"rays must be float32 [V,H,W,6] = {(V, H, W, 6)}, got {tuple(rays_c.shape)}")
-        if rays_c.device != dev:
-            raise RuntimeError(f"rays must live on {dev}, got {rays_c.device}")
-    cams = R.pack_cameras(settings_list, dev)
-    color, allmap, radii, state = R.forward_views_raw(
-        centers_c, shs_c, None, opac_c, scales_c, rot_c, None, cams, tfx, tfy, H, W, deg,
-        prefiltered=prefiltered, debug=debug, raw_activations=raw_activations, for_backward=for_backward,
-        keep_list=keep_list)
-    return ((*_epilogue_forward(color, allmap, rays_c, cams, depth_ratio), radii),
-            ((centers_c, shs_c, scales_c, rot_c), rays_c, cams, color, allmap, state, (H, W, tfx, tfy, deg, debug)))
-
-
 def _epilogue_forward(color, allmap, rays_c, cams, depth_ratio):
     """The six render_img outputs of the rasterizer's stacked color / allmap (only the clamped image without rays)."""
     V, _, H, W = color.shape
@@ -96,24 +70,42 @@ def _epilogue_backward(color, allmap, rays, cams, depth_ratio, has_rays, g_image
     return d_color, torch.zeros_like(allmap)
 
 
+def _views_forward(inputs, rays_c, settings, geometry, prefiltered, depth_ratio, raw_activations, for_backward,
+                   keep_list=False):
+    """The rasterizer forward of the S*V views of S scenes and the fused epilogue: ``inputs`` the checked [S,P,...]
+    centers, shs, opacity, scales and rotations, ``settings`` the S*V checked view settings (scene s's views are
+    s*V .. s*V+V-1), ``geometry`` (H, W, tan_fovx per scene, tan_fovy per scene, sh degree, debug), ``rays_c``
+    [S*V,H,W,6] or None.  Returns the outputs (image, depth, acc, rn, dn, dist, radii) stacked [S*V, ...] and (cams,
+    color, allmap, state)."""
+    H, W, tfx, tfy, deg, debug = geometry
+    dev = inputs[0].device
+    cams = R.pack_cameras(settings, dev)
+    centers, shs, opacity, scales, rotations = inputs
+    with _DeviceGuard(dev):
+        color, allmap, radii, state = R.forward_batch_raw(
+            centers, shs, None, opacity, scales, rotations, None, cams, list(zip(tfx, tfy)), H, W, deg,
+            prefiltered=prefiltered, debug=debug, raw_activations=raw_activations, for_backward=for_backward, keep_list=keep_list)
+        outs = (*_epilogue_forward(color, allmap, rays_c, cams, depth_ratio), radii)
+    return outs, (cams, color, allmap, state)
+
+
 class _RenderSceneViews(torch.autograd.Function):
+    """One autograd node over the S*V views of S scenes (arguments as :func:`_views_forward`); the gradients of the
+    [S,P,...] inputs are each scene's sum over its own views."""
+
     @staticmethod
-    def forward(ctx, centers, shs, opacity, scales, rotations, rays, settings_list, depth_ratio, raw_activations,
-                keep=None):
-        outs, (inputs, rays_c, cams, color, allmap, state, geometry) = _scene_views_forward(
-            centers, shs, opacity, scales, rotations, rays, settings_list, depth_ratio, raw_activations, True)
+    def forward(ctx, centers, shs, opacity, scales, rotations, rays_c, settings, geometry, prefiltered, depth_ratio,
+                raw_activations, keep=None):
+        outs, (cams, color, allmap, state) = _views_forward(
+            (centers, shs, opacity, scales, rotations), rays_c, settings, geometry, prefiltered, depth_ratio,
+            raw_activations, True)
         if keep is not None:
-            keep.append((inputs[0], rays_c, cams, state, geometry))
-        centers_c, shs_c, scales_c, rot_c = inputs
+            keep.append((cams, state))
         radii = outs[-1]
-        ctx.save_for_backward(centers_c, shs_c, scales_c, rot_c, rays_c if rays_c is not None else centers_c.new_empty(0),
+        ctx.save_for_backward(centers, shs, scales, rotations, rays_c if rays_c is not None else color.new_empty(0),
                               cams, color, allmap, radii, state.geom, state.tile, state.image)
-        ctx.state = state
-        ctx.geometry = geometry
-        ctx.has_rays = rays_c is not None
-        ctx.depth_ratio = float(depth_ratio)
-        ctx.raw_activations = bool(raw_activations)
-        ctx.opac_shape = tuple(opacity.shape)
+        ctx.state, ctx.geometry, ctx.has_rays = state, geometry, rays_c is not None
+        ctx.depth_ratio, ctx.raw_activations, ctx.opac_shape = float(depth_ratio), bool(raw_activations), tuple(opacity.shape)
         ctx.mark_non_differentiable(radii)
         return outs
 
@@ -121,13 +113,32 @@ class _RenderSceneViews(torch.autograd.Function):
     def backward(ctx, g_image, g_depth, g_acc, g_rn, g_dn, g_dist, _g_radii):
         centers, shs, scales, rot, rays, cams, color, allmap, radii, _geom, _tile, _image = ctx.saved_tensors
         H, W, tfx, tfy, deg, debug = ctx.geometry
-
         d_color, d_allmap = _epilogue_backward(color, allmap, rays, cams, ctx.depth_ratio, ctx.has_rays, g_image, g_depth,
                                                g_acc, g_rn, g_dn, g_dist)
-        g = R.backward_views_raw(ctx.state, radii, centers, shs, None, scales, rot, None, cams, tfx, tfy, H, W, deg,
-                                 d_color, d_allmap, need_means2D=False, raw_activations=ctx.raw_activations, debug=debug)
+        g = R.backward_batch_raw(ctx.state, radii, centers, shs, scales, rot, cams, list(zip(tfx, tfy)), H, W, deg,
+                                 d_color, d_allmap,
+                                 raw_activations=ctx.raw_activations, debug=debug)
         return (g["means3D"], g["sh"], g["opacities"].view(ctx.opac_shape), g["scales"], g["rotations"],
-                None, None, None, None, None)
+                None, None, None, None, None, None, None)
+
+
+def _render_views(inputs, rays_c, settings, geometry, prefiltered, depth_ratio, raw_activations, keep_binning, tensors):
+    """:class:`_RenderSceneViews` when a gradient can flow, else the forward-only path; returns the outputs of
+    :func:`_views_forward` and, with ``keep_binning``, the :class:`SceneBinning` of the call (``tensors``: the caller's
+    five Gaussian tensors), else None."""
+    keep = [] if keep_binning else None
+    if R.needs_backward(*tensors, rays_c):
+        outs = _RenderSceneViews.apply(*inputs, rays_c, settings, geometry, prefiltered, depth_ratio, raw_activations,
+                                       keep)
+    else:
+        outs, (cams, _, _, state) = _views_forward(inputs, rays_c, settings, geometry, prefiltered, depth_ratio,
+                                                   raw_activations, False, keep_list=keep_binning)
+        if keep is not None:
+            keep.append((cams, state))
+    if not keep_binning:
+        return outs, None
+    cams, state = keep[0]
+    return outs, SceneBinning(state, outs[-1], inputs[0], cams, geometry, rays_c, depth_ratio, raw_activations, tensors)
 
 
 def render_scene_views(centers, shs, opacity, scales, rotations, settings_list: Sequence[R.GaussianRasterizationSettings],
@@ -144,20 +155,30 @@ def render_scene_views(centers, shs, opacity, scales, rotations, settings_list: 
     :func:`render_subset_views` renders a masked subset of these Gaussians from."""
     if len(settings_list) == 0:
         raise ValueError("render_scene_views needs at least one view")
-    args = (centers, shs, opacity, scales, rotations, rays, list(settings_list), float(depth_ratio), bool(raw_activations))
-    keep = [] if keep_binning else None
-    if R.needs_backward(centers, shs, opacity, scales, rotations, rays):
-        image, depth, acc, rn, dn, dist, radii = _RenderSceneViews.apply(*args, keep)
-    else:
-        (image, depth, acc, rn, dn, dist, radii), (inputs, rays_c, cams, _, _, state, geometry) = _scene_views_forward(
-            *args, False, keep_list=keep_binning)
-        if keep is not None:
-            keep.append((inputs[0], rays_c, cams, state, geometry))
-    out = _out_dict(image, depth, acc, rn, dn, dist, radii, rays is not None, prex)
-    if keep_binning:
-        means, rays_c, cams, state, geometry = keep[0]
-        out["binning" + prex] = SceneBinning(state, radii, means, cams, geometry, rays_c, float(depth_ratio),
-                                             bool(raw_activations), (centers, shs, opacity, scales, rotations))
+    dev = centers.device
+    V = len(settings_list)
+    centers_c, shs_c, _, opac_c, scales_c, rot_c, _ = R._normalise_inputs(
+        centers, shs, None, opacity, scales, rotations, None)
+    settings = [R._check_settings(rs, dev) for rs in settings_list]
+    H, W, tfx, tfy, deg, prefiltered, debug = shared_view_settings(settings)
+    rays_c = None
+    if rays is not None:
+        rays_c = rays.contiguous()
+        if rays_c.dtype != torch.float32 or tuple(rays_c.shape) != (V, H, W, 6):
+            raise RuntimeError(f"rays must be float32 [V,H,W,6] = {(V, H, W, 6)}, got {tuple(rays_c.shape)}")
+        if rays_c.device != dev:
+            raise RuntimeError(f"rays must live on {dev}, got {rays_c.device}")
+    # one scene: S = 1, whose [S*V, ...] outputs are the [V, ...] ones.  With P = 0 the checks read the empty scales and
+    # rotations as absent; the node takes the caller's empty tensors instead, which then receive empty gradients
+    inputs = tuple(None if t is None else t.unsqueeze(0)
+                   for t in (centers_c, shs_c, opac_c, scales if scales_c is None else scales_c,
+                             rotations if rot_c is None else rot_c))
+    outs, binning = _render_views(inputs, rays_c, settings, (H, W, (tfx,), (tfy,), deg, debug), prefiltered,
+                                  float(depth_ratio), bool(raw_activations), keep_binning,
+                                  (centers, shs, opacity, scales, rotations))
+    out = _out_dict(*outs, rays is not None, prex)
+    if binning is not None:
+        out["binning" + prex] = binning
     return out
 
 
@@ -172,15 +193,18 @@ def _out_dict(image, depth, acc, rn, dn, dist, radii, has_rays, prex):
 
 
 class SceneBinning:
-    """What a ``render_scene_views(..., keep_binning=True)`` call leaves for :func:`render_subset_views`: the coarse
-    forward's state (records, depths, tile rectangles, radii and depth-sorted tile lists of every view), its cameras,
-    settings, rays, ``depth_ratio`` and ``raw_activations`` flag, and the five Gaussian tensors with their
-    ``_version`` at the call.  Opaque: hand it to :func:`render_subset_views` as it is."""
-    __slots__ = ("state", "radii", "means", "cams", "geometry", "rays", "depth_ratio", "raw_activations", "tensors",
-                 "versions")
+    """What a ``render_scene_views`` / ``render_batch_views(..., keep_binning=True)`` call leaves for
+    :func:`render_subset_views` / :func:`render_batch_subset_views`: the coarse forward's state (records, depths, tile
+    rectangles, radii and depth-sorted tile lists of every view), its ``scenes`` S, the checked centers ([P,3] or
+    [S,P,3]), its cameras, geometry (H, W, tan_fovx and tan_fovy per scene, SH degree, debug), rays, ``depth_ratio`` and
+    ``raw_activations`` flag, and the caller's five Gaussian tensors with their ``_version`` at the call.  Opaque: hand
+    it to the subset render as it is."""
+    __slots__ = ("state", "radii", "means", "scenes", "cams", "geometry", "rays", "depth_ratio", "raw_activations",
+                 "tensors", "versions")
 
     def __init__(self, state, radii, means, cams, geometry, rays, depth_ratio, raw_activations, tensors):
         self.state, self.radii, self.means, self.cams, self.geometry = state, radii, means, cams, geometry
+        self.scenes = int(means.shape[0]) if means.ndim == 3 else 1
         self.rays, self.depth_ratio, self.raw_activations, self.tensors = rays, depth_ratio, raw_activations, tensors
         # inference tensors keep no version counter (None: not checked)
         self.versions = tuple(None if t.is_inference() else t._version for t in tensors + (radii,))
@@ -193,81 +217,116 @@ class SceneBinning:
                                    "render_scene_views call, so its binning no longer describes these Gaussians")
 
 
-def _subset_forward(b: SceneBinning, idx, shs_c, for_backward):
-    """srf_views_subset_forward on the coarse state and the fused epilogue.  Returns the outputs (image, depth, acc, rn,
-    dn, dist, radii) and (color, allmap, state) for the backward."""
+def _subset_forward(b: SceneBinning, idx, shs_c, for_backward, offsets=None, counts=None):
+    """srf_scenes_subset_forward on the coarse state and the fused epilogue: ``idx`` the concatenated per-scene subsets,
+    ``offsets`` / ``counts`` their device [S+1] bounds and host counts (None: one scene, its n = idx.numel()).  Returns
+    the outputs (image, depth, acc, rn, dn, dist, radii [S*V, n_max]) and (color, allmap, state) for the backward."""
     lib = _lib.load()
     st = b.state
     dev = b.means.device
     H, W, _, _, deg, debug = b.geometry
-    V, P, n, M = st.nviews, int(b.means.shape[0]), int(idx.numel()), int(shs_c.shape[1])
+    S, P = b.scenes, int(b.means.shape[-2])
+    n, M = int(idx.numel()), int(shs_c.shape[1])
+    counts = [n] if counts is None else counts
+    V, n_max = st.nviews, max(counts)
     color = torch.empty((V, 3, H, W), dtype=torch.float32, device=dev)
     allmap = torch.empty((V, 8, H, W), dtype=torch.float32, device=dev)
-    radii = torch.empty((V, n), dtype=torch.int32, device=dev)
-    if n == 0:
-        # what a forward of zero Gaussians returns (rasterizer._forward): zero-filled outputs, nothing rendered
-        color.zero_(); allmap.zero_()
-        geom_b, tile_b, image_b = R._views_sizes(lib, V, 0, H, W, 0, for_backward)[:3]
-        image = torch.zeros(image_b, dtype=torch.uint8, device=dev) if for_backward else None
-        pl = torch.empty((0,), dtype=torch.int32, device=dev)
-        state = R.ForwardState(R._blob(geom_b, dev), torch.zeros(tile_b, dtype=torch.uint8, device=dev), image,
-                               pl if for_backward else None, 0, 0, nviews=V, cams=b.cams, for_backward=for_backward)
-    else:
-        counts = st.resolve()       # capacity verified (stage 2 re-run if it overflowed) before the lists are read
-        capacity = st.capacity
-        geom_b, tile_b, image_b, _, pl_b = R._views_sizes(lib, V, n, H, W, capacity, for_backward)[:5]
-        blob = R._blob(geom_b + tile_b + image_b, dev)
-        geom, tile = blob[:geom_b], blob[geom_b:geom_b + tile_b]
-        image = blob[geom_b + tile_b:] if for_backward else None
-        point_list = R._blob(pl_b, dev)
-        _lib.launch(
-            "srf_views_subset_forward", dev, V, P, n, int(deg), M, idx.data_ptr(), b.means.data_ptr(), shs_c.data_ptr(),
-            None, b.cams.data_ptr(), H, W, capacity, b.radii.data_ptr(), st.geom.data_ptr(), st.tile.data_ptr(),
-            st.point_list.data_ptr(), capacity, 1 if st.for_backward else 0, radii.data_ptr(), geom.data_ptr(),
-            tile.data_ptr(), point_list.data_ptr(), _ptr(image), color.data_ptr(), allmap.data_ptr(),
-            R._blob(_lib.subset_workspace_bytes(lib, P), dev).data_ptr(), 1 if for_backward else 0)
-        # the kept entries sit at the coarse list positions: the list's extent is the coarse one
-        state = R.ForwardState(geom, tile, image, point_list if for_backward else None, capacity, counts, nviews=V,
-                               cams=b.cams, for_backward=for_backward)
-        if debug:
-            torch.cuda.synchronize(dev)
+    radii = torch.empty((V, n_max), dtype=torch.int32, device=dev)
+    counts_coarse = st.resolve()    # capacity verified (stage 2 re-run if it overflowed) before the lists are read
+    capacity = st.capacity
+    geom_b, tile_b, image_b, _, pl_b = R._views_sizes(lib, V, n_max, H, W, capacity, for_backward)[:5]
+    blob = R._blob(geom_b + tile_b + image_b, dev)
+    geom, tile = blob[:geom_b], blob[geom_b:geom_b + tile_b]
+    image = blob[geom_b + tile_b:] if for_backward else None
+    point_list = R._blob(pl_b, dev)
+    _lib.launch(
+        "srf_scenes_subset_forward", dev, S, V // S, P, n, n_max, int(deg), M, _ptr(idx), _ptr(offsets),
+        b.means.data_ptr(), _ptr(shs_c), None, b.cams.data_ptr(), H, W, capacity, b.radii.data_ptr(),
+        st.geom.data_ptr(), st.tile.data_ptr(), _ptr(st.point_list), capacity, 1 if st.for_backward else 0,
+        radii.data_ptr(), geom.data_ptr(), tile.data_ptr(), point_list.data_ptr(), _ptr(image), color.data_ptr(),
+        allmap.data_ptr(), R._blob(_lib.subset_workspace_bytes(lib, S * P), dev).data_ptr(), 1 if for_backward else 0)
+    Vs = V // S
+    for s, c in enumerate(counts):
+        if c == 0:      # a scene with an empty mask renders what a forward of zero Gaussians renders: zeros
+            color[s * Vs:(s + 1) * Vs].zero_()
+            allmap[s * Vs:(s + 1) * Vs].zero_()
+    # the kept entries sit at the coarse list positions: the list's extent is the coarse one
+    state = R.ForwardState(geom, tile, image, point_list if for_backward else None, capacity, counts_coarse, nviews=V,
+                           cams=b.cams, for_backward=for_backward)
+    if debug:
+        torch.cuda.synchronize(dev)
     return ((*_epilogue_forward(color, allmap, b.rays, b.cams, b.depth_ratio), radii), (color, allmap, state))
 
 
 class _RenderSubsetViews(torch.autograd.Function):
-    """Inputs: the full-size coarse centers, opacity, scales and rotations and ``shs_fine``; the gradients of the coarse
-    tensors are the subset's in rows ``idx`` and zero elsewhere."""
+    """Inputs: the coarse centers, opacity, scales and rotations as the coarse render took them (S*P rows) and the
+    concatenated ``shs_fine``; the gradients of the coarse tensors are the subsets' in their rows and zero elsewhere."""
 
     @staticmethod
-    def forward(ctx, binning, idx, shs_c, centers, opacity, scales, rotations):
-        outs, (color, allmap, state) = _subset_forward(binning, idx, shs_c, True)
+    def forward(ctx, binning, nz, idx, offsets, counts, shs_c, centers, opacity, scales, rotations):
+        outs, (color, allmap, state) = _subset_forward(binning, idx, shs_c, True, offsets, counts)
         radii = outs[-1]
-        ctx.save_for_backward(idx, shs_c, centers, scales, rotations, color, allmap, radii, state.geom, state.tile,
-                              state.image)
-        ctx.binning, ctx.state, ctx.opac_shape = binning, state, tuple(opacity.shape)
+        ctx.save_for_backward(nz, idx, offsets, shs_c, centers, scales, rotations, color, allmap, radii, state.geom,
+                              state.tile, state.image)
+        ctx.binning, ctx.state, ctx.n_max, ctx.opac_shape = binning, state, max(counts), tuple(opacity.shape)
         ctx.mark_non_differentiable(radii)
         return outs
 
     @staticmethod
     def backward(ctx, g_image, g_depth, g_acc, g_rn, g_dn, g_dist, _g_radii):
-        idx, shs, centers, scales, rotations, color, allmap, radii, _geom, _tile, _image = ctx.saved_tensors
+        nz, idx, offsets, shs, centers, scales, rotations, color, allmap, radii, _geom, _tile, _image = ctx.saved_tensors
         b = ctx.binning
         H, W, tfx, tfy, deg, debug = b.geometry
+        P = int(b.means.shape[-2])
+        SP = b.scenes * P
         d_color, d_allmap = _epilogue_backward(color, allmap, b.rays, b.cams, b.depth_ratio, b.rays is not None,
                                                g_image, g_depth, g_acc, g_rn, g_dn, g_dist)
-        # the per-Gaussian backward reads the n rows of the subset (a gather, exact); its gradients go to rows idx
-        rows = [t.index_select(0, idx).contiguous() for t in (centers, scales, rotations)]
-        g = R.backward_views_raw(ctx.state, radii, rows[0], shs, None, rows[1], rows[2], None, b.cams, tfx, tfy, H, W,
-                                 deg, d_color, d_allmap, need_means2D=False, raw_activations=b.raw_activations,
-                                 debug=debug)
+        # the per-Gaussian backward reads the n subset rows of the flattened [S*P] coarse tensors (a gather, exact):
+        # scene s's local index + s*P; its gradients go back to those rows
+        rows_idx = nz[:, 0] * P + idx
+        rows = [t.reshape(SP, -1).index_select(0, rows_idx).contiguous() for t in (centers, scales, rotations)]
+        g = R.backward_batch_raw(ctx.state, radii, rows[0], shs, rows[1], rows[2], b.cams, list(zip(tfx, tfy)), H, W,
+                                 deg, d_color, d_allmap, offsets=offsets, P=ctx.n_max, raw_activations=b.raw_activations, debug=debug)
 
         def scatter(gn, shape):
             full = torch.zeros(shape, dtype=torch.float32, device=idx.device)
             if idx.numel():
-                full.view(shape[0], -1)[idx] = gn.view(idx.numel(), -1)      # idx is unique: an exact copy per row
+                full.view(SP, -1)[rows_idx] = gn.reshape(idx.numel(), -1)     # unique rows: an exact copy per row
             return full
-        return (None, None, g["sh"], scatter(g["means3D"], tuple(centers.shape)), scatter(g["opacities"], ctx.opac_shape),
-                scatter(g["scales"], tuple(scales.shape)), scatter(g["rotations"], tuple(rotations.shape)))
+        return (None, None, None, None, None, g["sh"], scatter(g["means3D"], tuple(centers.shape)),
+                scatter(g["opacities"], ctx.opac_shape), scatter(g["scales"], tuple(scales.shape)),
+                scatter(g["rotations"], tuple(rotations.shape)))
+
+
+def _render_subset(fn, binning: SceneBinning, masks, shs_fine):
+    """The subset render of every scene of ``binning`` (checked, unchanged) with ``masks`` [S,P] (checked) and
+    ``shs_fine`` [n,M,3]; ``fn`` names the caller in messages.  Returns the outputs of :func:`_subset_forward` and the
+    per-scene counts.  One host sync, for the counts."""
+    centers, _, opacity, scales, rotations = binning.tensors
+    S, dev = binning.scenes, binning.means.device
+    deg = binning.geometry[4]
+    if not isinstance(shs_fine, torch.Tensor) or shs_fine.dtype != torch.float32 or shs_fine.device != dev or \
+            shs_fine.ndim != 3 or shs_fine.shape[2] != 3 or shs_fine.shape[1] < (deg + 1) ** 2:
+        raise RuntimeError(f"{fn}: shs_fine must be float32 [n, M >= {(deg + 1) ** 2}, 3] on {dev}, got "
+                           f"{getattr(shs_fine, 'dtype', type(shs_fine))} {tuple(getattr(shs_fine, 'shape', ()))}")
+    counts_d = masks.sum(1)
+    counts = [int(c) for c in counts_d.tolist()]        # the host sync
+    n = sum(counts)
+    if shs_fine.shape[0] != n:
+        raise RuntimeError(f"{fn}: shs_fine has {shs_fine.shape[0]} rows, the mask selects {n}")
+    nz = torch.nonzero_static(masks, size=n)        # (scene, index) pairs, scene-major, ascending within a scene
+    idx = nz[:, 1].contiguous()
+    offsets = None          # one scene: the C entry takes idx[0..n) without offsets and waits for nothing
+    if S > 1:
+        offsets = torch.zeros(S + 1, dtype=torch.int64, device=dev)
+        torch.cumsum(counts_d, 0, out=offsets[1:])
+    shs_c = shs_fine.contiguous()
+    with _DeviceGuard(dev):
+        if R.needs_backward(centers, shs_fine, opacity, scales, rotations):
+            outs = _RenderSubsetViews.apply(binning, nz, idx, offsets, counts, shs_c, centers, opacity, scales, rotations)
+        else:
+            outs = _subset_forward(binning, idx, shs_c, False, offsets, counts)[0]
+    return outs, counts
 
 
 def render_subset_views(binning: SceneBinning, mask: torch.Tensor, shs_fine: torch.Tensor,
@@ -277,31 +336,17 @@ def render_subset_views(binning: SceneBinning, mask: torch.Tensor, shs_fine: tor
     a bool tensor [P] on the Gaussians' device, ``shs_fine`` the subset's SH coefficients [n, M, 3].  Returns the dict
     ``render_scene_views`` returns for the gathered subset (same keys, layout and bits, ``radii`` [V, n]) without a
     preprocess, scatter or sort: the coarse records are copied with a new colour and the coarse tile lists filtered to
-    the mask.  One host sync (the ``nonzero`` of the mask).  The gradients of the coarse centers, opacity, scales and
+    the mask.  One host sync (the mask count).  The gradients of the coarse centers, opacity, scales and
     rotations are those of the gathered path; under ``no_grad`` / ``inference_mode`` the forward-only path is taken."""
-    if not isinstance(binning, SceneBinning):
+    if not isinstance(binning, SceneBinning) or binning.scenes != 1:
         raise TypeError("render_subset_views: binning must be out['binning'] of render_scene_views(..., keep_binning=True)")
     binning.check_unchanged()
-    centers, _, opacity, scales, rotations = binning.tensors
-    P, dev = int(binning.means.shape[0]), binning.means.device
+    P, dev = int(binning.means.shape[-2]), binning.means.device
     if not isinstance(mask, torch.Tensor) or mask.dtype != torch.bool or tuple(mask.shape) != (P,) or mask.device != dev:
         raise RuntimeError(f"render_subset_views: mask must be a bool tensor [{P}] on {dev}, got "
                            f"{getattr(mask, 'dtype', type(mask))} {tuple(getattr(mask, 'shape', ()))} on "
                            f"{getattr(mask, 'device', None)}")
-    deg = binning.geometry[4]
-    if not isinstance(shs_fine, torch.Tensor) or shs_fine.dtype != torch.float32 or shs_fine.device != dev or \
-            shs_fine.ndim != 3 or shs_fine.shape[2] != 3 or shs_fine.shape[1] < (deg + 1) ** 2:
-        raise RuntimeError(f"render_subset_views: shs_fine must be float32 [n, M >= {(deg + 1) ** 2}, 3] on {dev}, got "
-                           f"{getattr(shs_fine, 'dtype', type(shs_fine))} {tuple(getattr(shs_fine, 'shape', ()))}")
-    idx = mask.nonzero().view(-1)
-    if shs_fine.shape[0] != idx.numel():
-        raise RuntimeError(f"render_subset_views: shs_fine has {shs_fine.shape[0]} rows, the mask selects {idx.numel()}")
-    shs_c = shs_fine.contiguous()
-    with _DeviceGuard(dev):
-        if R.needs_backward(centers, shs_fine, opacity, scales, rotations):
-            outs = _RenderSubsetViews.apply(binning, idx, shs_c, centers, opacity, scales, rotations)
-        else:
-            outs = _subset_forward(binning, idx, shs_c, False)[0]
+    outs, _ = _render_subset("render_subset_views", binning, mask[None], shs_fine)
     return _out_dict(*outs, binning.rays is not None, prex)
 
 
@@ -359,59 +404,6 @@ def _batch_inputs(centers, shs, opacity, scales, rotations):
                                             (scales, "scales"), (rotations, "rotations")))
 
 
-def _batch_forward(centers, shs, opacity, scales, rotations, rays, settings, depth_ratio, raw_activations, for_backward,
-                   keep_list=False):
-    """Checks, the batched rasterizer forward and the fused epilogue over the B*V views.  Returns the outputs (image,
-    depth, acc, rn, dn, dist, radii), stacked [B*V, ...], and (inputs, rays, cams, color, allmap, state, geometry)."""
-    dev = centers.device
-    inputs = _batch_inputs(centers, shs, opacity, scales, rotations)
-    settings = [[R._check_settings(rs, dev) for rs in s] for s in settings]
-    H, W, tan_fov, deg, prefiltered, debug = batch_view_settings(settings)
-    B, V = len(settings), len(settings[0])
-    rays_c = None
-    if rays is not None:
-        rays_c = rays.contiguous()
-        if rays_c.dtype != torch.float32 or tuple(rays_c.shape) != (B, V, H, W, 6) or rays_c.device != dev:
-            raise RuntimeError(f"rays must be float32 [B,V,H,W,6] = {(B, V, H, W, 6)} on {dev}, got "
-                               f"{rays_c.dtype} {tuple(rays_c.shape)} on {rays_c.device}")
-        rays_c = rays_c.view(B * V, H, W, 6)
-    cams = R.pack_cameras([rs for s in settings for rs in s], dev)
-    centers_c, shs_c, opac_c, scales_c, rot_c = inputs
-    with _DeviceGuard(dev):
-        color, allmap, radii, state = R.forward_batch_raw(
-            centers_c, shs_c, None, opac_c, scales_c, rot_c, None, cams, tan_fov, H, W, deg, prefiltered=prefiltered,
-            debug=debug, raw_activations=raw_activations, for_backward=for_backward, keep_list=keep_list)
-        outs = (*_epilogue_forward(color, allmap, rays_c, cams, depth_ratio), radii)
-    return outs, ((centers_c, shs_c, scales_c, rot_c), rays_c, cams, color, allmap, state, (H, W, tan_fov, deg, debug))
-
-
-class _RenderBatchViews(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, centers, shs, opacity, scales, rotations, rays, settings, depth_ratio, raw_activations, keep=None):
-        outs, (inputs, rays_c, cams, color, allmap, state, geometry) = _batch_forward(
-            centers, shs, opacity, scales, rotations, rays, settings, depth_ratio, raw_activations, True)
-        if keep is not None:
-            keep.append((inputs[0], rays_c, cams, state, geometry))
-        radii = outs[-1]
-        ctx.save_for_backward(*inputs, rays_c if rays_c is not None else color.new_empty(0), cams, color, allmap, radii,
-                              state.geom, state.tile, state.image)
-        ctx.state, ctx.geometry, ctx.has_rays = state, geometry, rays_c is not None
-        ctx.depth_ratio, ctx.raw_activations, ctx.opac_shape = float(depth_ratio), bool(raw_activations), tuple(opacity.shape)
-        ctx.mark_non_differentiable(radii)
-        return outs
-
-    @staticmethod
-    def backward(ctx, g_image, g_depth, g_acc, g_rn, g_dn, g_dist, _g_radii):
-        centers, shs, scales, rot, rays, cams, color, allmap, radii, _geom, _tile, _image = ctx.saved_tensors
-        H, W, tan_fov, deg, debug = ctx.geometry
-        d_color, d_allmap = _epilogue_backward(color, allmap, rays, cams, ctx.depth_ratio, ctx.has_rays, g_image, g_depth,
-                                               g_acc, g_rn, g_dn, g_dist)
-        g = R.backward_batch_raw(ctx.state, radii, centers, shs, scales, rot, cams, tan_fov, H, W, deg, d_color, d_allmap,
-                                 raw_activations=ctx.raw_activations, debug=debug)
-        return (g["means3D"], g["sh"], g["opacities"].view(ctx.opac_shape), g["scales"], g["rotations"],
-                None, None, None, None, None)
-
-
 def _batch_out_dict(outs, B, has_rays, prex):
     """{key: [B,V,...]} of the [B*V,...] outputs, the layout of :func:`render_scene_views` per scene."""
     out = _out_dict(*outs, has_rays, prex)
@@ -427,164 +419,51 @@ def render_batch_views(centers, shs, opacity, scales, rotations,
     view settings, ``rays`` [B,V,H,W,6] or None.  Returns ``{key+prex: [B,V,...]}``, where ``out[k][b]`` is what
     :func:`render_scene_views` returns for scene b alone (bit for bit), and ``radii+prex`` [B,V,P].  Scenes may differ
     in field of view and background; they must share V, the image size and the SH degree.  No-grad renders take the
-    forward-only path.  ``keep_binning=True`` adds ``out["binning"+prex]``, a :class:`BatchBinning` for
+    forward-only path.  ``keep_binning=True`` adds ``out["binning"+prex]``, a :class:`SceneBinning` of B scenes for
     :func:`render_batch_subset_views`."""
-    settings = [list(s) for s in settings]
-    args = (centers, shs, opacity, scales, rotations, rays, settings, float(depth_ratio), bool(raw_activations))
-    keep = [] if keep_binning else None
-    if R.needs_backward(centers, shs, opacity, scales, rotations, rays):
-        outs = _RenderBatchViews.apply(*args, keep)
-    else:
-        outs, (inputs, rays_c, cams, _, _, state, geometry) = _batch_forward(*args, False, keep_list=keep_binning)
-        if keep is not None:
-            keep.append((inputs[0], rays_c, cams, state, geometry))
-    B = len(settings)
+    dev = centers.device
+    inputs = _batch_inputs(centers, shs, opacity, scales, rotations)
+    settings = [[R._check_settings(rs, dev) for rs in s] for s in settings]
+    H, W, tan_fov, deg, prefiltered, debug = batch_view_settings(settings)
+    B, V = len(settings), len(settings[0])
+    rays_c = None
+    if rays is not None:
+        rays_c = rays.contiguous()
+        if rays_c.dtype != torch.float32 or tuple(rays_c.shape) != (B, V, H, W, 6) or rays_c.device != dev:
+            raise RuntimeError(f"rays must be float32 [B,V,H,W,6] = {(B, V, H, W, 6)} on {dev}, got "
+                               f"{rays_c.dtype} {tuple(rays_c.shape)} on {rays_c.device}")
+        rays_c = rays_c.view(B * V, H, W, 6)
+    tfx, tfy = zip(*tan_fov)
+    outs, binning = _render_views(inputs, rays_c, [rs for s in settings for rs in s], (H, W, tfx, tfy, deg, debug),
+                                  prefiltered, float(depth_ratio), bool(raw_activations), keep_binning,
+                                  (centers, shs, opacity, scales, rotations))
     out = _batch_out_dict(outs, B, rays is not None, prex)
-    if keep_binning:
-        means, rays_c, cams, state, geometry = keep[0]
-        out["binning" + prex] = BatchBinning(state, outs[-1], means, cams, geometry, rays_c, float(depth_ratio),
-                                             bool(raw_activations), (centers, shs, opacity, scales, rotations))
+    if binning is not None:
+        out["binning" + prex] = binning
     return out
 
 
-class BatchBinning(SceneBinning):
-    """What ``render_batch_views(..., keep_binning=True)`` leaves for :func:`render_batch_subset_views`: a
-    :class:`SceneBinning` of the batch's B*V views, whose ``means`` are [B,P,3] and whose ``geometry`` holds the
-    per-scene fields of view.  Opaque."""
-    __slots__ = ()
-
-
-def _batch_subset_forward(b: BatchBinning, idx, offsets, counts, shs_c, for_backward):
-    """srf_scenes_subset_forward on the coarse state and the fused epilogue.  Returns the outputs (image, depth, acc, rn,
-    dn, dist, radii [B*V, n_max]) and (color, allmap, state, n_max) for the backward."""
-    lib = _lib.load()
-    st = b.state
-    dev = b.means.device
-    H, W, _, deg, debug = b.geometry
-    B, P = int(b.means.shape[0]), int(b.means.shape[1])
-    V, n, M, n_max = st.nviews, int(idx.numel()), int(shs_c.shape[1]), max(counts)
-    color = torch.empty((V, 3, H, W), dtype=torch.float32, device=dev)
-    allmap = torch.empty((V, 8, H, W), dtype=torch.float32, device=dev)
-    radii = torch.empty((V, n_max), dtype=torch.int32, device=dev)
-    st.resolve()       # capacity verified (stage 2 re-run if it overflowed) before the lists are read
-    capacity = st.capacity
-    geom_b, tile_b, image_b, _, pl_b = R._views_sizes(lib, V, n_max, H, W, capacity, for_backward)[:5]
-    blob = R._blob(geom_b + tile_b + image_b, dev)
-    geom, tile = blob[:geom_b], blob[geom_b:geom_b + tile_b]
-    image = blob[geom_b + tile_b:] if for_backward else None
-    point_list = R._blob(pl_b, dev)
-    _lib.launch(
-        "srf_scenes_subset_forward", dev, B, V // B, P, n, n_max, int(deg), M, idx.data_ptr(), offsets.data_ptr(),
-        b.means.data_ptr(), shs_c.data_ptr(), None, b.cams.data_ptr(), H, W, capacity, b.radii.data_ptr(),
-        st.geom.data_ptr(), st.tile.data_ptr(), st.point_list.data_ptr(), capacity, 1 if st.for_backward else 0,
-        radii.data_ptr(), geom.data_ptr(), tile.data_ptr(), point_list.data_ptr(), _ptr(image), color.data_ptr(),
-        allmap.data_ptr(), R._blob(_lib.subset_workspace_bytes(lib, B * P), dev).data_ptr(), 1 if for_backward else 0)
-    Vs = V // B
-    for s, c in enumerate(counts):
-        if c == 0:      # a scene with an empty mask renders what a forward of zero Gaussians renders: zeros
-            color[s * Vs:(s + 1) * Vs].zero_()
-            allmap[s * Vs:(s + 1) * Vs].zero_()
-    state = R.ForwardState(geom, tile, image, point_list if for_backward else None, capacity, st.resolve(), nviews=V,
-                           cams=b.cams, for_backward=for_backward)
-    if debug:
-        torch.cuda.synchronize(dev)
-    return ((*_epilogue_forward(color, allmap, b.rays, b.cams, b.depth_ratio), radii), (color, allmap, state, n_max))
-
-
-class _RenderBatchSubsetViews(torch.autograd.Function):
-    """Inputs: the full-size [B,P,...] coarse centers, opacity, scales and rotations and the concatenated ``shs_fine``;
-    the gradients of the coarse tensors are the subsets' in their rows and zero elsewhere."""
-
-    @staticmethod
-    def forward(ctx, binning, idx, offsets, counts, shs_c, centers, opacity, scales, rotations):
-        outs, (color, allmap, state, n_max) = _batch_subset_forward(binning, idx, offsets, counts, shs_c, True)
-        radii = outs[-1]
-        ctx.save_for_backward(idx, offsets, shs_c, centers, scales, rotations, color, allmap, radii, state.geom,
-                              state.tile, state.image)
-        ctx.binning, ctx.state, ctx.n_max, ctx.counts, ctx.opac_shape = binning, state, n_max, counts, tuple(opacity.shape)
-        ctx.mark_non_differentiable(radii)
-        return outs
-
-    @staticmethod
-    def backward(ctx, g_image, g_depth, g_acc, g_rn, g_dn, g_dist, _g_radii):
-        idx, offsets, shs, centers, scales, rotations, color, allmap, radii, _geom, _tile, _image = ctx.saved_tensors
-        b = ctx.binning
-        H, W, tan_fov, deg, debug = b.geometry
-        B, P = int(centers.shape[0]), int(centers.shape[1])
-        d_color, d_allmap = _epilogue_backward(color, allmap, b.rays, b.cams, b.depth_ratio, b.rays is not None,
-                                               g_image, g_depth, g_acc, g_rn, g_dn, g_dist)
-        # rows of the flattened [B*P] coarse tensors: scene s's local index + s*P
-        scene = torch.repeat_interleave(torch.arange(B, device=idx.device),
-                                        torch.tensor(ctx.counts, device=idx.device), output_size=int(idx.numel()))
-        rows_idx = idx + scene * P
-        rows = [t.reshape(B * P, -1).index_select(0, rows_idx).contiguous() for t in (centers, scales, rotations)]
-        g = R.backward_batch_raw(ctx.state, radii, rows[0], shs, rows[1], rows[2], b.cams, tan_fov, H, W, deg, d_color,
-                                 d_allmap, offsets=offsets, P=ctx.n_max, raw_activations=b.raw_activations, debug=debug)
-
-        def scatter(gn, shape):
-            full = torch.zeros(shape, dtype=torch.float32, device=idx.device)
-            if idx.numel():
-                full.view(B * P, -1)[rows_idx] = gn.reshape(idx.numel(), -1)     # unique rows: an exact copy per row
-            return full
-        return (None, None, None, None, g["sh"], scatter(g["means3D"], tuple(centers.shape)),
-                scatter(g["opacities"], ctx.opac_shape), scatter(g["scales"], tuple(scales.shape)),
-                scatter(g["rotations"], tuple(rotations.shape)))
-
-
-def render_batch_subset_views(binning: BatchBinning, masks: torch.Tensor, shs_fine: torch.Tensor,
+def render_batch_subset_views(binning: SceneBinning, masks: torch.Tensor, shs_fine: torch.Tensor,
                               prex: str = "_fine") -> Dict[str, object]:
     """LaRa's fine pass for all B scenes of a batch from the coarse pass's binning: ``binning`` is ``out["binning"]`` of
     ``render_batch_views(..., keep_binning=True)``, ``masks`` a bool tensor [B,P], ``shs_fine`` [n,M,3] the subsets' SH
     coefficients concatenated in scene order (B calls of ``FineHead.fine_shs`` concatenated).  Returns ``{key+prex:
     [B,V,...]}`` where ``out[k][b]`` is what :func:`render_subset_views` returns for scene b alone, bit for bit, and
-    ``radii+prex`` a list of B tensors [V, n_b].  One host sync for the mask counts (and the C entry's check of the
-    offsets, which waits for the stream).  Gradients go to the [B,P,...] coarse tensors and to ``shs_fine``."""
-    if not isinstance(binning, BatchBinning):
+    ``radii+prex`` a list of B tensors [V, n_b].  One host sync for the mask counts (and, for B > 1, the C entry's check
+    of the offsets, which waits for the stream).  Gradients go to the [B,P,...] coarse tensors and to ``shs_fine``."""
+    if not isinstance(binning, SceneBinning):
         raise TypeError("render_batch_subset_views: binning must be out['binning'] of render_batch_views(..., "
                         "keep_binning=True)")
     binning.check_unchanged()
-    centers, _, opacity, scales, rotations = binning.tensors
-    B, P, dev = int(binning.means.shape[0]), int(binning.means.shape[1]), binning.means.device
+    B, P, dev = binning.scenes, int(binning.means.shape[-2]), binning.means.device
     if not isinstance(masks, torch.Tensor) or masks.dtype != torch.bool or tuple(masks.shape) != (B, P) or \
             masks.device != dev:
         raise RuntimeError(f"render_batch_subset_views: masks must be a bool tensor [{B},{P}] on {dev}, got "
                            f"{getattr(masks, 'dtype', type(masks))} {tuple(getattr(masks, 'shape', ()))} on "
                            f"{getattr(masks, 'device', None)}")
-    deg = binning.geometry[3]
-    if not isinstance(shs_fine, torch.Tensor) or shs_fine.dtype != torch.float32 or shs_fine.device != dev or \
-            shs_fine.ndim != 3 or shs_fine.shape[2] != 3 or shs_fine.shape[1] < (deg + 1) ** 2:
-        raise RuntimeError(f"render_batch_subset_views: shs_fine must be float32 [n, M >= {(deg + 1) ** 2}, 3] on {dev}, "
-                           f"got {getattr(shs_fine, 'dtype', type(shs_fine))} {tuple(getattr(shs_fine, 'shape', ()))}")
-    counts_d = masks.sum(1)
-    counts = [int(c) for c in counts_d.tolist()]        # the host sync
-    n = sum(counts)
-    if shs_fine.shape[0] != n:
-        raise RuntimeError(f"render_batch_subset_views: shs_fine has {shs_fine.shape[0]} rows, the masks select {n}")
-    idx = torch.nonzero_static(masks, size=n)[:, 1].contiguous()      # scene-major, ascending within a scene
-    offsets = torch.zeros(B + 1, dtype=torch.int64, device=dev)
-    torch.cumsum(counts_d, 0, out=offsets[1:])
-    shs_c = shs_fine.contiguous()
-    with _DeviceGuard(dev):
-        if n == 0:
-            # every mask empty: B*V renders of zero Gaussians, as render_subset_views gives them
-            outs = _empty_subset(binning, B, shs_c)
-        elif R.needs_backward(centers, shs_fine, opacity, scales, rotations):
-            outs = _RenderBatchSubsetViews.apply(binning, idx, offsets, counts, shs_c, centers, opacity, scales, rotations)
-        else:
-            outs = _batch_subset_forward(binning, idx, offsets, counts, shs_c, False)[0]
+    outs, counts = _render_subset("render_batch_subset_views", binning, masks, shs_fine)
     radii = outs[-1]
-    out = _batch_out_dict(outs[:-1] + (radii,), B, binning.rays is not None, prex)
+    out = _batch_out_dict(outs, B, binning.rays is not None, prex)
     V = radii.shape[0] // B
     out["radii" + prex] = [radii[b * V:(b + 1) * V, :counts[b]] for b in range(B)]
     return out
-
-
-def _empty_subset(b: BatchBinning, B, shs_c):
-    """The outputs of a batch subset render of zero Gaussians: the backgrounds (what a forward of zero Gaussians
-    renders, rasterizer._forward), through the epilogue; the autograd graph still reaches ``shs_fine``."""
-    V = b.state.nviews
-    H, W = b.geometry[0], b.geometry[1]
-    color = torch.zeros((V, 3, H, W), dtype=torch.float32, device=shs_c.device)
-    allmap = torch.zeros((V, 8, H, W), dtype=torch.float32, device=shs_c.device)
-    return (*_epilogue_forward(color, allmap, b.rays, b.cams, b.depth_ratio),
-            torch.empty((V, 0), dtype=torch.int32, device=shs_c.device))

@@ -278,7 +278,7 @@ def forward_raw(means3D, shs, colors_precomp, opacities, scales, rotations, tran
     rs = raster_settings
     with _DeviceGuard(means3D.device):
         return _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp,
-                        pack_cameras([rs], means3D.device), rs.tanfovx, rs.tanfovy, int(rs.image_height),
+                        pack_cameras([rs], means3D.device), [(rs.tanfovx, rs.tanfovy)], int(rs.image_height),
                         int(rs.image_width), rs.sh_degree, rs.prefiltered, rs.debug, raw_activations, single=True,
                         for_backward=for_backward)
 
@@ -287,17 +287,17 @@ def forward_views_raw(means3D, shs, colors_precomp, opacities, scales, rotations
                       cams: torch.Tensor, tanfovx: float, tanfovy: float, H: int, W: int, sh_degree: int,
                       prefiltered: bool = False, debug: bool = False, raw_activations: bool = False, *,
                       for_backward: bool = True, keep_list: bool = False):
-    """All V views of one Gaussian set in ONE launch set (srf_views_*): every kernel carries a view
+    """All V views of one Gaussian set in ONE launch set (srf_scenes_forward with S = 1): every kernel carries a view
     dimension.  `cams` is the [V, 24] device tensor of camera records (pack_cameras).
     Returns (color [V,3,H,W], allmap [V,8,H,W], radii [V,P], ForwardState with V back-to-back workspaces).
-    ``for_backward=False``: the forward-only forward (srf_views_forward with for_backward = 0), bit-identical outputs
+    ``for_backward=False``: the forward-only forward (srf_scenes_forward with for_backward = 0), bit-identical outputs
     without the blend's contribution record and image state; the returned state cannot feed :func:`backward_views_raw`.
     ``keep_list``: a forward-only state keeps its point list too (the tile lists a subset render filters)."""
     with _DeviceGuard(means3D.device):
         if cams.dtype != torch.float32 or not cams.is_cuda or cams.shape[1] != _lib.CAM_FLOATS or not cams.is_contiguous():
             raise RuntimeError(f"cams must be a contiguous float32 CUDA tensor [V,{_lib.CAM_FLOATS}]")
-        return _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp, cams, tanfovx,
-                        tanfovy, H, W, sh_degree, prefiltered, debug, raw_activations, single=False,
+        return _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp, cams,
+                        [(tanfovx, tanfovy)], H, W, sh_degree, prefiltered, debug, raw_activations, single=False,
                         for_backward=for_backward, keep_list=keep_list)
 
 
@@ -312,18 +312,18 @@ def forward_batch_raw(means3D, shs, colors_precomp, opacities, scales, rotations
     with _DeviceGuard(means3D.device):
         if cams.dtype != torch.float32 or not cams.is_cuda or cams.shape[1] != _lib.CAM_FLOATS or not cams.is_contiguous():
             raise RuntimeError(f"cams must be a contiguous float32 CUDA tensor [S*Vs,{_lib.CAM_FLOATS}]")
-        return _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp, cams, None, None,
+        return _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp, cams, tan_fov,
                         H, W, sh_degree, prefiltered, debug, raw_activations, single=False, for_backward=for_backward,
-                        keep_list=keep_list, tan_fov=tan_fov)
+                        keep_list=keep_list)
 
 
-def _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp, cams, tanfovx, tanfovy,
-             H, W, sh_degree, prefiltered, debug, raw_activations, single, for_backward, keep_list=False, tan_fov=None):
-    """srf_views_forward on the current stream: stage 1 (preprocess + tile scan + async count read-back) and stage 2
+def _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMat_precomp, cams, tan_fov,
+             H, W, sh_degree, prefiltered, debug, raw_activations, single, for_backward, keep_list=False):
+    """srf_scenes_forward on the current stream: stage 1 (preprocess + tile scan + async count read-back) and stage 2
     (binning + blend) with an optimistic capacity, then an event for whoever eventually asks for the instance counts.
+    `tan_fov`: (tan_fovx, tan_fovy) of each of the S scenes, whose Gaussian inputs are [S,P,...] ([P,...] for one).
     `single`: one view, with the outputs in the reference's one-view shapes.  `for_backward` False: the forward-only
-    forward and its smaller workspaces, no image state and, unless `keep_list`, no point list kept.  `tan_fov`: the
-    per-scene fields of view of srf_scenes_forward, whose Gaussian inputs are [S,P,...]."""
+    forward and its smaller workspaces, no image state and, unless `keep_list`, no point list kept."""
     lib = _lib.load()
     device = means3D.device
     V, P = int(cams.shape[0]), int(means3D.shape[-2])
@@ -360,18 +360,13 @@ def _forward(means3D, shs, colors_precomp, opacities, scales, rotations, transMa
     # the tile scan, never for the blend.
     # the forward-only point list and entries are scratch of this call: they go back to the caching allocator when
     # it returns, stream-ordered behind the kernels that use them
-    inputs = (_ptr(means3D), _ptr(shs), _ptr(colors_precomp), _ptr(opacities), _ptr(scales), _ptr(rotations),
-              _ptr(transMat_precomp), cams.data_ptr())
-    tail = (H, W, 1 if prefiltered else 0, capacity,
-            radii.data_ptr(), geom.data_ptr(), tile.data_ptr(), _blob(ent_b, device).data_ptr(), point_list.data_ptr(),
-            _ptr(image), color.data_ptr(), allmap.data_ptr(), slot.data_ptr(), ev.cuda_event,
-            1 if raw_activations else 0, 1 if for_backward else 0)
-    if tan_fov is None:
-        _lib.launch("srf_views_forward", device, V, P, int(sh_degree), M, *inputs, float(tanfovx), float(tanfovy), *tail)
-    else:
-        S = len(tan_fov)
-        _lib.launch("srf_scenes_forward", device, S, V // S, P, int(sh_degree), M, *inputs, _lib.tan_fov_array(tan_fov),
-                    *tail)
+    S = len(tan_fov)
+    _lib.launch("srf_scenes_forward", device, S, V // S, P, int(sh_degree), M, _ptr(means3D), _ptr(shs),
+                _ptr(colors_precomp), _ptr(opacities), _ptr(scales), _ptr(rotations), _ptr(transMat_precomp),
+                cams.data_ptr(), _lib.tan_fov_array(tan_fov), H, W, 1 if prefiltered else 0, capacity,
+                radii.data_ptr(), geom.data_ptr(), tile.data_ptr(), _blob(ent_b, device).data_ptr(), point_list.data_ptr(),
+                _ptr(image), color.data_ptr(), allmap.data_ptr(), slot.data_ptr(), ev.cuda_event,
+                1 if raw_activations else 0, 1 if for_backward else 0)
     state = ForwardState(geom, tile, image, point_list if for_backward or keep_list else None, capacity, nviews=V,
                          cams=cams, for_backward=for_backward)
 
@@ -458,34 +453,9 @@ def backward_views_raw(state: ForwardState, radii, means3D, shs, colors_precomp,
     """Backward of forward_views_raw: grad_color [V,3,H,W], grad_allmap [V,8,H,W]; the per-Gaussian backward
     sums the V views in registers and writes (accumulate: adds into) every parameter-gradient row once.
     ``deterministic`` as in :func:`backward_raw`."""
-    if not state.for_backward:
-        raise RuntimeError("backward of a forward-only render: this state comes from a forward with "
-                           "for_backward=False, which keeps no contribution record or image state; run the "
-                           "forward with for_backward=True to take its gradient")
-    lib = _lib.load()
-    device = means3D.device
-    V, P = int(cams.shape[0]), int(means3D.shape[0])
-    M = int(shs.shape[1]) if shs is not None else 0
-    g = _grad_outputs(P, M, device, shs, colors_precomp, transMat_precomp, out or {}, accumulate, need_means2D)
-    if P == 0:
-        return g
-    state.resolve()                 # capacity verified (re-run if it overflowed) before the lists are walked again
-    det = _lib.deterministic(deterministic)
-    scratch_b = (_lib.det_backward_scratch_bytes(lib, V, P) if det
-                 else _views_sizes(lib, V, P, H, W, state.capacity)[5])
-    _lib.launch(
-        "srf_views_backward", device, V, P, int(sh_degree), M, H, W, state.capacity, cams.data_ptr(),
-        _ptr(means3D), _ptr(shs), 1 if colors_precomp is not None else 0,
-        _ptr(scales), _ptr(rotations), 1 if transMat_precomp is not None else 0,
-        float(tanfovx), float(tanfovy), radii.data_ptr(),
-        state.geom.data_ptr(), state.tile.data_ptr(), state.point_list.data_ptr(), state.image.data_ptr(),
-        grad_color.data_ptr(), grad_allmap.data_ptr(), _blob(scratch_b, device).data_ptr(), 1 if accumulate else 0,
-        _ptr(g["means3D"]), _ptr(g["means2D"]), _ptr(g["sh"]), _ptr(g["colors_precomp"]),
-        _ptr(g["opacities"]), _ptr(g["scales"]), _ptr(g["rotations"]), _ptr(g["cov3Ds_precomp"]),
-        1 if raw_activations else 0, 1 if det else 0)
-    if debug:
-        torch.cuda.synchronize(device)
-    return g
+    return _backward(state, radii, means3D, shs, colors_precomp, scales, rotations, transMat_precomp, cams,
+                     [(tanfovx, tanfovy)], H, W, sh_degree, grad_color, grad_allmap, None, None, out, accumulate,
+                     need_means2D, raw_activations, debug, deterministic)
 
 
 def backward_batch_raw(state: ForwardState, radii, means3D, shs, scales, rotations, cams: torch.Tensor, tan_fov: Sequence,
@@ -496,6 +466,18 @@ def backward_batch_raw(state: ForwardState, radii, means3D, shs, scales, rotatio
     scene's rows the sum of its own views.  With ``offsets`` (device int64 [S+1]) the state is a subset forward's, of
     ``P`` Gaussians per view, and the inputs and gradients are the scenes' rows concatenated, [n,...].
     ``deterministic`` as in :func:`backward_raw`."""
+    lead = tuple(means3D.shape[:-1])
+    g = _backward(state, radii, means3D, shs, None, scales, rotations, None, cams, tan_fov, H, W, sh_degree, grad_color,
+                  grad_allmap, offsets, P, None, False, False, raw_activations, debug, deterministic)
+    return {k: (t.view(lead + tuple(t.shape[1:])) if t is not None else None) for k, t in g.items()}
+
+
+def _backward(state: ForwardState, radii, means3D, shs, colors_precomp, scales, rotations, transMat_precomp, cams,
+              tan_fov, H, W, sh_degree, grad_color, grad_allmap, offsets, P, out, accumulate, need_means2D,
+              raw_activations, debug, deterministic):
+    """srf_scenes_backward on the current stream for the S = len(tan_fov) scenes of ``state``: ``P`` Gaussians per view
+    (None: ``means3D.shape[-2]``), ``offsets`` as in :func:`backward_batch_raw`.  Returns the gradient rows of the
+    ``means3D.numel() // 3`` input rows, flat ([rows, ...]); ``out`` / ``accumulate`` as in :func:`backward_raw`."""
     if not state.for_backward:
         raise RuntimeError("backward of a forward-only render: this state comes from a forward with "
                            "for_backward=False, which keeps no contribution record or image state; run the "
@@ -503,13 +485,11 @@ def backward_batch_raw(state: ForwardState, radii, means3D, shs, scales, rotatio
     lib = _lib.load()
     device = means3D.device
     S, V = len(tan_fov), int(cams.shape[0])
-    lead = tuple(means3D.shape[:-1])
     rows = means3D.numel() // 3
     if P is None:
         P = int(means3D.shape[-2])
     M = int(shs.shape[-2]) if shs is not None else 0
-    g = _grad_outputs(rows, M, device, shs, None, None, {}, False, False)
-    g = {k: (t.view(lead + tuple(t.shape[1:])) if t is not None else None) for k, t in g.items()}
+    g = _grad_outputs(rows, M, device, shs, colors_precomp, transMat_precomp, out or {}, accumulate, need_means2D)
     if P == 0 or rows == 0:
         return g
     state.resolve()                 # capacity verified (re-run if it overflowed) before the lists are walked again
@@ -518,11 +498,13 @@ def backward_batch_raw(state: ForwardState, radii, means3D, shs, scales, rotatio
                  else _views_sizes(lib, V, P, H, W, state.capacity)[5])
     _lib.launch(
         "srf_scenes_backward", device, S, V // S, P, _ptr(offsets), int(sh_degree), M, H, W, state.capacity,
-        cams.data_ptr(), _ptr(means3D), _ptr(shs), 0, _ptr(scales), _ptr(rotations), 0, _lib.tan_fov_array(tan_fov),
+        cams.data_ptr(), _ptr(means3D), _ptr(shs), 1 if colors_precomp is not None else 0,
+        _ptr(scales), _ptr(rotations), 1 if transMat_precomp is not None else 0, _lib.tan_fov_array(tan_fov),
         radii.data_ptr(), state.geom.data_ptr(), state.tile.data_ptr(), state.point_list.data_ptr(),
-        state.image.data_ptr(), grad_color.data_ptr(), grad_allmap.data_ptr(), _blob(scratch_b, device).data_ptr(), 0,
-        _ptr(g["means3D"]), None, _ptr(g["sh"]), None, _ptr(g["opacities"]), _ptr(g["scales"]), _ptr(g["rotations"]),
-        None, 1 if raw_activations else 0, 1 if det else 0)
+        state.image.data_ptr(), grad_color.data_ptr(), grad_allmap.data_ptr(), _blob(scratch_b, device).data_ptr(),
+        1 if accumulate else 0, _ptr(g["means3D"]), _ptr(g["means2D"]), _ptr(g["sh"]), _ptr(g["colors_precomp"]),
+        _ptr(g["opacities"]), _ptr(g["scales"]), _ptr(g["rotations"]), _ptr(g["cov3Ds_precomp"]),
+        1 if raw_activations else 0, 1 if det else 0)
     if debug:
         torch.cuda.synchronize(device)
     return g

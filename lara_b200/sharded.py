@@ -3,7 +3,7 @@
 Every target view of a scene is an independent forward+backward over the same read-only
 Gaussian set; only the parameter gradients sum across views.  One process per GPU
 (``torch.distributed``, NCCL over NVLink): rank r renders views ``r, r+G, r+2G, ...`` in ONE
-launch set (``srf_views_*``), the per-Gaussian backward sums the rank's views in registers and adds
+launch set (``srf_scenes_*`` with one scene), the per-Gaussian backward sums the rank's views in registers and adds
 the result into one flat fp32 buffer (segment-major: means3D | sh | opacity | scales | rotations),
 and a single ``all_reduce(sum)`` of that buffer finishes the step.  Images / aux maps stay on the rank
 that owns the view.  The reference has nothing like this (it is single-GPU; LaRa only

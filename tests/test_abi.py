@@ -18,9 +18,9 @@ def declared_symbols():
     return sorted(names)
 
 
-def test_header_declares_the_views_boundary():
+def test_header_declares_the_scenes_boundary():
     syms = declared_symbols()
-    for must in ("srf_views_forward", "srf_views_forward_render", "srf_views_backward", "srf_mark_visible",
+    for must in ("srf_scenes_forward", "srf_views_forward_render", "srf_scenes_backward", "srf_mark_visible",
                  "srf_views_workspace_bytes", "srf_last_error"):
         assert must in syms
 
@@ -55,16 +55,18 @@ def test_views_workspace_sizes_host_only(lib):
     assert g0 > 0 and s0 > 0
 
 
-def test_views_entries_and_size_query_reject_bad_arguments(lib):
+def test_scenes_entries_and_size_query_reject_bad_arguments(lib):
+    from lara_b200 import _lib
     n = (ctypes.c_size_t * 6)()
     assert lib.srf_views_workspace_bytes(1, -1, 16, 16, 0, 1, n) != 0
     assert b"srf_views_workspace_bytes" in lib.srf_last_error()
     assert lib.srf_views_workspace_bytes(1, 0, 0, 16, 0, 1, n) != 0
     # null / misaligned workspaces are rejected before any CUDA call
     cams = (ctypes.c_float * 24)()
-    args = [None, 1, 4, 0, 1, None, None, None, None, None, None, None, ctypes.addressof(cams),
-            1.0, 1.0, 16, 16, 0, 0, None, None, None, None, None, None, None, None, None, None, 0, 1]
-    assert lib.srf_views_forward(*args) != 0
+    args = [None, 1, 1, 4, 0, 1, None, None, None, None, None, None, None, ctypes.addressof(cams),
+            _lib.tan_fov_array([(1.0, 1.0)]), 16, 16, 0, 0, None, None, None, None, None, None, None, None, None, None,
+            0, 1]
+    assert lib.srf_scenes_forward(*args) != 0
     assert lib.srf_last_error() != b""
 
 

@@ -44,6 +44,8 @@ def test_scenes_subset_forward_rejects_bad_sizes(lib):
     assert call(2, 0, 4, 0, 0, None) != 0
     assert call(2, 1, 4, 0, 5, None) != 0 and b"bad sizes" in lib.srf_last_error()
     assert call(2, 1, 4, 0, 2, None) != 0 and b"null offsets" in lib.srf_last_error()
+    assert call(2, 1, 4, 0, 0, None) != 0 and b"null offsets" in lib.srf_last_error()         # NULL offsets with S > 1
+    assert call(1, 1, 4, 2, 3, None) != 0 and b"n_max == n" in lib.srf_last_error()        # NULL offsets, n_max != n
 
 
 def _settings(n, H=16, W=16, fov=1.0, deg=1):

@@ -177,12 +177,13 @@ def test_scratch_queries(lib):
     assert lib.srf_loss_deterministic_workspace_bytes(1, 4, -1, ctypes.byref(n)) != 0
 
 
-def test_bad_arguments_and_misaligned_workspaces_rejected_before_any_launch(lib):
+def test_scenes_backward_and_fused_ops_reject_bad_arguments_before_any_launch(lib):
     # null cameras / null input / misaligned workspace: status and message, no CUDA call
-    args = [None, 1, 10, 0, 1, 16, 16, 0, None, None, None, 0, None, None, 0, 1.0, 1.0, None, None, None, None, None,
-            None, None, None, 0, None, None, None, None, None, None, None, None, 0, 1]
-    assert lib.srf_views_backward(*args) != 0
-    assert b"srf_views_backward" in lib.srf_last_error()
+    from lara_b200 import _lib
+    args = [None, 1, 1, 10, None, 0, 1, 16, 16, 0, None, None, None, 0, None, None, 0, _lib.tan_fov_array([(1.0, 1.0)]),
+            None, None, None, None, None, None, None, None, 0, None, None, None, None, None, None, None, None, 0, 1]
+    assert lib.srf_scenes_backward(*args) != 0
+    assert b"srf_scenes_backward" in lib.srf_last_error()
     assert lib.srf_loss_forward(None, 1, 8, 8, 0, None, 1, None, None, None, None, 1, None) != 0
     assert b"null pointer" in lib.srf_last_error()
     assert lib.srf_loss_forward(None, 1, 8, 8, 0, 1, 1, None, None, None, None, 1, 1) != 0

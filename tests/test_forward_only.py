@@ -1,5 +1,5 @@
-"""Forward-only rendering, host side (no GPU needed): the for_backward flag of srf_views_forward, its stage-2 re-run and
-the workspace query, their argument checks, and the rule by which the public wrappers pick the forward-only path --
+"""Forward-only rendering, host side (no GPU needed): the for_backward flag of srf_scenes_forward, its stage-2 re-run
+and the workspace query, their argument checks, and the rule by which the public wrappers pick the forward-only path --
 taken iff no gradient can flow (grad mode off, or no tensor input requires grad) -- driven with stand-ins for the raw
 forward functions."""
 import ctypes
@@ -15,22 +15,24 @@ from lara_b200 import rasterizer as R
 
 from test_abi import ROOT, declared_symbols
 
-# the forward-only twins of ABI 11, folded into the flag
-REMOVED = ("srf_views_forward_inference", "srf_views_forward_inference_render", "srf_views_inference_workspace_bytes")
+# the forward-only twins of ABI 11, folded into the flag, and the one-scene entries of ABI 12, now S = 1 of the scene
+# entries
+REMOVED = ("srf_views_forward_inference", "srf_views_forward_inference_render", "srf_views_inference_workspace_bytes",
+           "srf_views_forward", "srf_views_subset_forward", "srf_views_backward")
 
 
 def align256(x):
     return (x + 255) // 256 * 256
 
 
-def test_forward_only_is_a_flag_of_the_forward_entries(lib):
+def test_forward_only_is_a_flag_of_the_scene_forward_entries(lib):
     syms = declared_symbols()
     for name in REMOVED:
         assert name not in syms and name not in _lib.SIGNATURES and not hasattr(lib, name), name
-    assert lib.srf_abi_version() == _lib.ABI_VERSION == 12
+    assert lib.srf_abi_version() == _lib.ABI_VERSION == 13
     header = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "surfel_rasterizer.h")).read(), flags=re.S)
     header = re.sub(r"\s+", " ", header)
-    for name in ("srf_views_forward", "srf_views_forward_render"):
+    for name in ("srf_scenes_forward", "srf_views_forward_render"):
         assert re.search(rf"\b{name}\([^;]*, int for_backward\);", header), name
         assert _lib.SIGNATURES[name][1][-1] is ctypes.c_int, name
     assert "srf_views_workspace_bytes(int V, int P, int H, int W, size_t capacity, int for_backward, size_t bytes[6]);" \
@@ -61,26 +63,28 @@ def test_workspace_query_rejects_bad_arguments_with_either_flag(lib):
 
 def _forward_args(V=1, P=4, D=0, H=16, W=16, capacity=0, geom=None, tile=None, entries=None, plist=None, image=None,
                   out=None, for_backward=0):
+    """srf_scenes_forward's arguments for one scene (S = 1) of V views."""
     cams = (ctypes.c_float * 24)()
-    args = [None, V, P, D, 1, None, None, None, None, None, None, None, ctypes.addressof(cams),
-            1.0, 1.0, H, W, 0, capacity, None, geom, tile, entries, plist, image, out, out, None, None, 0, for_backward]
+    args = [None, 1, V, P, D, 1, None, None, None, None, None, None, None, ctypes.addressof(cams),
+            _lib.tan_fov_array([(1.0, 1.0)]), H, W, 0, capacity, None, geom, tile, entries, plist, image, out, out,
+            None, None, 0, for_backward]
     return args, cams
 
 
 @pytest.mark.parametrize("case", [dict(V=0), dict(H=16 * 65535 + 1), dict(), dict(tile=0x1010),
                                   dict(tile=0x1000, D=4)])
-def test_forward_only_rejects_what_the_training_forward_rejects(lib, case):
+def test_scenes_forward_only_rejects_what_the_training_forward_rejects(lib, case):
     """Same arguments, the same message byte for byte with either flag; every case fails before anything is
     enqueued."""
     msgs = []
     for for_backward in (0, 1):
         args, _cams = _forward_args(**case, for_backward=for_backward)
-        assert lib.srf_views_forward(*args) != 0
+        assert lib.srf_scenes_forward(*args) != 0
         msgs.append(lib.srf_last_error())
-    assert msgs[0].startswith(b"srf_views_forward: ") and msgs[0] == msgs[1]
+    assert msgs[0].startswith(b"srf_scenes_forward: ") and msgs[0] == msgs[1]
 
 
-def test_forward_rejects_null_or_misaligned_workspaces_before_any_cuda_call(lib):
+def test_scenes_forward_rejects_null_or_misaligned_workspaces_before_any_cuda_call(lib):
     """Without a device any CUDA call would fail with a CUDA error; these fail with the argument check's message, with
     either flag: the checks of both stages come before stage 1 enqueues anything."""
     x = 0x10000          # a 256-byte aligned address that is never dereferenced: every call below fails its checks
@@ -95,11 +99,11 @@ def test_forward_rejects_null_or_misaligned_workspaces_before_any_cuda_call(lib)
         image = x if for_backward else None
         for kw, msg in cases:
             args, _cams = _forward_args(**kw, image=image, for_backward=for_backward)
-            assert lib.srf_views_forward(*args) != 0
-            assert lib.srf_last_error().decode() == f"srf_views_forward: {msg}", (kw, for_backward)
+            assert lib.srf_scenes_forward(*args) != 0
+            assert lib.srf_last_error().decode() == f"srf_scenes_forward: {msg}", (kw, for_backward)
     args, _cams = _forward_args(P=0, tile=x, capacity=64, entries=x, plist=x, out=x, image=None, for_backward=1)
-    assert lib.srf_views_forward(*args) != 0
-    assert lib.srf_last_error() == b"srf_views_forward: null required pointer"
+    assert lib.srf_scenes_forward(*args) != 0
+    assert lib.srf_last_error() == b"srf_scenes_forward: null required pointer"
 
     # stage 2 alone: a misaligned geom_state or point_list is rejected; image_state may be NULL when forward-only
     cams = (ctypes.c_float * 24)()
@@ -144,20 +148,20 @@ def _fake_outputs(V, for_backward, single):
 
 @pytest.fixture
 def stand_ins(monkeypatch):
-    """forward_raw / forward_views_raw record which path was asked for; the CUDA-only input checks pass CPU tensors."""
+    """forward_raw / forward_batch_raw record which path was asked for; the CUDA-only input checks pass CPU tensors."""
     calls = []
 
     def forward_raw(*a, raw_activations=False, for_backward=True):
         calls.append(("forward_raw", for_backward, raw_activations))
         return _fake_outputs(1, for_backward, True)
 
-    def forward_views_raw(*a, raw_activations=False, for_backward=True, **kw):
+    def forward_batch_raw(*a, raw_activations=False, for_backward=True, **kw):
         V = int(a[7].shape[0])
-        calls.append(("forward_views_raw", for_backward, raw_activations))
+        calls.append(("forward_batch_raw", for_backward, raw_activations))
         return _fake_outputs(V, for_backward, False)
 
     monkeypatch.setattr(R, "forward_raw", forward_raw)
-    monkeypatch.setattr(R, "forward_views_raw", forward_views_raw)
+    monkeypatch.setattr(R, "forward_batch_raw", forward_batch_raw)
     monkeypatch.setattr(R, "_f32c", lambda t, name: t.contiguous())
     monkeypatch.setattr(R, "_check_settings", lambda rs, device: rs)
     return calls
@@ -216,20 +220,20 @@ def test_dropin_selection_rule(stand_ins, entry, mode, requires, training):
 
 
 @pytest.mark.parametrize("mode,requires,training", [m for m in MATRIX if "means2D" not in m[1] or len(m[1]) > 1])
-def test_scene_views_selection_rule(stand_ins, mode, requires, training):
+def test_scene_views_selection_rule_on_the_scene_body(stand_ins, mode, requires, training):
     t = _inputs(requires)
     V = 3
     sets = [_settings() for _ in range(V)]
     with _mode(mode):
         out = MV.render_scene_views(t["means3D"], t["shs"], t["opacities"], t["scales"], t["rotations"], sets,
                                     raw_activations=True)
-    assert stand_ins == [("forward_views_raw", training, True)]
+    assert stand_ins == [("forward_batch_raw", training, True)]
     ref_c, _, ref_r, _ = _fake_outputs(V, True, False)
     assert torch.equal(out["image"].detach(), ref_c.clamp(0, 1)) and torch.equal(out["radii"], ref_r)
     assert out["image"].requires_grad == training
 
 
-def test_scene_views_rays_requiring_grad_keep_the_training_path(stand_ins, monkeypatch):
+def test_scene_views_rays_requiring_grad_keep_the_training_path_on_the_scene_body(stand_ins, monkeypatch):
     """rays get no gradient, but a call whose only grad-requiring input is rays built an autograd node before; it
     still does."""
     monkeypatch.setattr(MV, "epilogue_views_forward_raw", lambda *a: None)
@@ -237,7 +241,7 @@ def test_scene_views_rays_requiring_grad_keep_the_training_path(stand_ins, monke
     rays = torch.zeros((1, H, W, 6), requires_grad=True)
     out = MV.render_scene_views(t["means3D"], t["shs"], t["opacities"], t["scales"], t["rotations"], [_settings()],
                                 rays=rays)
-    assert stand_ins == [("forward_views_raw", True, False)]
+    assert stand_ins == [("forward_batch_raw", True, False)]
     assert out["image"].requires_grad
 
 

@@ -1,5 +1,5 @@
-"""The subset render's argument checks (``srf_views_subset_forward``, ``render_subset_views``), no GPU needed: the C entry
-rejects every bad argument before it makes a CUDA call, and the Python entry before it launches anything."""
+"""The subset render's argument checks (``srf_scenes_subset_forward``, ``render_subset_views``), no GPU needed: the C
+entry rejects every bad argument before it makes a CUDA call, and the Python entry before it launches anything."""
 import ctypes
 
 import pytest
@@ -10,20 +10,22 @@ MIS = A + 16
 
 
 def _args(**kw):
-    """srf_views_subset_forward's arguments for V = 2 views of a P = 1000 coarse forward, n = 10, 64 x 48, each
-    overridable by name."""
-    a = dict(stream=None, V=2, P=1000, n=10, D=1, M=4, idx=A, means3D=A, shs=A, colors_precomp=None, cams=A, H=64, W=48,
-             capacity=4096, coarse_radii=A, coarse_geom=A, coarse_tile=A, coarse_point_list=A, coarse_capacity=4096,
-             coarse_for_backward=1, radii=A, geom=A, tile=A, point_list=A, image=A, out_color=A, out_others=A,
-             workspace=A, for_backward=1)
+    """srf_scenes_subset_forward's arguments for one scene (S = 1, offsets = NULL) of V = 2 views of a P = 1000 coarse
+    forward, n = n_max = 10, 64 x 48, each overridable by name."""
+    a = dict(stream=None, S=1, V=2, P=1000, n=10, n_max=None, D=1, M=4, idx=A, offsets=None, means3D=A, shs=A,
+             colors_precomp=None, cams=A, H=64, W=48, capacity=4096, coarse_radii=A, coarse_geom=A, coarse_tile=A,
+             coarse_point_list=A, coarse_capacity=4096, coarse_for_backward=1, radii=A, geom=A, tile=A, point_list=A,
+             image=A, out_color=A, out_others=A, workspace=A, for_backward=1)
     a.update(kw)
+    if a["n_max"] is None:
+        a["n_max"] = a["n"]
     return list(a.values())
 
 
 @pytest.mark.parametrize("bad,msg", [
-    (dict(n=1001), b"n = 1001 > P"),
+    (dict(n=1001), b"n_max = 1001 > P"),
     (dict(n=-1), b"bad sizes"),
-    (dict(V=0), b"bad sizes"),
+    (dict(V=0), b"Vs > 0"),
     (dict(H=0), b"bad sizes"),
     (dict(D=4), b"sh degree"),
     (dict(M=3), b"SH coefficients"),
@@ -44,15 +46,15 @@ def _args(**kw):
     (dict(coarse_point_list=MIS), b"256-byte aligned"),
     (dict(image=MIS), b"256-byte aligned"),
 ])
-def test_c_entry_rejects_bad_arguments(lib, bad, msg):
-    assert lib.srf_views_subset_forward(*_args(**bad)) != 0
+def test_scenes_c_entry_rejects_bad_arguments(lib, bad, msg):
+    assert lib.srf_scenes_subset_forward(*_args(**bad)) != 0
     err = lib.srf_last_error()
-    assert b"srf_views_subset_forward" in err and msg in err, err
+    assert b"srf_scenes_subset_forward" in err and msg in err, err
 
 
-def test_c_entry_forward_only_needs_no_image_state(lib):
+def test_scenes_c_entry_forward_only_needs_no_image_state(lib):
     # for_backward = 0 takes no image state: the checks then fail only on what is really wrong
-    assert lib.srf_views_subset_forward(*_args(image=None, for_backward=0, D=5)) != 0
+    assert lib.srf_scenes_subset_forward(*_args(image=None, for_backward=0, D=5)) != 0
     assert b"sh degree" in lib.srf_last_error()
 
 

@@ -1,4 +1,4 @@
-"""What the forward-only path saves (DESIGN §3.14): the training forward (srf_views_forward with for_backward = 1, with
+"""What the forward-only path saves (DESIGN §3.14): the training forward (srf_scenes_forward with for_backward = 1, with
 the contribution record and the image state the backward reads) against the forward-only one (for_backward = 0) on the
 same inputs, alternated in one process.
 
