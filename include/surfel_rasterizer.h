@@ -321,6 +321,21 @@ int srf_ms_ssim_backward(srf_stream_t stream, int B, int C, int H, int W,
                          float data_range, int size_average, void* workspace, const float* upstream,
                          float* dx, const srf_ms_ssim_addr* dx_addr);
 
+/* ---- fused single-scale SSIM (pytorch-msssim 1.0.0 ssim; evaluation.py:93 and the D-SSIM loss term) -----------------
+ * Level 0 of the MS-SSIM above on its own: the same window, C1, C2, image addressing, workspace rules and determinism.
+ * ssim_per_channel[b,c] = mean of the valid ssim_map, relu'd when nonnegative_ssim != 0; out[0] is its mean over (b, c)
+ * (size_average != 0), else out[b] is its mean over c.  H and W must be at least 11 (the library instead skips the
+ * filter along a shorter side with a warning).  The backward needs the forward's workspace and the same arguments;
+ * through a plane whose relu'd value is 0 its gradient is exactly 0.                                                    */
+int srf_ssim_workspace_bytes(int B, int C, int H, int W, size_t* bytes);
+int srf_ssim_forward(srf_stream_t stream, int B, int C, int H, int W,
+                     const float* x, const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
+                     float data_range, int size_average, int nonnegative_ssim, void* workspace, float* out);
+int srf_ssim_backward(srf_stream_t stream, int B, int C, int H, int W,
+                      const float* x, const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
+                      float data_range, int size_average, int nonnegative_ssim, void* workspace,
+                      const float* upstream, float* dx, const srf_ms_ssim_addr* dx_addr);
+
 /* ---- optional per-kernel timing (no reference counterpart; used by bench.py's roofline) --
  * Between srf_profile_begin() and srf_profile_end() every kernel launch made by this
  * library is bracketed by CUDA events on its launching stream.  srf_profile_end waits for

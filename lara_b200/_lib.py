@@ -94,6 +94,10 @@ SIGNATURES = {
                                              POINTER(c_int)]),
     "srf_ms_ssim_forward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _A, _P, _A, c_float, c_int, _P, _P]),
     "srf_ms_ssim_backward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _A, _P, _A, c_float, c_int, _P, _P, _P, _A]),
+    "srf_ssim_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, POINTER(c_size_t)]),
+    "srf_ssim_forward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _A, _P, _A, c_float, c_int, c_int, _P, _P]),
+    "srf_ssim_backward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _A, _P, _A, c_float, c_int, c_int, _P, _P, _P,
+                                  _A]),
     "srf_mark_visible": (c_int, [_P, c_int, _P, _P, _P, _P]),
     # include/surfel_mesh.h
     "srf_tsdf_integrate": (c_int, [_P, _I3, _I3, c_float, c_float, _P, _P, _P, c_int, c_int, c_int, _P, _P, _P, _P,
@@ -151,6 +155,15 @@ SIGNATURES = {
     "srf_add_layernorm_backward": (c_int, [_P, c_int, c_int, c_float,
                                            _P, _P, _P, _P, _P,                       # y, gamma, dL_dn, dL_dy, workspace
                                            _P, _P, _P]),                             # dL_da, d_gamma, d_beta
+    # include/surfel_eval.h
+    "srf_eval_workspace_bytes": (c_int, [POINTER(c_size_t)]),
+    "srf_eval_metrics": (c_int, [_P, c_int, c_int, c_int, c_int, c_int,   # stream, V, H, W, v0, v1
+                                 _P, _A, _P, _A,                          # image, target
+                                 _P, _A, _P, _A, _P, _A,                  # depth, depth_gt, mask
+                                 c_int, POINTER(c_double), _P, _P]),      # n_thresholds, thresholds, workspace, out
+    "srf_video_frames": (c_int, [_P, c_int, c_int, c_int,                 # stream, N, H, W
+                                 _P, _A, _P, _A, _P, _A,                  # image, normal, alpha
+                                 _P, _P]),                                # rgb, nrm
     "srf_profile_begin": (c_int, []),
     "srf_profile_end": (c_int, [POINTER(c_float), POINTER(c_int), c_int]),
 }
@@ -268,6 +281,14 @@ def subset_workspace_bytes(lib, P: int) -> int:
 
 def ms_ssim_workspace_bytes(lib, B: int, C: int, H: int, W: int) -> int:
     return _size_query(lib.srf_ms_ssim_workspace_bytes, B, C, H, W)
+
+
+def ssim_workspace_bytes(lib, B: int, C: int, H: int, W: int) -> int:
+    return _size_query(lib.srf_ssim_workspace_bytes, B, C, H, W)
+
+
+def eval_workspace_bytes(lib) -> int:
+    return _size_query(lib.srf_eval_workspace_bytes)
 
 
 def det_point_feats_workspace_bytes(lib, V: int, H: int, W: int) -> int:

@@ -17,7 +17,8 @@
 //                        and adds the pooling backward: dX_l = G^T A + 2 X G^T B + Y G^T C + dX_{l+1}(parent) / 4.
 // No atomics anywhere: two identical calls give identical bits.  The level-0 image is read (and its gradient
 // written) through MsAddr, so a channel-last tensor and V planar views side by side are read in place.
-// The C entries srf_ms_ssim_* (include/surfel_rasterizer.h) are defined here.
+// The C entries srf_ms_ssim_* (include/surfel_rasterizer.h) are defined here, and so are srf_ssim_*: single-scale
+// SSIM, the kLast level alone on the caller's image, with ssim_finalize_kernel in place of the pyramid's finalize.
 #include <math.h>
 #include <string.h>
 
@@ -253,6 +254,44 @@ __global__ void __launch_bounds__(kThreads) ms_ssim_finalize_kernel(const FinalA
     }
 }
 
+// Single-scale SSIM (srf_ssim_*): the per-plane mean of the level-0 ssim_map from ms_ssim_fwd_kernel<true>'s partials,
+// summed in the same fixed order, optionally relu'd; coef = dvalue/dmean * scale / count for ms_ssim_bwd_kernel<true>.
+struct SsimFinalArgs {
+    int B, C, planes, ntiles, size_average, nonnegative;
+    double count;                // valid output pixels per plane, (H - 10)(W - 10)
+    const double* part;          // [planes][ntiles]
+    double* val;                 // [planes]
+    float* coef;                 // [planes]
+    float* out;                  // [1] or [B]
+};
+
+__global__ void __launch_bounds__(kThreads) ssim_finalize_kernel(const SsimFinalArgs f) {
+    const int lane = threadIdx.x & 31, P = f.planes;
+    const double scale = 1.0 / (f.size_average ? (double)P : (double)f.C);
+    for (int p = threadIdx.x >> 5; p < P; p += kThreads / 32) {
+        const double* src = f.part + (size_t)p * f.ntiles;
+        double s = 0.0;
+        for (int i = lane; i < f.ntiles; i += 32) s += src[i];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+        if (lane == 0) {
+            const double m = s / f.count;
+            // relu's backward is a select: no gradient through a plane whose mean is <= 0
+            const bool pass = !f.nonnegative || m > 0.0;
+            f.val[p] = pass ? m : 0.0;
+            f.coef[p] = pass ? (float)(scale / f.count) : 0.f;
+        }
+    }
+    __syncthreads();
+    const int nout = f.size_average ? 1 : f.B;
+    for (int o = threadIdx.x; o < nout; o += kThreads) {
+        const int p0 = f.size_average ? 0 : o * f.C, np = f.size_average ? P : f.C;
+        double s = 0.0;
+        for (int p = 0; p < np; ++p) s += f.val[p0 + p];
+        f.out[o] = (float)(s / np);
+    }
+}
+
 template <bool kLast>
 __global__ void __launch_bounds__(kThreads) ms_ssim_bwd_kernel(const LevelArgs a) {
     constexpr int IW = kTW + 2 * kR, IH = kTH + 2 * kR;   // inputs under the windows of the outputs below
@@ -383,11 +422,8 @@ MsAddr planar(int C, int H, int W) {
 }
 
 // level l's inputs and the window / constants shared by both directions
-LevelArgs level_args(const MsSsimArgs& m, const Layout& L, char* ws, int l) {
-    LevelArgs a;
-    memset(&a, 0, sizeof(a));
-    a.C = m.C; a.H = L.h[l]; a.W = L.w[l]; a.px = L.px[l]; a.py = L.py[l];
-    const double c1 = 0.01 * m.data_range, c2 = 0.03 * m.data_range;
+void level_constants(LevelArgs& a, float data_range) {
+    const double c1 = 0.01 * data_range, c2 = 0.03 * data_range;
     a.c1 = (float)(c1 * c1); a.c2 = (float)(c2 * c2);
     // the library's fp32 window: g = exp(-(i - 5)^2 / (2 * 1.5^2)) in fp32, g / sum(g); the sum is rounded once
     float e[kR + 1];
@@ -398,6 +434,13 @@ LevelArgs level_args(const MsSsimArgs& m, const Layout& L, char* ws, int l) {
         sum += e[i];
     }
     for (int i = 0; i <= kR; ++i) a.win[i] = e[i] / (float)sum;
+}
+
+LevelArgs level_args(const MsSsimArgs& m, const Layout& L, char* ws, int l) {
+    LevelArgs a;
+    memset(&a, 0, sizeof(a));
+    a.C = m.C; a.H = L.h[l]; a.W = L.w[l]; a.px = L.px[l]; a.py = L.py[l];
+    level_constants(a, m.data_range);
     float* pyr = reinterpret_cast<float*>(ws + L.o_pyr);
     if (l == 0) {
         a.x = m.x; a.y = m.y; a.ax = m.ax; a.ay = m.ay;
@@ -411,6 +454,31 @@ LevelArgs level_args(const MsSsimArgs& m, const Layout& L, char* ws, int l) {
         a.nx = pyr + L.pyr[l + 1];
         a.ny = a.nx + (size_t)m.B * m.C * a.nh * a.nw;
     }
+    return a;
+}
+
+// single-scale SSIM: one level, no pyramid; the forward's tile grid, then per-CTA partials, values and coefficients
+struct SsimLayout { int ntx, nty; size_t o_part, o_val, o_coef, total; };
+
+SsimLayout make_ssim_layout(int B, int C, int H, int W) {
+    SsimLayout L;
+    const size_t planes = (size_t)B * C;
+    L.ntx = (W + kTW - 1) / kTW;
+    L.nty = (H + kTH - 1) / kTH;
+    size_t o = 0;
+    L.o_part = o; o = align_up(o + planes * L.ntx * L.nty * sizeof(double));
+    L.o_val = o;  o = align_up(o + planes * sizeof(double));
+    L.o_coef = o; o = align_up(o + planes * sizeof(float));
+    L.total = o;
+    return L;
+}
+
+LevelArgs ssim_level_args(const MsSsimArgs& m) {
+    LevelArgs a;
+    memset(&a, 0, sizeof(a));
+    a.C = m.C; a.H = m.H; a.W = m.W;
+    level_constants(a, m.data_range);
+    a.x = m.x; a.y = m.y; a.ax = m.ax; a.ay = m.ay;
     return a;
 }
 
@@ -543,4 +611,88 @@ extern "C" int srf_ms_ssim_backward(srf_stream_t stream_, int B, int C, int H, i
     }
     const cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? 0 : cuda_error("ms_ssim_bwd launch", e);
+}
+
+// ---- single-scale SSIM (pytorch-msssim 1.0.0 ssim): level 0 of the MS-SSIM kernels, kLast form ----
+
+static int ssim_sizes(const char* fn, int B, int C, int H, int W) {
+    if (B <= 0 || C <= 0 || H <= 0 || W <= 0) return set_error("%s: bad sizes (B=%d, C=%d, H=%d, W=%d)", fn, B, C, H, W);
+    if (H < 11 || W < 11) return set_error("%s: H and W must be at least the window size 11 (H=%d, W=%d)", fn, H, W);
+    if ((long long)B * C > 65535) return set_error("%s: B*C=%lld planes exceeds 65535", fn, (long long)B * C);
+    return 0;
+}
+
+static int ssim_prepare(const char* fn, int B, int C, int H, int W, const float* x, const srf_ms_ssim_addr* x_addr,
+                        const float* y, const srf_ms_ssim_addr* y_addr, float data_range, int size_average,
+                        void* workspace, srf::MsSsimArgs* a) {
+    memset(a, 0, sizeof(*a));
+    if (ssim_sizes(fn, B, C, H, W)) return 1;
+    if (ms_ssim_addr(fn, "x", x, x_addr, &a->ax) || ms_ssim_addr(fn, "y", y, y_addr, &a->ay)) return 1;
+    if (!(data_range > 0.f) || !(data_range < 3.0e38f)) return set_error("%s: data_range must be positive and finite", fn);
+    if (!workspace || srf::misaligned(workspace)) return set_error("%s: workspace must be 256-byte aligned", fn);
+    a->B = B; a->C = C; a->H = H; a->W = W; a->size_average = size_average ? 1 : 0; a->data_range = data_range;
+    a->x = x; a->y = y; a->workspace = workspace;
+    return 0;
+}
+
+extern "C" int srf_ssim_workspace_bytes(int B, int C, int H, int W, size_t* bytes) {
+    if (ssim_sizes("srf_ssim_workspace_bytes", B, C, H, W)) return 1;
+    if (!bytes) return set_error("srf_ssim_workspace_bytes: null pointer");
+    *bytes = srf::make_ssim_layout(B, C, H, W).total;
+    return 0;
+}
+
+extern "C" int srf_ssim_forward(srf_stream_t stream_, int B, int C, int H, int W, const float* x,
+                                const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
+                                float data_range, int size_average, int nonnegative_ssim, void* workspace, float* out) {
+    using namespace srf;
+    const char* fn = "srf_ssim_forward";
+    MsSsimArgs m;
+    if (ssim_prepare(fn, B, C, H, W, x, x_addr, y, y_addr, data_range, size_average, workspace, &m)) return 1;
+    if (!out) return set_error("%s: null output pointer", fn);
+    const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    const SsimLayout L = make_ssim_layout(B, C, H, W);
+    char* ws = static_cast<char*>(workspace);
+    const int planes = B * C;
+    LevelArgs a = ssim_level_args(m);
+    a.ntx = L.ntx;
+    a.part = reinterpret_cast<double*>(ws + L.o_part);
+    ms_ssim_fwd_kernel<true><<<dim3((unsigned)(L.ntx * L.nty), (unsigned)planes), kThreads, 0, stream>>>(a);
+    SsimFinalArgs f;
+    memset(&f, 0, sizeof(f));
+    f.B = B; f.C = C; f.planes = planes; f.ntiles = L.ntx * L.nty;
+    f.size_average = m.size_average; f.nonnegative = nonnegative_ssim ? 1 : 0;
+    f.count = (double)(H - kR) * (double)(W - kR);
+    f.part = reinterpret_cast<const double*>(ws + L.o_part);
+    f.val = reinterpret_cast<double*>(ws + L.o_val);
+    f.coef = reinterpret_cast<float*>(ws + L.o_coef);
+    f.out = out;
+    ssim_finalize_kernel<<<1, kThreads, 0, stream>>>(f);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : cuda_error("ssim_fwd launch", e);
+}
+
+extern "C" int srf_ssim_backward(srf_stream_t stream_, int B, int C, int H, int W, const float* x,
+                                 const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
+                                 float data_range, int size_average, int nonnegative_ssim, void* workspace,
+                                 const float* upstream, float* dx, const srf_ms_ssim_addr* dx_addr) {
+    using namespace srf;
+    const char* fn = "srf_ssim_backward";
+    (void)nonnegative_ssim;      // the forward folded the relu into the coefficients it left in the workspace
+    MsSsimArgs m;
+    if (ssim_prepare(fn, B, C, H, W, x, x_addr, y, y_addr, data_range, size_average, workspace, &m)) return 1;
+    if (!upstream) return set_error("%s: null upstream gradient", fn);
+    if (ms_ssim_addr(fn, "dx", dx, dx_addr, &m.ag)) return 1;
+    const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    const SsimLayout L = make_ssim_layout(B, C, H, W);
+    char* ws = static_cast<char*>(workspace);
+    LevelArgs a = ssim_level_args(m);
+    a.ntx = (W + kTW - 1) / kTW;
+    a.coef = reinterpret_cast<const float*>(ws + L.o_coef);
+    a.gout = upstream; a.gout_per_b = m.size_average ? 0 : 1;
+    a.gx = dx; a.ag = m.ag;
+    const dim3 grid((unsigned)(a.ntx * ((H + kTH - 1) / kTH)), (unsigned)(B * C));
+    ms_ssim_bwd_kernel<true><<<grid, kThreads, 0, stream>>>(a);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : cuda_error("ssim_bwd launch", e);
 }

@@ -15,7 +15,7 @@ bits reach the candidate, the reference build and the CPU oracle.
 from __future__ import annotations
 
 import math
-from typing import Dict, List, NamedTuple
+from typing import Dict, List, NamedTuple, Optional
 
 import torch
 
@@ -117,11 +117,14 @@ def settings_for(cam: Camera, bg: torch.Tensor, sh_degree: int, device, settings
 
 class PathCamera:
     """A camera with the attributes and ``get_rays`` of LaRa's ``tools/camera.MiniCam`` (tools/camera.py:21-56), which
-    ``MeshExtractor`` and ``Renderer.render_views`` read; ``c2w`` in OpenCV axes."""
+    ``MeshExtractor`` and ``Renderer.render_views`` read; ``c2w`` in OpenCV axes.  ``fov`` is the horizontal field of
+    view and, unless ``fovy`` is given, the vertical one too."""
 
-    def __init__(self, c2w: torch.Tensor, H: int, W: int, fov: float, znear: float = 0.5, zfar: float = 2.5):
-        cam = camera_from_c2w(c2w, H, W, fov, fov, znear, zfar)
-        self.image_width, self.image_height, self.FoVx, self.FoVy = W, H, fov, fov
+    def __init__(self, c2w: torch.Tensor, H: int, W: int, fov: float, znear: float = 0.5, zfar: float = 2.5,
+                 fovy: Optional[float] = None):
+        fovy = fov if fovy is None else fovy
+        cam = camera_from_c2w(c2w, H, W, fov, fovy, znear, zfar)
+        self.image_width, self.image_height, self.FoVx, self.FoVy = W, H, fov, fovy
         self.world_view_transform = cam.viewmatrix
         self.full_proj_transform = cam.projmatrix
         self.camera_center = cam.campos

@@ -120,3 +120,106 @@ class MS_SSIM(torch.nn.Module):
         assert min(X.shape[-2:]) > _MIN_SIDE, \
             "Image size should be larger than %d due to the 4 downsamplings in ms-ssim" % _MIN_SIDE
         return _MsSsim.apply(X, Y, False, self.data_range, self.size_average)
+
+
+# ---- single-scale SSIM (pytorch-msssim 1.0.0 ``ssim`` / ``SSIM``) ----------------------------------------------------
+
+def _check_ssim_args(fn: str, win_size, win_sigma, win, K) -> None:
+    for name, val, default in (("win_size", win_size, 11), ("win_sigma", win_sigma, 1.5), ("K", tuple(K), (0.01, 0.03))):
+        if val != default:
+            raise ValueError(f"{fn}: {name}={val!r} is not supported (only the default {default!r})")
+    if win is not None:
+        raise ValueError(f"{fn}: a custom win is not supported (only the default 11-tap, sigma 1.5 window)")
+
+
+def _check_ssim_size(fn: str, H: int, W: int) -> None:
+    if H < 11 or W < 11:
+        raise ValueError(f"{fn}: H and W must be at least the window size 11, got {H} x {W} (pytorch_msssim skips the "
+                         "filter along a shorter side with a warning; the fused SSIM does not)")
+
+
+def ssim_launch(dev: torch.device, x_ptr: int, ax, y_ptr: int, ay, shape, data_range: float, size_average: bool,
+                nonnegative_ssim: bool):
+    """srf_ssim_forward on logical [B,C,H,W] images at device addresses ``x_ptr`` / ``y_ptr`` read through ``ax`` /
+    ``ay``: (out, workspace); the workspace is what srf_ssim_backward needs."""
+    B, C, H, W = shape
+    ws = torch.empty(_lib.ssim_workspace_bytes(_lib.load(), B, C, H, W), dtype=torch.uint8, device=dev)
+    out = torch.empty(() if size_average else (B,), dtype=torch.float32, device=dev)
+    _lib.launch("srf_ssim_forward", dev, B, C, H, W, x_ptr, ctypes.byref(ax), y_ptr, ctypes.byref(ay),
+                float(data_range), 1 if size_average else 0, 1 if nonnegative_ssim else 0, ws.data_ptr(),
+                out.data_ptr())
+    return out, ws
+
+
+class _Ssim(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, X, Y, views, data_range, size_average, nonnegative_ssim):
+        if not X.is_cuda or Y.device != X.device:
+            raise RuntimeError(f"ssim: X and Y must be CUDA tensors on one device, got {X.device} and {Y.device}")
+        shape = _logical_shape(X, views)
+        out, ws = ssim_launch(X.device, X.data_ptr(), _addr(X, views), Y.data_ptr(), _addr(Y, views), shape,
+                              data_range, size_average, nonnegative_ssim)
+        ctx.save_for_backward(X, Y, ws)
+        ctx.cfg = (views, float(data_range), bool(size_average), bool(nonnegative_ssim), shape)
+        return out
+
+    @staticmethod
+    def backward(ctx, g_out):
+        X, Y, ws = ctx.saved_tensors
+        views, data_range, size_average, nonneg, (B, C, H, W) = ctx.cfg
+        up = g_out.to(torch.float32).reshape(-1).contiguous()
+        gX = torch.empty_like(X)
+        ax, ay, ag = _addr(X, views), _addr(Y, views), _addr(gX, views)
+        _lib.launch("srf_ssim_backward", X.device, B, C, H, W, X.data_ptr(), ctypes.byref(ax), Y.data_ptr(),
+                    ctypes.byref(ay), data_range, 1 if size_average else 0, 1 if nonneg else 0, ws.data_ptr(),
+                    up.data_ptr(), gX.data_ptr(), ctypes.byref(ag))
+        return gX, None, None, None, None, None
+
+
+def ssim(X: torch.Tensor, Y: torch.Tensor, data_range=255, size_average=True, win_size=11, win_sigma=1.5, win=None,
+         K=(0.01, 0.03), nonnegative_ssim=False) -> torch.Tensor:
+    """Drop-in for ``pytorch_msssim.ssim`` (same signature and defaults) on 4-D float32 CUDA inputs of any strides.
+
+    Returns the mean over (batch, channel) of the per-channel SSIM (``size_average=True``) or the per-batch mean over
+    channels; ``nonnegative_ssim`` relu's the per-channel values first.  Differentiable wrt ``X`` only.  H and W must
+    be at least 11; arguments other than the library's window and K raise."""
+    _check_ssim_args("ssim", win_size, win_sigma, win, K)
+    check_inputs("ssim", X, Y)
+    _check_ssim_size("ssim", X.shape[2], X.shape[3])
+    return _Ssim.apply(X, Y, False, data_range, size_average, nonnegative_ssim)
+
+
+class SSIM(torch.nn.Module):
+    """Drop-in for ``pytorch_msssim.SSIM``: ``forward(X, Y)`` is :func:`ssim` with the module's settings."""
+
+    def __init__(self, data_range=255, size_average=True, win_size=11, win_sigma=1.5, channel=3, spatial_dims=2,
+                 K=(0.01, 0.03), nonnegative_ssim=False):
+        super().__init__()
+        _check_ssim_args("SSIM", win_size, win_sigma, None, K)
+        if spatial_dims != 2:
+            raise ValueError(f"SSIM: spatial_dims={spatial_dims!r} is not supported (only 2)")
+        self.data_range = data_range
+        self.size_average = size_average
+        self.channel = int(channel)
+        self.nonnegative_ssim = nonnegative_ssim
+
+    def forward(self, X: torch.Tensor, Y: torch.Tensor) -> torch.Tensor:
+        check_inputs("SSIM", X, Y)
+        if X.shape[1] != self.channel:
+            raise ValueError(f"SSIM: expected {self.channel} channels, got {X.shape[1]}")
+        _check_ssim_size("SSIM", X.shape[2], X.shape[3])
+        return _Ssim.apply(X, Y, False, self.data_range, self.size_average, self.nonnegative_ssim)
+
+
+def ssim_views(image: torch.Tensor, target: torch.Tensor, data_range: float = 1.0, view_range=None) -> torch.Tensor:
+    """SSIM (mean over channels) of V planar views [V,C,H,W] read as one [1,C,H,V*W] image, the views side by side
+    along the width as LaRa concatenates them (evaluation.py:93); target as image (any strides, e.g. a permuted
+    [V,H,W,C]).  ``view_range`` (v0, v1) keeps views v0 .. v1 - 1 of both, as ``eval_novel_view_only`` does."""
+    if view_range is not None:
+        v0, v1 = (int(v) for v in view_range)
+        if not 0 <= v0 < v1 <= image.shape[0]:
+            raise ValueError(f"ssim_views: view range [{v0}, {v1}) is empty or outside the {image.shape[0]} views")
+        image, target = image[v0:v1], target[v0:v1]
+    check_inputs("ssim_views", image, target)
+    _check_ssim_size("ssim_views", image.shape[2], image.shape[0] * image.shape[3])
+    return _Ssim.apply(image, target, True, data_range, True, False)
