@@ -164,6 +164,11 @@ SIGNATURES = {
     "srf_video_frames": (c_int, [_P, c_int, c_int, c_int,                 # stream, N, H, W
                                  _P, _A, _P, _A, _P, _A,                  # image, normal, alpha
                                  _P, _P]),                                # rgb, nrm
+    # include/surfel_batch.h
+    "srf_batch_assemble": (c_int, [_P, c_int, c_int, c_int, c_int,      # stream, B, N, H, W
+                                   _P, _P, _P,                           # rgba, normal, bg
+                                   _P, _P, _P, _P,                       # i2w, i2w_down, origin, nrm_rot
+                                   _P, _P, _P, _P, _P]),                 # tar_rgb, tar_msk, tar_nrm, tar_rays, tar_rays_down
     "srf_profile_begin": (c_int, []),
     "srf_profile_end": (c_int, [POINTER(c_float), POINTER(c_int), c_int]),
 }
