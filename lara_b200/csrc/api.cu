@@ -175,7 +175,7 @@ int scene_fov(const char* fn, int S, const float* tan_fov, int image_height, int
         const float tx = tan_fov[2 * i], ty = tan_fov[2 * i + 1];
         if (!isfinite(tx) || !isfinite(ty) || !(tx > 0.f) || !(ty > 0.f))
             return set_error("%s: tan_fov of scene %d is (%g, %g), not finite and positive", fn, i, tx, ty);
-        // the focal lengths of forward_preprocess_impl / backward_impl, rasterizer_impl.cu:223-224
+        // rasterizer_impl.cu:223-224; the only place the kernels' focal lengths are computed
         s.fov[i] = make_float4(image_width / (2.0f * tx), image_height / (2.0f * ty), tx, ty);
     }
     return 0;
@@ -329,10 +329,10 @@ int forward_preprocess_check(const char* fn, int V, int P, int D, int M,
 int forward_preprocess_impl(cudaStream_t stream, int V, int P, int D, int M,
                             const float* means3D, const float* shs, const float* colors_precomp,
                             const float* opacities, const float* scales, const float* rotations,
-                            const float* transMat_precomp, const float* cams,
-                            float tan_fovx, float tan_fovy, int image_height, int image_width,
+                            const float* transMat_precomp, const float* cams, const srf::SceneArgs& scenes,
+                            int image_height, int image_width,
                             int prefiltered, int* radii, void* geom_state, void* tile_state,
-                            uint32_t* num_rendered_host, int raw_activations, const srf::SceneArgs* scenes) {
+                            uint32_t* num_rendered_host, int raw_activations) {
     const TileLayout tl = tile_layout(image_height, image_width);
     // tile blocks + counters of every view are zeroed by one 2-D memset
     cudaError_t e = cudaMemset2DAsync(at<char>(tile_state, tl.count), tl.total, 0,
@@ -351,8 +351,6 @@ int forward_preprocess_impl(cudaStream_t stream, int V, int P, int D, int M,
         a.shs = shs; a.transMat_precomp = transMat_precomp; a.colors_precomp = colors_precomp;
         a.viewmatrix = cams + SRF_CAM_VIEW; a.campos = cams + SRF_CAM_CAMPOS; a.cam_stride = SRF_CAM_FLOATS;
         a.W = image_width; a.H = image_height;
-        a.focal_y = image_height / (2.0f * tan_fovy);   // rasterizer_impl.cu:223-224
-        a.focal_x = image_width / (2.0f * tan_fovx);
         a.gx = tl.gx; a.gy = tl.gy;
         a.prefiltered = prefiltered;
         a.raw_act = (raw_activations && !transMat_precomp) ? 1 : 0;
@@ -363,7 +361,7 @@ int forward_preprocess_impl(cudaStream_t stream, int V, int P, int D, int M,
         a.tile_count = b.tile_count;
         a.geom_stride = gl.total;
         a.tile_stride = b.tile_stride;
-        e = scenes ? srf::launch_preprocess_fwd_scenes(a, *scenes, stream) : srf::launch_preprocess_fwd(a, stream);
+        e = srf::launch_preprocess_fwd(a, scenes, stream);
         if (e != cudaSuccess) return cuda_error("preprocess_fwd launch", e);
     }
     // num_rendered read-back: pinned host memory is device-visible under UVA, so the scan kernel stores the counts there
@@ -438,14 +436,14 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
                   size_t capacity, const float* cams,
                   const float* means3D, const float* shs, int colors_were_precomputed,
                   const float* scales, const float* rotations, int transmat_was_precomputed,
-                  float tan_fovx, float tan_fovy, const int* radii,
+                  const int* radii,
                   const void* geom_state, const void* tile_state, const uint32_t* point_list,
                   const void* image_state,
                   const float* dL_dout_color, const float* dL_dout_others,
                   void* scratch, int accumulate,
                   float* dL_dmeans3D, float* dL_dmeans2D, float* dL_dsh, float* dL_dcolors,
                   float* dL_dopacity, float* dL_dscales, float* dL_drotations, float* dL_dtransMat,
-                  int raw_activations, bool deterministic, const srf::SceneArgs* scenes, int S) {
+                  int raw_activations, bool deterministic, const srf::SceneArgs& scenes, int S) {
     if (!cams) return set_error("%s: null camera records", fn);
     if (V <= 0 || P < 0 || image_height <= 0 || image_width <= 0) return set_error("%s: bad sizes", fn);
     if (P == 0) return 0;
@@ -499,14 +497,10 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
 
     srf::PreprocessBwdArgs p;
     memset(&p, 0, sizeof(p));
-    p.P = P; p.D = D; p.M = (shs && !colors_were_precomputed) ? M : 0; p.nviews = V;
+    p.P = P; p.D = D; p.M = (shs && !colors_were_precomputed) ? M : 0;
     p.means3D = means3D; p.scales = scales; p.rotations = rotations;
     p.shs = colors_were_precomputed ? nullptr : shs;
     p.viewmatrix = cams + SRF_CAM_VIEW; p.campos = cams + SRF_CAM_CAMPOS; p.cam_stride = SRF_CAM_FLOATS;
-    p.W = image_width; p.H = image_height;
-    p.focal_y = image_height / (2.0f * tan_fovy);
-    p.focal_x = image_width / (2.0f * tan_fovx);
-    p.tan_fovx = tan_fovx; p.tan_fovy = tan_fovy;
     p.has_precomp_T = transmat_was_precomputed ? 1 : 0;
     p.has_precomp_color = colors_were_precomputed ? 1 : 0;
     p.raw_act = (raw_activations && !transmat_was_precomputed) ? 1 : 0;
@@ -519,7 +513,7 @@ int backward_impl(const char* fn, cudaStream_t stream, int V, int P, int D, int 
     p.dL_dsh = p.M > 0 ? dL_dsh : nullptr;
     p.dL_dcolors = dL_dcolors; p.dL_dopacity = dL_dopacity;
     p.dL_dscales = dL_dscales; p.dL_drotations = dL_drotations; p.dL_dtransMat = dL_dtransMat;
-    e = scenes ? srf::launch_preprocess_bwd_scenes(p, *scenes, S, stream) : srf::launch_preprocess_bwd(p, stream);
+    e = srf::launch_preprocess_bwd(p, scenes, S, stream);
     if (e != cudaSuccess) return cuda_error("preprocess_bwd launch", e);
     return deterministic ? srf::check_overflow_flag(fn, overflow, stream) : 0;
 }
@@ -561,12 +555,9 @@ int srf_scenes_forward(srf_stream_t stream_, int S, int Vs, int P, int D, int M,
                              image_state, cams, out_color, out_others, for_backward != 0))
         return 1;
     if ((size_t)S * P > 0x7fffffffull) return set_error("%s: S * P exceeds 32-bit Gaussian indices", fn);
-    // one scene runs the preprocess instantiation without scene arguments (NoScenes): it reads the focal lengths
-    // scene_fov computed from the same tan_fov, and it is the lighter kernel (DESIGN §3.21)
     int rc = forward_preprocess_impl(stream, V, P, D, M, means3D, shs, colors_precomp, opacities, scales, rotations,
-                                     transMat_precomp, cams, scenes.fov[0].z, scenes.fov[0].w, image_height, image_width,
-                                     prefiltered, radii, geom_state, tile_state, num_rendered_host, raw_activations,
-                                     S == 1 ? nullptr : &scenes);
+                                     transMat_precomp, cams, scenes, image_height, image_width, prefiltered, radii,
+                                     geom_state, tile_state, num_rendered_host, raw_activations);
     if (rc != 0) return rc;
     if (count_event) {      // lets the caller wait for the instance counts without waiting for the blend
         cudaError_t e = cudaEventRecord(static_cast<cudaEvent_t>(count_event), stream);
@@ -598,11 +589,10 @@ int srf_scenes_backward(srf_stream_t stream_, int S, int Vs, int P, const int64_
     scenes.views_per_scene = Vs;
     scenes.offsets = offsets;
     return backward_impl(fn, stream, S * Vs, P, D, M, image_height, image_width, capacity, cams, means3D, shs,
-                         colors_were_precomputed, scales, rotations, transmat_was_precomputed, scenes.fov[0].z,
-                         scenes.fov[0].w, radii, geom_state, tile_state, point_list, image_state, dL_dout_color,
-                         dL_dout_others, scratch, accumulate, dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity,
-                         dL_dscales, dL_drotations, dL_dtransMat, raw_activations, deterministic != 0,
-                         S == 1 && !offsets ? nullptr : &scenes, S);
+                         colors_were_precomputed, scales, rotations, transmat_was_precomputed, radii, geom_state,
+                         tile_state, point_list, image_state, dL_dout_color, dL_dout_others, scratch, accumulate,
+                         dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drotations,
+                         dL_dtransMat, raw_activations, deterministic != 0, scenes, S);
 }
 
 int srf_views_backward_deterministic_scratch_bytes(int V, int P, size_t* bytes) {

@@ -14,8 +14,6 @@
 #include <cuda_fp16.h>
 #include <stdio.h>
 
-#include <type_traits>
-
 #include "surfel_common.cuh"
 #include "surfel_kernels.h"
 #include "sh_eval.cuh"
@@ -37,23 +35,14 @@ __device__ __forceinline__ void stage_rows(float* __restrict__ dst, const float*
     }
 }
 
-template <typename T>
-__device__ __forceinline__ const T* rows_at(const T* p, size_t row, int width) {
-    return p ? p + row * width : p;
-}
-
 // Adds one instance to every tile of rect [x0,x1) x [y0,y1).
 __device__ __forceinline__ void count_tiles_serial(uint32_t* tile_count, int gx, int x0, int y0, int x1, int y1) {
     for (int y = y0; y < y1; ++y)
         for (int x = x0; x < x1; ++x) atomicAdd(&tile_count[(size_t)(y * gx + x) * SRF_TILE_CTR_STRIDE], 1u);
 }
 
-// For one scene (srf_scenes_forward with S = 1) the kernel takes an empty second argument; with S > 1 scenes the
-// view's scene gives the Gaussian rows and the field of view.
-struct NoScenes {};
-
-template <typename Scenes>
-__global__ void __launch_bounds__(256) preprocess_fwd_kernel(PreprocessArgs a, const __grid_constant__ Scenes s) {
+// The view's scene (blockIdx.y / Vs) gives the Gaussian rows and the field of view; one scene is S = 1.
+__global__ void __launch_bounds__(256) preprocess_fwd_kernel(PreprocessArgs a, const __grid_constant__ SceneArgs s) {
     __shared__ __align__(16) float s_means[256 * 3];
     __shared__ float s_view[16];
     __shared__ float s_cam[3];
@@ -64,29 +53,24 @@ __global__ void __launch_bounds__(256) preprocess_fwd_kernel(PreprocessArgs a, c
     const int idx = base + tid;
     const int nrows = min(256, a.P - base);
     const bool in_range = idx < a.P;
-    {   // view of this CTA (blockIdx.y): own camera, own geom / tile workspace, own radii row
-        const int view = blockIdx.y;
-        a.viewmatrix += (size_t)view * a.cam_stride;
-        a.campos += (size_t)view * a.cam_stride;
-        a.radii += (size_t)view * a.P;
-        a.rec = view_ptr(a.rec, view, a.geom_stride);
-        a.depths = view_ptr(a.depths, view, a.geom_stride);
-        a.rects = view_ptr(a.rects, view, a.geom_stride);
-        a.tile_count = view_ptr(a.tile_count, view, a.tile_stride);
-        if constexpr (!std::is_same<Scenes, NoScenes>::value) {
-            const int scene = view / s.views_per_scene;
-            const size_t row = (size_t)scene * a.P;
-            a.means3D = rows_at(a.means3D, row, 3);
-            a.scales = rows_at(a.scales, row, 2);
-            a.rotations = rows_at(a.rotations, row, 4);
-            a.opacities = rows_at(a.opacities, row, 1);
-            a.shs = rows_at(a.shs, row, 3 * a.M);
-            a.transMat_precomp = rows_at(a.transMat_precomp, row, 9);
-            a.colors_precomp = rows_at(a.colors_precomp, row, 3);
-            a.focal_x = s.fov[scene].x;
-            a.focal_y = s.fov[scene].y;
-        }
-    }
+    // view of this CTA (blockIdx.y): own camera, own geom / tile workspace, own radii row; its scene's Gaussian rows
+    const int view = blockIdx.y, scene = view / s.views_per_scene;
+    a.viewmatrix += (size_t)view * a.cam_stride;
+    a.campos += (size_t)view * a.cam_stride;
+    a.radii += (size_t)view * a.P;
+    a.rec = view_ptr(a.rec, view, a.geom_stride);
+    a.depths = view_ptr(a.depths, view, a.geom_stride);
+    a.rects = view_ptr(a.rects, view, a.geom_stride);
+    a.tile_count = view_ptr(a.tile_count, view, a.tile_stride);
+    const size_t row = (size_t)scene * a.P;
+    a.means3D = rows_at(a.means3D, row, 3);
+    a.scales = rows_at(a.scales, row, 2);
+    a.rotations = rows_at(a.rotations, row, 4);
+    a.opacities = rows_at(a.opacities, row, 1);
+    a.shs = rows_at(a.shs, row, 3 * a.M);
+    a.transMat_precomp = rows_at(a.transMat_precomp, row, 9);
+    a.colors_precomp = rows_at(a.colors_precomp, row, 3);
+    const float focal_x = s.fov[scene].x, focal_y = s.fov[scene].y;
 
     stage_rows(s_means, a.means3D + (size_t)base * 3, nrows * 3, tid, 256);
     if (tid < 16) s_view[tid] = __ldg(a.viewmatrix + tid);
@@ -170,12 +154,12 @@ __global__ void __launch_bounds__(256) preprocess_fwd_kernel(PreprocessArgs a, c
                 const float M1y = fma_(v9, a1z, fma_(v1, a1x, fmul_(v5, a1y)));
                 const float M1z = fma_(v10, a1z, fma_(v2, a1x, fmul_(v6, a1y)));
                 const float cxh = fmul_((float)a.W, 0.5f), cyh = fmul_((float)a.H, 0.5f);
-                Tux = fma_(M0z, cxh, fmul_(M0x, a.focal_x));
-                Tuy = fma_(M1z, cxh, fmul_(M1x, a.focal_x));
-                Tuz = fma_(pvz, cxh, fmul_(pvx, a.focal_x));
-                Tvx = fma_(M0z, cyh, fmul_(M0y, a.focal_y));
-                Tvy = fma_(M1z, cyh, fmul_(M1y, a.focal_y));
-                Tvz = fma_(pvz, cyh, fmul_(pvy, a.focal_y));
+                Tux = fma_(M0z, cxh, fmul_(M0x, focal_x));
+                Tuy = fma_(M1z, cxh, fmul_(M1x, focal_x));
+                Tuz = fma_(pvz, cxh, fmul_(pvx, focal_x));
+                Tvx = fma_(M0z, cyh, fmul_(M0y, focal_y));
+                Tvy = fma_(M1z, cyh, fmul_(M1y, focal_y));
+                Tvz = fma_(pvz, cyh, fmul_(pvy, focal_y));
                 Twx = M0z; Twy = M1z; Twz = pvz;
                 const float mult = cosv > 0.0f ? 1.0f : -1.0f;
                 nx = fmul_(tnx, mult); ny = fmul_(tny, mult); nz = fmul_(tnz, mult);
@@ -345,8 +329,7 @@ __global__ void __launch_bounds__(256) mark_visible_kernel(int P, const float* _
     present[idx] = (pvz <= 0.2f) ? 0 : 1;
 }
 
-template <typename Scenes>
-static cudaError_t launch_preprocess(const PreprocessArgs& a, const Scenes& s, cudaStream_t stream) {
+cudaError_t launch_preprocess_fwd(const PreprocessArgs& a, const SceneArgs& s, cudaStream_t stream) {
     if (a.P <= 0 || a.nviews <= 0) return cudaSuccess;
     PreprocessArgs args = a;
     const size_t sh_bytes = (size_t)256 * 3 * a.M * sizeof(float);
@@ -358,17 +341,9 @@ static cudaError_t launch_preprocess(const PreprocessArgs& a, const Scenes& s, c
     const size_t dyn = args.stage_sh ? sh_bytes : 0;
     const int grid = (a.P + 255) / 256;
     prof_start(K_PREPROCESS_FWD, stream);
-    preprocess_fwd_kernel<Scenes><<<dim3(grid, a.nviews), 256, dyn, stream>>>(args, s);
+    preprocess_fwd_kernel<<<dim3(grid, a.nviews), 256, dyn, stream>>>(args, s);
     prof_stop(K_PREPROCESS_FWD, stream);
     return cudaGetLastError();
-}
-
-cudaError_t launch_preprocess_fwd(const PreprocessArgs& a, cudaStream_t stream) {
-    return launch_preprocess(a, NoScenes(), stream);
-}
-
-cudaError_t launch_preprocess_fwd_scenes(const PreprocessArgs& a, const SceneArgs& s, cudaStream_t stream) {
-    return launch_preprocess(a, s, stream);
 }
 
 cudaError_t launch_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present,

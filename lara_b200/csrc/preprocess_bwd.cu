@@ -3,13 +3,11 @@
 // (preprocessCUDA backward), :451-529 (computeTransMat vjp), :20-139 (SH vjp) and
 // auxiliary.h:213-257 (quat_to_rotmat_vjp), :125-135 (dnormvdv).
 //
-// One thread per Gaussian.  Reads the 80 B gradient record accumulated by the blend
+// One thread per (Gaussian, scene), summing the scene's views.  Reads the 80 B gradient record accumulated by the blend
 // backward plus the forward's GeomRecord, and writes *every* output gradient row --
 // zeros for culled Gaussians -- so the host never pre-fills nine zero tensors as the
 // reference does (rasterize_points.cu:194-202).  With accumulate=1 the kernel adds into
 // the outputs instead (view-sharded accumulation before the NCCL all-reduce).
-#include <type_traits>
-
 #include "surfel_common.cuh"
 #include "surfel_kernels.h"
 
@@ -46,55 +44,43 @@ __device__ __forceinline__ void put2(float* p, float2 v) {   // p must be 8-byte
     *q = v;
 }
 
-template <typename T>
-__device__ __forceinline__ T* rows_at(T* p, size_t row, int width) {
-    return p ? p + row * width : p;
-}
-
-// For one scene without offsets (srf_scenes_backward with S = 1) the kernel takes an empty second argument.  Else it
-// runs one thread per (Gaussian, scene = blockIdx.y) and sums that scene's Vs views: the scene gives the rows of the
-// inputs and outputs, the first view and the field of view.
-struct NoScenes {};
-
-template <bool ACC, typename Scenes>
-__global__ void __launch_bounds__(256) preprocess_bwd_kernel(PreprocessBwdArgs a, const __grid_constant__ Scenes s) {
+// One thread per (Gaussian, scene = blockIdx.y); it sums that scene's Vs views.  The scene gives the rows of the inputs
+// and outputs, the first view and the field of view.  One scene is S = 1.  Both instantiations fit 2 CTAs per SM
+// (128 registers) without spills or a local frame.
+template <bool ACC>
+__global__ void __launch_bounds__(256, 2) preprocess_bwd_kernel(PreprocessBwdArgs a, const __grid_constant__ SceneArgs s) {
     const int idx = blockIdx.x * 256 + threadIdx.x;
-    if constexpr (std::is_same<Scenes, NoScenes>::value) {
-        if (idx >= a.P) return;
-    } else {
-        const int scene = blockIdx.y;
-        size_t row = (size_t)scene * a.P;
-        int n = a.P;
-        if (s.offsets) {
-            row = (size_t)s.offsets[scene];
-            n = (int)(s.offsets[scene + 1] - s.offsets[scene]);
-        }
-        const int v0 = scene * s.views_per_scene;
-        a.nviews = s.views_per_scene;
-        a.radii += (size_t)v0 * a.P;
-        a.rec = view_ptr(a.rec, v0, a.geom_stride);
-        a.ggrad = view_ptr(a.ggrad, v0, a.ggrad_stride);
-        a.viewmatrix += (size_t)v0 * a.cam_stride;
-        a.campos += (size_t)v0 * a.cam_stride;
-        a.focal_x = s.fov[scene].x; a.focal_y = s.fov[scene].y;
-        a.tan_fovx = s.fov[scene].z; a.tan_fovy = s.fov[scene].w;
-        a.means3D = rows_at(a.means3D, row, 3);
-        a.scales = rows_at(a.scales, row, 2);
-        a.rotations = rows_at(a.rotations, row, 4);
-        a.shs = rows_at(a.shs, row, 3 * a.M);
-        a.dL_dmeans3D = rows_at(a.dL_dmeans3D, row, 3);
-        a.dL_dmeans2D = rows_at(a.dL_dmeans2D, row, 3);
-        a.dL_dsh = rows_at(a.dL_dsh, row, 3 * a.M);
-        a.dL_dcolors = rows_at(a.dL_dcolors, row, 3);
-        a.dL_dopacity = rows_at(a.dL_dopacity, row, 1);
-        a.dL_dscales = rows_at(a.dL_dscales, row, 2);
-        a.dL_drotations = rows_at(a.dL_drotations, row, 4);
-        a.dL_dtransMat = rows_at(a.dL_dtransMat, row, 9);
-        if (idx >= n) return;
+    const int scene = blockIdx.y;
+    size_t row = (size_t)scene * a.P;
+    int n = a.P;
+    if (s.offsets) {
+        row = (size_t)s.offsets[scene];
+        n = (int)(s.offsets[scene + 1] - s.offsets[scene]);
     }
+    const int nviews = s.views_per_scene, v0 = scene * nviews;
+    a.radii += (size_t)v0 * a.P;
+    a.rec = view_ptr(a.rec, v0, a.geom_stride);
+    a.ggrad = view_ptr(a.ggrad, v0, a.ggrad_stride);
+    a.viewmatrix += (size_t)v0 * a.cam_stride;
+    a.campos += (size_t)v0 * a.cam_stride;
+    const float focal_x = s.fov[scene].x, focal_y = s.fov[scene].y;
+    const float tan_fovx = s.fov[scene].z, tan_fovy = s.fov[scene].w;
+    a.means3D = rows_at(a.means3D, row, 3);
+    a.scales = rows_at(a.scales, row, 2);
+    a.rotations = rows_at(a.rotations, row, 4);
+    a.shs = rows_at(a.shs, row, 3 * a.M);
+    a.dL_dmeans3D = rows_at(a.dL_dmeans3D, row, 3);
+    a.dL_dmeans2D = rows_at(a.dL_dmeans2D, row, 3);
+    a.dL_dsh = rows_at(a.dL_dsh, row, 3 * a.M);
+    a.dL_dcolors = rows_at(a.dL_dcolors, row, 3);
+    a.dL_dopacity = rows_at(a.dL_dopacity, row, 1);
+    a.dL_dscales = rows_at(a.dL_dscales, row, 2);
+    a.dL_drotations = rows_at(a.dL_drotations, row, 4);
+    a.dL_dtransMat = rows_at(a.dL_dtransMat, row, 9);
+    if (idx >= n) return;
     const int M3 = 3 * a.M;
 
-    // sums over the views of the call (one view in the drop-in path)
+    // sums over the scene's views
     float dmean3D[3] = {0.f, 0.f, 0.f};
     float dmean2D[2] = {0.f, 0.f};
     float dscale[2] = {0.f, 0.f};
@@ -135,7 +121,7 @@ __global__ void __launch_bounds__(256) preprocess_bwd_kernel(PreprocessBwdArgs a
     }
     const float* sh = want_sh ? a.shs + (size_t)idx * M3 : nullptr;
 
-    for (int view = 0; view < a.nviews; ++view) {
+    for (int view = 0; view < nviews; ++view) {
         if (!(a.radii[(size_t)view * a.P + idx] > 0)) continue;
         any_visible = true;
         const float4* r = view_ptr(a.rec, view, a.geom_stride) + (size_t)idx * SRF_REC_QUADS;
@@ -174,7 +160,7 @@ __global__ void __launch_bounds__(256) preprocess_bwd_kernel(PreprocessBwdArgs a
             vT[3] += dT1.x; vT[4] += dT1.y; vT[5] += dT1.z;
             vT[6] += dT3.x; vT[7] += dT3.y; vT[8] += dT3.z;
             // the value Python receives as grad_means2D (densification statistic, :645-648)
-            const float Wc = a.focal_x * a.tan_fovx, Hc = a.focal_y * a.tan_fovy;
+            const float Wc = focal_x * tan_fovx, Hc = focal_y * tan_fovy;
             dmean2D[0] += vT[2] * Tw.z * Wc;
             dmean2D[1] += vT[5] * Tw.z * Hc;
         }
@@ -188,8 +174,8 @@ __global__ void __launch_bounds__(256) preprocess_bwd_kernel(PreprocessBwdArgs a
             const float v4 = __ldg(vm + 4), v5 = __ldg(vm + 5), v6 = __ldg(vm + 6);
             const float v8 = __ldg(vm + 8), v9 = __ldg(vm + 9), v10 = __ldg(vm + 10);
             const float v12 = __ldg(vm + 12), v13 = __ldg(vm + 13), v14 = __ldg(vm + 14);
-            const float fx = a.focal_x, fy = a.focal_y;
-            const float cx = a.focal_x * a.tan_fovx, cy = a.focal_y * a.tan_fovy;
+            const float fx = focal_x, fy = focal_y;
+            const float cx = focal_x * tan_fovx, cy = focal_y * tan_fovy;
             const float w = qw, x = qx, y = qy, z = qz;
 
             const V3 pview = v3(v0 * px + v4 * py + v8 * pz + v12, v1 * px + v5 * py + v9 * pz + v13,
@@ -239,35 +225,50 @@ __global__ void __launch_bounds__(256) preprocess_bwd_kernel(PreprocessBwdArgs a
             const V3 dir_orig = v3(px - __ldg(cp), py - __ldg(cp + 1), pz - __ldg(cp + 2));
             const float len = sqrtf(dir_orig.x * dir_orig.x + dir_orig.y * dir_orig.y + dir_orig.z * dir_orig.z);
             const V3 dir = v3(dir_orig.x / len, dir_orig.y / len, dir_orig.z / len);
-            float coef[16];
+            // the basis values (coefficient rows): rows 0..3 for the M = 4 path, every row written as it is
+            // computed on the general-M path, where rows accumulate in place (same thread re-reads its own stores)
+            float coef[4] = {0.f, 0.f, 0.f, 0.f};
+            float* const rows = (a.dL_dsh != nullptr && !sh_fast) ? a.dL_dsh + (size_t)idx * M3 : nullptr;
+            const bool add = ACC || sh_rows_written;
+            auto row = [&](int k, float ck) {
+                if (rows == nullptr || k >= a.M) return;
 #pragma unroll
-            for (int k = 0; k < 16; ++k) coef[k] = 0.f;
+                for (int c = 0; c < 3; ++c) {
+                    float* o = rows + 3 * k + c;
+                    const float val = ck * dRGB[c];
+                    *o = add ? (*o + val) : val;
+                }
+            };
+            int nrows = 1;                       // rows set from the basis; the rest up to M get zero coefficients
             const float x = dir.x, y = dir.y, z = dir.z;
             V3 dRGBdx = v3(0.f, 0.f, 0.f), dRGBdy = v3(0.f, 0.f, 0.f), dRGBdz = v3(0.f, 0.f, 0.f);
             auto SH = [&](int k) { return v3(__ldg(sh + 3 * k), __ldg(sh + 3 * k + 1), __ldg(sh + 3 * k + 2)); };
             coef[0] = kC0;
             if (a.D > 0) {
                 coef[1] = -kC1 * y; coef[2] = kC1 * z; coef[3] = -kC1 * x;
+                nrows = 4;
                 dRGBdx = (-kC1) * SH(3);
                 dRGBdy = (-kC1) * SH(1);
                 dRGBdz = kC1 * SH(2);
                 if (a.D > 1) {
                     const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
-                    coef[4] = kC2[0] * xy; coef[5] = kC2[1] * yz; coef[6] = kC2[2] * (2.f * zz - xx - yy);
-                    coef[7] = kC2[3] * xz; coef[8] = kC2[4] * (xx - yy);
+                    row(4, kC2[0] * xy); row(5, kC2[1] * yz); row(6, kC2[2] * (2.f * zz - xx - yy));
+                    row(7, kC2[3] * xz); row(8, kC2[4] * (xx - yy));
+                    nrows = 9;
                     dRGBdx = dRGBdx + (kC2[0] * y) * SH(4) + (kC2[2] * 2.f * -x) * SH(6) + (kC2[3] * z) * SH(7) +
                              (kC2[4] * 2.f * x) * SH(8);
                     dRGBdy = dRGBdy + (kC2[0] * x) * SH(4) + (kC2[1] * z) * SH(5) + (kC2[2] * 2.f * -y) * SH(6) +
                              (kC2[4] * 2.f * -y) * SH(8);
                     dRGBdz = dRGBdz + (kC2[1] * y) * SH(5) + (kC2[2] * 2.f * 2.f * z) * SH(6) + (kC2[3] * x) * SH(7);
                     if (a.D > 2) {
-                        coef[9] = kC3[0] * y * (3.f * xx - yy);
-                        coef[10] = kC3[1] * xy * z;
-                        coef[11] = kC3[2] * y * (4.f * zz - xx - yy);
-                        coef[12] = kC3[3] * z * (2.f * zz - 3.f * xx - 3.f * yy);
-                        coef[13] = kC3[4] * x * (4.f * zz - xx - yy);
-                        coef[14] = kC3[5] * z * (xx - yy);
-                        coef[15] = kC3[6] * x * (xx - 3.f * yy);
+                        row(9, kC3[0] * y * (3.f * xx - yy));
+                        row(10, kC3[1] * xy * z);
+                        row(11, kC3[2] * y * (4.f * zz - xx - yy));
+                        row(12, kC3[3] * z * (2.f * zz - 3.f * xx - 3.f * yy));
+                        row(13, kC3[4] * x * (4.f * zz - xx - yy));
+                        row(14, kC3[5] * z * (xx - yy));
+                        row(15, kC3[6] * x * (xx - 3.f * yy));
+                        nrows = 16;
                         dRGBdx = dRGBdx + (kC3[0] * 3.f * 2.f * xy) * SH(9) + (kC3[1] * yz) * SH(10) +
                                  (kC3[2] * -2.f * xy) * SH(11) + (kC3[3] * -3.f * 2.f * xz) * SH(12) +
                                  (kC3[4] * (-3.f * xx + 4.f * zz - yy)) * SH(13) + (kC3[5] * 2.f * xz) * SH(14) +
@@ -301,19 +302,9 @@ __global__ void __launch_bounds__(256) preprocess_bwd_kernel(PreprocessBwdArgs a
                         dsh4[3 * k + 2] += coef[k] * dRGB[2];
                     }
                 } else {
-                    // general M: rows accumulate in place (same thread re-reads its own stores)
-                    float* out = a.dL_dsh + (size_t)idx * M3;
-                    const int ncoef = a.M < 16 ? a.M : 16;
-                    const bool add = ACC || sh_rows_written;
-                    for (int k = 0; k < a.M; ++k) {
-                        const float ck = (k < ncoef) ? coef[k] : 0.f;
 #pragma unroll
-                        for (int c = 0; c < 3; ++c) {
-                            float* o = out + 3 * k + c;
-                            const float val = ck * dRGB[c];
-                            *o = add ? (*o + val) : val;
-                        }
-                    }
+                    for (int k = 0; k < 4; ++k) row(k, coef[k]);
+                    for (int k = nrows; k < a.M; ++k) row(k, 0.f);
                     sh_rows_written = true;
                 }
             }
@@ -377,9 +368,8 @@ __global__ void __launch_bounds__(256) preprocess_bwd_kernel(PreprocessBwdArgs a
     }
 }
 
-template <typename Scenes>
-static cudaError_t launch(const PreprocessBwdArgs& a, const Scenes& s, int S, cudaStream_t stream) {
-    if (a.P <= 0 || a.nviews <= 0) return cudaSuccess;
+cudaError_t launch_preprocess_bwd(const PreprocessBwdArgs& a, const SceneArgs& s, int S, cudaStream_t stream) {
+    if (a.P <= 0) return cudaSuccess;
     const dim3 grid((a.P + 255) / 256, S);
     PreprocessBwdArgs args = a;
     // every row is a whole number of 16-byte rotation / 8-byte scale / (M = 4) 48-byte SH rows from the base
@@ -387,19 +377,11 @@ static cudaError_t launch(const PreprocessBwdArgs& a, const Scenes& s, int S, cu
     args.vec_ok = (al(a.dL_drotations, 16) && al(a.dL_dscales, 8) && (a.dL_dsh == nullptr || al(a.dL_dsh, 16))) ? 1 : 0;
     prof_start(K_PREPROCESS_BWD, stream);
     if (a.accumulate)
-        preprocess_bwd_kernel<true, Scenes><<<grid, 256, 0, stream>>>(args, s);
+        preprocess_bwd_kernel<true><<<grid, 256, 0, stream>>>(args, s);
     else
-        preprocess_bwd_kernel<false, Scenes><<<grid, 256, 0, stream>>>(args, s);
+        preprocess_bwd_kernel<false><<<grid, 256, 0, stream>>>(args, s);
     prof_stop(K_PREPROCESS_BWD, stream);
     return cudaGetLastError();
-}
-
-cudaError_t launch_preprocess_bwd(const PreprocessBwdArgs& a, cudaStream_t stream) {
-    return launch(a, NoScenes(), 1, stream);
-}
-
-cudaError_t launch_preprocess_bwd_scenes(const PreprocessBwdArgs& a, const SceneArgs& s, int S, cudaStream_t stream) {
-    return launch(a, s, S, stream);
 }
 
 }  // namespace srf

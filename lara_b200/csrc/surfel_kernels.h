@@ -51,7 +51,6 @@ struct PreprocessArgs {
     const float* campos;         // [3]                             (per view)
     size_t cam_stride;           // floats
     int W, H;
-    float focal_x, focal_y;
     int gx, gy;                  // tile grid
     int prefiltered;
     int stage_sh;                // set by the launcher
@@ -121,7 +120,6 @@ struct RenderBwdArgs {
 
 struct PreprocessBwdArgs {
     int P, D, M;
-    int nviews;                  // gradients of all views are summed in registers and written once
     const float* means3D;
     const float* scales;
     const float* rotations;
@@ -129,8 +127,6 @@ struct PreprocessBwdArgs {
     const float* viewmatrix;
     const float* campos;
     size_t cam_stride;
-    int W, H;
-    float focal_x, focal_y, tan_fovx, tan_fovy;
     int has_precomp_T;           // transMat_precomp was given: only dL_dtransMat is produced
     int has_precomp_color;
     int raw_act;                 // as in PreprocessArgs; gradients are then wrt the raw parameters
@@ -151,14 +147,21 @@ struct PreprocessBwdArgs {
 };
 
 // The scenes of an srf_scenes_* call (include/surfel_rasterizer.h): S scenes of Vs views each, laid out as V = S*Vs
-// views; view v belongs to scene v / Vs.  Passed as a __grid_constant__ kernel parameter (the kernels index `fov` by
-// the scene without a local copy) next to the per-view arguments, whose Gaussian pointers are those of scene 0.
+// views; view v belongs to scene v / Vs.  One scene is S = 1.  Passed as a __grid_constant__ kernel parameter (the
+// kernels index `fov` by the scene without a local copy) next to the per-view arguments, whose Gaussian pointers are
+// those of scene 0.  scene_fov is the one place the focal lengths are computed.
 struct SceneArgs {
     int views_per_scene;         // Vs
     const int64_t* offsets;      // [S+1] device: scene s's Gaussians are rows [offsets[s], offsets[s+1]) of the inputs
                                  //   and gradients; null: rows [s*P, (s+1)*P)
     float4 fov[SRF_MAX_SCENES];  // per scene: focal_x, focal_y, tan_fovx, tan_fovy
 };
+
+// pointer to row `row` of a `width`-float row array; null stays null
+template <typename T>
+__device__ __forceinline__ T* rows_at(T* p, size_t row, int width) {
+    return p ? p + row * width : p;
+}
 
 // Optional per-kernel CUDA-event timing (srf_profile_begin/end in the C ABI); no-ops unless enabled.
 enum KernelId { K_PREPROCESS_FWD = 0, K_TILE_SCAN, K_SCATTER, K_SORT_SMALL, K_SORT_BIG, K_RENDER_FWD,
@@ -193,7 +196,8 @@ int check_scenes(const char* fn, int S, int Vs);
 int scene_fov(const char* fn, int S, const float* tan_fov, int image_height, int image_width, SceneArgs& s);
 int check_offsets(const char* fn, cudaStream_t stream, int S, const int64_t* offsets, int n_max, int n);
 
-cudaError_t launch_preprocess_fwd(const PreprocessArgs& a, cudaStream_t stream);
+// a.nviews = S * Vs views, each reading the Gaussian inputs of its scene in `s`
+cudaError_t launch_preprocess_fwd(const PreprocessArgs& a, const SceneArgs& s, cudaStream_t stream);
 cudaError_t launch_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present,
                                 cudaStream_t stream);
 cudaError_t launch_tile_scan(const BinArgs& a, cudaStream_t stream);
@@ -207,10 +211,7 @@ cudaError_t launch_render_bwd(const RenderBwdArgs& a, cudaStream_t stream);
 size_t det_record_bytes();
 cudaError_t launch_render_bwd_det(const RenderBwdArgs& a, int P, float* ggrad, size_t ggrad_stride, uint32_t* overflow,
                                   cudaStream_t stream);
-cudaError_t launch_preprocess_bwd(const PreprocessBwdArgs& a, cudaStream_t stream);
-// The same kernels over the scenes of `s`: a.nviews = S * Vs views whose Gaussian inputs are those of their scene.  The
-// backward runs one thread per (Gaussian, scene) and sums that scene's Vs views only.
-cudaError_t launch_preprocess_fwd_scenes(const PreprocessArgs& a, const SceneArgs& s, cudaStream_t stream);
-cudaError_t launch_preprocess_bwd_scenes(const PreprocessBwdArgs& a, const SceneArgs& s, int S, cudaStream_t stream);
+// one thread per (Gaussian, scene of `s`), summing that scene's Vs views
+cudaError_t launch_preprocess_bwd(const PreprocessBwdArgs& a, const SceneArgs& s, int S, cudaStream_t stream);
 
 }  // namespace srf
