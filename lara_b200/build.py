@@ -24,7 +24,7 @@ LIB = os.path.join(HERE, "libsurfel_b200.so")
 SOURCES = ["api.cu", "preprocess.cu", "binning.cu", "render_fwd.cu", "render_bwd.cu", "preprocess_bwd.cu", "epilogue.cu", "loss.cu", "decoder.cu", "point_feats.cu", "ms_ssim.cu", "mesh.cu", "fine_head.cu",
            "feat_volume.cu", "subset.cu", "vol_transformer.cu", "coarse_head.cu", "eval.cu",
            "batch.cu"]
-HEADERS = ["surfel_common.cuh", "surfel_kernels.h", "det_sum.cuh", "mc_table.cuh", "sample_taps.cuh", "sh_eval.cuh", "decoder_layout.cuh",
+HEADERS = ["surfel_common.cuh", "surfel_kernels.h", "det_sum.cuh", "fixed_sums.cuh", "mc_table.cuh", "sample_taps.cuh", "sh_eval.cuh", "decoder_layout.cuh",
            os.path.join("..", "..", "include", "surfel_rasterizer.h"), os.path.join("..", "..", "include", "surfel_mesh.h"),
            os.path.join("..", "..", "include", "surfel_fine_head.h"),
            os.path.join("..", "..", "include", "surfel_feat_volume.h"),

@@ -21,6 +21,7 @@
 
 #include "../../include/surfel_coarse_head.h"
 #include "decoder_layout.cuh"
+#include "fixed_sums.cuh"
 #include "surfel_kernels.h"
 
 namespace srf {
@@ -398,27 +399,6 @@ __global__ void __launch_bounds__(bwd_warps(WS) * 32, 1) coarse_head_bwd_kernel(
     }
 }
 
-// the six parameter gradients: the per-CTA partials summed over the CTAs, in CTA order, in fp64
-__global__ void coarse_head_reduce_kernel(const float* partials, int nparts, int D, int O, float* d_w0, float* d_b0,
-                                          float* d_w1, float* d_b1, float* d_w2, float* d_b2) {
-    const int nacc = nacc_of(D, O);
-    int e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= nacc) return;
-    double s = 0.0;
-    for (int b = 0; b < nparts; ++b) s += (double)partials[(size_t)b * nacc + e];
-    const float v = (float)s;
-    if (e < D * D) { d_w0[e] = v; return; }
-    e -= D * D;
-    if (e < D) { d_b0[e] = v; return; }
-    e -= D;
-    if (e < D * D) { d_w1[e] = v; return; }
-    e -= D * D;
-    if (e < D) { d_b1[e] = v; return; }
-    e -= D;
-    if (e < O * D) { d_w2[e] = v; return; }
-    d_b2[e - O * D] = v;
-}
-
 using Kernel = void (*)(Args);
 
 template <int D>
@@ -563,9 +543,10 @@ extern "C" int srf_coarse_head_backward(void* stream_, int rows, int N, int D, i
         kern<<<grid, srf::bwd_warps(ws) * 32, smem, stream>>>(a);
         if ((e = cudaGetLastError()) != cudaSuccess) return cuda_error("coarse_head_bwd launch", e);
     }
-    const int nacc = srf::nacc_of(D, a.O);
-    srf::coarse_head_reduce_kernel<<<(nacc + 255) / 256, 256, 0, stream>>>(a.partials, grid, D, a.O, d_w0, d_b0, d_w1,
-                                                                          d_b1, d_w2, d_b2);
+    // the six parameter gradients: the per-CTA partials summed over the CTAs, in CTA order, in fp64
+    const int O = a.O;
+    srf::part_sums(stream, a.partials, grid, (size_t)srf::nacc_of(D, O), srf::seg(d_w0, D * D), srf::seg(d_b0, D),
+                   srf::seg(d_w1, D * D), srf::seg(d_b1, D), srf::seg(d_w2, O * D), srf::seg(d_b2, O));
     e = cudaGetLastError();
     return e == cudaSuccess ? 0 : cuda_error("coarse_head backward launch", e);
 }

@@ -5,12 +5,14 @@
 //                       over all pixels of the depth maps (masked absolute error, count, threshold counts).  Each
 //                       thread accumulates in fp64 (counts in 64-bit integers), each CTA reduces in a fixed order and
 //                       writes one record of partials.
-// eval_finalize_kernel: sums the kGrid records in CTA order.  No atomics: two identical calls give identical bits.
+// part_sums_kernel    : sums the kGrid records in CTA order (fixed_sums.cuh).  No atomics: two identical calls give
+//                       identical bits.
 // video_frames_kernel : one thread per frame pixel, LaRa's rounding chain with every operation rounded on its own.
 #include <math.h>
 #include <string.h>
 
 #include "../../include/surfel_eval.h"
+#include "fixed_sums.cuh"
 #include "surfel_common.cuh"
 #include "surfel_kernels.h"
 
@@ -83,14 +85,6 @@ __global__ void __launch_bounds__(kThreads) eval_metrics_kernel(const MetricArgs
         for (int w = 0; w < kThreads / 32; ++w) s += s_w[w][threadIdx.x];
         a.part[(size_t)blockIdx.x * kSums + threadIdx.x] = s;
     }
-}
-
-__global__ void __launch_bounds__(32) eval_finalize_kernel(const double* part, int nout, double* out) {
-    const int k = threadIdx.x;
-    if (k >= nout) return;
-    double s = 0.0;
-    for (int b = 0; b < kGrid; ++b) s += part[(size_t)b * kSums + k];
-    out[k] = s;
 }
 
 struct FrameArgs {
@@ -188,7 +182,7 @@ extern "C" int srf_eval_metrics(srf_stream_t stream_, int V, int H, int W, int v
     a.out = out;
     const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     eval_metrics_kernel<<<kGrid, kThreads, 0, stream>>>(a);
-    eval_finalize_kernel<<<1, 32, 0, stream>>>(a.part, 3 + n_thresholds, out);
+    part_sums(stream, a.part, kGrid, kSums, seg(out, 3 + n_thresholds));
     const cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? 0 : cuda_error("eval_metrics launch", e);
 }

@@ -22,10 +22,11 @@
 //   fv_token_bwd_kernel   recomputes the token forward per tile and forms the modulation and LayerNorm vjp; the
 //                         parameter gradients of the tile are summed per CTA in a fixed order (per-CTA partials).
 //   fv_view_embed_kernel  per-slice sums of the view-embedding columns of dL/dout.
-//   fv_reduce_kernel      the partials summed over the CTAs in CTA order in fp64, as fine_head_reduce_kernel does.
+//   part_sums_kernel      the partials summed over the CTAs in CTA order in fp64 (fixed_sums.cuh).
 #include <string.h>
 
 #include "../../include/surfel_feat_volume.h"
+#include "fixed_sums.cuh"
 #include "sample_taps.cuh"
 #include "surfel_kernels.h"
 
@@ -180,12 +181,6 @@ __global__ void __launch_bounds__(kThreads) fv_token_fwd_kernel(Args a) {
         }
         __syncthreads();
     }
-}
-
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
 }
 
 __global__ void __launch_bounds__(kThreads, 1) fv_token_bwd_kernel(Args a) {
@@ -496,22 +491,6 @@ __global__ void __launch_bounds__(kThreads) fv_view_embed_kernel(Args a) {
     }
 }
 
-struct Seg { float* dst; int n; };
-
-// sums of the partials over the parts, in part order, in fp64; element e goes to the segment it falls in
-__global__ void fv_reduce_kernel(const float* parts, int nparts, int nacc, Seg s0, Seg s1, Seg s2, Seg s3) {
-    int e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= nacc) return;
-    double s = 0.0;
-    for (int p = 0; p < nparts; ++p) s += (double)parts[(size_t)p * nacc + e];
-    const Seg segs[4] = {s0, s1, s2, s3};
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        if (e < segs[k].n) { segs[k].dst[e] = (float)s; return; }
-        e -= segs[k].n;
-    }
-}
-
 struct WsLayout { size_t y, wts, cell, count, start, list, parts, ve_parts, total; };
 
 WsLayout ws_layout(int B, int V, int C, int h, int w, int R, int E) {
@@ -646,16 +625,13 @@ extern "C" int srf_feat_volume_backward(void* stream_, int B, int V, int C, int 
     if (n_group > 0) srf::fv_gather_kernel<true><<<ggrid, srf::kThreads, 0, stream>>>(a);
     else srf::fv_gather_kernel<false><<<ggrid, srf::kThreads, 0, stream>>>(a);
     srf::fv_token_bwd_kernel<<<dim3((unsigned)a.ntiles, BV), srf::kThreads, 0, stream>>>(a);
-    const int nacc = C * srf::kAcc;
-    srf::fv_reduce_kernel<<<(nacc + 255) / 256, 256, 0, stream>>>(
-        a.parts, (int)BV * a.ntiles, nacc, srf::Seg{d_mlp_w, 2 * C * srf::kSH}, srf::Seg{d_mlp_b, 2 * C},
-        srf::Seg{d_norm_w, C}, srf::Seg{d_norm_b, C});
+    srf::part_sums(stream, a.parts, (int)BV * a.ntiles, (size_t)C * srf::kAcc,
+                   srf::seg(d_mlp_w, 2 * C * srf::kSH), srf::seg(d_mlp_b, 2 * C), srf::seg(d_norm_w, C),
+                   srf::seg(d_norm_b, C));
     if (E > 0) {
         srf::fv_view_embed_kernel<<<dim3((unsigned)V, (unsigned)((E + 31) / 32), srf::kVeSlices), srf::kThreads, 0,
                                     stream>>>(a);
-        srf::fv_reduce_kernel<<<(V * E + 255) / 256, 256, 0, stream>>>(a.ve_parts, srf::kVeSlices, V * E,
-                                                                       srf::Seg{d_view_embed, V * E}, srf::Seg{nullptr, 0},
-                                                                       srf::Seg{nullptr, 0}, srf::Seg{nullptr, 0});
+        srf::part_sums(stream, a.ve_parts, srf::kVeSlices, (size_t)V * E, srf::seg(d_view_embed, V * E));
     }
     e = cudaGetLastError();
     return e == cudaSuccess ? 0 : cuda_error("feat_volume backward launch", e);

@@ -17,6 +17,7 @@
 // Wq, Wk, Wv, Wo and W1 follow from dA and dW1c by the chain rule through the compositions, in fp64.  The voxel-row
 // gradient of the gather mode is a gather over the per-point rows (idx is strictly increasing).  No atomics.
 #include "../../include/surfel_fine_head.h"
+#include "fixed_sums.cuh"
 #include "surfel_kernels.h"
 
 namespace srf {
@@ -437,15 +438,6 @@ __global__ void __launch_bounds__(kThreads, 1) fine_head_bwd_kernel(Args a) {
     for (int e = tid; e < l.nacc; e += kThreads) part[e] = acc[e];
 }
 
-// sums of the per-CTA partials over the CTAs, in CTA order, in fp64
-__global__ void fine_head_reduce_kernel(const float* partials, int nparts, int nacc, double* totals) {
-    const int e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= nacc) return;
-    double s = 0.0;
-    for (int b = 0; b < nparts; ++b) s += (double)partials[(size_t)b * nacc + e];
-    totals[e] = s;
-}
-
 struct GradArgs {
     int D, S, Sp;
     const double* tot;               // reduced accumulators (Layout offsets)
@@ -666,7 +658,7 @@ extern "C" int srf_fine_head_backward(void* stream_, int n, int V, int D, int sh
         if ((e = cudaGetLastError()) != cudaSuccess) return cuda_error("fine_head_bwd launch", e);
     }
     double* tot = reinterpret_cast<double*>(ws + w.tot);
-    srf::fine_head_reduce_kernel<<<(l.nacc + 255) / 256, 256, 0, stream>>>(a.partials, grid, l.nacc, tot);
+    srf::part_sums(stream, a.partials, grid, (size_t)l.nacc, srf::seg(tot, l.nacc));   // in CTA order, in fp64
     srf::GradArgs g = {D, sh_dim, a.Sp, tot, reinterpret_cast<double*>(ws + w.B), reinterpret_cast<double*>(ws + w.dB),
                        wq, wk, wv, wo, w1, d_norm_w, d_norm_b, d_wq, d_wk, d_wv, d_wo, d_w1, d_b1, d_w2, d_b2};
     const int n0 = D + 64 + sh_dim + sh_dim * 64 + D * D + D * 8 + D * 64, n1 = 64 * D + D * D + D * 8;

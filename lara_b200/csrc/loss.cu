@@ -16,6 +16,7 @@
 #include <string.h>
 
 #include "../../include/surfel_rasterizer.h"
+#include "fixed_sums.cuh"
 #include "surfel_common.cuh"
 #include "surfel_kernels.h"
 
@@ -85,12 +86,9 @@ static size_t loss_det_blocks(size_t total) { return min((size_t)1024, (total + 
 
 // deterministic path: the per-block partials of loss_sums_kernel<true> summed in a fixed order, warp w for term w
 __global__ void __launch_bounds__(96) loss_sums_finalize_kernel(const double* partials, int nblocks, double* sums) {
-    const int lane = threadIdx.x & 31, term = threadIdx.x >> 5;
-    double t = 0.0;
-    for (int b = lane; b < nblocks; b += 32) t += partials[3 * b + term];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-    if (lane == 0) sums[term] = t;
+    const int term = threadIdx.x >> 5;
+    const double t = warp_strided_sum(partials + term, nblocks, 3);
+    if ((threadIdx.x & 31) == 0) sums[term] = t;
 }
 
 __global__ void __launch_bounds__(256) loss_grads_kernel(LossArgs a) {

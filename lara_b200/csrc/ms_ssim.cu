@@ -9,8 +9,9 @@
 // ms_ssim_fwd_kernel   : one CTA per 32x16 tile of one plane: stages X, Y with the 10-pixel halo, filters the five
 //                        quantities (H pass into shared memory, W pass in registers), writes one partial sum per CTA
 //                        and the 2x2 average pool of the pixels it owns (the next level's input).
-// ms_ssim_finalize_kernel: reduces the partials in a fixed order in fp64, applies relu / pow / prod / mean and writes
-//                        the result and dvalue/dm_l per plane, already divided by the level's valid-pixel count.
+// ms_ssim_finalize_kernel: reduces the partials in a fixed order in fp64 (fixed_sums.cuh's warp_strided_sum), applies
+//                        relu / pow / prod / mean and writes the result and dvalue/dm_l per plane, already divided by
+//                        the level's valid-pixel count.
 // ms_ssim_bwd_kernel   : levels 4 -> 0, gather form, one thread per input pixel: recomputes the filtered maps on the
 //                        outputs whose windows cover the tile (20-pixel input halo), forms the coefficient maps
 //                        A = dm/dmu_x, B = dm/dG(XX), C = dm/dG(XY) (times the level's coefficient), filters them back
@@ -18,11 +19,13 @@
 // No atomics anywhere: two identical calls give identical bits.  The level-0 image is read (and its gradient
 // written) through MsAddr, so a channel-last tensor and V planar views side by side are read in place.
 // The C entries srf_ms_ssim_* (include/surfel_rasterizer.h) are defined here, and so are srf_ssim_*: single-scale
-// SSIM, the kLast level alone on the caller's image, with ssim_finalize_kernel in place of the pyramid's finalize.
+// SSIM, the same code with a one-level pyramid (its only level is the kLast level, on the caller's image).  The
+// level count changes only the size rule and the finalize's value / coefficient rule.
 #include <math.h>
 #include <string.h>
 
 #include "../../include/surfel_rasterizer.h"
+#include "fixed_sums.cuh"
 #include "surfel_common.cuh"
 #include "surfel_kernels.h"
 
@@ -47,9 +50,10 @@ namespace {
 constexpr int kTW = 32, kTH = 16;          // tile of output pixels (forward) / input pixels (backward)
 constexpr int kR = 10;                     // window size - 1
 constexpr int kThreads = 256;
-constexpr int kLevels = 5;
+constexpr int kLevels = 5;                 // MS-SSIM's; single-scale SSIM has 1
 
 struct Layout {
+    int levels;
     int h[kLevels], w[kLevels];
     int px[kLevels], py[kLevels];          // pooling padding from level l to l + 1 (0 at the last level)
     int ntx[kLevels], nty[kLevels];        // forward tile grid
@@ -59,15 +63,16 @@ struct Layout {
     size_t o_pyr, o_gpyr, o_part, o_mean, o_val, o_coef, total;   // byte offsets in the workspace
 };
 
-Layout make_layout(int B, int C, int H, int W) {
+Layout make_layout(int levels, int B, int C, int H, int W) {
     Layout L;
+    L.levels = levels;
     const size_t planes = (size_t)B * C;
     size_t np = 0, ng = 0, nq = 0;
-    for (int l = 0; l < kLevels; ++l) {
+    for (int l = 0; l < levels; ++l) {
         L.h[l] = l ? (L.h[l - 1] + 1) / 2 : H;      // avg_pool2d(2, padding = s % 2): floor((s + 2 (s % 2)) / 2)
         L.w[l] = l ? (L.w[l - 1] + 1) / 2 : W;
-        L.px[l] = l < kLevels - 1 ? L.w[l] % 2 : 0;
-        L.py[l] = l < kLevels - 1 ? L.h[l] % 2 : 0;
+        L.px[l] = l < levels - 1 ? L.w[l] % 2 : 0;
+        L.py[l] = l < levels - 1 ? L.h[l] % 2 : 0;
         L.ntx[l] = (L.w[l] + L.px[l] + kTW - 1) / kTW;
         L.nty[l] = (L.h[l] + L.py[l] + kTH - 1) / kTH;
         const size_t n = planes * L.h[l] * L.w[l];
@@ -80,9 +85,9 @@ Layout make_layout(int B, int C, int H, int W) {
     L.o_pyr = o;  o = align_up(o + np * sizeof(float));
     L.o_gpyr = o; o = align_up(o + ng * sizeof(float));
     L.o_part = o; o = align_up(o + nq * sizeof(double));
-    L.o_mean = o; o = align_up(o + kLevels * planes * sizeof(double));
+    L.o_mean = o; o = align_up(o + levels * planes * sizeof(double));
     L.o_val = o;  o = align_up(o + planes * sizeof(double));
-    L.o_coef = o; o = align_up(o + kLevels * planes * sizeof(float));
+    L.o_coef = o; o = align_up(o + levels * planes * sizeof(float));
     L.total = o;
     return L;
 }
@@ -106,13 +111,15 @@ struct LevelArgs {
 
 struct FinalArgs {
     int B, C, planes, size_average;
+    int levels;
+    int nonnegative;             // one level: relu the mean (MS-SSIM always does)
     int ntiles[kLevels];
     size_t part_off[kLevels];
     double count[kLevels];       // valid output pixels per plane, (h - 10)(w - 10)
     const double* part;
-    double* mean;                // [5][planes]
+    double* mean;                // [levels][planes]
     double* val;                 // [planes]
-    float* coef;                 // [5][planes]
+    float* coef;                 // [levels][planes]
     float* out;                  // [1] or [B]
 };
 
@@ -212,20 +219,24 @@ __global__ void __launch_bounds__(kThreads) ms_ssim_fwd_kernel(const LevelArgs a
 
 __global__ void __launch_bounds__(kThreads) ms_ssim_finalize_kernel(const FinalArgs f) {
     const double kWeights[kLevels] = {0.0448, 0.2856, 0.3001, 0.2363, 0.1333};
-    const int lane = threadIdx.x & 31, P = f.planes;
-    // one warp per (level, plane): lane-strided sums, then a fixed butterfly
-    for (int j = threadIdx.x >> 5; j < kLevels * P; j += kThreads / 32) {
+    const int P = f.planes;
+    // one warp per (level, plane)
+    for (int j = threadIdx.x >> 5; j < f.levels * P; j += kThreads / 32) {
         const int l = j / P, p = j - l * P, n = f.ntiles[l];
-        const double* src = f.part + f.part_off[l] + (size_t)p * n;
-        double s = 0.0;
-        for (int i = lane; i < n; i += 32) s += src[i];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-        if (lane == 0) f.mean[j] = s / f.count[l];
+        const double s = warp_strided_sum(f.part + f.part_off[l] + (size_t)p * n, n, 1);
+        if ((threadIdx.x & 31) == 0) f.mean[j] = s / f.count[l];
     }
     __syncthreads();
     const double scale = 1.0 / (f.size_average ? (double)P : (double)f.C);
     for (int p = threadIdx.x; p < P; p += kThreads) {
+        if (f.levels == 1) {
+            // SSIM: the mean, optionally relu'd; relu's backward is a select, so no gradient through a mean <= 0
+            const double m = f.mean[p];
+            const bool pass = !f.nonnegative || m > 0.0;
+            f.val[p] = pass ? m : 0.0;
+            f.coef[p] = pass ? (float)(scale / f.count[0]) : 0.f;
+            continue;
+        }
         double m[kLevels];
         bool pos = true;
 #pragma unroll
@@ -243,44 +254,6 @@ __global__ void __launch_bounds__(kThreads) ms_ssim_finalize_kernel(const FinalA
 #pragma unroll
         for (int l = 0; l < kLevels; ++l)
             f.coef[l * P + p] = pos ? (float)(kWeights[l] * v / m[l] * scale / f.count[l]) : 0.f;
-    }
-    __syncthreads();
-    const int nout = f.size_average ? 1 : f.B;
-    for (int o = threadIdx.x; o < nout; o += kThreads) {
-        const int p0 = f.size_average ? 0 : o * f.C, np = f.size_average ? P : f.C;
-        double s = 0.0;
-        for (int p = 0; p < np; ++p) s += f.val[p0 + p];
-        f.out[o] = (float)(s / np);
-    }
-}
-
-// Single-scale SSIM (srf_ssim_*): the per-plane mean of the level-0 ssim_map from ms_ssim_fwd_kernel<true>'s partials,
-// summed in the same fixed order, optionally relu'd; coef = dvalue/dmean * scale / count for ms_ssim_bwd_kernel<true>.
-struct SsimFinalArgs {
-    int B, C, planes, ntiles, size_average, nonnegative;
-    double count;                // valid output pixels per plane, (H - 10)(W - 10)
-    const double* part;          // [planes][ntiles]
-    double* val;                 // [planes]
-    float* coef;                 // [planes]
-    float* out;                  // [1] or [B]
-};
-
-__global__ void __launch_bounds__(kThreads) ssim_finalize_kernel(const SsimFinalArgs f) {
-    const int lane = threadIdx.x & 31, P = f.planes;
-    const double scale = 1.0 / (f.size_average ? (double)P : (double)f.C);
-    for (int p = threadIdx.x >> 5; p < P; p += kThreads / 32) {
-        const double* src = f.part + (size_t)p * f.ntiles;
-        double s = 0.0;
-        for (int i = lane; i < f.ntiles; i += 32) s += src[i];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-        if (lane == 0) {
-            const double m = s / f.count;
-            // relu's backward is a select: no gradient through a plane whose mean is <= 0
-            const bool pass = !f.nonnegative || m > 0.0;
-            f.val[p] = pass ? m : 0.0;
-            f.coef[p] = pass ? (float)(scale / f.count) : 0.f;
-        }
     }
     __syncthreads();
     const int nout = f.size_average ? 1 : f.B;
@@ -449,36 +422,11 @@ LevelArgs level_args(const MsSsimArgs& m, const Layout& L, char* ws, int l) {
         a.x = pyr + L.pyr[l]; a.y = a.x + n;
         a.ax = a.ay = planar(m.C, L.h[l], L.w[l]);
     }
-    if (l + 1 < kLevels) {
+    if (l + 1 < L.levels) {
         a.nh = L.h[l + 1]; a.nw = L.w[l + 1];
         a.nx = pyr + L.pyr[l + 1];
         a.ny = a.nx + (size_t)m.B * m.C * a.nh * a.nw;
     }
-    return a;
-}
-
-// single-scale SSIM: one level, no pyramid; the forward's tile grid, then per-CTA partials, values and coefficients
-struct SsimLayout { int ntx, nty; size_t o_part, o_val, o_coef, total; };
-
-SsimLayout make_ssim_layout(int B, int C, int H, int W) {
-    SsimLayout L;
-    const size_t planes = (size_t)B * C;
-    L.ntx = (W + kTW - 1) / kTW;
-    L.nty = (H + kTH - 1) / kTH;
-    size_t o = 0;
-    L.o_part = o; o = align_up(o + planes * L.ntx * L.nty * sizeof(double));
-    L.o_val = o;  o = align_up(o + planes * sizeof(double));
-    L.o_coef = o; o = align_up(o + planes * sizeof(float));
-    L.total = o;
-    return L;
-}
-
-LevelArgs ssim_level_args(const MsSsimArgs& m) {
-    LevelArgs a;
-    memset(&a, 0, sizeof(a));
-    a.C = m.C; a.H = m.H; a.W = m.W;
-    level_constants(a, m.data_range);
-    a.x = m.x; a.y = m.y; a.ax = m.ax; a.ay = m.ay;
     return a;
 }
 
@@ -489,10 +437,15 @@ LevelArgs ssim_level_args(const MsSsimArgs& m) {
 using srf::cuda_error;
 using srf::set_error;
 
-static int ms_ssim_sizes(const char* fn, int B, int C, int H, int W) {
+
+// min(H, W) > 10 * 2^(levels - 1): every level of the pyramid keeps at least one valid window
+static int ms_ssim_sizes(const char* fn, int levels, int B, int C, int H, int W) {
     if (B <= 0 || C <= 0 || H <= 0 || W <= 0) return set_error("%s: bad sizes (B=%d, C=%d, H=%d, W=%d)", fn, B, C, H, W);
-    if ((H < W ? H : W) <= 160)
-        return set_error("%s: Image size should be larger than 160 due to the 4 downsamplings in ms-ssim (H=%d, W=%d)", fn, H, W);
+    if ((H < W ? H : W) <= srf::kR << (levels - 1)) {
+        if (levels > 1)
+            return set_error("%s: Image size should be larger than 160 due to the 4 downsamplings in ms-ssim (H=%d, W=%d)", fn, H, W);
+        return set_error("%s: H and W must be at least the window size 11 (H=%d, W=%d)", fn, H, W);
+    }
     if ((long long)B * C > 65535) return set_error("%s: B*C=%lld planes exceeds 65535", fn, (long long)B * C);
     return 0;
 }
@@ -505,11 +458,11 @@ static int ms_ssim_addr(const char* fn, const char* what, const float* p, const 
     return 0;
 }
 
-static int ms_ssim_prepare(const char* fn, int B, int C, int H, int W, const float* x, const srf_ms_ssim_addr* x_addr,
-                           const float* y, const srf_ms_ssim_addr* y_addr, float data_range, int size_average,
-                           void* workspace, srf::MsSsimArgs* a) {
+static int ms_ssim_prepare(const char* fn, int levels, int B, int C, int H, int W, const float* x,
+                           const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
+                           float data_range, int size_average, void* workspace, srf::MsSsimArgs* a) {
     memset(a, 0, sizeof(*a));
-    if (ms_ssim_sizes(fn, B, C, H, W)) return 1;
+    if (ms_ssim_sizes(fn, levels, B, C, H, W)) return 1;
     if (ms_ssim_addr(fn, "x", x, x_addr, &a->ax) || ms_ssim_addr(fn, "y", y, y_addr, &a->ay)) return 1;
     if (!(data_range > 0.f) || !(data_range < 3.0e38f)) return set_error("%s: data_range must be positive and finite", fn);
     if (!workspace || srf::misaligned(workspace)) return set_error("%s: workspace must be 256-byte aligned", fn);
@@ -518,53 +471,40 @@ static int ms_ssim_prepare(const char* fn, int B, int C, int H, int W, const flo
     return 0;
 }
 
-extern "C" int srf_ms_ssim_workspace_bytes(int B, int C, int H, int W, size_t* bytes) {
-    if (ms_ssim_sizes("srf_ms_ssim_workspace_bytes", B, C, H, W)) return 1;
-    if (!bytes) return set_error("srf_ms_ssim_workspace_bytes: null pointer");
-    *bytes = srf::make_layout(B, C, H, W).total;
+static int ms_ssim_workspace_bytes(const char* fn, int levels, int B, int C, int H, int W, size_t* bytes) {
+    if (ms_ssim_sizes(fn, levels, B, C, H, W)) return 1;
+    if (!bytes) return set_error("%s: null pointer", fn);
+    *bytes = srf::make_layout(levels, B, C, H, W).total;
     return 0;
 }
 
-extern "C" int srf_ms_ssim_workspace_layout(int B, int C, int H, int W, size_t regions[7], size_t levels[15],
-                                            int dims[30]) {
-    if (ms_ssim_sizes("srf_ms_ssim_workspace_layout", B, C, H, W)) return 1;
-    if (!regions || !levels || !dims) return set_error("srf_ms_ssim_workspace_layout: null pointer");
-    const srf::Layout L = srf::make_layout(B, C, H, W);
-    const size_t r[7] = {L.o_pyr, L.o_gpyr, L.o_part, L.o_mean, L.o_val, L.o_coef, L.total};
-    for (int i = 0; i < 7; ++i) regions[i] = r[i];
-    for (int l = 0; l < srf::kLevels; ++l) {
-        levels[l] = L.pyr[l]; levels[srf::kLevels + l] = L.gpyr[l]; levels[2 * srf::kLevels + l] = L.part[l];
-        const int d[6] = {L.h[l], L.w[l], L.px[l], L.py[l], L.ntx[l], L.nty[l]};
-        for (int i = 0; i < 6; ++i) dims[i * srf::kLevels + l] = d[i];
-    }
-    return 0;
-}
-
-extern "C" int srf_ms_ssim_forward(srf_stream_t stream_, int B, int C, int H, int W, const float* x,
-                                   const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
-                                   float data_range, int size_average, void* workspace, float* out) {
+// the pyramid's levels 0 .. levels - 1, then the finalize
+static int ms_ssim_forward(const char* fn, int levels, int nonnegative, srf_stream_t stream_, int B, int C, int H,
+                           int W, const float* x, const srf_ms_ssim_addr* x_addr, const float* y,
+                           const srf_ms_ssim_addr* y_addr, float data_range, int size_average, void* workspace,
+                           float* out) {
     using namespace srf;
-    const char* fn = "srf_ms_ssim_forward";
     MsSsimArgs m;
-    if (ms_ssim_prepare(fn, B, C, H, W, x, x_addr, y, y_addr, data_range, size_average, workspace, &m)) return 1;
+    if (ms_ssim_prepare(fn, levels, B, C, H, W, x, x_addr, y, y_addr, data_range, size_average, workspace, &m)) return 1;
     if (!out) return set_error("%s: null output pointer", fn);
     m.out = out;
     const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    const Layout L = make_layout(B, C, H, W);
+    const Layout L = make_layout(levels, B, C, H, W);
     char* ws = static_cast<char*>(workspace);
     const int planes = B * C;
-    for (int l = 0; l < kLevels; ++l) {
+    for (int l = 0; l < levels; ++l) {
         LevelArgs a = level_args(m, L, ws, l);
         a.ntx = L.ntx[l];
         a.part = reinterpret_cast<double*>(ws + L.o_part) + L.part[l];
         const dim3 grid((unsigned)(L.ntx[l] * L.nty[l]), (unsigned)planes);
-        if (l + 1 < kLevels) ms_ssim_fwd_kernel<false><<<grid, kThreads, 0, stream>>>(a);
+        if (l + 1 < levels) ms_ssim_fwd_kernel<false><<<grid, kThreads, 0, stream>>>(a);
         else ms_ssim_fwd_kernel<true><<<grid, kThreads, 0, stream>>>(a);
     }
     FinalArgs f;
     memset(&f, 0, sizeof(f));
     f.B = B; f.C = C; f.planes = planes; f.size_average = m.size_average;
-    for (int l = 0; l < kLevels; ++l) {
+    f.levels = levels; f.nonnegative = nonnegative ? 1 : 0;
+    for (int l = 0; l < levels; ++l) {
         f.ntiles[l] = L.ntx[l] * L.nty[l];
         f.part_off[l] = L.part[l];
         f.count[l] = (double)(L.h[l] - kR) * (double)(L.w[l] - kR);
@@ -576,123 +516,95 @@ extern "C" int srf_ms_ssim_forward(srf_stream_t stream_, int B, int C, int H, in
     f.out = out;
     ms_ssim_finalize_kernel<<<1, kThreads, 0, stream>>>(f);
     const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : cuda_error("ms_ssim_fwd launch", e);
+    return e == cudaSuccess ? 0 : cuda_error(levels > 1 ? "ms_ssim_fwd launch" : "ssim_fwd launch", e);
 }
 
-extern "C" int srf_ms_ssim_backward(srf_stream_t stream_, int B, int C, int H, int W, const float* x,
-                                    const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
-                                    float data_range, int size_average, void* workspace, const float* upstream,
-                                    float* dx, const srf_ms_ssim_addr* dx_addr) {
+// levels - 1 .. 0 with the coefficients the forward left in the workspace
+static int ms_ssim_backward(const char* fn, int levels, srf_stream_t stream_, int B, int C, int H, int W,
+                            const float* x, const srf_ms_ssim_addr* x_addr, const float* y,
+                            const srf_ms_ssim_addr* y_addr, float data_range, int size_average, void* workspace,
+                            const float* upstream, float* dx, const srf_ms_ssim_addr* dx_addr) {
     using namespace srf;
-    const char* fn = "srf_ms_ssim_backward";
     MsSsimArgs m;
-    if (ms_ssim_prepare(fn, B, C, H, W, x, x_addr, y, y_addr, data_range, size_average, workspace, &m)) return 1;
+    if (ms_ssim_prepare(fn, levels, B, C, H, W, x, x_addr, y, y_addr, data_range, size_average, workspace, &m)) return 1;
     if (!upstream) return set_error("%s: null upstream gradient", fn);
     if (ms_ssim_addr(fn, "dx", dx, dx_addr, &m.ag)) return 1;
     m.gout = upstream; m.gx = dx;
     const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    const Layout L = make_layout(B, C, H, W);
+    const Layout L = make_layout(levels, B, C, H, W);
     char* ws = static_cast<char*>(workspace);
     const int planes = B * C;
     float* coef = reinterpret_cast<float*>(ws + L.o_coef);
     float* gpyr = reinterpret_cast<float*>(ws + L.o_gpyr);
-    for (int l = kLevels - 1; l >= 0; --l) {
+    for (int l = levels - 1; l >= 0; --l) {
         LevelArgs a = level_args(m, L, ws, l);
         a.ntx = (L.w[l] + kTW - 1) / kTW;
         const int nty = (L.h[l] + kTH - 1) / kTH;
         a.coef = coef + (size_t)l * planes;
         a.gout = m.gout; a.gout_per_b = m.size_average ? 0 : 1;
-        if (l + 1 < kLevels) a.gnext = gpyr + L.gpyr[l + 1];
+        if (l + 1 < levels) a.gnext = gpyr + L.gpyr[l + 1];
         if (l == 0) { a.gx = m.gx; a.ag = m.ag; }
         else { a.gx = gpyr + L.gpyr[l]; a.ag = planar(m.C, L.h[l], L.w[l]); }
         const dim3 grid((unsigned)(a.ntx * nty), (unsigned)planes);
-        if (l + 1 < kLevels) ms_ssim_bwd_kernel<false><<<grid, kThreads, 0, stream>>>(a);
+        if (l + 1 < levels) ms_ssim_bwd_kernel<false><<<grid, kThreads, 0, stream>>>(a);
         else ms_ssim_bwd_kernel<true><<<grid, kThreads, 0, stream>>>(a);
     }
     const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : cuda_error("ms_ssim_bwd launch", e);
+    return e == cudaSuccess ? 0 : cuda_error(levels > 1 ? "ms_ssim_bwd launch" : "ssim_bwd launch", e);
 }
 
-// ---- single-scale SSIM (pytorch-msssim 1.0.0 ssim): level 0 of the MS-SSIM kernels, kLast form ----
+extern "C" int srf_ms_ssim_workspace_bytes(int B, int C, int H, int W, size_t* bytes) {
+    return ms_ssim_workspace_bytes("srf_ms_ssim_workspace_bytes", srf::kLevels, B, C, H, W, bytes);
+}
 
-static int ssim_sizes(const char* fn, int B, int C, int H, int W) {
-    if (B <= 0 || C <= 0 || H <= 0 || W <= 0) return set_error("%s: bad sizes (B=%d, C=%d, H=%d, W=%d)", fn, B, C, H, W);
-    if (H < 11 || W < 11) return set_error("%s: H and W must be at least the window size 11 (H=%d, W=%d)", fn, H, W);
-    if ((long long)B * C > 65535) return set_error("%s: B*C=%lld planes exceeds 65535", fn, (long long)B * C);
+extern "C" int srf_ms_ssim_workspace_layout(int B, int C, int H, int W, size_t regions[7], size_t levels[15],
+                                            int dims[30]) {
+    if (ms_ssim_sizes("srf_ms_ssim_workspace_layout", srf::kLevels, B, C, H, W)) return 1;
+    if (!regions || !levels || !dims) return set_error("srf_ms_ssim_workspace_layout: null pointer");
+    const srf::Layout L = srf::make_layout(srf::kLevels, B, C, H, W);
+    const size_t r[7] = {L.o_pyr, L.o_gpyr, L.o_part, L.o_mean, L.o_val, L.o_coef, L.total};
+    for (int i = 0; i < 7; ++i) regions[i] = r[i];
+    for (int l = 0; l < srf::kLevels; ++l) {
+        levels[l] = L.pyr[l]; levels[srf::kLevels + l] = L.gpyr[l]; levels[2 * srf::kLevels + l] = L.part[l];
+        const int d[6] = {L.h[l], L.w[l], L.px[l], L.py[l], L.ntx[l], L.nty[l]};
+        for (int i = 0; i < 6; ++i) dims[i * srf::kLevels + l] = d[i];
+    }
     return 0;
 }
 
-static int ssim_prepare(const char* fn, int B, int C, int H, int W, const float* x, const srf_ms_ssim_addr* x_addr,
-                        const float* y, const srf_ms_ssim_addr* y_addr, float data_range, int size_average,
-                        void* workspace, srf::MsSsimArgs* a) {
-    memset(a, 0, sizeof(*a));
-    if (ssim_sizes(fn, B, C, H, W)) return 1;
-    if (ms_ssim_addr(fn, "x", x, x_addr, &a->ax) || ms_ssim_addr(fn, "y", y, y_addr, &a->ay)) return 1;
-    if (!(data_range > 0.f) || !(data_range < 3.0e38f)) return set_error("%s: data_range must be positive and finite", fn);
-    if (!workspace || srf::misaligned(workspace)) return set_error("%s: workspace must be 256-byte aligned", fn);
-    a->B = B; a->C = C; a->H = H; a->W = W; a->size_average = size_average ? 1 : 0; a->data_range = data_range;
-    a->x = x; a->y = y; a->workspace = workspace;
-    return 0;
+extern "C" int srf_ms_ssim_forward(srf_stream_t stream, int B, int C, int H, int W, const float* x,
+                                   const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
+                                   float data_range, int size_average, void* workspace, float* out) {
+    return ms_ssim_forward("srf_ms_ssim_forward", srf::kLevels, 1, stream, B, C, H, W, x, x_addr, y, y_addr,
+                           data_range, size_average, workspace, out);
 }
+
+extern "C" int srf_ms_ssim_backward(srf_stream_t stream, int B, int C, int H, int W, const float* x,
+                                    const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
+                                    float data_range, int size_average, void* workspace, const float* upstream,
+                                    float* dx, const srf_ms_ssim_addr* dx_addr) {
+    return ms_ssim_backward("srf_ms_ssim_backward", srf::kLevels, stream, B, C, H, W, x, x_addr, y, y_addr, data_range,
+                            size_average, workspace, upstream, dx, dx_addr);
+}
+
+// ---- single-scale SSIM (pytorch-msssim 1.0.0 ssim): the one-level pyramid ----
 
 extern "C" int srf_ssim_workspace_bytes(int B, int C, int H, int W, size_t* bytes) {
-    if (ssim_sizes("srf_ssim_workspace_bytes", B, C, H, W)) return 1;
-    if (!bytes) return set_error("srf_ssim_workspace_bytes: null pointer");
-    *bytes = srf::make_ssim_layout(B, C, H, W).total;
-    return 0;
+    return ms_ssim_workspace_bytes("srf_ssim_workspace_bytes", 1, B, C, H, W, bytes);
 }
 
-extern "C" int srf_ssim_forward(srf_stream_t stream_, int B, int C, int H, int W, const float* x,
+extern "C" int srf_ssim_forward(srf_stream_t stream, int B, int C, int H, int W, const float* x,
                                 const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
                                 float data_range, int size_average, int nonnegative_ssim, void* workspace, float* out) {
-    using namespace srf;
-    const char* fn = "srf_ssim_forward";
-    MsSsimArgs m;
-    if (ssim_prepare(fn, B, C, H, W, x, x_addr, y, y_addr, data_range, size_average, workspace, &m)) return 1;
-    if (!out) return set_error("%s: null output pointer", fn);
-    const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    const SsimLayout L = make_ssim_layout(B, C, H, W);
-    char* ws = static_cast<char*>(workspace);
-    const int planes = B * C;
-    LevelArgs a = ssim_level_args(m);
-    a.ntx = L.ntx;
-    a.part = reinterpret_cast<double*>(ws + L.o_part);
-    ms_ssim_fwd_kernel<true><<<dim3((unsigned)(L.ntx * L.nty), (unsigned)planes), kThreads, 0, stream>>>(a);
-    SsimFinalArgs f;
-    memset(&f, 0, sizeof(f));
-    f.B = B; f.C = C; f.planes = planes; f.ntiles = L.ntx * L.nty;
-    f.size_average = m.size_average; f.nonnegative = nonnegative_ssim ? 1 : 0;
-    f.count = (double)(H - kR) * (double)(W - kR);
-    f.part = reinterpret_cast<const double*>(ws + L.o_part);
-    f.val = reinterpret_cast<double*>(ws + L.o_val);
-    f.coef = reinterpret_cast<float*>(ws + L.o_coef);
-    f.out = out;
-    ssim_finalize_kernel<<<1, kThreads, 0, stream>>>(f);
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : cuda_error("ssim_fwd launch", e);
+    return ms_ssim_forward("srf_ssim_forward", 1, nonnegative_ssim, stream, B, C, H, W, x, x_addr, y, y_addr,
+                           data_range, size_average, workspace, out);
 }
 
-extern "C" int srf_ssim_backward(srf_stream_t stream_, int B, int C, int H, int W, const float* x,
+extern "C" int srf_ssim_backward(srf_stream_t stream, int B, int C, int H, int W, const float* x,
                                  const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
                                  float data_range, int size_average, int nonnegative_ssim, void* workspace,
                                  const float* upstream, float* dx, const srf_ms_ssim_addr* dx_addr) {
-    using namespace srf;
-    const char* fn = "srf_ssim_backward";
     (void)nonnegative_ssim;      // the forward folded the relu into the coefficients it left in the workspace
-    MsSsimArgs m;
-    if (ssim_prepare(fn, B, C, H, W, x, x_addr, y, y_addr, data_range, size_average, workspace, &m)) return 1;
-    if (!upstream) return set_error("%s: null upstream gradient", fn);
-    if (ms_ssim_addr(fn, "dx", dx, dx_addr, &m.ag)) return 1;
-    const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    const SsimLayout L = make_ssim_layout(B, C, H, W);
-    char* ws = static_cast<char*>(workspace);
-    LevelArgs a = ssim_level_args(m);
-    a.ntx = (W + kTW - 1) / kTW;
-    a.coef = reinterpret_cast<const float*>(ws + L.o_coef);
-    a.gout = upstream; a.gout_per_b = m.size_average ? 0 : 1;
-    a.gx = dx; a.ag = m.ag;
-    const dim3 grid((unsigned)(a.ntx * ((H + kTH - 1) / kTH)), (unsigned)(B * C));
-    ms_ssim_bwd_kernel<true><<<grid, kThreads, 0, stream>>>(a);
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : cuda_error("ssim_bwd launch", e);
+    return ms_ssim_backward("srf_ssim_backward", 1, stream, B, C, H, W, x, x_addr, y, y_addr, data_range,
+                            size_average, workspace, upstream, dx, dx_addr);
 }

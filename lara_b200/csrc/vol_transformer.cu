@@ -14,11 +14,12 @@
 //   ln_fwd_kernel   y = a + b, the mean, the centred variance (two passes over the registers), n = LN(y).
 //   ln_bwd_kernel   a CTA per block of 64 rows: recomputes the statistics from y, writes dL/da = dL/dy + the vjp,
 //                   and the block's dgamma / dbeta partials, its warps added in warp order.
-//   ln_reduce_kernel  the partials summed over the blocks in block order in fp64, as fv_reduce_kernel does.
+//   part_sums_kernel  the partials summed over the blocks in block order in fp64 (fixed_sums.cuh).
 #include <math.h>
 #include <string.h>
 
 #include "../../include/surfel_vol_transformer.h"
+#include "fixed_sums.cuh"
 #include "surfel_kernels.h"
 
 namespace srf {
@@ -171,12 +172,6 @@ struct LnArgs {
     float *y, *n, *ga, *parts;
 };
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
 // mean and 1 / sqrt(var + eps) of the lane's nj values of a row of C
 __device__ __forceinline__ void ln_stats(const float* y, int nj, int C, float eps, float& mean, float& rstd) {
     float s = 0.0f;
@@ -264,15 +259,6 @@ __global__ void __launch_bounds__(kLnWarps * 32) ln_bwd_kernel(LnArgs a) {
     }
     float* part = a.parts + (size_t)blockIdx.x * 2 * C;
     for (int e = threadIdx.x; e < 2 * C; e += kLnWarps * 32) part[e] = acc_s[e / C][e % C];
-}
-
-__global__ void ln_reduce_kernel(const float* parts, int nparts, int C, float* dgamma, float* dbeta) {
-    const int e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= 2 * C) return;
-    double s = 0.0;
-    for (int p = 0; p < nparts; ++p) s += (double)parts[(size_t)p * 2 * C + e];
-    if (e < C) dgamma[e] = (float)s;
-    else dbeta[e - C] = (float)s;
 }
 
 bool misaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
@@ -402,8 +388,8 @@ extern "C" int srf_add_layernorm_backward(void* stream_, int rows, int C, float 
         la.ga = dL_da; la.parts = static_cast<float*>(workspace);
         srf::ln_bwd_kernel<<<(unsigned)nparts, srf::kLnWarps * 32, 0, stream>>>(la);
     }
-    srf::ln_reduce_kernel<<<(2 * C + 255) / 256, 256, 0, stream>>>(static_cast<const float*>(workspace), nparts, C,
-                                                                     d_gamma, d_beta);
+    srf::part_sums(stream, static_cast<const float*>(workspace), nparts, 2 * (size_t)C, srf::seg(d_gamma, C),
+                   srf::seg(d_beta, C));
     const cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? 0 : cuda_error("add_layernorm backward launch", e);
 }

@@ -21,7 +21,8 @@ import torch
 
 from . import _lib
 
-_MIN_SIDE = (11 - 1) * 2 ** 4
+_MS_LEVELS = 5
+_MIN_SIDE = (11 - 1) * 2 ** (_MS_LEVELS - 1)
 
 
 def _addr(t: torch.Tensor, views: bool) -> _lib.MsSsimAddr:
@@ -54,33 +55,54 @@ def check_inputs(fn: str, X: torch.Tensor, Y: torch.Tensor) -> None:
         raise RuntimeError(f"{fn}: Y requires grad, but the fused MS-SSIM gives no gradient for the target; detach it")
 
 
-class _MsSsim(torch.autograd.Function):
+def _entry(levels: int, what: str, nonnegative_ssim: bool):
+    """The C entry srf_ssim_<what> (one level) or srf_ms_ssim_<what> (MS-SSIM's pyramid) and its relu argument;
+    MS-SSIM always relu's, so its entries take none."""
+    if levels > 1:
+        return f"srf_ms_ssim_{what}", ()
+    return f"srf_ssim_{what}", (1 if nonnegative_ssim else 0,)
+
+
+def ssim_launch(dev: torch.device, x_ptr: int, ax, y_ptr: int, ay, shape, data_range: float, size_average: bool,
+                nonnegative_ssim: bool, levels: int = 1):
+    """The forward (SSIM for levels=1, MS-SSIM for _MS_LEVELS) on logical [B,C,H,W] images at device addresses
+    ``x_ptr`` / ``y_ptr`` read through ``ax`` / ``ay``: (out, workspace); the workspace is what the backward needs."""
+    B, C, H, W = shape
+    nbytes = (_lib.ms_ssim_workspace_bytes if levels > 1 else _lib.ssim_workspace_bytes)(_lib.load(), B, C, H, W)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    out = torch.empty(() if size_average else (B,), dtype=torch.float32, device=dev)
+    name, relu = _entry(levels, "forward", nonnegative_ssim)
+    _lib.launch(name, dev, B, C, H, W, x_ptr, ctypes.byref(ax), y_ptr, ctypes.byref(ay), float(data_range),
+                1 if size_average else 0, *relu, ws.data_ptr(), out.data_ptr())
+    return out, ws
+
+
+class _Ssim(torch.autograd.Function):
+    """SSIM (levels=1) or MS-SSIM (levels=_MS_LEVELS) of X against Y, differentiable wrt X."""
+
     @staticmethod
-    def forward(ctx, X, Y, views, data_range, size_average):
-        dev = X.device
-        if not X.is_cuda or Y.device != dev:
-            raise RuntimeError(f"MS_SSIM: X and Y must be CUDA tensors on one device, got {X.device} and {Y.device}")
-        B, C, H, W = _logical_shape(X, views)
-        ws = torch.empty(_lib.ms_ssim_workspace_bytes(_lib.load(), B, C, H, W), dtype=torch.uint8, device=dev)
-        out = torch.empty(() if size_average else (B,), dtype=torch.float32, device=dev)
-        ax, ay = _addr(X, views), _addr(Y, views)
-        _lib.launch("srf_ms_ssim_forward", dev, B, C, H, W, X.data_ptr(), ctypes.byref(ax), Y.data_ptr(),
-                    ctypes.byref(ay), float(data_range), 1 if size_average else 0, ws.data_ptr(), out.data_ptr())
+    def forward(ctx, X, Y, views, data_range, size_average, nonnegative_ssim, levels):
+        if not X.is_cuda or Y.device != X.device:
+            raise RuntimeError(f"{'MS_SSIM' if levels > 1 else 'ssim'}: X and Y must be CUDA tensors on one device, "
+                               f"got {X.device} and {Y.device}")
+        shape = _logical_shape(X, views)
+        out, ws = ssim_launch(X.device, X.data_ptr(), _addr(X, views), Y.data_ptr(), _addr(Y, views), shape,
+                              data_range, size_average, nonnegative_ssim, levels)
         ctx.save_for_backward(X, Y, ws)
-        ctx.cfg = (views, float(data_range), bool(size_average), (B, C, H, W))
+        ctx.cfg = (views, float(data_range), bool(size_average), _entry(levels, "backward", nonnegative_ssim), shape)
         return out
 
     @staticmethod
     def backward(ctx, g_out):
         X, Y, ws = ctx.saved_tensors
-        views, data_range, size_average, (B, C, H, W) = ctx.cfg
+        views, data_range, size_average, (name, relu), (B, C, H, W) = ctx.cfg
         up = g_out.to(torch.float32).reshape(-1).contiguous()
         gX = torch.empty_like(X)
         ax, ay, ag = _addr(X, views), _addr(Y, views), _addr(gX, views)
-        _lib.launch("srf_ms_ssim_backward", X.device, B, C, H, W, X.data_ptr(), ctypes.byref(ax), Y.data_ptr(),
-                    ctypes.byref(ay), data_range, 1 if size_average else 0, ws.data_ptr(), up.data_ptr(),
-                    gX.data_ptr(), ctypes.byref(ag))
-        return gX, None, None, None, None
+        _lib.launch(name, X.device, B, C, H, W, X.data_ptr(), ctypes.byref(ax), Y.data_ptr(), ctypes.byref(ay),
+                    data_range, 1 if size_average else 0, *relu, ws.data_ptr(), up.data_ptr(), gX.data_ptr(),
+                    ctypes.byref(ag))
+        return gX, None, None, None, None, None, None
 
 
 def ms_ssim_views(image: torch.Tensor, target: torch.Tensor, data_range: float = 1.0) -> torch.Tensor:
@@ -89,7 +111,7 @@ def ms_ssim_views(image: torch.Tensor, target: torch.Tensor, data_range: float =
     check_inputs("ms_ssim_views", image, target)
     if min(image.shape[2], image.shape[0] * image.shape[3]) <= _MIN_SIDE:
         raise AssertionError(f"Image size should be larger than {_MIN_SIDE} due to the 4 downsamplings in ms-ssim")
-    return _MsSsim.apply(image, target, True, data_range, True)
+    return _Ssim.apply(image, target, True, data_range, True, True, _MS_LEVELS)
 
 
 class MS_SSIM(torch.nn.Module):
@@ -119,7 +141,7 @@ class MS_SSIM(torch.nn.Module):
             raise ValueError(f"MS_SSIM: expected {self.channel} channels, got {X.shape[1]}")
         assert min(X.shape[-2:]) > _MIN_SIDE, \
             "Image size should be larger than %d due to the 4 downsamplings in ms-ssim" % _MIN_SIDE
-        return _MsSsim.apply(X, Y, False, self.data_range, self.size_average)
+        return _Ssim.apply(X, Y, False, self.data_range, self.size_average, True, _MS_LEVELS)
 
 
 # ---- single-scale SSIM (pytorch-msssim 1.0.0 ``ssim`` / ``SSIM``) ----------------------------------------------------
@@ -138,44 +160,6 @@ def _check_ssim_size(fn: str, H: int, W: int) -> None:
                          "filter along a shorter side with a warning; the fused SSIM does not)")
 
 
-def ssim_launch(dev: torch.device, x_ptr: int, ax, y_ptr: int, ay, shape, data_range: float, size_average: bool,
-                nonnegative_ssim: bool):
-    """srf_ssim_forward on logical [B,C,H,W] images at device addresses ``x_ptr`` / ``y_ptr`` read through ``ax`` /
-    ``ay``: (out, workspace); the workspace is what srf_ssim_backward needs."""
-    B, C, H, W = shape
-    ws = torch.empty(_lib.ssim_workspace_bytes(_lib.load(), B, C, H, W), dtype=torch.uint8, device=dev)
-    out = torch.empty(() if size_average else (B,), dtype=torch.float32, device=dev)
-    _lib.launch("srf_ssim_forward", dev, B, C, H, W, x_ptr, ctypes.byref(ax), y_ptr, ctypes.byref(ay),
-                float(data_range), 1 if size_average else 0, 1 if nonnegative_ssim else 0, ws.data_ptr(),
-                out.data_ptr())
-    return out, ws
-
-
-class _Ssim(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, X, Y, views, data_range, size_average, nonnegative_ssim):
-        if not X.is_cuda or Y.device != X.device:
-            raise RuntimeError(f"ssim: X and Y must be CUDA tensors on one device, got {X.device} and {Y.device}")
-        shape = _logical_shape(X, views)
-        out, ws = ssim_launch(X.device, X.data_ptr(), _addr(X, views), Y.data_ptr(), _addr(Y, views), shape,
-                              data_range, size_average, nonnegative_ssim)
-        ctx.save_for_backward(X, Y, ws)
-        ctx.cfg = (views, float(data_range), bool(size_average), bool(nonnegative_ssim), shape)
-        return out
-
-    @staticmethod
-    def backward(ctx, g_out):
-        X, Y, ws = ctx.saved_tensors
-        views, data_range, size_average, nonneg, (B, C, H, W) = ctx.cfg
-        up = g_out.to(torch.float32).reshape(-1).contiguous()
-        gX = torch.empty_like(X)
-        ax, ay, ag = _addr(X, views), _addr(Y, views), _addr(gX, views)
-        _lib.launch("srf_ssim_backward", X.device, B, C, H, W, X.data_ptr(), ctypes.byref(ax), Y.data_ptr(),
-                    ctypes.byref(ay), data_range, 1 if size_average else 0, 1 if nonneg else 0, ws.data_ptr(),
-                    up.data_ptr(), gX.data_ptr(), ctypes.byref(ag))
-        return gX, None, None, None, None, None
-
-
 def ssim(X: torch.Tensor, Y: torch.Tensor, data_range=255, size_average=True, win_size=11, win_sigma=1.5, win=None,
          K=(0.01, 0.03), nonnegative_ssim=False) -> torch.Tensor:
     """Drop-in for ``pytorch_msssim.ssim`` (same signature and defaults) on 4-D float32 CUDA inputs of any strides.
@@ -186,7 +170,7 @@ def ssim(X: torch.Tensor, Y: torch.Tensor, data_range=255, size_average=True, wi
     _check_ssim_args("ssim", win_size, win_sigma, win, K)
     check_inputs("ssim", X, Y)
     _check_ssim_size("ssim", X.shape[2], X.shape[3])
-    return _Ssim.apply(X, Y, False, data_range, size_average, nonnegative_ssim)
+    return _Ssim.apply(X, Y, False, data_range, size_average, nonnegative_ssim, 1)
 
 
 class SSIM(torch.nn.Module):
@@ -208,7 +192,7 @@ class SSIM(torch.nn.Module):
         if X.shape[1] != self.channel:
             raise ValueError(f"SSIM: expected {self.channel} channels, got {X.shape[1]}")
         _check_ssim_size("SSIM", X.shape[2], X.shape[3])
-        return _Ssim.apply(X, Y, False, self.data_range, self.size_average, self.nonnegative_ssim)
+        return _Ssim.apply(X, Y, False, self.data_range, self.size_average, self.nonnegative_ssim, 1)
 
 
 def ssim_views(image: torch.Tensor, target: torch.Tensor, data_range: float = 1.0, view_range=None) -> torch.Tensor:
@@ -222,4 +206,4 @@ def ssim_views(image: torch.Tensor, target: torch.Tensor, data_range: float = 1.
         image, target = image[v0:v1], target[v0:v1]
     check_inputs("ssim_views", image, target)
     _check_ssim_size("ssim_views", image.shape[2], image.shape[0] * image.shape[3])
-    return _Ssim.apply(image, target, True, data_range, True, False)
+    return _Ssim.apply(image, target, True, data_range, True, False, 1)
