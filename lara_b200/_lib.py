@@ -29,6 +29,7 @@ class MsSsimAddr(Structure):
 
 _A = POINTER(MsSsimAddr)
 _I3 = POINTER(c_int)            # host int[3]
+_P5 = POINTER(c_void_p)         # host void*[5]
 MESH_CAM_FLOATS = 24            # include/surfel_mesh.h SRF_MESH_CAM_FLOATS
 
 # name -> (restype, argtypes); mirrors include/surfel_rasterizer.h one to one
@@ -169,6 +170,10 @@ SIGNATURES = {
                                    _P, _P, _P,                           # rgba, normal, bg
                                    _P, _P, _P, _P,                       # i2w, i2w_down, origin, nrm_rot
                                    _P, _P, _P, _P, _P]),                 # tar_rgb, tar_msk, tar_nrm, tar_rays, tar_rays_down
+    # include/surfel_finetune.h
+    "srf_gaussian_adam_step": (c_int, [_P, c_int, c_int, _P5, _P5, _P,  # stream, n, M, params, grads, moments
+                                       POINTER(c_double), c_double, c_double, c_double,   # lr (host [6]), beta1, beta2, eps
+                                       c_double, c_double, c_int]),     # bias_correction1, _2_sqrt, zero_grads
     "srf_profile_begin": (c_int, []),
     "srf_profile_end": (c_int, [POINTER(c_float), POINTER(c_int), c_int]),
 }
