@@ -15,13 +15,11 @@ its achieved bytes/s against the H100 SXM's 3.35 TB/s; the same without normals;
 from __future__ import annotations
 
 import argparse
+import itertools
 import json
 import os
 import random
-import statistics
-import subprocess
 import sys
-import time
 
 import numpy as np
 import torch
@@ -30,16 +28,9 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from lara_b200 import _lib  # noqa: E402
 from lara_b200.batch import GobjverseViews, assemble_batch  # noqa: E402
+from timing import alternate, card, cuda_ms, host_ms, summary  # noqa: E402  (tools/ is on sys.path as a script)
 
 PEAK_BYTES_PER_S = 3.35e12     # H100 SXM HBM3, data sheet
-
-
-def gpu_info():
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                              capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as ex:            # noqa: BLE001
-        return f"unknown ({ex})"
 
 
 class Cfg:
@@ -96,18 +87,6 @@ def nbytes(batch):
     return sum(v.numel() * v.element_size() for v in batch.values() if isinstance(v, torch.Tensor))
 
 
-def timed_ms(fn):
-    torch.cuda.synchronize()
-    t = time.perf_counter()
-    fn()
-    torch.cuda.synchronize()
-    return (time.perf_counter() - t) * 1e3
-
-
-def summary(xs):
-    return {"median": round(statistics.median(xs), 4), "min": round(min(xs), 4), "max": round(max(xs), 4), "n": len(xs)}
-
-
 def kernel_time(raw_dev, dev, iters):
     """ms per srf_batch_assemble launch (CUDA events over ``iters`` launches) and the bytes it moves."""
     out = assemble_batch(raw_dev, dev)
@@ -119,16 +98,10 @@ def kernel_time(raw_dev, dev, iters):
     args = (B, N, H, W, rgba.data_ptr(), _lib._ptr(nrm), small[0].data_ptr(), small[1].data_ptr(), small[2].data_ptr(),
             origin.data_ptr(), _lib._ptr(rot), out["tar_rgb"].data_ptr(), out["tar_msk"].data_ptr(),
             _lib._ptr(out.get("tar_nrm")), out["tar_rays"].data_ptr(), out["tar_rays_down"].data_ptr())
+    launch = lambda: _lib.launch("srf_batch_assemble", dev, *args)      # noqa: E731
     for _ in range(5):
-        _lib.launch("srf_batch_assemble", dev, *args)
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    e0.record()
-    for _ in range(iters):
-        _lib.launch("srf_batch_assemble", dev, *args)
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / iters
+        launch()
+    ms = cuda_ms(launch, iters)
     written = sum(out[k].numel() * out[k].element_size()
                   for k in ("tar_rgb", "tar_msk", "tar_nrm", "tar_rays", "tar_rays_down") if k in out)
     read = rgba.numel() + (0 if nrm is None else nrm.numel())
@@ -147,8 +120,7 @@ def main():
     a = ap.parse_args()
     assert torch.cuda.is_available(), "bench_batch.py needs a GPU"
     dev = torch.device("cuda:0")
-    info = gpu_info()
-    res = {"gpu": info, "B": a.B, "N": 8, "H": a.size, "W": a.size}
+    res = {"card": card(), "B": a.B, "N": 8, "H": a.size, "W": a.size}
     metas = synthetic_metas(0, a.size, a.size, a.B + 1)
 
     for normals in (True, False):
@@ -162,28 +134,22 @@ def main():
         lara = {k: v.cpu() if isinstance(v, torch.Tensor) else v for k, v in assemble_batch(raw, dev).items()}
         lara = {k: v for k, v in lara.items() if k not in ("i2w", "i2w_down")}
         tag = "normals" if normals else "no_normals"
-        arm_a, arm_b = [], []
-        for _ in range(3):         # warm-up of both arms
-            timed_ms(lambda: [v.to(dev) for v in lara.values() if isinstance(v, torch.Tensor)])
-            timed_ms(lambda: assemble_batch(raw_pinned, dev))
-        for _ in range(a.reps):
-            arm_a.append(timed_ms(lambda: [v.to(dev) for v in lara.values() if isinstance(v, torch.Tensor)]))
-            arm_b.append(timed_ms(lambda: assemble_batch(raw_pinned, dev)))
+        arms = {"ms_a_lara_transfer": lambda: [v.to(dev) for v in lara.values() if isinstance(v, torch.Tensor)],
+                "ms_b_assemble_batch": lambda: assemble_batch(raw_pinned, dev)}
+        alternate(arms, 3, host_ms)          # warm-up of both arms
+        times = alternate(arms, a.reps, host_ms)
         raw_dev = {k: (v.to(dev) if isinstance(v, torch.Tensor) else v) for k, v in raw.items()}
         res[tag] = {
             "bytes_a_lara_pageable_float32": nbytes(lara),
             "bytes_b_uint8_pinned": nbytes(raw),
-            "ms_a_lara_transfer": summary(arm_a),
-            "ms_b_assemble_batch": summary(arm_b),
+            **{k: summary(v) for k, v in times.items()},
             "kernel": kernel_time(raw_dev, dev, a.kernel_iters),
         }
         if normals:
-            host_a, host_b = [], []
-            for r in range(a.host_reps):
-                t = time.perf_counter(); lara_float_sample(ds, r % a.B); host_a.append((time.perf_counter() - t) * 1e3)
-                t = time.perf_counter(); ds[r % a.B]; host_b.append((time.perf_counter() - t) * 1e3)
-            res["host_only_getitem_ms"] = {"lara_float32_restatement": summary(host_a),
-                                           "GobjverseViews": summary(host_b)}
+            ia, ib = itertools.cycle(range(a.B)), itertools.cycle(range(a.B))      # sample r % B in repeat r
+            host = alternate({"lara_float32_restatement": lambda: lara_float_sample(ds, next(ia)),
+                              "GobjverseViews": lambda: ds[next(ib)]}, a.host_reps, host_ms)
+            res["host_only_getitem_ms"] = {k: summary(v) for k, v in host.items()}
         del raw_pinned, raw_dev, lara
         torch.cuda.empty_cache()
     print(json.dumps(res))

@@ -23,7 +23,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from bench_deterministic import card  # noqa: E402  (tools/ is on sys.path when run as a script)
+from timing import alternate, card, cuda_ms, peak_mib, summary  # noqa: E402  (tools/ is on sys.path as a script)
 
 
 def main() -> None:
@@ -92,31 +92,19 @@ def main() -> None:
     arms = {"loop": loop_step, "batch": batch_step}
     a, bt = loop_step(), batch_step()
     same = all(torch.equal(x[0], y[0]) and torch.equal(x[1], y[1]) for x, y in zip(a, bt))
-    times = defaultdict(list)
     for _ in range(2):
         for fn in arms.values():
             fn()
-    for _ in range(args.rounds):
-        for name, fn in arms.items():
-            torch.cuda.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(args.iters):
-                for t in leaves + [fine_b] + fine_s:
-                    t.grad = None
-                fn()
-            e1.record()
-            torch.cuda.synchronize()
-            times[name].append(e0.elapsed_time(e1) / args.iters)
+
+    def clear_then(fn):
+        for t in leaves + [fine_b] + fine_s:
+            t.grad = None
+        fn()
+
+    times = alternate(arms, args.rounds, lambda fn: cuda_ms(lambda: clear_then(fn), args.iters))
     res = {}
     for name, fn in arms.items():
-        ts = sorted(times[name])
-        torch.cuda.synchronize()
-        torch.cuda.reset_peak_memory_stats()
-        base = torch.cuda.memory_allocated()
-        fn()
-        torch.cuda.synchronize()
-        peak = torch.cuda.max_memory_allocated() - base
+        peak = peak_mib(fn)
         from torch.profiler import ProfilerActivity, profile
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             fn()
@@ -126,12 +114,13 @@ def main() -> None:
             if ev.device_type.name == "CUDA" and ev.self_device_time_total > 0:
                 kern[ev.key[:60]] += ev.self_device_time_total / 1000.0
         top = dict(sorted(kern.items(), key=lambda kv: -kv[1])[:14])
-        res[name] = {"ms_median": ts[len(ts) // 2], "ms_min": ts[0], "ms_max": ts[-1],
-                     "kernel_ms_total": round(sum(kern.values()), 3), "peak_MB": round(peak / 2**20, 1),
+        res[name] = {"ms": summary(times[name]),
+                     "kernel_ms_total": round(sum(kern.values()), 3), "peak_MB": round(peak, 1),
                      "kernels_ms": {k: round(v, 3) for k, v in top.items()}}
         print(json.dumps({"arm": name, **res[name]}), flush=True)
-    print(json.dumps({"bit_identical": same, "speedup": res["loop"]["ms_median"] / res["batch"]["ms_median"],
-                      "saved_ms": res["loop"]["ms_median"] - res["batch"]["ms_median"]}), flush=True)
+    loop_ms, batch_ms = res["loop"]["ms"]["median"], res["batch"]["ms"]["median"]
+    print(json.dumps({"bit_identical": same, "speedup": loop_ms / batch_ms, "saved_ms": loop_ms - batch_ms}),
+          flush=True)
 
 
 if __name__ == "__main__":

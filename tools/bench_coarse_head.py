@@ -26,7 +26,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from bench_deterministic import card  # noqa: E402  (tools/ is on sys.path when run as a script)
+from timing import alternate, card, cuda_ms, peak_mib, summary  # noqa: E402  (tools/ is on sys.path as a script)
 
 B, R, D, K, SH = 3, 64, 80, 2, 12
 OPACITY_SHIFT, SCALING_SHIFT, HALF_CELL = -2.1792, -4.2, 0.5 * 0.5 / 32
@@ -96,25 +96,12 @@ def main() -> None:
             step(fn)
             forward(fn)
             clear()
-        torch.cuda.synchronize()
-        base = torch.cuda.memory_allocated()
-        torch.cuda.reset_peak_memory_stats()
-        step(fn)
-        torch.cuda.synchronize()
-        peak[name] = (torch.cuda.max_memory_allocated() - base) / 2 ** 20
+        peak[name] = peak_mib(lambda: step(fn))
         clear()
-    times = {(k, m): [] for k in arms for m in ("fwd_bwd", "fwd")}
-    for _ in range(args.repeats):
-        for name, fn in arms.items():             # arms alternate within each repeat
-            for mode, run in (("fwd_bwd", step), ("fwd", forward)):
-                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                a.record()
-                for _ in range(args.iters):
-                    run(fn)
-                    clear()
-                b.record()
-                torch.cuda.synchronize()
-                times[(name, mode)].append(1e3 * a.elapsed_time(b) / args.iters)
+    # each arm's forward + backward, then its forward alone; the arms alternate within each repeat
+    calls = {(name, mode): (lambda run=run, fn=fn: (run(fn), clear()))
+             for name, fn in arms.items() for mode, run in (("fwd_bwd", step), ("fwd", forward))}
+    times = alternate(calls, args.repeats, lambda call: 1e3 * cuda_ms(call, args.iters))
     c = card()
     fl = floors()
     print(f"card: {c['name']}, power limit {c['power_limit']}; B={B} voxels={R}^3 D={D} K={K} sh_dim={SH}")
@@ -126,10 +113,9 @@ def main() -> None:
         r = {"peak_increase_mb": round(peak[name], 1)}
         line = f"  {name:10s}"
         for mode in ("fwd_bwd", "fwd"):
-            ts = sorted(times[(name, mode)])
-            med = ts[len(ts) // 2]
-            line += f"  {mode} {med:8.1f} us ({ts[0]:.1f} - {ts[-1]:.1f})"
-            r[mode] = {"median_us": round(med, 1), "min_us": round(ts[0], 1), "max_us": round(ts[-1], 1)}
+            t = summary(times[(name, mode)])
+            r[mode + "_us"] = t
+            line += f"  {mode} {t['median']:8.1f} us ({t['min']:.1f} - {t['max']:.1f})"
         print(line + f"  peak +{peak[name]:7.1f} MB")
         res[name] = r
     print(json.dumps(res))

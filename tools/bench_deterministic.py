@@ -11,22 +11,13 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-
-def card() -> dict:
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power = [s.strip() for s in out.split(",")]
-    except Exception:
-        name, power = torch.cuda.get_device_name(), "unknown"
-    return {"name": name, "power_limit": power}
+from timing import alternate, card, cuda_ms, summary  # noqa: E402  (tools/ is on sys.path when run as a script)
 
 
 def main() -> None:
@@ -55,22 +46,10 @@ def main() -> None:
         R.backward_views_raw(state, radii, t["means3D"], t["shs"], None, t["scales"], t["rotations"], None, camt,
                              cams[0].tanfovx, cams[0].tanfovy, H, W, sc["sh_degree"], gc, ga, deterministic=det)
 
-    def timed(det):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(args.iters):
-            bwd(det)
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / args.iters
-
-    for det in (False, True, False, True):      # warm-up of both paths
-        bwd(det)
-    torch.cuda.synchronize()
-    res = {False: [], True: []}
-    for _ in range(args.rounds):
-        for det in (False, True):
-            res[det].append(timed(det))
+    arms = {"default": lambda: bwd(False), "deterministic": lambda: bwd(True)}
+    for fn in (*arms.values(), *arms.values()):      # warm-up of both paths
+        fn()
+    res = {k: summary(v) for k, v in alternate(arms, args.rounds, lambda fn: cuda_ms(fn, args.iters)).items()}
     _lib.profile_begin()
     bwd(False)
     kd = _lib.profile_end()["render_bwd"]
@@ -80,10 +59,10 @@ def main() -> None:
     PL, VL = 524288, 8
     extra = _lib.det_backward_scratch_bytes(lib, VL, PL) - _lib.views_sizes(lib, VL, PL, 512, 512, 0)[5]
     out = {"card": card(), "point": {"P": P, "H": H, "W": W, "views": V},
-           "backward_ms": {"default": res[False], "deterministic": res[True]},
+           "backward_ms": res,
            "render_bwd_ms": {"default": kd[0], "default_launches": kd[1], "deterministic": kt[0],
                              "deterministic_launches": kt[1]},
-           "ratio_median": sorted(res[True])[len(res[True]) // 2] / sorted(res[False])[len(res[False]) // 2],
+           "ratio_median": res["deterministic"]["median"] / res["default"]["median"],
            "extra_scratch_bytes_lara": {"P": PL, "views": VL, "bytes": extra}}
     print(json.dumps(out))
 

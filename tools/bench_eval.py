@@ -15,9 +15,7 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 
 import numpy as np
 import torch
@@ -25,24 +23,7 @@ import torch.nn.functional as F
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-
-def gpu_info():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as ex:            # noqa: BLE001
-        q = f"unknown ({ex})"
-    return q
-
-
-def timed(fn):
-    torch.cuda.synchronize()
-    torch.cuda.reset_peak_memory_stats()
-    base = torch.cuda.memory_allocated()
-    t = time.perf_counter()
-    fn()
-    torch.cuda.synchronize()
-    return (time.perf_counter() - t) * 1e3, (torch.cuda.max_memory_allocated() - base) / 2 ** 20
+from timing import alternate, card, host_ms, peak_mib, summary  # noqa: E402  (tools/ is on sys.path as a script)
 
 
 def ssim_torch(X, Y, data_range=1.0):
@@ -112,10 +93,9 @@ def main():
 
     fused = lambda: render_video_frames(renderer, params, cams, device=dev)      # noqa: E731
     lara_loop(), fused()                      # warm-up of every shape
-    res = {"lara_loop": [], "fused": []}
-    for _ in range(a.reps):
-        for k, fn in (("lara_loop", lara_loop), ("fused", fused)):
-            res[k].append(timed(fn))
+    arms = {"lara_loop": lara_loop, "fused": fused}
+    res = alternate(arms, a.reps, host_ms)
+    peak = {k: peak_mib(fn) for k, fn in arms.items()}
     r1, n1 = lara_loop()
     r2, n2 = fused()
     same = bool(np.array_equal(np.stack(r1), r2) and np.array_equal(np.stack(n1), n2))
@@ -135,21 +115,16 @@ def main():
     m_fused = lambda: novel_view_metrics(out, sample, nv, True, thr)               # noqa: E731
     with torch.no_grad():
         m_lara(), m_fused()
-        mres = {"lara_metrics": [], "fused_metrics": []}
-        for _ in range(max(a.reps, 10)):
-            for k, fn in (("lara_metrics", m_lara), ("fused_metrics", m_fused)):
-                mres[k].append(timed(fn))
+        marms = {"lara_metrics": m_lara, "fused_metrics": m_fused}
+        mres = alternate(marms, max(a.reps, 10), host_ms)
+        peak.update({k: peak_mib(fn) for k, fn in marms.items()})
         ml, mf = m_lara(), m_fused()
 
-    def summary(v):
-        t = [x[0] for x in v]
-        return {"median_ms": round(float(np.median(t)), 2), "min_ms": round(min(t), 2), "max_ms": round(max(t), 2),
-                "peak_mib": round(max(x[1] for x in v), 1)}
     print(json.dumps({
-        "gpu": gpu_info(), "P": a.P, "frames": a.frames, "size": a.size,
+        "card": card(), "P": a.P, "frames": a.frames, "size": a.size,
         "chunk": default_chunk(a.P, H, W, a.frames, dev),
-        **{k: summary(v) for k, v in res.items()}, "frames_identical": same,
-        **{k: summary(v) for k, v in mres.items()},
+        **{k: {"ms": summary(v), "peak_mib": round(peak[k], 1)} for k, v in res.items()}, "frames_identical": same,
+        **{k: {"ms": summary(v), "peak_mib": round(peak[k], 1)} for k, v in mres.items()},
         "metrics_lara": ml, "metrics_fused": [mf["psnr"], mf["ssim"]] + mf["depth_acc"],
     }))
 

@@ -24,7 +24,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from bench_deterministic import card  # noqa: E402  (tools/ is on sys.path when run as a script)
+from timing import alternate, card, cuda_ms, peak_mib, summary  # noqa: E402  (tools/ is on sys.path as a script)
 
 B, V, HW, IMG, R, E, NG = 3, 4, 32, 512, 16, 32, 16
 HBM_BYTES_PER_S = 3.35e12
@@ -90,36 +90,20 @@ def run(C: int, repeats: int, iters: int) -> dict:
         for _ in range(2):                         # warm-up (and the first-call allocations)
             fn()
             clear()
-        torch.cuda.synchronize()
-        base = torch.cuda.memory_allocated()
-        torch.cuda.reset_peak_memory_stats()
-        fn()
-        torch.cuda.synchronize()
-        peak[name] = (torch.cuda.max_memory_allocated() - base) / 2 ** 20
+        peak[name] = peak_mib(fn)
         clear()
-    times = {k: [] for k in arms}
-    for _ in range(repeats):
-        for name, fn in arms.items():             # arms alternate within each repeat
-            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            a.record()
-            for _ in range(iters):
-                fn()
-                clear()
-            b.record()
-            torch.cuda.synchronize()
-            times[name].append(1e3 * a.elapsed_time(b) / iters)
+    times = alternate(arms, repeats, lambda fn: 1e3 * cuda_ms(lambda: (fn(), clear()), iters))
     fl = floors_us(C)
     floor = fl["fwd_us"] + fl["bwd_us"]
     print(f"B={B} V={V} C={C} tokens {HW}x{HW} image {IMG}^2 R={R} E={E} n_group={NG}; HBM floor fwd "
           f"{fl['fwd_mb']:.0f} MB {fl['fwd_us']:.0f} us, bwd {fl['bwd_mb']:.0f} MB {fl['bwd_us']:.0f} us")
     res = {"C": C, "floor": {k: round(v, 1) for k, v in fl.items()}}
     for name, ts in times.items():
-        ts = sorted(ts)
-        med = ts[len(ts) // 2]
-        print(f"  {name:22s} fwd+bwd {med:9.1f} us (range {ts[0]:.1f} - {ts[-1]:.1f})  peak +{peak[name]:8.1f} MB  "
-              f"HBM-floor share {floor / med:.2f}")
-        res[name] = {"median_us": round(med, 1), "min_us": round(ts[0], 1), "max_us": round(ts[-1], 1),
-                     "peak_increase_mb": round(peak[name], 1), "floor_share": round(floor / med, 3)}
+        t = summary(ts)
+        print(f"  {name:22s} fwd+bwd {t['median']:9.1f} us (range {t['min']:.1f} - {t['max']:.1f})  "
+              f"peak +{peak[name]:8.1f} MB  HBM-floor share {floor / t['median']:.2f}")
+        res[name] = {"fwd_bwd_us": t, "peak_increase_mb": round(peak[name], 1),
+                     "floor_share": round(floor / t["median"], 3)}
     for name, msg in failed.items():
         print(f"  {name:22s} fails at this size: {msg}")
         res[name] = {"error": msg}

@@ -4,8 +4,8 @@ source views, N = 262144 voxels, K = 2, a mask keeping half the Gaussians, so n 
 Three arms, alternating in one process after a warm-up: the fused head (``FineHead.fine_shs``), and LaRa's torch head
 (the same ``norm`` / ``cross_att`` / ``mlp_fine`` modules called as ``Decoder.forward_fine`` calls them, with the gathers,
 einsum and residual around it) in fp32 and under bf16 autocast.  Each is timed with CUDA events; the median and range
-over --repeats are printed, with the peak-memory increase (``torch.cuda.max_memory_allocated`` over the allocation
-before the call) of one forward + backward.  Prints the card's name and power limit, then one JSON line.
+over --repeats are printed, with the peak-memory increase (the peak allocation over the allocation before the call)
+of one forward + backward.  Prints the card's name and power limit, then one JSON line.
 
     python tools/bench_fine_head.py [--repeats 7] [--iters 10]
 """
@@ -20,7 +20,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from bench_deterministic import card  # noqa: E402  (tools/ is on sys.path when run as a script)
+from timing import alternate, card, cuda_ms, peak_mib, summary  # noqa: E402  (tools/ is on sys.path as a script)
 
 V, N, K, D, SH = 4, 262144, 2, 80, 12
 
@@ -80,33 +80,17 @@ def main() -> None:
         for _ in range(2):                         # warm-up (and the first-call allocations)
             fn()
             clear()
-        torch.cuda.synchronize()
-        base = torch.cuda.memory_allocated()
-        torch.cuda.reset_peak_memory_stats()
-        fn()
-        torch.cuda.synchronize()
-        peak[name] = (torch.cuda.max_memory_allocated() - base) / 2 ** 20
+        peak[name] = peak_mib(fn)
         clear()
-    times = {k: [] for k in arms}
-    for _ in range(args.repeats):
-        for name, fn in arms.items():             # arms alternate within each repeat
-            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            a.record()
-            for _ in range(args.iters):
-                fn()
-                clear()
-            b.record()
-            torch.cuda.synchronize()
-            times[name].append(1e3 * a.elapsed_time(b) / args.iters)
+    times = alternate(arms, args.repeats, lambda fn: 1e3 * cuda_ms(lambda: (fn(), clear()), args.iters))
     c = card()
     print(f"card: {c['name']}, power limit {c['power_limit']}; V={V} n={n} D={D} sh_dim={SH}")
     res = {"card": c, "V": V, "n": n, "D": D, "sh_dim": SH}
     for name, ts in times.items():
-        ts = sorted(ts)
-        med = ts[len(ts) // 2]
-        print(f"  {name:22s} fwd+bwd {med:9.1f} us (range {ts[0]:.1f} - {ts[-1]:.1f})  peak +{peak[name]:8.1f} MB")
-        res[name] = {"median_us": round(med, 1), "min_us": round(ts[0], 1), "max_us": round(ts[-1], 1),
-                     "peak_increase_mb": round(peak[name], 1)}
+        t = summary(ts)
+        print(f"  {name:22s} fwd+bwd {t['median']:9.1f} us (range {t['min']:.1f} - {t['max']:.1f})  "
+              f"peak +{peak[name]:8.1f} MB")
+        res[name] = {"fwd_bwd_us": t, "peak_increase_mb": round(peak[name], 1)}
     for name, msg in failed.items():
         print(f"  {name:22s} fails at this size: {msg}")
         res[name] = {"error": msg}

@@ -20,11 +20,8 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 
-import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -33,18 +30,10 @@ from lara_b200 import finetune as F  # noqa: E402
 from lara_b200.loss import scene_loss  # noqa: E402
 from lara_b200.renderer import Renderer  # noqa: E402
 from lara_b200.scene import PathCamera, cameras, scene  # noqa: E402
+from timing import alternate, card, cuda_ms, host_ms, summary  # noqa: E402  (tools/ is on sys.path as a script)
 
 LRS = dict(position_lr=0.000016, feature_lr=0.0025, opacity_lr=0.05, scaling_lr=0.005, rotation_lr=0.001)
 HBM_BYTES_PER_S = 3.35e12
-
-
-def gpu_info():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as ex:            # noqa: BLE001
-        q = f"unknown ({ex})"
-    return q
 
 
 def make_case(P, V, H, dev, seed=0):
@@ -109,13 +98,7 @@ def kernel_time(P, M, dev, iters):
         t.grad = torch.randn_like(t)
     for _ in range(10):
         opt.step()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        opt.step()
-    b.record()
-    torch.cuda.synchronize()
-    ms = a.elapsed_time(b) / iters
+    ms = cuda_ms(opt.step, iters)
     nbytes = 32 * P * (10 + 3 * M)         # reads param, grad, two moments; writes param, two moments, zeroed grad
     return ms, nbytes
 
@@ -132,7 +115,7 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("bench_finetune: needs a CUDA device")
     dev = torch.device("cuda:0")
-    card = gpu_info()
+    gpu = card()
     V = args.views
     for P in args.P:
         renderer, sample, gs = make_case(P, V, args.size, dev)
@@ -141,19 +124,14 @@ def main():
                 "C_render_img": lambda: torch_adam_loop(renderer, gs, sample, V, args.steps, True)}
         for fn in arms.values():           # warm every shape
             fn()
-        times = {k: [] for k in arms}
-        for _ in range(args.reps):
-            for k, fn in arms.items():
-                torch.cuda.synchronize()
-                t = time.perf_counter()
-                fn()
-                torch.cuda.synchronize()
-                times[k].append(time.perf_counter() - t)
+        times = alternate(arms, args.reps, host_ms)
         ms, nbytes = kernel_time(P, int(gs[1].shape[1]), dev, args.kernel_iters)
-        res = {"card": card, "P": P, "views": V, "size": args.size, "steps": args.steps, "reps": args.reps}
+        res = {"card": gpu, "P": P, "views": V, "size": args.size, "steps": args.steps, "reps": args.reps}
         for k, v in times.items():
-            res[f"{k}_steps_per_s"] = round(args.steps / float(np.median(v)), 2)
-            res[f"{k}_steps_per_s_range"] = [round(args.steps / max(v), 2), round(args.steps / min(v), 2)]
+            t = summary(v)
+            res[f"{k}_steps_per_s"] = round(1e3 * args.steps / t["median"], 2)
+            res[f"{k}_steps_per_s_range"] = [round(1e3 * args.steps / t["max"], 2),
+                                             round(1e3 * args.steps / t["min"], 2)]
         res["adam_kernel_ms"] = round(ms, 4)
         res["adam_kernel_TBps"] = round(nbytes / (ms * 1e-3) / 1e12, 3)
         res["adam_kernel_share_of_3.35TBps"] = round(nbytes / (ms * 1e-3) / HBM_BYTES_PER_S, 3)

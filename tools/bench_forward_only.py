@@ -3,10 +3,10 @@ the contribution record and the image state the backward reads) against the forw
 same inputs, alternated in one process.
 
 Per point: the whole call (forward_views_raw, enqueue to completion) timed with CUDA events, the mean of --iters calls
-in each of --rounds alternations, the blend forward's device time per view (srf_profile_*, render_fwd), and the peak of
-torch.cuda.max_memory_allocated over one call.  The default points are the bench point (131 072 Gaussians, 512 x 512,
-8 views), LaRa's Gaussian count (524 288) at 8 views and at the mesh extractor's 48 cameras.  Prints the card name and
-power limit, then one JSON line per point.
+in each of --rounds alternations, the blend forward's device time per view (srf_profile_*, render_fwd), and the peak
+allocation over one call above the allocation before it.  The default points are the bench point (131 072 Gaussians,
+512 x 512, 8 views), LaRa's Gaussian count (524 288) at 8 views and at the mesh extractor's 48 cameras.  Prints the card
+name and power limit, then one JSON line per point.
 
     python tools/bench_forward_only.py [--iters 10] [--rounds 4] [--points 131072x8,524288x8,524288x48]
 """
@@ -21,11 +21,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from bench_deterministic import card  # noqa: E402  (tools/ is on sys.path when run as a script)
-
-
-def median(xs):
-    return sorted(xs)[len(xs) // 2]
+from timing import alternate, card, cuda_ms, peak_mib, summary  # noqa: E402  (tools/ is on sys.path as a script)
 
 
 def run_point(P: int, V: int, H: int, W: int, iters: int, rounds: int) -> dict:
@@ -53,23 +49,16 @@ def run_point(P: int, V: int, H: int, W: int, iters: int, rounds: int) -> dict:
     same = all(torch.equal(a, b) for a, b in zip(fwd(True)[:3], fwd(False)[:3]))
     settle()
 
-    def timed(fb):
+    def timed(fn):
         # one call at a time, each to completion: an unresolved call keeps its state alive, so calls queued back to
         # back would hold several launch sets' workspaces at the 48-view point
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         total = 0.0
         for _ in range(iters):
-            e0.record()
-            fwd(fb)
-            e1.record()
+            total += cuda_ms(fn, 1)
             settle()
-            total += e0.elapsed_time(e1)
         return total / iters
 
-    ms = {True: [], False: []}
-    for _ in range(rounds):
-        for fb in (True, False):
-            ms[fb].append(timed(fb))
+    ms = alternate({True: lambda: fwd(True), False: lambda: fwd(False)}, rounds, timed)
 
     blend, peak, capacity = {}, {}, {}
     for fb in (True, False):
@@ -77,20 +66,17 @@ def run_point(P: int, V: int, H: int, W: int, iters: int, rounds: int) -> dict:
         fwd(fb)
         settle()
         blend[fb] = _lib.profile_end()["render_fwd"]
-        base = torch.cuda.memory_allocated()
-        torch.cuda.reset_peak_memory_stats()
-        out = fwd(fb)
+        out = []
+        peak[fb] = round(peak_mib(lambda: out.append(fwd(fb))) * 2 ** 20)
         settle()
-        peak[fb] = torch.cuda.max_memory_allocated() - base
-        capacity[fb] = out[3].capacity
+        capacity[fb] = out[0][3].capacity
         del out
         settle()
     name = {True: "training", False: "forward_only"}
     return {
         "point": {"P": P, "H": H, "W": W, "views": V, "capacity_per_view": capacity[False]},
         "outputs_bit_identical": same,
-        "call_ms": {name[fb]: ms[fb] for fb in ms},
-        "call_ms_median": {name[fb]: median(ms[fb]) for fb in ms},
+        "call_ms": {name[fb]: summary(ms[fb]) for fb in ms},
         "render_fwd_us_per_view": {name[fb]: 1000.0 * blend[fb][0] / V for fb in blend},
         "render_fwd_launches": {name[fb]: blend[fb][1] for fb in blend},
         "peak_bytes": {name[fb]: peak[fb] for fb in peak},

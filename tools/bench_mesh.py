@@ -25,7 +25,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from bench_deterministic import card  # noqa: E402  (tools/ is on sys.path when run as a script)
+from timing import card, summary  # noqa: E402  (tools/ is on sys.path when run as a script)
 
 HBM_BPS = 3.35e12           # H100 SXM data sheet HBM3 bandwidth
 FP32_FLOPS = 67e12          # H100 SXM data sheet dense FP32
@@ -118,11 +118,11 @@ def run_point(P: int, rounds: int) -> dict:
     V, HW = len(cams), 512 * 512
     floor_bytes = 40 * N + V * HW * 4 * 5           # state read + written once; depth, acc, image read once
     floor_ops = N * V * FLOPS_PER_PROJECTION
-    t_int = float(np.median(times["integrate"])) * 1e-3
+    ms = {k: summary(v) for k, v in times.items()}
+    t_int = ms["integrate"]["median"] * 1e-3
     out.update({
         "point": {"P": P, "views": V, "H": 512, "W": 512},
-        "ms_median": {k: float(np.median(v)) for k, v in times.items()},
-        "ms_range": {k: [float(min(v)), float(max(v))] for k, v in times.items()},
+        "ms": ms,
         "integrate_floor": {"bytes": floor_bytes, "hbm_floor_ms": 1e3 * floor_bytes / HBM_BPS,
                             "voxel_view_projections": N * V, "fp32_floor_ms": 1e3 * floor_ops / FP32_FLOPS,
                             "achieved_GBps": floor_bytes / t_int / 1e9,

@@ -7,11 +7,13 @@ Two workloads at LaRa's training size (configs/base.yaml: 3 scenes x 8 target vi
 Both arms of a workload alternate in this call, every shape is warmed up first, the profiler is off, and the outputs
 are compared at the same size.  The card name and power limit are read in the same call.
 
+Prints the times and the agreement, then one JSON line.
+
     python tools/bench_ms_ssim.py [--reps 5] [--iters 50]
 """
 import argparse
+import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -22,6 +24,7 @@ from helpers import rel_err  # noqa: E402
 from lara_b200.loss import scene_loss  # noqa: E402
 from lara_b200.ssim import MS_SSIM  # noqa: E402
 from test_ms_ssim import ms_ssim_torch, smooth_pair  # noqa: E402
+from timing import alternate, card, cuda_ms, summary  # noqa: E402
 
 
 def main():
@@ -35,8 +38,6 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("bench_ms_ssim: no CUDA device")
     dev = torch.device("cuda:0")
-    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
-                          capture_output=True, text=True).stdout.strip()
     B, V, H = args.scenes, args.views, args.size
     X, Y = smooth_pair(B * V, 3, H, H, 7, dtype=torch.float32)
     # planar per-scene views [B][V,3,H,W] as the fused epilogue writes them; targets [B][V,H,W,3] as the batch holds them
@@ -99,31 +100,26 @@ def main():
         if "scene_loss" in wname:
             gf = gf - mse_grad()
         agree[wname] = (abs(float(vf) - float(vt)), rel_err(gf.cpu().numpy(), gt.cpu().numpy()), float(vt))
-    times = {w: {a: [] for a in arms} for w, arms in workloads.items()}
     for arms in workloads.values():
         for _ in range(5):
             for fn in arms.values():
                 fn()
-    torch.cuda.synchronize()
-    for _ in range(args.reps):
-        for wname, arms in workloads.items():
-            for name, fn in arms.items():
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                for _ in range(args.iters):
-                    fn()
-                e1.record()
-                torch.cuda.synchronize()
-                times[wname][name].append(e0.elapsed_time(e1) / args.iters * 1e3)
-    print(f"card: {card}")
+    calls = {(w, a): fn for w, arms in workloads.items() for a, fn in arms.items()}
+    times = alternate(calls, args.reps, lambda fn: 1e3 * cuda_ms(fn, args.iters))
+    c = card()
+    print(f"card: {c['name']}, power limit {c['power_limit']}")
     print(f"fwd+bwd of the MS-SSIM term, {args.reps} alternating reps of {args.iters} steps (CUDA events), us per step")
-    for wname, arms in times.items():
+    res = {"card": c, "iters": args.iters}
+    for wname, arms in workloads.items():
         print(f"{wname}:")
-        for name, ts in arms.items():
-            ts = sorted(ts)
-            print(f"  {name:40s} median {ts[len(ts) // 2]:10.1f}   min {ts[0]:10.1f}   max {ts[-1]:10.1f}")
         d, g, v = agree[wname]
+        res[wname] = {"agreement": {"value": v, "abs_value_diff": d, "grad_rel_err": g}}
+        for name in arms:
+            t = summary(times[(wname, name)])
+            res[wname][name] = {"fwd_bwd_us": t}
+            print(f"  {name:40s} median {t['median']:10.1f}   min {t['min']:10.1f}   max {t['max']:10.1f}")
         print(f"  agreement: value {v:.7f}, |fused - torch| {d:.2e}; dL/dimage max|fused - torch| / max|torch| {g:.2e}")
+    print(json.dumps(res))
 
 
 if __name__ == "__main__":

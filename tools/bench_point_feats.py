@@ -4,11 +4,13 @@ LaRa's training size: V = 4 source views, n = 262 144 masked points, 512 x 512 i
 over as render_scene_views hands them over (channel-last views of planar buffers).  Both arms run in this call and
 alternate; their outputs are compared at the same size.  The card name and power limit are read in the same call.
 
+Prints the times and the agreement, then one JSON line.
+
     python tools/bench_point_feats.py [--reps 5] [--iters 50]
 """
 import argparse
+import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -18,6 +20,7 @@ sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 from helpers import rel_err  # noqa: E402
 from lara_b200.point_feats import sample_point_feats  # noqa: E402
 from test_point_feats import make_case, point_feats_torch  # noqa: E402
+from timing import alternate, card, cuda_ms, summary  # noqa: E402
 
 
 def restated_coords(points, w2c, ixt, H, W):
@@ -49,8 +52,6 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("bench_point_feats: no CUDA device")
     dev = torch.device("cuda:0")
-    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
-                          capture_output=True, text=True).stdout.strip()
     V, n, H = args.views, args.points, args.size
     W = H
     points, img_ref, rend, w2c, ixt = make_case(V, H, W, n, n, coarse=8)
@@ -75,28 +76,23 @@ def main():
     agree.update({f"g_{k}": rel_err(a.cpu().numpy(), b.cpu().numpy()) for k, a, b in zip(planar, g1[1:], g2[1:])})
     del res, f1, f2, g1, g2
 
-    times = {k: [] for k in arms}
     for _ in range(10):
         for fn in arms.values():
             step(fn)
-    torch.cuda.synchronize()
-    for _ in range(args.reps):
-        for name, fn in arms.items():
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(args.iters):
-                step(fn)
-            e1.record()
-            torch.cuda.synchronize()
-            times[name].append(e0.elapsed_time(e1) / args.iters * 1e3)
-    print(f"card: {card}")
+    times = alternate(arms, args.reps, lambda fn: 1e3 * cuda_ms(lambda: step(fn), args.iters))
+    c = card()
+    print(f"card: {c['name']}, power limit {c['power_limit']}")
     print(f"V={V} n={n} {H}x{W}, fwd+bwd per scene, {args.reps} alternating reps of {args.iters} steps (CUDA events)")
+    res = {"card": c, "V": V, "n": n, "H": H, "W": W, "iters": args.iters}
     for name, ts in times.items():
-        ts = sorted(ts)
-        print(f"  {name:24s} median {ts[len(ts) // 2]:9.1f} us   min {ts[0]:9.1f}   max {ts[-1]:9.1f}")
+        t = summary(ts)
+        res[name] = {"fwd_bwd_us": t}
+        print(f"  {name:24s} median {t['median']:9.1f} us   min {t['min']:9.1f}   max {t['max']:9.1f}")
     print("agreement (max |fused - torch| / max |torch|):")
     for k, v in agree.items():
         print(f"  {k:28s} {v:.2e}")
+    res["agreement"] = agree
+    print(json.dumps(res))
 
 
 if __name__ == "__main__":

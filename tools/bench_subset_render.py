@@ -24,11 +24,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from bench_deterministic import card  # noqa: E402  (tools/ is on sys.path when run as a script)
-
-
-def median(xs):
-    return sorted(xs)[len(xs) // 2]
+from timing import alternate, card, cuda_ms, summary  # noqa: E402  (tools/ is on sys.path when run as a script)
 
 
 def main() -> None:
@@ -86,17 +82,8 @@ def main() -> None:
         for bwd in (True, False):
             for arm in ("gathered", "subset", "gathered", "subset"):       # warm-up
                 call(arm, mask, shs_f, bwd)
-            torch.cuda.synchronize()
-            times = {"gathered": [], "subset": []}
-            for _ in range(args.rounds):
-                for arm in ("gathered", "subset"):
-                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                    e0.record()
-                    for _ in range(args.iters):
-                        call(arm, mask, shs_f, bwd)
-                    e1.record()
-                    torch.cuda.synchronize()
-                    times[arm].append(e0.elapsed_time(e1) / args.iters)
+            arms = {arm: (lambda arm=arm: call(arm, mask, shs_f, bwd)) for arm in ("gathered", "subset")}
+            t = {k: summary(v) for k, v in alternate(arms, args.rounds, lambda fn: cuda_ms(fn, args.iters)).items()}
             split = {}
             for arm in ("gathered", "subset"):
                 torch.cuda.synchronize()
@@ -106,14 +93,12 @@ def main() -> None:
                 torch.cuda.synchronize()
                 k = _lib.profile_end()
                 per = {kk: round(ms / args.iters, 4) for kk, (ms, cnt) in k.items() if cnt}
-                per["other"] = round(median(times[arm]) - sum(per.values()), 4)
+                per["other"] = round(t[arm]["median"] - sum(per.values()), 4)
                 split[arm] = per
             rec = {"mask": name, "n": n, "fraction": round(n / P, 4), "mode": "fwd+bwd" if bwd else "fwd",
                    "bit_identical_forward": same,
-                   "gathered_ms": round(median(times["gathered"]), 4), "subset_ms": round(median(times["subset"]), 4),
-                   "gathered_ms_all": [round(x, 4) for x in times["gathered"]],
-                   "subset_ms_all": [round(x, 4) for x in times["subset"]], "kernels_ms": split}
-            rec["speedup"] = round(rec["gathered_ms"] / rec["subset_ms"], 3)
+                   "gathered_ms": t["gathered"], "subset_ms": t["subset"], "kernels_ms": split,
+                   "speedup": round(t["gathered"]["median"] / t["subset"]["median"], 3)}
             print(json.dumps(rec), flush=True)
 
 

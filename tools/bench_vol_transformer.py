@@ -26,7 +26,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
-from bench_deterministic import card  # noqa: E402  (tools/ is on sys.path when run as a script)
+from timing import alternate, card, cuda_ms, peak_mib, summary  # noqa: E402  (tools/ is on sys.path as a script)
 
 B, V, C, CC, H, R, RC, NG, OUT = 3, 4, 256, 800, 16, 32, 16, [16], 80
 ATTN = ("fmha", "sdpa", "attention")          # torch's SDPA kernels (LaRa's attention core), before DENSE
@@ -132,32 +132,16 @@ def main() -> None:
         for _ in range(2):                         # warm-up (and the first-call allocations)
             fn()
             clear()
-        torch.cuda.synchronize()
-        base = torch.cuda.memory_allocated()
-        torch.cuda.reset_peak_memory_stats()
-        fn()
-        torch.cuda.synchronize()
-        peak[name] = (torch.cuda.max_memory_allocated() - base) / 2 ** 20
+        peak[name] = peak_mib(fn)
         clear()
-    times = {k: [] for k in arms}
-    for _ in range(args.repeats):
-        for name, fn in arms.items():             # arms alternate within each repeat
-            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            a.record()
-            for _ in range(args.iters):
-                fn()
-                clear()
-            b.record()
-            torch.cuda.synchronize()
-            times[name].append(a.elapsed_time(b) / args.iters)
+    times = alternate(arms, args.repeats, lambda fn: cuda_ms(lambda: (fn(), clear()), args.iters))
     print(f"B={B} V={V} C={C} cond {CC} H={H} R={R} n_groups={NG} layers={args.layers} out {OUT}")
     res = {"card": c, "layers": args.layers}
     for name, ts in times.items():
-        ts = sorted(ts)
-        med = ts[len(ts) // 2]
-        print(f"  {name:24s} fwd+bwd {med:8.2f} ms (range {ts[0]:.2f} - {ts[-1]:.2f})  peak +{peak[name]:8.1f} MB")
-        res[name] = {"median_ms": round(med, 3), "min_ms": round(ts[0], 3), "max_ms": round(ts[-1], 3),
-                     "peak_increase_mb": round(peak[name], 1)}
+        t = summary(ts)
+        print(f"  {name:24s} fwd+bwd {t['median']:8.2f} ms (range {t['min']:.2f} - {t['max']:.2f})  "
+              f"peak +{peak[name]:8.1f} MB")
+        res[name] = {"fwd_bwd_ms": t, "peak_increase_mb": round(peak[name], 1)}
     for name, fn in arms.items():
         split = profile_split(fn, clear)
         res[name]["profile"] = split

@@ -29,7 +29,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-from bench_deterministic import card  # noqa: E402
+from timing import alternate, card, summary  # noqa: E402
 
 KERNELS = ("preprocess_fwd", "preprocess_bwd")
 
@@ -133,30 +133,28 @@ def main() -> None:
     if parity:
         print(json.dumps({"bit_identical": parity}), flush=True)
 
+    def profiled(step, lname):
+        """us per launch of each of KERNELS over --steps steps with library ``lname``."""
+        use(lname)
+        torch.cuda.synchronize()
+        _lib.profile_begin()
+        for _ in range(args.steps):
+            step()
+        torch.cuda.synchronize()
+        prof = _lib.profile_end()
+        return {k: prof[k][0] * 1e3 / max(prof[k][1], 1) for k in KERNELS}
+
     results = []
     for pname, step in paths.items():
-        times = {l: {k: [] for k in KERNELS} for l in libs}
         for lname in libs:
             use(lname)
             for _ in range(3):
                 step()
-        for _ in range(args.rounds):
-            for lname in libs:
-                use(lname)
-                torch.cuda.synchronize()
-                _lib.profile_begin()
-                for _ in range(args.steps):
-                    step()
-                torch.cuda.synchronize()
-                prof = _lib.profile_end()
-                for k in KERNELS:
-                    ms, n = prof[k]
-                    times[lname][k].append(ms * 1e3 / max(n, 1))
+        times = alternate({l: l for l in libs}, args.rounds, lambda lname: profiled(step, lname))
         for lname in libs:
             row = {"path": pname, "lib": lname}
             for k in KERNELS:
-                ts = sorted(times[lname][k])
-                row[k + "_us"] = {"median": round(ts[len(ts) // 2], 2), "min": round(ts[0], 2), "max": round(ts[-1], 2)}
+                row[k + "_us"] = summary([t[k] for t in times[lname]])
             results.append(row)
             print(json.dumps(row), flush=True)
     if args.out:
