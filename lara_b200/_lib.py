@@ -174,6 +174,29 @@ SIGNATURES = {
     "srf_gaussian_adam_step": (c_int, [_P, c_int, c_int, _P5, _P5, _P,  # stream, n, M, params, grads, moments
                                        POINTER(c_double), c_double, c_double, c_double,   # lr (host [6]), beta1, beta2, eps
                                        c_double, c_double, c_int]),     # bias_correction1, _2_sqrt, zero_grads
+    # include/surfel_image_encoder.h
+    "srf_vit_patchify": (c_int, [_P, c_int, c_int, c_int,                 # stream, N, H, W
+                                 c_int64, c_int64, c_int64, c_int64,      # sn, sc, sy, sx
+                                 _P, _P]),                                # image, patches
+    "srf_vit_tokens_forward": (c_int, [_P, c_int, c_int, c_int, c_float,  # stream, N, L, C, eps
+                                       _P, _P, _P, _P, _P, _P, _P,        # patch_out, bias, cls, pos0, pos_r, gamma, beta
+                                       _P, _P]),                          # x, n1
+    "srf_vit_tokens_workspace_bytes": (c_int, [c_int, c_int, c_int, POINTER(c_size_t)]),
+    "srf_vit_tokens_backward": (c_int, [_P, c_int, c_int, c_int, c_float,
+                                        _P, _P, _P, _P, _P,               # x, gamma, dL_dn1, dL_dx, workspace
+                                        _P, _P, _P, _P, _P, _P]),         # dL_dtokens, d_bias, d_cls, d_pos_r, d_gamma, d_beta
+    "srf_vit_layernorm_forward": (c_int, [_P, c_int, c_int, c_float,      # stream, rows, C, eps
+                                          _P, _P, _P, _P, _P, _P]),       # a, b, gamma, beta, y, n
+    "srf_vit_layernorm_workspace_bytes": (c_int, [c_int, c_int, POINTER(c_size_t)]),
+    "srf_vit_layernorm_backward": (c_int, [_P, c_int, c_int, c_float,
+                                           _P, _P, _P, _P, _P,            # y, gamma, dL_dn, dL_dy, workspace
+                                           _P, _P, _P]),                  # dL_da, d_gamma, d_beta
+    "srf_vit_final_norm_forward": (c_int, [_P, c_int, c_int, c_int, c_float,   # stream, N, L, C, eps
+                                           _P, _P, _P, _P, _P, _P]),      # a, b, gamma, beta, y, maps
+    "srf_vit_final_norm_workspace_bytes": (c_int, [c_int, c_int, c_int, POINTER(c_size_t)]),
+    "srf_vit_final_norm_backward": (c_int, [_P, c_int, c_int, c_int, c_float,
+                                            _P, _P, _P, _P,               # y, gamma, dL_dmaps, workspace
+                                            _P, _P, _P]),                 # dL_da, d_gamma, d_beta
     "srf_profile_begin": (c_int, []),
     "srf_profile_end": (c_int, [POINTER(c_float), POINTER(c_int), c_int]),
 }
@@ -342,6 +365,21 @@ def feat_volume_workspace_bytes(lib, B: int, V: int, C: int, h: int, w: int, R: 
 def add_layernorm_workspace_bytes(lib, rows: int, C: int) -> int:
     """Workspace of srf_add_layernorm_backward."""
     return _size_query(lib.srf_add_layernorm_workspace_bytes, rows, C)
+
+
+def layernorm_workspace_bytes(lib, entry: str, rows: int, C: int) -> int:
+    """Workspace of ``{entry}_backward``, ``entry`` srf_add_layernorm or srf_vit_layernorm."""
+    return _size_query(getattr(lib, entry + "_workspace_bytes"), rows, C)
+
+
+def vit_tokens_workspace_bytes(lib, N: int, L: int, C: int) -> int:
+    """Workspace of srf_vit_tokens_backward."""
+    return _size_query(lib.srf_vit_tokens_workspace_bytes, N, L, C)
+
+
+def vit_final_norm_workspace_bytes(lib, N: int, L: int, C: int) -> int:
+    """Workspace of srf_vit_final_norm_backward."""
+    return _size_query(lib.srf_vit_final_norm_workspace_bytes, N, L, C)
 
 
 def int3(v) -> ctypes.Array:

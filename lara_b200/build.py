@@ -23,8 +23,8 @@ OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libsurfel_b200.so")
 SOURCES = ["api.cu", "preprocess.cu", "binning.cu", "render_fwd.cu", "render_bwd.cu", "preprocess_bwd.cu", "epilogue.cu", "loss.cu", "decoder.cu", "point_feats.cu", "ms_ssim.cu", "mesh.cu", "fine_head.cu",
            "feat_volume.cu", "subset.cu", "vol_transformer.cu", "coarse_head.cu", "eval.cu",
-           "batch.cu", "finetune.cu"]
-HEADERS = ["surfel_common.cuh", "surfel_kernels.h", "det_sum.cuh", "fixed_sums.cuh", "mc_table.cuh", "sample_taps.cuh", "sh_eval.cuh", "decoder_layout.cuh",
+           "batch.cu", "finetune.cu", "image_encoder.cu"]
+HEADERS = ["surfel_common.cuh", "surfel_kernels.h", "det_sum.cuh", "fixed_sums.cuh", "layer_norm.cuh", "mc_table.cuh", "sample_taps.cuh", "sh_eval.cuh", "decoder_layout.cuh",
            os.path.join("..", "..", "include", "surfel_rasterizer.h"), os.path.join("..", "..", "include", "surfel_mesh.h"),
            os.path.join("..", "..", "include", "surfel_fine_head.h"),
            os.path.join("..", "..", "include", "surfel_feat_volume.h"),
@@ -32,7 +32,8 @@ HEADERS = ["surfel_common.cuh", "surfel_kernels.h", "det_sum.cuh", "fixed_sums.c
            os.path.join("..", "..", "include", "surfel_coarse_head.h"),
            os.path.join("..", "..", "include", "surfel_eval.h"),
            os.path.join("..", "..", "include", "surfel_batch.h"),
-           os.path.join("..", "..", "include", "surfel_finetune.h")]
+           os.path.join("..", "..", "include", "surfel_finetune.h"),
+           os.path.join("..", "..", "include", "surfel_image_encoder.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",

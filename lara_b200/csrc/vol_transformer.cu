@@ -10,16 +10,13 @@
 //                   dS_j = P_j (dO . v_j - Di), adds dS_j k_j into its dq, and stages P_j dO and dS_j q in shared
 //                   memory; after a barrier the CTA sums the staged rows over the bs^3 queries in query order into
 //                   dv[G, j] and dk[G, j] of its heads.  No atomics: every output element has one writer.
-// Residual add + LayerNorm, a warp per row of C <= 512 channels (C / 32 values per lane):
-//   ln_fwd_kernel   y = a + b, the mean, the centred variance (two passes over the registers), n = LN(y).
-//   ln_bwd_kernel   a CTA per block of 64 rows: recomputes the statistics from y, writes dL/da = dL/dy + the vjp,
-//                   and the block's dgamma / dbeta partials, its warps added in warp order.
-//   part_sums_kernel  the partials summed over the blocks in block order in fp64 (fixed_sums.cuh).
+// Residual add + LayerNorm: ln_fwd_kernel<16> / ln_bwd_kernel<16> of layer_norm.cuh (C <= 512).
 #include <math.h>
 #include <string.h>
 
 #include "../../include/surfel_vol_transformer.h"
 #include "fixed_sums.cuh"
+#include "layer_norm.cuh"
 #include "surfel_kernels.h"
 
 namespace srf {
@@ -27,8 +24,6 @@ namespace {
 
 constexpr int kGaMaxThreadCols = 4096;   // threads x D of an attention CTA: 2 x 16 KB of backward staging
 constexpr int kGaMaxS = 4096;
-constexpr int kLnWarps = 8;
-constexpr int kLnRows = 64;              // rows per CTA of the LayerNorm backward (one partial each)
 constexpr int kLnMaxJ = 16;              // C <= 512
 
 struct GaArgs {
@@ -165,102 +160,6 @@ __global__ void __launch_bounds__(256) ga_bwd_kernel(GaArgs a) {
     store_row<D>(a.gq + t.n * C + col, gq, a.scale);
 }
 
-struct LnArgs {
-    int rows, C;
-    float eps;
-    const float *a, *b, *gamma, *beta, *ys, *gn, *gy;    // ys: the backward's y
-    float *y, *n, *ga, *parts;
-};
-
-// mean and 1 / sqrt(var + eps) of the lane's nj values of a row of C
-__device__ __forceinline__ void ln_stats(const float* y, int nj, int C, float eps, float& mean, float& rstd) {
-    float s = 0.0f;
-#pragma unroll
-    for (int j = 0; j < kLnMaxJ; ++j)
-        if (j < nj) s += y[j];
-    mean = warp_sum(s) / (float)C;
-    float v = 0.0f;
-#pragma unroll
-    for (int j = 0; j < kLnMaxJ; ++j)
-        if (j < nj) { const float d = y[j] - mean; v = fmaf(d, d, v); }
-    rstd = 1.0f / sqrtf(warp_sum(v) / (float)C + eps);
-}
-
-__global__ void __launch_bounds__(kLnWarps * 32) ln_fwd_kernel(LnArgs a) {
-    const int lane = threadIdx.x & 31, row = blockIdx.x * kLnWarps + (threadIdx.x >> 5);
-    if (row >= a.rows) return;
-    const int C = a.C, nj = C / 32;
-    const size_t base = (size_t)row * C + lane;
-    float y[kLnMaxJ];
-#pragma unroll
-    for (int j = 0; j < kLnMaxJ; ++j)
-        if (j < nj) y[j] = a.b ? __ldg(a.a + base + 32 * j) + __ldg(a.b + base + 32 * j) : __ldg(a.a + base + 32 * j);
-    float mean, rstd;
-    ln_stats(y, nj, C, a.eps, mean, rstd);
-#pragma unroll
-    for (int j = 0; j < kLnMaxJ; ++j) {
-        if (j >= nj) continue;
-        const int c = lane + 32 * j;
-        if (a.y) a.y[base + 32 * j] = y[j];
-        a.n[base + 32 * j] = fmaf((y[j] - mean) * rstd, __ldg(a.gamma + c), __ldg(a.beta + c));
-    }
-}
-
-__global__ void __launch_bounds__(kLnWarps * 32) ln_bwd_kernel(LnArgs a) {
-    __shared__ float acc_s[2][kLnMaxJ * 32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, C = a.C, nj = C / 32;
-    const int r0 = blockIdx.x * kLnRows, r1 = min(r0 + kLnRows, a.rows);
-    float gam[kLnMaxJ], dg[kLnMaxJ], db[kLnMaxJ];
-#pragma unroll
-    for (int j = 0; j < kLnMaxJ; ++j) {
-        gam[j] = j < nj ? __ldg(a.gamma + lane + 32 * j) : 0.0f;
-        dg[j] = 0.0f;
-        db[j] = 0.0f;
-    }
-    for (int row = r0 + warp; row < r1; row += kLnWarps) {
-        const size_t base = (size_t)row * C + lane;
-        float y[kLnMaxJ], g[kLnMaxJ];
-#pragma unroll
-        for (int j = 0; j < kLnMaxJ; ++j)
-            if (j < nj) { y[j] = __ldg(a.ys + base + 32 * j); g[j] = __ldg(a.gn + base + 32 * j); }
-        float mean, rstd;
-        ln_stats(y, nj, C, a.eps, mean, rstd);
-        float s1 = 0.0f, s2 = 0.0f;
-#pragma unroll
-        for (int j = 0; j < kLnMaxJ; ++j) {
-            if (j >= nj) continue;
-            y[j] = (y[j] - mean) * rstd;                  // the normalised value from here on
-            dg[j] = fmaf(g[j], y[j], dg[j]);
-            db[j] += g[j];
-            g[j] *= gam[j];
-            s1 += g[j];
-            s2 = fmaf(g[j], y[j], s2);
-        }
-        const float m1 = warp_sum(s1) / (float)C, m2 = warp_sum(s2) / (float)C;
-#pragma unroll
-        for (int j = 0; j < kLnMaxJ; ++j) {
-            if (j >= nj) continue;
-            const float d = rstd * (g[j] - m1 - y[j] * m2);
-            a.ga[base + 32 * j] = a.gy ? __ldg(a.gy + base + 32 * j) + d : d;
-        }
-    }
-    // the warps' sums, added in warp order
-    for (int w = 0; w < kLnWarps; ++w) {
-        if (warp == w) {
-#pragma unroll
-            for (int j = 0; j < kLnMaxJ; ++j) {
-                if (j >= nj) continue;
-                const int c = lane + 32 * j;
-                acc_s[0][c] = w ? acc_s[0][c] + dg[j] : dg[j];
-                acc_s[1][c] = w ? acc_s[1][c] + db[j] : db[j];
-            }
-        }
-        __syncthreads();
-    }
-    float* part = a.parts + (size_t)blockIdx.x * 2 * C;
-    for (int e = threadIdx.x; e < 2 * C; e += kLnWarps * 32) part[e] = acc_s[e / C][e % C];
-}
-
 bool misaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
 
 // the heads per CTA: the largest divisor Hs of H with bs^3 Hs D <= kGaMaxThreadCols
@@ -352,12 +251,7 @@ extern "C" int srf_add_layernorm_forward(void* stream_, int rows, int C, float e
     if (srf::ln_check(fn, rows, C, eps)) return 1;
     if (!a || !gamma || !beta || !n) return set_error("%s: null pointer", fn);
     if (b && !y) return set_error("%s: null y with a residual b", fn);
-    if (rows == 0) return 0;
-    srf::LnArgs la;
-    memset(&la, 0, sizeof(la));
-    la.rows = rows; la.C = C; la.eps = eps; la.a = a; la.b = b; la.gamma = gamma; la.beta = beta; la.y = y; la.n = n;
-    const unsigned grid = (unsigned)((rows + srf::kLnWarps - 1) / srf::kLnWarps);
-    srf::ln_fwd_kernel<<<grid, srf::kLnWarps * 32, 0, static_cast<cudaStream_t>(stream_)>>>(la);
+    srf::ln_forward<srf::kLnMaxJ>(static_cast<cudaStream_t>(stream_), rows, C, eps, a, b, gamma, beta, y, n);
     const cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? 0 : cuda_error("add_layernorm forward launch", e);
 }
@@ -366,8 +260,7 @@ extern "C" int srf_add_layernorm_workspace_bytes(int rows, int C, size_t* bytes)
     const char* fn = "srf_add_layernorm_workspace_bytes";
     if (srf::ln_check(fn, rows, C, 1.0f)) return 1;
     if (!bytes) return set_error("%s: null output", fn);
-    const size_t nparts = ((size_t)rows + srf::kLnRows - 1) / srf::kLnRows;
-    *bytes = srf::align_up(sizeof(float) * 2 * (size_t)C * (nparts ? nparts : 1));
+    *bytes = srf::align_up(srf::ln_parts_bytes(rows, C));
     return 0;
 }
 
@@ -379,17 +272,8 @@ extern "C" int srf_add_layernorm_backward(void* stream_, int rows, int C, float 
     if (!y || !gamma || !dL_dn) return set_error("%s: null input pointer", fn);
     if (!dL_da || !d_gamma || !d_beta) return set_error("%s: null gradient pointer", fn);
     if (!workspace || srf::misaligned(workspace)) return set_error("%s: workspace must be 256-byte aligned", fn);
-    const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    const int nparts = (rows + srf::kLnRows - 1) / srf::kLnRows;
-    if (nparts > 0) {
-        srf::LnArgs la;
-        memset(&la, 0, sizeof(la));
-        la.rows = rows; la.C = C; la.eps = eps; la.ys = y; la.gamma = gamma; la.gn = dL_dn; la.gy = dL_dy;
-        la.ga = dL_da; la.parts = static_cast<float*>(workspace);
-        srf::ln_bwd_kernel<<<(unsigned)nparts, srf::kLnWarps * 32, 0, stream>>>(la);
-    }
-    srf::part_sums(stream, static_cast<const float*>(workspace), nparts, 2 * (size_t)C, srf::seg(d_gamma, C),
-                   srf::seg(d_beta, C));
+    srf::ln_backward<srf::kLnMaxJ>(static_cast<cudaStream_t>(stream_), rows, C, eps, y, gamma, dL_dn, dL_dy,
+                                   static_cast<float*>(workspace), dL_da, d_gamma, d_beta);
     const cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? 0 : cuda_error("add_layernorm backward launch", e);
 }

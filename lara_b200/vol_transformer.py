@@ -69,11 +69,13 @@ class _GroupAttn(torch.autograd.Function):
 
 
 class _AddLayerNorm(torch.autograd.Function):
-    """(a, b or None, gamma, beta, eps) -> (y = a + b, n = LN(y)), or n = LN(a) when b is None."""
+    """(a, b or None, gamma, beta, eps, entry) -> (y = a + b, n = LN(y)), or n = LN(a) when b is None, on the C entries
+    ``{entry}_forward`` / ``_workspace_bytes`` / ``_backward``: ``srf_add_layernorm`` (C <= 512) or
+    ``srf_vit_layernorm`` (C in {384, 768})."""
 
     @staticmethod
     @torch.amp.custom_fwd(device_type="cuda", cast_inputs=torch.float32)
-    def forward(ctx, a, b, gamma, beta, eps):
+    def forward(ctx, a, b, gamma, beta, eps, entry="srf_add_layernorm"):
         a = a.contiguous()
         C = int(a.shape[-1])
         rows = a.numel() // C
@@ -81,11 +83,11 @@ class _AddLayerNorm(torch.autograd.Function):
         y = torch.empty_like(a) if b is not None else None
         if b is not None:
             b = b.contiguous()
-        _lib.launch("srf_add_layernorm_forward", a.device, rows, C, eps, a.data_ptr(),
+        _lib.launch(entry + "_forward", a.device, rows, C, eps, a.data_ptr(),
                     b.data_ptr() if b is not None else None, gamma.data_ptr(), beta.data_ptr(),
                     y.data_ptr() if y is not None else None, n.data_ptr())
         ctx.save_for_backward(y if y is not None else a, gamma)
-        ctx.eps, ctx.has_b = eps, b is not None
+        ctx.eps, ctx.has_b, ctx.entry = eps, b is not None, entry
         return (y, n) if b is not None else n
 
     @staticmethod
@@ -100,12 +102,12 @@ class _AddLayerNorm(torch.autograd.Function):
         ga = torch.empty_like(y)
         g_gamma, g_beta = torch.empty_like(gamma), torch.empty_like(gamma)
         with _lib._DeviceGuard(y.device):
-            nbytes = _lib.add_layernorm_workspace_bytes(_lib.load(), rows, C)
+            nbytes = _lib.layernorm_workspace_bytes(_lib.load(), ctx.entry, rows, C)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=y.device)
-        _lib.launch("srf_add_layernorm_backward", y.device, rows, C, ctx.eps, y.data_ptr(), gamma.data_ptr(),
+        _lib.launch(ctx.entry + "_backward", y.device, rows, C, ctx.eps, y.data_ptr(), gamma.data_ptr(),
                     gn.data_ptr(), gy.data_ptr() if gy is not None else None, ws.data_ptr(), ga.data_ptr(),
                     g_gamma.data_ptr(), g_beta.data_ptr())
-        return ga, (ga if ctx.has_b else None), g_gamma, g_beta, None
+        return ga, (ga if ctx.has_b else None), g_gamma, g_beta, None, None
 
 
 def add_layer_norm(a, b, norm: nn.LayerNorm, fn="add_layer_norm"):
