@@ -110,11 +110,14 @@ def dot(pairs) -> EB:
     return sum_any_order([mul(a, b) for a, b in pairs])
 
 
-def source_coord(xs: EB, size: int) -> EB:
-    """network.py:401, then grid_sample's unnormalisation (align_corners=False), one rounding per torch operation."""
-    b = div(add(xs, 0.5), float(size))
+def source_coord(xs: EB, image_size: int, map_size: int = None) -> EB:
+    """network.py:401 (the normalisation by the image size), then grid_sample's unnormalisation onto a map of map_size
+    pixels (align_corners=False), one rounding per torch operation: sample_taps.cuh's pf_source_coord.  The point
+    sampler samples maps of the image's size."""
+    map_size = image_size if map_size is None else map_size
+    b = div(add(xs, 0.5), float(image_size))
     g = add(scale(b, 2.0), -1.0)
-    return scale(add(mul(add(g, 1.0), float(size)), -1.0), 0.5)
+    return scale(add(mul(add(g, 1.0), float(map_size)), -1.0), 0.5)
 
 
 def _f64(a):
@@ -126,9 +129,10 @@ def _f64(a):
 # --------------------------------------------------------------------------------------------------------- one view
 
 class _View:
-    """One source view: the projection of every point with its bound, and the decisions of floor(ix), floor(iy)."""
+    """One source view: the projection of every point with its bound, and the decisions of floor(ix), floor(iy) on a
+    W x H map (of an image of W_img x H_img pixels, by default the map's size)."""
 
-    def __init__(self, pts, E, Km, W, H):
+    def __init__(self, pts, E, Km, W, H, W_img=None, H_img=None):
         x = [EB(pts[:, k]) for k in range(3)]
         q = [sum_any_order([mul(x[0], E[r, 0]), mul(x[1], E[r, 1]), mul(x[2], E[r, 2]), EB.w(E[r, 3])])
              for r in range(3)]
@@ -136,7 +140,8 @@ class _View:
         self.pz = p[2]
         self.xs, self.ys = div(p[0], p[2]), div(p[1], p[2])
         self.zero = _zero(p[2])                       # z = 0 exactly: coordinates not finite, decided
-        self.ix, self.iy = source_coord(self.xs, W), source_coord(self.ys, H)
+        self.ix = source_coord(self.xs, W if W_img is None else W_img, W)
+        self.iy = source_coord(self.ys, H if H_img is None else H_img, H)
         self.ax = self._axis(self.ix, W)
         self.ay = self._axis(self.iy, H)
         with np.errstate(invalid="ignore"):
@@ -196,18 +201,79 @@ class _Hull:
             self.lo, self.hi, self.r = np.minimum(self.lo, x.v), np.maximum(self.hi, x.v), np.maximum(self.r, x.e)
 
 
-def _eval(planes, vw, idx, xs, ys, signs, g, W, H, want_grad, Km, E, only_d=False):
-    """Evaluate the pairs idx at every (x side, y side, sign) combination.  planes [8,H*W] float64 of the view,
-    g [8,n] the view's upstream (or None).  Returns hulls of the features [8], the stencil weights [9] (3x3 around the
-    lower candidate cell) and touch flags, d = s_depth - z, and the point gradient [3]."""
+def _valid(cx, cy, W, H):
+    """The four taps' in-image tests of the cells (cx, cy)."""
+    return [(cx + _DX[k] >= 0) & (cx + _DX[k] <= W - 1) & (cy + _DY[k] >= 0) & (cy + _DY[k] <= H - 1) for k in range(4)]
+
+
+def _stencil_hull(vw, idx, xs, ys, W, H):
+    """Hulls, over every (x side, y side) combination of the pairs idx, of the weight each slot of the 3x3 stencil
+    around the lower candidate cell (cA, cA) receives (0 where a combination's taps miss the slot), and the slots some
+    combination taps."""
     m = idx.size
     baseX, baseY = vw.ax["cA"][idx], vw.ay["cA"][idx]
+    exx, exy = vw.ax["ex"][idx], vw.ay["ex"][idx]
+    wst = [_Hull() for _ in range(9)]
+    touched = np.zeros((9, m), bool)
+    for cx, px in xs:
+        for cy, py in ys:
+            tx0, tx1, ty0, ty1 = _weights(cx, px, exx, cy, py, exy)
+            w = [mul(tx1, ty1), mul(tx0, ty1), mul(tx1, ty0), mul(tx0, ty0)]
+            valid = _valid(cx, cy, W, H)
+            sv, se = np.zeros((9, m)), np.zeros((9, m))
+            for k in range(4):
+                slot = ((cy - baseY + _DY[k]) * 3 + (cx - baseX + _DX[k])).astype(np.int64)
+                for s_ in range(9):
+                    here = valid[k] & (slot == s_)
+                    touched[s_] |= here
+                    sv[s_] = np.where(here, w[k].v, sv[s_])
+                    se[s_] = np.where(here, w[k].e, se[s_])
+            for s_ in range(9):
+                wst[s_].add(EB(sv[s_], se[s_]))
+    return wst, touched
+
+
+def stencil(vw, W, H, und):
+    """The tap weight each slot s of the 3x3 stencil around every pair's lower candidate cell receives, for both
+    statements: ``touched`` [9,n] (some side of the pair's box taps the slot), the slot's pixel ``X``, ``Y`` [9,n]
+    (cA + s % 3, cA + s // 3), and the weight as a value ``v`` with its spread ``d`` over the box and a rounding bound
+    ``r`` [9,n]: any weight an fp32 evaluation gives lies within v +- (d + r).  A decided pair (und False) takes the
+    value at the float64 coordinates and the corners' largest distance from it; an undecided one the hull of every
+    side, its midpoint and half-range."""
+    n = vw.ax["v"].size
+    allidx = np.arange(n)
+    c0x, c0y = vw.ax["c0"], vw.ay["c0"]
+    cen, _ = _stencil_hull(vw, allidx, [(c0x, np.clip(vw.ax["v"], c0x, c0x + 1))],
+                           [(c0y, np.clip(vw.ay["v"], c0y, c0y + 1))], W, H)
+    out = {k: np.zeros((9, n)) for k in ("v", "d", "r")}
+    out["touched"] = np.zeros((9, n), bool)
+    for sub, u in ((allidx[~und], False), (allidx[und], True)):
+        if sub.size == 0:
+            continue
+        hull, touched = _stencil_hull(vw, sub, _positions(vw.ax, sub, u), _positions(vw.ay, sub, u), W, H)
+        for s_ in range(9):
+            h = hull[s_]
+            out["touched"][s_, sub] = touched[s_]
+            if u:
+                out["v"][s_, sub], out["d"][s_, sub], out["r"][s_, sub] = 0.5 * (h.lo + h.hi), 0.5 * (h.hi - h.lo), h.r
+            else:
+                c = cen[s_].lo[sub]
+                out["v"][s_, sub], out["d"][s_, sub] = c, np.maximum(h.hi - c, c - h.lo)
+                out["r"][s_, sub] = np.maximum(h.r, cen[s_].r[sub])
+    s = np.arange(9)[:, None]
+    out["X"], out["Y"] = vw.ax["cA"][None] + s % 3, vw.ay["cA"][None] + s // 3
+    return out
+
+
+def _eval(planes, vw, idx, xs, ys, signs, g, W, H, want_grad, Km, E, only_d=False):
+    """Evaluate the pairs idx at every (x side, y side, sign) combination.  planes [8,H*W] float64 of the view,
+    g [8,n] the view's upstream (or None).  Returns hulls of the features [8], d = s_depth - z, and the point gradient
+    [3]."""
+    m = idx.size
     exx, exy = vw.ax["ex"][idx], vw.ay["ex"][idx]
     pz = EB(vw.pz.v[idx], vw.pz.e[idx])
     xsE, ysE = EB(vw.xs.v[idx], vw.xs.e[idx]), EB(vw.ys.v[idx], vw.ys.e[idx])
     feats = [_Hull() for _ in range(8)]
-    wst = [_Hull() for _ in range(9)]
-    touched = np.zeros((9, m), bool)
     dh = _Hull()
     grad = [_Hull() for _ in range(3)]
     Wf, Hf = float(W), float(H)
@@ -215,13 +281,11 @@ def _eval(planes, vw, idx, xs, ys, signs, g, W, H, want_grad, Km, E, only_d=Fals
         for cy, py in ys:
             tx0, tx1, ty0, ty1 = _weights(cx, px, exx, cy, py, exy)
             w = [mul(tx1, ty1), mul(tx0, ty1), mul(tx1, ty0), mul(tx0, ty0)]
-            valid, vals = [], []
+            valid = _valid(cx, cy, W, H)
+            vals = []
             for k in range(4):
-                X, Y = cx + _DX[k], cy + _DY[k]
-                ok = (X >= 0) & (X <= W - 1) & (Y >= 0) & (Y <= H - 1)
-                off = np.where(ok, Y * W + X, 0).astype(np.int64)
-                valid.append(ok)
-                vals.append(np.where(ok[None], planes[:, off], 0.0))         # [8, m]
+                off = np.where(valid[k], (cy + _DY[k]) * W + cx + _DX[k], 0).astype(np.int64)
+                vals.append(np.where(valid[k][None], planes[:, off], 0.0))         # [8, m]
             any_ = (((cx >= 0) & (cx <= W - 1)) | ((cx >= -1) & (cx <= W - 2))) & \
                 (((cy >= 0) & (cy <= H - 1)) | ((cy >= -1) & (cy <= H - 2)))
             samp = []
@@ -236,17 +300,6 @@ def _eval(planes, vw, idx, xs, ys, signs, g, W, H, want_grad, Km, E, only_d=Fals
                 continue
             for c in range(7):
                 feats[c].add(samp[c])
-            # the weight each of the 3x3 slots receives; a slot no tap of this combination touches receives 0
-            sv, se = np.zeros((9, m)), np.zeros((9, m))
-            for k in range(4):
-                slot = ((cy - baseY + _DY[k]) * 3 + (cx - baseX + _DX[k])).astype(np.int64)
-                for s_ in range(9):
-                    here = valid[k] & (slot == s_)
-                    touched[s_] |= here
-                    sv[s_] = np.where(here, w[k].v, sv[s_])
-                    se[s_] = np.where(here, w[k].e, se[s_])
-            for s_ in range(9):
-                wst[s_].add(EB(sv[s_], se[s_]))
             if not want_grad:
                 continue
             for sg in signs:
@@ -271,7 +324,7 @@ def _eval(planes, vw, idx, xs, ys, signs, g, W, H, want_grad, Km, E, only_d=Fals
         h = feats[7]
         h.hi, h.r = np.maximum(np.abs(dh.lo), np.abs(dh.hi)), dh.r
         h.lo = np.where((dh.lo <= 0) & (dh.hi >= 0), 0.0, np.minimum(np.abs(dh.lo), np.abs(dh.hi)))
-    return dict(feats=feats, w=wst, touched=touched, d=dh, grad=grad, baseX=baseX, baseY=baseY)
+    return dict(feats=feats, d=dh, grad=grad)
 
 
 def _sign_set(d: _Hull):
@@ -362,23 +415,14 @@ def point_feats64(points, w2cs, ixts, img_ref, image, acc, depth, g_feats=None):
             a, b = combine("grad", k)
             gp[k].append(EB(a, np.where(vw.inf, np.inf, b)))
         # rendering gradients: per (pair, slot) the tap weight's hull, times each channel's upstream
-        for u, (sub, r) in res.items():
+        st = stencil(vw, W, H, und)
+        for u in (False, True):
             for s_ in range(9):
-                t = r["touched"][s_]
-                if not t.any():
+                i = np.nonzero(st["touched"][s_] & (und == u))[0]
+                if i.size == 0:
                     continue
-                i = sub[t]
-                h = r["w"][s_]
-                if u:
-                    wv = 0.5 * (h.lo + h.hi)[t]
-                    wd = 0.5 * (h.hi - h.lo)[t]
-                else:
-                    c = cen["w"][s_].lo[i]
-                    wv, wd = c, np.maximum(h.hi[t] - c, c - h.lo[t])
-                wr = np.maximum(h.r[t], cen["w"][s_].r[i]) if not u else h.r[t]
-                X = r["baseX"][t] + s_ % 3
-                Y = r["baseY"][t] + s_ // 3
-                pix = (Y * W + X).astype(np.int64)
+                wv, wd, wr = st["v"][s_, i], st["d"][s_, i], st["r"][s_, i]
+                pix = (st["Y"][s_, i] * W + st["X"][s_, i]).astype(np.int64)
                 for c in range(3, 8):
                     go = g[v, c, i]
                     if c < 7:
