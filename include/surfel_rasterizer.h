@@ -290,6 +290,32 @@ int srf_point_feats_backward(srf_stream_t stream, int V, int n, int H, int W,
                              const float* g_feats, float* g_points, float* g_image, float* g_acc, float* g_depth,
                              void* workspace);
 int srf_point_feats_deterministic_workspace_bytes(int V, int H, int W, size_t* bytes);
+/* The same over the S scenes of a batch in one launch per direction (DESIGN §3.26).  Scene s's points are
+ * [offsets[s], offsets[s+1]) of the n points (`offsets`: HOST int64 [S+1], from 0, non-decreasing, ending at n, at most
+ * P per scene; checked without waiting for the stream).  Point i's centre is row rows[i] of centers [S*P,3] (`rows`
+ * [n] int32, the global row b*P + index; NULL: row i, with n <= S*P); a row outside [0, S*P) is never read: that
+ * point's features are 0 and it gets no gradient.  Scene s's Vs source views use cameras w2cs / ixts [S*Vs,...] at
+ * s*Vs + v, img_ref [S,Vs,3,H,W] at the element strides of `img_ref_addr` (host; any layout, e.g. a channel-last view),
+ * and the renderings image [S*Vr,3,H,W], acc and depth [S*Vr,H,W] at view s*Vr + v, Vr >= Vs (a batch render's own
+ * planar outputs).  feats [Vs,8,n] as above.  The backward writes g_centers [S*P,3] (the points' rows: their sum over
+ * the views; every other row 0; no atomics) and the rendering gradients in the full [S*Vr,...] planes (0 for views
+ * v >= Vs).  Per point, the float operations are those of the one-scene call; with a `workspace`
+ * (srf_point_feats_scenes_deterministic_workspace_bytes(S, Vs, H, W)) each scene's rendering gradients are summed under
+ * its own fixed-point scale, so they equal the one-scene call's on that scene bit for bit.  srf_point_feats_forward /
+ * _backward are this with S = 1, rows NULL, Vr = V and a contiguous img_ref.  0 < S <= SRF_MAX_SCENES, S*P < 2^31. */
+typedef struct srf_pf_image_addr { int64_t ss, sv, sc, sy, sx; } srf_pf_image_addr;
+int srf_point_feats_scenes_forward(srf_stream_t stream, int S, int Vs, int Vr, int P, int n, int H, int W,
+                                   const int64_t* offsets, const int32_t* rows, const float* centers,
+                                   const float* w2cs, const float* ixts, const float* img_ref,
+                                   const srf_pf_image_addr* img_ref_addr, const float* image, const float* acc,
+                                   const float* depth, float* feats);
+int srf_point_feats_scenes_backward(srf_stream_t stream, int S, int Vs, int Vr, int P, int n, int H, int W,
+                                    const int64_t* offsets, const int32_t* rows, const float* centers,
+                                    const float* w2cs, const float* ixts, const float* img_ref,
+                                    const srf_pf_image_addr* img_ref_addr, const float* image, const float* acc,
+                                    const float* depth, const float* g_feats, float* g_centers, float* g_image,
+                                    float* g_acc, float* g_depth, void* workspace);
+int srf_point_feats_scenes_deterministic_workspace_bytes(int S, int Vs, int H, int W, size_t* bytes);
 
 /* ---- fused MS-SSIM (next-row: lightning/loss.py:44-47, pytorch-msssim 1.0.0 MS_SSIM, channel = C) -------------
  * The 5-level MS-SSIM of X (rendering) and Y (target), logical images B x C x H x W, with the library's valid 11-tap

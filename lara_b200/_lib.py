@@ -27,6 +27,11 @@ class MsSsimAddr(Structure):
     _fields_ = [("sb", c_int64), ("sc", c_int64), ("sy", c_int64), ("sx", c_int64), ("sv", c_int64), ("wv", c_int64)]
 
 
+class PfImageAddr(Structure):
+    """srf_pf_image_addr: element strides (ss, sv, sc, sy, sx) of img_ref [S,Vs,3,H,W]."""
+    _fields_ = [("ss", c_int64), ("sv", c_int64), ("sc", c_int64), ("sy", c_int64), ("sx", c_int64)]
+
+
 _A = POINTER(MsSsimAddr)
 _I3 = POINTER(c_int)            # host int[3]
 _P5 = POINTER(c_void_p)         # host void*[5]
@@ -90,6 +95,16 @@ SIGNATURES = {
     "srf_point_feats_backward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
                                          _P]),
     "srf_point_feats_deterministic_workspace_bytes": (c_int, [c_int, c_int, c_int, POINTER(c_size_t)]),
+    "srf_point_feats_scenes_forward": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, c_int,  # stream .. n, H, W
+                                               _P, _P, _P, _P, _P,        # offsets (host), rows, centers, w2cs, ixts
+                                               _P, POINTER(PfImageAddr),  # img_ref and its strides (host)
+                                               _P, _P, _P, _P]),          # image, acc, depth, feats
+    "srf_point_feats_scenes_backward": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                                _P, _P, _P, _P, _P,
+                                                _P, POINTER(PfImageAddr),
+                                                _P, _P, _P, _P,           # image, acc, depth, g_feats
+                                                _P, _P, _P, _P, _P]),     # g_centers, g_image, g_acc, g_depth, workspace
+    "srf_point_feats_scenes_deterministic_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, POINTER(c_size_t)]),
     "srf_ms_ssim_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, POINTER(c_size_t)]),
     "srf_ms_ssim_workspace_layout": (c_int, [c_int, c_int, c_int, c_int, POINTER(c_size_t), POINTER(c_size_t),
                                              POINTER(c_int)]),
@@ -326,6 +341,10 @@ def eval_workspace_bytes(lib) -> int:
 
 def det_point_feats_workspace_bytes(lib, V: int, H: int, W: int) -> int:
     return _size_query(lib.srf_point_feats_deterministic_workspace_bytes, V, H, W)
+
+
+def det_point_feats_scenes_workspace_bytes(lib, S: int, Vs: int, H: int, W: int) -> int:
+    return _size_query(lib.srf_point_feats_scenes_deterministic_workspace_bytes, S, Vs, H, W)
 
 
 def det_loss_workspace_bytes(lib, V: int, H: int, W: int) -> int:

@@ -10,6 +10,7 @@ struct PfTaps {
     float tx0, tx1, ty0, ty1;    // ix - floor(ix), floor(ix) + 1 - ix, same for y
     float w[4];                  // nw, ne, sw, se
     int off[4];                  // y * W + x of each tap, -1 = not used
+    int xi, yi;                  // the nw tap's pixel (0 on an axis where neither tap column / row is in the image)
     bool any;
 };
 
@@ -54,6 +55,7 @@ __device__ __forceinline__ PfTaps pf_taps(float ix, float iy, int W, int H) {
     const bool x0 = fx >= 0.0f && fx <= (float)(W - 1), x1 = fx >= -1.0f && fx <= (float)(W - 2);
     const bool y0 = fy >= 0.0f && fy <= (float)(H - 1), y1 = fy >= -1.0f && fy <= (float)(H - 2);
     const int xi = (x0 || x1) ? (int)fx : 0, yi = (y0 || y1) ? (int)fy : 0;
+    t.xi = xi; t.yi = yi;
     t.off[0] = (x0 && y0) ? yi * W + xi : -1;
     t.off[1] = (x1 && y0) ? yi * W + xi + 1 : -1;
     t.off[2] = (x0 && y1) ? (yi + 1) * W + xi : -1;

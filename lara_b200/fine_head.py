@@ -132,17 +132,25 @@ class FineHead(nn.Module):
         pf = point_feats.permute(1, 2, 0).contiguous()      # the kernel reads [V,8,n]
         return _FineHead.apply(volume_feat, pf, None, None, 1, *params).unsqueeze(1)
 
-    def fine_shs(self, volume_feat_up: torch.Tensor, K: int, mask: torch.Tensor, point_feats: torch.Tensor,
+    def fine_shs(self, volume_feat_up: torch.Tensor, K: int, mask, point_feats: torch.Tensor,
                  shs_coarse: torch.Tensor) -> torch.Tensor:
         """network.py:508-512 in one call: ``_shs_fine`` [n,M,3] of the masked Gaussians.
 
-        volume_feat_up [N,D] (one scene's voxel features), K Gaussians per voxel, mask [N*K] bool (after
+        One scene: volume_feat_up [N,D] (its voxel features), K Gaussians per voxel, mask [N*K] bool (after
         ``_check_mask``), point_feats [V,8,n] (``sample_point_feats``' output for those n Gaussians), shs_coarse
-        [N*K,M,3] with 3 M = sh_dim."""
+        [N*K,M,3] with 3 M = sh_dim.
+
+        All B scenes of a batch in one call: volume_feat_up [B,N,D], ``mask`` the
+        :class:`lara_b200.multiview.FineSubset` of the masks [B,N*K] (or those masks), point_feats [V,8,n]
+        (``sample_batch_point_feats``' output) and shs_coarse [B,N*K,M,3]; returns [n,M,3] in scene order, what
+        ``render_batch_subset_views`` takes.  Each row is bit for bit the one-scene call's; the parameter gradients are
+        summed over all scenes at once."""
         fn = "FineHead.fine_shs"
         D, S = self.in_dim, self.sh_dim
         if isinstance(K, bool) or not isinstance(K, int) or K < 1:
             raise RuntimeError(f"{fn}: K must be a positive int, got {K!r}")
+        if volume_feat_up.ndim == 3:
+            return self._fine_shs_batch(fn, volume_feat_up, K, mask, point_feats, shs_coarse)
         if volume_feat_up.ndim != 2 or volume_feat_up.shape[1] != D:
             raise RuntimeError(f"{fn}: volume_feat_up must be [N,{D}], got {tuple(volume_feat_up.shape)}")
         NK = int(volume_feat_up.shape[0]) * K
@@ -151,8 +159,7 @@ class FineHead(nn.Module):
                                f"{tuple(mask.shape)}")
         if tuple(shs_coarse.shape) != (NK, S // 3, 3):
             raise RuntimeError(f"{fn}: shs_coarse must be {(NK, S // 3, 3)}, got {tuple(shs_coarse.shape)}")
-        if point_feats.ndim != 3 or point_feats.shape[1] != COND or not 1 <= point_feats.shape[0] <= 8:
-            raise RuntimeError(f"{fn}: point_feats must be [V,8,n] with 1 <= V <= 8, got {tuple(point_feats.shape)}")
+        self._check_point_feats(fn, point_feats)
         if NK >= 2 ** 31:
             raise RuntimeError(f"{fn}: N*K = {NK} is over the int32 index range")
         params = self._prepared(fn, volume_feat_up, point_feats, shs_coarse)
@@ -163,6 +170,53 @@ class FineHead(nn.Module):
         if point_feats.shape[2] != n:
             raise RuntimeError(f"{fn}: point_feats has {point_feats.shape[2]} points but mask selects {n}")
         out = _FineHead.apply(volume_feat_up, point_feats, shs_coarse.reshape(NK, S), idx, K, *params)
+        return out.view(n, S // 3, 3)
+
+    @staticmethod
+    def _check_point_feats(fn, point_feats):
+        if not isinstance(point_feats, torch.Tensor) or point_feats.ndim != 3 or point_feats.shape[1] != COND or \
+                not 1 <= point_feats.shape[0] <= 8:
+            raise RuntimeError(f"{fn}: point_feats must be [V,8,n] with 1 <= V <= 8, got "
+                               f"{tuple(getattr(point_feats, 'shape', ()))}")
+
+    def _fine_shs_batch(self, fn, volume_feat_up, K, subset, point_feats, shs_coarse):
+        """The batch form of :meth:`fine_shs`: the subset's global rows b*N*K + i index the flattened [B*N*K] Gaussians,
+        so the kernel's voxel row, row // K, is b*N + i // K of the flattened [B*N, D] features."""
+        from .multiview import FineSubset
+        D, S = self.in_dim, self.sh_dim
+        if volume_feat_up.shape[2] != D:
+            raise RuntimeError(f"{fn}: volume_feat_up must be [B,N,{D}], got {tuple(volume_feat_up.shape)}")
+        B, N = int(volume_feat_up.shape[0]), int(volume_feat_up.shape[1])
+        NK = N * K
+        if isinstance(subset, torch.Tensor):
+            if subset.dtype != torch.bool or tuple(subset.shape) != (B, NK):
+                raise RuntimeError(f"{fn}: masks must be a bool tensor of shape ({B}, {NK}), got {subset.dtype} "
+                                   f"{tuple(subset.shape)}")
+            if B * NK >= 2 ** 31:
+                raise RuntimeError(f"{fn}: B*N*K = {B * NK} is over the int32 index range")
+            if not subset.is_cuda or subset.device != volume_feat_up.device:
+                raise RuntimeError(f"{fn}: masks must be a CUDA tensor on {volume_feat_up.device}, got {subset.device}")
+            subset = FineSubset(subset)
+        elif not isinstance(subset, FineSubset):
+            raise RuntimeError(f"{fn}: with volume_feat_up [B,N,D], mask must be a FineSubset or bool masks [B,N*K], "
+                               f"got {type(subset).__name__}")
+        if (subset.scenes, subset.P) != (B, NK):
+            raise RuntimeError(f"{fn}: the subset's masks are [{subset.scenes},{subset.P}], expected [{B},{NK}]")
+        if B * NK >= 2 ** 31:
+            raise RuntimeError(f"{fn}: B*N*K = {B * NK} is over the int32 index range")
+        if tuple(shs_coarse.shape) != (B, NK, S // 3, 3):
+            raise RuntimeError(f"{fn}: shs_coarse must be {(B, NK, S // 3, 3)}, got {tuple(shs_coarse.shape)}")
+        self._check_point_feats(fn, point_feats)
+        params = self._prepared(fn, volume_feat_up, point_feats, shs_coarse)
+        if subset.rows.device != volume_feat_up.device:
+            raise RuntimeError(f"{fn}: the subset is on {subset.rows.device}, volume_feat_up on {volume_feat_up.device}")
+        n = subset.n
+        if point_feats.shape[2] != n:
+            raise RuntimeError(f"{fn}: point_feats has {point_feats.shape[2]} points but the masks select {n}")
+        if n == 0:          # nothing selected: no launch, an empty result that still leads back to shs_coarse
+            return shs_coarse.reshape(B * NK, S // 3, 3)[:0]
+        out = _FineHead.apply(volume_feat_up.reshape(B * N, D), point_feats, shs_coarse.reshape(B * NK, S),
+                              subset.rows, K, *params)
         return out.view(n, S // 3, 3)
 
     def _prepared(self, fn, *inputs):

@@ -21,6 +21,7 @@ from __future__ import annotations
 
 from typing import Dict, Optional, Sequence
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -298,35 +299,85 @@ class _RenderSubsetViews(torch.autograd.Function):
                 scatter(g["rotations"], tuple(rotations.shape)))
 
 
-def _render_subset(fn, binning: SceneBinning, masks, shs_fine):
-    """The subset render of every scene of ``binning`` (checked, unchanged) with ``masks`` [S,P] (checked) and
-    ``shs_fine`` [n,M,3]; ``fn`` names the caller in messages.  Returns the outputs of :func:`_subset_forward` and the
-    per-scene counts.  One host sync, for the counts."""
+_F32_RATIO_LOW, _F32_RATIO_HIGH = np.float32(1e-3), np.float32(0.5)     # LaRa's thresholds as torch compares them
+
+
+class FineSubset:
+    """One compaction of the fine pass's masks [B,P] bool, shared by the point features, the fine head and the subset
+    render: ``counts`` (host list, one read of ``masks.sum(1)``), ``offsets`` (host list [B+1]), ``offsets_d`` (the same
+    on the device, int64, None for B = 1), ``nz`` the (scene, index) pairs [n,2] scene-major and ascending within a
+    scene, ``idx`` their indices and ``rows`` the global rows b*P + index as int32.  ``masks`` are the masks the subset
+    was built from.
+
+    ``check=True`` first applies LaRa's ``Network._check_mask`` (lightning/network.py:381-388) to each scene in scene
+    order, with the same ``torch.rand`` draws where LaRa draws, so that under one seed the masks are LaRa's bit for bit:
+    the ratio is fp32(count) / fp32(P) compared with 1e-3 and 0.5 in fp32, as torch computes ``torch.sum(mask) /
+    np.prod(mask.shape)``; a sparse scene becomes ``(mask + r) > 0.8`` and, with ``training``, a dense one
+    ``(mask * r) > 0.5``.  The counts are read a second time only if some scene took a branch."""
+    __slots__ = ("masks", "counts", "offsets", "offsets_d", "nz", "idx", "rows", "scenes", "P", "n")
+
+    def __init__(self, masks: torch.Tensor, check: bool = False, training: bool = False):
+        if not isinstance(masks, torch.Tensor) or masks.dtype != torch.bool or masks.ndim != 2:
+            raise RuntimeError(f"FineSubset: masks must be a bool tensor [B,P], got {getattr(masks, 'dtype', type(masks))} "
+                               f"{tuple(getattr(masks, 'shape', ()))}")
+        B, P = (int(x) for x in masks.shape)
+        if B < 1:
+            raise RuntimeError("FineSubset: masks must hold at least one scene")
+        if B * P >= 2 ** 31:
+            raise RuntimeError(f"FineSubset: B*P = {B * P} rows are over the int32 index range")
+        counts_d = masks.sum(1)
+        counts = [int(c) for c in counts_d.tolist()]          # the host read
+        if check:
+            checked, changed = [], False
+            for b, c in enumerate(counts):
+                mask = masks[b]
+                ratio = np.float32(c) / np.float32(P) if P else np.float32(np.nan)
+                if ratio < _F32_RATIO_LOW:
+                    mask = mask + torch.rand(mask.shape, device=mask.device) > 0.8
+                    changed = True
+                elif ratio > _F32_RATIO_HIGH and training:
+                    mask = mask * torch.rand(mask.shape, device=mask.device) > 0.5
+                    changed = True
+                checked.append(mask)
+            if changed:
+                masks = torch.stack(checked)
+                counts_d = masks.sum(1)
+                counts = [int(c) for c in counts_d.tolist()]      # the second host read
+        n = sum(counts)
+        self.masks, self.counts, self.scenes, self.P, self.n = masks, counts, B, P, n
+        self.offsets = [0]
+        for c in counts:
+            self.offsets.append(self.offsets[-1] + c)
+        self.nz = torch.nonzero_static(masks, size=n)        # (scene, index) pairs, scene-major, ascending in a scene
+        self.idx = self.nz[:, 1].contiguous()
+        self.rows = (self.nz[:, 0] * P + self.nz[:, 1]).to(torch.int32)
+        self.offsets_d = None      # one scene: the subset render takes idx[0..n) without offsets and waits for nothing
+        if B > 1:
+            self.offsets_d = torch.zeros(B + 1, dtype=torch.int64, device=masks.device)
+            torch.cumsum(counts_d, 0, out=self.offsets_d[1:])
+
+
+def _render_subset(fn, binning: SceneBinning, subset: FineSubset, shs_fine):
+    """The subset render of every scene of ``binning`` (checked, unchanged) with the :class:`FineSubset` of its masks
+    and ``shs_fine`` [n,M,3]; ``fn`` names the caller in messages.  Returns the outputs of :func:`_subset_forward`."""
     centers, _, opacity, scales, rotations = binning.tensors
-    S, dev = binning.scenes, binning.means.device
+    dev = binning.means.device
     deg = binning.geometry[4]
     if not isinstance(shs_fine, torch.Tensor) or shs_fine.dtype != torch.float32 or shs_fine.device != dev or \
             shs_fine.ndim != 3 or shs_fine.shape[2] != 3 or shs_fine.shape[1] < (deg + 1) ** 2:
         raise RuntimeError(f"{fn}: shs_fine must be float32 [n, M >= {(deg + 1) ** 2}, 3] on {dev}, got "
                            f"{getattr(shs_fine, 'dtype', type(shs_fine))} {tuple(getattr(shs_fine, 'shape', ()))}")
-    counts_d = masks.sum(1)
-    counts = [int(c) for c in counts_d.tolist()]        # the host sync
-    n = sum(counts)
+    counts, n = subset.counts, subset.n
     if shs_fine.shape[0] != n:
         raise RuntimeError(f"{fn}: shs_fine has {shs_fine.shape[0]} rows, the mask selects {n}")
-    nz = torch.nonzero_static(masks, size=n)        # (scene, index) pairs, scene-major, ascending within a scene
-    idx = nz[:, 1].contiguous()
-    offsets = None          # one scene: the C entry takes idx[0..n) without offsets and waits for nothing
-    if S > 1:
-        offsets = torch.zeros(S + 1, dtype=torch.int64, device=dev)
-        torch.cumsum(counts_d, 0, out=offsets[1:])
+    nz, idx, offsets = subset.nz, subset.idx, subset.offsets_d
     shs_c = shs_fine.contiguous()
     with _DeviceGuard(dev):
         if R.needs_backward(centers, shs_fine, opacity, scales, rotations):
             outs = _RenderSubsetViews.apply(binning, nz, idx, offsets, counts, shs_c, centers, opacity, scales, rotations)
         else:
             outs = _subset_forward(binning, idx, shs_c, False, offsets, counts)[0]
-    return outs, counts
+    return outs
 
 
 def render_subset_views(binning: SceneBinning, mask: torch.Tensor, shs_fine: torch.Tensor,
@@ -346,7 +397,7 @@ def render_subset_views(binning: SceneBinning, mask: torch.Tensor, shs_fine: tor
         raise RuntimeError(f"render_subset_views: mask must be a bool tensor [{P}] on {dev}, got "
                            f"{getattr(mask, 'dtype', type(mask))} {tuple(getattr(mask, 'shape', ()))} on "
                            f"{getattr(mask, 'device', None)}")
-    outs, _ = _render_subset("render_subset_views", binning, mask[None], shs_fine)
+    outs = _render_subset("render_subset_views", binning, FineSubset(mask[None]), shs_fine)
     return _out_dict(*outs, binning.rays is not None, prex)
 
 
@@ -443,27 +494,31 @@ def render_batch_views(centers, shs, opacity, scales, rotations,
     return out
 
 
-def render_batch_subset_views(binning: SceneBinning, masks: torch.Tensor, shs_fine: torch.Tensor,
+def render_batch_subset_views(binning: SceneBinning, masks, shs_fine: torch.Tensor,
                               prex: str = "_fine") -> Dict[str, object]:
     """LaRa's fine pass for all B scenes of a batch from the coarse pass's binning: ``binning`` is ``out["binning"]`` of
-    ``render_batch_views(..., keep_binning=True)``, ``masks`` a bool tensor [B,P], ``shs_fine`` [n,M,3] the subsets' SH
-    coefficients concatenated in scene order (B calls of ``FineHead.fine_shs`` concatenated).  Returns ``{key+prex:
-    [B,V,...]}`` where ``out[k][b]`` is what :func:`render_subset_views` returns for scene b alone, bit for bit, and
-    ``radii+prex`` a list of B tensors [V, n_b].  One host sync for the mask counts (and, for B > 1, the C entry's check
-    of the offsets, which waits for the stream).  Gradients go to the [B,P,...] coarse tensors and to ``shs_fine``."""
+    ``render_batch_views(..., keep_binning=True)``, ``masks`` a bool tensor [B,P] or the :class:`FineSubset` of those
+    masks (whose counts are then not read again), ``shs_fine`` [n,M,3] the subsets' SH coefficients concatenated in scene
+    order (``FineHead.fine_shs``' batch form, or B of its calls concatenated).  Returns ``{key+prex: [B,V,...]}`` where
+    ``out[k][b]`` is what :func:`render_subset_views` returns for scene b alone, bit for bit, and ``radii+prex`` a list of
+    B tensors [V, n_b].  One host sync for the mask counts when given masks (and, for B > 1, the C entry's check of the
+    offsets, which waits for the stream).  Gradients go to the [B,P,...] coarse tensors and to ``shs_fine``."""
+    fn = "render_batch_subset_views"
     if not isinstance(binning, SceneBinning):
         raise TypeError("render_batch_subset_views: binning must be out['binning'] of render_batch_views(..., "
                         "keep_binning=True)")
     binning.check_unchanged()
     B, P, dev = binning.scenes, int(binning.means.shape[-2]), binning.means.device
-    if not isinstance(masks, torch.Tensor) or masks.dtype != torch.bool or tuple(masks.shape) != (B, P) or \
-            masks.device != dev:
-        raise RuntimeError(f"render_batch_subset_views: masks must be a bool tensor [{B},{P}] on {dev}, got "
-                           f"{getattr(masks, 'dtype', type(masks))} {tuple(getattr(masks, 'shape', ()))} on "
-                           f"{getattr(masks, 'device', None)}")
-    outs, counts = _render_subset("render_batch_subset_views", binning, masks, shs_fine)
+    given = masks.masks if isinstance(masks, FineSubset) else masks
+    if not isinstance(given, torch.Tensor) or given.dtype != torch.bool or tuple(given.shape) != (B, P) or \
+            given.device != dev:
+        raise RuntimeError(f"{fn}: masks must be a bool tensor [{B},{P}] on {dev} or its FineSubset, got "
+                           f"{getattr(given, 'dtype', type(given))} {tuple(getattr(given, 'shape', ()))} on "
+                           f"{getattr(given, 'device', None)}")
+    subset = masks if isinstance(masks, FineSubset) else FineSubset(masks)
+    outs = _render_subset(fn, binning, subset, shs_fine)
     radii = outs[-1]
     out = _batch_out_dict(outs, B, binning.rays is not None, prex)
     V = radii.shape[0] // B
-    out["radii" + prex] = [radii[b * V:(b + 1) * V, :counts[b]] for b in range(B)]
+    out["radii" + prex] = [radii[b * V:(b + 1) * V, :subset.counts[b]] for b in range(B)]
     return out

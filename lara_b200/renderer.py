@@ -132,7 +132,7 @@ class Renderer(nn.Module):
                                   raw_activations=fuse, prex=prex, keep_binning=keep_binning)
 
     def render_batch_subset_views(self, binning, masks, shs_fine, prex: str = "_fine"):
-        """The fine pass of all scenes of a :meth:`render_batch_views` call with ``keep_binning=True``:
-        ``lara_b200.multiview.render_batch_subset_views``."""
+        """The fine pass of all scenes of a :meth:`render_batch_views` call with ``keep_binning=True``, ``masks`` [B,P]
+        bool or their ``lara_b200.multiview.FineSubset``: ``lara_b200.multiview.render_batch_subset_views``."""
         from .multiview import render_batch_subset_views
         return render_batch_subset_views(binning, masks, shs_fine, prex=prex)
