@@ -251,6 +251,27 @@ int srf_loss_backward(srf_stream_t stream, int V, int image_height, int image_wi
                       const float* image, const float* target_hwc, const float* rend_normal, const float* depth_normal,
                       const float* acc_map, const float* upstream,
                       float* g_image, float* g_rend_normal, float* g_depth_normal, float* g_rend_dist);
+/* Both passes of LaRa's step in one launch per direction (DESIGN §3.27): V may be the B*V views of a batch
+ * ([B*V,3,H,W] planar buffers of the batch render), and `image_fine` (NULL: none) is the fine pass, read against the
+ * same target.  srf_loss_passes_forward then writes sums[3] = sum (image_fine - target)^2 as well (sums [4]; [3]
+ * without image_fine), each target pixel read once; the fine pass has no regulariser terms, as in LaRa.  The
+ * backward writes g_image_fine = 2 w_mse (image_fine - target) with the same w_mse and upstream; image_fine and
+ * g_image_fine are both given or both NULL.  Buffers must be 4-byte aligned (sums and workspace 8-byte).  With
+ * image_fine NULL these are srf_loss_forward / _backward (which run them), bit for bit; the deterministic workspace
+ * (srf_loss_passes_deterministic_workspace_bytes, with_fine != 0 for image_fine) holds one partial per term and block,
+ * so with a fine image each of the first three sums has the bits of the call without it.                     */
+int srf_loss_passes_forward(srf_stream_t stream, int V, int image_height, int image_width, int with_reg,
+                            const float* image, const float* image_fine, const float* target_hwc,
+                            const float* rend_normal, const float* depth_normal, const float* acc_map,
+                            const float* rend_dist, double* sums, void* workspace);
+int srf_loss_passes_deterministic_workspace_bytes(int V, int image_height, int image_width, int with_fine,
+                                                  size_t* bytes);
+int srf_loss_passes_backward(srf_stream_t stream, int V, int image_height, int image_width, int with_reg,
+                             float w_mse, float w_dist, float w_normal,
+                             const float* image, const float* image_fine, const float* target_hwc,
+                             const float* rend_normal, const float* depth_normal, const float* acc_map,
+                             const float* upstream, float* g_image, float* g_image_fine, float* g_rend_normal,
+                             float* g_depth_normal, float* g_rend_dist);
 
 /* ---- decoder epilogue: MLP output -> Gaussian-parameter tensors (next-row: lightning/network.py:261-278,425-429) ----
  * `params` is the decoder MLP's fp32 output [B, N, K*C], C = 10 + sh_dim, each row = offset[3] | sh[sh_dim] |
@@ -346,6 +367,23 @@ int srf_ms_ssim_backward(srf_stream_t stream, int B, int C, int H, int W,
                          const float* x, const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
                          float data_range, int size_average, void* workspace, const float* upstream,
                          float* dx, const srf_ms_ssim_addr* dx_addr);
+/* Both passes of a batch against one target in one launch set per direction (DESIGN §3.27): X is the coarse pass `x`
+ * and, when `x_fine` is not NULL, the fine pass `x_fine`, both B x C x H x W images read through `x_addr`; Y is read
+ * once per pass.  out[0] is the coarse pass's mean over (b, c), out[1] the fine pass's (out [2]; [1] without x_fine).
+ * Each (scene, pass, channel) plane's value and coefficients have the bits of srf_ms_ssim_forward on that pass alone
+ * (size_average = 1), which is this with x_fine NULL.  The backward takes upstream [2] (or [1]) and writes, or with
+ * accumulate != 0 adds, dL/dX into dx and dx_fine through dx_addr (dx_fine given exactly when x_fine is).  Needs
+ * 2 B C <= 65535 with x_fine; the workspace is srf_ms_ssim_passes_workspace_bytes(..., with_fine = x_fine != NULL). */
+int srf_ms_ssim_passes_workspace_bytes(int B, int C, int H, int W, int with_fine, size_t* bytes);
+int srf_ms_ssim_passes_forward(srf_stream_t stream, int B, int C, int H, int W,
+                               const float* x, const float* x_fine, const srf_ms_ssim_addr* x_addr,
+                               const float* y, const srf_ms_ssim_addr* y_addr, float data_range, void* workspace,
+                               float* out);
+int srf_ms_ssim_passes_backward(srf_stream_t stream, int B, int C, int H, int W,
+                                const float* x, const float* x_fine, const srf_ms_ssim_addr* x_addr,
+                                const float* y, const srf_ms_ssim_addr* y_addr, float data_range, void* workspace,
+                                const float* upstream, float* dx, float* dx_fine, const srf_ms_ssim_addr* dx_addr,
+                                int accumulate);
 
 /* ---- fused single-scale SSIM (pytorch-msssim 1.0.0 ssim; evaluation.py:93 and the D-SSIM loss term) -----------------
  * Level 0 of the MS-SSIM above on its own: the same window, C1, C2, image addressing, workspace rules and determinism.

@@ -89,6 +89,11 @@ SIGNATURES = {
     "srf_loss_forward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P]),
     "srf_loss_deterministic_workspace_bytes": (c_int, [c_int, c_int, c_int, POINTER(c_size_t)]),
     "srf_loss_backward": (c_int, [_P, c_int, c_int, c_int, c_int, c_float, c_float, c_float, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "srf_loss_passes_forward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "srf_loss_passes_deterministic_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, POINTER(c_size_t)]),
+    "srf_loss_passes_backward": (c_int, [_P, c_int, c_int, c_int, c_int, c_float, c_float, c_float,
+                                         _P, _P, _P, _P, _P, _P, _P,   # image, image_fine, target, rn, dn, acc, upstream
+                                         _P, _P, _P, _P, _P]),         # g_image, g_image_fine, g_rn, g_dn, g_dist
     "srf_decoder_layout_forward": (c_int, [_P, c_size_t, c_int, c_int, c_int, c_float, c_float, c_float, _P, _P, _P, _P, _P, _P, _P]),
     "srf_decoder_layout_backward": (c_int, [_P, c_size_t, c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P]),
     "srf_point_feats_forward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P]),
@@ -110,6 +115,10 @@ SIGNATURES = {
                                              POINTER(c_int)]),
     "srf_ms_ssim_forward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _A, _P, _A, c_float, c_int, _P, _P]),
     "srf_ms_ssim_backward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _A, _P, _A, c_float, c_int, _P, _P, _P, _A]),
+    "srf_ms_ssim_passes_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, c_int, POINTER(c_size_t)]),
+    "srf_ms_ssim_passes_forward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _A, _P, _A, c_float, _P, _P]),
+    "srf_ms_ssim_passes_backward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _A, _P, _A, c_float, _P, _P, _P,
+                                            _P, _A, c_int]),
     "srf_ssim_workspace_bytes": (c_int, [c_int, c_int, c_int, c_int, POINTER(c_size_t)]),
     "srf_ssim_forward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _A, _P, _A, c_float, c_int, c_int, _P, _P]),
     "srf_ssim_backward": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _A, _P, _A, c_float, c_int, c_int, _P, _P, _P,
@@ -349,6 +358,14 @@ def det_point_feats_scenes_workspace_bytes(lib, S: int, Vs: int, H: int, W: int)
 
 def det_loss_workspace_bytes(lib, V: int, H: int, W: int) -> int:
     return _size_query(lib.srf_loss_deterministic_workspace_bytes, V, H, W)
+
+
+def det_loss_passes_workspace_bytes(lib, V: int, H: int, W: int, with_fine: bool) -> int:
+    return _size_query(lib.srf_loss_passes_deterministic_workspace_bytes, V, H, W, 1 if with_fine else 0)
+
+
+def ms_ssim_passes_workspace_bytes(lib, B: int, C: int, H: int, W: int, with_fine: bool) -> int:
+    return _size_query(lib.srf_ms_ssim_passes_workspace_bytes, B, C, H, W, 1 if with_fine else 0)
 
 
 def use_deterministic(requested: Optional[bool], enabled: bool, warn_only: bool) -> bool:

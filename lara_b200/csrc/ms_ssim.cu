@@ -18,6 +18,11 @@
 //                        and adds the pooling backward: dX_l = G^T A + 2 X G^T B + Y G^T C + dX_{l+1}(parent) / 4.
 // No atomics anywhere: two identical calls give identical bits.  The level-0 image is read (and its gradient
 // written) through MsAddr, so a channel-last tensor and V planar views side by side are read in place.
+// Two sources (srf_ms_ssim_passes_*, LaRa's coarse and fine passes against one target): the batch has 2 B entries;
+// at level 0 entry b < B reads X from x, entry b >= B from x2 at b - B, and both read Y at b mod B; levels >= 1 are
+// planar over all 2 B C planes.  Each plane runs the same code as in a one-source call, so its value and coefficients
+// have the same bits; the finalize writes one mean per source.  The backward can add its level-0 gradient into dX
+// instead of writing it.
 // The C entries srf_ms_ssim_* (include/surfel_rasterizer.h) are defined here, and so are srf_ssim_*: single-scale
 // SSIM, the same code with a one-level pyramid (its only level is the kLast level, on the caller's image).  The
 // level count changes only the size rule and the finalize's value / coefficient rule.
@@ -35,14 +40,16 @@ namespace srf {
 // column x % wv.
 struct MsAddr { long long sb, sc, sy, sx, sv; int wv; };
 struct MsSsimArgs {
-    int B, C, H, W;
-    int size_average;            // out[0] = mean over (b, c); else out[b] = mean over c
+    int B, C, H, W;              // B: entries of all sources, nsrc * nb
+    int nb, nsrc;                // entries per source, sources (1, or 2 with x2)
+    int size_average;            // out[s] = mean over (b, c) of source s; else out[b] = mean over c
     float data_range;
-    const float* x; const float* y; MsAddr ax, ay;
+    const float* x; const float* x2; const float* y; MsAddr ax, ay;   // x2: the second source (null: one), read via ax
     void* workspace;             // srf_ms_ssim_workspace_bytes: pyramid, its gradient, partial sums, coefficients
     float* out;                  // forward output
     const float* gout;           // backward: upstream gradient of out (device)
-    float* gx; MsAddr ag;        // backward output, dL/dX
+    float* gx; float* gx2; MsAddr ag;   // backward output, dL/dX of each source
+    int accumulate;              // backward: add dL/dX into gx / gx2 instead of writing it
 };
 
 namespace {
@@ -99,18 +106,21 @@ struct LevelArgs {
     float c1, c2;
     float win[kR + 1];
     const float* x; const float* y; MsAddr ax, ay;   // this level's input
+    const float* x2; int nb;     // level 0 of two sources: entries b >= nb read x2 at b - nb, and Y at b - nb
     // forward
     float* nx; float* ny; int nh, nw;                // next level's planar X, Y (null at the last level)
     double* part;                // [planes][ntiles] per-CTA partial sums
     // backward
     const float* coef;           // [planes] dvalue/dm_l / count_l
-    const float* gout; int gout_per_b;               // upstream gradient: [1] or [B]
+    const float* gout; int gout_planes;              // upstream gradient: entry plane / gout_planes
     const float* gnext;          // planar dX_{l+1} (null at the last level)
-    float* gx; MsAddr ag;        // dX_l
+    float* gx; float* gx2; MsAddr ag;                // dX_l (gx2: level 0's for the entries that read x2)
+    int accumulate;              // add into gx / gx2
+
 };
 
 struct FinalArgs {
-    int B, C, planes, size_average;
+    int B, C, planes, size_average, nsrc;
     int levels;
     int nonnegative;             // one level: relu the mean (MS-SSIM always does)
     int ntiles[kLevels];
@@ -120,12 +130,19 @@ struct FinalArgs {
     double* mean;                // [levels][planes]
     double* val;                 // [planes]
     float* coef;                 // [levels][planes]
-    float* out;                  // [1] or [B]
+    float* out;                  // [nsrc] or [B]
 };
 
 __device__ __forceinline__ long long addr_of(const MsAddr& a, int b, int c, int y, int x) {
     const int v = x / a.wv;
     return b * a.sb + c * a.sc + y * a.sy + v * a.sv + (x - v * a.wv) * a.sx;
+}
+
+// Level 0 of two sources: the X base of entry b, which becomes its scene b mod nb (the index of X, Y and dX).
+__device__ __forceinline__ bool second_source(const LevelArgs& a, int& b) {
+    if (!a.x2 || b < a.nb) return false;
+    b -= a.nb;
+    return true;
 }
 
 // Sum over the CTA of one double per thread, in a fixed order; the result is valid in thread 0.
@@ -148,7 +165,9 @@ __global__ void __launch_bounds__(kThreads) ms_ssim_fwd_kernel(const LevelArgs a
     constexpr int IW = kTW + kR, IH = kTH + kR;
     __shared__ float s_in[2][IH][IW];
     __shared__ float s_h[5][kTH][IW];
-    const int plane = blockIdx.y, b = plane / a.C, c = plane - b * a.C;
+    const int plane = blockIdx.y, c = plane % a.C;
+    int b = plane / a.C;
+    const float* xs = second_source(a, b) ? a.x2 : a.x;
     const int tx = blockIdx.x % a.ntx, ty = blockIdx.x / a.ntx;
     // tiles start at -padding so that each CTA owns whole 2x2 pooling cells
     const int x0 = tx * kTW - a.px, y0 = ty * kTH - a.py;
@@ -156,7 +175,7 @@ __global__ void __launch_bounds__(kThreads) ms_ssim_fwd_kernel(const LevelArgs a
         const int r = i / IW, q = i - r * IW, y = y0 + r, x = x0 + q;
         float vx = 0.f, vy = 0.f;
         if (y >= 0 && y < a.H && x >= 0 && x < a.W) {
-            vx = __ldg(a.x + addr_of(a.ax, b, c, y, x));
+            vx = __ldg(xs + addr_of(a.ax, b, c, y, x));
             vy = __ldg(a.y + addr_of(a.ay, b, c, y, x));
         }
         s_in[0][r][q] = vx;
@@ -227,7 +246,8 @@ __global__ void __launch_bounds__(kThreads) ms_ssim_finalize_kernel(const FinalA
         if ((threadIdx.x & 31) == 0) f.mean[j] = s / f.count[l];
     }
     __syncthreads();
-    const double scale = 1.0 / (f.size_average ? (double)P : (double)f.C);
+    const int per_src = P / f.nsrc;
+    const double scale = 1.0 / (f.size_average ? (double)per_src : (double)f.C);
     for (int p = threadIdx.x; p < P; p += kThreads) {
         if (f.levels == 1) {
             // SSIM: the mean, optionally relu'd; relu's backward is a select, so no gradient through a mean <= 0
@@ -256,9 +276,9 @@ __global__ void __launch_bounds__(kThreads) ms_ssim_finalize_kernel(const FinalA
             f.coef[l * P + p] = pos ? (float)(kWeights[l] * v / m[l] * scale / f.count[l]) : 0.f;
     }
     __syncthreads();
-    const int nout = f.size_average ? 1 : f.B;
+    const int nout = f.size_average ? f.nsrc : f.B;
     for (int o = threadIdx.x; o < nout; o += kThreads) {
-        const int p0 = f.size_average ? 0 : o * f.C, np = f.size_average ? P : f.C;
+        const int np = f.size_average ? per_src : f.C, p0 = o * np;
         double s = 0.0;
         for (int p = 0; p < np; ++p) s += f.val[p0 + p];
         f.out[o] = (float)(s / np);
@@ -272,17 +292,21 @@ __global__ void __launch_bounds__(kThreads) ms_ssim_bwd_kernel(const LevelArgs a
     __shared__ float s_a[2 * IH * IW];     // X, Y; then the coefficient maps [3][OH][OW]
     __shared__ float s_b[5 * OH * IW];     // H pass of the five quantities; then the H pass of G^T [3][kTH][OW]
     static_assert(3 * OH * OW <= 2 * IH * IW && 3 * kTH * OW <= 5 * OH * IW, "shared-memory aliasing");
-    const int plane = blockIdx.y, b = plane / a.C, c = plane - b * a.C;
+    const int plane = blockIdx.y, c = plane % a.C;
+    int b = plane / a.C;
+    const bool second = second_source(a, b);
+    const float* xs = second ? a.x2 : a.x;
+    float* gxs = second ? a.gx2 : a.gx;
     const int x0 = (blockIdx.x % a.ntx) * kTW, y0 = (blockIdx.x / a.ntx) * kTH;
     const int lane = threadIdx.x & 31, wr = threadIdx.x >> 5;
-    const float k = a.coef[plane] * __ldg(a.gout + (a.gout_per_b ? b : 0));
+    const float k = a.coef[plane] * __ldg(a.gout + plane / a.gout_planes);
     float ga[2] = {0.f, 0.f}, gb[2] = {0.f, 0.f}, gc[2] = {0.f, 0.f};
     if (k != 0.f) {     // uniform over the CTA
         for (int i = threadIdx.x; i < IH * IW; i += kThreads) {
             const int r = i / IW, q = i - r * IW, y = y0 - kR + r, x = x0 - kR + q;
             float vx = 0.f, vy = 0.f;
             if (y >= 0 && y < a.H && x >= 0 && x < a.W) {
-                vx = __ldg(a.x + addr_of(a.ax, b, c, y, x));
+                vx = __ldg(xs + addr_of(a.ax, b, c, y, x));
                 vy = __ldg(a.y + addr_of(a.ay, b, c, y, x));
             }
             s_a[r * IW + q] = vx;
@@ -376,12 +400,14 @@ __global__ void __launch_bounds__(kThreads) ms_ssim_bwd_kernel(const LevelArgs a
         if (y >= a.H || x >= a.W) continue;
         float d = 0.f;
         if (k != 0.f) {
-            const float vx = __ldg(a.x + addr_of(a.ax, b, c, y, x)), vy = __ldg(a.y + addr_of(a.ay, b, c, y, x));
+            const float vx = __ldg(xs + addr_of(a.ax, b, c, y, x)), vy = __ldg(a.y + addr_of(a.ay, b, c, y, x));
             d = fmaf(2.f * vx, gb[h], ga[h]);
             d = fmaf(vy, gc[h], d);
         }
         if (!kLast) d += 0.25f * __ldg(a.gnext + ((size_t)plane * a.nh + (y + a.py) / 2) * a.nw + (x + a.px) / 2);
-        a.gx[addr_of(a.ag, b, c, y, x)] = d;
+        float* g = gxs + addr_of(a.ag, b, c, y, x);
+        if (a.accumulate) *g += d;
+        else *g = d;
     }
 }
 
@@ -417,6 +443,7 @@ LevelArgs level_args(const MsSsimArgs& m, const Layout& L, char* ws, int l) {
     float* pyr = reinterpret_cast<float*>(ws + L.o_pyr);
     if (l == 0) {
         a.x = m.x; a.y = m.y; a.ax = m.ax; a.ay = m.ay;
+        a.x2 = m.x2; a.nb = m.nb;
     } else {
         const size_t n = (size_t)m.B * m.C * L.h[l] * L.w[l];
         a.x = pyr + L.pyr[l]; a.y = a.x + n;
@@ -458,36 +485,45 @@ static int ms_ssim_addr(const char* fn, const char* what, const float* p, const 
     return 0;
 }
 
-static int ms_ssim_prepare(const char* fn, int levels, int B, int C, int H, int W, const float* x,
+// B scenes per source; x2 (read through x_addr) null for one source
+static int ms_ssim_prepare(const char* fn, int levels, int B, int C, int H, int W, const float* x, const float* x2,
                            const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
                            float data_range, int size_average, void* workspace, srf::MsSsimArgs* a) {
     memset(a, 0, sizeof(*a));
+    const int nsrc = x2 ? 2 : 1;
     if (ms_ssim_sizes(fn, levels, B, C, H, W)) return 1;
+    if (nsrc > 1 && ms_ssim_sizes(fn, levels, nsrc * B, C, H, W)) return 1;
     if (ms_ssim_addr(fn, "x", x, x_addr, &a->ax) || ms_ssim_addr(fn, "y", y, y_addr, &a->ay)) return 1;
+    if (x2 && (reinterpret_cast<uintptr_t>(x2) & 3)) return set_error("%s: x_fine must be 4-byte aligned", fn);
     if (!(data_range > 0.f) || !(data_range < 3.0e38f)) return set_error("%s: data_range must be positive and finite", fn);
     if (!workspace || srf::misaligned(workspace)) return set_error("%s: workspace must be 256-byte aligned", fn);
-    a->B = B; a->C = C; a->H = H; a->W = W; a->size_average = size_average ? 1 : 0; a->data_range = data_range;
-    a->x = x; a->y = y; a->workspace = workspace;
+    a->B = nsrc * B; a->nb = B; a->nsrc = nsrc; a->C = C; a->H = H; a->W = W;
+    a->size_average = size_average ? 1 : 0; a->data_range = data_range;
+    a->x = x; a->x2 = x2; a->y = y; a->workspace = workspace;
     return 0;
 }
 
-static int ms_ssim_workspace_bytes(const char* fn, int levels, int B, int C, int H, int W, size_t* bytes) {
+static int ms_ssim_workspace_bytes(const char* fn, int levels, int nsrc, int B, int C, int H, int W, size_t* bytes) {
     if (ms_ssim_sizes(fn, levels, B, C, H, W)) return 1;
+    if (nsrc > 1 && ms_ssim_sizes(fn, levels, nsrc * B, C, H, W)) return 1;
     if (!bytes) return set_error("%s: null pointer", fn);
-    *bytes = srf::make_layout(levels, B, C, H, W).total;
+    *bytes = srf::make_layout(levels, nsrc * B, C, H, W).total;
     return 0;
 }
 
 // the pyramid's levels 0 .. levels - 1, then the finalize
 static int ms_ssim_forward(const char* fn, int levels, int nonnegative, srf_stream_t stream_, int B, int C, int H,
-                           int W, const float* x, const srf_ms_ssim_addr* x_addr, const float* y,
+                           int W, const float* x, const float* x2, const srf_ms_ssim_addr* x_addr, const float* y,
                            const srf_ms_ssim_addr* y_addr, float data_range, int size_average, void* workspace,
                            float* out) {
     using namespace srf;
     MsSsimArgs m;
-    if (ms_ssim_prepare(fn, levels, B, C, H, W, x, x_addr, y, y_addr, data_range, size_average, workspace, &m)) return 1;
+    if (ms_ssim_prepare(fn, levels, B, C, H, W, x, x2, x_addr, y, y_addr, data_range, size_average, workspace, &m))
+        return 1;
     if (!out) return set_error("%s: null output pointer", fn);
+    if (reinterpret_cast<uintptr_t>(out) & 3) return set_error("%s: out must be 4-byte aligned", fn);
     m.out = out;
+    B = m.B;
     const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     const Layout L = make_layout(levels, B, C, H, W);
     char* ws = static_cast<char*>(workspace);
@@ -502,7 +538,7 @@ static int ms_ssim_forward(const char* fn, int levels, int nonnegative, srf_stre
     }
     FinalArgs f;
     memset(&f, 0, sizeof(f));
-    f.B = B; f.C = C; f.planes = planes; f.size_average = m.size_average;
+    f.B = B; f.C = C; f.planes = planes; f.size_average = m.size_average; f.nsrc = m.nsrc;
     f.levels = levels; f.nonnegative = nonnegative ? 1 : 0;
     for (int l = 0; l < levels; ++l) {
         f.ntiles[l] = L.ntx[l] * L.nty[l];
@@ -521,15 +557,21 @@ static int ms_ssim_forward(const char* fn, int levels, int nonnegative, srf_stre
 
 // levels - 1 .. 0 with the coefficients the forward left in the workspace
 static int ms_ssim_backward(const char* fn, int levels, srf_stream_t stream_, int B, int C, int H, int W,
-                            const float* x, const srf_ms_ssim_addr* x_addr, const float* y,
+                            const float* x, const float* x2, const srf_ms_ssim_addr* x_addr, const float* y,
                             const srf_ms_ssim_addr* y_addr, float data_range, int size_average, void* workspace,
-                            const float* upstream, float* dx, const srf_ms_ssim_addr* dx_addr) {
+                            const float* upstream, float* dx, float* dx2, const srf_ms_ssim_addr* dx_addr,
+                            int accumulate) {
     using namespace srf;
     MsSsimArgs m;
-    if (ms_ssim_prepare(fn, levels, B, C, H, W, x, x_addr, y, y_addr, data_range, size_average, workspace, &m)) return 1;
+    if (ms_ssim_prepare(fn, levels, B, C, H, W, x, x2, x_addr, y, y_addr, data_range, size_average, workspace, &m))
+        return 1;
     if (!upstream) return set_error("%s: null upstream gradient", fn);
+    if (reinterpret_cast<uintptr_t>(upstream) & 3) return set_error("%s: upstream must be 4-byte aligned", fn);
     if (ms_ssim_addr(fn, "dx", dx, dx_addr, &m.ag)) return 1;
-    m.gout = upstream; m.gx = dx;
+    if (!x2 != !dx2) return set_error("%s: x_fine and dx_fine go together", fn);
+    if (dx2 && (reinterpret_cast<uintptr_t>(dx2) & 3)) return set_error("%s: dx_fine must be 4-byte aligned", fn);
+    m.gout = upstream; m.gx = dx; m.gx2 = dx2; m.accumulate = accumulate ? 1 : 0;
+    B = m.B;
     const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     const Layout L = make_layout(levels, B, C, H, W);
     char* ws = static_cast<char*>(workspace);
@@ -541,9 +583,9 @@ static int ms_ssim_backward(const char* fn, int levels, srf_stream_t stream_, in
         a.ntx = (L.w[l] + kTW - 1) / kTW;
         const int nty = (L.h[l] + kTH - 1) / kTH;
         a.coef = coef + (size_t)l * planes;
-        a.gout = m.gout; a.gout_per_b = m.size_average ? 0 : 1;
+        a.gout = m.gout; a.gout_planes = m.size_average ? m.nb * C : C;
         if (l + 1 < levels) a.gnext = gpyr + L.gpyr[l + 1];
-        if (l == 0) { a.gx = m.gx; a.ag = m.ag; }
+        if (l == 0) { a.gx = m.gx; a.gx2 = m.gx2; a.ag = m.ag; a.accumulate = m.accumulate; }
         else { a.gx = gpyr + L.gpyr[l]; a.ag = planar(m.C, L.h[l], L.w[l]); }
         const dim3 grid((unsigned)(a.ntx * nty), (unsigned)planes);
         if (l + 1 < levels) ms_ssim_bwd_kernel<false><<<grid, kThreads, 0, stream>>>(a);
@@ -554,7 +596,7 @@ static int ms_ssim_backward(const char* fn, int levels, srf_stream_t stream_, in
 }
 
 extern "C" int srf_ms_ssim_workspace_bytes(int B, int C, int H, int W, size_t* bytes) {
-    return ms_ssim_workspace_bytes("srf_ms_ssim_workspace_bytes", srf::kLevels, B, C, H, W, bytes);
+    return ms_ssim_workspace_bytes("srf_ms_ssim_workspace_bytes", srf::kLevels, 1, B, C, H, W, bytes);
 }
 
 extern "C" int srf_ms_ssim_workspace_layout(int B, int C, int H, int W, size_t regions[7], size_t levels[15],
@@ -575,7 +617,7 @@ extern "C" int srf_ms_ssim_workspace_layout(int B, int C, int H, int W, size_t r
 extern "C" int srf_ms_ssim_forward(srf_stream_t stream, int B, int C, int H, int W, const float* x,
                                    const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
                                    float data_range, int size_average, void* workspace, float* out) {
-    return ms_ssim_forward("srf_ms_ssim_forward", srf::kLevels, 1, stream, B, C, H, W, x, x_addr, y, y_addr,
+    return ms_ssim_forward("srf_ms_ssim_forward", srf::kLevels, 1, stream, B, C, H, W, x, nullptr, x_addr, y, y_addr,
                            data_range, size_average, workspace, out);
 }
 
@@ -583,20 +625,42 @@ extern "C" int srf_ms_ssim_backward(srf_stream_t stream, int B, int C, int H, in
                                     const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
                                     float data_range, int size_average, void* workspace, const float* upstream,
                                     float* dx, const srf_ms_ssim_addr* dx_addr) {
-    return ms_ssim_backward("srf_ms_ssim_backward", srf::kLevels, stream, B, C, H, W, x, x_addr, y, y_addr, data_range,
-                            size_average, workspace, upstream, dx, dx_addr);
+    return ms_ssim_backward("srf_ms_ssim_backward", srf::kLevels, stream, B, C, H, W, x, nullptr, x_addr, y, y_addr,
+                            data_range, size_average, workspace, upstream, dx, nullptr, dx_addr, 0);
+}
+
+extern "C" int srf_ms_ssim_passes_workspace_bytes(int B, int C, int H, int W, int with_fine, size_t* bytes) {
+    return ms_ssim_workspace_bytes("srf_ms_ssim_passes_workspace_bytes", srf::kLevels, with_fine ? 2 : 1, B, C, H, W,
+                                   bytes);
+}
+
+extern "C" int srf_ms_ssim_passes_forward(srf_stream_t stream, int B, int C, int H, int W, const float* x,
+                                          const float* x_fine, const srf_ms_ssim_addr* x_addr, const float* y,
+                                          const srf_ms_ssim_addr* y_addr, float data_range, void* workspace,
+                                          float* out) {
+    return ms_ssim_forward("srf_ms_ssim_passes_forward", srf::kLevels, 1, stream, B, C, H, W, x, x_fine, x_addr, y,
+                           y_addr, data_range, 1, workspace, out);
+}
+
+extern "C" int srf_ms_ssim_passes_backward(srf_stream_t stream, int B, int C, int H, int W, const float* x,
+                                           const float* x_fine, const srf_ms_ssim_addr* x_addr, const float* y,
+                                           const srf_ms_ssim_addr* y_addr, float data_range, void* workspace,
+                                           const float* upstream, float* dx, float* dx_fine,
+                                           const srf_ms_ssim_addr* dx_addr, int accumulate) {
+    return ms_ssim_backward("srf_ms_ssim_passes_backward", srf::kLevels, stream, B, C, H, W, x, x_fine, x_addr, y,
+                            y_addr, data_range, 1, workspace, upstream, dx, dx_fine, dx_addr, accumulate);
 }
 
 // ---- single-scale SSIM (pytorch-msssim 1.0.0 ssim): the one-level pyramid ----
 
 extern "C" int srf_ssim_workspace_bytes(int B, int C, int H, int W, size_t* bytes) {
-    return ms_ssim_workspace_bytes("srf_ssim_workspace_bytes", 1, B, C, H, W, bytes);
+    return ms_ssim_workspace_bytes("srf_ssim_workspace_bytes", 1, 1, B, C, H, W, bytes);
 }
 
 extern "C" int srf_ssim_forward(srf_stream_t stream, int B, int C, int H, int W, const float* x,
                                 const srf_ms_ssim_addr* x_addr, const float* y, const srf_ms_ssim_addr* y_addr,
                                 float data_range, int size_average, int nonnegative_ssim, void* workspace, float* out) {
-    return ms_ssim_forward("srf_ssim_forward", 1, nonnegative_ssim, stream, B, C, H, W, x, x_addr, y, y_addr,
+    return ms_ssim_forward("srf_ssim_forward", 1, nonnegative_ssim, stream, B, C, H, W, x, nullptr, x_addr, y, y_addr,
                            data_range, size_average, workspace, out);
 }
 
@@ -605,6 +669,6 @@ extern "C" int srf_ssim_backward(srf_stream_t stream, int B, int C, int H, int W
                                  float data_range, int size_average, int nonnegative_ssim, void* workspace,
                                  const float* upstream, float* dx, const srf_ms_ssim_addr* dx_addr) {
     (void)nonnegative_ssim;      // the forward folded the relu into the coefficients it left in the workspace
-    return ms_ssim_backward("srf_ssim_backward", 1, stream, B, C, H, W, x, x_addr, y, y_addr, data_range,
-                            size_average, workspace, upstream, dx, dx_addr);
+    return ms_ssim_backward("srf_ssim_backward", 1, stream, B, C, H, W, x, nullptr, x_addr, y, y_addr, data_range,
+                            size_average, workspace, upstream, dx, nullptr, dx_addr, 0);
 }
