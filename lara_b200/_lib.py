@@ -194,6 +194,7 @@ SIGNATURES = {
                                    _P, _P, _P,                           # rgba, normal, bg
                                    _P, _P, _P, _P,                       # i2w, i2w_down, origin, nrm_rot
                                    _P, _P, _P, _P, _P]),                 # tar_rgb, tar_msk, tar_nrm, tar_rays, tar_rays_down
+    "srf_batch_cameras": (c_int, [_P, c_int, _P, _P, _P]),                 # stream, n, c2w, bg, cams
     # include/surfel_finetune.h
     "srf_gaussian_adam_step": (c_int, [_P, c_int, c_int, _P5, _P5, _P,  # stream, n, M, params, grads, moments
                                        POINTER(c_double), c_double, c_double, c_double,   # lr (host [6]), beta1, beta2, eps

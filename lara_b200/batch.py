@@ -10,6 +10,8 @@ workers keep the uint8 views and the few small per-view matrices, and one kernel
   ``tar_nrm_u8`` in place of the float32 images, normals and rays.
 * :func:`assemble_batch` -- the collated raw batch (host, pinned or not, or device) -> ``tar_rgb``, ``tar_msk``,
   ``tar_nrm``, ``tar_rays``, ``tar_rays_down`` on the device plus the small tensors moved.
+* :func:`batch_cameras` -- the camera records of the batch's target views from ``tar_c2w`` and ``bg_color``, in one
+  launch (DESIGN §3.28).
 
 Rounding follows LaRa's NumPy lines: colour and mask bit for bit, the rays bit for bit wherever their three-term fp64
 sum is exact, the normals within a stated bound (DESIGN §3.23).
@@ -213,3 +215,34 @@ def assemble_batch(raw: Dict, device: Optional[torch.device] = None) -> Dict:
                 out["tar_msk"].data_ptr(), _lib._ptr(out.get("tar_nrm")), out["tar_rays"].data_ptr(),
                 out["tar_rays_down"].data_ptr())
     return out
+
+
+def batch_cameras(tar_c2w: torch.Tensor, bg_color: torch.Tensor) -> torch.Tensor:
+    """The camera records ``[B*V, SRF_CAM_FLOATS]`` of a batch's target views, built in one launch from the batch's
+    ``tar_c2w`` f32 ``[B,V,4,4]`` (or ``[B*V,4,4]``) and ``bg_color`` ``[B,V,3]`` on the device: what
+    ``rasterizer.pack_cameras`` builds from LaRa's ``MiniCam`` of each view (lightning/network.py:489-492,
+    lightning/utils.py:22-48), with no host read.  The view matrix is ``inverse(c2w)^T`` computed in fp64 and rounded
+    once to fp32 (MiniCam's is torch's fp32 inverse), ``campos`` is MiniCam's ``-c2w[:3,3]``.  A pose with a
+    non-finite entry or ``|det| < 1e-12`` gets a record that renders the view's background only, where ``MiniCam``'s
+    ``torch.inverse`` would raise (include/surfel_batch.h)."""
+    fn = "batch_cameras"
+    for name, t in (("tar_c2w", tar_c2w), ("bg_color", bg_color)):
+        if not isinstance(t, torch.Tensor):
+            raise TypeError(f"{fn}: {name} must be a tensor")
+        if t.dtype != torch.float32:
+            raise TypeError(f"{fn}: {name} must be float32, got {t.dtype}")
+    if tar_c2w.ndim < 3 or tuple(tar_c2w.shape[-2:]) != (4, 4):
+        raise ValueError(f"{fn}: tar_c2w must be [B,V,4,4] or [B*V,4,4], got {list(tar_c2w.shape)}")
+    n = tar_c2w.numel() // 16
+    if bg_color.numel() != 3 * n or bg_color.shape[-1] != 3 or tuple(bg_color.shape[:-1]) != tuple(tar_c2w.shape[:-2]):
+        raise ValueError(f"{fn}: bg_color must be {list(tar_c2w.shape[:-2]) + [3]}, got {list(bg_color.shape)}")
+    if not 0 < n <= 65535:
+        raise ValueError(f"{fn}: {n} views; the records are built for 1 to 65535 views")
+    dev = tar_c2w.device
+    if dev.type != "cuda" or bg_color.device != dev:
+        raise RuntimeError(f"{fn}: tar_c2w and bg_color must be CUDA tensors on one device, got {dev} and "
+                           f"{bg_color.device}")
+    c2w, bg = tar_c2w.detach().contiguous(), bg_color.detach().contiguous()
+    cams = torch.empty((n, _lib.CAM_FLOATS), dtype=torch.float32, device=dev)
+    _lib.launch("srf_batch_cameras", dev, n, c2w.data_ptr(), bg.data_ptr(), cams.data_ptr())
+    return cams

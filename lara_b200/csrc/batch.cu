@@ -140,6 +140,56 @@ __global__ void __launch_bounds__(kThreads) batch_assemble_kernel(const Assemble
     if (d_nrm) flush(d_nrm, st_nrm, npx * 3);
 }
 
+// One camera record per view (include/surfel_batch.h): the 4x4 inverse by cofactors of 2x2 minors, all in fp64, each
+// element divided by the fp64 determinant and rounded once to fp32.
+__global__ void __launch_bounds__(kThreads) batch_cameras_kernel(int n, const float* __restrict__ c2w,
+                                                                 const float* __restrict__ bg, float* __restrict__ cams) {
+    const int v = blockIdx.x * kThreads + threadIdx.x;
+    if (v >= n) return;
+    const float* m = c2w + (size_t)v * 16;
+    double a[16];
+    bool finite = true;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+        const float x = __ldg(m + i);
+        finite = finite && isfinite(x);
+        a[i] = (double)x;
+    }
+    const double s0 = a[0] * a[5] - a[4] * a[1], s1 = a[0] * a[6] - a[4] * a[2], s2 = a[0] * a[7] - a[4] * a[3];
+    const double s3 = a[1] * a[6] - a[5] * a[2], s4 = a[1] * a[7] - a[5] * a[3], s5 = a[2] * a[7] - a[6] * a[3];
+    const double c5 = a[10] * a[15] - a[14] * a[11], c4 = a[9] * a[15] - a[13] * a[11], c3 = a[9] * a[14] - a[13] * a[10];
+    const double c2 = a[8] * a[15] - a[12] * a[11], c1 = a[8] * a[14] - a[12] * a[10], c0 = a[8] * a[13] - a[12] * a[9];
+    const double det = s0 * c5 - s1 * c4 + s2 * c3 + s3 * c2 - s4 * c1 + s5 * c0;
+    float* r = cams + (size_t)v * SRF_CAM_FLOATS;
+    if (!finite || !(fabs(det) >= 1e-12)) {
+        // every finite point lands at view depth -1, behind the near plane: the view renders its background only
+#pragma unroll
+        for (int i = 0; i < SRF_CAM_BG; ++i) r[i] = 0.f;
+        r[SRF_CAM_VIEW + 14] = -1.f;
+        r[SRF_CAM_VIEW + 15] = 1.f;
+    } else {
+        const double inv[16] = {
+            a[5] * c5 - a[6] * c4 + a[7] * c3,   -a[1] * c5 + a[2] * c4 - a[3] * c3,
+            a[13] * s5 - a[14] * s4 + a[15] * s3, -a[9] * s5 + a[10] * s4 - a[11] * s3,
+            -a[4] * c5 + a[6] * c2 - a[7] * c1,  a[0] * c5 - a[2] * c2 + a[3] * c1,
+            -a[12] * s5 + a[14] * s2 - a[15] * s1, a[8] * s5 - a[10] * s2 + a[11] * s1,
+            a[4] * c4 - a[5] * c2 + a[7] * c0,   -a[0] * c4 + a[1] * c2 - a[3] * c0,
+            a[12] * s4 - a[13] * s2 + a[15] * s0, -a[8] * s4 + a[9] * s2 - a[11] * s0,
+            -a[4] * c3 + a[5] * c1 - a[6] * c0,  a[0] * c3 - a[1] * c1 + a[2] * c0,
+            -a[12] * s3 + a[13] * s1 - a[14] * s0, a[8] * s3 - a[9] * s1 + a[10] * s0};
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) r[SRF_CAM_VIEW + 4 * i + j] = __double2float_rn(inv[4 * j + i] / det);   // w2c^T
+#pragma unroll
+        for (int i = 0; i < 3; ++i) r[SRF_CAM_CAMPOS + i] = -__ldg(m + 4 * i + 3);
+    }
+#pragma unroll
+    for (int i = 0; i < 3; ++i) r[SRF_CAM_BG + i] = __ldg(bg + (size_t)v * 3 + i);
+#pragma unroll
+    for (int i = SRF_CAM_BG + 3; i < SRF_CAM_FLOATS; ++i) r[i] = 0.f;
+}
+
 int check_ptr(const char* fn, const char* what, const void* p, int align) {
     if (!p) return set_error("%s: null %s pointer", fn, what);
     if (reinterpret_cast<uintptr_t>(p) & (align - 1)) return set_error("%s: %s must be %d-byte aligned", fn, what, align);
@@ -184,4 +234,15 @@ extern "C" int srf_batch_assemble(srf_stream_t stream_, int B, int N, int H, int
     batch_assemble_kernel<<<(unsigned)ctas, kThreads, 0, stream>>>(a);
     const cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? 0 : cuda_error("batch_assemble launch", e);
+}
+
+extern "C" int srf_batch_cameras(srf_stream_t stream_, int n, const float* c2w, const float* bg, float* cams) {
+    using namespace srf;
+    const char* fn = "srf_batch_cameras";
+    if (n <= 0 || n > 65535) return set_error("%s: bad sizes: n = %d views must be in (0, 65535]", fn, n);
+    if (check_ptr(fn, "c2w", c2w, 4) || check_ptr(fn, "bg", bg, 4) || check_ptr(fn, "cams", cams, 4)) return 1;
+    const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    batch_cameras_kernel<<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, 0, stream>>>(n, c2w, bg, cams);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : cuda_error("batch_cameras launch", e);
 }

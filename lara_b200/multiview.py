@@ -19,7 +19,7 @@ per-view drop-in API is unchanged.
 """
 from __future__ import annotations
 
-from typing import Dict, Optional, Sequence
+from typing import Dict, NamedTuple, Optional, Sequence
 
 import numpy as np
 import torch
@@ -71,16 +71,15 @@ def _epilogue_backward(color, allmap, rays, cams, depth_ratio, has_rays, g_image
     return d_color, torch.zeros_like(allmap)
 
 
-def _views_forward(inputs, rays_c, settings, geometry, prefiltered, depth_ratio, raw_activations, for_backward,
+def _views_forward(inputs, rays_c, cams, geometry, prefiltered, depth_ratio, raw_activations, for_backward,
                    keep_list=False):
     """The rasterizer forward of the S*V views of S scenes and the fused epilogue: ``inputs`` the checked [S,P,...]
-    centers, shs, opacity, scales and rotations, ``settings`` the S*V checked view settings (scene s's views are
+    centers, shs, opacity, scales and rotations, ``cams`` the [S*V, SRF_CAM_FLOATS] camera records (scene s's views are
     s*V .. s*V+V-1), ``geometry`` (H, W, tan_fovx per scene, tan_fovy per scene, sh degree, debug), ``rays_c``
     [S*V,H,W,6] or None.  Returns the outputs (image, depth, acc, rn, dn, dist, radii) stacked [S*V, ...] and (cams,
     color, allmap, state)."""
     H, W, tfx, tfy, deg, debug = geometry
     dev = inputs[0].device
-    cams = R.pack_cameras(settings, dev)
     centers, shs, opacity, scales, rotations = inputs
     with _DeviceGuard(dev):
         color, allmap, radii, state = R.forward_batch_raw(
@@ -95,10 +94,10 @@ class _RenderSceneViews(torch.autograd.Function):
     [S,P,...] inputs are each scene's sum over its own views."""
 
     @staticmethod
-    def forward(ctx, centers, shs, opacity, scales, rotations, rays_c, settings, geometry, prefiltered, depth_ratio,
+    def forward(ctx, centers, shs, opacity, scales, rotations, rays_c, cams, geometry, prefiltered, depth_ratio,
                 raw_activations, keep=None):
         outs, (cams, color, allmap, state) = _views_forward(
-            (centers, shs, opacity, scales, rotations), rays_c, settings, geometry, prefiltered, depth_ratio,
+            (centers, shs, opacity, scales, rotations), rays_c, cams, geometry, prefiltered, depth_ratio,
             raw_activations, True)
         if keep is not None:
             keep.append((cams, state))
@@ -123,16 +122,16 @@ class _RenderSceneViews(torch.autograd.Function):
                 None, None, None, None, None, None, None)
 
 
-def _render_views(inputs, rays_c, settings, geometry, prefiltered, depth_ratio, raw_activations, keep_binning, tensors):
+def _render_views(inputs, rays_c, cams, geometry, prefiltered, depth_ratio, raw_activations, keep_binning, tensors):
     """:class:`_RenderSceneViews` when a gradient can flow, else the forward-only path; returns the outputs of
     :func:`_views_forward` and, with ``keep_binning``, the :class:`SceneBinning` of the call (``tensors``: the caller's
     five Gaussian tensors), else None."""
     keep = [] if keep_binning else None
     if R.needs_backward(*tensors, rays_c):
-        outs = _RenderSceneViews.apply(*inputs, rays_c, settings, geometry, prefiltered, depth_ratio, raw_activations,
+        outs = _RenderSceneViews.apply(*inputs, rays_c, cams, geometry, prefiltered, depth_ratio, raw_activations,
                                        keep)
     else:
-        outs, (cams, _, _, state) = _views_forward(inputs, rays_c, settings, geometry, prefiltered, depth_ratio,
+        outs, (cams, _, _, state) = _views_forward(inputs, rays_c, cams, geometry, prefiltered, depth_ratio,
                                                    raw_activations, False, keep_list=keep_binning)
         if keep is not None:
             keep.append((cams, state))
@@ -174,13 +173,19 @@ def render_scene_views(centers, shs, opacity, scales, rotations, settings_list: 
     inputs = tuple(None if t is None else t.unsqueeze(0)
                    for t in (centers_c, shs_c, opac_c, scales if scales_c is None else scales_c,
                              rotations if rot_c is None else rot_c))
-    outs, binning = _render_views(inputs, rays_c, settings, (H, W, (tfx,), (tfy,), deg, debug), prefiltered,
+    outs, binning = _render_views(inputs, rays_c, _pack(settings, dev), (H, W, (tfx,), (tfy,), deg, debug), prefiltered,
                                   float(depth_ratio), bool(raw_activations), keep_binning,
                                   (centers, shs, opacity, scales, rotations))
     out = _out_dict(*outs, rays is not None, prex)
     if binning is not None:
         out["binning" + prex] = binning
     return out
+
+
+def _pack(settings, dev):
+    """The camera records of checked view settings (``rasterizer.pack_cameras``), built outside autograd."""
+    with torch.no_grad():
+        return R.pack_cameras(settings, dev)
 
 
 def _out_dict(image, depth, acc, rn, dn, dist, radii, has_rays, prex):
@@ -461,22 +466,65 @@ def _batch_out_dict(outs, B, has_rays, prex):
     return {k: t.view((B, t.shape[0] // B) + tuple(t.shape[1:])) for k, t in out.items()}
 
 
+class BatchCameras(NamedTuple):
+    """The cameras of a batch as records: ``cams`` f32 [B*V, SRF_CAM_FLOATS] on the Gaussians' device (scene b's views
+    are rows b*V .. b*V+V-1; ``lara_b200.batch.batch_cameras`` builds them), the image size ``H``, ``W``, ``tan_fov``
+    one pair (tan_fovx, tan_fovy) of finite positive values per scene, and ``sh_degree``."""
+    cams: torch.Tensor
+    H: int
+    W: int
+    tan_fov: Sequence
+    sh_degree: int
+
+
+def _batch_cameras(cameras: BatchCameras, dev, B):
+    """(cams, H, W, tan_fov, sh_degree, prefiltered, debug) of checked :class:`BatchCameras` for B scenes."""
+    fn = "render_batch_views"
+    cams, H, W, tan_fov, deg = cameras
+    tan_fov = [(float(x), float(y)) for x, y in tan_fov]
+    if len(tan_fov) != B:
+        raise RuntimeError(f"{fn}: cameras.tan_fov must hold one pair per scene ({B}), got {len(tan_fov)}")
+    if not all(0.0 < t < float("inf") for p in tan_fov for t in p):
+        raise RuntimeError(f"{fn}: cameras.tan_fov must be finite and positive, got {tan_fov}")
+    if not isinstance(cams, torch.Tensor) or cams.dtype != torch.float32 or cams.ndim != 2 or \
+            cams.shape[1] != _lib.CAM_FLOATS or cams.shape[0] % B != 0 or cams.shape[0] == 0 or cams.device != dev:
+        raise RuntimeError(f"{fn}: cameras.cams must be float32 [B*V,{_lib.CAM_FLOATS}] with B = {B} on {dev}, got "
+                           f"{getattr(cams, 'dtype', type(cams))} {tuple(getattr(cams, 'shape', ()))} on "
+                           f"{getattr(cams, 'device', None)}")
+    if int(H) < 1 or int(W) < 1 or not 0 <= int(deg) <= 3:
+        raise RuntimeError(f"{fn}: cameras need H, W >= 1 and sh_degree in [0, 3], got {H}, {W}, {deg}")
+    return cams.detach().contiguous(), int(H), int(W), tan_fov, int(deg), False, False
+
+
 def render_batch_views(centers, shs, opacity, scales, rotations,
-                       settings: Sequence[Sequence[R.GaussianRasterizationSettings]],
+                       settings: Optional[Sequence[Sequence[R.GaussianRasterizationSettings]]] = None,
                        rays: Optional[torch.Tensor] = None, depth_ratio: float = 0.0, raw_activations: bool = False,
-                       prex: str = "", keep_binning: bool = False) -> Dict[str, object]:
+                       prex: str = "", keep_binning: bool = False,
+                       cameras: Optional[BatchCameras] = None) -> Dict[str, object]:
     """All views of all B scenes of a batch in one autograd node and one launch set: ``centers`` [B,P,3], ``shs``
     [B,P,M,3], ``opacity`` [B,P] or [B,P,1], ``scales`` [B,P,2], ``rotations`` [B,P,4], ``settings[b]`` scene b's V
     view settings, ``rays`` [B,V,H,W,6] or None.  Returns ``{key+prex: [B,V,...]}``, where ``out[k][b]`` is what
     :func:`render_scene_views` returns for scene b alone (bit for bit), and ``radii+prex`` [B,V,P].  Scenes may differ
     in field of view and background; they must share V, the image size and the SH degree.  No-grad renders take the
     forward-only path.  ``keep_binning=True`` adds ``out["binning"+prex]``, a :class:`SceneBinning` of B scenes for
-    :func:`render_batch_subset_views`."""
+    :func:`render_batch_subset_views`.
+
+    ``cameras`` (a :class:`BatchCameras`, in place of ``settings``) gives the views as camera records already on the
+    device, so that no per-view settings object is built; the records of ``pack_cameras`` over ``settings`` render
+    the same bits."""
     dev = centers.device
     inputs = _batch_inputs(centers, shs, opacity, scales, rotations)
-    settings = [[R._check_settings(rs, dev) for rs in s] for s in settings]
-    H, W, tan_fov, deg, prefiltered, debug = batch_view_settings(settings)
-    B, V = len(settings), len(settings[0])
+    if (settings is None) == (cameras is None):
+        raise TypeError("render_batch_views: pass either settings or cameras")
+    if cameras is None:
+        settings = [[R._check_settings(rs, dev) for rs in s] for s in settings]
+        H, W, tan_fov, deg, prefiltered, debug = batch_view_settings(settings)
+        B, V = len(settings), len(settings[0])
+        cams = _pack([rs for s in settings for rs in s], dev)
+    else:
+        B = int(centers.shape[0])
+        cams, H, W, tan_fov, deg, prefiltered, debug = _batch_cameras(cameras, dev, B)
+        V = int(cams.shape[0]) // B
     rays_c = None
     if rays is not None:
         rays_c = rays.contiguous()
@@ -485,7 +533,7 @@ def render_batch_views(centers, shs, opacity, scales, rotations,
                                f"{rays_c.dtype} {tuple(rays_c.shape)} on {rays_c.device}")
         rays_c = rays_c.view(B * V, H, W, 6)
     tfx, tfy = zip(*tan_fov)
-    outs, binning = _render_views(inputs, rays_c, [rs for s in settings for rs in s], (H, W, tfx, tfy, deg, debug),
+    outs, binning = _render_views(inputs, rays_c, cams, (H, W, tfx, tfy, deg, debug),
                                   prefiltered, float(depth_ratio), bool(raw_activations), keep_binning,
                                   (centers, shs, opacity, scales, rotations))
     out = _batch_out_dict(outs, B, rays is not None, prex)
