@@ -49,6 +49,7 @@ int srf_vit_tokens_backward(void* stream, int N, int L, int C, float eps, const 
                             const float* dL_dn1, const float* dL_dx, void* workspace, float* dL_dtokens,
                             float* d_bias, float* d_cls, float* d_pos_r, float* d_gamma, float* d_beta);
 
+/* rows may be 0: then the row arrays may be NULL, nothing is written but d_gamma = d_beta = 0. */
 int srf_vit_layernorm_forward(void* stream, int rows, int C, float eps, const float* a, const float* b,
                               const float* gamma, const float* beta, float* y, float* n);
 

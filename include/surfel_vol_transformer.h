@@ -15,6 +15,7 @@
  *
  * Residual add + LayerNorm on `rows` rows of C channels (C a multiple of 32 up to 512):
  *   y = a + b (b may be NULL: then y = a and y may be NULL),  n = (y - mean(y)) / sqrt(var(y) + eps) gamma + beta.
+ * rows may be 0: then the row arrays may be NULL, nothing is written but d_gamma = d_beta = 0.
  */
 #ifndef SURFEL_VOL_TRANSFORMER_H_
 #define SURFEL_VOL_TRANSFORMER_H_

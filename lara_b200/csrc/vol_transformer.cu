@@ -249,8 +249,9 @@ extern "C" int srf_add_layernorm_forward(void* stream_, int rows, int C, float e
                                          const float* gamma, const float* beta, float* y, float* n) {
     const char* fn = "srf_add_layernorm_forward";
     if (srf::ln_check(fn, rows, C, eps)) return 1;
-    if (!a || !gamma || !beta || !n) return set_error("%s: null pointer", fn);
-    if (b && !y) return set_error("%s: null y with a residual b", fn);
+    // an empty tensor may have no storage: the row arrays may be NULL when rows == 0
+    if ((rows > 0 && (!a || !n)) || !gamma || !beta) return set_error("%s: null pointer", fn);
+    if (rows > 0 && b && !y) return set_error("%s: null y with a residual b", fn);
     srf::ln_forward<srf::kLnMaxJ>(static_cast<cudaStream_t>(stream_), rows, C, eps, a, b, gamma, beta, y, n);
     const cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? 0 : cuda_error("add_layernorm forward launch", e);
@@ -269,8 +270,8 @@ extern "C" int srf_add_layernorm_backward(void* stream_, int rows, int C, float 
                                           void* workspace, float* dL_da, float* d_gamma, float* d_beta) {
     const char* fn = "srf_add_layernorm_backward";
     if (srf::ln_check(fn, rows, C, eps)) return 1;
-    if (!y || !gamma || !dL_dn) return set_error("%s: null input pointer", fn);
-    if (!dL_da || !d_gamma || !d_beta) return set_error("%s: null gradient pointer", fn);
+    if ((rows > 0 && (!y || !dL_dn)) || !gamma) return set_error("%s: null input pointer", fn);
+    if ((rows > 0 && !dL_da) || !d_gamma || !d_beta) return set_error("%s: null gradient pointer", fn);
     if (!workspace || srf::misaligned(workspace)) return set_error("%s: workspace must be 256-byte aligned", fn);
     srf::ln_backward<srf::kLnMaxJ>(static_cast<cudaStream_t>(stream_), rows, C, eps, y, gamma, dL_dn, dL_dy,
                                    static_cast<float*>(workspace), dL_da, d_gamma, d_beta);

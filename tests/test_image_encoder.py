@@ -7,8 +7,10 @@ embedding and the residual LayerNorms in CUDA (lara_b200.image_encoder, csrc/ima
   the patch matrix against ``transforms.Normalize`` + ``F.conv2d``; timm's state-dict keys and shapes, a LaRa checkpoint
   loaded strictly, and the argument checks of the Python and C entries.  With timm importable, the restatement against
   ``timm.create_model``; otherwise that test skips.
-* GPU (TF32 off for the fp32 comparisons): each kernel, forward and backward, against float64 (every element within
-  1e-5 of the tensor's float64 maximum); the whole encoder's output and its 150 parameter gradients against float64,
+* GPU (TF32 off for the fp32 comparisons): the patch, token and final-norm kernels, forward and backward, against
+  float64 (every element within 1e-5 of the tensor's float64 maximum); the residual LayerNorm (``srf_vit_layernorm``)
+  element by element against a float64 statement with a bound per element, in
+  tests/test_vol_transformer_per_element.py; the whole encoder's output and its 150 parameter gradients against float64,
   beside the fp32 restatement; bit-reproducibility under ``torch.use_deterministic_algorithms(True)`` and the same bits
   under ``no_grad``; the chain to ``FeatVolume`` through LaRa's einsum / reshape.
 """
@@ -292,29 +294,6 @@ def test_tokens_and_final_norm_kernels_match_float64(cuda_device, name):
                  "final_dgamma": _err(gam.grad, gd.grad), "final_dbeta": _err(bet.grad, bed.grad)})
     assert torch.equal(ai.grad, bi.grad) and not ai.grad[:, 0].any()
     print(name, {k: f"{e:.2e}" for k, e in errs.items()})
-    assert all(e <= TOL for e in errs.values()), errs
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("C", sorted(WIDTHS))
-@pytest.mark.parametrize("rows", [12 * 1025, 1, 777])
-def test_vit_layernorm_kernels_match_float64(cuda_device, C, rows):
-    from lara_b200.vol_transformer import _AddLayerNorm
-    dev = cuda_device
-    g = torch.Generator().manual_seed(rows + C)
-    a, b = torch.randn((rows, C), generator=g) * 2 + 0.5, torch.randn((rows, C), generator=g)
-    gn, gy = torch.randn((rows, C), generator=g), torch.randn((rows, C), generator=g)
-    w, bb = 1 + 0.2 * torch.randn(C, generator=g), 0.1 * torch.randn(C, generator=g)
-    a, b, gn, gy, w, bb = (t.to(dev) for t in (a, b, gn, gy, w, bb))
-    ins = [t.clone().requires_grad_(True) for t in (a, b, w, bb)]
-    y, n = _AddLayerNorm.apply(*ins, 1e-6, "srf_vit_layernorm")
-    torch.autograd.backward([y, n], [gy, gn])
-    ref = [t.double().requires_grad_(True) for t in (a, b, w, bb)]
-    ry = ref[0] + ref[1]
-    rn = F.layer_norm(ry, (C,), ref[2], ref[3], 1e-6)
-    torch.autograd.backward([ry, rn], [gy.double(), gn.double()])
-    errs = {"y": _err(y.detach(), ry.detach()), "n": _err(n.detach(), rn.detach())}
-    errs.update({k: _err(m.grad, r.grad) for k, m, r in zip(("da", "db", "dgamma", "dbeta"), ins, ref)})
     assert all(e <= TOL for e in errs.values()), errs
 
 

@@ -10,10 +10,11 @@ on a channels-last volume, with the group cross-attention and the residual add +
 
   The channels-last restatement equals LaRa's layout in float64 to 1e-12; the drop-in's state-dict keys and shapes
   equal LaRa's; the argument checks of the Python and C entries run without a GPU.
-* GPU (TF32 off for the fp32 comparisons): both kernels, forward and backward, against float64 (every element within
-  1e-5 of the tensor's float64 maximum); one block and a 3-layer transformer against the float64 restatement, beside
-  LaRa's own fp32 block on the same inputs; bit-reproducibility with the deterministic switch off and on; bf16
-  autocast against LaRa's block under autocast.
+* GPU (TF32 off for the fp32 comparisons): one block and a 3-layer transformer against the float64 restatement,
+  beside LaRa's own fp32 block on the same inputs; bit-reproducibility with the deterministic switch off and on; bf16
+  autocast against LaRa's block under autocast.  The attention and LayerNorm kernels themselves, forward and backward,
+  are checked element by element against a float64 statement with a bound per element in
+  tests/test_vol_transformer_per_element.py.
 """
 import ctypes
 import os
@@ -25,8 +26,6 @@ import torch
 
 from helpers import fingerprint, reference_record
 from test_decoder_layout import _import_reference_network
-
-TOL = 1e-5
 
 # ---- seeded parameters and inputs --------------------------------------------------------------------------------
 
@@ -293,90 +292,17 @@ def _err(a, ref):
     return float((a - ref).abs().max()) / (m if m > 0 else 1.0) if ref.numel() else 0.0
 
 
-# B, R, g, S, C, H, score scale (None: unit inputs)
-ATTN_CASES = {
-    "lara_v2": (3, 32, 16, 2, 256, 16, None),
-    "lara_v3": (3, 32, 16, 3, 256, 16, None),
-    "lara_v4": (3, 32, 16, 4, 256, 16, None),
-    "g8_v4": (2, 32, 8, 32, 256, 16, None),
-    "bs1": (2, 8, 8, 4, 256, 16, None),
-    "hd32": (2, 32, 16, 4, 256, 8, None),
-    "hd32_g8": (1, 32, 8, 24, 256, 8, None),
-    "score100": (2, 32, 16, 4, 256, 16, 100.0),
-}
+LARA_V4 = (3, 32, 16, 4, 256, 16)       # B, R, g, S, C, H
 
 
-def _attn_inputs(name, dev):
-    B, R, g, S, C, H, top = ATTN_CASES[name]
-    gen = torch.Generator().manual_seed(len(name) + 17)
+def _attn_inputs(dev):
+    B, R, g, S, C, H = LARA_V4
+    gen = torch.Generator().manual_seed(24)
     q = torch.randn((B, R, R, R, C), generator=gen)
     k = torch.randn((B * g ** 3, S, C), generator=gen)
     v = torch.randn((B * g ** 3, S, C), generator=gen)
-    if top is not None:                  # scale q so that the largest score is `top`
-        from oracle.vol_transformer_torch import to_groups
-        D = C // H
-        s = (to_groups(q.double(), g).view(B * g ** 3, -1, H, D).transpose(1, 2) @
-             k.double().view(B * g ** 3, S, H, D).permute(0, 2, 3, 1)) / D ** 0.5
-        q = q * (top / float(s.max()))
     up = torch.randn(q.shape, generator=gen)
     return [t.to(dev) for t in (q, k, v, up)], g, H
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("name", list(ATTN_CASES))
-def test_group_attention_kernels_match_float64(cuda_device, name):
-    from lara_b200.vol_transformer import group_attention
-    from oracle.vol_transformer_torch import group_attention_cl
-    (q, k, v, up), g, H = _attn_inputs(name, cuda_device)
-    mine_in = [t.clone().requires_grad_(True) for t in (q, k, v)]
-    o = group_attention(*mine_in, g, H)
-    o.backward(up)
-    ref_in = [t.double().requires_grad_(True) for t in (q, k, v)]
-    ro = group_attention_cl(*ref_in, g, H)
-    ro.backward(up.double())
-    errs = {"o": _err(o.detach(), ro.detach())}
-    errs.update({"d" + n: _err(a.grad, r.grad) for n, a, r in zip("qkv", mine_in, ref_in)})
-    print(name, {k_: f"{e:.2e}" for k_, e in errs.items()})
-    assert all(e <= TOL for e in errs.values()), errs
-
-
-# rows, C, eps, residual b, extra dy
-LN_CASES = {"lara_add": (3 * 32 ** 3, 256, 1e-5, True, True), "lara_norm": (3 * 32 ** 3, 256, 1e-6, True, False),
-            "first_norm1": (3 * 32 ** 3, 256, 1e-5, False, False), "c32": (1001, 32, 1e-5, True, True),
-            "c512": (777, 512, 1e-6, True, False), "one_row": (1, 256, 1e-5, True, True)}
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("name", list(LN_CASES))
-def test_add_layernorm_kernels_match_float64(cuda_device, name):
-    from lara_b200.vol_transformer import add_layer_norm
-    rows, C, eps, has_b, has_dy = LN_CASES[name]
-    gen = torch.Generator().manual_seed(rows + C)
-    dev = cuda_device
-    a, b = torch.randn((rows, C), generator=gen) * 2 + 0.5, torch.randn((rows, C), generator=gen)
-    gn, gy = torch.randn((rows, C), generator=gen), torch.randn((rows, C), generator=gen)
-    norm = torch.nn.LayerNorm(C, eps=eps)
-    with torch.no_grad():
-        norm.weight.copy_(1 + 0.2 * torch.randn(C, generator=gen))
-        norm.bias.copy_(0.1 * torch.randn(C, generator=gen))
-    norm = norm.to(dev)
-    a, b, gn, gy = (t.to(dev) for t in (a, b, gn, gy))
-    ai, bi = a.clone().requires_grad_(True), b.clone().requires_grad_(True) if has_b else None
-    out = add_layer_norm(ai, bi, norm)
-    y, n = out if has_b else (None, out)
-    torch.autograd.backward([n] + ([y] if has_dy else []), [gn] + ([gy] if has_dy else []))
-    ad, bd = a.double().requires_grad_(True), b.double().requires_grad_(True) if has_b else None
-    wd, bb = norm.weight.detach().double().requires_grad_(True), norm.bias.detach().double().requires_grad_(True)
-    yd = ad + bd if has_b else ad
-    nd = torch.nn.functional.layer_norm(yd, (C,), wd, bb, eps)
-    torch.autograd.backward([nd] + ([yd] if has_dy else []), [gn.double()] + ([gy.double()] if has_dy else []))
-    errs = {"n": _err(n.detach(), nd.detach()), "da": _err(ai.grad, ad.grad), "dgamma": _err(norm.weight.grad, wd.grad),
-            "dbeta": _err(norm.bias.grad, bb.grad)}
-    if has_b:
-        errs["y"] = _err(y.detach(), yd.detach())
-        assert torch.equal(ai.grad, bi.grad)
-    print(name, {k_: f"{e:.2e}" for k_, e in errs.items()})
-    assert all(e <= TOL for e in errs.values()), errs
 
 
 # a reduced LaRa: C, Cc, H, B, V, R, Rc, n_groups
@@ -478,7 +404,7 @@ def test_vol_transformer_matches_float64_beside_laras_fp32_transformer(cuda_devi
 def test_vol_transformer_kernels_are_bit_reproducible_with_the_deterministic_switch_off_and_on(cuda_device):
     from lara_b200.vol_transformer import add_layer_norm, group_attention
     dev = cuda_device
-    (q, k, v, up), g, H = _attn_inputs("lara_v4", dev)
+    (q, k, v, up), g, H = _attn_inputs(dev)
     rows = q.numel() // q.shape[-1]
     a, b = q.view(rows, -1), up.view(rows, -1)
     norm = torch.nn.LayerNorm(256).to(dev)
